@@ -48,8 +48,8 @@ constexpr int N_STAGE = 2;                 // activation operand stages in share
 constexpr int N_ACC = 4;                   // per-tile table ring depth
 
 // warp roles of k_edge_tc: 20 warps = 5 warpgroups. The two MMA warpgroups hold a 64 x 128 fp32 accumulator each (64
-// registers a thread), so registers are re-balanced with setmaxnreg: launch 96/thread, the control group gives 56 back,
-// the MMA groups take 24 more (256 x 120 + 128 x 40 + 256 x 96 = 60,416 of the 61,440 the launch holds).
+// registers a thread), so registers are re-balanced with setmaxnreg: launch 96/thread, the control group gives 32 back,
+// the MMA groups take 16 more (256 x 112 + 128 x 64 + 256 x 96 = all 61,440 the launch holds; no role spills).
 constexpr int W_EPI = 0;                   // warps 0-7   (WG 0,1): wgmma issue + epilogue, WG g = channel (GCL) / edge (COORD) half
 constexpr int N_EPI_WARPS = 8;
 constexpr int W_LOAD = 8;                  // warp  8     (WG 2)  : W2 bulk copy
@@ -58,7 +58,9 @@ constexpr int N_TBL_WARPS = 3;
 constexpr int W_PROD = 12;                 // warps 12-19 (WG 3,4): producers (first Linear + SiLU -> fp16 operand tile)
 constexpr int N_PROD_WARPS = 8;
 constexpr int EDGE_TC_THREADS = 32 * (W_PROD + N_PROD_WARPS);   // 640
-constexpr int REGS_EPI = 120, REGS_CTRL = 40;
+constexpr int REGS_EPI = 112, REGS_CTRL = 64;
+// GCL: named barriers that pass the wgmma issue turn between the two MMA warpgroups (id 2 is the COORD epilogue's)
+constexpr int BAR_TURN0 = 3, BAR_TURN1 = 4;
 
 // shared memory map (bytes from a 1024-aligned base)
 constexpr int OFF_WHI = 0;
@@ -138,6 +140,9 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 }
 __device__ __forceinline__ void named_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+__device__ __forceinline__ void named_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 // Same, for roles that run far ahead of (or lag behind) the critical path: back off between polls so the spin does
 // not steal issue slots from the producer / epilogue warps sharing the scheduler.
@@ -351,8 +356,12 @@ __device__ __forceinline__ typename std::conditional<SPARSE, RecIter, TileIter<C
 //                      bias + SiLU + edge weight + segment sum                              [empty[s], tempty[a]]
 //   loader (1)       : W2 hi|lo, one bulk copy per launch                                    [w]
 //
-// Every role works on a different tile at any moment, so L2 latency (producers) and the tensor pipe + epilogue overlap;
-// the two SiLUs per edge-channel (MUFU) are the shared bottleneck by design.
+// Every role works on a different tile at any moment, so L2 latency (producers) and the tensor pipe + epilogue overlap.
+// GCL: the two MMA warpgroups take turns at the tensor pipe (ping-pong, named barriers BAR_TURN0/1): WG 0 issues tile t,
+// WG 1 issues tile t as soon as WG 0 has committed, WG 0 runs its epilogue of t while WG 1's wgmma run, then issues t + 1
+// as soon as WG 1 has committed, and so on. The accumulator lives in the registers of the group that runs the epilogue,
+// so this alternation is what keeps the tensor pipe busy during epilogues. COORD keeps both groups in lockstep: its
+// epilogue combines the two edge halves through shared memory.
 // SPARSE = true: cut-off (pocket) graphs -- tiles are packed from the per-row neighbour lists k_nbr built for this
 // forward call, so only edges the reference creates are processed (egnn.py:554-596); FC graphs use SPARSE = false.
 // ---------------------------------------------------------------------------------------------------------
@@ -587,17 +596,31 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
     mbar_wait(bars + BAR_W, 0);
     for (int t = 0;; ++t) {
       const int acc = t & (N_ACC - 1), s = t & (N_STAGE - 1);
+      // GCL ping-pong: WG 0 issues tile t once WG 1 has issued tile t - 1 (also before the end marker, so every arrive on a
+      // turn barrier is matched by a sync), and WG 1 issues tile t once WG 0 has.
+      if (!COORD && g == 0 && t > 0) named_sync(BAR_TURN0, 32 * N_EPI_WARPS);
       mbar_wait(bars + BAR_TBL + 8 * acc, (t / N_ACC) & 1);
       const uint8_t* tb = sm + OFF_TBL + acc * TBL_BYTES;
       const int* hdr = reinterpret_cast<const int*>(tb + TBL_HDR);
       const int Et = hdr[0];
       if (Et <= 0) break;
-      mbar_wait(bars + BAR_FULL + 8 * s, (t / N_STAGE) & 1);
       const uint32_t bhi = sbase + OFF_ST + s * STAGE_BYTES, blo = bhi + B_BYTES;
-      if (!COORD)
-        gemm_3xf16(d, sbase + OFF_WHI + g * 1024, sbase + OFF_WLO + g * 1024, W_LBO, bhi, blo, B_LBO, 2 * B_LBO, 8, false);
-      else
+      if (!COORD) {
+        if (g == 1) named_sync(BAR_TURN1, 32 * N_EPI_WARPS);
+        mbar_wait(bars + BAR_FULL + 8 * s, (t / N_STAGE) & 1);
+        fence_acc(d);
+        wg_fence();
+        mma_3xf16(d, sbase + OFF_WHI + g * 1024, sbase + OFF_WLO + g * 1024, W_LBO, bhi, blo, B_LBO, 2 * B_LBO, 8, false);
+        wg_commit();
+        // Hand the turn over once committed, not completed: the other group's wgmma queue behind these and the tensor
+        // pipe never drains, while this group's epilogue below overlaps them.
+        named_arrive(g == 0 ? BAR_TURN1 : BAR_TURN0, 32 * N_EPI_WARPS);
+        wg_wait_all();
+        fence_acc(d);
+      } else {
+        mbar_wait(bars + BAR_FULL + 8 * s, (t / N_STAGE) & 1);
         gemm_3xf16(d, bhi + g * 1024, blo + g * 1024, B_LBO, sbase + OFF_WHI, sbase + OFF_WLO, W_LBO, 2 * W_LBO, 8, false);
+      }
       __syncwarp();
       if (lane == 0) mbar_arrive(bars + BAR_EMPTY + 8 * s);   // operand stage reusable: this warpgroup's wgmma are complete
 
@@ -608,9 +631,11 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
       const int* rownode = reinterpret_cast<const int*>(tb + TBL_ROWNODE);
       const int* rowstart = reinterpret_cast<const int*>(tb + TBL_ROWSTART);
       if (!COORD) {
-        // Thread = channels (r0, r0 + 8) x edges E0 .. E0 + 31. Rows are contiguous edge ranges: walk the edges, write every
-        // row that starts and ends inside the run, and pass the partial sum of a row that leaves the run to the next quad
-        // lane (hsum: the run's first row, lsum: the row currently open).
+        // Thread = channels (r0, r0 + 8) x edges E0 .. E0 + 31. Rows are contiguous edge ranges. Bit tt of bmask marks a
+        // row start at edge E0 + tt inside the run; the tile end Et counts as one, so edges past it land in a sum nobody
+        // reads. The per-edge path is arithmetic plus one running sum: at a boundary the sum closes the run's first row
+        // (hsum, finished below with the carry from earlier lanes) or a row that lies wholly inside the run (written at
+        // once); the partial sum of a row that leaves the run is passed to the next quad lane.
         const float2 bias = make_float2(b2w5[r0].x * -1.4426950408889634f, b2w5[r0 + 8].x * -1.4426950408889634f);
         const float inv_norm = 1.0f / gm.normalization_factor;
         const int E0 = 32 * q;
@@ -618,30 +643,36 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
         int cur = 0;
         if (has) { while (rowstart[cur + 1] <= E0) ++cur; }
         const int hrow = cur;
-        int nxt = rowstart[cur + 1];
-        float2 hsum = make_float2(0.f, 0.f), lsum = make_float2(0.f, 0.f);
+        uint32_t bmask = 0;
+        int nr = cur + 1;
+        if (has) { for (; nr <= nrt && rowstart[nr] < E0 + 32; ++nr) bmask |= 1u << (rowstart[nr] - E0); }
+        const bool open_end = has && nr <= nrt && rowstart[nr] > E0 + 32;   // the last row continues in the next lane's run
+        const bool cut = Et < E0 + 32;                     // the tile ends inside the run
+        const uint32_t wmask = __reduce_or_sync(0xffffffffu, bmask);
+        float2 hsum = make_float2(0.f, 0.f), sum = make_float2(0.f, 0.f);
         bool in_head = true;
 #pragma unroll
         for (int tt = 0; tt < 32; ++tt) {
-          const int e = E0 + tt;
-          if (e < Et) {
-            if (e == nxt) {                                // leaving row `cur` inside the run
-              if (!in_head) {
-                float* dst = a.agg + (gb + rownode[cur]) * H;
-                dst[r0] = lsum.x * inv_norm; dst[r0 + 8] = lsum.y * inv_norm;
-              }
-              in_head = false; lsum = make_float2(0.f, 0.f);
-              ++cur; nxt = rowstart[cur + 1];
+          if (wmask & (1u << tt)) {                        // warp-uniform: some lane's run has a row start at tt
+            const bool here = (bmask >> tt) & 1u;          // this lane leaves row `cur`
+            if (here && !in_head) {
+              float* dst = a.agg + (gb + rownode[cur]) * H;
+              dst[r0] = sum.x * inv_norm; dst[r0 + 8] = sum.y * inv_norm;
             }
-            const float2 ed = emds[e];
-            const float2 u = ffma2(make_float2(d[(tt >> 1) * 4 + (tt & 1)], d[(tt >> 1) * 4 + 2 + (tt & 1)]),
-                                   make_float2(ed.y, ed.y), bias);
-            const float2 v = fmul2(usig2(u), make_float2(ed.x, ed.x));
-            if (in_head) hsum = fadd2(hsum, v); else lsum = fadd2(lsum, v);
+            hsum = here && in_head ? sum : hsum;
+            sum = here ? make_float2(0.f, 0.f) : sum;
+            in_head = in_head && !here;
+            cur += here ? 1 : 0;
           }
+          const float2 ed = emds[E0 + tt];
+          const float2 u = ffma2(make_float2(d[(tt >> 1) * 4 + (tt & 1)], d[(tt >> 1) * 4 + 2 + (tt & 1)]),
+                                 make_float2(ed.y, ed.y), bias);
+          const float2 v = fmul2(usig2(u), make_float2(ed.x, ed.x));
+          sum = fadd2(sum, v);
         }
+        if (in_head) hsum = sum;
+        const float2 lsum = sum;                           // the row open at the run's end (unless `cut`)
         // carry across the quad in lane order (fixed order: deterministic)
-        const bool open_end = has && nxt > E0 + 32;        // the open row continues in the next lane's run
         const bool cont_in = has && rowstart[hrow] < E0;   // this run's first row started in an earlier lane
         float2 cin = (q == 0 && nrt == 1 && !first_chunk) ? run : make_float2(0.f, 0.f);
 #pragma unroll
@@ -660,7 +691,7 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
             float* dst = a.agg + (gb + rownode[hrow]) * H;
             dst[r0] = htot.x * inv_norm; dst[r0 + 8] = htot.y * inv_norm;   // egnn.py:312-313
           }
-          if (!in_head && !open_end) {                     // so does the last one
+          if (!in_head && !open_end && !cut) {             // so does the last one, unless the tile end closed it above
             float* dst = a.agg + (gb + rownode[cur]) * H;
             dst[r0] = lsum.x * inv_norm; dst[r0 + 8] = lsum.y * inv_norm;
           }
