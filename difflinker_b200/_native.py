@@ -46,6 +46,7 @@ SYMBOLS = {
                                    _P, _P]),
     "dl_set_noise_slice": (_I32, [_P, _I32, _I32]),
     "dl_noise_fill": (_I32, [_P, _I32, _I32, _I32, C.c_uint64, C.c_uint64, _P, _P, _P]),
+    "dl_noise_fill_inpaint": (_I32, [_P, _I32, _I32, _I32, _P, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "dl_sample_chain_host": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "dl_launch_count": (_I64, [_P]),
     "dl_last_elapsed_ms": (_F, [_P]),

@@ -448,7 +448,8 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     InpaintArgs ia{};
     ia.mode = io.inpaint ? 1 : 0;
     ia.eps = io.inpaint ? ws.eps : io.out; ia.nm = ws.nm; ia.z = ws.z; ia.xh0 = io.xh0;
-    ia.fragment_mask = io.fragment_mask; ia.linker_mask = io.upd_linker_mask; ia.noise = io.noise; ia.coef = e->coef_dev;
+    ia.fragment_mask = io.fragment_mask; ia.linker_mask = io.upd_linker_mask; ia.noise = io.noise; ia.rng = io.rng;
+    ia.coef = e->coef_dev;
     ia.step_prep = e->step_ctr; ia.step_fin = e->step_ctr + 1; ia.T = io.T;
     ia.norm0 = io.norm0; ia.norm1 = io.norm1; ia.bias1 = io.bias1; ia.chain = io.chain;
     k_inpaint<<<B, 256, 0, st>>>(gm, ia);
@@ -777,10 +778,10 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
   dl_status s = check_shapes(e, B, N);
   if (s != DL_OK) return s;
   if (e->slice_B_full > 0 && e->slice_b0 + B > e->slice_B_full) { set_err("batch slice [%d, %d) exceeds the full batch %d", e->slice_b0, e->slice_b0 + B, e->slice_B_full); return DL_ERR_INVALID; }
-  if (sampler != DL_SAMPLER_LINKER) { set_err("device-side noise is implemented for the linker sampler (the inpainting sampler takes prepared slabs)"); return DL_ERR_UNSUPPORTED; }
   if (offset % 4 != 0) { set_err("philox offset must be a multiple of 4 (torch.Generator.get_offset())"); return DL_ERR_INVALID; }
   const NoiseRng q = make_rng(e, B, N, seed, offset);
-  if (offset_consumed) *offset_consumed = (uint64_t)(T + 2) * q.per_draw;
+  const uint64_t n_draws = sampler == DL_SAMPLER_INPAINT ? (uint64_t)2 * T + 3 : (uint64_t)T + 2;
+  if (offset_consumed) *offset_consumed = n_draws * q.per_draw;
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, nullptr,
                            &q, coef, norm, chain, nan_flags, stream);
 }
@@ -801,6 +802,23 @@ dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uin
   const NoiseRng q = make_rng(e, B, N, seed, offset);
   if (offset_consumed) *offset_consumed = (uint64_t)n_draws * q.per_draw;
   k_noise_fill<<<e->num_sms * 4, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(n_draws, B * N, 3 + e->cfg.in_node_nf, q, out);
+  LAUNCH_CHECK();
+  return DL_OK;
+}
+
+dl_status dl_noise_fill_inpaint(dl_engine* e, int32_t T, int32_t B, int32_t N, const int8_t* node_mask,
+                                const float* fragment_mask, uint64_t seed, uint64_t offset, float* out,
+                                uint64_t* offset_consumed, void* stream) {
+  dl_status s = check_shapes(e, B, N);
+  if (s != DL_OK) return s;
+  if (!node_mask || !fragment_mask || !out) { set_err("null argument"); return DL_ERR_INVALID; }
+  if (T < 1 || 2 * T + 3 > 65535) { set_err("need 1 <= T <= 32766 (got %d)", T); return DL_ERR_INVALID; }
+  if (e->slice_B_full > 0 && e->slice_b0 + B > e->slice_B_full) { set_err("batch slice [%d, %d) exceeds the full batch %d", e->slice_b0, e->slice_b0 + B, e->slice_B_full); return DL_ERR_INVALID; }
+  CK(cudaSetDevice(e->cfg.device));
+  const NoiseRng q = make_rng(e, B, N, seed, offset);
+  if (offset_consumed) *offset_consumed = (uint64_t)(2 * T + 3) * q.per_draw;
+  k_com_free_draws<<<dim3(B, 2 * T + 3), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      N, 3 + e->cfg.in_node_nf, T, q, node_mask, fragment_mask, out);
   LAUNCH_CHECK();
   return DL_OK;
 }
@@ -847,8 +865,13 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   const int n = B * N, xd = 3 + e->cfg.in_node_nf;
   // frames that no reverse step is the last writer of stay zero, as torch.zeros in edm.py:143
   CK(cudaMemsetAsync(chain, 0, (size_t)keep_frames * n * xd * sizeof(float), st));
-  if (inpaint) {
-    // z_T = COM-free masked noise on every atom (edm.py:565); the caller's slab 0 is already masked and projected
+  if (inpaint && rng) {
+    // z_T = COM-free masked noise on every atom (edm.py:565): draw 0 of the device-side stream
+    k_com_free_draws<<<dim3(B, 1), 256, 0, st>>>(N, xd, T, *rng, node_mask, fragment_mask, e->ws.z);
+    LAUNCH_CHECK();
+    e->launches += 1;
+  } else if (inpaint) {
+    // the caller's slab 0 is already masked and projected
     CK(cudaMemcpyAsync(e->ws.z, noise, (size_t)n * xd * sizeof(float), cudaMemcpyDeviceToDevice, st));
   } else {
     k_init_z<<<(n * xd + 255) / 256, 256, 0, st>>>(n, xd, xh, fragment_mask, linker_mask, noise, rng ? *rng : NoiseRng{}, e->ws.z);

@@ -948,8 +948,9 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
 //   mode 1: one reverse step of InpaintingEDM.sample_chain (edm.py:549-612): centred eps, p(z_s|z_t) on all atoms,
 //           q(z_s|z_t,x) on the fragment atoms, recombination, centre-of-mass projection, chain frame;
 //           the last row does sample_p_xh_given_z0 / sample_q_xh_given_z0_and_x (edm.py:689-721).
-// Noise slabs arrive already masked and COM-projected (utils.py:158-168): slab 0 = init, 1+2r / 2+2r = step r
-// (all atoms / fragment atoms), 2T+1 / 2T+2 = final draws.
+// The draws are masked and COM-projected (utils.py:158-168): draw 0 = init, 1+2r / 2+2r = step r (all atoms / fragment
+// atoms), 2T+1 / 2T+2 = final draws. They arrive as prepared slabs, or with rng.on are regenerated in the CTA
+// (com_free_means / com_free_value below).
 // ------------------------------------------------------------------------------------------------
 struct InpaintArgs {
   int mode;
@@ -958,7 +959,8 @@ struct InpaintArgs {
   float* z;                 // (B*N,3+F)
   const float* xh0;         // (B*N,3+F) normalised input (fragments are re-noised from it)
   const float* fragment_mask; const float* linker_mask;
-  const float* noise;
+  const float* noise;       // (2T+3,B*N,3+F) prepared draws, or null with rng.on
+  NoiseRng rng;
   const float* coef;
   int* step_prep; const int* step_fin;
   int T;
@@ -977,6 +979,43 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
 #pragma unroll
   for (int w = 0; w < 8; ++w) s += red[w];
   return s;
+}
+
+// ------------------------------------------------------------------------------------------------
+// The inpainting sampler's draws from the device-side stream. Draw r of a molecule is what
+// InpaintingEDM.draw_noise_inpaint makes of the raw draw r = noise_draw(q, r, ...):
+//   coordinates  xm - (sum_n xm / sum_n m) * m,  xm = raw * m   (sample_center_gravity_zero_gaussian_with_mask)
+//   features     raw * m
+// with m the fragment mask for draws 2, 4, ..., 2T (q(z_s|z_t,x) of the reverse steps) and the node mask otherwise.
+// com_free_means reduces a molecule's three coordinate sums and its mask count in a fixed order (strided per-thread
+// partials, then block_sum_256), so a molecule's draw depends neither on the batch split nor on the launch; every thread
+// of the 256-thread CTA must call it. com_free_value then regenerates any element. Nothing is stored: the CTA draws the
+// 3 coordinate normals of every atom once for the sums and again for the values. A per-molecule copy does not fit in
+// shared memory at N = 4000 (pocket graphs), and a workspace copy would trade that second Philox evaluation of 3 of the
+// 3+F columns for a global write and read of the whole draw. An empty mask gives 0/0 means, as in the tensor path.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool com_free_on_fragments(int r, int T) { return r >= 2 && r <= 2 * T && (r & 1) == 0; }
+
+template <typename M>
+__device__ float3 com_free_means(const NoiseRng& q, int r, int b, int N, const M* __restrict__ mask, float* red) {
+  // one (atom, coordinate) pair per thread and pass: ceil(3N / 256) Philox evaluations in a row, not 3 ceil(N / 256)
+  float cnt = 0.f, sx = 0.f, sy = 0.f, sz = 0.f;
+  for (int idx = threadIdx.x; idx < 3 * N; idx += 256) {
+    const int n = idx / 3, d = idx - 3 * n, g = b * N + n;
+    const float m = (float)mask[g];
+    const float v = __fmul_rn(noise_draw(q, r, g, d), m);
+    if (d == 0) { cnt += m; sx += v; } else if (d == 1) sy += v; else sz += v;
+  }
+  cnt = block_sum_256(cnt, red);
+  sx = block_sum_256(sx, red); sy = block_sum_256(sy, red); sz = block_sum_256(sz, red);
+  return make_float3(sx / cnt, sy / cnt, sz / cnt);
+}
+
+// element d of node g of draw r, mask value m, means from com_free_means (rounded step by step as the torch ops are)
+__device__ __forceinline__ float com_free_value(const NoiseRng& q, int r, int g, int d, float m, float3 mean) {
+  const float xm = __fmul_rn(noise_draw(q, r, g, d), m);
+  if (d >= 3) return xm;
+  return __fsub_rn(xm, __fmul_rn(d == 0 ? mean.x : d == 1 ? mean.y : mean.z, m));
 }
 
 __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
@@ -1007,8 +1046,16 @@ __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
   const float ca = cf[1], cb = cf[2], cc = cf[3], qa = cf[5], qb = cf[6];
   const int frame = __float_as_int(cf[4]);
   const size_t slab = (size_t)gm.B * N * xd;
-  const float* nA = a.noise + (size_t)(1 + 2 * step) * slab;
-  const float* nB = nA + slab;
+  // draw rA: p(z_s|z_t) on all atoms; draw rB: q(z_s|z_t,x) on the fragment atoms, or the final q draw on all atoms
+  const int rA = 1 + 2 * step, rB = rA + 1;
+  const float* nA = a.rng.on ? nullptr : a.noise + (size_t)rA * slab;
+  const float* nB = a.rng.on ? nullptr : a.noise + (size_t)rB * slab;
+  float3 meanA{}, meanB{};
+  if (a.rng.on) {
+    meanA = com_free_means(a.rng, rA, b, N, a.nm, red);
+    meanB = com_free_on_fragments(rB, a.T) ? com_free_means(a.rng, rB, b, N, a.fragment_mask, red)
+                                           : com_free_means(a.rng, rB, b, N, a.nm, red);
+  }
   if (step < a.T) {
     // pass 1: new latent before the centre-of-mass projection
     float cx = 0.f, cy = 0.f, cz = 0.f;
@@ -1019,8 +1066,10 @@ __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
       float e = a.eps[gi];
       if (d < 3) e -= (d == 0 ? mvx : d == 1 ? mvy : mvz) * m;
       const float zt = a.z[gi];
-      const float zl = (zt / ca - cb * e) + cc * nA[gi];                         // edm.py:634-642
-      const float zf = (qa * zt + qb * (a.xh0[gi] * fm)) + cc * nB[gi];           // edm.py:655-668
+      const float na = a.rng.on ? com_free_value(a.rng, rA, (int)(g0 + n), d, m, meanA) : nA[gi];
+      const float nb = a.rng.on ? com_free_value(a.rng, rB, (int)(g0 + n), d, fm, meanB) : nB[gi];
+      const float zl = (zt / ca - cb * e) + cc * na;                             // edm.py:634-642
+      const float zf = (qa * zt + qb * (a.xh0[gi] * fm)) + cc * nb;               // edm.py:655-668
       const float zn = zl * lm + zf * fm;                                        // edm.py:589
       a.z[gi] = zn;
       if (d == 0) cx += zn; else if (d == 1) cy += zn; else if (d == 2) cz += zn;
@@ -1046,8 +1095,10 @@ __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
         float e = a.eps[gi];
         if (d < 3) e -= (d == 0 ? mvx : d == 1 ? mvy : mvz) * m;
         const float zt = a.z[gi];
-        const float xl = ca * (zt - cb * e) + cc * nA[gi];                       // edm.py:701-702 (ca = 1/alpha_0, cb = sigma_0)
-        const float xf = ca * zt - qa * nB[gi];                                  // edm.py:716 (qa = sigma_0/alpha_0)
+        const float na = a.rng.on ? com_free_value(a.rng, rA, (int)(g0 + n), d, m, meanA) : nA[gi];
+        const float nb = a.rng.on ? com_free_value(a.rng, rB, (int)(g0 + n), d, m, meanB) : nB[gi];
+        const float xl = ca * (zt - cb * e) + cc * na;                           // edm.py:701-702 (ca = 1/alpha_0, cb = sigma_0)
+        const float xf = ca * zt - qa * nb;                                      // edm.py:716 (qa = sigma_0/alpha_0)
         if (d < 3) {
           a.chain[gi] = (xl * a.norm0) * lm + (xf * a.norm0) * fm;
         } else {
@@ -1081,6 +1132,22 @@ __global__ void k_noise_fill(int n_draws, int n_total, int xd, NoiseRng rng, flo
     const int d = (int)(i % xd);
     const long long gi = i / xd;
     out[i] = noise_draw(rng, (int)(gi / n_total), (int)(gi % n_total), d);
+  }
+}
+
+// Draws [0, gridDim.y) of the inpainting sampler's stream, masked and COM-projected, one CTA per (molecule, draw):
+// out is (gridDim.y, B = gridDim.x, N, xd). All 2T+3 for dl_noise_fill_inpaint; draw 0 -- the initial z (edm.py:565) --
+// straight into the workspace when the sampler draws on the device.
+__global__ void __launch_bounds__(256) k_com_free_draws(int N, int xd, int T, NoiseRng rng, const int8_t* __restrict__ node_mask,
+                                                        const float* __restrict__ fragment_mask, float* __restrict__ out) {
+  __shared__ float red[8];
+  const int b = blockIdx.x, r = blockIdx.y;
+  const bool frag = com_free_on_fragments(r, T);
+  const float3 mean = frag ? com_free_means(rng, r, b, N, fragment_mask, red) : com_free_means(rng, r, b, N, node_mask, red);
+  float* o = out + ((size_t)blockIdx.y * gridDim.x + b) * N * xd;
+  for (int idx = threadIdx.x; idx < N * xd; idx += 256) {
+    const int n = idx / xd, d = idx - n * xd, g = b * N + n;
+    o[idx] = com_free_value(rng, r, g, d, frag ? fragment_mask[g] : (float)node_mask[g], mean);
   }
 }
 

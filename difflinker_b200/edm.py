@@ -16,6 +16,24 @@ from .noise import PredefinedNoiseSchedule
 from .utils import FoundNaNException, nan_exception_class
 
 
+def _sample_chain_rng(lib, eng, dev, batch_slice, head, tail):
+    """dl_sample_chain_rng(eng, *head, seed, offset, &consumed, *tail) from the state of `dev`'s default CUDA generator, with
+    the engine's batch slice set for the duration of the call; then advances the generator as if the reference's randn
+    calls had run."""
+    gen = torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
+    seed, offset = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF, gen.get_offset()
+    used = C.c_uint64(0)
+    if batch_slice is not None:
+        _native.check(lib.dl_set_noise_slice(eng, int(batch_slice[1]), int(batch_slice[0])), "dl_set_noise_slice")
+    try:
+        st = lib.dl_sample_chain_rng(eng, *head, seed, offset, C.byref(used), *tail)
+    finally:
+        if batch_slice is not None:
+            lib.dl_set_noise_slice(eng, 0, 0)
+    _native.check(st, "dl_sample_chain_rng")
+    gen.set_offset(offset + used.value)
+
+
 class EDM(torch.nn.Module):
     def __init__(
             self,
@@ -176,18 +194,9 @@ class EDM(torch.nn.Module):
             with torch.cuda.device(dev):
                 stream = torch.cuda.current_stream(dev).cuda_stream
                 if on_device:
-                    gen = torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
-                    seed, offset = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF, gen.get_offset()
-                    used = C.c_uint64(0)
-                    if batch_slice is not None:
-                        _native.check(lib.dl_set_noise_slice(eng, int(batch_slice[1]), int(batch_slice[0])), "dl_set_noise_slice")
-                    st = lib.dl_sample_chain_rng(eng, _native.SAMPLER_LINKER, n_samples, n_nodes, T, keep_frames, ptr(xh),
-                                                 ptr(nm), ptr(fm), ptr(lm), ptr(em), ptr(ctx), seed, offset, C.byref(used),
-                                                 coef, norm, ptr(chain), ptr(flags), stream)
-                    if batch_slice is not None:
-                        lib.dl_set_noise_slice(eng, 0, 0)
-                    _native.check(st, "dl_sample_chain_rng")
-                    gen.set_offset(offset + used.value)          # as if the reference's (T+2) x 2 randn calls had run
+                    _sample_chain_rng(lib, eng, dev, batch_slice,
+                                      (_native.SAMPLER_LINKER, n_samples, n_nodes, T, keep_frames, ptr(xh), ptr(nm), ptr(fm),
+                                       ptr(lm), ptr(em), ptr(ctx)), (coef, norm, ptr(chain), ptr(flags), stream))
                 else:
                     st = lib.dl_sample_chain(eng, _native.SAMPLER_LINKER, n_samples, n_nodes, T, keep_frames, ptr(xh),
                                              ptr(nm), ptr(fm), ptr(lm), ptr(em), ptr(ctx), ptr(noise), coef, norm,
@@ -261,7 +270,11 @@ class InpaintingEDM(EDM):
 
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
-                     noise=None):
+                     noise=None, batch_slice=None):
+        """`noise` optionally injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA
+        and with noise_mode 'reference_stream', the draws are made inside the kernels from the default generator's state
+        (dl_sample_chain_rng), unless `draw_noise_inpaint` is replaced -- on the instance, in a subclass or on the class --
+        in which case the replacement draws them. `batch_slice=(b0, B_full)` as in EDM.sample_chain."""
         lib = _native.load_library()
         n_samples, n_nodes = x.size(0), x.size(1)
         dev = x.device
@@ -273,10 +286,16 @@ class InpaintingEDM(EDM):
         d = self.n_dims + self.in_node_nf
         xn, hn = self.normalize(x, h)
         xh = torch.cat([xn, hn], dim=2).to(torch.float32).contiguous()
-        if noise is None:
-            noise = self.draw_noise_inpaint(n_samples, n_nodes, dev, node_mask, fragment_mask)
-        noise = noise.to(device=dev, dtype=torch.float32).contiguous()
-        assert noise.shape == (2 * T + 3, n_samples, n_nodes, d), noise.shape
+        on_device = (noise is None and dev.type == 'cuda' and self.noise_mode == 'reference_stream'
+                     and 'draw_noise_inpaint' not in self.__dict__
+                     and type(self).draw_noise_inpaint is _DRAW_NOISE_INPAINT)
+        if batch_slice is not None and not on_device:
+            raise ValueError("batch_slice needs the device-side noise stream (CUDA tensors, noise_mode='reference_stream')")
+        if not on_device:
+            if noise is None:
+                noise = self.draw_noise_inpaint(n_samples, n_nodes, dev, node_mask, fragment_mask)
+            noise = noise.to(device=dev, dtype=torch.float32).contiguous()
+            assert noise.shape == (2 * T + 3, n_samples, n_nodes, d), noise.shape
         eng = self.dynamics.engine(self.dynamics._device_index(x))
         self.dynamics._check_graph_type()
         prep = lambda v, dt: None if v is None else v.detach().to(device=dev, dtype=dt).contiguous()
@@ -293,18 +312,26 @@ class InpaintingEDM(EDM):
         chain = torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32)
         flags = torch.zeros(n_samples, dtype=torch.int32, device=dev)
         ptr = lambda v: None if v is None else v.data_ptr()
-        args = (eng, _native.SAMPLER_INPAINT, n_samples, n_nodes, T, keep_frames, ptr(xh), ptr(nm), ptr(fm), ptr(lm),
-                ptr(em), ptr(ctx), ptr(noise), coef, norm, ptr(chain), ptr(flags))
+        head = (_native.SAMPLER_INPAINT, n_samples, n_nodes, T, keep_frames, ptr(xh), ptr(nm), ptr(fm), ptr(lm), ptr(em),
+                ptr(ctx))
+        tail = (coef, norm, ptr(chain), ptr(flags))
         if dev.type == 'cuda':
             with torch.cuda.device(dev):
-                st = lib.dl_sample_chain(*args, torch.cuda.current_stream(dev).cuda_stream)
-                _native.check(st, "dl_sample_chain")
+                stream = torch.cuda.current_stream(dev).cuda_stream
+                if on_device:
+                    _sample_chain_rng(lib, eng, dev, batch_slice, head, tail + (stream,))
+                else:
+                    _native.check(lib.dl_sample_chain(eng, *head, ptr(noise), *tail, stream), "dl_sample_chain")
                 bad = bool(flags.any().item())
         else:
-            st = lib.dl_sample_chain_host(*args)
+            st = lib.dl_sample_chain_host(eng, *head, ptr(noise), *tail)
             _native.check(st, "dl_sample_chain_host")
             bad = st == _native.DL_NAN_DETECTED
         self.last_loop_ms = float(lib.dl_last_elapsed_ms(eng))
         if bad:
             raise nan_exception_class()(flags=flags.cpu().tolist())
         return chain
+
+
+# the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path
+_DRAW_NOISE_INPAINT = InpaintingEDM.draw_noise_inpaint

@@ -1,6 +1,7 @@
 """Serialise one sampling job for a caller that has no Python: the engine configuration, the weights under the reference's
-state_dict names, the prepared inputs of `EDM.sample_chain` (reference src/edm.py:126-176), the per-step coefficient table of
-the noise schedule and a Philox (seed, offset) pair. `examples/c_sampler.c` reads the file and samples through the C-ABI
+state_dict names, the prepared inputs of `EDM.sample_chain` (reference src/edm.py:126-176) or `InpaintingEDM.sample_chain`
+(its configuration has centering = 1; its coefficient table carries qa / qb), the per-step coefficient table of the noise
+schedule and a Philox (seed, offset) pair. `examples/c_sampler.c` reads the file and samples through the C-ABI
 (`dl_sample_chain_rng`); `read_result` parses what it writes back."""
 import ctypes as C
 import struct

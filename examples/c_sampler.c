@@ -1,14 +1,16 @@
 /*
  * A plain C caller of the drop-in boundary (include/difflinker_b200.h): the reverse-diffusion sampler of
- * EDM.sample_chain (reference src/edm.py:126-235) without Python and without a noise tensor.
+ * EDM.sample_chain (reference src/edm.py:126-235), or of InpaintingEDM.sample_chain (edm.py:549-727) for a model built
+ * with centering, without Python and without a noise tensor.
  *
  *   c_sampler <job.bin> <out.bin>
  *
  * job.bin (little endian, written by difflinker_b200/export_job.py from a DDPM and a batch) holds the dl_config, the
  * weights under the reference's state_dict names, the normalised inputs and masks of one batch, the per-step
- * coefficient table of the noise schedule and a Philox (seed, offset) pair; the noise of the T+2 draws is generated
- * inside the kernels (dl_sample_chain_rng) in the order the reference's torch.randn calls would have produced it on
- * this GPU. out.bin: int32 status, uint64 philox offset consumed, the (keep_frames, B, N, 3+F) chain, B NaN flags.
+ * coefficient table of the noise schedule and a Philox (seed, offset) pair; the noise of the T+2 draws (2T+3 for
+ * inpainting) is generated inside the kernels (dl_sample_chain_rng) in the order the reference's torch.randn calls would
+ * have produced it on this GPU. out.bin: int32 status, uint64 philox offset consumed, the (keep_frames, B, N, 3+F) chain,
+ * B NaN flags.
  *
  * Build: gcc -std=c99 -O2 examples/c_sampler.c -Iinclude -I/usr/local/cuda/include -Ldifflinker_b200 -ldifflinker_b200 \
  *            -L/usr/local/cuda/lib64 -lcudart -Wl,-rpath,$PWD/difflinker_b200 -o c_sampler
@@ -109,7 +111,9 @@ int main(int argc, char** argv) {
   if (cudaStreamCreate(&stream) != cudaSuccess) { fprintf(stderr, "c_sampler: cudaStreamCreate failed\n"); return 2; }
 
   uint64_t consumed = 0;
-  const dl_status st = dl_sample_chain_rng(e, DL_SAMPLER_LINKER, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, rng[0], rng[1],
+  /* inpainting models are the ones built with centering (lightning.py:99); the engine refuses any other pairing */
+  const int32_t sampler = cfg.centering ? DL_SAMPLER_INPAINT : DL_SAMPLER_LINKER;
+  const dl_status st = dl_sample_chain_rng(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, rng[0], rng[1],
                                            &consumed, coef, norm, d_chain, d_flags, stream);
   if (st < 0) die("dl_sample_chain_rng");
   if (cudaStreamSynchronize(stream) != cudaSuccess) { fprintf(stderr, "c_sampler: the sampler's stream failed\n"); return 2; }

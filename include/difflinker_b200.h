@@ -15,7 +15,7 @@
  *   EDM.sample_chain             src/edm.py:126-176      dl_sample_chain (+ _host)
  *     sample_p_zs_given_zt_only_linker  edm.py:178-208
  *     sample_p_xh_given_z0_only_linker  edm.py:210-235
- *   InpaintingEDM.sample_chain   src/edm.py:549-612      dl_sample_chain with DL_SAMPLER_INPAINT
+ *   InpaintingEDM.sample_chain   src/edm.py:549-612      dl_sample_chain (+ _rng) with DL_SAMPLER_INPAINT
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   build_xae_molecule           src/molecule_builder.py:44-102       dl_bond_orders
  *   frame restore + .xyz text    generate.py:163-171, src/visualizer.py:14-31   dl_restore_frame, dl_format_xyz
@@ -147,8 +147,6 @@ dl_status dl_sample_chain(dl_engine* e, int32_t sampler, int32_t B, int32_t N, i
                           const float* noise, const dl_step_coef* coef, const float* norm, float* chain,
                           int32_t* nan_flags, void* stream);
 
-/* HOST-buffer variant (pinned or pageable): H2D of all inputs incl. noise, loop, D2H of chain and flags,
- * synchronises. Returns DL_NAN_DETECTED if any flag is set. */
 /*
  * Same loop with the noise drawn ON THE DEVICE in the reference's stream order (edm.py:328-345, utils.py:189-192): per draw
  * torch.randn(B,N,3) then torch.randn(B,N,F). For a CUDA generator in state (seed, offset) those calls are Philox4x32-10
@@ -157,8 +155,13 @@ dl_status dl_sample_chain(dl_engine* e, int32_t sampler, int32_t B, int32_t N, i
  * drawn -- without the tensor ((T+2) B N (3+F) floats: 226 MB for B=256, N=40, T=500), its 2(T+2) launches and its
  * interleaving copy. A plain C caller can sample with nothing but a seed.
  *   seed, offset      the generator state on entry (torch.Generator.initial_seed() / get_offset(); offset % 4 == 0)
- *   offset_consumed   HOST out (may be NULL): what the (T+2) draws consumed -- advance the generator by it
- * DL_SAMPLER_LINKER only (the inpainting sampler needs centre-of-mass projected draws: pass prepared slabs).
+ *   offset_consumed   HOST out (may be NULL): what the draws consumed -- advance the generator by it
+ * DL_SAMPLER_LINKER: T+2 raw draws, offset_consumed = (T+2) * per_draw.
+ * DL_SAMPLER_INPAINT: the 2T+3 draws of InpaintingEDM in the same call order, offset_consumed = (2T+3) * per_draw. Each is
+ *              masked and its coordinates are projected to zero centre of mass inside the per-molecule kernel, as the
+ *              prepared slabs of dl_sample_chain describe (dl_noise_fill_inpaint writes them out). The raw draws are
+ *              bit-identical to torch's; the projection sums each molecule in its own fixed order, so the coordinates
+ *              agree with torch's projection to rounding (below 1e-6 absolute).
  */
 dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
                               const float* xh, const int8_t* node_mask, const float* fragment_mask,
@@ -166,14 +169,21 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
                               uint64_t offset, uint64_t* offset_consumed, const dl_step_coef* coef, const float* norm,
                               float* chain, int32_t* nan_flags, void* stream);
 /* Strong scaling (SURVEY 8(e)): this engine samples molecules [b0, b0 + B) of a batch of B_full. The device-side noise of
- * the following dl_sample_chain_rng / dl_noise_fill calls is then the slice's ROWS of the full-batch draws (and
- * offset_consumed is the full batch's), so the gathered result is bit-identical to the single-GPU run whatever the split.
- * B_full = 0 switches it off. */
+ * the following dl_sample_chain_rng / dl_noise_fill / dl_noise_fill_inpaint calls is then the slice's ROWS of the
+ * full-batch draws (and offset_consumed is the full batch's), so the gathered result is bit-identical to the single-GPU
+ * run whatever the split. B_full = 0 switches it off. */
 dl_status dl_set_noise_slice(dl_engine* e, int32_t B_full, int32_t b0);
 /* The (n_draws,B,N,3+F) tensor the device-side stream of dl_sample_chain_rng stands for (tests, debugging). DEVICE out. */
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream);
+/* The (2T+3,B,N,3+F) prepared draws the device-side stream of dl_sample_chain_rng(DL_SAMPLER_INPAINT) stands for, computed by
+ * the same device code (tests, debugging). node_mask (B,N) int8, fragment_mask (B,N) fp32, out: DEVICE. */
+dl_status dl_noise_fill_inpaint(dl_engine* e, int32_t T, int32_t B, int32_t N, const int8_t* node_mask,
+                                const float* fragment_mask, uint64_t seed, uint64_t offset, float* out,
+                                uint64_t* offset_consumed, void* stream);
 
+/* HOST-buffer variant of dl_sample_chain (pinned or pageable): H2D of all inputs incl. noise, loop, D2H of chain and flags,
+ * synchronises. Returns DL_NAN_DETECTED if any flag is set. */
 dl_status dl_sample_chain_host(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
                                const float* xh, const int8_t* node_mask, const float* fragment_mask,
                                const float* linker_mask, const int8_t* edge_mask, const float* context,
