@@ -89,26 +89,21 @@ __device__ __forceinline__ float2 silu2(float2 x) {
   return fmul2(x, sigmoid_pair_log2(fmul2(x, make_float2(-1.4426950408889634f, -1.4426950408889634f))));
 }
 
-// Packed fp32 weights of one GCL (src/egnn.py:19-30). *_t = k-major ("transposed") [K][128].
-struct GclW {
-  const float* W1a_t;  // [128][128]  edge_mlp.0.weight[:, 0:H]^T     (h_row part)
-  const float* W1b_t;  // [128][128]  edge_mlp.0.weight[:, H:2H]^T    (h_col part)
+// Packed weights of an edge MLP: a GCL's edge_mlp (src/egnn.py:19-30) or an EquivariantUpdate's coord_mlp (src/egnn.py:90-97),
+// whose first Linear reads [h_i, h_j, d, d0] (SizeGNN: [h_i, h_j, d], w0 = 0). *_t = k-major ("transposed") [K][128].
+struct EdgeMlpW {
+  const float* W1a_t;  // [128][128]  .0.weight[:, 0:H]^T     (h_row part)
+  const float* W1b_t;  // [128][128]  .0.weight[:, H:2H]^T    (h_col part)
   const float* b1;     // [128]
-  const float* wd;     // [128]       edge_mlp.0.weight[:, 2H]        (block distance column)
-  const float* w0;     // [128]       edge_mlp.0.weight[:, 2H+1]      (input distance column)
-  const float* W2_t;   // [128][128]  edge_mlp.2.weight^T
+  const float* wd;     // [128]       .0.weight[:, 2H]        (block distance column)
+  const float* w0;     // [128]       .0.weight[:, 2H+1]      (input distance column)
+  const float* W2_t;   // [128][128]  .2.weight^T
   const float* b2;     // [128]
-  const float* W3_t;   // [256][128]  node_mlp.0.weight^T  (rows 0..127: h part, 128..255: agg part)
-  const float* b3;     // [128]
-  const float* W4_t;   // [128][128]  node_mlp.2.weight^T
-  const float* b4;     // [128]
-  const void* W2_tc;   // fp16 hi/lo wgmma-canonical tiles of edge_mlp.2.weight (tensor-core path)
+  const void* W2_tc;   // fp16 hi/lo wgmma-canonical tiles of .2.weight (tensor-core path)
   float w2_descale;    // 1 / (power-of-two scale applied to W2_tc)
   float wdmax, w0max;  // max|wd|, max|w0|: per-edge bound on the first-layer activations
-  const void* W1_tc;   // edge_mlp.0.weight[:, 0:2H] as two packed 128x128 fp16 hi/lo blocks (node kernel projections)
-  const void* W3_tc;   // node_mlp.0.weight as two packed blocks
-  const void* W4_tc;   // node_mlp.2.weight as one packed block
-  float w1_descale, w3_descale, w4_descale;
+  const void* W1_tc;   // .0.weight[:, 0:2H] as two packed 128x128 fp16 hi/lo blocks (node kernel projections)
+  float w1_descale;
   // tensor-core path, log2-domain first layer (kernels_tc.cuh pack_w2): b1, wd, w0 times -log2(e); W1_tc is packed from the
   // scaled matrix, W2_tc carries the compensating -ln2.
   const float* b1_u;
@@ -116,24 +111,20 @@ struct GclW {
   const float* w0_u;
 };
 
-// Packed weights of one EquivariantUpdate (src/egnn.py:90-97).
-struct EqW {
-  const float* W1a_t;
-  const float* W1b_t;
-  const float* b1;
-  const float* wd;
-  const float* w0;
-  const float* W2_t;
-  const float* b2;
+// Packed weights of one GCL: its edge MLP plus node_mlp.
+struct GclW : EdgeMlpW {
+  const float* W3_t;   // [256][128]  node_mlp.0.weight^T  (rows 0..127: h part, 128..255: agg part)
+  const float* b3;     // [128]
+  const float* W4_t;   // [128][128]  node_mlp.2.weight^T
+  const float* b4;     // [128]
+  const void* W3_tc;   // node_mlp.0.weight as two packed blocks
+  const void* W4_tc;   // node_mlp.2.weight as one packed block
+  float w3_descale, w4_descale;
+};
+
+// Packed weights of one EquivariantUpdate: its coord MLP plus the output row.
+struct EqW : EdgeMlpW {
   const float* w5;     // [128] coord_mlp.4.weight (no bias)
-  const void* W2_tc;
-  float w2_descale;
-  float wdmax, w0max;
-  const void* W1_tc;   // coord_mlp.0.weight[:, 0:2H] as two packed blocks
-  float w1_descale;
-  const float* b1_u;   // log2-domain copies (see GclW)
-  const float* wd_u;
-  const float* w0_u;
 };
 
 // First-layer projection of an edge MLP applied per node: A = h W1a^T + b1, B = h W1b^T.

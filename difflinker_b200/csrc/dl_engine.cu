@@ -72,7 +72,7 @@ struct dl_engine {
   bool finalized = false;
   std::map<std::string, std::vector<float>> raw;
   float* wblob = nullptr;      // packed fp32 weights
-  void* wblob_tc = nullptr;    // packed fp16 hi/lo tiles
+  __half* wblob_tc = nullptr;  // packed fp16 hi/lo tiles
   std::vector<GclW> gcl;       // [L*S]
   std::vector<EqW> eq;         // [L]
   const float *We_t = nullptr, *be = nullptr, *Wo = nullptr, *bo = nullptr;
@@ -177,14 +177,24 @@ std::vector<ExpectedParam> expected_params(const dl_config& c) {
   return v;
 }
 
-// Host-side packer: appends 16-byte aligned segments to one blob and remembers offsets.
+using RawWeights = std::map<std::string, std::vector<float>>;
+
+// Host-side packer: appends 16-byte aligned fp32 segments to one blob and fp16 tensor-core tiles to another, and remembers
+// which weight-record field each belongs to; point() aims those fields at the uploaded blobs.
 struct Packer {
   std::vector<float> blob;
-  size_t add(const std::vector<float>& seg) {
+  std::vector<__half> tc;
+  std::vector<std::pair<const float**, size_t>> fields;
+  std::vector<std::pair<const void**, size_t>> tc_fields;
+  void add(const float** field, const std::vector<float>& seg) {
     while (blob.size() % 4) blob.push_back(0.f);
-    size_t off = blob.size();
+    fields.push_back({field, blob.size()});
     blob.insert(blob.end(), seg.begin(), seg.end());
-    return off;
+  }
+  void add_tc(const void** field, size_t off) { tc_fields.push_back({field, off}); }
+  void point(const float* base, const __half* tc_base) const {
+    for (auto& f : fields) *f.first = base + f.second;
+    for (auto& f : tc_fields) *f.first = tc_base + f.second;
   }
 };
 
@@ -199,6 +209,53 @@ std::vector<float> column(const std::vector<float>& W, int out, int in_stride, i
   std::vector<float> t(out);
   for (int o = 0; o < out; ++o) t[o] = W[(size_t)o * in_stride + c];
   return t;
+}
+
+// fp32 k-major copies of an edge MLP (prefix p: "...edge_mlp." or "...coord_mlp.") whose first Linear reads in1 inputs:
+// everything but the input-distance column w0, which only the denoiser has.
+void pack_edge_mlp(Packer& pk, EdgeMlpW& w, const RawWeights& raw, const std::string& p, int in1) {
+  const auto& W1 = raw.at(p + "0.weight");
+  pk.add(&w.W1a_t, transpose_block(W1, H, in1, 0, H));
+  pk.add(&w.W1b_t, transpose_block(W1, H, in1, H, H));
+  pk.add(&w.b1, raw.at(p + "0.bias"));
+  pk.add(&w.wd, column(W1, H, in1, 2 * H));
+  pk.add(&w.W2_t, transpose_block(raw.at(p + "2.weight"), H, H, 0, H));
+  pk.add(&w.b2, raw.at(p + "2.bias"));
+}
+
+// fp32 k-major copies of a GCL (prefix p ends in '.'): its edge MLP and its node MLP.
+void pack_gcl(Packer& pk, GclW& w, const RawWeights& raw, const std::string& p, int in1) {
+  pack_edge_mlp(pk, w, raw, p + "edge_mlp.", in1);
+  pk.add(&w.W3_t, transpose_block(raw.at(p + "node_mlp.0.weight"), H, 2 * H, 0, 2 * H));
+  pk.add(&w.b3, raw.at(p + "node_mlp.0.bias"));
+  pk.add(&w.W4_t, transpose_block(raw.at(p + "node_mlp.2.weight"), H, H, 0, H));
+  pk.add(&w.b4, raw.at(p + "node_mlp.2.bias"));
+}
+
+// The denoiser's additions to an edge MLP (first Linear over 2H+2 inputs): the input-distance column w0, the bounds of the
+// distance columns, and the tensor-core copies -- W2 and the log2-domain first layer (kernels_tc.cuh pack_w2).
+void pack_edge_mlp_denoiser(Packer& pk, EdgeMlpW& w, const RawWeights& raw, const std::string& p) {
+  constexpr int IN1 = 2 * H + 2;
+  auto scaled = [](const std::vector<float>& v) { std::vector<float> o(v.size()); for (size_t i = 0; i < v.size(); ++i) o[i] = (float)((double)v[i] * tc::NEG_LOG2E); return o; };
+  auto absmax = [](const std::vector<float>& v) { float m = 0.f; for (float x : v) m = std::max(m, std::fabs(x)); return m; };
+  const auto& W1 = raw.at(p + "0.weight");
+  const std::vector<float> wd = column(W1, H, IN1, 2 * H), w0 = column(W1, H, IN1, 2 * H + 1);
+  pk.add(&w.w0, w0);
+  pk.add_tc(&w.W2_tc, tc::pack_w2(raw.at(p + "2.weight"), pk.tc, &w.w2_descale));
+  pk.add_tc(&w.W1_tc, tcn::pack_blocks(scaled(W1), IN1, 2, pk.tc, &w.w1_descale));
+  pk.add(&w.b1_u, scaled(raw.at(p + "0.bias")));
+  pk.add(&w.wd_u, scaled(wd));
+  pk.add(&w.w0_u, scaled(w0));
+  w.wdmax = absmax(wd); w.w0max = absmax(w0);
+}
+
+template <typename T>
+dl_status upload_blob(const std::vector<T>& host, T** dev) {
+  if (*dev) cudaFree(*dev);
+  *dev = nullptr;
+  CK(cudaMalloc((void**)dev, std::max<size_t>(host.size(), 1) * sizeof(T)));
+  CK(cudaMemcpy(*dev, host.data(), host.size() * sizeof(T), cudaMemcpyHostToDevice));
+  return DL_OK;
 }
 
 template <typename T>
@@ -258,21 +315,27 @@ Geom make_geom(const dl_engine* e, int B, int N) {
     }                                                                                     \
   } while (0)
 
-// Masks are constant over a whole sample_chain: build the work plan once.
-dl_status build_plan(dl_engine* e, int B, int N, const int8_t* node_mask, const float* linker_mask,
-                     const int8_t* edge_mask, cudaStream_t st) {
-  Workspace& ws = e->ws;
+// The work plan of ws (2 launches): live rows and columns of every molecule, then work items of at most tile_edges edges and
+// max_rows rows. Masks are constant over a whole sample_chain: the plan is built once per call.
+dl_status build_plan(Workspace& ws, int B, int N, int graph_type, const int8_t* node_mask, const float* linker_mask,
+                     const int8_t* edge_mask, int tile_edges, int max_rows, cudaStream_t st) {
   CK(cudaMemsetAsync(ws.agg, 0, (size_t)B * N * H * sizeof(float), st));  // dead rows aggregate to exactly 0
-  k_plan_mol<<<B, 256, 2 * N * sizeof(int), st>>>(N, e->cfg.graph_type, edge_mask, node_mask, linker_mask, ws.rowidx,
+  k_plan_mol<<<B, 256, 2 * N * sizeof(int), st>>>(N, graph_type, edge_mask, node_mask, linker_mask, ws.rowidx,
                                                   ws.colidx, ws.xrowidx, ws.nr, ws.nc, ws.nxr);
   LAUNCH_CHECK();
-  const int tile_edges = e->use_tc ? tc::TN : ET;
-  const int max_rows = e->use_tc ? tc::MAXR : MAXR;
   k_plan_items<<<1, 1, 0, st>>>(B, tile_edges, max_rows, 1, max_rows, ws.nr, ws.nc, ws.nxr, ws.items, ws.n_items, ws.xmols,
                                 ws.n_xmols, ws.xitems, ws.n_xitems);
   LAUNCH_CHECK();
-  e->launches += 2;
   return DL_OK;
+}
+
+// The denoiser's plan, tiled for the edge kernel it runs.
+dl_status build_forward_plan(dl_engine* e, int B, int N, const int8_t* node_mask, const float* linker_mask,
+                             const int8_t* edge_mask, cudaStream_t st) {
+  const dl_status s = build_plan(e->ws, B, N, e->cfg.graph_type, node_mask, linker_mask, edge_mask,
+                                 e->use_tc ? tc::TN : ET, e->use_tc ? tc::MAXR : MAXR, st);
+  if (s == DL_OK) e->launches += 2;
+  return s;
 }
 
 struct FwdIO {
@@ -288,8 +351,58 @@ struct FwdIO {
   int T = 0; float norm0 = 1.f, norm1 = 1.f, bias1 = 0.f;
 };
 
-ProjW proj_of(const GclW& w) { return ProjW{w.W1a_t, w.W1b_t, w.b1}; }
-ProjW proj_of(const EqW& w) { return ProjW{w.W1a_t, w.W1b_t, w.b1}; }
+ProjW proj_of(const EdgeMlpW& w) { return ProjW{w.W1a_t, w.W1b_t, w.b1}; }
+
+// Arguments of one edge-kernel launch over the coordinates x / x4: a GCL's edge MLP, which aggregates into ws.agg, or
+// (coord) a coordinate MLP, which writes x_out / x4_out.
+EdgeArgs edge_args(const dl_engine* e, const EdgeMlpW& w, bool coord, const int8_t* edge_mask, const float* linker_mask,
+                   const float* x, const float4* x4, float* x_out = nullptr, float4* x4_out = nullptr,
+                   const float* w5 = nullptr) {
+  const Workspace& ws = e->ws;
+  const float ksc = e->use_tc ? 1.4426950408889634f : 1.0f;   // log2-domain first layer on the tensor-core path
+  EdgeArgs ea{};
+  ea.AB = coord ? ws.ABc : ws.ABg; ea.ABmax = coord ? ws.ABcmax : ws.ABgmax;
+  ea.w2_descale = w.w2_descale; ea.wdmax = w.wdmax * ksc; ea.w0max = w.w0max * ksc;
+  ea.x = x; ea.x0 = ws.x0; ea.x4 = x4; ea.x04 = ws.x04; ea.x4_out = x4_out;
+  ea.edge_mask = edge_mask; ea.cls = ws.cls; ea.nm = ws.nm; ea.linker_mask = linker_mask;
+  ea.W2_t = w.W2_t; ea.b2 = w.b2; ea.wd = e->use_tc ? w.wd_u : w.wd; ea.w0 = e->use_tc ? w.w0_u : w.w0; ea.w5 = w5;
+  ea.plan = make_plan(ws); ea.agg = coord ? nullptr : ws.agg; ea.x_out = x_out; ea.nbr = ws.nbr;
+  ea.recs = coord ? ws.xrecs : ws.recs;
+  ea.n_recs = coord && ws.n_recs ? ws.n_recs + 1 : ws.n_recs;
+  return ea;
+}
+
+// The edge MLPs whose first-layer projections are taken from the h that GCL s of block l writes, with the AB / ABmax
+// buffers they go to: the next GCL; after a block's last GCL, the block's coordinate MLP and the next block's GCL 0.
+// s = -1 stands for the embedding, consumed by GCL 0 of block 0. Returns the count (1 or 2).
+struct NodeConsumer { const EdgeMlpW* w; float* AB; float* ABmax; };
+int node_consumers(const dl_engine* e, int l, int s, NodeConsumer c[2]) {
+  const int L = e->cfg.n_layers, S = e->cfg.inv_sublayers;
+  const Workspace& ws = e->ws;
+  if (s + 1 < S) { c[0] = {&e->gcl[l * S + s + 1], ws.ABg, ws.ABgmax}; return 1; }
+  c[0] = {&e->eq[l], ws.ABc, ws.ABcmax};
+  if (l + 1 == L) return 1;
+  c[1] = {&e->gcl[(l + 1) * S], ws.ABg, ws.ABgmax};
+  return 2;
+}
+
+// The tensor-core node kernel after GCL s of block l (weights w): its node MLP, then the projections of the new h for the
+// consumers. s = -1 skips the node MLP and only projects the embedded h for GCL 0 (w = that GCL).
+tcn::NodeTcArgs node_tc_args(const dl_engine* e, const GclW& w, int l, int s) {
+  const Workspace& ws = e->ws;
+  tcn::NodeTcArgs ta{};
+  ta.h = ws.h; ta.agg = ws.agg; ta.nm = ws.nm; ta.proj_only = s < 0;
+  ta.w3 = reinterpret_cast<const __half*>(w.W3_tc); ta.w4 = reinterpret_cast<const __half*>(w.W4_tc);
+  ta.b3 = w.b3; ta.b4 = w.b4; ta.w3_descale = w.w3_descale; ta.w4_descale = w.w4_descale;
+  NodeConsumer c[2];
+  ta.n_proj = node_consumers(e, l, s, c);
+  for (int i = 0; i < ta.n_proj; ++i) {
+    ta.pw[i] = reinterpret_cast<const __half*>(c[i].w->W1_tc); ta.pb1[i] = c[i].w->b1_u;
+    ta.p_descale[i] = c[i].w->w1_descale; ta.AB[i] = c[i].AB; ta.ABmax[i] = c[i].ABmax;
+  }
+  ta.tile_nodes = tcn::pick_tile_nodes(ws.B * ws.N, e->num_sms);
+  return ta;
+}
 
 dl_status launch_edge(dl_engine* e, const Geom& gm, const EdgeArgs& ea, bool coord, const void* w2_tc, cudaStream_t st) {
   if (e->use_tc) {
@@ -328,14 +441,7 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
   e->launches += 1;
   if (e->use_tc) {
     // A | B projections of block 0 / gcl 0 from the embedded h, on the tensor cores
-    const GclW& w0 = e->gcl[0];
-    tcn::NodeTcArgs ta{};
-    ta.h = ws.h; ta.agg = ws.h; ta.nm = ws.nm; ta.proj_only = 1;
-    ta.w3 = reinterpret_cast<const __half*>(w0.W3_tc); ta.w4 = reinterpret_cast<const __half*>(w0.W4_tc);
-    ta.b3 = w0.b3; ta.b4 = w0.b4; ta.w3_descale = 1.f; ta.w4_descale = 1.f;
-    ta.n_proj = 1; ta.pw[0] = reinterpret_cast<const __half*>(w0.W1_tc); ta.pb1[0] = w0.b1_u;
-    ta.p_descale[0] = w0.w1_descale; ta.AB[0] = ws.ABg; ta.ABmax[0] = ws.ABgmax;
-    ta.tile_nodes = tcn::pick_tile_nodes(n, e->num_sms);
+    const tcn::NodeTcArgs ta = node_tc_args(e, e->gcl[0], 0, -1);
     TIMED("k_node_tc(proj only)", st, (tcn::launch_node(n, ta, st)));
     LAUNCH_CHECK();
     e->launches += 1;
@@ -355,55 +461,26 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
   float* xout = ws.xb;
   float4* xin4 = ws.xa4;
   float4* xout4 = ws.xb4;
-  const Plan plan = make_plan(ws);
-  const float ksc = e->use_tc ? 1.4426950408889634f : 1.0f;   // log2-domain first layer on the tensor-core path
   e->last_edge_mask = io.edge_mask; e->last_linker_mask = io.linker_mask; e->last_B = B; e->last_N = N;
   for (int l = 0; l < L; ++l) {
     for (int s = 0; s < S; ++s) {
       const GclW& w = e->gcl[l * S + s];
-      EdgeArgs ea{};
-      ea.AB = ws.ABg; ea.ABmax = ws.ABgmax; ea.w2_descale = w.w2_descale; ea.wdmax = w.wdmax * ksc; ea.w0max = w.w0max * ksc;
-      ea.x = xin; ea.x0 = ws.x0; ea.x4 = xin4; ea.x04 = ws.x04; ea.x4_out = nullptr;
-      ea.edge_mask = io.edge_mask; ea.cls = ws.cls; ea.nm = ws.nm;
-      ea.linker_mask = io.linker_mask; ea.W2_t = w.W2_t; ea.b2 = w.b2; ea.wd = e->use_tc ? w.wd_u : w.wd; ea.w0 = e->use_tc ? w.w0_u : w.w0; ea.w5 = nullptr;
-      ea.plan = plan; ea.agg = ws.agg; ea.x_out = nullptr; ea.nbr = ws.nbr; ea.recs = ws.recs; ea.n_recs = ws.n_recs;
+      const EdgeArgs ea = edge_args(e, w, false, io.edge_mask, io.linker_mask, xin, xin4);
       g_times.begin(st, "edge GCL");
       dl_status st2 = launch_edge(e, gm, ea, false, w.W2_tc, st);
       g_times.end(st);
       if (st2 != DL_OK) return st2;
 
-      const bool last_sub = s + 1 >= S;
       if (e->use_tc) {
-        tcn::NodeTcArgs ta{};
-        ta.h = ws.h; ta.agg = ws.agg; ta.nm = ws.nm;
-        ta.w3 = reinterpret_cast<const __half*>(w.W3_tc); ta.w4 = reinterpret_cast<const __half*>(w.W4_tc);
-        ta.b3 = w.b3; ta.b4 = w.b4; ta.w3_descale = w.w3_descale; ta.w4_descale = w.w4_descale;
-        if (!last_sub) {
-          const GclW& nx = e->gcl[l * S + s + 1];
-          ta.n_proj = 1; ta.pw[0] = reinterpret_cast<const __half*>(nx.W1_tc); ta.pb1[0] = nx.b1_u;
-          ta.p_descale[0] = nx.w1_descale; ta.AB[0] = ws.ABg; ta.ABmax[0] = ws.ABgmax;
-        } else {
-          const EqW& q = e->eq[l];
-          ta.n_proj = 1; ta.pw[0] = reinterpret_cast<const __half*>(q.W1_tc); ta.pb1[0] = q.b1_u;
-          ta.p_descale[0] = q.w1_descale; ta.AB[0] = ws.ABc; ta.ABmax[0] = ws.ABcmax;
-          if (l + 1 < L) {
-            const GclW& nx = e->gcl[(l + 1) * S];
-            ta.n_proj = 2; ta.pw[1] = reinterpret_cast<const __half*>(nx.W1_tc); ta.pb1[1] = nx.b1_u;
-            ta.p_descale[1] = nx.w1_descale; ta.AB[1] = ws.ABg; ta.ABmax[1] = ws.ABgmax;
-          }
-        }
-        ta.tile_nodes = tcn::pick_tile_nodes(n, e->num_sms);
+        const tcn::NodeTcArgs ta = node_tc_args(e, w, l, s);
         TIMED(ta.n_proj == 2 ? "k_node_tc(2 proj)" : "k_node_tc(1 proj)", st, (tcn::launch_node(n, ta, st)));
       } else {
         NodeArgs na{};
         na.h = ws.h; na.agg = ws.agg; na.nm = ws.nm; na.W3_t = w.W3_t; na.b3 = w.b3; na.W4_t = w.W4_t; na.b4 = w.b4;
-        if (!last_sub) {
-          na.proj1 = proj_of(e->gcl[l * S + s + 1]); na.AB1 = ws.ABg; na.ABmax1 = ws.ABgmax; na.AB2 = nullptr;
-        } else {
-          na.proj1 = proj_of(e->eq[l]); na.AB1 = ws.ABc; na.ABmax1 = ws.ABcmax;
-          if (l + 1 < L) { na.proj2 = proj_of(e->gcl[(l + 1) * S]); na.AB2 = ws.ABg; na.ABmax2 = ws.ABgmax; }
-          else na.AB2 = nullptr;
-        }
+        NodeConsumer c[2];
+        const int n_proj = node_consumers(e, l, s, c);
+        na.proj1 = proj_of(*c[0].w); na.AB1 = c[0].AB; na.ABmax1 = c[0].ABmax;
+        if (n_proj == 2) { na.proj2 = proj_of(*c[1].w); na.AB2 = c[1].AB; na.ABmax2 = c[1].ABmax; }
         k_node<ACT_SILU><<<node_blocks, 256, node_smem, st>>>(n, na);
       }
       LAUNCH_CHECK();
@@ -413,12 +490,7 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     LAUNCH_CHECK();
     e->launches += 1;
     const EqW& w = e->eq[l];
-    EdgeArgs ea{};
-    ea.AB = ws.ABc; ea.ABmax = ws.ABcmax; ea.w2_descale = w.w2_descale; ea.wdmax = w.wdmax * ksc; ea.w0max = w.w0max * ksc;
-    ea.x = xin; ea.x0 = ws.x0; ea.x4 = xin4; ea.x04 = ws.x04; ea.x4_out = xout4;
-    ea.edge_mask = io.edge_mask; ea.cls = ws.cls; ea.nm = ws.nm;
-    ea.linker_mask = io.linker_mask; ea.W2_t = w.W2_t; ea.b2 = w.b2; ea.wd = e->use_tc ? w.wd_u : w.wd; ea.w0 = e->use_tc ? w.w0_u : w.w0; ea.w5 = w.w5;
-    ea.plan = plan; ea.agg = nullptr; ea.x_out = xout; ea.nbr = ws.nbr; ea.recs = ws.xrecs; ea.n_recs = ws.n_recs ? ws.n_recs + 1 : nullptr;
+    const EdgeArgs ea = edge_args(e, w, true, io.edge_mask, io.linker_mask, xin, xin4, xout, xout4, w.w5);
     g_times.begin(st, "edge COORD");
     dl_status st2 = launch_edge(e, gm, ea, true, w.W2_tc, st);
     g_times.end(st);
@@ -470,16 +542,77 @@ dl_status check_shapes(const dl_engine* e, int B, int N) {
   return DL_OK;
 }
 
-dl_status stage_reserve(dl_engine* e, size_t bytes) {
-  if (e->stage.cap >= bytes) return DL_OK;
-  if (e->stage.buf) cudaFree(e->stage.buf);
-  e->stage.buf = nullptr; e->stage.cap = 0;
-  CK(cudaMalloc((void**)&e->stage.buf, bytes));
-  e->stage.cap = bytes;
+size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// Device copies of a *_host entry point's arguments, in 256-byte aligned sub-buffers of the engine's stage. in() adds a
+// host input (a null input gets no buffer), out() an output buffer; stage_inputs() grows the stage to fit and enqueues
+// the input copies. at(i) is then buffer i's device address, or null for a null input.
+struct StageLayout {
+  struct Buf { const void* src; size_t bytes, off; bool used; };
+  std::vector<Buf> bufs;
+  size_t total = 0;
+  char* base = nullptr;
+  int add(const void* src, size_t bytes, bool used) {
+    bufs.push_back({src, bytes, total, used});
+    total += used ? align256(bytes) : 0;
+    return (int)bufs.size() - 1;
+  }
+  int in(const void* src, size_t bytes) { return add(src, bytes, src != nullptr); }
+  int out(size_t bytes) { return add(nullptr, bytes, true); }
+  template <typename T> T* at(int i) const { return bufs[i].used ? reinterpret_cast<T*>(base + bufs[i].off) : nullptr; }
+};
+
+dl_status stage_inputs(dl_engine* e, StageLayout& sl, cudaStream_t st) {
+  HostStage& sg = e->stage;
+  if (sg.cap < sl.total) {
+    if (sg.buf) cudaFree(sg.buf);
+    sg.buf = nullptr; sg.cap = 0;
+    CK(cudaMalloc((void**)&sg.buf, sl.total));
+    sg.cap = sl.total;
+  }
+  sl.base = sg.buf;
+  for (const auto& b : sl.bufs)
+    if (b.src) CK(cudaMemcpyAsync(sl.base + b.off, b.src, b.bytes, cudaMemcpyHostToDevice, st));
   return DL_OK;
 }
 
-size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+// Copies a *_host call's result and its B NaN flags back, waits for them, and reports whether any flag is set.
+dl_status stage_results(void* out, const void* d_out, size_t bytes, const int32_t* d_flags, int B, int32_t* nan_flags,
+                        cudaStream_t st) {
+  std::vector<int32_t> flags(B);
+  CK(cudaMemcpyAsync(out, d_out, bytes, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(flags.data(), d_flags, B * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  bool any = false;
+  for (int i = 0; i < B; ++i) { any |= flags[i] != 0; if (nan_flags) nan_flags[i] = flags[i]; }
+  return any ? DL_NAN_DETECTED : DL_OK;
+}
+
+// dl_set_noise_slice: the B rows of this call must lie inside the full batch
+dl_status check_slice(const dl_engine* e, int B) {
+  if (e->slice_B_full > 0 && e->slice_b0 + B > e->slice_B_full) {
+    set_err("batch slice [%d, %d) exceeds the full batch %d", e->slice_b0, e->slice_b0 + B, e->slice_B_full);
+    return DL_ERR_INVALID;
+  }
+  return DL_OK;
+}
+
+// Arguments every sampler entry point takes alike; has_draws: a noise tensor or the device-side stream supplies the draws.
+dl_status check_sampler(const dl_engine* e, int sampler, int T, int keep_frames, bool has_draws, const float* xh,
+                        const int8_t* node_mask, const float* fragment_mask, const float* linker_mask, const float* context,
+                        const dl_step_coef* coef, const float* norm, const float* chain) {
+  if (sampler != DL_SAMPLER_LINKER && sampler != DL_SAMPLER_INPAINT) { set_err("unknown sampler %d", sampler); return DL_ERR_INVALID; }
+  if ((sampler == DL_SAMPLER_INPAINT) != (e->cfg.centering != 0)) { set_err("the inpainting sampler needs a model built with centering=1 (and vice versa)"); return DL_ERR_INVALID; }
+  if (!xh || !node_mask || !fragment_mask || !linker_mask || !has_draws || !coef || !norm || !chain) {
+    set_err("null argument"); return DL_ERR_INVALID;
+  }
+  if (T < 1 || keep_frames < 1 || keep_frames > T) { set_err("need 1 <= keep_frames <= T"); return DL_ERR_INVALID; }
+  if (e->cfg.context_node_nf > 0 && !context) { set_err("context required"); return DL_ERR_INVALID; }
+  return DL_OK;
+}
+
+// standard-normal draws of one chain: init + one per step + final (linker), or their masked pairs (inpainting)
+uint64_t sampler_draws(int sampler, int T) { return sampler == DL_SAMPLER_INPAINT ? (uint64_t)2 * T + 3 : (uint64_t)T + 2; }
 
 }  // namespace
 
@@ -589,89 +722,36 @@ dl_status dl_finalize_weights(dl_engine* e) {
   for (auto& p : expected_params(e->cfg))
     if (!e->raw.count(p.name)) { set_err("missing weight %s", p.name.c_str()); return DL_ERR_WEIGHTS; }
   const int L = e->cfg.n_layers, S = e->cfg.inv_sublayers, D = e->D;
-  const int IN1 = 2 * H + 2;
+  const RawWeights& raw = e->raw;
   Packer pk;
-  std::vector<__half> tcblob;
-  struct GOff { size_t W1a, W1b, b1, wd, w0, W2, b2, W3, b3, W4, b4, w5, tc, tc1, tc3, tc4, b1u, wdu, w0u; float descale, wdmax, w0max, d1, d3, d4; };
-  // log2-domain copies for the tensor-core path (kernels_tc.cuh pack_w2): everything that feeds the first Linear of an edge MLP
-  auto scaled = [](const std::vector<float>& v) { std::vector<float> o(v.size()); for (size_t i = 0; i < v.size(); ++i) o[i] = (float)((double)v[i] * tc::NEG_LOG2E); return o; };
-  auto absmax = [](const std::vector<float>& v) { float m = 0.f; for (float x : v) m = std::max(m, std::fabs(x)); return m; };
-  std::vector<GOff> goff(L * S), eoff(L);
-  auto R = [&](const std::string& k) -> const std::vector<float>& { return e->raw[k]; };
-  size_t oWe = pk.add(transpose_block(R("dynamics.embedding.weight"), H, D, 0, D));
-  size_t obe = pk.add(R("dynamics.embedding.bias"));
-  size_t oWo = pk.add(R("dynamics.embedding_out.weight"));
-  size_t obo = pk.add(R("dynamics.embedding_out.bias"));
+  e->gcl.assign(L * S, GclW{});
+  e->eq.assign(L, EqW{});
+  pk.add(&e->We_t, transpose_block(raw.at("dynamics.embedding.weight"), H, D, 0, D));
+  pk.add(&e->be, raw.at("dynamics.embedding.bias"));
+  pk.add(&e->Wo, raw.at("dynamics.embedding_out.weight"));
+  pk.add(&e->bo, raw.at("dynamics.embedding_out.bias"));
   char buf[160];
   for (int l = 0; l < L; ++l) {
     for (int s = 0; s < S; ++s) {
       snprintf(buf, sizeof(buf), "dynamics.e_block_%d.gcl_%d.", l, s);
-      std::string p(buf);
-      GOff& o = goff[l * S + s];
-      const auto& W1 = R(p + "edge_mlp.0.weight");
-      o.W1a = pk.add(transpose_block(W1, H, IN1, 0, H));
-      o.W1b = pk.add(transpose_block(W1, H, IN1, H, H));
-      o.b1 = pk.add(R(p + "edge_mlp.0.bias"));
-      o.wd = pk.add(column(W1, H, IN1, 2 * H));
-      o.w0 = pk.add(column(W1, H, IN1, 2 * H + 1));
-      o.W2 = pk.add(transpose_block(R(p + "edge_mlp.2.weight"), H, H, 0, H));
-      o.b2 = pk.add(R(p + "edge_mlp.2.bias"));
-      o.W3 = pk.add(transpose_block(R(p + "node_mlp.0.weight"), H, 2 * H, 0, 2 * H));
-      o.b3 = pk.add(R(p + "node_mlp.0.bias"));
-      o.W4 = pk.add(transpose_block(R(p + "node_mlp.2.weight"), H, H, 0, H));
-      o.b4 = pk.add(R(p + "node_mlp.2.bias"));
-      o.tc = tc::pack_w2(R(p + "edge_mlp.2.weight"), tcblob, &o.descale);
-      o.tc1 = tcn::pack_blocks(scaled(W1), IN1, 2, tcblob, &o.d1);
-      o.b1u = pk.add(scaled(R(p + "edge_mlp.0.bias")));
-      o.wdu = pk.add(scaled(column(W1, H, IN1, 2 * H)));
-      o.w0u = pk.add(scaled(column(W1, H, IN1, 2 * H + 1)));
-      o.tc3 = tcn::pack_blocks(R(p + "node_mlp.0.weight"), 2 * H, 2, tcblob, &o.d3);
-      o.tc4 = tcn::pack_blocks(R(p + "node_mlp.2.weight"), H, 1, tcblob, &o.d4);
-      o.wdmax = absmax(column(W1, H, IN1, 2 * H)); o.w0max = absmax(column(W1, H, IN1, 2 * H + 1));
+      const std::string p(buf);
+      GclW& w = e->gcl[l * S + s];
+      pack_gcl(pk, w, raw, p, 2 * H + 2);
+      pack_edge_mlp_denoiser(pk, w, raw, p + "edge_mlp.");
+      pk.add_tc(&w.W3_tc, tcn::pack_blocks(raw.at(p + "node_mlp.0.weight"), 2 * H, 2, pk.tc, &w.w3_descale));
+      pk.add_tc(&w.W4_tc, tcn::pack_blocks(raw.at(p + "node_mlp.2.weight"), H, 1, pk.tc, &w.w4_descale));
     }
-    snprintf(buf, sizeof(buf), "dynamics.e_block_%d.gcl_equiv.", l);
-    std::string p(buf);
-    GOff& o = eoff[l];
-    const auto& W1 = R(p + "coord_mlp.0.weight");
-    o.W1a = pk.add(transpose_block(W1, H, IN1, 0, H));
-    o.W1b = pk.add(transpose_block(W1, H, IN1, H, H));
-    o.b1 = pk.add(R(p + "coord_mlp.0.bias"));
-    o.wd = pk.add(column(W1, H, IN1, 2 * H));
-    o.w0 = pk.add(column(W1, H, IN1, 2 * H + 1));
-    o.W2 = pk.add(transpose_block(R(p + "coord_mlp.2.weight"), H, H, 0, H));
-    o.b2 = pk.add(R(p + "coord_mlp.2.bias"));
-    o.w5 = pk.add(R(p + "coord_mlp.4.weight"));
-    o.tc = tc::pack_w2(R(p + "coord_mlp.2.weight"), tcblob, &o.descale);
-    o.tc1 = tcn::pack_blocks(scaled(W1), IN1, 2, tcblob, &o.d1);
-    o.b1u = pk.add(scaled(R(p + "coord_mlp.0.bias")));
-    o.wdu = pk.add(scaled(column(W1, H, IN1, 2 * H)));
-    o.w0u = pk.add(scaled(column(W1, H, IN1, 2 * H + 1)));
-    o.wdmax = absmax(column(W1, H, IN1, 2 * H)); o.w0max = absmax(column(W1, H, IN1, 2 * H + 1));
+    snprintf(buf, sizeof(buf), "dynamics.e_block_%d.gcl_equiv.coord_mlp.", l);
+    const std::string p(buf);
+    EqW& q = e->eq[l];
+    pack_edge_mlp(pk, q, raw, p, 2 * H + 2);
+    pack_edge_mlp_denoiser(pk, q, raw, p);
+    pk.add(&q.w5, raw.at(p + "4.weight"));
   }
-  if (e->wblob) { cudaFree(e->wblob); e->wblob = nullptr; }
-  if (e->wblob_tc) { cudaFree(e->wblob_tc); e->wblob_tc = nullptr; }
-  CK(cudaMalloc((void**)&e->wblob, pk.blob.size() * sizeof(float)));
-  CK(cudaMemcpy(e->wblob, pk.blob.data(), pk.blob.size() * sizeof(float), cudaMemcpyHostToDevice));
-  CK(cudaMalloc(&e->wblob_tc, std::max<size_t>(tcblob.size(), 1) * sizeof(__half)));
-  CK(cudaMemcpy(e->wblob_tc, tcblob.data(), tcblob.size() * sizeof(__half), cudaMemcpyHostToDevice));
-  const float* base = e->wblob;
-  const __half* tbase = reinterpret_cast<const __half*>(e->wblob_tc);
-  e->We_t = base + oWe; e->be = base + obe; e->Wo = base + oWo; e->bo = base + obo;
-  e->gcl.assign(L * S, GclW{});
-  e->eq.assign(L, EqW{});
-  for (int i = 0; i < L * S; ++i) {
-    const GOff& o = goff[i];
-    e->gcl[i] = GclW{base + o.W1a, base + o.W1b, base + o.b1, base + o.wd, base + o.w0, base + o.W2, base + o.b2,
-                     base + o.W3,  base + o.b3,  base + o.W4, base + o.b4, tbase + o.tc, o.descale, o.wdmax, o.w0max,
-                     tbase + o.tc1, tbase + o.tc3, tbase + o.tc4, o.d1, o.d3, o.d4,
-                     base + o.b1u, base + o.wdu, base + o.w0u};
-  }
-  for (int l = 0; l < L; ++l) {
-    const GOff& o = eoff[l];
-    e->eq[l] = EqW{base + o.W1a, base + o.W1b, base + o.b1, base + o.wd, base + o.w0,
-                   base + o.W2,  base + o.b2,  base + o.w5, tbase + o.tc, o.descale, o.wdmax, o.w0max, tbase + o.tc1, o.d1,
-                   base + o.b1u, base + o.wdu, base + o.w0u};
-  }
+  dl_status s = upload_blob(pk.blob, &e->wblob);
+  if (s == DL_OK) s = upload_blob(pk.tc, &e->wblob_tc);
+  if (s != DL_OK) return s;
+  pk.point(e->wblob, e->wblob_tc);
   e->finalized = true;
   return DL_OK;
 }
@@ -689,7 +769,7 @@ dl_status dl_dynamics_forward(dl_engine* e, int32_t B, int32_t N, const float* t
   if ((s = ensure_workspace(e, B, N)) != DL_OK) return s;
   CK(cudaEventRecord(e->ev_t0, st));
   if (nan_flags) CK(cudaMemsetAsync(nan_flags, 0, B * sizeof(int32_t), st));
-  if ((s = build_plan(e, B, N, node_mask, linker_mask, edge_mask, st)) != DL_OK) return s;
+  if ((s = build_forward_plan(e, B, N, node_mask, linker_mask, edge_mask, st)) != DL_OK) return s;
   FwdIO io;
   io.xh = xh; io.t = t; io.t_numel = t_numel; io.out = out; io.node_mask = node_mask; io.linker_mask = linker_mask;
   io.edge_mask = edge_mask; io.context = context; io.nan_flags = nan_flags;
@@ -705,33 +785,19 @@ dl_status dl_dynamics_forward_host(dl_engine* e, int32_t B, int32_t N, const flo
   dl_status s = check_shapes(e, B, N);
   if (s != DL_OK) return s;
   CK(cudaSetDevice(e->cfg.device));
-  const size_t n = (size_t)B * N;
-  const int xd = 3 + e->cfg.in_node_nf, C = e->cfg.context_node_nf;
-  const size_t o_t = 0, o_xh = o_t + align256(sizeof(float) * std::max(t_numel, 1)), o_nm = o_xh + align256(n * xd * 4),
-               o_lm = o_nm + align256(n), o_em = o_lm + align256(n * 4), o_ctx = o_em + align256(n * N),
-               o_out = o_ctx + align256(n * std::max(C, 1) * 4), o_fl = o_out + align256(n * xd * 4),
-               total = o_fl + align256(B * 4);
-  if ((s = stage_reserve(e, total)) != DL_OK) return s;
-  char* d = e->stage.buf;
+  const size_t n = (size_t)B * N, xh_bytes = n * (3 + e->cfg.in_node_nf) * 4;
+  const bool fc_em = edge_mask && e->cfg.graph_type == DL_GRAPH_FC;
+  StageLayout sl;
+  const int i_t = sl.in(t, sizeof(float) * t_numel), i_xh = sl.in(xh, xh_bytes), i_nm = sl.in(node_mask, n),
+            i_lm = sl.in(linker_mask, n * 4), i_em = sl.in(fc_em ? edge_mask : nullptr, n * N),
+            i_ctx = sl.in(context, n * e->cfg.context_node_nf * 4), i_out = sl.out(xh_bytes), i_fl = sl.out(B * 4);
   cudaStream_t st = e->loop_stream;
-  if (t) CK(cudaMemcpyAsync(d + o_t, t, sizeof(float) * t_numel, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d + o_xh, xh, n * xd * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d + o_nm, node_mask, n, cudaMemcpyHostToDevice, st));
-  if (linker_mask) CK(cudaMemcpyAsync(d + o_lm, linker_mask, n * 4, cudaMemcpyHostToDevice, st));
-  if (edge_mask && e->cfg.graph_type == DL_GRAPH_FC) CK(cudaMemcpyAsync(d + o_em, edge_mask, n * N, cudaMemcpyHostToDevice, st));
-  if (context) CK(cudaMemcpyAsync(d + o_ctx, context, n * C * 4, cudaMemcpyHostToDevice, st));
-  s = dl_dynamics_forward(e, B, N, t ? (const float*)(d + o_t) : nullptr, t_numel, (const float*)(d + o_xh),
-                          (const int8_t*)(d + o_nm), linker_mask ? (const float*)(d + o_lm) : nullptr,
-                          (edge_mask && e->cfg.graph_type == DL_GRAPH_FC) ? (const int8_t*)(d + o_em) : nullptr,
-                          context ? (const float*)(d + o_ctx) : nullptr, (float*)(d + o_out), (int32_t*)(d + o_fl), st);
+  if ((s = stage_inputs(e, sl, st)) != DL_OK) return s;
+  s = dl_dynamics_forward(e, B, N, sl.at<const float>(i_t), t_numel, sl.at<const float>(i_xh), sl.at<const int8_t>(i_nm),
+                          sl.at<const float>(i_lm), sl.at<const int8_t>(i_em), sl.at<const float>(i_ctx),
+                          sl.at<float>(i_out), sl.at<int32_t>(i_fl), st);
   if (s != DL_OK) return s;
-  std::vector<int32_t> flags(B);
-  CK(cudaMemcpyAsync(out, d + o_out, n * xd * 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(flags.data(), d + o_fl, B * 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  bool any = false;
-  for (int i = 0; i < B; ++i) { any |= flags[i] != 0; if (nan_flags) nan_flags[i] = flags[i]; }
-  return any ? DL_NAN_DETECTED : DL_OK;
+  return stage_results(out, sl.at<float>(i_out), xh_bytes, sl.at<int32_t>(i_fl), B, nan_flags, st);
 }
 
 // torch's launch geometry for randn(numel) on this device (see NoiseRng)
@@ -776,12 +842,11 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
                               uint64_t offset, uint64_t* offset_consumed, const dl_step_coef* coef, const float* norm,
                               float* chain, int32_t* nan_flags, void* stream) {
   dl_status s = check_shapes(e, B, N);
+  if (s == DL_OK) s = check_slice(e, B);
   if (s != DL_OK) return s;
-  if (e->slice_B_full > 0 && e->slice_b0 + B > e->slice_B_full) { set_err("batch slice [%d, %d) exceeds the full batch %d", e->slice_b0, e->slice_b0 + B, e->slice_B_full); return DL_ERR_INVALID; }
   if (offset % 4 != 0) { set_err("philox offset must be a multiple of 4 (torch.Generator.get_offset())"); return DL_ERR_INVALID; }
   const NoiseRng q = make_rng(e, B, N, seed, offset);
-  const uint64_t n_draws = sampler == DL_SAMPLER_INPAINT ? (uint64_t)2 * T + 3 : (uint64_t)T + 2;
-  if (offset_consumed) *offset_consumed = n_draws * q.per_draw;
+  if (offset_consumed) *offset_consumed = sampler_draws(sampler, T) * q.per_draw;
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, nullptr,
                            &q, coef, norm, chain, nan_flags, stream);
 }
@@ -813,7 +878,7 @@ dl_status dl_noise_fill_inpaint(dl_engine* e, int32_t T, int32_t B, int32_t N, c
   if (s != DL_OK) return s;
   if (!node_mask || !fragment_mask || !out) { set_err("null argument"); return DL_ERR_INVALID; }
   if (T < 1 || 2 * T + 3 > 65535) { set_err("need 1 <= T <= 32766 (got %d)", T); return DL_ERR_INVALID; }
-  if (e->slice_B_full > 0 && e->slice_b0 + B > e->slice_B_full) { set_err("batch slice [%d, %d) exceeds the full batch %d", e->slice_b0, e->slice_b0 + B, e->slice_B_full); return DL_ERR_INVALID; }
+  if ((s = check_slice(e, B)) != DL_OK) return s;
   CK(cudaSetDevice(e->cfg.device));
   const NoiseRng q = make_rng(e, B, N, seed, offset);
   if (offset_consumed) *offset_consumed = (uint64_t)(2 * T + 3) * q.per_draw;
@@ -829,15 +894,10 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
                                    const float* noise, const NoiseRng* rng, const dl_step_coef* coef, const float* norm,
                                    float* chain, int32_t* nan_flags, void* stream) {
   dl_status s = check_shapes(e, B, N);
+  if (s == DL_OK) s = check_sampler(e, sampler, T, keep_frames, noise || rng, xh, node_mask, fragment_mask, linker_mask, context,
+                                    coef, norm, chain);
   if (s != DL_OK) return s;
-  if (sampler != DL_SAMPLER_LINKER && sampler != DL_SAMPLER_INPAINT) { set_err("unknown sampler %d", sampler); return DL_ERR_INVALID; }
   const bool inpaint = sampler == DL_SAMPLER_INPAINT;
-  if (inpaint != (e->cfg.centering != 0)) { set_err("the inpainting sampler needs a model built with centering=1 (and vice versa)"); return DL_ERR_INVALID; }
-  if (!xh || !node_mask || !fragment_mask || !linker_mask || (!noise && !rng) || !coef || !norm || !chain) {
-    set_err("null argument"); return DL_ERR_INVALID;
-  }
-  if (T < 1 || keep_frames < 1 || keep_frames > T) { set_err("need 1 <= keep_frames <= T"); return DL_ERR_INVALID; }
-  if (e->cfg.context_node_nf > 0 && !context) { set_err("context required"); return DL_ERR_INVALID; }
   static_assert(sizeof(dl_step_coef) == 32, "dl_step_coef layout");
   CK(cudaSetDevice(e->cfg.device));
   cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
@@ -879,7 +939,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     e->launches += 1;
   }
   // inpainting: the dynamics see linker_mask=None (edm.py:632), so every live row gets a coordinate update
-  if ((s = build_plan(e, B, N, node_mask, inpaint ? nullptr : linker_mask, edge_mask, st)) != DL_OK) return s;
+  if ((s = build_forward_plan(e, B, N, node_mask, inpaint ? nullptr : linker_mask, edge_mask, st)) != DL_OK) return s;
 
   if (time_chain) { cudaStreamSynchronize(st); tc_plan = now_ms(); }
   FwdIO io;
@@ -940,42 +1000,24 @@ dl_status dl_sample_chain_host(dl_engine* e, int32_t sampler, int32_t B, int32_t
                                const float* noise, const dl_step_coef* coef, const float* norm, float* chain,
                                int32_t* nan_flags) {
   dl_status s = check_shapes(e, B, N);
+  if (s == DL_OK) s = check_sampler(e, sampler, T, keep_frames, noise != nullptr, xh, node_mask, fragment_mask, linker_mask,
+                                    context, coef, norm, chain);
   if (s != DL_OK) return s;
-  if (!xh || !node_mask || !fragment_mask || !linker_mask || !noise || !coef || !norm || !chain) {
-    set_err("null argument"); return DL_ERR_INVALID;
-  }
-  if (T < 1 || keep_frames < 1 || keep_frames > T) { set_err("need 1 <= keep_frames <= T"); return DL_ERR_INVALID; }
   CK(cudaSetDevice(e->cfg.device));
-  const size_t n = (size_t)B * N;
-  const int xd = 3 + e->cfg.in_node_nf, C = e->cfg.context_node_nf;
-  const bool has_em = edge_mask && e->cfg.graph_type == DL_GRAPH_FC;
-  const size_t n_slabs = sampler == DL_SAMPLER_INPAINT ? (size_t)2 * T + 3 : (size_t)T + 2;
-  const size_t o_xh = 0, o_nm = o_xh + align256(n * xd * 4), o_fm = o_nm + align256(n), o_lm = o_fm + align256(n * 4),
-               o_em = o_lm + align256(n * 4), o_ctx = o_em + align256(has_em ? n * N : 1),
-               o_nz = o_ctx + align256(n * std::max(C, 1) * 4), o_ch = o_nz + align256((size_t)n_slabs * n * xd * 4),
-               o_fl = o_ch + align256((size_t)keep_frames * n * xd * 4), total = o_fl + align256(B * 4);
-  if ((s = stage_reserve(e, total)) != DL_OK) return s;
-  char* d = e->stage.buf;
+  const size_t n = (size_t)B * N, frame_bytes = n * (3 + e->cfg.in_node_nf) * 4;
+  const bool fc_em = edge_mask && e->cfg.graph_type == DL_GRAPH_FC;
+  StageLayout sl;
+  const int i_xh = sl.in(xh, frame_bytes), i_nm = sl.in(node_mask, n), i_fm = sl.in(fragment_mask, n * 4),
+            i_lm = sl.in(linker_mask, n * 4), i_em = sl.in(fc_em ? edge_mask : nullptr, n * N),
+            i_ctx = sl.in(context, n * e->cfg.context_node_nf * 4), i_nz = sl.in(noise, sampler_draws(sampler, T) * frame_bytes),
+            i_ch = sl.out(keep_frames * frame_bytes), i_fl = sl.out(B * 4);
   cudaStream_t st = e->loop_stream;
-  CK(cudaMemcpyAsync(d + o_xh, xh, n * xd * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d + o_nm, node_mask, n, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d + o_fm, fragment_mask, n * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d + o_lm, linker_mask, n * 4, cudaMemcpyHostToDevice, st));
-  if (has_em) CK(cudaMemcpyAsync(d + o_em, edge_mask, n * N, cudaMemcpyHostToDevice, st));
-  if (context) CK(cudaMemcpyAsync(d + o_ctx, context, n * C * 4, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d + o_nz, noise, n_slabs * n * xd * 4, cudaMemcpyHostToDevice, st));
-  s = dl_sample_chain(e, sampler, B, N, T, keep_frames, (const float*)(d + o_xh), (const int8_t*)(d + o_nm),
-                      (const float*)(d + o_fm), (const float*)(d + o_lm), has_em ? (const int8_t*)(d + o_em) : nullptr,
-                      context ? (const float*)(d + o_ctx) : nullptr, (const float*)(d + o_nz), coef, norm,
-                      (float*)(d + o_ch), (int32_t*)(d + o_fl), st);
+  if ((s = stage_inputs(e, sl, st)) != DL_OK) return s;
+  s = dl_sample_chain(e, sampler, B, N, T, keep_frames, sl.at<const float>(i_xh), sl.at<const int8_t>(i_nm),
+                      sl.at<const float>(i_fm), sl.at<const float>(i_lm), sl.at<const int8_t>(i_em), sl.at<const float>(i_ctx),
+                      sl.at<const float>(i_nz), coef, norm, sl.at<float>(i_ch), sl.at<int32_t>(i_fl), st);
   if (s != DL_OK) return s;
-  std::vector<int32_t> flags(B);
-  CK(cudaMemcpyAsync(chain, d + o_ch, (size_t)keep_frames * n * xd * 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(flags.data(), d + o_fl, B * 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  bool any = false;
-  for (int i = 0; i < B; ++i) { any |= flags[i] != 0; if (nan_flags) nan_flags[i] = flags[i]; }
-  return any ? DL_NAN_DETECTED : DL_OK;
+  return stage_results(chain, sl.at<float>(i_ch), keep_frames * frame_bytes, sl.at<int32_t>(i_fl), B, nan_flags, st);
 }
 
 int64_t dl_launch_count(const dl_engine* e) { return e ? e->launches : 0; }
@@ -1017,15 +1059,10 @@ dl_status dl_cut_graph_stats(dl_engine* e, int64_t* out) {
 float dl_time_edge_kernel(dl_engine* e, int32_t reps) {
   if (!e || !e->finalized || e->last_B == 0 || reps < 1) { set_err("dl_time_edge_kernel: no previous forward"); return -1.f; }
   if (cudaSetDevice(e->cfg.device) != cudaSuccess) return -1.f;
-  Workspace& ws = e->ws;
   const Geom gm = make_geom(e, e->last_B, e->last_N);
   const GclW& w = e->gcl[0];
-  EdgeArgs ea{};
-  const float ksc = e->use_tc ? 1.4426950408889634f : 1.0f;
-  ea.AB = ws.ABg; ea.ABmax = ws.ABgmax; ea.w2_descale = w.w2_descale; ea.wdmax = w.wdmax * ksc; ea.w0max = w.w0max * ksc;
-  ea.x = ws.xa; ea.x0 = ws.x0; ea.x4 = ws.xa4; ea.x04 = ws.x04; ea.x4_out = nullptr; ea.edge_mask = e->last_edge_mask; ea.cls = ws.cls; ea.nm = ws.nm;
-  ea.linker_mask = e->last_linker_mask; ea.W2_t = w.W2_t; ea.b2 = w.b2; ea.wd = e->use_tc ? w.wd_u : w.wd; ea.w0 = e->use_tc ? w.w0_u : w.w0; ea.w5 = nullptr;
-  ea.plan = make_plan(ws); ea.agg = ws.agg; ea.x_out = nullptr; ea.nbr = ws.nbr; ea.recs = ws.recs; ea.n_recs = ws.n_recs;
+  // the forward's first GCL launch: block 0 reads the coordinates from ws.xa
+  const EdgeArgs ea = edge_args(e, w, false, e->last_edge_mask, e->last_linker_mask, e->ws.xa, e->ws.xa4);
   cudaStream_t st = e->loop_stream;
   for (int i = 0; i < 2; ++i) if (launch_edge(e, gm, ea, false, w.W2_tc, st) != DL_OK) return -1.f;
   if (cudaEventRecord(e->ev_t0, st) != cudaSuccess) return -1.f;

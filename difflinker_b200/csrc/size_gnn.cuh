@@ -16,7 +16,7 @@ struct dl_sizegnn {
   std::map<std::string, std::vector<float>> raw;
   float* wblob = nullptr;
   std::vector<GclW> layers;
-  const float *We_t = nullptr, *be = nullptr, *Wo = nullptr, *bo = nullptr, *zeros = nullptr;
+  const float *We_t = nullptr, *be = nullptr, *Wo = nullptr, *bo = nullptr;
   Workspace ws;
   int64_t launches = 0;
 };
@@ -123,46 +123,24 @@ dl_status dl_sizegnn_finalize_weights(dl_sizegnn* e) {
   CK(cudaSetDevice(e->cfg.device));
   for (auto& p : sz_expected_params(e->cfg))
     if (!e->raw.count(p.name)) { set_err("missing weight %s", p.name.c_str()); return DL_ERR_WEIGHTS; }
-  const int L = e->cfg.n_layers, F_in = e->cfg.in_node_nf, IN1 = 2 * H + 1;
+  const int L = e->cfg.n_layers, F_in = e->cfg.in_node_nf;
+  const RawWeights& raw = e->raw;
   Packer pk;
-  auto R = [&](const std::string& k) -> const std::vector<float>& { return e->raw[k]; };
-  struct Off { size_t W1a, W1b, b1, wd, W2, b2, W3, b3, W4, b4; };
-  std::vector<Off> off(L);
-  const size_t oWe = pk.add(transpose_block(R("embedding_in.weight"), H, F_in, 0, F_in));
-  const size_t obe = pk.add(R("embedding_in.bias"));
-  const size_t oWo = pk.add(R("embedding_out.weight"));
-  const size_t obo = pk.add(R("embedding_out.bias"));
-  const size_t oz = pk.add(std::vector<float>(H, 0.f));
+  e->layers.assign(L, GclW{});
+  pk.add(&e->We_t, transpose_block(raw.at("embedding_in.weight"), H, F_in, 0, F_in));
+  pk.add(&e->be, raw.at("embedding_in.bias"));
+  pk.add(&e->Wo, raw.at("embedding_out.weight"));
+  pk.add(&e->bo, raw.at("embedding_out.bias"));
   char buf[64];
   for (int l = 0; l < L; ++l) {
     snprintf(buf, sizeof(buf), "layer%d.", l);
-    std::string p(buf);
-    const auto& W1 = R(p + "edge_mlp.0.weight");
-    Off& o = off[l];
-    o.W1a = pk.add(transpose_block(W1, H, IN1, 0, H));
-    o.W1b = pk.add(transpose_block(W1, H, IN1, H, H));
-    o.b1 = pk.add(R(p + "edge_mlp.0.bias"));
-    o.wd = pk.add(column(W1, H, IN1, 2 * H));
-    o.W2 = pk.add(transpose_block(R(p + "edge_mlp.2.weight"), H, H, 0, H));
-    o.b2 = pk.add(R(p + "edge_mlp.2.bias"));
-    o.W3 = pk.add(transpose_block(R(p + "node_mlp.0.weight"), H, 2 * H, 0, 2 * H));
-    o.b3 = pk.add(R(p + "node_mlp.0.bias"));
-    o.W4 = pk.add(transpose_block(R(p + "node_mlp.2.weight"), H, H, 0, H));
-    o.b4 = pk.add(R(p + "node_mlp.2.bias"));
+    GclW& w = e->layers[l];
+    pack_gcl(pk, w, raw, buf, 2 * H + 1);
+    pk.add(&w.w0, std::vector<float>(H, 0.f));   // no input-distance column
   }
-  if (e->wblob) { cudaFree(e->wblob); e->wblob = nullptr; }
-  CK(cudaMalloc((void**)&e->wblob, pk.blob.size() * sizeof(float)));
-  CK(cudaMemcpy(e->wblob, pk.blob.data(), pk.blob.size() * sizeof(float), cudaMemcpyHostToDevice));
-  const float* base = e->wblob;
-  e->We_t = base + oWe; e->be = base + obe; e->Wo = base + oWo; e->bo = base + obo; e->zeros = base + oz;
-  e->layers.assign(L, GclW{});
-  for (int l = 0; l < L; ++l) {
-    const Off& o = off[l];
-    GclW w{};
-    w.W1a_t = base + o.W1a; w.W1b_t = base + o.W1b; w.b1 = base + o.b1; w.wd = base + o.wd; w.w0 = e->zeros;
-    w.W2_t = base + o.W2; w.b2 = base + o.b2; w.W3_t = base + o.W3; w.b3 = base + o.b3; w.W4_t = base + o.W4; w.b4 = base + o.b4;
-    e->layers[l] = w;
-  }
+  const dl_status s = upload_blob(pk.blob, &e->wblob);
+  if (s != DL_OK) return s;
+  pk.point(e->wblob, nullptr);
   e->finalized = true;
   return DL_OK;
 }
@@ -181,28 +159,19 @@ dl_status dl_sizegnn_forward(dl_sizegnn* e, int32_t B, int32_t N, const float* x
   gm.B = B; gm.N = N; gm.F = e->cfg.in_node_nf; gm.C = 0; gm.D = e->cfg.in_node_nf;
   gm.graph_type = 4; gm.norm_constant = 0.f; gm.normalization_factor = 1.f;
 
-  CK(cudaMemsetAsync(ws.agg, 0, (size_t)n * H * sizeof(float), st));     // rows without a live edge aggregate to exactly 0
-  k_plan_mol<<<B, 256, 2 * N * sizeof(int), st>>>(N, gm.graph_type, edge_mask, fragment_mask, nullptr, ws.rowidx, ws.colidx,
-                                                  ws.xrowidx, ws.nr, ws.nc, ws.nxr);
-  LAUNCH_CHECK();
-  k_plan_items<<<1, 1, 0, st>>>(B, ET, MAXR, 1, MAXR, ws.nr, ws.nc, ws.nxr, ws.items, ws.n_items, ws.xmols, ws.n_xmols, ws.xitems,
-                                ws.n_xitems);
-  LAUNCH_CHECK();
+  if ((s = build_plan(ws, B, N, gm.graph_type, fragment_mask, nullptr, edge_mask, ET, MAXR, st)) != DL_OK) return s;
 
   const int node_blocks = (n + NODE_TM - 1) / NODE_TM;
   PrepArgs pa{};
   pa.xh = xh; pa.node_mask = fragment_mask; pa.linker_mask = nullptr; pa.t = nullptr; pa.t_numel = 0; pa.context = nullptr;
   pa.We_t = e->We_t; pa.be = e->be;
-  pa.proj = ProjW{e->layers[0].W1a_t, e->layers[0].W1b_t, e->layers[0].b1};
+  pa.proj = proj_of(e->layers[0]);
   pa.nm = ws.nm; pa.x0 = ws.x0; pa.x = ws.xa; pa.x04 = nullptr; pa.x4 = nullptr; pa.cls = ws.cls; pa.h = ws.h;
   pa.AB = ws.ABg; pa.ABmax = ws.ABgmax;
   k_prep<<<node_blocks, 256, 0, st>>>(gm, pa);
   LAUNCH_CHECK();
 
-  Plan plan{};
-  plan.rowidx = ws.rowidx; plan.colidx = ws.colidx; plan.xrowidx = ws.xrowidx; plan.nr = ws.nr; plan.nc = ws.nc; plan.nxr = ws.nxr;
-  plan.items = ws.items; plan.n_items = ws.n_items; plan.xmols = ws.xmols; plan.n_xmols = ws.n_xmols;
-  plan.xitems = ws.xitems; plan.n_xitems = ws.n_xitems;
+  const Plan plan = make_plan(ws);
   const size_t node_smem = 3 * NODE_TM * LDX * sizeof(float);
   for (int l = 0; l < L; ++l) {
     const GclW& w = e->layers[l];
@@ -214,8 +183,7 @@ dl_status dl_sizegnn_forward(dl_sizegnn* e, int32_t B, int32_t N, const float* x
     NodeArgs na{};
     na.h = ws.h; na.agg = ws.agg; na.nm = ws.nm; na.W3_t = w.W3_t; na.b3 = w.b3; na.W4_t = w.W4_t; na.b4 = w.b4;
     if (l + 1 < L) {
-      const GclW& nx = e->layers[l + 1];
-      na.proj1 = ProjW{nx.W1a_t, nx.W1b_t, nx.b1}; na.AB1 = ws.ABg; na.ABmax1 = ws.ABgmax;
+      na.proj1 = proj_of(e->layers[l + 1]); na.AB1 = ws.ABg; na.ABmax1 = ws.ABgmax;
     }
     k_node<ACT_RELU><<<node_blocks, 256, node_smem, st>>>(n, na);
     LAUNCH_CHECK();

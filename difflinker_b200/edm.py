@@ -93,6 +93,21 @@ class EDM(torch.nn.Module):
     def unnormalize(self, x, h):
         return x * self.norm_values[0], h * self.norm_values[1] + self.norm_biases[1]
 
+    def _cpu_gamma(self):
+        """The noise schedule as a CPU module: the coefficients are evaluated on the CPU whatever the model's device."""
+        gamma = PredefinedNoiseSchedule.__new__(PredefinedNoiseSchedule)
+        torch.nn.Module.__init__(gamma)
+        gamma.timesteps = self.gamma.timesteps
+        gamma.gamma = torch.nn.Parameter(self.gamma.gamma.detach().cpu(), requires_grad=False)
+        return gamma
+
+    def _q_coefficients(self, g_s, sigma_s, sigma_t, sigma2_ts, alpha_ts):
+        """(qa, qb) of a reverse step: the linker sampler does not re-noise known atoms."""
+        return 0.0, 0.0
+
+    def _final_qa(self, g0):
+        return 0.0
+
     def step_coefficients(self, keep_frames, n_samples=1):
         """(T+1) rows of dl_step_coef: row r is reverse step s = T-1-r (edm.py:146-163, 178-208); row T is the
         final p(x,h|z_0) step (edm.py:210-235).  Evaluated on (n_samples,1) fp32 CPU tensors exactly as the
@@ -102,10 +117,7 @@ class EDM(torch.nn.Module):
         key = (T, keep_frames, n_samples, self.gamma.gamma._version, self.gamma.gamma.data_ptr())
         if getattr(self, '_coef_cache', None) is not None and self._coef_cache[0] == key:
             return self._coef_cache[1]
-        gamma = PredefinedNoiseSchedule.__new__(PredefinedNoiseSchedule)
-        torch.nn.Module.__init__(gamma)
-        gamma.timesteps = self.gamma.timesteps
-        gamma.gamma = torch.nn.Parameter(self.gamma.gamma.detach().cpu(), requires_grad=False)
+        gamma = self._cpu_gamma()
         rows = (_native.DLStepCoef * (T + 1))()
         for r in range(T):
             s = T - 1 - r
@@ -117,15 +129,16 @@ class EDM(torch.nn.Module):
             sigma_s, sigma_t = self.sigma(g_s), self.sigma(g_t)
             b = sigma2_ts / alpha_ts / sigma_t       # edm.py:199
             c = sigma_ts * sigma_s / sigma_t         # edm.py:202
+            qa, qb = self._q_coefficients(g_s, sigma_s, sigma_t, sigma2_ts, alpha_ts)
             frame = (s * keep_frames) // T
             # only the last writer of a frame matters; frame 0 is finally overwritten by chain[0] (edm.py:174)
             last_writer = frame > 0 and (s == 0 or ((s - 1) * keep_frames) // T != frame)
             rows[r] = _native.DLStepCoef(float(t_arr[0]), float(alpha_ts[0]), float(b[0]), float(c[0]),
-                                         frame if last_writer else -1, 0.0, 0.0, 0.0)
+                                         frame if last_writer else -1, qa, qb, 0.0)
         g0 = gamma(torch.zeros(size=(n_samples, 1)))
         inv_alpha0 = 1. / self.alpha(g0)
         rows[T] = _native.DLStepCoef(0.0, float(inv_alpha0[0]), float(self.sigma(g0)[0]),
-                                     float(self.SNR(-0.5 * g0)[0]), -1, 0.0, 0.0, 0.0)
+                                     float(self.SNR(-0.5 * g0)[0]), -1, self._final_qa(g0), 0.0, 0.0)
         self._coef_cache = (key, rows)
         return rows
 
@@ -143,6 +156,19 @@ class EDM(torch.nn.Module):
             torch.randn((n_samples, n_nodes, self.n_dims), generator=generator, out=zx[r])
             torch.randn((n_samples, n_nodes, self.in_node_nf), generator=generator, out=zh[r])
         return torch.cat([zx, zh], dim=3)
+
+    # ---- what the two samplers differ in: the device sampler, the number of draws and how a noise tensor is drawn ----
+    _SAMPLER = _native.SAMPLER_LINKER
+
+    def _n_draws(self):
+        return self.T + 2
+
+    def _draw_tensor(self, n_samples, n_nodes, device, node_mask, fragment_mask):
+        return self.draw_noise(self.T + 2, n_samples, n_nodes, device)
+
+    def _draws_replaced(self):
+        """A draw_noise replaced on the instance supplies the draws instead of the device-side stream."""
+        return 'draw_noise' in self.__dict__
 
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
@@ -162,16 +188,16 @@ class EDM(torch.nn.Module):
         d = self.n_dims + self.in_node_nf
         xn, hn = self.normalize(x, h)
         xh = torch.cat([xn, hn], dim=2).to(torch.float32).contiguous()
-        # device-side stream unless a tensor is injected (tests), draw_noise is overridden on the instance, or another mode is set
+        # device-side stream unless a tensor is injected (tests), the draw function is replaced, or another mode is set
         on_device = (noise is None and dev.type == 'cuda' and self.noise_mode == 'reference_stream'
-                     and 'draw_noise' not in self.__dict__)
+                     and not self._draws_replaced())
         if batch_slice is not None and not on_device:
             raise ValueError("batch_slice needs the device-side noise stream (CUDA tensors, noise_mode='reference_stream')")
         if not on_device:
             if noise is None:
-                noise = self.draw_noise(T + 2, n_samples, n_nodes, dev)
+                noise = self._draw_tensor(n_samples, n_nodes, dev, node_mask, fragment_mask)
             noise = noise.to(device=dev, dtype=torch.float32).contiguous()
-            assert noise.shape == (T + 2, n_samples, n_nodes, d), noise.shape
+            assert noise.shape == (self._n_draws(), n_samples, n_nodes, d), noise.shape
 
         eng = self.dynamics.engine(self.dynamics._device_index(x))
         self.dynamics._check_graph_type()
@@ -190,23 +216,18 @@ class EDM(torch.nn.Module):
         chain = torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32)
         flags = torch.zeros(n_samples, dtype=torch.int32, device=dev)
         ptr = lambda v: None if v is None else v.data_ptr()
+        head = (self._SAMPLER, n_samples, n_nodes, T, keep_frames, ptr(xh), ptr(nm), ptr(fm), ptr(lm), ptr(em), ptr(ctx))
+        tail = (coef, norm, ptr(chain), ptr(flags))
         if dev.type == 'cuda':
             with torch.cuda.device(dev):
                 stream = torch.cuda.current_stream(dev).cuda_stream
                 if on_device:
-                    _sample_chain_rng(lib, eng, dev, batch_slice,
-                                      (_native.SAMPLER_LINKER, n_samples, n_nodes, T, keep_frames, ptr(xh), ptr(nm), ptr(fm),
-                                       ptr(lm), ptr(em), ptr(ctx)), (coef, norm, ptr(chain), ptr(flags), stream))
+                    _sample_chain_rng(lib, eng, dev, batch_slice, head, tail + (stream,))
                 else:
-                    st = lib.dl_sample_chain(eng, _native.SAMPLER_LINKER, n_samples, n_nodes, T, keep_frames, ptr(xh),
-                                             ptr(nm), ptr(fm), ptr(lm), ptr(em), ptr(ctx), ptr(noise), coef, norm,
-                                             ptr(chain), ptr(flags), stream)
-                    _native.check(st, "dl_sample_chain")
+                    _native.check(lib.dl_sample_chain(eng, *head, ptr(noise), *tail, stream), "dl_sample_chain")
                 bad = bool(flags.any().item())   # one sync per chain instead of one per step (egnn.py:441)
         else:
-            st = lib.dl_sample_chain_host(eng, _native.SAMPLER_LINKER, n_samples, n_nodes, T, keep_frames, ptr(xh),
-                                          ptr(nm), ptr(fm), ptr(lm), ptr(em), ptr(ctx), ptr(noise), coef, norm,
-                                          ptr(chain), ptr(flags))
+            st = lib.dl_sample_chain_host(eng, *head, ptr(noise), *tail)
             _native.check(st, "dl_sample_chain_host")
             bad = st == _native.DL_NAN_DETECTED
         self.last_loop_ms = float(lib.dl_last_elapsed_ms(eng))
@@ -220,6 +241,7 @@ class InpaintingEDM(EDM):
     (`linker_mask=None`, dynamics built with centering=True), fragment atoms are then re-noised from the known
     fragments with q(z_s | z_t, x), and the centre of mass is projected out every step.
     NB the reference's positional order differs from EDM.sample_chain (edge_mask comes third): call by keyword."""
+    _SAMPLER = _native.SAMPLER_INPAINT
 
     @staticmethod
     def _com_free(x, mask):
@@ -239,98 +261,35 @@ class InpaintingEDM(EDM):
             out[r, :, :, nd:] = torch.randn((n_samples, n_nodes, nf), device=device, generator=generator) * m
         return out
 
-    def step_coefficients(self, keep_frames, n_samples=1):
-        rows = super().step_coefficients(keep_frames, n_samples)
-        if getattr(self, '_qcoef_key', None) == self._coef_cache[0]:
-            return rows
-        T = self.T
-        gamma = PredefinedNoiseSchedule.__new__(PredefinedNoiseSchedule)
-        torch.nn.Module.__init__(gamma)
-        gamma.timesteps = self.gamma.timesteps
-        gamma.gamma = torch.nn.Parameter(self.gamma.gamma.detach().cpu(), requires_grad=False)
-        for r in range(T):
-            s = T - 1 - r
-            s_arr = torch.full((n_samples, 1), fill_value=s)
-            t_arr = (s_arr + 1) / T
-            s_arr = s_arr / T
-            g_s, g_t = gamma(s_arr), gamma(t_arr)
-            sigma2_ts, _, alpha_ts = self.sigma_and_alpha_t_given_s(g_t, g_s)
-            sigma_s, sigma_t, alpha_s = self.sigma(g_s), self.sigma(g_t), self.alpha(g_s)
-            rows[r].qa = float((alpha_ts * (sigma_s ** 2) / (sigma_t ** 2))[0])      # edm.py:661-664
-            rows[r].qb = float((alpha_s * sigma2_ts / (sigma_t ** 2))[0])
-            # the chain frame is written after the COM projection by the per-molecule kernel; frame 0 is left to the final
-            # step, which overwrites chain[0] with the sampled x, h (edm.py:716-725) -- hence `frame > 0`
-            frame = (s * keep_frames) // T
-            last_writer = (s == 0 or ((s - 1) * keep_frames) // T != frame) and frame > 0
-            rows[r].frame = frame if last_writer else -1
-        g0 = gamma(torch.zeros(size=(n_samples, 1)))
-        rows[T].qa = float((self.sigma(g0) / self.alpha(g0))[0])                      # edm.py:716
-        self._qcoef_key = self._coef_cache[0]
-        return rows
+    def _q_coefficients(self, g_s, sigma_s, sigma_t, sigma2_ts, alpha_ts):
+        """q(z_s | z_t, x), which re-noises the fragment atoms from the known fragments (edm.py:661-664)."""
+        qa = float((alpha_ts * (sigma_s ** 2) / (sigma_t ** 2))[0])
+        qb = float((self.alpha(g_s) * sigma2_ts / (sigma_t ** 2))[0])
+        return qa, qb
 
-    @torch.no_grad()
+    def _final_qa(self, g0):
+        return float((self.sigma(g0) / self.alpha(g0))[0])                         # edm.py:716
+
+    def _n_draws(self):
+        return 2 * self.T + 3
+
+    def _draw_tensor(self, n_samples, n_nodes, device, node_mask, fragment_mask):
+        return self.draw_noise_inpaint(n_samples, n_nodes, device, node_mask, fragment_mask)
+
+    def _draws_replaced(self):
+        """draw_noise_inpaint replaced on the instance, in a subclass or on the class supplies the draws."""
+        return 'draw_noise_inpaint' in self.__dict__ or type(self).draw_noise_inpaint is not _DRAW_NOISE_INPAINT
+
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
                      noise=None, batch_slice=None):
-        """`noise` optionally injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA
-        and with noise_mode 'reference_stream', the draws are made inside the kernels from the default generator's state
+        """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
+        injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
+        'reference_stream', the draws are made inside the kernels from the default generator's state
         (dl_sample_chain_rng), unless `draw_noise_inpaint` is replaced -- on the instance, in a subclass or on the class --
         in which case the replacement draws them. `batch_slice=(b0, B_full)` as in EDM.sample_chain."""
-        lib = _native.load_library()
-        n_samples, n_nodes = x.size(0), x.size(1)
-        dev = x.device
-        T = self.T
-        if keep_frames is None:
-            keep_frames = T
-        else:
-            assert keep_frames <= T
-        d = self.n_dims + self.in_node_nf
-        xn, hn = self.normalize(x, h)
-        xh = torch.cat([xn, hn], dim=2).to(torch.float32).contiguous()
-        on_device = (noise is None and dev.type == 'cuda' and self.noise_mode == 'reference_stream'
-                     and 'draw_noise_inpaint' not in self.__dict__
-                     and type(self).draw_noise_inpaint is _DRAW_NOISE_INPAINT)
-        if batch_slice is not None and not on_device:
-            raise ValueError("batch_slice needs the device-side noise stream (CUDA tensors, noise_mode='reference_stream')")
-        if not on_device:
-            if noise is None:
-                noise = self.draw_noise_inpaint(n_samples, n_nodes, dev, node_mask, fragment_mask)
-            noise = noise.to(device=dev, dtype=torch.float32).contiguous()
-            assert noise.shape == (2 * T + 3, n_samples, n_nodes, d), noise.shape
-        eng = self.dynamics.engine(self.dynamics._device_index(x))
-        self.dynamics._check_graph_type()
-        prep = lambda v, dt: None if v is None else v.detach().to(device=dev, dtype=dt).contiguous()
-        nm = prep(node_mask.reshape(n_samples, n_nodes), torch.int8)
-        fm = prep(fragment_mask.reshape(n_samples, n_nodes), torch.float32)
-        lm = prep(linker_mask.reshape(n_samples, n_nodes), torch.float32)
-        em = None
-        if self.dynamics.graph_type == 'FC' and edge_mask is not None:
-            em = prep(edge_mask.reshape(-1), torch.int8)
-        ctx = None if context is None else prep(
-            context.reshape(n_samples, n_nodes, self.dynamics.context_node_nf), torch.float32)   # wrong width -> raises
-        coef = self.step_coefficients(keep_frames, n_samples)
-        norm = (C.c_float * 3)(float(self.norm_values[0]), float(self.norm_values[1]), float(self.norm_biases[1]))
-        chain = torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32)
-        flags = torch.zeros(n_samples, dtype=torch.int32, device=dev)
-        ptr = lambda v: None if v is None else v.data_ptr()
-        head = (_native.SAMPLER_INPAINT, n_samples, n_nodes, T, keep_frames, ptr(xh), ptr(nm), ptr(fm), ptr(lm), ptr(em),
-                ptr(ctx))
-        tail = (coef, norm, ptr(chain), ptr(flags))
-        if dev.type == 'cuda':
-            with torch.cuda.device(dev):
-                stream = torch.cuda.current_stream(dev).cuda_stream
-                if on_device:
-                    _sample_chain_rng(lib, eng, dev, batch_slice, head, tail + (stream,))
-                else:
-                    _native.check(lib.dl_sample_chain(eng, *head, ptr(noise), *tail, stream), "dl_sample_chain")
-                bad = bool(flags.any().item())
-        else:
-            st = lib.dl_sample_chain_host(eng, *head, ptr(noise), *tail)
-            _native.check(st, "dl_sample_chain_host")
-            bad = st == _native.DL_NAN_DETECTED
-        self.last_loop_ms = float(lib.dl_last_elapsed_ms(eng))
-        if bad:
-            raise nan_exception_class()(flags=flags.cpu().tolist())
-        return chain
+        return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
+                                    edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
+                                    batch_slice=batch_slice)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path
