@@ -9,6 +9,8 @@ DL_OK, DL_NAN_DETECTED = 0, 1
 GRAPH_TYPES = {"FC": 0, "4A": 1, "FC-4A": 2, "FC-10A-4A": 3}
 EDGE_IMPLS = {"auto": 0, "simt": 1, "wgmma": 2}
 SAMPLER_LINKER, SAMPLER_INPAINT = 0, 1
+AGGREGATIONS = {"sum": 0, "mean": 1}
+COORDS_RANGE = 15.0   # EGNN hands its own coords_range=15 to every EquivariantBlock (src/egnn.py:183,209)
 
 
 class DLConfig(C.Structure):
@@ -17,6 +19,14 @@ class DLConfig(C.Structure):
                 ("condition_time", C.c_int32), ("centering", C.c_int32), ("graph_type", C.c_int32),
                 ("device", C.c_int32), ("edge_impl", C.c_int32), ("norm_constant", C.c_float),
                 ("normalization_factor", C.c_float)]
+
+
+class DLEgnnOptions(C.Structure):
+    _fields_ = [("tanh", C.c_int32), ("coords_range", C.c_float), ("sin_embedding", C.c_int32),
+                ("aggregation", C.c_int32)]
+
+    def is_default(self):
+        return bytes(self) == bytes(DLEgnnOptions(0, COORDS_RANGE, 0, AGGREGATIONS["sum"]))
 
 
 class DLSizeGNNConfig(C.Structure):
@@ -35,6 +45,7 @@ SYMBOLS = {
     "dl_version": (C.c_char_p, []),
     "dl_last_error": (C.c_char_p, []),
     "dl_create": (_I32, [C.POINTER(DLConfig), C.POINTER(_P)]),
+    "dl_create_ex": (_I32, [C.POINTER(DLConfig), C.POINTER(DLEgnnOptions), C.POINTER(_P)]),
     "dl_destroy": (_I32, [_P]),
     "dl_set_weight": (_I32, [_P, C.c_char_p, _P, _I64]),
     "dl_finalize_weights": (_I32, [_P]),

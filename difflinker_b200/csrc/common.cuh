@@ -9,6 +9,23 @@ constexpr int H = 128;         // hidden_nf (configs/*.yml `nf: 128`), compile-t
 constexpr int MAX_DIN = 32;    // F + C + 1 upper bound
 constexpr int MAX_XHD = 16;    // 3 + F upper bound (threads per node in k_finish)
 
+// EGNN options of the edge kernels (template bits, dl_egnn_options): each set of options is its own instantiation, so the
+// default model's kernels carry no branch for them.
+constexpr int OPT_TANH = 1;    // coordinate update trans = coord_diff * tanh(phi) * coords_range (egnn.py:104-105)
+constexpr int OPT_MEAN = 2;    // aggregation_method='mean': divide by the row's edge count in the reference's edge list
+                               // (egnn.py:315-319): N for FC graphs, the cut-off degree (0 -> 1) otherwise
+constexpr int OPT_SIN = 4;     // sin_embedding: the two distance columns of every edge MLP's first layer become the 24
+                               // features [sin, cos](sqrt(r + 1e-8) f_k) of both radials (SinusoidsEmbeddingNew, egnn.py:281-292)
+constexpr int N_SIN_FREQ = 6;  // f_k = 2 pi 4^k / 15 (max_res 15, min_res 15/2000, div_factor 4)
+constexpr int N_SIN_FEAT = 4 * N_SIN_FREQ;
+// The fp32 values torch computes for 2 * math.pi * 4 ** torch.arange(6) / 15: exact power-of-4 multiples of f_0.
+__device__ __forceinline__ float sin_freq(int k) { return __int_as_float(__float_as_int(0x1.aceeap-2f) + (k << 24)); }
+// sqrt(r + 1e-8) * f_k in the reference's rounding order (no contraction); r itself must be (dx^2 + dy^2) + dz^2, each rounded
+__device__ __forceinline__ float sin_arg(float r, int k) { return __fmul_rn(__fsqrt_rn(__fadd_rn(r, 1e-8f)), sin_freq(k)); }
+__device__ __forceinline__ float radial_rn(float dx, float dy, float dz) {
+  return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+}
+
 // ---- programmatic dependent launch (PDL) ------------------------------------------------------------------------------
 // The kernels of one forward form a strict chain on one stream. Launched with the programmatic-stream-serialization
 // attribute (launch_chain below), a kernel's CTAs may become resident while the previous kernel is still draining: they run
@@ -109,6 +126,10 @@ struct EdgeMlpW {
   const float* b1_u;
   const float* wd_u;
   const float* w0_u;
+  // sin_embedding: .0.weight[:, 2H:2H+24]^T ([24][128]: features [sin d f_k, cos d f_k, sin d0 f_k, cos d0 f_k]) and its
+  // log2-domain copy; wdmax then holds sum_k max_c |w_k[c]| (|sin|, |cos| <= 1) and w0max 0
+  const float* we;
+  const float* we_u;
 };
 
 // Packed weights of one GCL: its edge MLP plus node_mlp.

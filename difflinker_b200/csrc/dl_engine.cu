@@ -65,6 +65,7 @@ struct HostStage {  // device staging for the *_host entry points
 
 struct dl_engine {
   dl_config cfg{};
+  dl_egnn_options opts{};
   int D = 0;
   int num_sms = 0;
   int max_threads_per_sm = 2048;
@@ -92,6 +93,9 @@ struct dl_engine {
 };
 
 namespace {
+
+// edge-attribute columns of every edge MLP's first layer: [d, d0], or their 24 sinusoidal features
+int edges_in(const dl_engine* e) { return e->opts.sin_embedding ? N_SIN_FEAT : 2; }
 
 // DL_TIME_KERNELS=1: CUDA-event time of every launch of a (non-captured) forward, accumulated per kernel label and printed
 // when the engine is destroyed -- the live (warm-cache, back-to-back) counterpart of the ncu launch list.
@@ -144,7 +148,8 @@ struct ExpectedParam {
   int64_t numel;
 };
 
-std::vector<ExpectedParam> expected_params(const dl_config& c) {
+// edges_in: width of the edge attributes of every edge MLP's first layer (2 distances, or 24 with sin_embedding)
+std::vector<ExpectedParam> expected_params(const dl_config& c, int edges_in) {
   const int D = c.in_node_nf + c.context_node_nf + (c.condition_time ? 1 : 0);
   const int Hh = c.hidden_nf;
   std::vector<ExpectedParam> v;
@@ -157,7 +162,7 @@ std::vector<ExpectedParam> expected_params(const dl_config& c) {
     for (int s = 0; s < c.inv_sublayers; ++s) {
       snprintf(buf, sizeof(buf), "dynamics.e_block_%d.gcl_%d.", l, s);
       std::string p(buf);
-      v.push_back({p + "edge_mlp.0.weight", (int64_t)Hh * (2 * Hh + 2)});
+      v.push_back({p + "edge_mlp.0.weight", (int64_t)Hh * (2 * Hh + edges_in)});
       v.push_back({p + "edge_mlp.0.bias", Hh});
       v.push_back({p + "edge_mlp.2.weight", (int64_t)Hh * Hh});
       v.push_back({p + "edge_mlp.2.bias", Hh});
@@ -168,7 +173,7 @@ std::vector<ExpectedParam> expected_params(const dl_config& c) {
     }
     snprintf(buf, sizeof(buf), "dynamics.e_block_%d.gcl_equiv.", l);
     std::string p(buf);
-    v.push_back({p + "coord_mlp.0.weight", (int64_t)Hh * (2 * Hh + 2)});
+    v.push_back({p + "coord_mlp.0.weight", (int64_t)Hh * (2 * Hh + edges_in)});
     v.push_back({p + "coord_mlp.0.bias", Hh});
     v.push_back({p + "coord_mlp.2.weight", (int64_t)Hh * Hh});
     v.push_back({p + "coord_mlp.2.bias", Hh});
@@ -232,10 +237,11 @@ void pack_gcl(Packer& pk, GclW& w, const RawWeights& raw, const std::string& p, 
   pk.add(&w.b4, raw.at(p + "node_mlp.2.bias"));
 }
 
-// The denoiser's additions to an edge MLP (first Linear over 2H+2 inputs): the input-distance column w0, the bounds of the
-// distance columns, and the tensor-core copies -- W2 and the log2-domain first layer (kernels_tc.cuh pack_w2).
-void pack_edge_mlp_denoiser(Packer& pk, EdgeMlpW& w, const RawWeights& raw, const std::string& p) {
-  constexpr int IN1 = 2 * H + 2;
+// The denoiser's additions to an edge MLP (first Linear over IN1 = 2H+2 inputs, or 2H+24 with sin_embedding): the
+// input-distance column w0 (or the 24 embedding columns), the bounds of the edge-attribute columns, and the tensor-core
+// copies -- W2 and the log2-domain first layer (kernels_tc.cuh pack_w2).
+void pack_edge_mlp_denoiser(Packer& pk, EdgeMlpW& w, const RawWeights& raw, const std::string& p, bool sin_embedding) {
+  const int IN1 = 2 * H + (sin_embedding ? N_SIN_FEAT : 2);
   auto scaled = [](const std::vector<float>& v) { std::vector<float> o(v.size()); for (size_t i = 0; i < v.size(); ++i) o[i] = (float)((double)v[i] * tc::NEG_LOG2E); return o; };
   auto absmax = [](const std::vector<float>& v) { float m = 0.f; for (float x : v) m = std::max(m, std::fabs(x)); return m; };
   const auto& W1 = raw.at(p + "0.weight");
@@ -247,6 +253,13 @@ void pack_edge_mlp_denoiser(Packer& pk, EdgeMlpW& w, const RawWeights& raw, cons
   pk.add(&w.wd_u, scaled(wd));
   pk.add(&w.w0_u, scaled(w0));
   w.wdmax = absmax(wd); w.w0max = absmax(w0);
+  if (sin_embedding) {
+    const std::vector<float> we = transpose_block(W1, H, IN1, 2 * H, N_SIN_FEAT);
+    pk.add(&w.we, we);
+    pk.add(&w.we_u, scaled(we));
+    w.wdmax = 0.f; w.w0max = 0.f;
+    for (int k = 0; k < N_SIN_FEAT; ++k) w.wdmax += absmax(std::vector<float>(we.begin() + k * H, we.begin() + (k + 1) * H));
+  }
 }
 
 template <typename T>
@@ -369,7 +382,15 @@ EdgeArgs edge_args(const dl_engine* e, const EdgeMlpW& w, bool coord, const int8
   ea.plan = make_plan(ws); ea.agg = coord ? nullptr : ws.agg; ea.x_out = x_out; ea.nbr = ws.nbr;
   ea.recs = coord ? ws.xrecs : ws.recs;
   ea.n_recs = coord && ws.n_recs ? ws.n_recs + 1 : ws.n_recs;
+  ea.coords_range = e->opts.coords_range;
+  ea.we = e->use_tc ? w.we_u : w.we;
   return ea;
+}
+
+// The edge-kernel OPT bits (common.cuh) of the engine's EGNN options; tanh only concerns the coordinate update.
+int edge_opt(const dl_engine* e, bool coord) {
+  return (coord && e->opts.tanh ? OPT_TANH : 0) | (e->opts.aggregation == DL_AGGR_MEAN ? OPT_MEAN : 0) |
+         (e->opts.sin_embedding ? OPT_SIN : 0);
 }
 
 // The edge MLPs whose first-layer projections are taken from the h that GCL s of block l writes, with the AB / ABmax
@@ -404,13 +425,39 @@ tcn::NodeTcArgs node_tc_args(const dl_engine* e, const GclW& w, int l, int s) {
   return ta;
 }
 
-dl_status launch_edge(dl_engine* e, const Geom& gm, const EdgeArgs& ea, bool coord, const void* w2_tc, cudaStream_t st) {
-  if (e->use_tc) {
-    dl_status s = tc::launch_edge_tc(gm, ea, coord, w2_tc, e->num_sms, st);
-    if (s != DL_OK) return s;
+// Every OPT combination of the SIMT edge kernel (tanh only for the coordinate update), walked at compile time.
+template <bool COORD, int OPT = 0>
+void launch_edge_simt(int opt, int num_sms, const Geom& gm, const EdgeArgs& ea, cudaStream_t st) {
+  if constexpr (OPT <= (OPT_TANH | OPT_MEAN | OPT_SIN)) {
+    if constexpr (COORD || !(OPT & OPT_TANH))
+      if (opt == OPT) { k_edge_simt<COORD, ACT_SILU, OPT><<<num_sms, 256, EDGE_SIMT_SMEM, st>>>(gm, ea); return; }
+    launch_edge_simt<COORD, OPT + 1>(opt, num_sms, gm, ea, st);
+  }
+}
+
+template <bool COORD, int OPT = 0>
+cudaError_t opt_in_edge_simt() {
+  if constexpr (OPT > (OPT_TANH | OPT_MEAN | OPT_SIN)) {
+    return cudaSuccess;
   } else {
-    if (coord) k_edge_simt<true><<<e->num_sms, 256, EDGE_SIMT_SMEM, st>>>(gm, ea);
-    else k_edge_simt<false><<<e->num_sms, 256, EDGE_SIMT_SMEM, st>>>(gm, ea);
+    if constexpr (COORD || !(OPT & OPT_TANH)) {
+      const cudaError_t err = cudaFuncSetAttribute(k_edge_simt<COORD, ACT_SILU, OPT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   (int)EDGE_SIMT_SMEM);
+      if (err != cudaSuccess) return err;
+    }
+    return opt_in_edge_simt<COORD, OPT + 1>();
+  }
+}
+
+dl_status launch_edge(dl_engine* e, const Geom& gm, const EdgeArgs& ea, bool coord, const void* w2_tc, cudaStream_t st) {
+  const int opt = edge_opt(e, coord);
+  if (e->use_tc) {
+    dl_status s = tc::launch_edge_tc(gm, ea, coord, opt, w2_tc, e->num_sms, st);
+    if (s != DL_OK) { set_err("no tensor-core edge kernel for graph type %d with options %d", gm.graph_type, opt); return s; }
+  } else if (coord) {
+    launch_edge_simt<true>(opt, e->num_sms, gm, ea, st);
+  } else {
+    launch_edge_simt<false>(opt, e->num_sms, gm, ea, st);
   }
   LAUNCH_CHECK();
   e->launches += 1;
@@ -621,8 +668,15 @@ extern "C" {
 const char* dl_version(void) { return "difflinker_b200 0.1 (sm_90a)"; }
 const char* dl_last_error(void) { return g_err; }
 
-dl_status dl_create(const dl_config* cfg, dl_engine** out) {
+dl_status dl_create(const dl_config* cfg, dl_engine** out) { return dl_create_ex(cfg, nullptr, out); }
+
+dl_status dl_create_ex(const dl_config* cfg, const dl_egnn_options* opts, dl_engine** out) {
   if (!cfg || !out) { set_err("null argument"); return DL_ERR_INVALID; }
+  const dl_egnn_options o = opts ? *opts : dl_egnn_options{0, 15.0f, 0, DL_AGGR_SUM};
+  if (o.sin_embedding != 0 && o.sin_embedding != 1) { set_err("sin_embedding must be 0 or 1 (got %d)", o.sin_embedding); return DL_ERR_INVALID; }
+  if (o.tanh != 0 && o.tanh != 1) { set_err("tanh must be 0 or 1 (got %d)", o.tanh); return DL_ERR_INVALID; }
+  if (o.aggregation != DL_AGGR_SUM && o.aggregation != DL_AGGR_MEAN) { set_err("unknown aggregation %d", o.aggregation); return DL_ERR_INVALID; }
+  if (!std::isfinite(o.coords_range)) { set_err("coords_range must be finite"); return DL_ERR_INVALID; }
   if (cfg->hidden_nf != H) { set_err("hidden_nf must be %d (got %d)", H, cfg->hidden_nf); return DL_ERR_UNSUPPORTED; }
   if (cfg->n_dims != 3) { set_err("n_dims must be 3"); return DL_ERR_UNSUPPORTED; }
   const int D = cfg->in_node_nf + cfg->context_node_nf + (cfg->condition_time ? 1 : 0);
@@ -647,6 +701,7 @@ dl_status dl_create(const dl_config* cfg, dl_engine** out) {
   }
   dl_engine* e = new dl_engine();
   e->cfg = *cfg;
+  e->opts = o;
   e->D = D;
   e->num_sms = prop.multiProcessorCount;
   e->max_threads_per_sm = prop.maxThreadsPerMultiProcessor;
@@ -658,8 +713,8 @@ dl_status dl_create(const dl_config* cfg, dl_engine** out) {
   CK(cudaEventCreate(&e->ev_t1));
   CK(cudaMalloc((void**)&e->step_ctr, 2 * sizeof(int)));
   CK(cudaFuncSetAttribute(k_node<ACT_SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * NODE_TM * LDX * sizeof(float)));
-  CK(cudaFuncSetAttribute(k_edge_simt<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EDGE_SIMT_SMEM));
-  CK(cudaFuncSetAttribute(k_edge_simt<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EDGE_SIMT_SMEM));
+  CK(opt_in_edge_simt<true>());
+  CK(opt_in_edge_simt<false>());
   CK(cudaFuncSetAttribute(k_nbr, cudaFuncAttributeMaxDynamicSharedMemorySize, 4000 * CUT_SMEM_PER_NODE));
   if (getenv("DL_TIME_KERNELS")) g_times.on = true;
   if (const char* v = getenv("DL_WAIT_MODE")) { const int m = atoi(v); cudaMemcpyToSymbol(tc::c_wait_mode, &m, sizeof(int)); }
@@ -695,13 +750,13 @@ dl_status dl_destroy(dl_engine* e) {
 int64_t dl_expected_param_count(const dl_engine* e) {
   if (!e) return 0;
   int64_t n = 0;
-  for (auto& p : expected_params(e->cfg)) n += p.numel;
+  for (auto& p : expected_params(e->cfg, edges_in(e))) n += p.numel;
   return n;
 }
 
 dl_status dl_set_weight(dl_engine* e, const char* name, const float* data, int64_t numel) {
   if (!e || !name || !data) { set_err("null argument"); return DL_ERR_INVALID; }
-  for (auto& p : expected_params(e->cfg)) {
+  for (auto& p : expected_params(e->cfg, edges_in(e))) {
     if (p.name == name) {
       if (p.numel != numel) {
         set_err("weight %s: expected %lld elements, got %lld", name, (long long)p.numel, (long long)numel);
@@ -719,7 +774,7 @@ dl_status dl_set_weight(dl_engine* e, const char* name, const float* data, int64
 dl_status dl_finalize_weights(dl_engine* e) {
   if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
   CK(cudaSetDevice(e->cfg.device));
-  for (auto& p : expected_params(e->cfg))
+  for (auto& p : expected_params(e->cfg, edges_in(e)))
     if (!e->raw.count(p.name)) { set_err("missing weight %s", p.name.c_str()); return DL_ERR_WEIGHTS; }
   const int L = e->cfg.n_layers, S = e->cfg.inv_sublayers, D = e->D;
   const RawWeights& raw = e->raw;
@@ -736,16 +791,16 @@ dl_status dl_finalize_weights(dl_engine* e) {
       snprintf(buf, sizeof(buf), "dynamics.e_block_%d.gcl_%d.", l, s);
       const std::string p(buf);
       GclW& w = e->gcl[l * S + s];
-      pack_gcl(pk, w, raw, p, 2 * H + 2);
-      pack_edge_mlp_denoiser(pk, w, raw, p + "edge_mlp.");
+      pack_gcl(pk, w, raw, p, 2 * H + edges_in(e));
+      pack_edge_mlp_denoiser(pk, w, raw, p + "edge_mlp.", e->opts.sin_embedding != 0);
       pk.add_tc(&w.W3_tc, tcn::pack_blocks(raw.at(p + "node_mlp.0.weight"), 2 * H, 2, pk.tc, &w.w3_descale));
       pk.add_tc(&w.W4_tc, tcn::pack_blocks(raw.at(p + "node_mlp.2.weight"), H, 1, pk.tc, &w.w4_descale));
     }
     snprintf(buf, sizeof(buf), "dynamics.e_block_%d.gcl_equiv.coord_mlp.", l);
     const std::string p(buf);
     EqW& q = e->eq[l];
-    pack_edge_mlp(pk, q, raw, p, 2 * H + 2);
-    pack_edge_mlp_denoiser(pk, q, raw, p);
+    pack_edge_mlp(pk, q, raw, p, 2 * H + edges_in(e));
+    pack_edge_mlp_denoiser(pk, q, raw, p, e->opts.sin_embedding != 0);
     pk.add(&q.w5, raw.at(p + "4.weight"));
   }
   dl_status s = upload_blob(pk.blob, &e->wblob);

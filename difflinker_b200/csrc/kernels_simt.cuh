@@ -582,14 +582,19 @@ struct EdgeArgs {
   const int* nbr;           // cut-off graphs, tensor-core path: per-row neighbour lists (k_nbr) or null
   const int* recs;          // ... and this launch's packed tile records (GCL or COORD list), CUT_REC ints each
   const int* n_recs;        // [1]
+  float coords_range;       // OPT_TANH: bound of the coordinate update
+  const float* we;          // OPT_SIN: [24][128] embedding columns of the first layer (log2 domain on the tensor-core path)
 };
 
 constexpr size_t EDGE_SIMT_SMEM =
     sizeof(float) * ((size_t)H * H /*W2s*/ + (size_t)H * ET /*S1*/ + (size_t)ET * LDB /*Bs*/ + (size_t)MAXR * H /*As*/ +
                      4 * H /*b2,wd,w0,w5*/ + ET /*ems*/ + ET * 3 /*cds*/ + ET /*phis*/);
 
-template <bool COORD, int ACT = ACT_SILU>
+// OPT (OPT_TANH | OPT_MEAN): with OPT_MEAN a row's divisor is N on FC graphs and its number of live edges (cut-off edges
+// have weight 1, every other pair 0) on cut-off graphs, counted alongside the sum.
+template <bool COORD, int ACT = ACT_SILU, int OPT = 0>
 __global__ void __launch_bounds__(256, 1) k_edge_simt(Geom gm, EdgeArgs a) {
+  constexpr bool MEAN = (OPT & OPT_MEAN) != 0, TANH = (OPT & OPT_TANH) != 0, EMB = (OPT & OPT_SIN) != 0;
   extern __shared__ __align__(16) float sm_edge[];
   float* W2s = sm_edge;
   float* S1 = W2s + H * H;
@@ -615,6 +620,8 @@ __global__ void __launch_bounds__(256, 1) k_edge_simt(Geom gm, EdgeArgs a) {
   }
   __syncthreads();
 
+  // aggregation divisor of a row with `cnt` live edges (egnn.py:312-319)
+  auto divisor = [&](float cnt) { return !MEAN ? gm.normalization_factor : gm.graph_type == 0 ? (float)N : fmaxf(cnt, 1.f); };
   const int n_work = COORD ? *a.plan.n_xmols : *a.plan.n_items;
   for (int wi = blockIdx.x; wi < n_work; wi += gridDim.x) {
     int b, r_begin, r_count;
@@ -637,6 +644,7 @@ __global__ void __launch_bounds__(256, 1) k_edge_simt(Geom gm, EdgeArgs a) {
       }
       float run = 0.f;                                    // GCL: running row sum across column chunks
       float xrun = 0.f;                                   // COORD: thread (r,dim) running sum
+      float runc = 0.f;                                   // OPT_MEAN: running live-edge count of the same row
       for (int c0 = 0; c0 < nc; c0 += ET) {
         const int ncc = min(ET, nc - c0);
         const int Et = nrt * ncc;
@@ -651,6 +659,7 @@ __global__ void __launch_bounds__(256, 1) k_edge_simt(Geom gm, EdgeArgs a) {
           const bool valid = e < Et;
           int rr = 0, jj = 0;
           float d = 0.f, d0 = 0.f;
+          float emb[EMB ? N_SIN_FEAT : 1];                // OPT_SIN: [sin d f_k, cos d f_k, sin d0 f_k, cos d0 f_k]
           if (valid) {
             rr = e / ncc; jj = e - rr * ncc;
             const int i = rows[r_begin + rt + rr], j = cols[c0 + jj];
@@ -660,6 +669,14 @@ __global__ void __launch_bounds__(256, 1) k_edge_simt(Geom gm, EdgeArgs a) {
             d = dx * dx + dy * dy + dz * dz;
             float ex = yi[0] - yj[0], ey = yi[1] - yj[1], ez = yi[2] - yj[2];
             d0 = ex * ex + ey * ey + ez * ez;
+            if constexpr (EMB) {                          // the reference's rounding order for the sinusoid arguments
+              d = radial_rn(dx, dy, dz); d0 = radial_rn(ex, ey, ez);
+#pragma unroll
+              for (int k = 0; k < N_SIN_FREQ; ++k) {
+                sincosf(sin_arg(d, k), &emb[k], &emb[N_SIN_FREQ + k]);
+                sincosf(sin_arg(d0, k), &emb[2 * N_SIN_FREQ + k], &emb[3 * N_SIN_FREQ + k]);
+              }
+            }
             if (kh == 0) {
               int ci = 0, cj = 0;
               if (gm.graph_type >= 1 && gm.graph_type <= 3) { ci = a.cls[gb + i]; cj = a.cls[gb + j]; }
@@ -678,7 +695,14 @@ __global__ void __launch_bounds__(256, 1) k_edge_simt(Geom gm, EdgeArgs a) {
 #pragma unroll 8
           for (int kk = 0; kk < H / 2; ++kk) {
             int k = kh * (H / 2) + kk;
-            float pre = Ar[k] + Br[k] + d * wds[k] + d0 * w0s[k];
+            float pre;
+            if constexpr (EMB) {
+              pre = Ar[k] + Br[k];
+#pragma unroll
+              for (int f = 0; f < N_SIN_FEAT; ++f) pre += (valid ? emb[f] : 0.f) * __ldg(a.we + f * H + k);
+            } else {
+              pre = Ar[k] + Br[k] + d * wds[k] + d0 * w0s[k];
+            }
             S1[k * ET + e] = valid ? act_f<ACT>(pre) : 0.f;
           }
         }
@@ -726,13 +750,19 @@ __global__ void __launch_bounds__(256, 1) k_edge_simt(Geom gm, EdgeArgs a) {
           const int c = tid & (H - 1);
           if (nc <= ET) {
             for (int rr = tid >> 7; rr < nrt; rr += 2) {
-              float s = 0.f;
-              for (int jj = 0; jj < ncc; ++jj) s += Outs[(rr * ncc + jj) * H + c];
-              a.agg[(gb + rows[r_begin + rt + rr]) * H + c] = s / gm.normalization_factor;
+              float s = 0.f, cnt = 0.f;
+              for (int jj = 0; jj < ncc; ++jj) {
+                s += Outs[(rr * ncc + jj) * H + c];
+                if (MEAN) cnt += ems[rr * ncc + jj] != 0.f ? 1.f : 0.f;
+              }
+              a.agg[(gb + rows[r_begin + rt + rr]) * H + c] = s / divisor(cnt);
             }
           } else if (tid < H) {
-            for (int jj = 0; jj < ncc; ++jj) run += Outs[jj * H + c];
-            if (c0 + ET >= nc) a.agg[(gb + rows[r_begin + rt]) * H + c] = run / gm.normalization_factor;
+            for (int jj = 0; jj < ncc; ++jj) {
+              run += Outs[jj * H + c];
+              if (MEAN) runc += ems[jj] != 0.f ? 1.f : 0.f;
+            }
+            if (c0 + ET >= nc) a.agg[(gb + rows[r_begin + rt]) * H + c] = run / divisor(runc);
           }
         } else {
           for (int e = warp; e < Et; e += 8) {            // phi_e = w5 . m_e  (coord_mlp.4, egnn.py:90-97)
@@ -741,19 +771,22 @@ __global__ void __launch_bounds__(256, 1) k_edge_simt(Geom gm, EdgeArgs a) {
             for (int q = 0; q < 4; ++q) s = fmaf(Outs[e * H + lane + 32 * q], w5s[lane + 32 * q], s);
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-            if (lane == 0) phis[e] = s * ems[e];
+            if (lane == 0) phis[e] = TANH ? tanhf(s) * a.coords_range * ems[e] : s * ems[e];   // egnn.py:104-109
           }
           __syncthreads();
           if (tid < nrt * 3) {
             int rr = tid / 3, dim = tid - rr * 3;
             float s = 0.f;
-            for (int jj = 0; jj < ncc; ++jj) s += cds[(rr * ncc + jj) * 3 + dim] * phis[rr * ncc + jj];
+            for (int jj = 0; jj < ncc; ++jj) {
+              s += cds[(rr * ncc + jj) * 3 + dim] * phis[rr * ncc + jj];
+              if (MEAN) runc += ems[rr * ncc + jj] != 0.f ? 1.f : 0.f;
+            }
             xrun += s;
             if (c0 + ET >= nc) {
               int i = rows[r_begin + rt + rr];
               float lm = a.linker_mask ? a.linker_mask[gb + i] : 1.f;
               float xv = a.x[(gb + i) * 3 + dim];
-              a.x_out[(gb + i) * 3 + dim] = (xv + (xrun / gm.normalization_factor) * lm) * a.nm[gb + i];
+              a.x_out[(gb + i) * 3 + dim] = (xv + (xrun / divisor(runc)) * lm) * a.nm[gb + i];
             }
           }
         }

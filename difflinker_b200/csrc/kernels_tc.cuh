@@ -364,9 +364,18 @@ __device__ __forceinline__ typename std::conditional<SPARSE, RecIter, TileIter<C
 // epilogue combines the two edge halves through shared memory.
 // SPARSE = true: cut-off (pocket) graphs -- tiles are packed from the per-row neighbour lists k_nbr built for this
 // forward call, so only edges the reference creates are processed (egnn.py:554-596); FC graphs use SPARSE = false.
+// OPT (OPT_TANH | OPT_MEAN, common.cuh): OPT_TANH bounds the COORD update, trans = (cd * tanh(phi)) * coords_range * EM;
+// OPT_MEAN divides each row's sum by its edge count in the reference's edge list: N on FC graphs; on cut-off graphs the
+// row's neighbour-list length, which is its degree, or 1 for an isolated row (its one padding edge) -- taken from the
+// tile's row starts, or from the header (hdr[6]) for the chunk tiles of a row with more than 128 neighbours.
 // ---------------------------------------------------------------------------------------------------------
-template <bool COORD, bool SPARSE = false>
+// OPT_SIN: the table's d / d0 are the radials in the reference's rounding order, and the producers replace d w_d + d0 w_0
+// by sum_k e_k w_k over the 24 sinusoidal features: lane k < 12 of an edge's 16-lane half evaluates sincos of one
+// (radial, frequency) pair, the features reach the other lanes by shuffles, and w_k comes through L1.
+template <bool COORD, bool SPARSE = false, int OPT = 0>
 __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArgs a, const __half* __restrict__ w2tc) {
+  constexpr bool MEAN = (OPT & OPT_MEAN) != 0, TANH = (OPT & OPT_TANH) != 0, EMB = (OPT & OPT_SIN) != 0;
+  static_assert(COORD || !TANH, "tanh only bounds the coordinate update");
   extern __shared__ uint8_t smem_raw[];
   // keep the pointer derived from the __shared__ array (no integer round trip) so accesses compile to LDS/STS
   uint8_t* sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -410,10 +419,16 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
       if (more) {
         const int Et = SPARSE ? cur.Et : cur.nrt * cur.ncc;
         const size_t gb = (size_t)cur.b * N;
+        int heavy_deg = 0;                                 // OPT_MEAN: degree of a row served in chunk tiles (its record)
+        if constexpr (MEAN && SPARSE) {
+          const int w1 = __shfl_sync(0xffffffffu, iter.cur, 1), v2 = __shfl_sync(0xffffffffu, iter.cur, 2);
+          heavy_deg = ((w1 >> 8) & 1) ? v2 : 0;
+        }
         if (lane == 0) {
           hdr[0] = Et; hdr[1] = cur.nrt; hdr[2] = cur.ncc;
           hdr[3] = (cur.first_chunk ? 1 : 0) | (cur.last_chunk ? 2 : 0);
           hdr[4] = cur.b;
+          if (MEAN && SPARSE) hdr[6] = heavy_deg;
         }
         if (SPARSE) {
           if (lane < cur.nrt) {
@@ -449,9 +464,14 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
           }
           const float4 xi = a.x4[gb + i], xj = a.x4[gb + j], yi = a.x04[gb + i], yj = a.x04[gb + j];   // 16-byte gathers
           const float dx = xi.x - xj.x, dy = xi.y - xj.y, dz = xi.z - xj.z;
-          const float d = dx * dx + dy * dy + dz * dz;                       // egnn.py:297-298
           const float ex = yi.x - yj.x, ey = yi.y - yj.y, ez = yi.z - yj.z;
-          const float d0 = ex * ex + ey * ey + ez * ez;                      // egnn.py:220
+          float d, d0;
+          if constexpr (EMB) {                                               // sinusoid arguments: torch's rounding order
+            d = radial_rn(dx, dy, dz); d0 = radial_rn(ex, ey, ez);
+          } else {
+            d = dx * dx + dy * dy + dz * dz;                                 // egnn.py:297-298
+            d0 = ex * ex + ey * ey + ez * ez;                                // egnn.py:220
+          }
           int ci = 0, cj = 0;
           if (!SPARSE && gm.graph_type != 0) { ci = a.cls[gb + i]; cj = a.cls[gb + j]; }
           reinterpret_cast<int*>(tb + TBL_ROWOFF)[e] = (int)((gb + i) * 2 * H);
@@ -460,7 +480,9 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
           reinterpret_cast<float*>(tb + TBL_D0)[e] = d0;
           // |silu(pre)| <= |pre| <= max|A_i| + max|B_j| + d max|wd| + d0 max|w0|: exact power-of-two scale that keeps the
           // fp16 hi/lo operands of this edge below 2^14 (activations of diverging samples exceed fp16's 65504).
-          const float bound = a.ABmax[(gb + i) * 2] + a.ABmax[(gb + j) * 2 + 1] + d * a.wdmax + d0 * a.w0max;
+          // (with OPT_SIN: + sum_k max|w_k|, since |sin|, |cos| <= 1)
+          const float bound = EMB ? a.ABmax[(gb + i) * 2] + a.ABmax[(gb + j) * 2 + 1] + a.wdmax
+                                  : a.ABmax[(gb + i) * 2] + a.ABmax[(gb + j) * 2 + 1] + d * a.wdmax + d0 * a.w0max;
           float sc = 1.0f;
           if (!(bound <= F16_TARGET)) {
             const int ex2 = ((__float_as_int(bound) >> 23) & 0xff) - 127;
@@ -553,15 +575,42 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
             pa0 = __ldg(reinterpret_cast<const float4*>(ap)); pa1 = __ldg(reinterpret_cast<const float4*>(ap + 4));
           }
           const float4 a0 = pa0, a1 = pa1;
+          float2 pre_emb[4];
+          if constexpr (EMB) {                             // all lanes (shuffles): slots past Et mirror the last edge
+            const int kf = kc < 12 ? kc : kc - 12;          // lanes 12-15 repeat lanes 0-3; their values are not read
+            float sn, cs;
+            sincosf(sin_arg(kf < N_SIN_FREQ ? dv[e] : d0v[e], kf % N_SIN_FREQ), &sn, &cs);
+            pre_emb[0] = fadd2(make_float2(a0.x, a0.y), make_float2(b0.x, b0.y));
+            pre_emb[1] = fadd2(make_float2(a0.z, a0.w), make_float2(b0.z, b0.w));
+            pre_emb[2] = fadd2(make_float2(a1.x, a1.y), make_float2(b1.x, b1.y));
+            pre_emb[3] = fadd2(make_float2(a1.z, a1.w), make_float2(b1.z, b1.w));
+#pragma unroll 2                                   // unrolled further, the weight loads are hoisted and spill
+            for (int k = 0; k < N_SIN_FEAT; ++k) {         // feature k: [sin d f, cos d f, sin d0 f, cos d0 f][k % 6]
+              const int src = (k / 12) * N_SIN_FREQ + k % N_SIN_FREQ;
+              const float ev = __shfl_sync(0xffffffffu, (k % 12) < N_SIN_FREQ ? sn : cs, src, 16);
+              const float4 w0 = __ldg(reinterpret_cast<const float4*>(a.we + k * H + kc * 8));
+              const float4 w1 = __ldg(reinterpret_cast<const float4*>(a.we + k * H + kc * 8 + 4));
+              const float2 ee = make_float2(ev, ev);
+              pre_emb[0] = ffma2(ee, make_float2(w0.x, w0.y), pre_emb[0]);
+              pre_emb[1] = ffma2(ee, make_float2(w0.z, w0.w), pre_emb[1]);
+              pre_emb[2] = ffma2(ee, make_float2(w1.x, w1.y), pre_emb[2]);
+              pre_emb[3] = ffma2(ee, make_float2(w1.z, w1.w), pre_emb[3]);
+            }
+          }
           if (e < Et) {
-            const float d = dv[e], d0 = d0v[e];
-            const float2 dd = make_float2(d, d), dd0 = make_float2(d0, d0);
-            const float2 av[4] = {make_float2(a0.x, a0.y), make_float2(a0.z, a0.w), make_float2(a1.x, a1.y), make_float2(a1.z, a1.w)};
-            const float2 bv[4] = {make_float2(b0.x, b0.y), make_float2(b0.z, b0.w), make_float2(b1.x, b1.y), make_float2(b1.z, b1.w)};
             float2 sv[4];
+            if constexpr (EMB) {
 #pragma unroll
-            for (int q = 0; q < 4; ++q)                     // egnn.py:49-50
-              sv[q] = usig2(ffma2(dd0, w0r[q], ffma2(dd, wdr[q], fadd2(av[q], bv[q]))));   // log2 domain (see pack_w2)
+              for (int q = 0; q < 4; ++q) sv[q] = usig2(pre_emb[q]);
+            } else {
+              const float d = dv[e], d0 = d0v[e];
+              const float2 dd = make_float2(d, d), dd0 = make_float2(d0, d0);
+              const float2 av[4] = {make_float2(a0.x, a0.y), make_float2(a0.z, a0.w), make_float2(a1.x, a1.y), make_float2(a1.z, a1.w)};
+              const float2 bv[4] = {make_float2(b0.x, b0.y), make_float2(b0.z, b0.w), make_float2(b1.x, b1.y), make_float2(b1.z, b1.w)};
+  #pragma unroll
+              for (int q = 0; q < 4; ++q)                     // egnn.py:49-50
+                sv[q] = usig2(ffma2(dd0, w0r[q], ffma2(dd, wdr[q], fadd2(av[q], bv[q]))));   // log2 domain (see pack_w2)
+            }
             if (rescale) {                                 // rare: diverging samples only (tile-uniform)
               const float sc = scv[e];
 #pragma unroll
@@ -638,6 +687,19 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
         // once); the partial sum of a row that leaves the run is passed to the next quad lane.
         const float2 bias = make_float2(b2w5[r0].x * -1.4426950408889634f, b2w5[r0 + 8].x * -1.4426950408889634f);
         const float inv_norm = 1.0f / gm.normalization_factor;
+        // agg_i = row sum / normalization_factor, or with OPT_MEAN / the row's edge count (egnn.py:312-319). Both multiply by a
+        // reciprocal, as the division by normalization_factor always has (within 2 ulp of the reference's division): an IEEE
+        // division in this unrolled loop costs 13 % of the launch.
+        const float inv_n = 1.0f / (float)N;
+        auto put = [&](int r, float2 v) {
+          float* dst = a.agg + (gb + rownode[r]) * H;
+          if constexpr (MEAN) {
+            const float inv = SPARSE ? rcp_approx((float)(hdr[6] > 0 ? hdr[6] : rowstart[r + 1] - rowstart[r])) : inv_n;
+            dst[r0] = v.x * inv; dst[r0 + 8] = v.y * inv;
+          } else {
+            dst[r0] = v.x * inv_norm; dst[r0 + 8] = v.y * inv_norm;
+          }
+        };
         const int E0 = 32 * q;
         const bool has = E0 < Et;
         int cur = 0;
@@ -655,10 +717,7 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
         for (int tt = 0; tt < 32; ++tt) {
           if (wmask & (1u << tt)) {                        // warp-uniform: some lane's run has a row start at tt
             const bool here = (bmask >> tt) & 1u;          // this lane leaves row `cur`
-            if (here && !in_head) {
-              float* dst = a.agg + (gb + rownode[cur]) * H;
-              dst[r0] = sum.x * inv_norm; dst[r0 + 8] = sum.y * inv_norm;
-            }
+            if (here && !in_head) put(cur, sum);
             hsum = here && in_head ? sum : hsum;
             sum = here ? make_float2(0.f, 0.f) : sum;
             in_head = in_head && !here;
@@ -687,14 +746,8 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
           run = make_float2(__shfl_sync(0xffffffffu, htot.x, src), __shfl_sync(0xffffffffu, htot.y, src));
         }
         if (has && last_chunk) {
-          if (!in_head || !open_end) {                     // the first row ends in this run
-            float* dst = a.agg + (gb + rownode[hrow]) * H;
-            dst[r0] = htot.x * inv_norm; dst[r0 + 8] = htot.y * inv_norm;   // egnn.py:312-313
-          }
-          if (!in_head && !open_end && !cut) {             // so does the last one, unless the tile end closed it above
-            float* dst = a.agg + (gb + rownode[cur]) * H;
-            dst[r0] = lsum.x * inv_norm; dst[r0 + 8] = lsum.y * inv_norm;
-          }
+          if (!in_head || !open_end) put(hrow, htot);     // the first row ends in this run (egnn.py:312-313)
+          if (!in_head && !open_end && !cut) put(cur, lsum);   // so does the last one, unless the tile end closed it above
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(bars + BAR_TEMPTY + 8 * acc);
@@ -714,14 +767,29 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
         phia += __shfl_xor_sync(0xffffffffu, phia, 1); phib += __shfl_xor_sync(0xffffffffu, phib, 1);
         phia += __shfl_xor_sync(0xffffffffu, phia, 2); phib += __shfl_xor_sync(0xffffffffu, phib, 2);
         const float* cds = reinterpret_cast<const float*>(tb + TBL_CD);
-        if (q == 0 && r0 < Et) {                           // egnn.py:107-109
-          const float w = phia * eda.x;
-          txs[r0 * 3 + 0] = cds[r0 * 3 + 0] * w; txs[r0 * 3 + 1] = cds[r0 * 3 + 1] * w; txs[r0 * 3 + 2] = cds[r0 * 3 + 2] * w;
-        }
-        if (q == 0 && r0 + 8 < Et) {
-          const int e = r0 + 8;
-          const float w = phib * edb.x;
-          txs[e * 3 + 0] = cds[e * 3 + 0] * w; txs[e * 3 + 1] = cds[e * 3 + 1] * w; txs[e * 3 + 2] = cds[e * 3 + 2] * w;
+        if constexpr (TANH) {                              // egnn.py:104-109, evaluated left to right
+          const float range = a.coords_range;
+          if (q == 0 && r0 < Et) {
+            const float th = tanhf(phia);
+#pragma unroll
+            for (int k = 0; k < 3; ++k) txs[r0 * 3 + k] = cds[r0 * 3 + k] * th * range * eda.x;
+          }
+          if (q == 0 && r0 + 8 < Et) {
+            const int e = r0 + 8;
+            const float th = tanhf(phib);
+#pragma unroll
+            for (int k = 0; k < 3; ++k) txs[e * 3 + k] = cds[e * 3 + k] * th * range * edb.x;
+          }
+        } else {
+          if (q == 0 && r0 < Et) {                         // egnn.py:107-109
+            const float w = phia * eda.x;
+            txs[r0 * 3 + 0] = cds[r0 * 3 + 0] * w; txs[r0 * 3 + 1] = cds[r0 * 3 + 1] * w; txs[r0 * 3 + 2] = cds[r0 * 3 + 2] * w;
+          }
+          if (q == 0 && r0 + 8 < Et) {
+            const int e = r0 + 8;
+            const float w = phib * edb.x;
+            txs[e * 3 + 0] = cds[e * 3 + 0] * w; txs[e * 3 + 1] = cds[e * 3 + 1] * w; txs[e * 3 + 2] = cds[e * 3 + 2] * w;
+          }
         }
         named_sync(2, 32 * N_EPI_WARPS);                   // both warpgroups: txs complete
         if (tid < nrt * 3) {
@@ -735,7 +803,9 @@ __global__ void __launch_bounds__(EDGE_TC_THREADS, 1) k_edge_tc(Geom gm, EdgeArg
             const int i = rownode[rr];
             const float lm = a.linker_mask ? a.linker_mask[gb + i] : 1.f;
             const float xv = a.x[(gb + i) * 3 + dim];
-            const float xn = (xv + (sacc / gm.normalization_factor) * lm) * a.nm[gb + i];                 // egnn.py:110-124
+            float div = gm.normalization_factor;
+            if constexpr (MEAN) div = SPARSE ? (float)(hdr[6] > 0 ? hdr[6] : ncc) : (float)N;
+            const float xn = (xv + (sacc / div) * lm) * a.nm[gb + i];                 // egnn.py:110-124
             a.x_out[(gb + i) * 3 + dim] = xn;
             reinterpret_cast<float*>(a.x4_out + gb + i)[dim] = xn;
           }
@@ -754,9 +824,20 @@ template <typename K>
 inline bool opt_in_smem(K kern) {
   return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) == cudaSuccess;
 }
+constexpr int OPT_ALL = OPT_TANH | OPT_MEAN | OPT_SIN;
+// The instantiations of one (COORD, SPARSE) pair, walked at compile time: every OPT, OPT_TANH only for the coordinate update.
+template <bool COORD, bool SPARSE, int OPT = 0>
+inline bool opt_in_all() {
+  if constexpr (OPT > OPT_ALL) {
+    return true;
+  } else {
+    if constexpr (COORD || !(OPT & OPT_TANH))
+      if (!opt_in_smem(k_edge_tc<COORD, SPARSE, OPT>)) return false;
+    return opt_in_all<COORD, SPARSE, OPT + 1>();
+  }
+}
 inline dl_status configure() {
-  const bool ok = opt_in_smem(k_edge_tc<true, false>) && opt_in_smem(k_edge_tc<true, true>) &&
-                  opt_in_smem(k_edge_tc<false, false>) && opt_in_smem(k_edge_tc<false, true>);
+  const bool ok = opt_in_all<true, false>() && opt_in_all<true, true>() && opt_in_all<false, false>() && opt_in_all<false, true>();
   return ok ? DL_OK : DL_ERR_CUDA;
 }
 
@@ -794,14 +875,27 @@ inline size_t pack_w2(const std::vector<float>& W_in, std::vector<__half>& blob,
   return off;
 }
 
-inline dl_status launch_edge_tc(const Geom& gm, const EdgeArgs& ea, bool coord, const void* w2_tc, int num_sms,
+template <bool COORD, bool SPARSE, int OPT = 0>
+inline void launch_opt(int opt, const Geom& gm, const EdgeArgs& ea, const __half* w, int num_sms, cudaStream_t st) {
+  if constexpr (OPT <= OPT_ALL) {
+    if constexpr (COORD || !(OPT & OPT_TANH))
+      if (opt == OPT) { k_edge_tc<COORD, SPARSE, OPT><<<num_sms, EDGE_TC_THREADS, SMEM_BYTES, st>>>(gm, ea, w); return; }
+    launch_opt<COORD, SPARSE, OPT + 1>(opt, gm, ea, w, num_sms, st);
+  }
+}
+
+// opt: the OPT bits of this launch (OPT_TANH only for the coordinate update). Cut-off graphs always come with the
+// neighbour-list records (ea.recs), so OPT_MEAN's FC divisor N is right whenever SPARSE is false.
+inline dl_status launch_edge_tc(const Geom& gm, const EdgeArgs& ea, bool coord, int opt, const void* w2_tc, int num_sms,
                                 cudaStream_t st) {
+  if (!coord && (opt & OPT_TANH)) return DL_ERR_INVALID;
+  if (ea.recs == nullptr && gm.graph_type != 0 && (opt & OPT_MEAN)) return DL_ERR_INVALID;
   const __half* w = reinterpret_cast<const __half*>(w2_tc);
   if (ea.recs != nullptr) {
-    if (coord) k_edge_tc<true, true><<<num_sms, EDGE_TC_THREADS, SMEM_BYTES, st>>>(gm, ea, w);
-    else k_edge_tc<false, true><<<num_sms, EDGE_TC_THREADS, SMEM_BYTES, st>>>(gm, ea, w);
-  } else if (coord) k_edge_tc<true, false><<<num_sms, EDGE_TC_THREADS, SMEM_BYTES, st>>>(gm, ea, w);
-  else k_edge_tc<false, false><<<num_sms, EDGE_TC_THREADS, SMEM_BYTES, st>>>(gm, ea, w);
+    if (coord) launch_opt<true, true>(opt, gm, ea, w, num_sms, st);
+    else launch_opt<false, true>(opt, gm, ea, w, num_sms, st);
+  } else if (coord) launch_opt<true, false>(opt, gm, ea, w, num_sms, st);
+  else launch_opt<false, false>(opt, gm, ea, w, num_sms, st);
   return DL_OK;
 }
 

@@ -16,6 +16,9 @@ from . import _native
 from .utils import FoundNaNException, nan_exception_class
 
 
+SIN_EMBEDDING_DIM = 12   # SinusoidsEmbeddingNew().dim: sin and cos of 6 frequencies (src/egnn.py:281-286)
+
+
 class _GCLParams(nn.Module):
     """Parameters of one GCL (src/egnn.py:19-30): edge_mlp.{0,2}, node_mlp.{0,2}."""
 
@@ -39,22 +42,24 @@ class _CoordParams(nn.Module):
 
 
 class _BlockParams(nn.Module):
-    def __init__(self, hidden_nf, inv_sublayers, act):
+    def __init__(self, hidden_nf, inv_sublayers, act, edge_feat_nf):
         super().__init__()
         for s in range(inv_sublayers):
-            self.add_module(f"gcl_{s}", _GCLParams(hidden_nf, 2, act))
-        self.add_module("gcl_equiv", _CoordParams(hidden_nf, 2, act))
+            self.add_module(f"gcl_{s}", _GCLParams(hidden_nf, edge_feat_nf, act))
+        self.add_module("gcl_equiv", _CoordParams(hidden_nf, edge_feat_nf, act))
 
 
 class _EGNNParams(nn.Module):
-    """Parameter tree of EGNN (src/egnn.py:203-212)."""
+    """Parameter tree of EGNN (src/egnn.py:195-212): with sin_embedding every first layer reads 2 x 12 sinusoidal
+    features instead of the two distances (SinusoidsEmbeddingNew has no parameters)."""
 
-    def __init__(self, in_node_nf, hidden_nf, n_layers, inv_sublayers, act):
+    def __init__(self, in_node_nf, hidden_nf, n_layers, inv_sublayers, act, sin_embedding=False):
         super().__init__()
+        edge_feat_nf = 2 * SIN_EMBEDDING_DIM if sin_embedding else 2
         self.embedding = nn.Linear(in_node_nf, hidden_nf)
         self.embedding_out = nn.Linear(hidden_nf, in_node_nf)
         for l in range(n_layers):
-            self.add_module(f"e_block_{l}", _BlockParams(hidden_nf, inv_sublayers, act))
+            self.add_module(f"e_block_{l}", _BlockParams(hidden_nf, inv_sublayers, act, edge_feat_nf))
 
 
 class Dynamics(nn.Module):
@@ -68,9 +73,7 @@ class Dynamics(nn.Module):
         unsupported = []
         if model != 'egnn_dynamics': unsupported.append(f"model={model!r}")
         if attention: unsupported.append("attention=True")
-        if tanh: unsupported.append("tanh=True")
-        if sin_embedding: unsupported.append("sin_embedding=True")
-        if aggregation_method != 'sum': unsupported.append(f"aggregation_method={aggregation_method!r}")
+        if aggregation_method not in _native.AGGREGATIONS: unsupported.append(f"aggregation_method={aggregation_method!r}")
         # `normalization` is accepted and ignored exactly as the reference does for model='egnn_dynamics': it is only
         # forwarded to GNN (src/egnn.py:355-368); every configs/*.yml and train_difflinker.py's default set
         # normalization='batch_norm', so every published checkpoint carries it in its hyper-parameters.
@@ -88,12 +91,15 @@ class Dynamics(nn.Module):
         self.condition_time = condition_time
         self.norm_constant = norm_constant
         self.normalization_factor = normalization_factor
+        self.aggregation_method = aggregation_method
+        self.tanh = tanh
+        self.sin_embedding = sin_embedding
         self.model = model
         self.centering = centering
         self.graph_type = graph_type
         self.edge_impl = edge_impl
         self.dynamics = _EGNNParams(in_node_nf + context_node_nf + int(condition_time), hidden_nf, n_layers,
-                                    inv_sublayers, activation)
+                                    inv_sublayers, activation, sin_embedding=bool(sin_embedding))
         self._engine = None
         self._engine_key = None
 
@@ -103,6 +109,12 @@ class Dynamics(nn.Module):
 
     def _check_graph_type(self):
         assert self.graph_type == 'FC'  # src/egnn.py:383
+
+    def egnn_options(self):
+        """The EGNN options the engine is created with (dl_create_ex)."""
+        return _native.DLEgnnOptions(tanh=int(bool(self.tanh)), coords_range=_native.COORDS_RANGE,
+                                     sin_embedding=int(bool(self.sin_embedding)),
+                                     aggregation=_native.AGGREGATIONS[self.aggregation_method])
 
     def engine(self, device_index: int):
         """Creates the native engine on first use and re-uploads weights whenever a parameter changed."""
@@ -120,7 +132,7 @@ class Dynamics(nn.Module):
                 edge_impl=_native.EDGE_IMPLS[self.edge_impl], norm_constant=float(self.norm_constant),
                 normalization_factor=float(self.normalization_factor))
             handle = C.c_void_p()
-            _native.check(lib.dl_create(C.byref(cfg), C.byref(handle)), "dl_create")
+            _native.check(lib.dl_create_ex(C.byref(cfg), C.byref(self.egnn_options()), C.byref(handle)), "dl_create_ex")
             self._engine = handle
         for name, p in self.dynamics.state_dict().items():
             w = p.detach().to(device='cpu', dtype=torch.float32).contiguous()

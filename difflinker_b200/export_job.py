@@ -12,6 +12,7 @@ import torch
 from . import _native
 
 MAGIC = b"DLJOB1\0\0"
+MAGIC_OPTS = b"DLJOB2\0\0"   # a model with non-default EGNN options: the dl_egnn_options follow the dl_config
 
 
 def write_job(path, edm, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames, seed, offset=0,
@@ -30,13 +31,19 @@ def write_job(path, edm, x, h, node_mask, fragment_mask, linker_mask, edge_mask,
         centering=int(dyn.centering), graph_type=_native.GRAPH_TYPES[dyn.graph_type], device=device_index,
         edge_impl=_native.EDGE_IMPLS[dyn.edge_impl], norm_constant=float(dyn.norm_constant),
         normalization_factor=float(dyn.normalization_factor))
-    assert C.sizeof(cfg) == 13 * 4 and C.sizeof(_native.DLStepCoef) == 32
+    opts = dyn.egnn_options()
+    assert C.sizeof(cfg) == 13 * 4 and C.sizeof(_native.DLStepCoef) == 32 and C.sizeof(opts) == 16
     coef = edm.step_coefficients(keep_frames, B)
     f32 = lambda t: t.detach().to(device='cpu', dtype=torch.float32).contiguous().numpy().tobytes()
     i8 = lambda t: t.detach().to(device='cpu', dtype=torch.int8).contiguous().numpy().tobytes()
     with open(path, "wb") as f:
-        f.write(MAGIC)
-        f.write(bytes(cfg))
+        if opts.is_default():                          # jobs of default models keep the first version, byte for byte
+            f.write(MAGIC)
+            f.write(bytes(cfg))
+        else:
+            f.write(MAGIC_OPTS)
+            f.write(bytes(cfg))
+            f.write(bytes(opts))
         sd = dyn.dynamics.state_dict()
         f.write(struct.pack("<i", len(sd)))
         for name, p in sd.items():

@@ -5,8 +5,8 @@
  *
  *   c_sampler <job.bin> <out.bin>
  *
- * job.bin (little endian, written by difflinker_b200/export_job.py from a DDPM and a batch) holds the dl_config, the
- * weights under the reference's state_dict names, the normalised inputs and masks of one batch, the per-step
+ * job.bin (little endian, written by difflinker_b200/export_job.py from a DDPM and a batch) holds the dl_config (magic
+ * DLJOB2: followed by the model's dl_egnn_options -- tanh, mean aggregation), the weights under the reference's state_dict names, the normalised inputs and masks of one batch, the per-step
  * coefficient table of the noise schedule and a Philox (seed, offset) pair; the noise of the T+2 draws (2T+3 for
  * inpainting) is generated inside the kernels (dl_sample_chain_rng) in the order the reference's torch.randn calls would
  * have produced it on this GPU. out.bin: int32 status, uint64 philox offset consumed, the (keep_frames, B, N, 3+F) chain,
@@ -51,12 +51,15 @@ int main(int argc, char** argv) {
   if (!f) { perror(argv[1]); return 2; }
   char magic[8];
   rd(f, magic, 8);
-  if (memcmp(magic, "DLJOB1\0\0", 8) != 0) { fprintf(stderr, "c_sampler: not a job file\n"); return 2; }
+  const int with_opts = memcmp(magic, "DLJOB2\0\0", 8) == 0;
+  if (!with_opts && memcmp(magic, "DLJOB1\0\0", 8) != 0) { fprintf(stderr, "c_sampler: not a job file\n"); return 2; }
 
   dl_config cfg;
   rd(f, &cfg, sizeof cfg);                       /* 11 int32 + 2 float, no padding (checked by the exporter) */
+  dl_egnn_options opts;
+  if (with_opts) rd(f, &opts, sizeof opts);      /* 3 int32 + 1 float */
   dl_engine* e = NULL;
-  if (dl_create(&cfg, &e) < 0) die("dl_create");
+  if (dl_create_ex(&cfg, with_opts ? &opts : NULL, &e) < 0) die("dl_create_ex");
 
   int32_t n_weights;
   rd(f, &n_weights, 4);

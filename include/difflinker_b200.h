@@ -9,6 +9,7 @@
  *   reference interface (file:line)                      entry point here
  *   ---------------------------------------------------  ------------------------------------------
  *   Dynamics.__init__            src/egnn.py:324-372     dl_create / dl_destroy
+ *     tanh, sin_embedding, aggregation_method  egnn.py:101-106,281-292,304-320  dl_create_ex (dl_egnn_options)
  *   Dynamics.load_state_dict     (ckpt keys, SURVEY 8b)  dl_set_weight / dl_finalize_weights
  *   Dynamics.forward             src/egnn.py:374-447     dl_dynamics_forward (+ _host)
  *   DynamicsWithPockets.forward  src/egnn.py:471-552     dl_dynamics_forward with graph_type != DL_GRAPH_FC
@@ -48,6 +49,7 @@ typedef enum dl_status {
 enum { DL_GRAPH_FC = 0, DL_GRAPH_4A = 1, DL_GRAPH_FC_4A = 2, DL_GRAPH_FC_10A_4A = 3 };
 enum { DL_EDGE_AUTO = 0, DL_EDGE_SIMT = 1, DL_EDGE_WGMMA = 2 };
 enum { DL_SAMPLER_LINKER = 0, DL_SAMPLER_INPAINT = 1 };
+enum { DL_AGGR_SUM = 0, DL_AGGR_MEAN = 1 };
 
 /* Mirrors the kwargs of Dynamics.__init__ (src/egnn.py:324-329) that reach the hot path. */
 typedef struct dl_config {
@@ -81,10 +83,27 @@ typedef struct dl_step_coef {
   float pad;
 } dl_step_coef;
 
+/* EGNN options of the reference trainer (train_difflinker.py --tanh, --sin_embedding, --aggregation_method). */
+typedef struct dl_egnn_options {
+  int32_t tanh;                 /* 0/1: EquivariantUpdate bounds its update, trans = coord_diff * tanh(phi) * coords_range
+                                   (egnn.py:101-106) */
+  float coords_range;           /* 15: EGNN hands its own coords_range to every block (egnn.py:183,209) */
+  int32_t sin_embedding;        /* 0/1: every edge MLP's first layer reads the 24 features [sin, cos](sqrt(r + 1e-8) f_k),
+                                   f_k = 2 pi 4^k / 15, k < 6, of the block's and the input's radial r instead of the two
+                                   radials (SinusoidsEmbeddingNew, egnn.py:281-292); edge_mlp.0 / coord_mlp.0 weights are then
+                                   (H, 2H + 24) */
+  int32_t aggregation;          /* DL_AGGR_SUM: sum / normalization_factor; DL_AGGR_MEAN: sum / the row's edge count in the
+                                   reference's edge list (egnn.py:304-320) -- N on FC graphs, the cut-off degree (0 -> 1)
+                                   on pocket graphs; normalization_factor is then unused */
+} dl_egnn_options;
+
 const char* dl_version(void);
 const char* dl_last_error(void);
 
+/* dl_create(cfg, out) is dl_create_ex(cfg, NULL, out); opts == NULL means {tanh 0, coords_range 15, sin_embedding 0,
+ * DL_AGGR_SUM}, the reference's Dynamics defaults. */
 dl_status dl_create(const dl_config* cfg, dl_engine** out);
+dl_status dl_create_ex(const dl_config* cfg, const dl_egnn_options* opts, dl_engine** out);
 dl_status dl_destroy(dl_engine* e);
 
 /* `name` is the reference state_dict key relative to the Dynamics module, e.g.
