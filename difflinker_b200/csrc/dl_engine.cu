@@ -61,44 +61,9 @@ struct HostStage {  // device staging for the *_host entry points
   char* buf = nullptr;
 };
 
-}  // namespace
-
-struct dl_engine {
-  dl_config cfg{};
-  dl_egnn_options opts{};
-  int D = 0;
-  int num_sms = 0;
-  int max_threads_per_sm = 2048;
-  int slice_B_full = 0, slice_b0 = 0;   // dl_set_noise_slice: this engine samples rows [b0, b0 + B) of a B_full batch
-  bool finalized = false;
-  std::map<std::string, std::vector<float>> raw;
-  float* wblob = nullptr;      // packed fp32 weights
-  __half* wblob_tc = nullptr;  // packed fp16 hi/lo tiles
-  std::vector<GclW> gcl;       // [L*S]
-  std::vector<EqW> eq;         // [L]
-  const float *We_t = nullptr, *be = nullptr, *Wo = nullptr, *bo = nullptr;
-  Workspace ws;
-  cudaStream_t loop_stream = nullptr;
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
-  float* coef_dev = nullptr;
-  int coef_cap = 0;
-  int* step_ctr = nullptr;     // [2]: step_prep, step_fin
-  int64_t launches = 0;
-  HostStage stage;
-  bool use_tc = false;
-  // pointers of the most recent forward (for dl_time_edge_kernel)
-  const int8_t* last_edge_mask = nullptr;
-  const float* last_linker_mask = nullptr;
-  int last_B = 0, last_N = 0;
-};
-
-namespace {
-
-// edge-attribute columns of every edge MLP's first layer: [d, d0], or their 24 sinusoidal features
-int edges_in(const dl_engine* e) { return e->opts.sin_embedding ? N_SIN_FEAT : 2; }
-
 // DL_TIME_KERNELS=1: CUDA-event time of every launch of a (non-captured) forward, accumulated per kernel label and printed
-// when the engine is destroyed -- the live (warm-cache, back-to-back) counterpart of the ncu launch list.
+// when the engine is destroyed -- the live (warm-cache, back-to-back) counterpart of the ncu launch list. One record per
+// engine, so engines driven from separate host threads (EDM.devices) share no state.
 struct KernelTimes {
   bool on = false;
   struct Rec { const char* label; cudaEvent_t a, b; };
@@ -140,8 +105,45 @@ struct KernelTimes {
               1e3 * kv.second.first / kv.second.second, 100.0 * kv.second.first / tot);
   }
 };
-KernelTimes g_times;
-#define TIMED(label, stream, stmt) do { g_times.begin(stream, label); stmt; g_times.end(stream); } while (0)
+
+}  // namespace
+
+struct dl_engine {
+  dl_config cfg{};
+  dl_egnn_options opts{};
+  int D = 0;
+  int num_sms = 0;
+  int max_threads_per_sm = 2048;
+  int slice_B_full = 0, slice_b0 = 0;   // dl_set_noise_slice: this engine samples rows [b0, b0 + B) of a B_full batch
+  bool finalized = false;
+  std::map<std::string, std::vector<float>> raw;
+  float* wblob = nullptr;      // packed fp32 weights
+  __half* wblob_tc = nullptr;  // packed fp16 hi/lo tiles
+  std::vector<GclW> gcl;       // [L*S]
+  std::vector<EqW> eq;         // [L]
+  const float *We_t = nullptr, *be = nullptr, *Wo = nullptr, *bo = nullptr;
+  Workspace ws;
+  cudaStream_t loop_stream = nullptr;
+  cudaEvent_t ev_in = nullptr, ev_out = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
+  float* coef_dev = nullptr;
+  int coef_cap = 0;
+  int* step_ctr = nullptr;     // [2]: step_prep, step_fin
+  int64_t launches = 0;
+  HostStage stage;
+  KernelTimes times;           // DL_TIME_KERNELS
+  bool use_tc = false;
+  // pointers of the most recent forward (for dl_time_edge_kernel)
+  const int8_t* last_edge_mask = nullptr;
+  const float* last_linker_mask = nullptr;
+  int last_B = 0, last_N = 0;
+};
+
+namespace {
+
+// edge-attribute columns of every edge MLP's first layer: [d, d0], or their 24 sinusoidal features
+int edges_in(const dl_engine* e) { return e->opts.sin_embedding ? N_SIN_FEAT : 2; }
+
+#define TIMED(label, stream, stmt) do { e->times.begin(stream, label); stmt; e->times.end(stream); } while (0)
 
 struct ExpectedParam {
   std::string name;
@@ -513,9 +515,9 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     for (int s = 0; s < S; ++s) {
       const GclW& w = e->gcl[l * S + s];
       const EdgeArgs ea = edge_args(e, w, false, io.edge_mask, io.linker_mask, xin, xin4);
-      g_times.begin(st, "edge GCL");
+      e->times.begin(st, "edge GCL");
       dl_status st2 = launch_edge(e, gm, ea, false, w.W2_tc, st);
-      g_times.end(st);
+      e->times.end(st);
       if (st2 != DL_OK) return st2;
 
       if (e->use_tc) {
@@ -538,9 +540,9 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     e->launches += 1;
     const EqW& w = e->eq[l];
     const EdgeArgs ea = edge_args(e, w, true, io.edge_mask, io.linker_mask, xin, xin4, xout, xout4, w.w5);
-    g_times.begin(st, "edge COORD");
+    e->times.begin(st, "edge COORD");
     dl_status st2 = launch_edge(e, gm, ea, true, w.W2_tc, st);
-    g_times.end(st);
+    e->times.end(st);
     if (st2 != DL_OK) return st2;
     std::swap(xin, xout);
     std::swap(xin4, xout4);
@@ -716,7 +718,7 @@ dl_status dl_create_ex(const dl_config* cfg, const dl_egnn_options* opts, dl_eng
   CK(opt_in_edge_simt<true>());
   CK(opt_in_edge_simt<false>());
   CK(cudaFuncSetAttribute(k_nbr, cudaFuncAttributeMaxDynamicSharedMemorySize, 4000 * CUT_SMEM_PER_NODE));
-  if (getenv("DL_TIME_KERNELS")) g_times.on = true;
+  if (getenv("DL_TIME_KERNELS")) e->times.on = true;
   if (const char* v = getenv("DL_WAIT_MODE")) { const int m = atoi(v); cudaMemcpyToSymbol(tc::c_wait_mode, &m, sizeof(int)); }
   if (const char* v = getenv("DL_CHAIN_OVERLAP")) chain_overlap_enabled() = atoi(v) != 0;   // 0: plain stream order between kernels
   dl_status s = tc::configure();
@@ -728,8 +730,7 @@ dl_status dl_create_ex(const dl_config* cfg, const dl_egnn_options* opts, dl_eng
 
 dl_status dl_destroy(dl_engine* e) {
   if (!e) return DL_OK;
-  g_times.report();
-  g_times.acc.clear();
+  e->times.report();
   cudaSetDevice(e->cfg.device);
   cudaDeviceSynchronize();
   free_workspace(e->ws);
@@ -830,7 +831,7 @@ dl_status dl_dynamics_forward(dl_engine* e, int32_t B, int32_t N, const float* t
   io.edge_mask = edge_mask; io.context = context; io.nan_flags = nan_flags;
   if ((s = enqueue_forward(e, B, N, io, st)) != DL_OK) return s;
   CK(cudaEventRecord(e->ev_t1, st));
-  g_times.collect(st);
+  e->times.collect(st);
   return DL_OK;
 }
 

@@ -6,6 +6,7 @@ Two ways in:
     (`edm.gamma.gamma`, `edm.dynamics.dynamics....`), for environments without pytorch_lightning;
   * `accelerate(ddpm)` -- swaps the `.edm` of an existing *reference* DDPM (e.g. one returned by
     `DDPM.load_from_checkpoint`) for the native one in place, so generate.py / sample.py run unchanged.
+Both take `devices=[...]` (or 'all') to split every sampling batch over several local GPUs from one process.
 Training, datasets, metrics and visualisation are out of scope (SURVEY.md section 2).
 """
 import torch
@@ -103,9 +104,10 @@ class DDPM(nn.Module):
         test_epochs=None, n_stability_samples=None,
         normalization=None, log_iterations=None, samples_dir=None, data_augmentation=False,
         center_of_mass='fragments', inpainting=False, anchors_context=True, graph_type=None, edge_impl='auto',
+        devices=None,
     ):
         super().__init__()
-        self.hparams = {k: v for k, v in locals().items() if k not in ('self', '__class__', 'edge_impl')}
+        self.hparams = {k: v for k, v in locals().items() if k not in ('self', '__class__', 'edge_impl', 'devices')}
         self.data_path, self.train_data_prefix, self.val_data_prefix = data_path, train_data_prefix, val_data_prefix
         self.batch_size, self.lr, self.torch_device = batch_size, lr, torch_device
         self.include_charges = include_charges
@@ -118,6 +120,7 @@ class DDPM(nn.Module):
         self.anchors_context = anchors_context
         self.is_geom = ('geom' in train_data_prefix) or ('MOAD' in train_data_prefix)
         self.edm = _build_edm(self.hparams, edge_impl=edge_impl)
+        self.edm.devices = devices          # EDM.devices: split each sampling batch over these CUDA devices
 
     def sample_chain(self, data, sample_fn=None, keep_frames=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames)
@@ -149,14 +152,17 @@ def _load_lightning_checkpoint(cls, checkpoint_path, map_location, strict, overr
     return model
 
 
-def accelerate(ddpm, edge_impl='auto'):
+def accelerate(ddpm, edge_impl='auto', devices=None):
     """Replace `ddpm.edm` of a *reference* DDPM (src/lightning.py) by the native EDM, copying its weights
-    (strict state_dict match) and its possibly overridden `.T` (generate.py:103-104). Returns `ddpm`."""
+    (strict state_dict match) and its possibly overridden `.T` (generate.py:103-104). Returns `ddpm`.
+    `devices` (a list of CUDA device indices, or 'all') makes `ddpm.sample_chain` split each batch over those devices from
+    this one process (EDM.devices); None samples on the data's device."""
     hp = dict(ddpm.hparams) if hasattr(ddpm, 'hparams') and len(dict(ddpm.hparams)) else None
     if hp is None:
         raise ValueError("the module carries no hparams; construct difflinker_b200.DDPM(**hparams) instead")
     new_edm = _build_edm(hp, edge_impl=edge_impl)
     new_edm.load_state_dict(ddpm.edm.state_dict(), strict=True)
     new_edm.T = ddpm.edm.T
+    new_edm.devices = devices
     ddpm.edm = new_edm
     return ddpm

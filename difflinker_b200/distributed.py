@@ -1,6 +1,9 @@
 """Replica-level data parallelism (SURVEY.md section 8(e)): molecules never interact across a batch, so sampling shards
 with no data-path collective. The only exchange is one broadcast of the weights at start-up (NCCL on GPUs,
-gloo in the CPU tests); optionally the final results are gathered."""
+gloo in the CPU tests); optionally the final results are gathered. `resolve_devices`, `device_slices` and `place_rows` plan and
+gather the split of one batch over several local GPUs that `EDM.devices` makes from a single process."""
+import operator
+
 import torch
 import torch.distributed as dist
 
@@ -10,6 +13,53 @@ def shard_range(n_items: int, rank: int, world: int):
     base, extra = divmod(n_items, world)
     lo = rank * base + min(rank, extra)
     return lo, lo + base + (1 if rank < extra else 0)
+
+
+def resolve_devices(devices, device_count=None):
+    """`EDM.devices` as a list of CUDA device indices: None stays None (the caller's device), 'all' is every visible device,
+    otherwise a non-empty list of visible indices (one may repeat: each listing gets an engine of its own)."""
+    if devices is None:
+        return None
+    n = torch.cuda.device_count() if device_count is None else device_count
+    if isinstance(devices, str):
+        if devices != 'all':
+            raise ValueError(f"devices must be a list of CUDA device indices, 'all' or None (got {devices!r})")
+        if n == 0:
+            raise ValueError("devices='all': no CUDA device is visible")
+        return list(range(n))
+    out = []
+    for d in devices:
+        if isinstance(d, bool):
+            raise TypeError(f"CUDA device indices are integers (got {d!r})")
+        d = operator.index(d)
+        if not 0 <= d < n:
+            raise ValueError(f"unknown CUDA device {d} ({n} visible)")
+        out.append(d)
+    if not out:
+        raise ValueError("devices is empty: list at least one CUDA device, or pass None for the caller's device")
+    return out
+
+
+def device_slices(n_items: int, devices):
+    """The split of one batch over `devices`: [(device, replica, lo, hi)], slot i getting shard_range(n_items, i, len(devices)).
+    `replica` counts earlier listings of the same device (each listing has an engine of its own); slots whose slice would be
+    empty (n_items < len(devices)) are left out."""
+    out, seen = [], {}
+    for i, d in enumerate(devices):
+        lo, hi = shard_range(n_items, i, len(devices))
+        replica = seen.get(d, 0)
+        seen[d] = replica + 1
+        if hi > lo:
+            out.append((d, replica, lo, hi))
+    return out
+
+
+def place_rows(out: torch.Tensor, parts, slices, dim: int = 0):
+    """Copies every slice's result into rows [lo, hi) of `out` along `dim` (stream-ordered, also across devices); returns `out`.
+    Per-molecule NaN flags placed this way carry batch-global molecule indices."""
+    for part, (_, _, lo, hi) in zip(parts, slices):
+        out.narrow(dim, lo, hi - lo).copy_(part)
+    return out
 
 
 def batch_ids_for_rank(n_batches: int, rank: int, world: int):
@@ -63,8 +113,9 @@ def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=T
     """Strong scaling of ONE batch (SURVEY.md section 8(e)): the template batch is built once (so every rank pads to the same
     N), each rank runs the reverse loop for its contiguous slice of the molecules with the slice's rows of the full-batch
     noise, and the chains are gathered -- the result equals `model.sample_chain(data)` on one GPU bit for bit, for any
-    world size. No collective inside the loop. Returns (chain, node_mask) with the full batch on every rank when
-    `gather`, else the local slice."""
+    world size, on the SIMT path and on the tensor-core path while no sample diverges far enough for the node GEMM to
+    rescale a tile's fp16 operands (DESIGN.md section 6). No collective inside the loop. Returns (chain, node_mask) with
+    the full batch on every rank when `gather`, else the local slice."""
     from .ddpm import sampler_inputs
     kw = sampler_inputs(model, data, sample_fn)
     B = kw['x'].shape[0]

@@ -7,21 +7,24 @@ are made with the reference's `torch.randn` call order and shapes (edm.py:328-34
 torch seed produces the same noise stream as the reference would on that device.
 """
 import ctypes as C
+import threading
 
 import torch
 import torch.nn.functional as F
 
 from . import _native
+from .distributed import device_slices, place_rows, resolve_devices, slice_sampler_inputs
 from .noise import PredefinedNoiseSchedule
 from .utils import FoundNaNException, nan_exception_class
 
 
-def _sample_chain_rng(lib, eng, dev, batch_slice, head, tail):
-    """dl_sample_chain_rng(eng, *head, seed, offset, &consumed, *tail) from the state of `dev`'s default CUDA generator, with
-    the engine's batch slice set for the duration of the call; then advances the generator as if the reference's randn
-    calls had run."""
-    gen = torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
-    seed, offset = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF, gen.get_offset()
+def _generator_of(dev):
+    return torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
+
+
+def _run_chain_rng(lib, eng, batch_slice, seed, offset, head, tail):
+    """dl_sample_chain_rng(eng, *head, seed, offset, &consumed, *tail) with the engine's batch slice set for the duration of
+    the call; returns what the draws consumed."""
     used = C.c_uint64(0)
     if batch_slice is not None:
         _native.check(lib.dl_set_noise_slice(eng, int(batch_slice[1]), int(batch_slice[0])), "dl_set_noise_slice")
@@ -31,7 +34,42 @@ def _sample_chain_rng(lib, eng, dev, batch_slice, head, tail):
         if batch_slice is not None:
             lib.dl_set_noise_slice(eng, 0, 0)
     _native.check(st, "dl_sample_chain_rng")
-    gen.set_offset(offset + used.value)
+    return used.value
+
+
+def _sample_chain_rng(lib, eng, dev, batch_slice, head, tail):
+    """_run_chain_rng from the state of `dev`'s default CUDA generator; then advances the generator as if the reference's
+    randn calls had run."""
+    gen = _generator_of(dev)
+    seed, offset = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF, gen.get_offset()
+    used = _run_chain_rng(lib, eng, batch_slice, seed, offset, head, tail)
+    gen.set_offset(offset + used)
+
+
+def _run_per_device(calls_by_device):
+    """Runs each device's calls, in order, on a host thread of its own (the C-ABI allows one host thread per engine, and ctypes
+    releases the GIL), so every device's reverse loop is enqueued even if one device's enqueue blocks. Every thread is joined
+    before the first error is re-raised."""
+    errors = []
+
+    def run(calls):
+        try:
+            for call in calls:
+                call()
+        except BaseException as e:                      # re-raised on the caller's thread below
+            errors.append(e)
+    threads = [threading.Thread(target=run, args=(calls,), name=f"difflinker_b200-cuda{d}")
+               for d, calls in calls_by_device.items()]
+    started = []
+    try:
+        for t in threads:
+            t.start()
+            started.append(t)
+    finally:
+        for t in started:
+            t.join()
+    if errors:
+        raise errors[0]
 
 
 class EDM(torch.nn.Module):
@@ -65,7 +103,25 @@ class EDM(torch.nn.Module):
         # 'reference_tensor': the same stream materialised with torch.randn (two launches per draw).
         # 'bulk': one randn call for the whole chain (a different stream).
         self.noise_mode = 'reference_stream'
-        self.last_loop_ms = None               # device time of the last reverse loop (CUDA events)
+        self.devices = None
+        self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
+        self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
+
+    @property
+    def devices(self):
+        """None (the default): sample on the inputs' device. A list of CUDA device indices, or 'all' when set: sample_chain
+        splits each batch into contiguous, balanced slices, one per listed device, samples them concurrently and returns the
+        whole chain on the inputs' device. That chain is the one a single device samples, bit for bit on the fp32 SIMT edge
+        path, and on the tensor-core path while no sample diverges: the node GEMM rescales the fp16 operands of a tile by a
+        power of two chosen from the tile's maximum once values approach the fp16 range, and since tiles span molecules and
+        follow the batch, such molecules round differently after a split (DESIGN.md section 6). A device may be listed more
+        than once: each listing gets an engine of its own, and engines sharing a device run their loops one after the other.
+        Calls without `devices` keep one engine, so switching between split and single-device calls re-creates engines."""
+        return self._devices
+
+    @devices.setter
+    def devices(self, devices):
+        self._devices = resolve_devices(devices)
 
     def forward(self, *args, **kwargs):
         raise NotImplementedError("training (src/edm.py:41-124) is outside the difflinker_b200 hot path")
@@ -170,54 +226,78 @@ class EDM(torch.nn.Module):
         """A draw_noise replaced on the instance supplies the draws instead of the device-side stream."""
         return 'draw_noise' in self.__dict__
 
-    @torch.no_grad()
-    def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None):
-        """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
-        final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
-        `batch_slice=(b0, B_full)`: the inputs are rows [b0, b0+B) of a batch of B_full molecules (strong scaling,
-        distributed.sample_chain_sharded); the device-side noise is then those rows of the full batch's draws."""
-        lib = _native.load_library()
+    def _sampler_tensors(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context):
+        """The engine's inputs on x's device, as keyword arguments of `distributed.slice_sampler_inputs`: the normalised xh
+        (B,N,3+F) fp32 under 'x', the node mask int8, fragment / linker masks fp32, the flattened FC edge mask int8 (None on
+        cut-off graphs) and the context fp32."""
         n_samples, n_nodes = x.size(0), x.size(1)
         dev = x.device
-        T = self.T
-        if keep_frames is None:
-            keep_frames = T
-        else:
-            assert keep_frames <= T
-        d = self.n_dims + self.in_node_nf
         xn, hn = self.normalize(x, h)
         xh = torch.cat([xn, hn], dim=2).to(torch.float32).contiguous()
-        # device-side stream unless a tensor is injected (tests), the draw function is replaced, or another mode is set
-        on_device = (noise is None and dev.type == 'cuda' and self.noise_mode == 'reference_stream'
-                     and not self._draws_replaced())
-        if batch_slice is not None and not on_device:
-            raise ValueError("batch_slice needs the device-side noise stream (CUDA tensors, noise_mode='reference_stream')")
-        if not on_device:
-            if noise is None:
-                noise = self._draw_tensor(n_samples, n_nodes, dev, node_mask, fragment_mask)
-            noise = noise.to(device=dev, dtype=torch.float32).contiguous()
-            assert noise.shape == (self._n_draws(), n_samples, n_nodes, d), noise.shape
-
-        eng = self.dynamics.engine(self.dynamics._device_index(x))
-        self.dynamics._check_graph_type()
         prep = lambda v, dt: None if v is None else v.detach().to(device=dev, dtype=dt).contiguous()
-        nm = prep(node_mask.reshape(n_samples, n_nodes), torch.int8)
-        fm = prep(fragment_mask.reshape(n_samples, n_nodes), torch.float32)
-        lm = prep(linker_mask.reshape(n_samples, n_nodes), torch.float32)
         em = None
         if self.dynamics.graph_type == 'FC' and edge_mask is not None:
             em = prep(edge_mask.reshape(-1), torch.int8)
             assert em.numel() == n_samples * n_nodes * n_nodes
         ctx = None if context is None else prep(
             context.reshape(n_samples, n_nodes, self.dynamics.context_node_nf), torch.float32)   # wrong width -> raises
+        return dict(x=xh, node_mask=prep(node_mask.reshape(n_samples, n_nodes), torch.int8),
+                    fragment_mask=prep(fragment_mask.reshape(n_samples, n_nodes), torch.float32),
+                    linker_mask=prep(linker_mask.reshape(n_samples, n_nodes), torch.float32), edge_mask=em, context=ctx)
+
+    def _noise(self, noise, x, node_mask, fragment_mask):
+        """(on_device, noise): the device-side stream unless a tensor is injected (tests), the draw function is replaced, or
+        another mode is set; otherwise the whole batch's draws on x's device."""
+        n_samples, n_nodes = x.size(0), x.size(1)
+        dev = x.device
+        on_device = (noise is None and dev.type == 'cuda' and self.noise_mode == 'reference_stream'
+                     and not self._draws_replaced())
+        if not on_device:
+            if noise is None:
+                noise = self._draw_tensor(n_samples, n_nodes, dev, node_mask, fragment_mask)
+            noise = noise.to(device=dev, dtype=torch.float32).contiguous()
+            assert noise.shape == (self._n_draws(), n_samples, n_nodes, self.n_dims + self.in_node_nf), noise.shape
+        return on_device, noise
+
+    def _head(self, n_samples, n_nodes, keep_frames, t):
+        ptr = lambda v: None if v is None else v.data_ptr()
+        return (self._SAMPLER, n_samples, n_nodes, self.T, keep_frames, ptr(t['x']), ptr(t['node_mask']),
+                ptr(t['fragment_mask']), ptr(t['linker_mask']), ptr(t['edge_mask']), ptr(t['context']))
+
+    def _norm(self):
+        return (C.c_float * 3)(float(self.norm_values[0]), float(self.norm_values[1]), float(self.norm_biases[1]))
+
+    @torch.no_grad()
+    def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
+                     noise=None, batch_slice=None):
+        """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
+        final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
+        `batch_slice=(b0, B_full)`: the inputs are rows [b0, b0+B) of a batch of B_full molecules (strong scaling,
+        distributed.sample_chain_sharded); the device-side noise is then those rows of the full batch's draws.
+        With `devices` set (and no batch_slice) the batch is split over those devices (_sample_chain_split)."""
+        if keep_frames is None:
+            keep_frames = self.T
+        else:
+            assert keep_frames <= self.T
+        if self.devices is not None and batch_slice is None:
+            return self._sample_chain_split(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames, noise)
+        lib = _native.load_library()
+        n_samples, n_nodes = x.size(0), x.size(1)
+        dev = x.device
+        d = self.n_dims + self.in_node_nf
+        t = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
+        on_device, noise = self._noise(noise, x, node_mask, fragment_mask)
+        if batch_slice is not None and not on_device:
+            raise ValueError("batch_slice needs the device-side noise stream (CUDA tensors, noise_mode='reference_stream')")
+
+        eng = self.dynamics.engine(self.dynamics._device_index(x))
+        self.dynamics._check_graph_type()
         coef = self.step_coefficients(keep_frames, n_samples)
-        norm = (C.c_float * 3)(float(self.norm_values[0]), float(self.norm_values[1]), float(self.norm_biases[1]))
         chain = torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32)
         flags = torch.zeros(n_samples, dtype=torch.int32, device=dev)
         ptr = lambda v: None if v is None else v.data_ptr()
-        head = (self._SAMPLER, n_samples, n_nodes, T, keep_frames, ptr(xh), ptr(nm), ptr(fm), ptr(lm), ptr(em), ptr(ctx))
-        tail = (coef, norm, ptr(chain), ptr(flags))
+        head = self._head(n_samples, n_nodes, keep_frames, t)
+        tail = (coef, self._norm(), ptr(chain), ptr(flags))
         if dev.type == 'cuda':
             with torch.cuda.device(dev):
                 stream = torch.cuda.current_stream(dev).cuda_stream
@@ -231,8 +311,88 @@ class EDM(torch.nn.Module):
             _native.check(st, "dl_sample_chain_host")
             bad = st == _native.DL_NAN_DETECTED
         self.last_loop_ms = float(lib.dl_last_elapsed_ms(eng))
+        self.last_slice_loop_ms = None
         if bad:
             raise nan_exception_class()(flags=flags.cpu().tolist())
+        return chain
+
+    def _sample_chain_split(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames, noise):
+        """sample_chain over `devices`: the inputs are prepared and the noise is chosen once, on x's device, as for one device;
+        slot i of `devices` samples molecules shard_range(B, i, len(devices)) on its own engine, with the full batch's step
+        coefficients and either batch_slice=(lo, B) from the caller's generator state or its rows of the noise tensor. Each
+        device's loops are enqueued from a thread of its own; the chains and NaN flags are then copied back into rows
+        [lo, hi) on x's device, and the caller's generator advances once, by what one device would have consumed."""
+        lib = _native.load_library()
+        n_samples, n_nodes = x.size(0), x.size(1)
+        dev = x.device
+        d = self.n_dims + self.in_node_nf
+        self.dynamics._check_graph_type()
+        full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
+        on_device, noise = self._noise(noise, x, node_mask, fragment_mask)
+        slices = device_slices(n_samples, self.devices)
+        if not slices:
+            raise ValueError("sample_chain needs at least one molecule")
+        if on_device:
+            # the device-side stream reproduces torch's randn launch geometry, which depends on the device's SM count
+            geometry = lambda i: (torch.cuda.get_device_properties(i).multi_processor_count,
+                                  torch.cuda.get_device_properties(i).max_threads_per_multi_processor)
+            caller = geometry(_generator_of(dev).device.index)
+            odd = sorted({s[0] for s in slices if geometry(s[0]) != caller})
+            if odd:
+                raise ValueError(f"devices {odd} differ from {dev} in SM count or threads per SM, so they cannot reproduce its "
+                                 "noise stream; list devices of one model, or inject the noise")
+            gen = _generator_of(dev)
+            seed, offset = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF, gen.get_offset()
+        coef = self.step_coefficients(keep_frames, n_samples)
+        norm = self._norm()
+        ptr = lambda v: None if v is None else v.data_ptr()
+        calls, inputs, chains, flags, consumed = {}, [], [], [], []
+        engines = self.dynamics.engines([(dev_i, replica) for dev_i, replica, _, _ in slices])
+        for (dev_i, replica, lo, hi), eng in zip(slices, engines):
+            cuda_i = torch.device('cuda', dev_i)
+            with torch.cuda.device(cuda_i):
+                t = {k: None if v is None else v.to(cuda_i).contiguous() for k, v in slice_sampler_inputs(full, lo, hi).items()}
+                nz = None if on_device else noise[:, lo:hi].to(cuda_i).contiguous()
+                chain_i = torch.empty((keep_frames, hi - lo, n_nodes, d), device=cuda_i, dtype=torch.float32)
+                flags_i = torch.zeros(hi - lo, dtype=torch.int32, device=cuda_i)
+                stream = torch.cuda.current_stream(cuda_i).cuda_stream
+            head = self._head(hi - lo, n_nodes, keep_frames, t)
+            tail = (coef, norm, ptr(chain_i), ptr(flags_i))
+            if on_device:
+                call = (lambda eng=eng, lo=lo, head=head, tail=tail, stream=stream:
+                        consumed.append(_run_chain_rng(lib, eng, (lo, n_samples), seed, offset, head, tail + (stream,))))
+            else:
+                call = (lambda eng=eng, head=head, nz=nz, tail=tail, stream=stream:
+                        _native.check(lib.dl_sample_chain(eng, *head, ptr(nz), *tail, stream), "dl_sample_chain"))
+            calls.setdefault(dev_i, []).append(call)
+            inputs.append((t, nz))          # alive until the loops are done (the host waits on the flags below)
+            chains.append(chain_i)
+            flags.append(flags_i)
+        try:
+            _run_per_device(calls)
+        except BaseException:
+            for dev_i in calls:             # let the loops that were enqueued finish before their inputs are released
+                try:
+                    torch.cuda.synchronize(dev_i)
+                except Exception:
+                    pass
+            raise
+        if on_device:
+            assert len(set(consumed)) == 1, consumed
+            gen.set_offset(offset + consumed[0])
+        chain = place_rows(torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32), chains, slices,
+                           dim=1)
+        all_flags = place_rows(torch.zeros(n_samples, dtype=torch.int32, device=dev), flags, slices)
+        bad = bool(all_flags.any().item())  # waits for every slice's loop and copy
+        loop_ms = []
+        for (dev_i, _, lo, hi), eng in zip(slices, engines):
+            with torch.cuda.device(dev_i):
+                loop_ms.append((dev_i, lo, hi, float(lib.dl_last_elapsed_ms(eng))))
+        self.last_slice_loop_ms = loop_ms
+        self.last_loop_ms = max(ms for *_, ms in loop_ms)
+        del inputs
+        if bad:
+            raise nan_exception_class()(flags=all_flags.cpu().tolist())
         return chain
 
 

@@ -100,12 +100,19 @@ class Dynamics(nn.Module):
         self.edge_impl = edge_impl
         self.dynamics = _EGNNParams(in_node_nf + context_node_nf + int(condition_time), hidden_nf, n_layers,
                                     inv_sublayers, activation, sin_embedding=bool(sin_embedding))
-        self._engine = None
-        self._engine_key = None
+        self._engines = {}          # (device index, replica) -> (handle, (edge_impl, weights version) uploaded)
+        self._host_weights = None   # (weights version, [(name, fp32 CPU tensor)]): read once, uploaded to every engine
 
     # ---- native engine management -------------------------------------------------------------------------
     def _weights_version(self):
         return tuple((p.data_ptr(), p._version) for p in self.dynamics.parameters())
+
+    def _weights_on_host(self, version):
+        """The parameters as fp32 host tensors under their C-ABI names, read from the module once per weights version."""
+        if self._host_weights is None or self._host_weights[0] != version:
+            self._host_weights = (version, [(f"dynamics.{name}".encode(), p.detach().to(device='cpu', dtype=torch.float32).contiguous())
+                                            for name, p in self.dynamics.state_dict().items()])
+        return self._host_weights[1]
 
     def _check_graph_type(self):
         assert self.graph_type == 'FC'  # src/egnn.py:383
@@ -117,13 +124,31 @@ class Dynamics(nn.Module):
                                      aggregation=_native.AGGREGATIONS[self.aggregation_method])
 
     def engine(self, device_index: int):
-        """Creates the native engine on first use and re-uploads weights whenever a parameter changed."""
+        """Creates the native engine on first use and re-uploads weights whenever a parameter changed. A module used on one
+        device keeps one engine: engines of other devices (the device the module was on before, or the slices of a split
+        batch) are destroyed."""
+        self._release_all_but({(device_index, 0)})
+        return self._engine_at(device_index, 0)
+
+    def engines(self, slots):
+        """The engines of `slots` [(device, replica)], for a batch split over several devices (EDM.devices): replica > 0 are
+        further engines on the same device, for a device listed more than once. Every engine gets the same host copy of the
+        weights; the module's engines outside `slots` are destroyed."""
+        self._release_all_but(set(slots))
+        out = []
+        for device_index, replica in slots:
+            with torch.cuda.device(device_index):            # dl_create_ex selects the device on the calling thread
+                out.append(self._engine_at(device_index, replica))
+        return out
+
+    def _engine_at(self, device_index: int, replica: int):
         lib = _native.load_library()
-        key = (device_index, self.edge_impl, self._weights_version())
-        if self._engine is not None and self._engine_key == key:
-            return self._engine
-        if self._engine is None or self._engine_key[:2] != key[:2]:
-            self.close()
+        slot, key = (device_index, replica), (self.edge_impl, self._weights_version())
+        handle, uploaded = self._engines.get(slot, (None, None))
+        if handle is not None and uploaded == key:
+            return handle
+        if handle is None or uploaded is None or uploaded[0] != key[0]:
+            self._destroy(slot)
             cfg = _native.DLConfig(
                 n_dims=self.n_dims, in_node_nf=self.in_node_nf, context_node_nf=self.context_node_nf,
                 hidden_nf=self.hidden_nf, n_layers=self.n_layers, inv_sublayers=self.inv_sublayers,
@@ -133,20 +158,26 @@ class Dynamics(nn.Module):
                 normalization_factor=float(self.normalization_factor))
             handle = C.c_void_p()
             _native.check(lib.dl_create_ex(C.byref(cfg), C.byref(self.egnn_options()), C.byref(handle)), "dl_create_ex")
-            self._engine = handle
-        for name, p in self.dynamics.state_dict().items():
-            w = p.detach().to(device='cpu', dtype=torch.float32).contiguous()
-            _native.check(lib.dl_set_weight(self._engine, f"dynamics.{name}".encode(), w.data_ptr(), w.numel()),
-                          f"dl_set_weight({name})")
-        _native.check(lib.dl_finalize_weights(self._engine), "dl_finalize_weights")
-        self._engine_key = key
-        return self._engine
+            self._engines[slot] = (handle, None)
+        for name, w in self._weights_on_host(key[1]):
+            _native.check(lib.dl_set_weight(handle, name, w.data_ptr(), w.numel()), f"dl_set_weight({name.decode()})")
+        _native.check(lib.dl_finalize_weights(handle), "dl_finalize_weights")
+        self._engines[slot] = (handle, key)
+        return handle
+
+    def _release_all_but(self, keep):
+        for slot in [slot for slot in self._engines if slot not in keep]:
+            self._destroy(slot)
+
+    def _destroy(self, slot):
+        handle, _ = self._engines.pop(slot, (None, None))
+        if handle is not None:
+            _native.load_library().dl_destroy(handle)
 
     def close(self):
-        if self._engine is not None:
-            _native.load_library().dl_destroy(self._engine)
-            self._engine = None
-            self._engine_key = None
+        for slot in list(getattr(self, '_engines', {})):
+            self._destroy(slot)
+        self._host_weights = None
 
     def __del__(self):
         try:

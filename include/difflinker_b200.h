@@ -190,7 +190,9 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
 /* Strong scaling (SURVEY 8(e)): this engine samples molecules [b0, b0 + B) of a batch of B_full. The device-side noise of
  * the following dl_sample_chain_rng / dl_noise_fill / dl_noise_fill_inpaint calls is then the slice's ROWS of the
  * full-batch draws (and offset_consumed is the full batch's), so the gathered result is bit-identical to the single-GPU
- * run whatever the split. B_full = 0 switches it off. */
+ * run whatever the split -- on the SIMT path, and on the tensor-core path while no sample diverges far enough for the node
+ * GEMM to rescale a tile's fp16 operands (tiles span molecules, so the split moves them; DESIGN.md section 6). B_full = 0
+ * switches it off. */
 dl_status dl_set_noise_slice(dl_engine* e, int32_t B_full, int32_t b0);
 /* The (n_draws,B,N,3+F) tensor the device-side stream of dl_sample_chain_rng stands for (tests, debugging). DEVICE out. */
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
