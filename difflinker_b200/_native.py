@@ -55,6 +55,7 @@ SYMBOLS = {
     "dl_sample_chain": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "dl_sample_chain_rng": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, _P, _P, _P, _P,
                                    _P, _P]),
+    "dl_sample_chain_seeded": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "dl_set_noise_slice": (_I32, [_P, _I32, _I32]),
     "dl_noise_fill": (_I32, [_P, _I32, _I32, _I32, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "dl_noise_fill_inpaint": (_I32, [_P, _I32, _I32, _I32, _P, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),

@@ -53,6 +53,7 @@ struct Workspace {
   int4* items = nullptr;
   int4* xitems = nullptr;
   int* tile_ctr = nullptr;
+  unsigned long long* seeds = nullptr;   // dl_sample_chain_seeded: the call's B seeds, read by the captured step
   std::vector<void*> allocs;
 };
 
@@ -298,7 +299,7 @@ dl_status ensure_workspace(dl_engine* e, int B, int N) {
   WSA(nm, n); WSA(x0, n * 3); WSA(xa, n * 3); WSA(xb, n * 3); WSA(h, n * H); WSA(ABg, n * 2 * H); WSA(ABc, n * 2 * H);
   WSA(agg, n * H); WSA(z, n * xd); WSA(eps, n * xd); WSA(cls, n); WSA(x04, n); WSA(xa4, n); WSA(xb4, n); WSA(ABgmax, n * 2); WSA(ABcmax, n * 2);
   WSA(rowidx, n); WSA(colidx, n); WSA(xrowidx, n); WSA(nr, B); WSA(nc, B); WSA(nxr, B); WSA(n_items, 1);
-  WSA(xmols, B); WSA(n_xmols, 1); WSA(items, n); WSA(xitems, n); WSA(n_xitems, 1); WSA(tile_ctr, 64);
+  WSA(xmols, B); WSA(n_xmols, 1); WSA(items, n); WSA(xitems, n); WSA(n_xitems, 1); WSA(tile_ctr, 64); WSA(seeds, B);
   if (e->use_tc && e->cfg.graph_type != 0) { WSA(nbr, n * N); WSA(recs, n * CUT_REC); WSA(xrecs, n * CUT_REC); WSA(n_recs, 2); }
 #undef WSA
   ws.B = B; ws.N = N;
@@ -560,7 +561,8 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
   } else if (io.sampler) {
     fa.tag_step = e->step_ctr + 1;
   }
-  TIMED("k_finish", st, (launch_chain(k_finish, dim3((n + 15) / 16), dim3(256), 0, st, gm, fa)));
+  const bool per_mol = io.rng.on == NOISE_PER_MOLECULE;
+  TIMED("k_finish", st, (launch_chain(per_mol ? k_finish<true> : k_finish<false>, dim3((n + 15) / 16), dim3(256), 0, st, gm, fa)));
   LAUNCH_CHECK();
   e->launches += 1;
   if (e->cfg.centering || io.inpaint) {
@@ -573,7 +575,8 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     ia.coef = e->coef_dev;
     ia.step_prep = e->step_ctr; ia.step_fin = e->step_ctr + 1; ia.T = io.T;
     ia.norm0 = io.norm0; ia.norm1 = io.norm1; ia.bias1 = io.bias1; ia.chain = io.chain;
-    k_inpaint<<<B, 256, 0, st>>>(gm, ia);
+    if (per_mol) k_inpaint<true><<<B, 256, 0, st>>>(gm, ia);
+    else k_inpaint<false><<<B, 256, 0, st>>>(gm, ia);
     LAUNCH_CHECK();
     e->launches += 1;
   }
@@ -871,7 +874,7 @@ static NoiseRng make_rng(const dl_engine* e, int B, int N, uint64_t seed, uint64
   const int B_full = e->slice_B_full > 0 ? e->slice_B_full : B;   // geometry of the FULL batch's randn calls
   randn_geometry(e, (long long)B_full * N * 3, &q.Sx, &cx);
   randn_geometry(e, (long long)B_full * N * F, &q.Sh, &ch);
-  q.seed = seed; q.offset = offset; q.cx = cx; q.per_draw = cx + ch; q.F = F; q.on = 1;
+  q.seed = seed; q.offset = offset; q.cx = cx; q.per_draw = cx + ch; q.F = F; q.on = NOISE_BATCH;
   q.g0 = e->slice_B_full > 0 ? e->slice_b0 * N : 0;
   return q;
 }
@@ -907,6 +910,20 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
                            &q, coef, norm, chain, nan_flags, stream);
 }
 
+dl_status dl_sample_chain_seeded(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                                 const float* xh, const int8_t* node_mask, const float* fragment_mask,
+                                 const float* linker_mask, const int8_t* edge_mask, const float* context,
+                                 const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
+                                 int32_t* nan_flags, void* stream) {
+  // the seeds name the molecules, so the engine's batch slice does not apply; sample_chain_impl copies them into the
+  // workspace and points the stream at that copy
+  NoiseRng q{};
+  q.seeds = reinterpret_cast<const unsigned long long*>(seeds);
+  q.F = e ? e->cfg.in_node_nf : 0; q.N = N; q.on = NOISE_PER_MOLECULE;
+  return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, nullptr,
+                           &q, coef, norm, chain, nan_flags, stream);
+}
+
 dl_status dl_set_noise_slice(dl_engine* e, int32_t B_full, int32_t b0) {
   if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
   if (B_full < 0 || b0 < 0 || (B_full > 0 && b0 >= B_full)) { set_err("bad batch slice (%d of %d)", b0, B_full); return DL_ERR_INVALID; }
@@ -938,7 +955,7 @@ dl_status dl_noise_fill_inpaint(dl_engine* e, int32_t T, int32_t B, int32_t N, c
   CK(cudaSetDevice(e->cfg.device));
   const NoiseRng q = make_rng(e, B, N, seed, offset);
   if (offset_consumed) *offset_consumed = (uint64_t)(2 * T + 3) * q.per_draw;
-  k_com_free_draws<<<dim3(B, 2 * T + 3), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  k_com_free_draws<false><<<dim3(B, 2 * T + 3), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       N, 3 + e->cfg.in_node_nf, T, q, node_mask, fragment_mask, out);
   LAUNCH_CHECK();
   return DL_OK;
@@ -949,9 +966,10 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
                                    const float* linker_mask, const int8_t* edge_mask, const float* context,
                                    const float* noise, const NoiseRng* rng, const dl_step_coef* coef, const float* norm,
                                    float* chain, int32_t* nan_flags, void* stream) {
+  const bool per_mol = rng && rng->on == NOISE_PER_MOLECULE;
   dl_status s = check_shapes(e, B, N);
-  if (s == DL_OK) s = check_sampler(e, sampler, T, keep_frames, noise || rng, xh, node_mask, fragment_mask, linker_mask, context,
-                                    coef, norm, chain);
+  if (s == DL_OK) s = check_sampler(e, sampler, T, keep_frames, noise || (rng && (!per_mol || rng->seeds)), xh, node_mask,
+                                    fragment_mask, linker_mask, context, coef, norm, chain);
   if (s != DL_OK) return s;
   const bool inpaint = sampler == DL_SAMPLER_INPAINT;
   static_assert(sizeof(dl_step_coef) == 32, "dl_step_coef layout");
@@ -976,6 +994,12 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     CK(cudaStreamWaitEvent(st, e->ev_in, 0));
   }
   CK(cudaMemcpyAsync(e->coef_dev, coef, (size_t)(T + 1) * sizeof(dl_step_coef), cudaMemcpyHostToDevice, st));
+  NoiseRng q = rng ? *rng : NoiseRng{};
+  if (per_mol) {
+    // the captured step reads the engine's copy: the caller's seeds buffer is free once the call has been enqueued
+    CK(cudaMemcpyAsync(e->ws.seeds, rng->seeds, (size_t)B * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
+    q.seeds = e->ws.seeds;
+  }
   CK(cudaMemsetAsync(e->step_ctr, 0, 2 * sizeof(int), st));
   if (nan_flags) CK(cudaMemsetAsync(nan_flags, 0, B * sizeof(int32_t), st));
   const int n = B * N, xd = 3 + e->cfg.in_node_nf;
@@ -983,14 +1007,16 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   CK(cudaMemsetAsync(chain, 0, (size_t)keep_frames * n * xd * sizeof(float), st));
   if (inpaint && rng) {
     // z_T = COM-free masked noise on every atom (edm.py:565): draw 0 of the device-side stream
-    k_com_free_draws<<<dim3(B, 1), 256, 0, st>>>(N, xd, T, *rng, node_mask, fragment_mask, e->ws.z);
+    if (per_mol) k_com_free_draws<true><<<dim3(B, 1), 256, 0, st>>>(N, xd, T, q, node_mask, fragment_mask, e->ws.z);
+    else k_com_free_draws<false><<<dim3(B, 1), 256, 0, st>>>(N, xd, T, q, node_mask, fragment_mask, e->ws.z);
     LAUNCH_CHECK();
     e->launches += 1;
   } else if (inpaint) {
     // the caller's slab 0 is already masked and projected
     CK(cudaMemcpyAsync(e->ws.z, noise, (size_t)n * xd * sizeof(float), cudaMemcpyDeviceToDevice, st));
   } else {
-    k_init_z<<<(n * xd + 255) / 256, 256, 0, st>>>(n, xd, xh, fragment_mask, linker_mask, noise, rng ? *rng : NoiseRng{}, e->ws.z);
+    if (per_mol) k_init_z<true><<<(n * xd + 255) / 256, 256, 0, st>>>(n, xd, xh, fragment_mask, linker_mask, noise, q, e->ws.z);
+    else k_init_z<false><<<(n * xd + 255) / 256, 256, 0, st>>>(n, xd, xh, fragment_mask, linker_mask, noise, q, e->ws.z);
     LAUNCH_CHECK();
     e->launches += 1;
   }
@@ -1002,7 +1028,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   io.sampler = true; io.inpaint = inpaint; io.xh0 = xh; io.upd_linker_mask = linker_mask;
   io.node_mask = node_mask; io.linker_mask = inpaint ? nullptr : linker_mask; io.edge_mask = edge_mask;
   io.context = context; io.nan_flags = nan_flags; io.fragment_mask = fragment_mask; io.noise = noise;
-  if (rng) io.rng = *rng;
+  io.rng = q;
   io.chain = chain; io.T = T; io.norm0 = norm[0]; io.norm1 = norm[1]; io.bias1 = norm[2];
 
   // capture ONE reverse step; the step index lives on the device, so the same graph serves all T+1 steps

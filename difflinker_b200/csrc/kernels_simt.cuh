@@ -819,17 +819,34 @@ __global__ void k_copy_x(int n3, const float* __restrict__ src, float* __restric
 // normal_and_transform). Reproducing that mapping with the same cuRAND device functions gives the SAME numbers the
 // reference would draw on this GPU for the same seed and offset -- without the (T+2) x 2 randn launches, the
 // (T+2,B,N,3+F) slab and its interleaving copy.
+//
+// Per-molecule stream (kernels instantiated with PER_MOL = true): molecule b draws what the batch stream gives a batch of
+// that one molecule from generator state (seeds[b], 0). Such a batch has numel <= S for both calls (up to 256 * 8 * SMs
+// elements), so element e of a call is component .x of the curand_normal4 of subsequence e, the x call of draw r sits at
+// offset 8r and the h call at 8r + 4:
+//   element d of atom n of molecule b in draw r = curand_normal4(curand_init(seeds[b], e, 8r + (d >= 3 ? 4 : 0))).x,
+//   e = 3n + d (d < 3) or F n + (d - 3)
+// Nothing in it depends on B, on N, on the molecule's row or on the device, so a molecule samples the same whatever its
+// batch. The per-molecule kernels read the seeds through the union below and N from the field that otherwise pads the
+// struct: the batch-stream instantiations see the parameter layout they always saw.
 // ------------------------------------------------------------------------------------------------
+enum { NOISE_TENSOR = 0, NOISE_BATCH = 1, NOISE_PER_MOLECULE = 2 };
 struct NoiseRng {
-  unsigned long long seed, offset;   // torch CUDA generator state when EDM.sample_chain was entered
+  union {
+    unsigned long long seed;         // batch stream: torch CUDA generator state when EDM.sample_chain was entered
+    const unsigned long long* seeds; // per-molecule stream: B seeds in device memory (the engine's copy)
+  };
+  unsigned long long offset;
   unsigned long long per_draw;       // offset consumed by one draw (x call + h call)
   unsigned long long cx;             // ... by the x call alone
   int Sx, Sh;                        // 256 * grid of the x / h call
   int F;
-  int on;                            // 0: read the caller's noise tensor instead
+  int on;                            // NOISE_TENSOR: read the caller's noise tensor instead; else NOISE_BATCH / _PER_MOLECULE
   int g0;                            // first node row of this engine's slice inside the full batch (strong scaling: the slice
                                      // consumes exactly the rows of the full-batch draw, so results do not depend on the split)
+  int N;                             // per-molecule stream: atoms per molecule (node g is atom g % N of molecule g / N)
 };
+static_assert(sizeof(NoiseRng) == 56, "NoiseRng: the batch-stream kernels' parameter layout");
 __device__ __forceinline__ float philox_normal_elem(unsigned long long seed, unsigned long long offset, int S, long long e) {
   const long long per_round = 4LL * S;
   const long long rr = e / per_round;
@@ -841,7 +858,15 @@ __device__ __forceinline__ float philox_normal_elem(unsigned long long seed, uns
   return ii == 0 ? v.x : ii == 1 ? v.y : ii == 2 ? v.z : v.w;
 }
 // element d of node g (of n_total) of noise draw r
+template <bool PER_MOL = false>
 __device__ __forceinline__ float noise_draw(const NoiseRng& q, int r, int g, int d) {
+  if constexpr (PER_MOL) {
+    const int b = g / q.N, n = g - b * q.N;
+    const unsigned long long e = d < 3 ? 3ULL * n + d : (unsigned long long)q.F * n + (d - 3);
+    curandStatePhilox4_32_10_t st;
+    curand_init(q.seeds[b], e, 8ULL * (unsigned long long)r + (d < 3 ? 0ULL : 4ULL), &st);
+    return curand_normal4(&st).x;
+  }
   const unsigned long long base = q.offset + (unsigned long long)r * q.per_draw;
   const long long gg = (long long)g + q.g0;
   if (d < 3) return philox_normal_elem(q.seed, base, q.Sx, gg * 3 + d);
@@ -870,6 +895,7 @@ struct FinishArgs {
   const int* tag_step;   // non-sampler mode inside the inpainting loop: step counter used to tag NaN flags (or null)
 };
 
+template <bool PER_MOL = false>
 __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
   const int tid = threadIdx.x;
   const int d = tid & 15, r = tid >> 4;
@@ -939,7 +965,7 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
     lm = a.linker_mask[g]; fm = a.fragment_mask[g];
     const float zt = a.z[(size_t)g * xd + d];
     const float eps = e * lm;                                                 // edm.py:196 / 225
-    const float nz = (a.rng.on ? noise_draw(a.rng, step + 1, g, d)
+    const float nz = (a.rng.on ? noise_draw<PER_MOL>(a.rng, step + 1, g, d)
                                : a.noise[((size_t)(step + 1) * n_total + g) * xd + d]) * lm;  // utils.py:189-192
     if (step < a.T) {
       float mu = zt / ca - cb * eps;                                          // edm.py:199
@@ -1029,14 +1055,14 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool com_free_on_fragments(int r, int T) { return r >= 2 && r <= 2 * T && (r & 1) == 0; }
 
-template <typename M>
+template <bool PER_MOL, typename M>
 __device__ float3 com_free_means(const NoiseRng& q, int r, int b, int N, const M* __restrict__ mask, float* red) {
   // one (atom, coordinate) pair per thread and pass: ceil(3N / 256) Philox evaluations in a row, not 3 ceil(N / 256)
   float cnt = 0.f, sx = 0.f, sy = 0.f, sz = 0.f;
   for (int idx = threadIdx.x; idx < 3 * N; idx += 256) {
     const int n = idx / 3, d = idx - 3 * n, g = b * N + n;
     const float m = (float)mask[g];
-    const float v = __fmul_rn(noise_draw(q, r, g, d), m);
+    const float v = __fmul_rn(noise_draw<PER_MOL>(q, r, g, d), m);
     if (d == 0) { cnt += m; sx += v; } else if (d == 1) sy += v; else sz += v;
   }
   cnt = block_sum_256(cnt, red);
@@ -1045,12 +1071,14 @@ __device__ float3 com_free_means(const NoiseRng& q, int r, int b, int N, const M
 }
 
 // element d of node g of draw r, mask value m, means from com_free_means (rounded step by step as the torch ops are)
+template <bool PER_MOL>
 __device__ __forceinline__ float com_free_value(const NoiseRng& q, int r, int g, int d, float m, float3 mean) {
-  const float xm = __fmul_rn(noise_draw(q, r, g, d), m);
+  const float xm = __fmul_rn(noise_draw<PER_MOL>(q, r, g, d), m);
   if (d >= 3) return xm;
   return __fsub_rn(xm, __fmul_rn(d == 0 ? mean.x : d == 1 ? mean.y : mean.z, m));
 }
 
+template <bool PER_MOL = false>
 __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
   __shared__ float red[8];
   __shared__ float means[4];
@@ -1085,9 +1113,9 @@ __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
   const float* nB = a.rng.on ? nullptr : a.noise + (size_t)rB * slab;
   float3 meanA{}, meanB{};
   if (a.rng.on) {
-    meanA = com_free_means(a.rng, rA, b, N, a.nm, red);
-    meanB = com_free_on_fragments(rB, a.T) ? com_free_means(a.rng, rB, b, N, a.fragment_mask, red)
-                                           : com_free_means(a.rng, rB, b, N, a.nm, red);
+    meanA = com_free_means<PER_MOL>(a.rng, rA, b, N, a.nm, red);
+    meanB = com_free_on_fragments(rB, a.T) ? com_free_means<PER_MOL>(a.rng, rB, b, N, a.fragment_mask, red)
+                                           : com_free_means<PER_MOL>(a.rng, rB, b, N, a.nm, red);
   }
   if (step < a.T) {
     // pass 1: new latent before the centre-of-mass projection
@@ -1099,8 +1127,8 @@ __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
       float e = a.eps[gi];
       if (d < 3) e -= (d == 0 ? mvx : d == 1 ? mvy : mvz) * m;
       const float zt = a.z[gi];
-      const float na = a.rng.on ? com_free_value(a.rng, rA, (int)(g0 + n), d, m, meanA) : nA[gi];
-      const float nb = a.rng.on ? com_free_value(a.rng, rB, (int)(g0 + n), d, fm, meanB) : nB[gi];
+      const float na = a.rng.on ? com_free_value<PER_MOL>(a.rng, rA, (int)(g0 + n), d, m, meanA) : nA[gi];
+      const float nb = a.rng.on ? com_free_value<PER_MOL>(a.rng, rB, (int)(g0 + n), d, fm, meanB) : nB[gi];
       const float zl = (zt / ca - cb * e) + cc * na;                             // edm.py:634-642
       const float zf = (qa * zt + qb * (a.xh0[gi] * fm)) + cc * nb;               // edm.py:655-668
       const float zn = zl * lm + zf * fm;                                        // edm.py:589
@@ -1128,8 +1156,8 @@ __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
         float e = a.eps[gi];
         if (d < 3) e -= (d == 0 ? mvx : d == 1 ? mvy : mvz) * m;
         const float zt = a.z[gi];
-        const float na = a.rng.on ? com_free_value(a.rng, rA, (int)(g0 + n), d, m, meanA) : nA[gi];
-        const float nb = a.rng.on ? com_free_value(a.rng, rB, (int)(g0 + n), d, m, meanB) : nB[gi];
+        const float na = a.rng.on ? com_free_value<PER_MOL>(a.rng, rA, (int)(g0 + n), d, m, meanA) : nA[gi];
+        const float nb = a.rng.on ? com_free_value<PER_MOL>(a.rng, rB, (int)(g0 + n), d, m, meanB) : nB[gi];
         const float xl = ca * (zt - cb * e) + cc * na;                           // edm.py:701-702 (ca = 1/alpha_0, cb = sigma_0)
         const float xf = ca * zt - qa * nb;                                      // edm.py:716 (qa = sigma_0/alpha_0)
         if (d < 3) {
@@ -1148,13 +1176,14 @@ __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
 }
 
 // z0 = xh*fragment_mask + (noise[0]*linker_mask)*linker_mask   (edm.py:136-137)
+template <bool PER_MOL = false>
 __global__ void k_init_z(int n_total, int xd, const float* __restrict__ xh, const float* __restrict__ fm,
                          const float* __restrict__ lm, const float* __restrict__ noise, NoiseRng rng, float* __restrict__ z) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n_total * xd) return;
   int g = idx / xd;
   float l = lm[g];
-  const float nz = rng.on ? noise_draw(rng, 0, g, idx - g * xd) : noise[idx];
+  const float nz = rng.on ? noise_draw<PER_MOL>(rng, 0, g, idx - g * xd) : noise[idx];
   z[idx] = xh[idx] * fm[g] + (nz * l) * l;
 }
 
@@ -1171,16 +1200,18 @@ __global__ void k_noise_fill(int n_draws, int n_total, int xd, NoiseRng rng, flo
 // Draws [0, gridDim.y) of the inpainting sampler's stream, masked and COM-projected, one CTA per (molecule, draw):
 // out is (gridDim.y, B = gridDim.x, N, xd). All 2T+3 for dl_noise_fill_inpaint; draw 0 -- the initial z (edm.py:565) --
 // straight into the workspace when the sampler draws on the device.
+template <bool PER_MOL = false>
 __global__ void __launch_bounds__(256) k_com_free_draws(int N, int xd, int T, NoiseRng rng, const int8_t* __restrict__ node_mask,
                                                         const float* __restrict__ fragment_mask, float* __restrict__ out) {
   __shared__ float red[8];
   const int b = blockIdx.x, r = blockIdx.y;
   const bool frag = com_free_on_fragments(r, T);
-  const float3 mean = frag ? com_free_means(rng, r, b, N, fragment_mask, red) : com_free_means(rng, r, b, N, node_mask, red);
+  const float3 mean = frag ? com_free_means<PER_MOL>(rng, r, b, N, fragment_mask, red)
+                           : com_free_means<PER_MOL>(rng, r, b, N, node_mask, red);
   float* o = out + ((size_t)blockIdx.y * gridDim.x + b) * N * xd;
   for (int idx = threadIdx.x; idx < N * xd; idx += 256) {
     const int n = idx / xd, d = idx - n * xd, g = b * N + n;
-    o[idx] = com_free_value(rng, r, g, d, frag ? fragment_mask[g] : (float)node_mask[g], mean);
+    o[idx] = com_free_value<PER_MOL>(rng, r, g, d, frag ? fragment_mask[g] : (float)node_mask[g], mean);
   }
 }
 

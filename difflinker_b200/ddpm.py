@@ -79,11 +79,12 @@ def sampler_inputs(model, data, sample_fn=None):
                 linker_mask=linker_mask, context=context)
 
 
-def sample_chain(model, data, sample_fn=None, keep_frames=None):
+def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
-    modules (`model` additionally needs .edm)."""
+    modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
+    `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size."""
     kw = sampler_inputs(model, data, sample_fn)
-    chain = model.edm.sample_chain(**kw, keep_frames=keep_frames)
+    chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **({} if seeds is None else {'seeds': seeds}))
     return chain, kw['node_mask']
 
 
@@ -122,8 +123,8 @@ class DDPM(nn.Module):
         self.edm = _build_edm(self.hparams, edge_impl=edge_impl)
         self.edm.devices = devices          # EDM.devices: split each sampling batch over these CUDA devices
 
-    def sample_chain(self, data, sample_fn=None, keep_frames=None):
-        return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames)
+    def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None):
+        return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

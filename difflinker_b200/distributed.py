@@ -109,21 +109,27 @@ def slice_sampler_inputs(kw: dict, lo: int, hi: int):
     return out
 
 
-def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=True):
+def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=True, seeds=None):
     """Strong scaling of ONE batch (SURVEY.md section 8(e)): the template batch is built once (so every rank pads to the same
     N), each rank runs the reverse loop for its contiguous slice of the molecules with the slice's rows of the full-batch
     noise, and the chains are gathered -- the result equals `model.sample_chain(data)` on one GPU bit for bit, for any
     world size, on the SIMT path and on the tensor-core path while no sample diverges far enough for the node GEMM to
     rescale a tile's fp16 operands (DESIGN.md section 6). No collective inside the loop. Returns (chain, node_mask) with
-    the full batch on every rank when `gather`, else the local slice."""
+    the full batch on every rank when `gather`, else the local slice.
+    `seeds`: the full batch's B per-molecule seeds (EDM.sample_chain); each rank samples its rows with its rows of them,
+    so the result equals `model.sample_chain(data, seeds=seeds)` on one GPU in the same sense."""
     from .ddpm import sampler_inputs
+    from .edm import seeds_tensor
     kw = sampler_inputs(model, data, sample_fn)
     B = kw['x'].shape[0]
     world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
     rank = dist.get_rank() if world > 1 else 0
     lo, hi = shard_range(B, rank, world)
     local = slice_sampler_inputs(kw, lo, hi)
-    chain = model.edm.sample_chain(**local, keep_frames=keep_frames, batch_slice=(lo, B) if world > 1 else None)
+    if seeds is not None:
+        chain = model.edm.sample_chain(**local, keep_frames=keep_frames, seeds=seeds_tensor(seeds, B)[lo:hi])
+    else:
+        chain = model.edm.sample_chain(**local, keep_frames=keep_frames, batch_slice=(lo, B) if world > 1 else None)
     if world == 1:
         return chain, kw['node_mask']
     if not gather:

@@ -7,6 +7,7 @@ are made with the reference's `torch.randn` call order and shapes (edm.py:328-34
 torch seed produces the same noise stream as the reference would on that device.
 """
 import ctypes as C
+import operator
 import threading
 
 import torch
@@ -44,6 +45,36 @@ def _sample_chain_rng(lib, eng, dev, batch_slice, head, tail):
     seed, offset = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF, gen.get_offset()
     used = _run_chain_rng(lib, eng, batch_slice, seed, offset, head, tail)
     gen.set_offset(offset + used)
+
+
+def seeds_tensor(seeds, n_samples):
+    """Per-molecule seeds -- an integer tensor or a sequence of ints, one per molecule -- as a CPU int64 tensor. Each seed is
+    reduced modulo 2^64 as torch.cuda.manual_seed reduces it (values in [-2^63, 2^64); -1 and 2^64 - 1 name the same
+    stream) and kept as the int64 with the same 64 bits, which torch.cuda.manual_seed accepts back unchanged."""
+    if torch.is_tensor(seeds):
+        if seeds.dim() != 1 or seeds.dtype.is_floating_point or seeds.dtype.is_complex or seeds.dtype == torch.bool:
+            raise ValueError(f"seeds must be a 1-D integer tensor (got {seeds.dtype} of shape {tuple(seeds.shape)})")
+        seeds = seeds.tolist()
+    out = []
+    for s in seeds:
+        if isinstance(s, bool):
+            raise ValueError(f"seeds are integers (got {s!r})")
+        try:
+            s = operator.index(s)
+        except TypeError:
+            raise ValueError(f"seeds are integers (got {s!r})") from None
+        if not -(1 << 63) <= s < (1 << 64):
+            raise ValueError(f"seed {s} is outside [-2^63, 2^64), the range torch.cuda.manual_seed accepts")
+        out.append(s - (1 << 64) if s >= (1 << 63) else s)
+    if len(out) != n_samples:
+        raise ValueError(f"seeds holds {len(out)} values for a batch of {n_samples} molecules")
+    return torch.tensor(out, dtype=torch.int64)
+
+
+def draw_seeds(n_samples, device):
+    """The seeds noise_mode='per_molecule' derives when none are given: one call on `device`'s default CUDA generator,
+    torch.randint(2**63 - 1, (n_samples,), dtype=torch.int64, device=device), so torch.manual_seed governs them."""
+    return torch.randint(2 ** 63 - 1, (n_samples,), dtype=torch.int64, device=device)
 
 
 def _run_per_device(calls_by_device):
@@ -102,7 +133,10 @@ class EDM(torch.nn.Module):
         #   generator's (seed, offset) -- same values as the randn calls, no tensor, no launches (dl_sample_chain_rng).
         # 'reference_tensor': the same stream materialised with torch.randn (two launches per draw).
         # 'bulk': one randn call for the whole chain (a different stream).
+        # 'per_molecule': every molecule draws from a stream of its own (see sample_chain's `seeds`); without `seeds` the B
+        #   seeds come from one draw_seeds call on the inputs' device, so torch.manual_seed still governs the run.
         self.noise_mode = 'reference_stream'
+        self.last_seeds = None                 # per-molecule stream: the (B,) CPU int64 seeds of the last call, else None
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
@@ -259,6 +293,33 @@ class EDM(torch.nn.Module):
             assert noise.shape == (self._n_draws(), n_samples, n_nodes, self.n_dims + self.in_node_nf), noise.shape
         return on_device, noise
 
+    def _per_molecule_seeds(self, seeds, noise, batch_slice, x):
+        """The (B,) int64 seeds on x's device when this call samples the per-molecule stream -- `seeds` are given, or
+        noise_mode is 'per_molecule' and no noise tensor is -- else None. Records them in `last_seeds` (None otherwise)."""
+        self.last_seeds = None
+        if seeds is None and (self.noise_mode != 'per_molecule' or noise is not None):
+            return None
+        what = "seeds" if seeds is not None else "noise_mode='per_molecule'"
+        if noise is not None:
+            raise ValueError("seeds and noise= both supply the draws: pass one of them")
+        if self._draws_replaced():
+            raise ValueError(f"{what} selects the device-side per-molecule stream, but this model's draw function is "
+                             "replaced; restore it or inject the noise")
+        if batch_slice is not None:
+            raise ValueError(f"{what} does not take batch_slice: the seeds already name the molecules, so pass each slice "
+                             "its rows of the seeds")
+        cpu = None if seeds is None else seeds_tensor(seeds, x.size(0))
+        if x.device.type != 'cuda':
+            raise ValueError(f"{what} needs CUDA inputs (got {x.device})")
+        if cpu is None:
+            with torch.cuda.device(x.device):
+                dev_seeds = draw_seeds(x.size(0), x.device)
+            cpu = dev_seeds.cpu()
+        else:
+            dev_seeds = cpu.to(x.device)
+        self.last_seeds = cpu
+        return dev_seeds
+
     def _head(self, n_samples, n_nodes, keep_frames, t):
         ptr = lambda v: None if v is None else v.data_ptr()
         return (self._SAMPLER, n_samples, n_nodes, self.T, keep_frames, ptr(t['x']), ptr(t['node_mask']),
@@ -269,24 +330,34 @@ class EDM(torch.nn.Module):
 
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None):
+                     noise=None, batch_slice=None, seeds=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `batch_slice=(b0, B_full)`: the inputs are rows [b0, b0+B) of a batch of B_full molecules (strong scaling,
         distributed.sample_chain_sharded); the device-side noise is then those rows of the full batch's draws.
+        `seeds` (B ints, or an integer tensor; CUDA inputs): molecule b draws exactly what the reference draws for it
+        sampled alone after torch.cuda.manual_seed(seeds[b]) (dl_sample_chain_seeded), whatever noise_mode is. Its chain
+        then depends neither on its batch-mates, the batch size, its row, the padding nor a split over devices -- on the
+        tensor-core path while no sample diverges far enough for the node GEMM to rescale a tile's fp16 operands (tiles
+        span molecules, DESIGN.md section 6), and with aggregation_method='mean' on FC graphs except for the padding,
+        which the reference's mean counts. The generator does not advance. noise_mode='per_molecule' samples that stream
+        without `seeds` from draw_seeds. Either way `last_seeds` records the seeds; replaying one molecule with its seed
+        reproduces its row, including a NaN divergence, so retry a diverged molecule with a new seed.
         With `devices` set (and no batch_slice) the batch is split over those devices (_sample_chain_split)."""
         if keep_frames is None:
             keep_frames = self.T
         else:
             assert keep_frames <= self.T
         if self.devices is not None and batch_slice is None:
-            return self._sample_chain_split(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames, noise)
+            return self._sample_chain_split(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames, noise,
+                                            seeds)
         lib = _native.load_library()
         n_samples, n_nodes = x.size(0), x.size(1)
         dev = x.device
         d = self.n_dims + self.in_node_nf
+        dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
         t = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
-        on_device, noise = self._noise(noise, x, node_mask, fragment_mask)
+        on_device, noise = (False, None) if dev_seeds is not None else self._noise(noise, x, node_mask, fragment_mask)
         if batch_slice is not None and not on_device:
             raise ValueError("batch_slice needs the device-side noise stream (CUDA tensors, noise_mode='reference_stream')")
 
@@ -301,7 +372,10 @@ class EDM(torch.nn.Module):
         if dev.type == 'cuda':
             with torch.cuda.device(dev):
                 stream = torch.cuda.current_stream(dev).cuda_stream
-                if on_device:
+                if dev_seeds is not None:
+                    _native.check(lib.dl_sample_chain_seeded(eng, *head, dev_seeds.data_ptr(), *tail, stream),
+                                  "dl_sample_chain_seeded")
+                elif on_device:
                     _sample_chain_rng(lib, eng, dev, batch_slice, head, tail + (stream,))
                 else:
                     _native.check(lib.dl_sample_chain(eng, *head, ptr(noise), *tail, stream), "dl_sample_chain")
@@ -316,19 +390,22 @@ class EDM(torch.nn.Module):
             raise nan_exception_class()(flags=flags.cpu().tolist())
         return chain
 
-    def _sample_chain_split(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames, noise):
+    def _sample_chain_split(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames, noise,
+                            seeds=None):
         """sample_chain over `devices`: the inputs are prepared and the noise is chosen once, on x's device, as for one device;
         slot i of `devices` samples molecules shard_range(B, i, len(devices)) on its own engine, with the full batch's step
-        coefficients and either batch_slice=(lo, B) from the caller's generator state or its rows of the noise tensor. Each
-        device's loops are enqueued from a thread of its own; the chains and NaN flags are then copied back into rows
-        [lo, hi) on x's device, and the caller's generator advances once, by what one device would have consumed."""
+        coefficients and either batch_slice=(lo, B) from the caller's generator state, its rows of the per-molecule seeds or
+        its rows of the noise tensor. Each device's loops are enqueued from a thread of its own; the chains and NaN flags are
+        then copied back into rows [lo, hi) on x's device, and the caller's generator advances once, by what one device
+        would have consumed."""
         lib = _native.load_library()
         n_samples, n_nodes = x.size(0), x.size(1)
         dev = x.device
         d = self.n_dims + self.in_node_nf
         self.dynamics._check_graph_type()
+        dev_seeds = self._per_molecule_seeds(seeds, noise, None, x)
         full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
-        on_device, noise = self._noise(noise, x, node_mask, fragment_mask)
+        on_device, noise = (False, None) if dev_seeds is not None else self._noise(noise, x, node_mask, fragment_mask)
         slices = device_slices(n_samples, self.devices)
         if not slices:
             raise ValueError("sample_chain needs at least one molecule")
@@ -352,20 +429,24 @@ class EDM(torch.nn.Module):
             cuda_i = torch.device('cuda', dev_i)
             with torch.cuda.device(cuda_i):
                 t = {k: None if v is None else v.to(cuda_i).contiguous() for k, v in slice_sampler_inputs(full, lo, hi).items()}
-                nz = None if on_device else noise[:, lo:hi].to(cuda_i).contiguous()
+                nz = None if noise is None else noise[:, lo:hi].to(cuda_i).contiguous()
+                sd = None if dev_seeds is None else dev_seeds[lo:hi].to(cuda_i).contiguous()
                 chain_i = torch.empty((keep_frames, hi - lo, n_nodes, d), device=cuda_i, dtype=torch.float32)
                 flags_i = torch.zeros(hi - lo, dtype=torch.int32, device=cuda_i)
                 stream = torch.cuda.current_stream(cuda_i).cuda_stream
             head = self._head(hi - lo, n_nodes, keep_frames, t)
             tail = (coef, norm, ptr(chain_i), ptr(flags_i))
-            if on_device:
+            if sd is not None:
+                call = (lambda eng=eng, head=head, sd=sd, tail=tail, stream=stream:
+                        _native.check(lib.dl_sample_chain_seeded(eng, *head, ptr(sd), *tail, stream), "dl_sample_chain_seeded"))
+            elif on_device:
                 call = (lambda eng=eng, lo=lo, head=head, tail=tail, stream=stream:
                         consumed.append(_run_chain_rng(lib, eng, (lo, n_samples), seed, offset, head, tail + (stream,))))
             else:
                 call = (lambda eng=eng, head=head, nz=nz, tail=tail, stream=stream:
                         _native.check(lib.dl_sample_chain(eng, *head, ptr(nz), *tail, stream), "dl_sample_chain"))
             calls.setdefault(dev_i, []).append(call)
-            inputs.append((t, nz))          # alive until the loops are done (the host waits on the flags below)
+            inputs.append((t, nz, sd))      # alive until the loops are done (the host waits on the flags below)
             chains.append(chain_i)
             flags.append(flags_i)
         try:
@@ -441,15 +522,17 @@ class InpaintingEDM(EDM):
         return 'draw_noise_inpaint' in self.__dict__ or type(self).draw_noise_inpaint is not _DRAW_NOISE_INPAINT
 
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None):
+                     noise=None, batch_slice=None, seeds=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
         (dl_sample_chain_rng), unless `draw_noise_inpaint` is replaced -- on the instance, in a subclass or on the class --
-        in which case the replacement draws them. `batch_slice=(b0, B_full)` as in EDM.sample_chain."""
+        in which case the replacement draws them. `batch_slice=(b0, B_full)` and `seeds` as in EDM.sample_chain: with
+        seeds, molecule b's 2T+3 raw draws are those of the molecule sampled alone after torch.cuda.manual_seed(seeds[b]),
+        masked and projected per molecule as always."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
-                                    batch_slice=batch_slice)
+                                    batch_slice=batch_slice, seeds=seeds)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

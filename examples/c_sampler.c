@@ -9,7 +9,10 @@
  * DLJOB2: followed by the model's dl_egnn_options -- tanh, mean aggregation), the weights under the reference's state_dict names, the normalised inputs and masks of one batch, the per-step
  * coefficient table of the noise schedule and a Philox (seed, offset) pair; the noise of the T+2 draws (2T+3 for
  * inpainting) is generated inside the kernels (dl_sample_chain_rng) in the order the reference's torch.randn calls would
- * have produced it on this GPU. out.bin: int32 status, uint64 philox offset consumed, the (keep_frames, B, N, 3+F) chain,
+ * have produced it on this GPU. A seeded job (magic DLJOB3: an int32 flag and, if set, the dl_egnn_options follow the
+ * dl_config) holds one uint64 seed per molecule instead of the pair and samples with dl_sample_chain_seeded: each molecule
+ * then draws what it would draw sampled alone, so any molecule can be replayed from its seed.
+ * out.bin: int32 status, uint64 philox offset consumed (0 for a seeded job), the (keep_frames, B, N, 3+F) chain,
  * B NaN flags.
  *
  * Build: gcc -std=c99 -O2 examples/c_sampler.c -Iinclude -I/usr/local/cuda/include -Ldifflinker_b200 -ldifflinker_b200 \
@@ -51,11 +54,13 @@ int main(int argc, char** argv) {
   if (!f) { perror(argv[1]); return 2; }
   char magic[8];
   rd(f, magic, 8);
-  const int with_opts = memcmp(magic, "DLJOB2\0\0", 8) == 0;
-  if (!with_opts && memcmp(magic, "DLJOB1\0\0", 8) != 0) { fprintf(stderr, "c_sampler: not a job file\n"); return 2; }
+  const int seeded = memcmp(magic, "DLJOB3\0\0", 8) == 0;
+  int32_t with_opts = memcmp(magic, "DLJOB2\0\0", 8) == 0;
+  if (!seeded && !with_opts && memcmp(magic, "DLJOB1\0\0", 8) != 0) { fprintf(stderr, "c_sampler: not a job file\n"); return 2; }
 
   dl_config cfg;
   rd(f, &cfg, sizeof cfg);                       /* 11 int32 + 2 float, no padding (checked by the exporter) */
+  if (seeded) rd(f, &with_opts, 4);
   dl_egnn_options opts;
   if (with_opts) rd(f, &opts, sizeof opts);      /* 3 int32 + 1 float */
   dl_engine* e = NULL;
@@ -77,13 +82,14 @@ int main(int argc, char** argv) {
   if (dl_finalize_weights(e) < 0) die("dl_finalize_weights");
 
   int32_t dims[6];                               /* B, N, T, keep_frames, xd = 3 + F, C */
-  uint64_t rng[2];                               /* philox seed, offset */
+  uint64_t rng[2] = {0, 0};                      /* philox seed, offset */
   float norm[3];
   rd(f, dims, sizeof dims);
-  rd(f, rng, sizeof rng);
-  rd(f, norm, sizeof norm);
   const int32_t B = dims[0], N = dims[1], T = dims[2], keep = dims[3], xd = dims[4], C = dims[5];
   const size_t n = (size_t)B * N;
+  uint64_t* seeds = seeded ? (uint64_t*)rd_alloc(f, (size_t)B * 8) : NULL;   /* seeded job: one seed per molecule */
+  if (!seeded) rd(f, rng, sizeof rng);
+  rd(f, norm, sizeof norm);
   dl_step_coef* coef = (dl_step_coef*)rd_alloc(f, (size_t)(T + 1) * sizeof(dl_step_coef));   /* host table, as the ABI asks */
   float* xh = (float*)rd_alloc(f, n * xd * 4);
   int8_t* node_mask = (int8_t*)rd_alloc(f, n);
@@ -103,6 +109,7 @@ int main(int argc, char** argv) {
   float* d_lm = (float*)to_device(linker_mask, n * 4);
   int8_t* d_em = has_em ? (int8_t*)to_device(edge_mask, n * N) : NULL;
   float* d_ctx = has_ctx ? (float*)to_device(context, n * C * 4) : NULL;
+  uint64_t* d_seeds = seeded ? (uint64_t*)to_device(seeds, (size_t)B * 8) : NULL;
   float* d_chain = NULL;
   int32_t* d_flags = NULL;
   const size_t chain_bytes = (size_t)keep * n * xd * 4;
@@ -116,9 +123,12 @@ int main(int argc, char** argv) {
   uint64_t consumed = 0;
   /* inpainting models are the ones built with centering (lightning.py:99); the engine refuses any other pairing */
   const int32_t sampler = cfg.centering ? DL_SAMPLER_INPAINT : DL_SAMPLER_LINKER;
-  const dl_status st = dl_sample_chain_rng(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, rng[0], rng[1],
-                                           &consumed, coef, norm, d_chain, d_flags, stream);
-  if (st < 0) die("dl_sample_chain_rng");
+  const dl_status st = seeded
+      ? dl_sample_chain_seeded(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, d_seeds, coef, norm, d_chain,
+                               d_flags, stream)
+      : dl_sample_chain_rng(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, rng[0], rng[1], &consumed, coef,
+                            norm, d_chain, d_flags, stream);
+  if (st < 0) die(seeded ? "dl_sample_chain_seeded" : "dl_sample_chain_rng");
   if (cudaStreamSynchronize(stream) != cudaSuccess) { fprintf(stderr, "c_sampler: the sampler's stream failed\n"); return 2; }
 
   float* chain = (float*)malloc(chain_bytes);

@@ -17,6 +17,7 @@
  *     sample_p_zs_given_zt_only_linker  edm.py:178-208
  *     sample_p_xh_given_z0_only_linker  edm.py:210-235
  *   InpaintingEDM.sample_chain   src/edm.py:549-612      dl_sample_chain (+ _rng) with DL_SAMPLER_INPAINT
+ *   either, one seed per molecule (no reference API)     dl_sample_chain_seeded
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   build_xae_molecule           src/molecule_builder.py:44-102       dl_bond_orders
  *   frame restore + .xyz text    generate.py:163-171, src/visualizer.py:14-31   dl_restore_frame, dl_format_xyz
@@ -187,6 +188,29 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
                               const float* linker_mask, const int8_t* edge_mask, const float* context, uint64_t seed,
                               uint64_t offset, uint64_t* offset_consumed, const dl_step_coef* coef, const float* norm,
                               float* chain, int32_t* nan_flags, void* stream);
+/*
+ * Same loop with a noise stream of each molecule's own: molecule b draws exactly what dl_sample_chain_rng gives a batch
+ * holding only that molecule from generator state (seeds[b], 0) -- what the reference draws for it sampled alone after
+ * torch.cuda.manual_seed(seeds[b]). So a molecule's chain depends neither on its batch-mates, nor on the batch size, its
+ * row or the padding, and one molecule of a large run can be replayed on its own from its seed. Explicitly, element d of
+ * atom n of molecule b in raw draw r (r < T+2 for DL_SAMPLER_LINKER, r < 2T+3 for DL_SAMPLER_INPAINT, in the call order of
+ * dl_sample_chain_rng) is
+ *     curandStatePhilox4_32_10_t st;
+ *     curand_init(seeds[b], e, 8 * r + (d < 3 ? 0 : 4), &st);   value = curand_normal4(&st).x
+ * with e = 3 n + d for the coordinates (d < 3) and e = F n + (d - 3) for the features. The inpainting sampler masks and
+ * projects each draw per molecule as dl_sample_chain_rng does. This equals torch's own randn while N max(3, F) <= 2048 x the
+ * device's SM count (about 17 k atoms on an H100); beyond that the formula above is the definition.
+ *   seeds   (B) uint64 DEVICE, read while the call is enqueued (the loop reads the engine's copy); NULL is DL_ERR_INVALID.
+ *           A torch seed s is reduced modulo 2^64, as torch.cuda.manual_seed does.
+ * dl_set_noise_slice does not apply: the seeds already name the molecules, so a slice passes its rows of the seeds. Nothing
+ * is consumed from any generator. Results also match across batches on the tensor-core path only while no sample diverges
+ * far enough for the node GEMM to rescale a tile's fp16 operands (tiles span molecules; DESIGN.md section 6).
+ */
+dl_status dl_sample_chain_seeded(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                                 const float* xh, const int8_t* node_mask, const float* fragment_mask,
+                                 const float* linker_mask, const int8_t* edge_mask, const float* context,
+                                 const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
+                                 int32_t* nan_flags, void* stream);
 /* Strong scaling (SURVEY 8(e)): this engine samples molecules [b0, b0 + B) of a batch of B_full. The device-side noise of
  * the following dl_sample_chain_rng / dl_noise_fill / dl_noise_fill_inpaint calls is then the slice's ROWS of the
  * full-batch draws (and offset_consumed is the full batch's), so the gathered result is bit-identical to the single-GPU
