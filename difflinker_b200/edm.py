@@ -7,6 +7,7 @@ are made with the reference's `torch.randn` call order and shapes (edm.py:328-34
 torch seed produces the same noise stream as the reference would on that device.
 """
 import ctypes as C
+import functools
 import operator
 import threading
 
@@ -23,28 +24,26 @@ def _generator_of(dev):
     return torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
 
 
-def _run_chain_rng(lib, eng, batch_slice, seed, offset, head, tail):
-    """dl_sample_chain_rng(eng, *head, seed, offset, &consumed, *tail) with the engine's batch slice set for the duration of
-    the call; returns what the draws consumed."""
+def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None):
+    """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
+    per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
+    B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
+    samples host inputs (dl_sample_chain_host). Returns (status, what the batch stream consumed)."""
+    if stream is None:
+        return _native.check(lib.dl_sample_chain_host(eng, *head, noise.data_ptr(), *tail), "dl_sample_chain_host"), 0
+    if seeds is not None:
+        return _native.check(lib.dl_sample_chain_seeded(eng, *head, seeds.data_ptr(), *tail, stream),
+                             "dl_sample_chain_seeded"), 0
+    if rng is None:
+        return _native.check(lib.dl_sample_chain(eng, *head, noise.data_ptr(), *tail, stream), "dl_sample_chain"), 0
+    seed, offset, b0, b_full = rng
     used = C.c_uint64(0)
-    if batch_slice is not None:
-        _native.check(lib.dl_set_noise_slice(eng, int(batch_slice[1]), int(batch_slice[0])), "dl_set_noise_slice")
+    _native.check(lib.dl_set_noise_slice(eng, b_full, b0), "dl_set_noise_slice")
     try:
-        st = lib.dl_sample_chain_rng(eng, *head, seed, offset, C.byref(used), *tail)
+        st = lib.dl_sample_chain_rng(eng, *head, seed, offset, C.byref(used), *tail, stream)
     finally:
-        if batch_slice is not None:
-            lib.dl_set_noise_slice(eng, 0, 0)
-    _native.check(st, "dl_sample_chain_rng")
-    return used.value
-
-
-def _sample_chain_rng(lib, eng, dev, batch_slice, head, tail):
-    """_run_chain_rng from the state of `dev`'s default CUDA generator; then advances the generator as if the reference's
-    randn calls had run."""
-    gen = _generator_of(dev)
-    seed, offset = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF, gen.get_offset()
-    used = _run_chain_rng(lib, eng, batch_slice, seed, offset, head, tail)
-    gen.set_offset(offset + used)
+        lib.dl_set_noise_slice(eng, 0, 0)
+    return _native.check(st, "dl_sample_chain_rng"), used.value
 
 
 def seeds_tensor(seeds, n_samples):
@@ -143,14 +142,15 @@ class EDM(torch.nn.Module):
 
     @property
     def devices(self):
-        """None (the default): sample on the inputs' device. A list of CUDA device indices, or 'all' when set: sample_chain
-        splits each batch into contiguous, balanced slices, one per listed device, samples them concurrently and returns the
-        whole chain on the inputs' device. That chain is the one a single device samples, bit for bit on the fp32 SIMT edge
-        path, and on the tensor-core path while no sample diverges: the node GEMM rescales the fp16 operands of a tile by a
-        power of two chosen from the tile's maximum once values approach the fp16 range, and since tiles span molecules and
-        follow the batch, such molecules round differently after a split (DESIGN.md section 6). A device may be listed more
-        than once: each listing gets an engine of its own, and engines sharing a device run their loops one after the other.
-        Calls without `devices` keep one engine, so switching between split and single-device calls re-creates engines."""
+        """None (the default): sample_chain samples each batch as one slice on the inputs' device. A list of CUDA device
+        indices, or 'all' when set: it makes one contiguous, balanced slice per listed device instead, samples them
+        concurrently and returns the whole chain on the inputs' device. That chain is the one a single device samples, bit
+        for bit on the fp32 SIMT edge path, and on the tensor-core path while no sample diverges: the node GEMM rescales the
+        fp16 operands of a tile by a power of two chosen from the tile's maximum once values approach the fp16 range, and
+        since tiles span molecules and follow the batch, such molecules round differently after a split (DESIGN.md section
+        6). A device may be listed more than once: each listing gets an engine of its own, and engines sharing a device run
+        their loops one after the other. Calls without `devices` keep one engine, so switching between split and
+        single-device calls re-creates engines."""
         return self._devices
 
     @devices.setter
@@ -343,114 +343,72 @@ class EDM(torch.nn.Module):
         which the reference's mean counts. The generator does not advance. noise_mode='per_molecule' samples that stream
         without `seeds` from draw_seeds. Either way `last_seeds` records the seeds; replaying one molecule with its seed
         reproduces its row, including a NaN divergence, so retry a diverged molecule with a new seed.
-        With `devices` set (and no batch_slice) the batch is split over those devices (_sample_chain_split)."""
+        The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
+        and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
+        device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
+        thread per device, and their chains and NaN flags are copied back. The batch stream advances the generator once."""
         if keep_frames is None:
             keep_frames = self.T
         else:
             assert keep_frames <= self.T
-        if self.devices is not None and batch_slice is None:
-            return self._sample_chain_split(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames, noise,
-                                            seeds)
         lib = _native.load_library()
         n_samples, n_nodes = x.size(0), x.size(1)
         dev = x.device
         d = self.n_dims + self.in_node_nf
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
-        t = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
+        full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
         on_device, noise = (False, None) if dev_seeds is not None else self._noise(noise, x, node_mask, fragment_mask)
         if batch_slice is not None and not on_device:
             raise ValueError("batch_slice needs the device-side noise stream (CUDA tensors, noise_mode='reference_stream')")
-
-        eng = self.dynamics.engine(self.dynamics._device_index(x))
         self.dynamics._check_graph_type()
-        coef = self.step_coefficients(keep_frames, n_samples)
-        chain = torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32)
-        flags = torch.zeros(n_samples, dtype=torch.int32, device=dev)
-        ptr = lambda v: None if v is None else v.data_ptr()
-        head = self._head(n_samples, n_nodes, keep_frames, t)
-        tail = (coef, self._norm(), ptr(chain), ptr(flags))
-        if dev.type == 'cuda':
-            with torch.cuda.device(dev):
-                stream = torch.cuda.current_stream(dev).cuda_stream
-                if dev_seeds is not None:
-                    _native.check(lib.dl_sample_chain_seeded(eng, *head, dev_seeds.data_ptr(), *tail, stream),
-                                  "dl_sample_chain_seeded")
-                elif on_device:
-                    _sample_chain_rng(lib, eng, dev, batch_slice, head, tail + (stream,))
-                else:
-                    _native.check(lib.dl_sample_chain(eng, *head, ptr(noise), *tail, stream), "dl_sample_chain")
-                bad = bool(flags.any().item())   # one sync per chain instead of one per step (egnn.py:441)
-        else:
-            st = lib.dl_sample_chain_host(eng, *head, ptr(noise), *tail)
-            _native.check(st, "dl_sample_chain_host")
-            bad = st == _native.DL_NAN_DETECTED
-        self.last_loop_ms = float(lib.dl_last_elapsed_ms(eng))
-        self.last_slice_loop_ms = None
-        if bad:
-            raise nan_exception_class()(flags=flags.cpu().tolist())
-        return chain
-
-    def _sample_chain_split(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames, noise,
-                            seeds=None):
-        """sample_chain over `devices`: the inputs are prepared and the noise is chosen once, on x's device, as for one device;
-        slot i of `devices` samples molecules shard_range(B, i, len(devices)) on its own engine, with the full batch's step
-        coefficients and either batch_slice=(lo, B) from the caller's generator state, its rows of the per-molecule seeds or
-        its rows of the noise tensor. Each device's loops are enqueued from a thread of its own; the chains and NaN flags are
-        then copied back into rows [lo, hi) on x's device, and the caller's generator advances once, by what one device
-        would have consumed."""
-        lib = _native.load_library()
-        n_samples, n_nodes = x.size(0), x.size(1)
-        dev = x.device
-        d = self.n_dims + self.in_node_nf
-        self.dynamics._check_graph_type()
-        dev_seeds = self._per_molecule_seeds(seeds, noise, None, x)
-        full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
-        on_device, noise = (False, None) if dev_seeds is not None else self._noise(noise, x, node_mask, fragment_mask)
-        slices = device_slices(n_samples, self.devices)
+        split = self.devices is not None and batch_slice is None
+        slices = device_slices(n_samples, self.devices) if split else [(self.dynamics._device_index(x), 0, 0, n_samples)]
         if not slices:
             raise ValueError("sample_chain needs at least one molecule")
         if on_device:
+            gen = _generator_of(dev)
             # the device-side stream reproduces torch's randn launch geometry, which depends on the device's SM count
             geometry = lambda i: (torch.cuda.get_device_properties(i).multi_processor_count,
                                   torch.cuda.get_device_properties(i).max_threads_per_multi_processor)
-            caller = geometry(_generator_of(dev).device.index)
-            odd = sorted({s[0] for s in slices if geometry(s[0]) != caller})
+            odd = sorted({s[0] for s in slices if geometry(s[0]) != geometry(gen.device.index)})
             if odd:
                 raise ValueError(f"devices {odd} differ from {dev} in SM count or threads per SM, so they cannot reproduce its "
                                  "noise stream; list devices of one model, or inject the noise")
-            gen = _generator_of(dev)
             seed, offset = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF, gen.get_offset()
+            b0, b_full = (0, n_samples) if batch_slice is None else map(int, batch_slice)
+        engines = self.dynamics.engines([(dev_i, replica) for dev_i, replica, _, _ in slices])
         coef = self.step_coefficients(keep_frames, n_samples)
         norm = self._norm()
-        ptr = lambda v: None if v is None else v.data_ptr()
-        calls, inputs, chains, flags, consumed = {}, [], [], [], []
-        engines = self.dynamics.engines([(dev_i, replica) for dev_i, replica, _, _ in slices])
-        for (dev_i, replica, lo, hi), eng in zip(slices, engines):
-            cuda_i = torch.device('cuda', dev_i)
-            with torch.cuda.device(cuda_i):
-                t = {k: None if v is None else v.to(cuda_i).contiguous() for k, v in slice_sampler_inputs(full, lo, hi).items()}
-                nz = None if noise is None else noise[:, lo:hi].to(cuda_i).contiguous()
-                sd = None if dev_seeds is None else dev_seeds[lo:hi].to(cuda_i).contiguous()
-                chain_i = torch.empty((keep_frames, hi - lo, n_nodes, d), device=cuda_i, dtype=torch.float32)
-                flags_i = torch.zeros(hi - lo, dtype=torch.int32, device=cuda_i)
-                stream = torch.cuda.current_stream(cuda_i).cuda_stream
-            head = self._head(hi - lo, n_nodes, keep_frames, t)
-            tail = (coef, norm, ptr(chain_i), ptr(flags_i))
-            if sd is not None:
-                call = (lambda eng=eng, head=head, sd=sd, tail=tail, stream=stream:
-                        _native.check(lib.dl_sample_chain_seeded(eng, *head, ptr(sd), *tail, stream), "dl_sample_chain_seeded"))
-            elif on_device:
-                call = (lambda eng=eng, lo=lo, head=head, tail=tail, stream=stream:
-                        consumed.append(_run_chain_rng(lib, eng, (lo, n_samples), seed, offset, head, tail + (stream,))))
+        chain = torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32)
+        flags = torch.zeros(n_samples, dtype=torch.int32, device=dev)
+        places = [torch.device('cuda', dev_i) for dev_i, *_ in slices] if split else [dev]
+        whole = places == [dev]             # one slice, the whole batch where it is: it samples the caller's tensors
+        results, calls, parts = [], {}, []  # (status, consumed) of every slice; each device's calls; every slice's tensors
+
+        def call(*args):
+            results.append(_sample_slice(lib, *args))
+        for (dev_i, _, lo, hi), eng, where in zip(slices, engines, places):
+            if whole:
+                part = (full, noise, dev_seeds, chain, flags)
             else:
-                call = (lambda eng=eng, head=head, nz=nz, tail=tail, stream=stream:
-                        _native.check(lib.dl_sample_chain(eng, *head, ptr(nz), *tail, stream), "dl_sample_chain"))
-            calls.setdefault(dev_i, []).append(call)
-            inputs.append((t, nz, sd))      # alive until the loops are done (the host waits on the flags below)
-            chains.append(chain_i)
-            flags.append(flags_i)
+                to = lambda v: None if v is None else v.to(where).contiguous()
+                with torch.cuda.device(where):
+                    part = ({k: to(v) for k, v in slice_sampler_inputs(full, lo, hi).items()},
+                            to(None if noise is None else noise[:, lo:hi]), to(None if dev_seeds is None else dev_seeds[lo:hi]),
+                            torch.empty((keep_frames, hi - lo, n_nodes, d), device=where, dtype=torch.float32),
+                            torch.zeros(hi - lo, dtype=torch.int32, device=where))
+            parts.append(part)              # alive until the flags have been read below
+            t, nz, sd, chain_i, flags_i = part
+            stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
+            calls.setdefault(dev_i, []).append(functools.partial(
+                call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
+                stream, nz, sd, (seed, offset, b0 + lo, b_full) if on_device else None))
         try:
-            _run_per_device(calls)
+            if len(slices) == 1:            # on the caller's thread
+                with torch.cuda.device(slices[0][0]):
+                    calls[slices[0][0]][0]()
+            else:
+                _run_per_device(calls)
         except BaseException:
             for dev_i in calls:             # let the loops that were enqueued finish before their inputs are released
                 try:
@@ -459,21 +417,23 @@ class EDM(torch.nn.Module):
                     pass
             raise
         if on_device:
+            consumed = [used for _, used in results]
             assert len(set(consumed)) == 1, consumed
             gen.set_offset(offset + consumed[0])
-        chain = place_rows(torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32), chains, slices,
-                           dim=1)
-        all_flags = place_rows(torch.zeros(n_samples, dtype=torch.int32, device=dev), flags, slices)
-        bad = bool(all_flags.any().item())  # waits for every slice's loop and copy
+        if not whole:
+            place_rows(chain, [p[3] for p in parts], slices, dim=1)
+            place_rows(flags, [p[4] for p in parts], slices)
+        # the host sampler reports NaNs in its status; on the device, one sync per chain instead of one per step
+        # (egnn.py:441), after every slice's loop and copy
+        bad = _native.DL_NAN_DETECTED in [st for st, _ in results] or bool(flags.any().item())
         loop_ms = []
         for (dev_i, _, lo, hi), eng in zip(slices, engines):
             with torch.cuda.device(dev_i):
                 loop_ms.append((dev_i, lo, hi, float(lib.dl_last_elapsed_ms(eng))))
-        self.last_slice_loop_ms = loop_ms
         self.last_loop_ms = max(ms for *_, ms in loop_ms)
-        del inputs
+        self.last_slice_loop_ms = loop_ms if split else None
         if bad:
-            raise nan_exception_class()(flags=all_flags.cpu().tolist())
+            raise nan_exception_class()(flags=flags.cpu().tolist())
         return chain
 
 

@@ -117,6 +117,16 @@ class Dynamics(nn.Module):
     def _check_graph_type(self):
         assert self.graph_type == 'FC'  # src/egnn.py:383
 
+    def dl_config(self, device_index: int):
+        """The dl_config the engine on CUDA device `device_index` is created with."""
+        return _native.DLConfig(
+            n_dims=self.n_dims, in_node_nf=self.in_node_nf, context_node_nf=self.context_node_nf,
+            hidden_nf=self.hidden_nf, n_layers=self.n_layers, inv_sublayers=self.inv_sublayers,
+            condition_time=int(self.condition_time), centering=int(self.centering),
+            graph_type=_native.GRAPH_TYPES[self.graph_type], device=device_index,
+            edge_impl=_native.EDGE_IMPLS[self.edge_impl], norm_constant=float(self.norm_constant),
+            normalization_factor=float(self.normalization_factor))
+
     def egnn_options(self):
         """The EGNN options the engine is created with (dl_create_ex)."""
         return _native.DLEgnnOptions(tanh=int(bool(self.tanh)), coords_range=_native.COORDS_RANGE,
@@ -149,13 +159,7 @@ class Dynamics(nn.Module):
             return handle
         if handle is None or uploaded is None or uploaded[0] != key[0]:
             self._destroy(slot)
-            cfg = _native.DLConfig(
-                n_dims=self.n_dims, in_node_nf=self.in_node_nf, context_node_nf=self.context_node_nf,
-                hidden_nf=self.hidden_nf, n_layers=self.n_layers, inv_sublayers=self.inv_sublayers,
-                condition_time=int(self.condition_time), centering=int(self.centering),
-                graph_type=_native.GRAPH_TYPES[self.graph_type], device=device_index,
-                edge_impl=_native.EDGE_IMPLS[self.edge_impl], norm_constant=float(self.norm_constant),
-                normalization_factor=float(self.normalization_factor))
+            cfg = self.dl_config(device_index)
             handle = C.c_void_p()
             _native.check(lib.dl_create_ex(C.byref(cfg), C.byref(self.egnn_options()), C.byref(handle)), "dl_create_ex")
             self._engines[slot] = (handle, None)

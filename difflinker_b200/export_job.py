@@ -46,12 +46,7 @@ def _write(path, edm, x, h, node_mask, fragment_mask, linker_mask, edge_mask, co
     assert 1 <= keep_frames <= T
     xn, hn = edm.normalize(x, h)
     xh = torch.cat([xn, hn], dim=2).to(torch.float32).cpu().contiguous()
-    cfg = _native.DLConfig(
-        n_dims=dyn.n_dims, in_node_nf=dyn.in_node_nf, context_node_nf=dyn.context_node_nf, hidden_nf=dyn.hidden_nf,
-        n_layers=dyn.n_layers, inv_sublayers=dyn.inv_sublayers, condition_time=int(dyn.condition_time),
-        centering=int(dyn.centering), graph_type=_native.GRAPH_TYPES[dyn.graph_type], device=device_index,
-        edge_impl=_native.EDGE_IMPLS[dyn.edge_impl], norm_constant=float(dyn.norm_constant),
-        normalization_factor=float(dyn.normalization_factor))
+    cfg = dyn.dl_config(device_index)
     opts = dyn.egnn_options()
     assert C.sizeof(cfg) == 13 * 4 and C.sizeof(_native.DLStepCoef) == 32 and C.sizeof(opts) == 16
     coef = edm.step_coefficients(keep_frames, B)

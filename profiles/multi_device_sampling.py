@@ -44,19 +44,19 @@ def sync_all():
         torch.cuda.synchronize(i)
 
 
-# host time each dl_sample_chain_rng call takes to return, per thread (wraps the function the split path calls)
+# host time each slice's dl_sample_chain_rng call takes to return, per thread (wraps the function every slice is sampled by)
 _enqueue = []
-_run_chain_rng = edm_module._run_chain_rng
+_sample_slice = edm_module._sample_slice
 
 
-def _timed_run_chain_rng(*args):
+def _timed_sample_slice(*args, **kwargs):
     t0 = time.perf_counter()
-    out = _run_chain_rng(*args)
+    out = _sample_slice(*args, **kwargs)
     _enqueue.append((threading.current_thread().name, 1e3 * (time.perf_counter() - t0)))
     return out
 
 
-edm_module._run_chain_rng = _timed_run_chain_rng
+edm_module._sample_slice = _timed_sample_slice
 
 
 def device_windows(prof):
