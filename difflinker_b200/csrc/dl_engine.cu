@@ -18,6 +18,7 @@
 #include "kernels_simt.cuh"
 #include "kernels_tc.cuh"
 #include "kernels_node_tc.cuh"
+#include "kernels_retry.cuh"
 
 using namespace dl;
 
@@ -57,7 +58,7 @@ struct Workspace {
   std::vector<void*> allocs;
 };
 
-struct HostStage {  // device staging for the *_host entry points
+struct HostStage {  // device staging for the *_host entry points, and the sub-batch rows of dl_sample_chain_seeded_retry
   size_t cap = 0;
   char* buf = nullptr;
 };
@@ -124,6 +125,13 @@ struct dl_engine {
   std::vector<EqW> eq;         // [L]
   const float *We_t = nullptr, *be = nullptr, *Wo = nullptr, *bo = nullptr;
   Workspace ws;
+  // dl_sample_chain_seeded_retry: the loop workspace of the failed molecules' sub-batch (cached by (B', N) like ws, which it
+  // never frees or resizes), their gathered inputs and chain, and the events of the rounds (ev_r*: the sub-batch loop's
+  // own, so ev_t0/ev_t1 keep timing the first loop; ev_g*: one round, gather to scatter)
+  Workspace ws_sub;
+  HostStage sub_rows;
+  cudaEvent_t ev_r0 = nullptr, ev_r1 = nullptr, ev_g0 = nullptr, ev_g1 = nullptr;
+  float retry_ms = 0.f;
   cudaStream_t loop_stream = nullptr;
   cudaEvent_t ev_in = nullptr, ev_out = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
   float* coef_dev = nullptr;
@@ -614,8 +622,7 @@ struct StageLayout {
   template <typename T> T* at(int i) const { return bufs[i].used ? reinterpret_cast<T*>(base + bufs[i].off) : nullptr; }
 };
 
-dl_status stage_inputs(dl_engine* e, StageLayout& sl, cudaStream_t st) {
-  HostStage& sg = e->stage;
+dl_status stage_inputs(HostStage& sg, StageLayout& sl, cudaStream_t st) {
   if (sg.cap < sl.total) {
     if (sg.buf) cudaFree(sg.buf);
     sg.buf = nullptr; sg.cap = 0;
@@ -665,6 +672,22 @@ dl_status check_sampler(const dl_engine* e, int sampler, int T, int keep_frames,
 
 // standard-normal draws of one chain: init + one per step + final (linker), or their masked pairs (inpainting)
 uint64_t sampler_draws(int sampler, int T) { return sampler == DL_SAMPLER_INPAINT ? (uint64_t)2 * T + 3 : (uint64_t)T + 2; }
+
+// While alive, the engine's loop runs on the sub-batch workspace and records its loop time on the ev_r* events: the
+// full batch's workspace, the first loop's dl_last_elapsed_ms and the forward state dl_time_edge_kernel replays stay put.
+struct SubBatchScope {
+  dl_engine* e;
+  const int8_t* edge_mask;
+  const float* linker_mask;
+  int B, N;
+  explicit SubBatchScope(dl_engine* e_)
+      : e(e_), edge_mask(e_->last_edge_mask), linker_mask(e_->last_linker_mask), B(e_->last_B), N(e_->last_N) { swap(); }
+  ~SubBatchScope() {
+    swap();
+    e->last_edge_mask = edge_mask; e->last_linker_mask = linker_mask; e->last_B = B; e->last_N = N;
+  }
+  void swap() { std::swap(e->ws, e->ws_sub); std::swap(e->ev_t0, e->ev_r0); std::swap(e->ev_t1, e->ev_r1); }
+};
 
 }  // namespace
 
@@ -716,6 +739,10 @@ dl_status dl_create_ex(const dl_config* cfg, const dl_egnn_options* opts, dl_eng
   CK(cudaEventCreateWithFlags(&e->ev_out, cudaEventDisableTiming));
   CK(cudaEventCreate(&e->ev_t0));
   CK(cudaEventCreate(&e->ev_t1));
+  CK(cudaEventCreate(&e->ev_r0));
+  CK(cudaEventCreate(&e->ev_r1));
+  CK(cudaEventCreate(&e->ev_g0));
+  CK(cudaEventCreate(&e->ev_g1));
   CK(cudaMalloc((void**)&e->step_ctr, 2 * sizeof(int)));
   CK(cudaFuncSetAttribute(k_node<ACT_SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * NODE_TM * LDX * sizeof(float)));
   CK(opt_in_edge_simt<true>());
@@ -737,6 +764,8 @@ dl_status dl_destroy(dl_engine* e) {
   cudaSetDevice(e->cfg.device);
   cudaDeviceSynchronize();
   free_workspace(e->ws);
+  free_workspace(e->ws_sub);
+  if (e->sub_rows.buf) cudaFree(e->sub_rows.buf);
   if (e->wblob) cudaFree(e->wblob);
   if (e->wblob_tc) cudaFree(e->wblob_tc);
   if (e->coef_dev) cudaFree(e->coef_dev);
@@ -747,6 +776,7 @@ dl_status dl_destroy(dl_engine* e) {
   if (e->ev_out) cudaEventDestroy(e->ev_out);
   if (e->ev_t0) cudaEventDestroy(e->ev_t0);
   if (e->ev_t1) cudaEventDestroy(e->ev_t1);
+  for (cudaEvent_t ev : {e->ev_r0, e->ev_r1, e->ev_g0, e->ev_g1}) if (ev) cudaEventDestroy(ev);
   delete e;
   return DL_OK;
 }
@@ -851,7 +881,7 @@ dl_status dl_dynamics_forward_host(dl_engine* e, int32_t B, int32_t N, const flo
             i_lm = sl.in(linker_mask, n * 4), i_em = sl.in(fc_em ? edge_mask : nullptr, n * N),
             i_ctx = sl.in(context, n * e->cfg.context_node_nf * 4), i_out = sl.out(xh_bytes), i_fl = sl.out(B * 4);
   cudaStream_t st = e->loop_stream;
-  if ((s = stage_inputs(e, sl, st)) != DL_OK) return s;
+  if ((s = stage_inputs(e->stage, sl, st)) != DL_OK) return s;
   s = dl_dynamics_forward(e, B, N, sl.at<const float>(i_t), t_numel, sl.at<const float>(i_xh), sl.at<const int8_t>(i_nm),
                           sl.at<const float>(i_lm), sl.at<const int8_t>(i_em), sl.at<const float>(i_ctx),
                           sl.at<float>(i_out), sl.at<int32_t>(i_fl), st);
@@ -1094,13 +1124,91 @@ dl_status dl_sample_chain_host(dl_engine* e, int32_t sampler, int32_t B, int32_t
             i_ctx = sl.in(context, n * e->cfg.context_node_nf * 4), i_nz = sl.in(noise, sampler_draws(sampler, T) * frame_bytes),
             i_ch = sl.out(keep_frames * frame_bytes), i_fl = sl.out(B * 4);
   cudaStream_t st = e->loop_stream;
-  if ((s = stage_inputs(e, sl, st)) != DL_OK) return s;
+  if ((s = stage_inputs(e->stage, sl, st)) != DL_OK) return s;
   s = dl_sample_chain(e, sampler, B, N, T, keep_frames, sl.at<const float>(i_xh), sl.at<const int8_t>(i_nm),
                       sl.at<const float>(i_fm), sl.at<const float>(i_lm), sl.at<const int8_t>(i_em), sl.at<const float>(i_ctx),
                       sl.at<const float>(i_nz), coef, norm, sl.at<float>(i_ch), sl.at<int32_t>(i_fl), st);
   if (s != DL_OK) return s;
   return stage_results(chain, sl.at<float>(i_ch), keep_frames * frame_bytes, sl.at<int32_t>(i_fl), B, nan_flags, st);
 }
+
+uint64_t dl_retry_seed(uint64_t seed, int32_t attempt) { return retry_seed(seed, attempt); }
+
+dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                                       const float* xh, const int8_t* node_mask, const float* fragment_mask,
+                                       const float* linker_mask, const int8_t* edge_mask, const float* context,
+                                       const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
+                                       int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
+                                       void* stream) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
+  if (!nan_flags || !seeds_used || !attempts) { set_err("null argument (nan_flags, seeds_used or attempts)"); return DL_ERR_INVALID; }
+  e->retry_ms = 0.f;
+  dl_status s = dl_sample_chain_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask,
+                                       context, seeds, coef, norm, chain, nan_flags, stream);
+  if (s != DL_OK) return s;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CK(cudaMemcpyAsync(seeds_used, seeds, (size_t)B * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemsetAsync(attempts, 0, (size_t)B * sizeof(int32_t), st));
+  std::vector<int32_t> flags(B);
+  CK(cudaMemcpyAsync(flags.data(), nan_flags, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  // cut-off graphs never read edge_mask (the reference's batch-id vector is implied by the layout): the sub-batch gets none
+  const bool fc_em = edge_mask && e->cfg.graph_type == DL_GRAPH_FC;
+  const int xd = 3 + e->cfg.in_node_nf, C = e->cfg.context_node_nf;
+  for (int a = 1; a <= max_retries; ++a) {
+    std::vector<int32_t> rows;
+    for (int b = 0; b < B; ++b) if (flags[b] != 0) rows.push_back(b);
+    if (rows.empty()) break;
+    const int Bs = (int)rows.size();
+    const size_t n = (size_t)Bs * N;
+    StageLayout sl;
+    const int i_rows = sl.in(rows.data(), (size_t)Bs * sizeof(int32_t)), i_xh = sl.out(n * xd * 4), i_nm = sl.out(n),
+              i_fm = sl.out(n * 4), i_lm = sl.out(n * 4), i_em = sl.add(nullptr, n * N, fc_em),
+              i_ctx = sl.add(nullptr, n * C * 4, context != nullptr && C > 0), i_sd = sl.out((size_t)Bs * 8),
+              i_ch = sl.out((size_t)keep_frames * n * xd * 4), i_fl = sl.out((size_t)Bs * 4);
+    if ((s = stage_inputs(e->sub_rows, sl, st)) != DL_OK) return s;   // the row list goes to the device once per round
+    CK(cudaEventRecord(e->ev_g0, st));
+    RowGatherArgs ga{};
+    ga.rows = sl.at<const int>(i_rows); ga.N = N; ga.xd = xd; ga.C = C; ga.attempt = a;
+    ga.xh = xh; ga.fragment_mask = fragment_mask; ga.linker_mask = linker_mask; ga.context = sl.at<float>(i_ctx) ? context : nullptr;
+    ga.node_mask = node_mask; ga.edge_mask = fc_em ? edge_mask : nullptr;
+    ga.seeds = reinterpret_cast<const unsigned long long*>(seeds);
+    ga.s_xh = sl.at<float>(i_xh); ga.s_fragment_mask = sl.at<float>(i_fm); ga.s_linker_mask = sl.at<float>(i_lm);
+    ga.s_context = sl.at<float>(i_ctx); ga.s_node_mask = sl.at<int8_t>(i_nm); ga.s_edge_mask = sl.at<int8_t>(i_em);
+    ga.s_seeds = sl.at<unsigned long long>(i_sd);
+    k_gather_rows<<<Bs, 256, 0, st>>>(ga);
+    LAUNCH_CHECK();
+    e->launches += 1;
+    {
+      SubBatchScope sub(e);
+      s = dl_sample_chain_seeded(e, sampler, Bs, N, T, keep_frames, ga.s_xh, ga.s_node_mask, ga.s_fragment_mask,
+                                 ga.s_linker_mask, ga.s_edge_mask, ga.s_context, reinterpret_cast<const uint64_t*>(ga.s_seeds),
+                                 coef, norm, sl.at<float>(i_ch), sl.at<int32_t>(i_fl), stream);
+    }
+    if (s != DL_OK) return s;
+    RowScatterArgs sa{};
+    sa.rows = ga.rows; sa.B = B; sa.Bs = Bs; sa.N = N; sa.xd = xd; sa.attempt = a;
+    sa.s_chain = sl.at<float>(i_ch); sa.s_flags = sl.at<int32_t>(i_fl); sa.s_seeds = ga.s_seeds;
+    sa.chain = chain; sa.flags = nan_flags; sa.seeds_used = reinterpret_cast<unsigned long long*>(seeds_used);
+    sa.attempts = attempts;
+    k_scatter_rows<<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
+    LAUNCH_CHECK();
+    e->launches += 1;
+    CK(cudaEventRecord(e->ev_g1, st));
+    std::vector<int32_t> sub_flags(Bs);
+    CK(cudaMemcpyAsync(sub_flags.data(), sa.s_flags, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, e->ev_g0, e->ev_g1));
+    e->retry_ms += ms;
+    for (int i = 0; i < Bs; ++i) flags[rows[i]] = sub_flags[i];
+  }
+  for (int b = 0; b < B; ++b) if (flags[b] != 0) return DL_NAN_DETECTED;
+  return DL_OK;
+}
+
+float dl_last_retry_ms(dl_engine* e) { return e ? e->retry_ms : -1.f; }
 
 int64_t dl_launch_count(const dl_engine* e) { return e ? e->launches : 0; }
 

@@ -79,12 +79,16 @@ def sampler_inputs(model, data, sample_fn=None):
                 linker_mask=linker_mask, context=context)
 
 
-def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None):
+def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
-    `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size."""
+    `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
+    `nan_retries`: rounds that resample only the diverged molecules (EDM.sample_chain; None uses `model.edm.nan_retries`)."""
     kw = sampler_inputs(model, data, sample_fn)
-    chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **({} if seeds is None else {'seeds': seeds}))
+    extra = {} if seeds is None else {'seeds': seeds}
+    if nan_retries is not None:
+        extra['nan_retries'] = nan_retries
+    chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **extra)
     return chain, kw['node_mask']
 
 
@@ -123,8 +127,8 @@ class DDPM(nn.Module):
         self.edm = _build_edm(self.hparams, edge_impl=edge_impl)
         self.edm.devices = devices          # EDM.devices: split each sampling batch over these CUDA devices
 
-    def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None):
-        return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds)
+    def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None):
+        return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

@@ -24,13 +24,19 @@ def _generator_of(dev):
     return torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
 
 
-def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None):
+def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
-    samples host inputs (dl_sample_chain_host). Returns (status, what the batch stream consumed)."""
+    samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts) resamples the
+    molecules that diverged (dl_sample_chain_seeded_retry, which blocks until its rounds are done). Returns (status, what
+    the batch stream consumed)."""
     if stream is None:
         return _native.check(lib.dl_sample_chain_host(eng, *head, noise.data_ptr(), *tail), "dl_sample_chain_host"), 0
+    if retry is not None:
+        max_retries, used, attempts = retry
+        return _native.check(lib.dl_sample_chain_seeded_retry(eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(),
+                                                              attempts.data_ptr(), stream), "dl_sample_chain_seeded_retry"), 0
     if seeds is not None:
         return _native.check(lib.dl_sample_chain_seeded(eng, *head, seeds.data_ptr(), *tail, stream),
                              "dl_sample_chain_seeded"), 0
@@ -68,6 +74,18 @@ def seeds_tensor(seeds, n_samples):
     if len(out) != n_samples:
         raise ValueError(f"seeds holds {len(out)} values for a batch of {n_samples} molecules")
     return torch.tensor(out, dtype=torch.int64)
+
+
+def retry_seed(seed, attempt):
+    """The seed of attempt `attempt` of a molecule seeded with `seed` (dl_retry_seed: attempt 0 is the seed itself, attempt
+    a >= 1 is output a of a splitmix64 generator started from it), in the int64 form `last_seeds` holds. The seed is reduced
+    as seeds_tensor reduces it, so replaying with the returned value samples that attempt's stream."""
+    s = int(seeds_tensor([seed], 1)[0]) % (1 << 64)
+    attempt = operator.index(attempt)
+    if not -(1 << 31) <= attempt < (1 << 31):
+        raise ValueError(f"attempt {attempt} does not fit an int32")
+    r = int(_native.load_library().dl_retry_seed(s, attempt))
+    return r - (1 << 64) if r >= (1 << 63) else r
 
 
 def draw_seeds(n_samples, device):
@@ -136,6 +154,10 @@ class EDM(torch.nn.Module):
         #   seeds come from one draw_seeds call on the inputs' device, so torch.manual_seed still governs the run.
         self.noise_mode = 'reference_stream'
         self.last_seeds = None                 # per-molecule stream: the (B,) CPU int64 seeds of the last call, else None
+        # NaN recovery: how many times sample_chain resamples the molecules that diverged, with new seeds derived from their
+        # own (dl_retry_seed); needs per-molecule streams. 0, the default, raises FoundNaNException for the batch as before.
+        self.nan_retries = 0
+        self.last_attempts = None              # calls with nan_retries > 0: the (B,) CPU int32 attempt of every row, else None
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
@@ -320,6 +342,35 @@ class EDM(torch.nn.Module):
         self.last_seeds = cpu
         return dev_seeds
 
+    def _nan_retries(self, nan_retries, seeds, noise, batch_slice, x):
+        """The recovery rounds of a call: `nan_retries`, or the `nan_retries` attribute when None. More than 0 needs the
+        per-molecule stream on CUDA inputs, and no noise tensor, replaced draw function or batch_slice."""
+        n = self.nan_retries if nan_retries is None else nan_retries
+        try:
+            if isinstance(n, bool):
+                raise TypeError
+            n = operator.index(n)
+        except TypeError:
+            raise ValueError(f"nan_retries is a count of rounds (got {n!r})") from None
+        if n < 0:
+            raise ValueError(f"nan_retries must be >= 0 (got {n})")
+        if n >= 1 << 31:
+            raise ValueError(f"nan_retries {n} does not fit an int32")
+        if n == 0:
+            return 0
+        if noise is not None:
+            raise ValueError("nan_retries resamples diverged molecules with new seeds; an injected noise= tensor has no new draws")
+        if self._draws_replaced():
+            raise ValueError("nan_retries needs the device-side per-molecule stream, but this model's draw function is replaced")
+        if batch_slice is not None:
+            raise ValueError("nan_retries does not take batch_slice: pass each slice its rows of the seeds instead")
+        if seeds is None and self.noise_mode != 'per_molecule':
+            raise ValueError("nan_retries needs per-molecule streams: pass seeds= or set noise_mode='per_molecule' (the batch "
+                             f"stream, noise_mode={self.noise_mode!r}, cannot give one molecule new draws)")
+        if x.device.type != 'cuda':
+            raise ValueError(f"nan_retries needs CUDA inputs (got {x.device})")
+        return n
+
     def _head(self, n_samples, n_nodes, keep_frames, t):
         ptr = lambda v: None if v is None else v.data_ptr()
         return (self._SAMPLER, n_samples, n_nodes, self.T, keep_frames, ptr(t['x']), ptr(t['node_mask']),
@@ -330,7 +381,7 @@ class EDM(torch.nn.Module):
 
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None, seeds=None):
+                     noise=None, batch_slice=None, seeds=None, nan_retries=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `batch_slice=(b0, B_full)`: the inputs are rows [b0, b0+B) of a batch of B_full molecules (strong scaling,
@@ -343,6 +394,14 @@ class EDM(torch.nn.Module):
         which the reference's mean counts. The generator does not advance. noise_mode='per_molecule' samples that stream
         without `seeds` from draw_seeds. Either way `last_seeds` records the seeds; replaying one molecule with its seed
         reproduces its row, including a NaN divergence, so retry a diverged molecule with a new seed.
+        `nan_retries` (None: the `nan_retries` attribute, default 0) does that on the device: after the loop, up to that many
+        rounds resample only the molecules whose flags are set, as a sub-batch, with seeds dl_retry_seed(seed, round)
+        (dl_sample_chain_seeded_retry). It needs the per-molecule stream -- `seeds` or noise_mode='per_molecule' -- and raises
+        ValueError with the batch stream, noise=, a replaced draw function, host inputs or batch_slice. Rows that did not fail
+        are untouched, bit for bit; `last_seeds[b]` is then the seed that produced row b, so molecule b sampled alone with it
+        reproduces the row -- bit for bit on the SIMT edge path, and on the tensor-core path while no node tile rescales
+        (DESIGN.md section 6) -- and `last_attempts[b]` the round (0 = the first draw). Rows that still fail after the last
+        round raise FoundNaNException with their batch-global indices only; its `chain` attribute holds the recovered chain.
         The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
         and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
         device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
@@ -355,6 +414,8 @@ class EDM(torch.nn.Module):
         n_samples, n_nodes = x.size(0), x.size(1)
         dev = x.device
         d = self.n_dims + self.in_node_nf
+        self.last_attempts = None
+        retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
         full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
         on_device, noise = (False, None) if dev_seeds is not None else self._noise(noise, x, node_mask, fragment_mask)
@@ -381,6 +442,9 @@ class EDM(torch.nn.Module):
         norm = self._norm()
         chain = torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32)
         flags = torch.zeros(n_samples, dtype=torch.int32, device=dev)
+        # recovery: the seed that produced every row and its attempt
+        used, attempts = ((torch.empty(n_samples, dtype=torch.int64, device=dev), torch.empty(n_samples, dtype=torch.int32, device=dev))
+                          if retries else (None, None))
         places = [torch.device('cuda', dev_i) for dev_i, *_ in slices] if split else [dev]
         whole = places == [dev]             # one slice, the whole batch where it is: it samples the caller's tensors
         results, calls, parts = [], {}, []  # (status, consumed) of every slice; each device's calls; every slice's tensors
@@ -389,20 +453,23 @@ class EDM(torch.nn.Module):
             results.append(_sample_slice(lib, *args))
         for (dev_i, _, lo, hi), eng, where in zip(slices, engines, places):
             if whole:
-                part = (full, noise, dev_seeds, chain, flags)
+                part = (full, noise, dev_seeds, chain, flags, used, attempts)
             else:
                 to = lambda v: None if v is None else v.to(where).contiguous()
                 with torch.cuda.device(where):
                     part = ({k: to(v) for k, v in slice_sampler_inputs(full, lo, hi).items()},
                             to(None if noise is None else noise[:, lo:hi]), to(None if dev_seeds is None else dev_seeds[lo:hi]),
                             torch.empty((keep_frames, hi - lo, n_nodes, d), device=where, dtype=torch.float32),
-                            torch.zeros(hi - lo, dtype=torch.int32, device=where))
+                            torch.zeros(hi - lo, dtype=torch.int32, device=where),
+                            *((torch.empty(hi - lo, dtype=torch.int64, device=where),
+                               torch.empty(hi - lo, dtype=torch.int32, device=where)) if retries else (None, None)))
             parts.append(part)              # alive until the flags have been read below
-            t, nz, sd, chain_i, flags_i = part
+            t, nz, sd, chain_i, flags_i, used_i, attempts_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
             calls.setdefault(dev_i, []).append(functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
-                stream, nz, sd, (seed, offset, b0 + lo, b_full) if on_device else None))
+                stream, nz, sd, (seed, offset, b0 + lo, b_full) if on_device else None,
+                (retries, used_i, attempts_i) if retries else None))
         try:
             if len(slices) == 1:            # on the caller's thread
                 with torch.cuda.device(slices[0][0]):
@@ -423,6 +490,9 @@ class EDM(torch.nn.Module):
         if not whole:
             place_rows(chain, [p[3] for p in parts], slices, dim=1)
             place_rows(flags, [p[4] for p in parts], slices)
+            if retries:
+                place_rows(used, [p[5] for p in parts], slices)
+                place_rows(attempts, [p[6] for p in parts], slices)
         # the host sampler reports NaNs in its status; on the device, one sync per chain instead of one per step
         # (egnn.py:441), after every slice's loop and copy
         bad = _native.DL_NAN_DETECTED in [st for st, _ in results] or bool(flags.any().item())
@@ -432,8 +502,13 @@ class EDM(torch.nn.Module):
                 loop_ms.append((dev_i, lo, hi, float(lib.dl_last_elapsed_ms(eng))))
         self.last_loop_ms = max(ms for *_, ms in loop_ms)
         self.last_slice_loop_ms = loop_ms if split else None
+        if retries:
+            self.last_seeds, self.last_attempts = used.cpu(), attempts.cpu()
         if bad:
-            raise nan_exception_class()(flags=flags.cpu().tolist())
+            exc = nan_exception_class()(flags=flags.cpu().tolist())
+            if retries:
+                exc.chain = chain           # the rows that did not fail, or were recovered, are good molecules
+            raise exc
         return chain
 
 
@@ -482,17 +557,17 @@ class InpaintingEDM(EDM):
         return 'draw_noise_inpaint' in self.__dict__ or type(self).draw_noise_inpaint is not _DRAW_NOISE_INPAINT
 
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None, seeds=None):
+                     noise=None, batch_slice=None, seeds=None, nan_retries=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
         (dl_sample_chain_rng), unless `draw_noise_inpaint` is replaced -- on the instance, in a subclass or on the class --
         in which case the replacement draws them. `batch_slice=(b0, B_full)` and `seeds` as in EDM.sample_chain: with
         seeds, molecule b's 2T+3 raw draws are those of the molecule sampled alone after torch.cuda.manual_seed(seeds[b]),
-        masked and projected per molecule as always."""
+        masked and projected per molecule as always. `nan_retries` as in EDM.sample_chain."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
-                                    batch_slice=batch_slice, seeds=seeds)
+                                    batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

@@ -3,7 +3,7 @@ state_dict names, the prepared inputs of `EDM.sample_chain` (reference src/edm.p
 (its configuration has centering = 1; its coefficient table carries qa / qb), the per-step coefficient table of the noise
 schedule and a Philox (seed, offset) pair -- or, in a seeded job (`write_seeded_job`), one seed per molecule.
 `examples/c_sampler.c` reads the file and samples through the C-ABI (`dl_sample_chain_rng`, or `dl_sample_chain_seeded`);
-`read_result` parses what it writes back."""
+`read_result` parses what it writes back (`read_retry_result` what it writes with `--retries k`)."""
 import ctypes as C
 import struct
 
@@ -101,3 +101,17 @@ def read_result(path, B, N, keep_frames, xd):
     flags = torch.from_numpy(np.frombuffer(raw, dtype=np.int32, count=B, offset=12 + 4 * n).copy())
     assert len(raw) == 12 + 4 * n + 4 * B
     return status, consumed, chain, flags
+
+
+def read_retry_result(path, B, N, keep_frames, xd):
+    """What `c_sampler --retries k` writes: read_result's (status, consumed, chain, flags), then the seeds that produced the
+    rows as a (B,) int64 tensor with their 64 bits (the form EDM.last_seeds holds) and the (B,) int32 attempts."""
+    raw = open(path, "rb").read()
+    n = 12 + 4 * keep_frames * B * N * xd + 4 * B
+    assert len(raw) == n + 12 * B
+    status, consumed = struct.unpack_from("<iQ", raw, 0)
+    chain = torch.from_numpy(np.frombuffer(raw, dtype=np.float32, count=keep_frames * B * N * xd, offset=12).copy())
+    flags = torch.from_numpy(np.frombuffer(raw, dtype=np.int32, count=B, offset=n - 4 * B).copy())
+    used = torch.from_numpy(np.frombuffer(raw, dtype="<i8", count=B, offset=n).copy())
+    attempts = torch.from_numpy(np.frombuffer(raw, dtype=np.int32, count=B, offset=n + 8 * B).copy())
+    return status, consumed, chain.view(keep_frames, B, N, xd), flags, used, attempts

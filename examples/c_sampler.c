@@ -3,7 +3,7 @@
  * EDM.sample_chain (reference src/edm.py:126-235), or of InpaintingEDM.sample_chain (edm.py:549-727) for a model built
  * with centering, without Python and without a noise tensor.
  *
- *   c_sampler <job.bin> <out.bin>
+ *   c_sampler [--retries k] <job.bin> <out.bin>
  *
  * job.bin (little endian, written by difflinker_b200/export_job.py from a DDPM and a batch) holds the dl_config (magic
  * DLJOB2: followed by the model's dl_egnn_options -- tanh, mean aggregation), the weights under the reference's state_dict names, the normalised inputs and masks of one batch, the per-step
@@ -13,7 +13,9 @@
  * dl_config) holds one uint64 seed per molecule instead of the pair and samples with dl_sample_chain_seeded: each molecule
  * then draws what it would draw sampled alone, so any molecule can be replayed from its seed.
  * out.bin: int32 status, uint64 philox offset consumed (0 for a seeded job), the (keep_frames, B, N, 3+F) chain,
- * B NaN flags.
+ * B NaN flags. `--retries k` (seeded jobs only) samples with dl_sample_chain_seeded_retry instead: up to k rounds resample
+ * the molecules that diverged with new seeds (dl_retry_seed), and out.bin goes on with the B uint64 seeds that produced the
+ * rows and the B int32 attempts (0 = the first draw); only rows that still fail keep their flags.
  *
  * Build: gcc -std=c99 -O2 examples/c_sampler.c -Iinclude -I/usr/local/cuda/include -Ldifflinker_b200 -ldifflinker_b200 \
  *            -L/usr/local/cuda/lib64 -lcudart -Wl,-rpath,$PWD/difflinker_b200 -o c_sampler
@@ -49,7 +51,16 @@ static void* to_device(const void* host, size_t n) {
 }
 
 int main(int argc, char** argv) {
-  if (argc != 3) { fprintf(stderr, "usage: %s job.bin out.bin\n", argv[0]); return 2; }
+  int32_t retries = -1;                          /* -1: no recovery rounds (dl_sample_chain_seeded) */
+  if (argc == 5 && strcmp(argv[1], "--retries") == 0) {
+    char* end = NULL;
+    const long k = strtol(argv[2], &end, 10);
+    if (*argv[2] == 0 || *end != 0 || k < 0 || k > 1000000) { fprintf(stderr, "c_sampler: bad --retries %s\n", argv[2]); return 2; }
+    retries = (int32_t)k;
+    argv += 2;
+    argc -= 2;
+  }
+  if (argc != 3) { fprintf(stderr, "usage: %s [--retries k] job.bin out.bin\n", argv[0]); return 2; }
   FILE* f = fopen(argv[1], "rb");
   if (!f) { perror(argv[1]); return 2; }
   char magic[8];
@@ -57,6 +68,7 @@ int main(int argc, char** argv) {
   const int seeded = memcmp(magic, "DLJOB3\0\0", 8) == 0;
   int32_t with_opts = memcmp(magic, "DLJOB2\0\0", 8) == 0;
   if (!seeded && !with_opts && memcmp(magic, "DLJOB1\0\0", 8) != 0) { fprintf(stderr, "c_sampler: not a job file\n"); return 2; }
+  if (retries >= 0 && !seeded) { fprintf(stderr, "c_sampler: --retries needs a seeded (DLJOB3) job\n"); return 2; }
 
   dl_config cfg;
   rd(f, &cfg, sizeof cfg);                       /* 11 int32 + 2 float, no padding (checked by the exporter) */
@@ -112,8 +124,11 @@ int main(int argc, char** argv) {
   uint64_t* d_seeds = seeded ? (uint64_t*)to_device(seeds, (size_t)B * 8) : NULL;
   float* d_chain = NULL;
   int32_t* d_flags = NULL;
+  uint64_t* d_used = NULL;
+  int32_t* d_attempts = NULL;
   const size_t chain_bytes = (size_t)keep * n * xd * 4;
-  if (cudaMalloc((void**)&d_chain, chain_bytes) != cudaSuccess || cudaMalloc((void**)&d_flags, (size_t)B * 4) != cudaSuccess) {
+  if (cudaMalloc((void**)&d_chain, chain_bytes) != cudaSuccess || cudaMalloc((void**)&d_flags, (size_t)B * 4) != cudaSuccess ||
+      cudaMalloc((void**)&d_used, (size_t)B * 8) != cudaSuccess || cudaMalloc((void**)&d_attempts, (size_t)B * 4) != cudaSuccess) {
     fprintf(stderr, "c_sampler: cudaMalloc failed\n");
     return 2;
   }
@@ -123,12 +138,17 @@ int main(int argc, char** argv) {
   uint64_t consumed = 0;
   /* inpainting models are the ones built with centering (lightning.py:99); the engine refuses any other pairing */
   const int32_t sampler = cfg.centering ? DL_SAMPLER_INPAINT : DL_SAMPLER_LINKER;
-  const dl_status st = seeded
-      ? dl_sample_chain_seeded(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, d_seeds, coef, norm, d_chain,
-                               d_flags, stream)
-      : dl_sample_chain_rng(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, rng[0], rng[1], &consumed, coef,
-                            norm, d_chain, d_flags, stream);
-  if (st < 0) die(seeded ? "dl_sample_chain_seeded" : "dl_sample_chain_rng");
+  dl_status st;
+  if (retries >= 0)   /* blocks until its rounds are done */
+    st = dl_sample_chain_seeded_retry(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, d_seeds, coef, norm,
+                                      d_chain, d_flags, retries, d_used, d_attempts, stream);
+  else if (seeded)
+    st = dl_sample_chain_seeded(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, d_seeds, coef, norm, d_chain,
+                                d_flags, stream);
+  else
+    st = dl_sample_chain_rng(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, rng[0], rng[1], &consumed, coef,
+                             norm, d_chain, d_flags, stream);
+  if (st < 0) die(retries >= 0 ? "dl_sample_chain_seeded_retry" : seeded ? "dl_sample_chain_seeded" : "dl_sample_chain_rng");
   if (cudaStreamSynchronize(stream) != cudaSuccess) { fprintf(stderr, "c_sampler: the sampler's stream failed\n"); return 2; }
 
   float* chain = (float*)malloc(chain_bytes);
@@ -142,6 +162,17 @@ int main(int argc, char** argv) {
   fwrite(&consumed, 8, 1, o);
   fwrite(chain, 1, chain_bytes, o);
   fwrite(flags, 4, (size_t)B, o);
+  if (retries >= 0) {
+    uint64_t* used = (uint64_t*)malloc((size_t)B * 8);
+    int32_t* attempts = (int32_t*)malloc((size_t)B * 4);
+    cudaMemcpy(used, d_used, (size_t)B * 8, cudaMemcpyDeviceToHost);
+    cudaMemcpy(attempts, d_attempts, (size_t)B * 4, cudaMemcpyDeviceToHost);
+    fwrite(used, 8, (size_t)B, o);
+    fwrite(attempts, 4, (size_t)B, o);
+    printf("c_sampler: %d recovery round(s) allowed, %.2f ms of retry rounds on the device\n", retries, dl_last_retry_ms(e));
+    free(used);
+    free(attempts);
+  }
   fclose(o);
   printf("c_sampler: %d molecules x %d atoms, T=%d: %.2f ms on the device, %lld kernels, philox offset +%llu\n", B, N, T,
          dl_last_elapsed_ms(e), (long long)dl_launch_count(e), (unsigned long long)consumed);

@@ -18,6 +18,8 @@
  *     sample_p_xh_given_z0_only_linker  edm.py:210-235
  *   InpaintingEDM.sample_chain   src/edm.py:549-612      dl_sample_chain (+ _rng) with DL_SAMPLER_INPAINT
  *   either, one seed per molecule (no reference API)     dl_sample_chain_seeded
+ *   either, resampling only the molecules that diverged  dl_sample_chain_seeded_retry, dl_retry_seed, dl_last_retry_ms
+ *     (the reference's callers resample the whole batch, generate.py:153-161)
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   build_xae_molecule           src/molecule_builder.py:44-102       dl_bond_orders
  *   frame restore + .xyz text    generate.py:163-171, src/visualizer.py:14-31   dl_restore_frame, dl_format_xyz
@@ -211,6 +213,40 @@ dl_status dl_sample_chain_seeded(dl_engine* e, int32_t sampler, int32_t B, int32
                                  const float* linker_mask, const int8_t* edge_mask, const float* context,
                                  const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
                                  int32_t* nan_flags, void* stream);
+/*
+ * The seed of attempt `attempt` of a molecule whose own seed is `seed` (dl_sample_chain_seeded_retry): attempt 0 (or below)
+ * is `seed` itself; attempt a >= 1 is output a of a splitmix64 generator started from `seed`:
+ *     z = seed + a * 0x9E3779B97F4A7C15;  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
+ *     z = (z ^ (z >> 27)) * 0x94D049BB133111EB;  return z ^ (z >> 31);            (all modulo 2^64)
+ * For one attempt distinct seeds give distinct retry seeds. A pure host function.
+ */
+uint64_t dl_retry_seed(uint64_t seed, int32_t attempt);
+/*
+ * dl_sample_chain_seeded that resamples only the molecules that diverged. BLOCKING, unlike the other sampling entries: it
+ * runs the seeded loop, synchronises `stream` once and reads the B flags; then, for up to max_retries rounds, it gathers the
+ * molecules whose flag is set into a sub-batch (B' molecules, same N), samples it with dl_retry_seed(seeds[b], a) in round
+ * a, and writes its rows back over those molecules' rows of every one of the keep_frames frames of `chain` and of nan_flags.
+ * Rows that did not fail are not touched. Molecule b's row is then what dl_sample_chain_seeded gives it alone with seed
+ * seeds_used[b] -- bit for bit on the SIMT edge path; on the tensor-core path while no node tile rescales its fp16 operands,
+ * and a sub-batch of diverging molecules is where that happens (DESIGN.md section 6). Both samplers, every graph type;
+ * cut-off graphs never read edge_mask, so the sub-batch gets none.
+ *   max_retries  >= 0 rounds (0: the seeded loop plus the synchronisation)
+ *   nan_flags    (B) int32 DEVICE out, required: after the last round only the rows that still fail are set
+ *   seeds_used   (B) uint64 DEVICE out: the seed that produced each returned row (its attempt's dl_retry_seed)
+ *   attempts     (B) int32 DEVICE out: the attempt that produced each row, 0 = the first draw
+ * Returns DL_NAN_DETECTED only if some row still fails after the last round. The sub-batch has a workspace of its own, cached
+ * by (B', N); the full batch's is neither freed nor resized. dl_last_elapsed_ms keeps timing the first loop.
+ */
+dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                                       const float* xh, const int8_t* node_mask, const float* fragment_mask,
+                                       const float* linker_mask, const int8_t* edge_mask, const float* context,
+                                       const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
+                                       int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
+                                       void* stream);
+/* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_seeded_retry, each from its row gather
+ * to its row scatter -- including the wait for the host to capture the sub-batch's step graph -- summed over the rounds; 0
+ * when no round ran. */
+float dl_last_retry_ms(dl_engine* e);
 /* Strong scaling (SURVEY 8(e)): this engine samples molecules [b0, b0 + B) of a batch of B_full. The device-side noise of
  * the following dl_sample_chain_rng / dl_noise_fill / dl_noise_fill_inpaint calls is then the slice's ROWS of the
  * full-batch draws (and offset_consumed is the full batch's), so the gathered result is bit-identical to the single-GPU
