@@ -59,6 +59,9 @@ SYMBOLS = {
     "dl_retry_seed": (C.c_uint64, [C.c_uint64, _I32]),
     "dl_sample_chain_seeded_retry": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32,
                                             _P, _P, _P]),
+    "dl_sample_chain_seeded_retry_connected": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                                      _P, _I32, _P, _P, _I32, _P, _P, _P]),
+    "dl_molecule_connected": (_I32, [_I32, _I32, _I32, _P, _I32, _P, _P, _I32, _I32, _P, _P, _P]),
     "dl_last_retry_ms": (_F, [_P]),
     "dl_set_noise_slice": (_I32, [_P, _I32, _I32]),
     "dl_noise_fill": (_I32, [_P, _I32, _I32, _I32, C.c_uint64, C.c_uint64, _P, _P, _P]),

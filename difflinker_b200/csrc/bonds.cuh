@@ -1,0 +1,23 @@
+// The bond predicate of molecule_builder.get_bond_order (src/molecule_builder.py:77-102), shared by dl_bond_orders
+// (output_stage.cu) and the connectivity check of the recovery rounds (kernels_retry.cuh), so both decide "bonded" with
+// the same arithmetic.
+#pragma once
+
+namespace dl {
+
+// get_bond_order(...) > 0 for atoms at xi, xj of types ti, tj: the pair's distance in pm ("we change the metric") is
+// below the single-bond threshold thr1 of the type pair ordered by type index, [min type][max type] of the (T x T) table,
+// and that threshold exists (>= 0). Returns the pair's table index min * T + max when the atoms bond, else -1;
+// *dist_pm receives the distance in pm for the double / triple tests.
+__device__ __forceinline__ int bond_pair(float3 xi, float3 xj, int ti, int tj, int T, const float* __restrict__ thr1,
+                                         float* dist_pm) {
+  const float dx = xi.x - xj.x, dy = xi.y - xj.y, dz = xi.z - xj.z;
+  const float dist = 100.0f * sqrtf(dx * dx + dy * dy + dz * dz);
+  *dist_pm = dist;
+  const int a = min(ti, tj), c = max(ti, tj);
+  if (a < 0 || c >= T) return -1;
+  const float t1 = thr1[a * T + c];
+  return (t1 >= 0.f && dist < t1) ? a * T + c : -1;
+}
+
+}  // namespace dl

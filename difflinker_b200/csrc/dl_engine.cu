@@ -1134,15 +1134,34 @@ dl_status dl_sample_chain_host(dl_engine* e, int32_t sampler, int32_t B, int32_t
 
 uint64_t dl_retry_seed(uint64_t seed, int32_t attempt) { return retry_seed(seed, attempt); }
 
-dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
-                                       const float* xh, const int8_t* node_mask, const float* fragment_mask,
-                                       const float* linker_mask, const int8_t* edge_mask, const float* context,
-                                       const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
-                                       int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
-                                       void* stream) {
-  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
-  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
-  if (!nan_flags || !seeds_used || !attempts) { set_err("null argument (nan_flags, seeds_used or attempts)"); return DL_ERR_INVALID; }
+}  // extern "C"
+
+namespace {
+
+// The connectivity check of dl_sample_chain_seeded_retry_connected: the bond table and the (B) flags it writes.
+struct ConnCheck {
+  int n_types;
+  const float* thr1;
+  int32_t* connected;
+};
+
+// k_connected over frame 0 of a (B, N) chain of this engine's model: ligand rows only on cut-off (pocket) graphs.
+ConnArgs conn_args(const dl_engine* e, const ConnCheck& cc, const float* chain, int N, const int8_t* node_mask,
+                   const float* context, int32_t* connected) {
+  ConnArgs ca{};
+  ca.xh = chain; ca.N = N; ca.row_stride = 3 + e->cfg.in_node_nf; ca.n_types = cc.n_types; ca.thr1 = cc.thr1;
+  ca.node_mask = node_mask; ca.C = e->cfg.context_node_nf; ca.context = context;
+  ca.drop_pocket = e->cfg.graph_type != DL_GRAPH_FC; ca.connected = connected;
+  return ca;
+}
+
+// dl_sample_chain_seeded_retry, and with `cc` its connectivity check: a row then fails if its NaN flag is set or it is not
+// connected, and a resampled row replaces the caller's unless the caller's row is finite and the new one diverged.
+dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames, const float* xh,
+                       const int8_t* node_mask, const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
+                       const float* context, const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
+                       int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts, const ConnCheck* cc,
+                       void* stream) {
   e->retry_ms = 0.f;
   dl_status s = dl_sample_chain_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask,
                                        context, seeds, coef, norm, chain, nan_flags, stream);
@@ -1150,7 +1169,12 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CK(cudaMemcpyAsync(seeds_used, seeds, (size_t)B * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(attempts, 0, (size_t)B * sizeof(int32_t), st));
-  std::vector<int32_t> flags(B);
+  std::vector<int32_t> flags(B), conn(B, 1);
+  if (cc) {
+    CK(launch_connected(conn_args(e, *cc, chain, N, node_mask, context, cc->connected), B, st));
+    e->launches += 1;
+    CK(cudaMemcpyAsync(conn.data(), cc->connected, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  }
   CK(cudaMemcpyAsync(flags.data(), nan_flags, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   // cut-off graphs never read edge_mask (the reference's batch-id vector is implied by the layout): the sub-batch gets none
@@ -1158,7 +1182,7 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
   const int xd = 3 + e->cfg.in_node_nf, C = e->cfg.context_node_nf;
   for (int a = 1; a <= max_retries; ++a) {
     std::vector<int32_t> rows;
-    for (int b = 0; b < B; ++b) if (flags[b] != 0) rows.push_back(b);
+    for (int b = 0; b < B; ++b) if (flags[b] != 0 || conn[b] == 0) rows.push_back(b);
     if (rows.empty()) break;
     const int Bs = (int)rows.size();
     const size_t n = (size_t)Bs * N;
@@ -1166,7 +1190,8 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
     const int i_rows = sl.in(rows.data(), (size_t)Bs * sizeof(int32_t)), i_xh = sl.out(n * xd * 4), i_nm = sl.out(n),
               i_fm = sl.out(n * 4), i_lm = sl.out(n * 4), i_em = sl.add(nullptr, n * N, fc_em),
               i_ctx = sl.add(nullptr, n * C * 4, context != nullptr && C > 0), i_sd = sl.out((size_t)Bs * 8),
-              i_ch = sl.out((size_t)keep_frames * n * xd * 4), i_fl = sl.out((size_t)Bs * 4);
+              i_ch = sl.out((size_t)keep_frames * n * xd * 4), i_fl = sl.out((size_t)Bs * 4),
+              i_cn = sl.add(nullptr, (size_t)Bs * 4, cc != nullptr), i_tk = sl.add(nullptr, (size_t)Bs * 4, cc != nullptr);
     if ((s = stage_inputs(e->sub_rows, sl, st)) != DL_OK) return s;   // the row list goes to the device once per round
     CK(cudaEventRecord(e->ev_g0, st));
     RowGatherArgs ga{};
@@ -1192,19 +1217,88 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
     sa.s_chain = sl.at<float>(i_ch); sa.s_flags = sl.at<int32_t>(i_fl); sa.s_seeds = ga.s_seeds;
     sa.chain = chain; sa.flags = nan_flags; sa.seeds_used = reinterpret_cast<unsigned long long*>(seeds_used);
     sa.attempts = attempts;
-    k_scatter_rows<<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
+    if (cc) {
+      ConnArgs ca = conn_args(e, *cc, sa.s_chain, N, ga.s_node_mask, ga.s_context, sl.at<int32_t>(i_cn));
+      ca.rows = ga.rows; ca.flags = nan_flags; ca.s_flags = sa.s_flags; ca.take = sl.at<int32_t>(i_tk);
+      CK(launch_connected(ca, Bs, st));
+      e->launches += 1;
+      sa.take = ca.take; sa.s_connected = ca.connected; sa.connected = cc->connected;
+      k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
+    } else {
+      k_scatter_rows<false><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
+    }
     LAUNCH_CHECK();
     e->launches += 1;
     CK(cudaEventRecord(e->ev_g1, st));
-    std::vector<int32_t> sub_flags(Bs);
+    std::vector<int32_t> sub_flags(Bs), sub_conn(Bs, 1), take(Bs, 1);
     CK(cudaMemcpyAsync(sub_flags.data(), sa.s_flags, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (cc) {
+      CK(cudaMemcpyAsync(sub_conn.data(), sa.s_connected, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(take.data(), sa.take, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    }
     CK(cudaStreamSynchronize(st));
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, e->ev_g0, e->ev_g1));
     e->retry_ms += ms;
-    for (int i = 0; i < Bs; ++i) flags[rows[i]] = sub_flags[i];
+    for (int i = 0; i < Bs; ++i)
+      if (take[i]) { flags[rows[i]] = sub_flags[i]; conn[rows[i]] = sub_conn[i]; }
   }
   for (int b = 0; b < B; ++b) if (flags[b] != 0) return DL_NAN_DETECTED;
+  return DL_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                                       const float* xh, const int8_t* node_mask, const float* fragment_mask,
+                                       const float* linker_mask, const int8_t* edge_mask, const float* context,
+                                       const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
+                                       int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
+                                       void* stream) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
+  if (!nan_flags || !seeds_used || !attempts) { set_err("null argument (nan_flags, seeds_used or attempts)"); return DL_ERR_INVALID; }
+  return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
+                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, nullptr, stream);
+}
+
+dl_status dl_sample_chain_seeded_retry_connected(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
+                                                 int32_t keep_frames, const float* xh, const int8_t* node_mask,
+                                                 const float* fragment_mask, const float* linker_mask,
+                                                 const int8_t* edge_mask, const float* context, const uint64_t* seeds,
+                                                 const dl_step_coef* coef, const float* norm, float* chain, int32_t* nan_flags,
+                                                 int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
+                                                 int32_t n_types, const float* thr1, int32_t* connected, void* stream) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
+  if (!nan_flags || !seeds_used || !attempts || !thr1 || !connected) {
+    set_err("null argument (nan_flags, seeds_used, attempts, thr1 or connected)");
+    return DL_ERR_INVALID;
+  }
+  if (n_types < 1 || n_types > e->cfg.in_node_nf) {
+    set_err("n_types must be in [1, in_node_nf = %d] (got %d)", e->cfg.in_node_nf, n_types);
+    return DL_ERR_INVALID;
+  }
+  if (N > CONN_MAX_N) { set_err("the connectivity check takes N <= %d (got %d)", CONN_MAX_N, N); return DL_ERR_INVALID; }
+  const ConnCheck cc{n_types, thr1, connected};
+  return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
+                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, &cc, stream);
+}
+
+dl_status dl_molecule_connected(int32_t B, int32_t N, int32_t n_types, const float* xh, int32_t xh_row_stride,
+                                const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
+                                const float* thr1, int32_t* connected, void* stream) {
+  if (B <= 0 || N <= 0 || N > CONN_MAX_N || n_types < 1 || xh_row_stride < 3 + n_types || !xh || !node_mask || !thr1 ||
+      !connected || (drop_pocket && (!context || context_nf < 1))) {
+    set_err("dl_molecule_connected: invalid argument");
+    return DL_ERR_INVALID;
+  }
+  ConnArgs ca{};
+  ca.xh = xh; ca.N = N; ca.row_stride = xh_row_stride; ca.n_types = n_types; ca.thr1 = thr1; ca.node_mask = node_mask;
+  ca.context = context; ca.C = context_nf; ca.drop_pocket = drop_pocket != 0; ca.connected = connected;
+  CK(launch_connected(ca, B, reinterpret_cast<cudaStream_t>(stream)));
   return DL_OK;
 }
 

@@ -3,6 +3,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "bonds.cuh"
+
 namespace dl {
 
 // dl_retry_seed: attempt 0 (or below) is the molecule's own seed; attempt a >= 1 is output a of a splitmix64 generator
@@ -55,12 +57,19 @@ struct RowScatterArgs {
   int32_t* flags;
   unsigned long long* seeds_used;
   int32_t* attempts;
+  // CONN rounds only: take[i] (k_connected) says whether sub-batch row i replaces the caller's row; s_connected / connected
+  // are the sub-batch's and the caller's connectivity flags
+  const int32_t *take, *s_connected;
+  int32_t* connected;
 };
 
 // grid (Bs, keep_frames): CTA (i, f) writes frame f of sub-batch row i over row rows[i] of the caller's chain; the f = 0
-// CTAs also write the molecule's flags, the seed that produced the row and the attempt.
+// CTAs also write the molecule's flags, the seed that produced the row and the attempt. CONN: only rows with take[i] set,
+// and their connectivity flag with them.
+template <bool CONN>
 __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a) {
   const int i = blockIdx.x, f = blockIdx.y;
+  if (CONN && !a.take[i]) return;
   const size_t b = a.rows[i], row = (size_t)a.N * a.xd;
   const float* src = a.s_chain + ((size_t)f * a.Bs + i) * row;
   float* dst = a.chain + ((size_t)f * a.B + b) * row;
@@ -69,7 +78,120 @@ __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a) {
     a.flags[b] = a.s_flags[i];
     a.seeds_used[b] = a.s_seeds[i];
     a.attempts[b] = a.attempt;
+    if (CONN) a.connected[b] = a.s_connected[i];
   }
+}
+
+// ---- connectivity: is the final molecule in one piece? ---------------------------------------------------------------
+// The atoms of molecule b are its rows n with node_mask != 0, minus the pocket atoms (context column C - 1 set) when
+// drop_pocket; atoms i and j bond iff bond_pair (get_bond_order > 0) with types argmax(h[:n_types]). connected[b] = 1 iff
+// that graph has exactly one component (a single atom is connected, no atom is not): len(Chem.GetMolFrags(mol)) == 1 for
+// the molecule build_molecule makes of them (lightning.py:364-377, metrics.py:20-27).
+constexpr int CONN_MAX_N = 8192;                                     // rows per molecule: 20 bytes of shared memory each
+constexpr int CONN_SMEM_MAX = CONN_MAX_N * (int)(sizeof(float4) + sizeof(int));
+
+struct ConnArgs {
+  const float* xh;                       // (B, N, row_stride): x at columns 0..2, h from column 3 -- chain[0]
+  int N, row_stride, n_types, C, drop_pocket;
+  const float* thr1;                     // (n_types, n_types) single-bond thresholds in pm, [min type][max type]
+  const int8_t* node_mask;               // (B, N)
+  const float* context;                  // (B, N, C); read only when drop_pocket
+  int32_t* connected;                    // (B) out
+  // recovery rounds (rows != null): the molecules are sub-batch rows; take[i] = whether row i replaces the caller's row
+  // rows[i] -- always, unless the caller's row is finite (flags == 0) and the resampled one diverged
+  const int* rows;
+  const int32_t *flags, *s_flags;
+  int32_t* take;
+};
+
+// One CTA per molecule. The checked atoms are compacted, in row order, into shared memory (coordinates and type; padded
+// and pocket rows are never read beyond their masks). Components are then found by min-label hooking: every bonded pair
+// whose trees differ hooks the larger root under the smaller (atomicMin), trees are flattened, and this repeats until a
+// pass over all pairs hooks nothing. Labels only ever decrease and each root is its tree's smallest atom, so the final
+// labels -- every atom's component minimum -- and the flag do not depend on the order the threads hook in.
+__global__ void __launch_bounds__(256) k_connected(ConnArgs a) {
+  extern __shared__ float4 s_at[];                    // [n]: x, y, z, type (int bits)
+  int* s_lab = reinterpret_cast<int*>(s_at + a.N);    // [n]: parent pointers
+  __shared__ int s_warp[8], s_n, s_changed;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int b = blockIdx.x;
+  const size_t g0 = (size_t)b * a.N;
+  if (tid == 0) s_n = 0;
+  __syncthreads();
+  for (int r0 = 0; r0 < a.N; r0 += 256) {
+    const int r = r0 + tid;
+    bool ok = r < a.N && a.node_mask[g0 + r] != 0;
+    if (ok && a.drop_pocket) ok = a.context[(g0 + r) * a.C + a.C - 1] == 0.f;
+    const unsigned m = __ballot_sync(0xffffffffu, ok);
+    if (lane == 0) s_warp[warp] = __popc(m);
+    __syncthreads();
+    int off = s_n + __popc(m & ((1u << lane) - 1u)), total = 0;
+    for (int w = 0; w < 8; ++w) { off += w < warp ? s_warp[w] : 0; total += s_warp[w]; }
+    if (ok) {
+      const float* row = a.xh + (g0 + r) * a.row_stride;
+      int best = 0;                                   // torch.argmax: the first maximum; NaN wins
+      for (int k = 1; k < a.n_types; ++k) {
+        const float v = row[3 + k], cur = row[3 + best];
+        if (v > cur || (isnan(v) && !isnan(cur))) best = k;
+      }
+      s_at[off] = make_float4(row[0], row[1], row[2], __int_as_float(best));
+      s_lab[off] = off;
+    }
+    __syncthreads();
+    if (tid == 0) s_n += total;
+    __syncthreads();
+  }
+  const int n = s_n;
+  volatile int* lab = s_lab;
+  for (;;) {
+    if (tid == 0) s_changed = 0;
+    __syncthreads();
+    for (int i = warp; i < n; i += 8) {               // warp per row i, lanes over the pairs (i, j < i)
+      const float4 pi = s_at[i];
+      for (int j = lane; j < i; j += 32) {
+        const float4 pj = s_at[j];
+        float dist;
+        if (bond_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
+                      __float_as_int(pj.w), a.n_types, a.thr1, &dist) < 0)
+          continue;
+        int ri = i, rj = j;
+        while (lab[ri] != ri) ri = lab[ri];
+        while (lab[rj] != rj) rj = lab[rj];
+        if (ri != rj) {
+          atomicMin(&s_lab[max(ri, rj)], min(ri, rj));
+          s_changed = 1;
+        }
+      }
+    }
+    __syncthreads();
+    const int changed = s_changed;
+    for (int i = tid; i < n; i += 256) {              // flatten: every atom points at its root
+      int r = i;
+      while (lab[r] != r) r = lab[r];
+      lab[i] = r;
+    }
+    __syncthreads();
+    if (!changed) break;
+  }
+  int roots = 0;
+  for (int i0 = 0; i0 < n; i0 += 256) roots += __syncthreads_count(i0 + tid < n && lab[i0 + tid] == i0 + tid);
+  if (tid == 0) {
+    const int conn = roots == 1;
+    a.connected[b] = conn;
+    if (a.rows) a.take[b] = !(a.flags[a.rows[b]] == 0 && a.s_flags[b] != 0);
+  }
+}
+
+// Launches k_connected over B molecules; N <= CONN_MAX_N. The shared-memory limit is raised to its one maximum the first
+// time a molecule needs more than the default, so concurrent callers never lower it under each other.
+inline cudaError_t launch_connected(const ConnArgs& a, int B, cudaStream_t st) {
+  const size_t smem = (size_t)a.N * (sizeof(float4) + sizeof(int));
+  if (smem > 48 * 1024) {
+    const cudaError_t err = cudaFuncSetAttribute(k_connected, cudaFuncAttributeMaxDynamicSharedMemorySize, CONN_SMEM_MAX);
+    if (err != cudaSuccess) return err;
+  }
+  k_connected<<<B, 256, smem, st>>>(a);
+  return cudaGetLastError();
 }
 
 }  // namespace dl

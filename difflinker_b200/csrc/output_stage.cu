@@ -10,6 +10,7 @@
 #include <cstring>
 
 #include "../../include/difflinker_b200.h"
+#include "bonds.cuh"
 
 namespace {
 
@@ -133,18 +134,15 @@ __global__ void __launch_bounds__(256) k_bond_orders(int N, int T, const float* 
     if (j < i && node_mask[g0 + i] && node_mask[g0 + j]) {
       const float* xi = x + (g0 + i) * x_stride;
       const float* xj = x + (g0 + j) * x_stride;
-      const float dx = xi[0] - xj[0], dy = xi[1] - xj[1], dz = xi[2] - xj[2];
-      const float dist = 100.0f * sqrtf(dx * dx + dy * dy + dz * dz);       // "we change the metric" (pm)
-      const int ti = types[g0 + i], tj = types[g0 + j];
-      const int a = min(ti, tj), c = max(ti, tj);
-      if (a >= 0 && c < T) {
-        const float t1 = thr1[a * T + c], t2 = thr2[a * T + c], t3 = thr3[a * T + c];
-        if (t1 >= 0.f && dist < t1) {
-          order = 1;
-          if (t2 >= 0.f && dist < t2) {
-            order = 2;
-            if (t3 >= 0.f && dist < t3) order = 3;
-          }
+      float dist;
+      const int k = dl::bond_pair(make_float3(xi[0], xi[1], xi[2]), make_float3(xj[0], xj[1], xj[2]), types[g0 + i],
+                                  types[g0 + j], T, thr1, &dist);
+      if (k >= 0) {
+        const float t2 = thr2[k], t3 = thr3[k];
+        order = 1;
+        if (t2 >= 0.f && dist < t2) {
+          order = 2;
+          if (t3 >= 0.f && dist < t3) order = 3;
         }
       }
     }

@@ -18,7 +18,13 @@ from .edm import EDM, InpaintingEDM
 from .egnn import Dynamics, DynamicsWithPockets
 
 
-def _build_edm(hp: dict, edge_impl='auto'):
+def _is_geom(hp: dict):
+    """The reference DDPM's is_geom (lightning.py:73): the GEOM / MOAD atom types, whose bond tables include P."""
+    prefix = hp.get('train_data_prefix') or ''
+    return ('geom' in prefix) or ('MOAD' in prefix)
+
+
+def _build_edm(hp: dict, edge_impl='auto', is_geom=None):
     pocket = '.' in (hp.get('train_data_prefix') or '')
     graph_type = hp.get('graph_type')
     if graph_type is None:
@@ -41,7 +47,7 @@ def _build_edm(hp: dict, edge_impl='auto'):
     return edm_cls(dynamics=dynamics, in_node_nf=hp['in_node_nf'], n_dims=hp['n_dims'],
                timesteps=hp['diffusion_steps'], noise_schedule=hp['diffusion_noise_schedule'],
                noise_precision=hp['diffusion_noise_precision'], loss_type=hp['diffusion_loss_type'],
-               norm_values=hp['normalize_factors'])
+               norm_values=hp['normalize_factors'], is_geom=_is_geom(hp) if is_geom is None else bool(is_geom))
 
 
 def sampler_inputs(model, data, sample_fn=None):
@@ -79,15 +85,18 @@ def sampler_inputs(model, data, sample_fn=None):
                 linker_mask=linker_mask, context=context)
 
 
-def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None):
+def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
-    `nan_retries`: rounds that resample only the diverged molecules (EDM.sample_chain; None uses `model.edm.nan_retries`)."""
+    `nan_retries`: rounds that resample only the diverged molecules (EDM.sample_chain; None uses `model.edm.nan_retries`).
+    `require_connected`: the rounds also resample the disconnected molecules (None uses `model.edm.require_connected`)."""
     kw = sampler_inputs(model, data, sample_fn)
     extra = {} if seeds is None else {'seeds': seeds}
     if nan_retries is not None:
         extra['nan_retries'] = nan_retries
+    if require_connected is not None:
+        extra['require_connected'] = require_connected
     chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **extra)
     return chain, kw['node_mask']
 
@@ -127,8 +136,9 @@ class DDPM(nn.Module):
         self.edm = _build_edm(self.hparams, edge_impl=edge_impl)
         self.edm.devices = devices          # EDM.devices: split each sampling batch over these CUDA devices
 
-    def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None):
-        return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries)
+    def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None):
+        return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
+                            require_connected=require_connected)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")
@@ -165,7 +175,7 @@ def accelerate(ddpm, edge_impl='auto', devices=None):
     hp = dict(ddpm.hparams) if hasattr(ddpm, 'hparams') and len(dict(ddpm.hparams)) else None
     if hp is None:
         raise ValueError("the module carries no hparams; construct difflinker_b200.DDPM(**hparams) instead")
-    new_edm = _build_edm(hp, edge_impl=edge_impl)
+    new_edm = _build_edm(hp, edge_impl=edge_impl, is_geom=getattr(ddpm, 'is_geom', None))
     new_edm.load_state_dict(ddpm.edm.state_dict(), strict=True)
     new_edm.T = ddpm.edm.T
     new_edm.devices = devices

@@ -109,7 +109,8 @@ def slice_sampler_inputs(kw: dict, lo: int, hi: int):
     return out
 
 
-def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=True, seeds=None, nan_retries=None):
+def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=True, seeds=None, nan_retries=None,
+                         require_connected=None):
     """Strong scaling of ONE batch (SURVEY.md section 8(e)): the template batch is built once (so every rank pads to the same
     N), each rank runs the reverse loop for its contiguous slice of the molecules with the slice's rows of the full-batch
     noise, and the chains are gathered -- the result equals `model.sample_chain(data)` on one GPU bit for bit, for any
@@ -118,7 +119,9 @@ def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=T
     the full batch on every rank when `gather`, else the local slice.
     `seeds`: the full batch's B per-molecule seeds (EDM.sample_chain); each rank samples its rows with its rows of them,
     so the result equals `model.sample_chain(data, seeds=seeds)` on one GPU in the same sense. `nan_retries` (with seeds):
-    each rank resamples its own diverged molecules (EDM.sample_chain); a FoundNaNException names the rank's local rows."""
+    each rank resamples its own diverged molecules (EDM.sample_chain); a FoundNaNException names the rank's local rows.
+    `require_connected` (with seeds): each rank also resamples its own disconnected molecules; `model.edm.last_connected`
+    holds the rank's rows."""
     from .ddpm import sampler_inputs
     from .edm import seeds_tensor
     kw = sampler_inputs(model, data, sample_fn)
@@ -128,6 +131,8 @@ def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=T
     lo, hi = shard_range(B, rank, world)
     local = slice_sampler_inputs(kw, lo, hi)
     extra = {} if nan_retries is None else {'nan_retries': nan_retries}
+    if require_connected is not None:
+        extra['require_connected'] = require_connected
     if seeds is not None:
         chain = model.edm.sample_chain(**local, keep_frames=keep_frames, seeds=seeds_tensor(seeds, B)[lo:hi], **extra)
     else:

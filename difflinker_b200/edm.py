@@ -28,13 +28,19 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
-    samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts) resamples the
-    molecules that diverged (dl_sample_chain_seeded_retry, which blocks until its rounds are done). Returns (status, what
-    the batch stream consumed)."""
+    samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, conn) resamples
+    the molecules that diverged (dl_sample_chain_seeded_retry, which blocks until its rounds are done) and, with `conn` =
+    (thr1, connected), those that are not connected (dl_sample_chain_seeded_retry_connected). Returns (status, what the
+    batch stream consumed)."""
     if stream is None:
         return _native.check(lib.dl_sample_chain_host(eng, *head, noise.data_ptr(), *tail), "dl_sample_chain_host"), 0
     if retry is not None:
-        max_retries, used, attempts = retry
+        max_retries, used, attempts, conn = retry
+        if conn is not None:
+            thr1, connected = conn
+            return _native.check(lib.dl_sample_chain_seeded_retry_connected(
+                eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr(), thr1.shape[0],
+                thr1.data_ptr(), connected.data_ptr(), stream), "dl_sample_chain_seeded_retry_connected"), 0
         return _native.check(lib.dl_sample_chain_seeded_retry(eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(),
                                                               attempts.data_ptr(), stream), "dl_sample_chain_seeded_retry"), 0
     if seeds is not None:
@@ -132,6 +138,7 @@ class EDM(torch.nn.Module):
             loss_type='vlb',
             norm_values=(1., 1., 1.),
             norm_biases=(None, 0., 0.),
+            is_geom=None,
     ):
         super().__init__()
         if noise_schedule == 'learned':
@@ -158,6 +165,13 @@ class EDM(torch.nn.Module):
         # own (dl_retry_seed); needs per-molecule streams. 0, the default, raises FoundNaNException for the batch as before.
         self.nan_retries = 0
         self.last_attempts = None              # calls with nan_retries > 0: the (B,) CPU int32 attempt of every row, else None
+        # Connectivity: sample_chain also resamples, in the nan_retries rounds, the molecules whose final molecule is in more
+        # than one piece (dl_sample_chain_seeded_retry_connected); needs per-molecule streams and the bond tables of
+        # `is_geom` (the ZINC or the GEOM / MOAD atom types, molecule_builder.threshold_tables), which DDPM, accelerate and
+        # load_from_checkpoint set from the model's training data. False, the default, checks nothing.
+        self.is_geom = is_geom
+        self.require_connected = False
+        self.last_connected = None             # calls with require_connected: the (B,) CPU bool connectivity of every row
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
@@ -371,6 +385,39 @@ class EDM(torch.nn.Module):
             raise ValueError(f"nan_retries needs CUDA inputs (got {x.device})")
         return n
 
+    def _require_connected(self, require_connected, seeds, noise, batch_slice, x):
+        """Whether a call checks connectivity: `require_connected`, or the `require_connected` attribute when None. True
+        needs what nan_retries > 0 needs -- the per-molecule stream on CUDA inputs, no noise tensor, replaced draw function
+        or batch_slice -- and the bond tables of `is_geom`."""
+        c = self.require_connected if require_connected is None else require_connected
+        if not isinstance(c, bool):
+            raise ValueError(f"require_connected is True or False (got {c!r})")
+        if not c:
+            return False
+        if noise is not None:
+            raise ValueError("require_connected resamples disconnected molecules with new seeds; an injected noise= tensor has "
+                             "no new draws")
+        if self._draws_replaced():
+            raise ValueError("require_connected needs the device-side per-molecule stream, but this model's draw function is "
+                             "replaced")
+        if batch_slice is not None:
+            raise ValueError("require_connected does not take batch_slice: pass each slice its rows of the seeds instead")
+        if seeds is None and self.noise_mode != 'per_molecule':
+            raise ValueError("require_connected needs per-molecule streams: pass seeds= or set noise_mode='per_molecule' (the "
+                             f"batch stream, noise_mode={self.noise_mode!r}, cannot give one molecule new draws)")
+        if self.is_geom is None:
+            raise ValueError("require_connected needs the bond tables: build the EDM with is_geom=True (GEOM / MOAD atom "
+                             "types) or False (ZINC), or set edm.is_geom")
+        if x.device.type != 'cuda':
+            raise ValueError(f"require_connected needs CUDA inputs (got {x.device})")
+        return True
+
+    def _bond_table(self):
+        """The (T,T) fp32 single-bond thresholds of `is_geom` (molecule_builder.threshold_tables), the table that decides
+        whether two atoms bond."""
+        from .molecule_builder import threshold_tables
+        return threshold_tables(bool(self.is_geom))[0].contiguous()
+
     def _head(self, n_samples, n_nodes, keep_frames, t):
         ptr = lambda v: None if v is None else v.data_ptr()
         return (self._SAMPLER, n_samples, n_nodes, self.T, keep_frames, ptr(t['x']), ptr(t['node_mask']),
@@ -381,7 +428,7 @@ class EDM(torch.nn.Module):
 
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None, seeds=None, nan_retries=None):
+                     noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `batch_slice=(b0, B_full)`: the inputs are rows [b0, b0+B) of a batch of B_full molecules (strong scaling,
@@ -402,6 +449,13 @@ class EDM(torch.nn.Module):
         reproduces the row -- bit for bit on the SIMT edge path, and on the tensor-core path while no node tile rescales
         (DESIGN.md section 6) -- and `last_attempts[b]` the round (0 = the first draw). Rows that still fail after the last
         round raise FoundNaNException with their batch-global indices only; its `chain` attribute holds the recovered chain.
+        `require_connected` (None: the `require_connected` attribute, default False) adds a second reason to resample a row:
+        its final molecule -- chain[0]'s atoms, without the pocket on cut-off graphs, bonded where get_bond_order > 0 with
+        the tables of `is_geom` -- is in more than one piece (dl_sample_chain_seeded_retry_connected). The check runs on the
+        device after the loop and after every round; the rounds are the nan_retries rounds, so nan_retries=0 only reports.
+        A resampled row replaces the old one unless the old one was finite and the new one diverged. Rows that are still
+        disconnected after the last round are returned; `last_connected` (B,) CPU bool tells which rows are connected. It
+        raises ValueError where nan_retries does, and without `is_geom`.
         The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
         and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
         device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
@@ -415,7 +469,10 @@ class EDM(torch.nn.Module):
         dev = x.device
         d = self.n_dims + self.in_node_nf
         self.last_attempts = None
+        self.last_connected = None
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
+        check = self._require_connected(require_connected, seeds, noise, batch_slice, x)
+        recover = retries > 0 or check      # the recovery entry point: seeds used and attempts come back
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
         full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
         on_device, noise = (False, None) if dev_seeds is not None else self._noise(noise, x, node_mask, fragment_mask)
@@ -444,7 +501,10 @@ class EDM(torch.nn.Module):
         flags = torch.zeros(n_samples, dtype=torch.int32, device=dev)
         # recovery: the seed that produced every row and its attempt
         used, attempts = ((torch.empty(n_samples, dtype=torch.int64, device=dev), torch.empty(n_samples, dtype=torch.int32, device=dev))
-                          if retries else (None, None))
+                          if recover else (None, None))
+        # connectivity: every row's flag, and the bond table on each slice's device
+        connected = torch.empty(n_samples, dtype=torch.int32, device=dev) if check else None
+        thr1 = self._bond_table() if check else None
         places = [torch.device('cuda', dev_i) for dev_i, *_ in slices] if split else [dev]
         whole = places == [dev]             # one slice, the whole batch where it is: it samples the caller's tensors
         results, calls, parts = [], {}, []  # (status, consumed) of every slice; each device's calls; every slice's tensors
@@ -453,7 +513,7 @@ class EDM(torch.nn.Module):
             results.append(_sample_slice(lib, *args))
         for (dev_i, _, lo, hi), eng, where in zip(slices, engines, places):
             if whole:
-                part = (full, noise, dev_seeds, chain, flags, used, attempts)
+                part = (full, noise, dev_seeds, chain, flags, used, attempts, connected)
             else:
                 to = lambda v: None if v is None else v.to(where).contiguous()
                 with torch.cuda.device(where):
@@ -462,14 +522,16 @@ class EDM(torch.nn.Module):
                             torch.empty((keep_frames, hi - lo, n_nodes, d), device=where, dtype=torch.float32),
                             torch.zeros(hi - lo, dtype=torch.int32, device=where),
                             *((torch.empty(hi - lo, dtype=torch.int64, device=where),
-                               torch.empty(hi - lo, dtype=torch.int32, device=where)) if retries else (None, None)))
+                               torch.empty(hi - lo, dtype=torch.int32, device=where)) if recover else (None, None)),
+                            torch.empty(hi - lo, dtype=torch.int32, device=where) if check else None)
+            part = part + (None if thr1 is None else thr1.to(where),)
             parts.append(part)              # alive until the flags have been read below
-            t, nz, sd, chain_i, flags_i, used_i, attempts_i = part
+            t, nz, sd, chain_i, flags_i, used_i, attempts_i, connected_i, thr1_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
             calls.setdefault(dev_i, []).append(functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, (seed, offset, b0 + lo, b_full) if on_device else None,
-                (retries, used_i, attempts_i) if retries else None))
+                (retries, used_i, attempts_i, (thr1_i, connected_i) if check else None) if recover else None))
         try:
             if len(slices) == 1:            # on the caller's thread
                 with torch.cuda.device(slices[0][0]):
@@ -490,9 +552,11 @@ class EDM(torch.nn.Module):
         if not whole:
             place_rows(chain, [p[3] for p in parts], slices, dim=1)
             place_rows(flags, [p[4] for p in parts], slices)
-            if retries:
+            if recover:
                 place_rows(used, [p[5] for p in parts], slices)
                 place_rows(attempts, [p[6] for p in parts], slices)
+            if check:
+                place_rows(connected, [p[7] for p in parts], slices)
         # the host sampler reports NaNs in its status; on the device, one sync per chain instead of one per step
         # (egnn.py:441), after every slice's loop and copy
         bad = _native.DL_NAN_DETECTED in [st for st, _ in results] or bool(flags.any().item())
@@ -502,11 +566,13 @@ class EDM(torch.nn.Module):
                 loop_ms.append((dev_i, lo, hi, float(lib.dl_last_elapsed_ms(eng))))
         self.last_loop_ms = max(ms for *_, ms in loop_ms)
         self.last_slice_loop_ms = loop_ms if split else None
-        if retries:
+        if recover:
             self.last_seeds, self.last_attempts = used.cpu(), attempts.cpu()
+        if check:
+            self.last_connected = connected.cpu() != 0
         if bad:
             exc = nan_exception_class()(flags=flags.cpu().tolist())
-            if retries:
+            if recover:
                 exc.chain = chain           # the rows that did not fail, or were recovered, are good molecules
             raise exc
         return chain
@@ -557,17 +623,19 @@ class InpaintingEDM(EDM):
         return 'draw_noise_inpaint' in self.__dict__ or type(self).draw_noise_inpaint is not _DRAW_NOISE_INPAINT
 
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None, seeds=None, nan_retries=None):
+                     noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
         (dl_sample_chain_rng), unless `draw_noise_inpaint` is replaced -- on the instance, in a subclass or on the class --
         in which case the replacement draws them. `batch_slice=(b0, B_full)` and `seeds` as in EDM.sample_chain: with
         seeds, molecule b's 2T+3 raw draws are those of the molecule sampled alone after torch.cuda.manual_seed(seeds[b]),
-        masked and projected per molecule as always. `nan_retries` as in EDM.sample_chain."""
+        masked and projected per molecule as always. `nan_retries` and `require_connected` as in EDM.sample_chain; the
+        connectivity check covers every atom of the molecule."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
-                                    batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries)
+                                    batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
+                                    require_connected=require_connected)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

@@ -61,6 +61,31 @@ def bond_orders(one_hot, x, node_mask, is_geom, margins=MARGINS_EDM):
     return E
 
 
+@torch.no_grad()
+def connected(xh, node_mask, is_geom, pocket_only=None):
+    """(B,) bool on the device: whether each molecule is in one piece (dl_molecule_connected, the check behind
+    sample_chain(require_connected=True)). Its atoms are the rows with node_mask != 0, minus those with pocket_only != 0
+    when given; atoms i and j bond iff get_bond_order > 0, i.e. E[i, j] != 0 of bond_orders. `xh` is chain[0]-style
+    (B,N,3+F): the atom types are argmax of its first T feature columns (T = 9 with is_geom, else 8). One atom is
+    connected, none is not."""
+    dev = xh.device
+    if dev.type != 'cuda':
+        raise RuntimeError("connected runs on the GPU (no CPU fallback); move the tensors to the device")
+    B, N = xh.shape[:2]
+    xs = xh.float().contiguous()
+    nm = (node_mask.reshape(B, N) != 0).to(torch.int8).contiguous()
+    po = None if pocket_only is None else pocket_only.reshape(B, N, 1).float().contiguous()
+    t1 = threshold_tables(is_geom)[0].to(dev).contiguous()
+    out = torch.empty(B, dtype=torch.int32, device=dev)
+    lib = _native.load_library()
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream().cuda_stream
+        _native.check(lib.dl_molecule_connected(B, N, t1.shape[0], xs.data_ptr(), xs.shape[2], nm.data_ptr(),
+                                                None if po is None else po.data_ptr(), 1, int(po is not None),
+                                                t1.data_ptr(), out.data_ptr(), st), "dl_molecule_connected")
+    return out != 0
+
+
 def build_xae_molecule(positions, atom_types, is_geom, margins=MARGINS_EDM):
     """Reference signature (molecule_builder.py:44): one molecule, positions (n,3) already masked, atom_types (n,).
     Returns (X, A, E) with A bool, E int32, lower-triangular ("the graph should be DIRECTED")."""

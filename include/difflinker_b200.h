@@ -20,6 +20,8 @@
  *   either, one seed per molecule (no reference API)     dl_sample_chain_seeded
  *   either, resampling only the molecules that diverged  dl_sample_chain_seeded_retry, dl_retry_seed, dl_last_retry_ms
  *     (the reference's callers resample the whole batch, generate.py:153-161)
+ *   either, also resampling the disconnected molecules  dl_sample_chain_seeded_retry_connected, dl_molecule_connected
+ *     (is_connected, src/metrics.py:20-27, on the molecules of src/lightning.py:364-377)
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   build_xae_molecule           src/molecule_builder.py:44-102       dl_bond_orders
  *   frame restore + .xyz text    generate.py:163-171, src/visualizer.py:14-31   dl_restore_frame, dl_format_xyz
@@ -243,7 +245,50 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
                                        const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
                                        int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
                                        void* stream);
-/* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_seeded_retry, each from its row gather
+/*
+ * dl_sample_chain_seeded_retry that also resamples the molecules whose final molecule is in more than one piece -- the
+ * reference's `is_connected` (src/metrics.py:20-27) on what src/lightning.py:364-377 builds from chain[0]:
+ *   atoms     molecule b's rows with node_mask != 0; on cut-off (pocket) graphs, graph_type != DL_GRAPH_FC, minus the pocket
+ *             atoms, the rows whose last context column (pocket_only, src/egnn.py:486-487) is non-zero (lightning.py:372-374).
+ *             Inpainting models are checked over all their atoms.
+ *   bonds     atoms i and j bond iff get_bond_order(...) > 0 (src/molecule_builder.py:77-102): with the types t = argmax of
+ *             the first n_types columns of h (the first maximum), 100 |x_i - x_j| < thr1[min t][max t] and that entry
+ *             >= 0 -- the arithmetic of dl_bond_orders, whose E != 0 is exactly this relation.
+ *   connected the graph of those atoms and bonds has exactly one component (one atom is connected; no atom is not), i.e.
+ *             len(Chem.GetMolFrags(mol)) == 1 for build_molecule's molecule. The AtomValenceException branch of
+ *             is_connected, which needs RDKit's valence model, is not reproduced; the reference applies is_connected to
+ *             sanitized molecules only (metrics.py:103-104), and for those the two agree.
+ * The check runs on the device after the seeded loop and after each round. A row fails if its NaN flag is set or it is not
+ * connected; rounds gather, resample and write back failing rows as dl_sample_chain_seeded_retry does, except that a
+ * resampled row does not replace a finite row with one that diverged. Rows that are only disconnected after the last round
+ * are valid samples: they are returned with connected[b] = 0 and do not make the call fail. DL_NAN_DETECTED means, as there,
+ * that some row still diverges. max_retries = 0 only reports connectivity.
+ *   n_types    columns of h that hold the atom type (the one-hot width without charges); 1 <= n_types <= in_node_nf
+ *   thr1       (n_types,n_types) fp32 DEVICE: single-bond thresholds in pm, [min type][max type], negative = no bond
+ *              (dl_bond_orders' thr1; molecule_builder.threshold_tables)
+ *   connected  (B) int32 DEVICE out: 1 if row b's returned molecule is connected, else 0
+ * N <= 8192.
+ */
+dl_status dl_sample_chain_seeded_retry_connected(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
+                                                 int32_t keep_frames, const float* xh, const int8_t* node_mask,
+                                                 const float* fragment_mask, const float* linker_mask,
+                                                 const int8_t* edge_mask, const float* context, const uint64_t* seeds,
+                                                 const dl_step_coef* coef, const float* norm, float* chain, int32_t* nan_flags,
+                                                 int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
+                                                 int32_t n_types, const float* thr1, int32_t* connected, void* stream);
+/*
+ * The connectivity check of dl_sample_chain_seeded_retry_connected alone, on any (B,N) batch: connected[b] = 1 iff the
+ * atoms of molecule b form one component under the bond relation above. DEVICE buffers, enqueued on `stream`.
+ *   xh          (B,N,>=3+n_types) fp32, row stride xh_row_stride: x at columns 0..2, the atom-type one-hot from column 3
+ *   node_mask   (B,N) int8
+ *   context     (B,N,context_nf) fp32; with drop_pocket != 0 the rows whose column context_nf - 1 is non-zero are not atoms
+ *               (read only then; may be NULL otherwise)
+ *   thr1, n_types, connected as above. 1 <= N <= 8192.
+ */
+dl_status dl_molecule_connected(int32_t B, int32_t N, int32_t n_types, const float* xh, int32_t xh_row_stride,
+                                const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
+                                const float* thr1, int32_t* connected, void* stream);
+/* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_seeded_retry(_connected), each from its row gather
  * to its row scatter -- including the wait for the host to capture the sub-batch's step graph -- summed over the rounds; 0
  * when no round ran. */
 float dl_last_retry_ms(dl_engine* e);

@@ -53,3 +53,15 @@ print("bonds", int((E != 0).sum()))
 x = output.restore_frame(torch.cat([sd['positions'], sd['one_hot']], dim=2).contiguous(), sd['positions'], sd['fragment_mask'],
                          sd['atom_mask'])
 print("restore", bool(torch.isfinite(x).all()))
+
+# connectivity check, alone and in the recovery rounds (FC and cut-off graphs)
+xh = torch.cat([sd['positions'], sd['one_hot']], dim=2).contiguous()
+print("connected", molecule_builder.connected(xh, sd['atom_mask'], False).tolist())
+chain, nm = ddpm.sample_chain(data, keep_frames=1, seeds=[1, 2, 3], nan_retries=2, require_connected=True)
+print("connected rounds", ddpm.edm.last_connected.tolist(), ddpm.edm.last_attempts.tolist())
+ddpm3, _ = helpers.build_ddpm(spec3, 0, edge_impl=IMPL)
+ddpm3 = ddpm3.to(d)
+ddpm3.edm.T = 2
+chain, nm = ddpm3.sample_chain({k: mv(v) for k, v in b3.items()}, keep_frames=1, seeds=[1, 2], nan_retries=1,
+                               require_connected=True)
+print("pocket connected rounds", ddpm3.edm.last_connected.tolist(), ddpm3.edm.last_attempts.tolist())
