@@ -20,15 +20,15 @@ The reference is the in-repo oracle run in float64 (on the GPU: it is not code u
 takes minutes). Each live row i of molecule b is checked on its own, separately on the coordinate columns and the feature
 columns: err_i = max|got - ref64| must satisfy err_i <= max(C_DRIFT * drift_i, TAU * S_b), where drift_i = max|ref32 - ref64|
 is the same oracle's own float32 error on that row (how well conditioned the row is) and S_b the largest |ref64| over the
-molecule's live rows. One layer with one GCL keeps a wrong aggregate in row i from reaching any other row, so a failure
-names the row, and through the molecule's size and linker count, the tile shape. Padded rows, and the coordinate rows
-outside the linker mask, must be exactly 0.
+molecule's live rows (fp64_rows.check_rows). One layer with one GCL keeps a wrong aggregate in row i from reaching any
+other row, so a failure names the row, and through the molecule's size and linker count, the tile shape. Padded rows, and
+the coordinate rows outside the linker mask, must be exactly 0.
 
-Out of scope: the fp16 range-rescale paths of the tensor-core kernels and batch-mate effects of tile-level scaling. Every
-input here keeps its operand scale factors at 1.
+Every input here keeps the tensor-core kernels' operand scale factors at 1. The fp16 range-rescale paths (the node
+kernel's per-tile scales and the edge kernel's per-edge scale and descale) are driven on purpose, and checked with the same
+per-row rule, in test_range_rescale_fp64.py. Batch-mate effects of tile-level scaling are out of scope for both files.
 """
 import collections
-import contextlib
 import ctypes as C
 import functools
 import itertools
@@ -36,24 +36,19 @@ import itertools
 import pytest
 import torch
 
-from difflinker_b200 import Dynamics, DynamicsWithPockets, synthetic
+from difflinker_b200 import synthetic
 from difflinker_b200.batching import collate
-import egnn_options_oracle as eo
+from fp64_rows import (build_model, check_rows, dev, make_case, node_tail_shape, node_tile, oracle_forward, pocket_item,
+                       run_dyn)
 from oracle import difflinker_oracle as orc
 
-# Measured on an H100 80GB HBM3 (400 W): where a row's error exceeds TAU * S_b it is at most 15.5 times the oracle's own fp32
-# error on that row (FC, 128 columns, tanh + mean + sin_embedding; 11.1 on the cut-off boundary batch, <= 9 elsewhere). Those
-# rows are coordinate rows far from the origin, where both fp32 runs round x + agg alike, and rows with the ill-conditioned
-# sinusoidal embedding.
-TAU = 1e-5          # floor of the per-row bound, relative to the molecule's scale
-C_DRIFT = 30.0      # multiple of the oracle's own fp32-vs-fp64 error on the row
 IMPLS = ["simt", "auto"]
 OPTIONS = list(itertools.product((False, True), repeat=3))      # (tanh, mean, sin_embedding)
 F_FC, F_PK = 8, 9
 FC_SIZES = (1, 2, 3, 4, 5, 16, 17, 31, 32, 33, 42, 43, 63, 64, 65, 127, 128, 129, 255, 256, 257)
 FC_SIZES_128 = (128, 127, 65, 64, 33, 2, 1)
 
-WORST = {}          # test label -> (worst err / bound, C needed beside TAU, worst err / S_b)
+WORST = {}          # test label -> (worst err / bound, C needed beside TAU, worst err / S_b, fraction within TAU)
 
 
 def opt_id(o):
@@ -61,30 +56,6 @@ def opt_id(o):
 
 
 # ------------------------------------------------------------------------------------------------------------ batches
-def _latent(batch, F, seed):
-    """z: the batch's positions, one_hot / 4 on context rows and N(0, 1) features on linker rows, garbage on padded rows."""
-    g = torch.Generator().manual_seed(seed)
-    B, N = batch['positions'].shape[:2]
-    live = batch['atom_mask'].reshape(B, N, 1) != 0
-    lk = batch['linker_mask'].reshape(B, N, 1) != 0
-    h = torch.where(lk, torch.randn((B, N, F), generator=g), batch['one_hot'].float() / 4)
-    z = torch.cat([batch['positions'].float(), h], dim=2)
-    z = torch.where(live, z, 3.0 * torch.randn(z.shape, generator=g))
-    t = torch.rand((B, 1), generator=g)
-    return z, t
-
-
-def _case(batch, F, graph_type, seed, **extra):
-    z, t = _latent(batch, F, seed)
-    if graph_type == 'FC':
-        ctx = batch['fragment_mask'].float()
-    else:
-        fo = batch['fragment_only_mask'].float()
-        ctx = torch.cat([fo, batch['fragment_mask'].float() - fo], dim=-1)
-    return dict(t=t, z=z, atom_mask=batch['atom_mask'], linker_mask=batch['linker_mask'].float(),
-                edge_mask=batch['edge_mask'], context=ctx, graph_type=graph_type, F=F, **extra)
-
-
 def _fc_batch(sizes, seed):
     g = torch.Generator().manual_seed(seed)
     items = []
@@ -102,7 +73,7 @@ def _fc_batch(sizes, seed):
 @functools.lru_cache(maxsize=None)
 def fc_case(name):
     sizes, seed = {"ragged257": (FC_SIZES, 31), "full128": (FC_SIZES_128, 32)}[name]
-    return _case(_fc_batch(sizes, seed), F_FC, 'FC', seed)
+    return make_case(_fc_batch(sizes, seed), F_FC, 'FC', seed)
 
 
 def _centres(k):
@@ -118,16 +89,6 @@ def _ball(g, m, centre, radius=1.4):
     v = v / v.norm(dim=1, keepdim=True)
     r = radius * 0.999 * torch.rand((m, 1), generator=g, dtype=torch.float64) ** (1 / 3)
     return centre + v * r
-
-
-def _pocket_item(g, pos, role):
-    """role per atom: 'f' fragment-only, 'p' pocket, 'l' linker."""
-    n = pos.shape[0]
-    mask = lambda c: torch.tensor([1.0 if r == c else 0.0 for r in role])
-    fo, pk, lm = mask('f'), mask('p'), mask('l')
-    types = torch.randint(0, F_PK, (n,), generator=g)
-    return {'positions': pos.float(), 'one_hot': torch.nn.functional.one_hot(types, F_PK).float(),
-            'fragment_mask': fo + pk, 'linker_mask': lm, 'fragment_only_mask': fo, 'pocket_mask': pk}
 
 
 # '4A' clusters per molecule: (atoms, linker atoms among them). A cluster of m atoms gives m rows of degree m - 1.
@@ -178,8 +139,8 @@ def cutoff_case(graph_type):
     else:
         off = 0.0 if graph_type == 'FC-4A' else 6.0                # FC-10A-4A: cross distances 3.2 .. 8.8 A
         mols = [_ligand_pocket_molecule(g, 150, 8, off, False), _ligand_pocket_molecule(g, 100, 3, off, True)]
-    batch = collate([_pocket_item(g, pos, role) for pos, role, _ in mols])
-    return _case(batch, F_PK, graph_type, 43, degrees=[deg for _, _, deg in mols])
+    batch = collate([pocket_item(g, pos, role, F_PK) for pos, role, _ in mols])
+    return make_case(batch, F_PK, graph_type, 43, degrees=[deg for _, _, deg in mols])
 
 
 # Exact cut-off boundaries: integer coordinates, so every squared distance is an exact integer in fp32 and fp64.
@@ -208,9 +169,9 @@ def boundary_case(graph_type):
     pos = torch.tensor([p for p, _ in BOUNDARY_ATOMS], dtype=torch.float64)
     role = [r for _, r in BOUNDARY_ATOMS]
     # a second, padded molecule: the same atoms without the far pocket pairs, shifted by an integer vector
-    batch = collate([_pocket_item(g, pos, role), _pocket_item(g, pos[:6] + torch.tensor([3.0, -2.0, 5.0], dtype=torch.float64),
-                                                               role[:6])])
-    return _case(batch, F_PK, graph_type, 53)
+    batch = collate([pocket_item(g, pos, role, F_PK), pocket_item(g, pos[:6] + torch.tensor([3.0, -2.0, 5.0], dtype=torch.float64),
+                                                              role[:6], F_PK)])
+    return make_case(batch, F_PK, graph_type, 53)
 
 
 def oracle_edges(case):
@@ -224,43 +185,6 @@ def oracle_edges(case):
 
 
 # -------------------------------------------------------------------------------------------------- models and oracle
-def build_model(graph_type, F, opts, impl, seed, n_layers=1, inv_sublayers=1):
-    """A Dynamics of the given depth (dl_helpers.build_dynamics fixes inv_sublayers from the spec) and its oracle config."""
-    tanh, mean, sin = opts
-    ctx_nf = 1 if graph_type == 'FC' else 2
-    kw = dict(n_layers=n_layers, inv_sublayers=inv_sublayers, norm_constant=1e-6, normalization_factor=100,
-              graph_type=graph_type)
-    torch.manual_seed(seed)
-    cls = Dynamics if graph_type == 'FC' else DynamicsWithPockets
-    dyn = cls(in_node_nf=F, n_dims=3, context_node_nf=ctx_nf, hidden_nf=128, edge_impl=impl, **kw,
-              **eo.options_kw(tanh, mean, sin))
-    synthetic.init_reference_like_weights(dyn)
-    cfg = eo.OptionsConfig(in_node_nf=F, context_node_nf=ctx_nf, aggregation_method='mean' if mean else 'sum',
-                           tanh=tanh, sin_embedding=sin, **kw)
-    return dyn, cfg
-
-
-@contextlib.contextmanager
-def _full_fp32_matmul():
-    old = torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    try:
-        yield
-    finally:
-        torch.backends.cuda.matmul.allow_tf32 = old
-
-
-def oracle_forward(sd, cfg, case, dtype, device):
-    """The option-aware oracle's Dynamics.forward in `dtype` on `device` (factory calls inside it follow the device)."""
-    def cast(v):
-        return v.to(device=device, dtype=dtype) if v.is_floating_point() else v.to(device)
-    with torch.no_grad(), torch.device(device), _full_fp32_matmul():
-        out = eo.dynamics_forward({k: cast(v) for k, v in sd.items()}, cfg, cast(case['t']), cast(case['z']),
-                                  cast(case['atom_mask']), cast(case['linker_mask']), cast(case['edge_mask']),
-                                  cast(case['context']))
-    return out.double().cpu()
-
-
 _REFS = {}
 
 
@@ -272,57 +196,13 @@ def references(key, dyn, cfg, case):
     return _REFS[key]
 
 
-def dev():
-    assert torch.cuda.is_available()
-    return torch.device("cuda", 0)
-
-
-def run_dyn(dyn, case):
-    d = dev()
-    with torch.no_grad():
-        return dyn(case['t'].to(d), case['z'].to(d), case['atom_mask'].to(d), case['linker_mask'].to(d),
-                   case['edge_mask'].to(d), case['context'].to(d)).double().cpu()
-
-
-# ------------------------------------------------------------------------------------------------- per-row criterion
-def check_rows(label, got, ref64, ref32, case):
-    """err_i <= max(C_DRIFT * drift_i, TAU * S_b) for every live row, on the coordinate and on the feature columns;
-    padded rows and coordinate rows outside the linker mask exactly 0."""
-    B, N = got.shape[:2]
-    live = case['atom_mask'].reshape(B, N) != 0
-    lk = (case['linker_mask'].reshape(B, N) != 0) & live
-    assert torch.equal(got[~live], torch.zeros_like(got[~live])), f"{label}: a padded row is not exactly 0"
-    still = got[..., :3][live & ~lk]
-    assert torch.equal(still, torch.zeros_like(still)), f"{label}: a coordinate row outside the linker mask is not exactly 0"
-    sizes, links = live.sum(1), lk.sum(1)
-    worst, need_c, rel = 0.0, 0.0, 0.0
-    fails = []
-    for part, cols in (("vel", slice(0, 3)), ("h", slice(3, None))):
-        err = (got[..., cols] - ref64[..., cols]).abs().amax(-1)
-        drift = (ref32[..., cols] - ref64[..., cols]).abs().amax(-1)
-        scale = torch.where(live, ref64[..., cols].abs().amax(-1), 0.0).amax(1, keepdim=True).expand(B, N)
-        bound = torch.maximum(C_DRIFT * drift, TAU * scale)
-        ratio = torch.where(err == 0, 0.0, err / bound)
-        ratio = torch.where(live, ratio, 0.0)
-        worst = max(worst, ratio.max().item())
-        over_tau = live & (err > TAU * scale)
-        if over_tau.any():
-            need_c = max(need_c, (err[over_tau] / drift[over_tau]).max().item())
-        rel = max(rel, torch.where(live & (scale > 0), err / scale, 0.0).max().item())
-        for b, i in torch.nonzero(ratio > 1).tolist()[:5]:
-            fails.append(f"{part} row {i} of molecule {b} ({int(sizes[b])} live, {int(links[b])} linker): err "
-                         f"{err[b, i].item():.3e}, drift {drift[b, i].item():.3e}, S_b {scale[b, i].item():.3e}")
-    WORST[label] = (worst, need_c, rel)
-    assert not fails, f"{label}:\n" + "\n".join(fails)
-
-
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
     if WORST:
-        print("\nworst per-row ratios (err / bound, C needed beside TAU, err / S_b):")
-        for k, (w, c, r) in WORST.items():
-            print(f"  {k:48s} {w:9.3e} {c:9.3e} {r:9.3e}")
+        print("\nworst per-row ratios (err / bound, C needed beside TAU, err / S_b, fraction of rows within TAU * S_b):")
+        for k, (w, c, r, f) in WORST.items():
+            print(f"  {k:48s} {w:9.3e} {c:9.3e} {r:9.3e} {f:6.3f}")
 
 
 # ---------------------------------------------------------------------------------------------------------------- CPU
@@ -429,7 +309,7 @@ def test_fc_tiles_match_fp64_per_row(batch, opts, impl):
     case = fc_case(batch)
     dyn, cfg = build_model('FC', F_FC, opts, impl, 71)
     ref64, ref32 = references(("fc", batch, opts), dyn, cfg, case)
-    check_rows(f"fc {batch} {opt_id(opts)} {impl}", run_dyn(dyn, case), ref64, ref32, case)
+    check_rows(f"fc {batch} {opt_id(opts)} {impl}", run_dyn(dyn, case), ref64, ref32, case, WORST)
 
 
 @pytest.mark.gpu
@@ -442,7 +322,7 @@ def test_cutoff_tiles_match_fp64_per_row(graph_type, opts, impl):
     case = cutoff_case(graph_type)
     dyn, cfg = build_model(graph_type, F_PK, opts, impl, 72)
     ref64, ref32 = references(("cut", graph_type, opts), dyn, cfg, case)
-    check_rows(f"cut {graph_type} {opt_id(opts)} {impl}", run_dyn(dyn, case), ref64, ref32, case)
+    check_rows(f"cut {graph_type} {opt_id(opts)} {impl}", run_dyn(dyn, case), ref64, ref32, case, WORST)
     if impl == "auto":
         from difflinker_b200 import _native
         stats = (C.c_int64 * 4)()
@@ -464,7 +344,7 @@ def test_boundary_edges_match_fp64_per_row(graph_type, opts, impl):
     case = boundary_case(graph_type)
     dyn, cfg = build_model(graph_type, F_PK, opts, impl, 73)
     ref64, ref32 = references(("edge", graph_type, opts), dyn, cfg, case)
-    check_rows(f"boundary {graph_type} {opt_id(opts)} {impl}", run_dyn(dyn, case), ref64, ref32, case)
+    check_rows(f"boundary {graph_type} {opt_id(opts)} {impl}", run_dyn(dyn, case), ref64, ref32, case, WORST)
     if impl == "auto":
         from difflinker_b200 import _native
         stats = (C.c_int64 * 4)()
@@ -489,25 +369,6 @@ def test_size_gnn_boundary_edges_match_the_oracle():
     assert (got - want).abs().max().item() <= 1e-5 * want.abs().max().item()
 
 
-def node_tile(n, num_sms):
-    """The node kernel's tile size for n = B * N nodes (kernels_node_tc.cuh pick_tile_nodes)."""
-    per = -(-n // max(num_sms, 1))
-    return min(128, max(8, (per + 7) & ~7))
-
-
-def node_tail_shape(kind, num_sms):
-    """(B, N) with B * N nodes giving the requested node-kernel tiling: the tile size and the last tile's node count."""
-    tile, tail = {"tile8_tail1": (8, 1), "tile8_exact": (8, 0), "tile64_tail1": (64, 1), "tile128_tail1": (128, 1)}[kind]
-    lo = 1 if tile == 8 else (tile - 8) * num_sms + 1
-    for n in range(max(lo, 16), 64 * 1024):
-        if node_tile(n, num_sms) != tile or n % tile != tail:
-            continue
-        for N in range(64, 11, -1):
-            if n % N == 0 and n // N >= 2:
-                return n // N, N
-    raise AssertionError(f"no (B, N) for {kind} on {num_sms} SMs")
-
-
 def test_node_tail_shapes_give_the_requested_tiles():
     for sms in (132, 114, 78):
         for kind in ("tile8_tail1", "tile8_exact", "tile64_tail1", "tile128_tail1"):
@@ -525,7 +386,7 @@ def test_node_tile_tails_match_fp64_per_row(kind):
     B, N = node_tail_shape(kind, torch.cuda.get_device_properties(0).multi_processor_count)
     spec = synthetic.WorkloadSpec(f"tail_{kind}", B=B, N=N, n_min=max(3, N // 2), l_min=1, l_max=8, F=F_FC, L=2, T=10,
                                   seed=81)
-    case = _case(collate(synthetic.make_items(spec)), F_FC, 'FC', 82)
+    case = make_case(collate(synthetic.make_items(spec)), F_FC, 'FC', 82)
     dyn, cfg = build_model('FC', F_FC, (False, False, False), "auto", 74, n_layers=2, inv_sublayers=2)
     ref64, ref32 = references(("node", kind), dyn, cfg, case)
-    check_rows(f"node {kind} B={B} N={N}", run_dyn(dyn, case), ref64, ref32, case)
+    check_rows(f"node {kind} B={B} N={N}", run_dyn(dyn, case), ref64, ref32, case, WORST)
