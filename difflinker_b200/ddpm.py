@@ -1,5 +1,6 @@
 """Outer drop-in boundary: `DDPM.sample_chain(data, sample_fn=None, keep_frames=None) -> (chain, node_mask)`
-(reference: src/lightning.py:405-463; constructor wiring src/lightning.py:39-113).
+(reference: src/lightning.py:405-463; constructor wiring src/lightning.py:39-113), and `DDPM.sample_many(datas, ...)`,
+which samples many such batches in shared launches.
 
 Two ways in:
   * `DDPM(**hparams)` -- a plain nn.Module with the reference's hyper-parameter names and state_dict layout
@@ -14,7 +15,7 @@ import torch.nn as nn
 
 from . import utils
 from .batching import create_templates_for_linker_generation
-from .edm import EDM, InpaintingEDM
+from .edm import EDM, InpaintingEDM, draw_seeds
 from .egnn import Dynamics, DynamicsWithPockets
 
 
@@ -101,6 +102,32 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     return chain, kw['node_mask']
 
 
+def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
+                max_molecules=256):
+    """The body of sample_chain for many batches `datas` at once, sampled in shared launches by EDM.sample_many: returns
+    [(chain_k, node_mask_k)] in the order of `datas`, each equal to what sample_chain(model, datas[k], ...) returns (with
+    seeds[k]) in the sense of EDM.sample_many. `model` as for sample_chain, so accelerated reference modules take it too.
+    `sample_fn`, and with noise_mode='per_molecule' and no `seeds` draw_seeds, are called once per batch, in the order the
+    sequential sample_chain calls call them: linker sizes, seeds and the generator's final state are theirs."""
+    edm = model.edm
+    derive = seeds is None and edm.noise_mode == 'per_molecule'
+    requests, drawn = [], []
+    for data in datas:
+        kw = sampler_inputs(model, data, sample_fn)
+        requests.append(kw)
+        x = kw['x']
+        if derive and x.is_cuda:                # a host batch is refused by EDM.sample_many
+            with torch.cuda.device(x.device):
+                drawn.append(draw_seeds(x.shape[0], x.device))
+    if derive and len(drawn) == len(requests):
+        seeds = drawn
+    extra = {} if nan_retries is None else {'nan_retries': nan_retries}
+    if require_connected is not None:
+        extra['require_connected'] = require_connected
+    chains = edm.sample_many(requests, keep_frames=keep_frames, seeds=seeds, max_molecules=max_molecules, **extra)
+    return [(chain, kw['node_mask']) for chain, kw in zip(chains, requests)]
+
+
 class DDPM(nn.Module):
     """Hyper-parameter-compatible stand-in for the Lightning module (sampling API only)."""
     train_dataset = None
@@ -139,6 +166,11 @@ class DDPM(nn.Module):
     def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                             require_connected=require_connected)
+
+    def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
+                    max_molecules=256):
+        return sample_many(self, datas, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
+                           require_connected=require_connected, max_molecules=max_molecules)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

@@ -1,7 +1,8 @@
 """Replica-level data parallelism (SURVEY.md section 8(e)): molecules never interact across a batch, so sampling shards
 with no data-path collective. The only exchange is one broadcast of the weights at start-up (NCCL on GPUs,
 gloo in the CPU tests); optionally the final results are gathered. `resolve_devices`, `device_slices` and `place_rows` plan and
-gather the split of one batch over several local GPUs that `EDM.devices` makes from a single process."""
+gather the split of one batch over several local GPUs that `EDM.devices` makes from a single process; `plan_launches`,
+`deal_launches`, `pack_requests` and `unpack_rows` plan, assemble and take apart the shared launches of `EDM.sample_many`."""
 import operator
 
 import torch
@@ -59,6 +60,84 @@ def place_rows(out: torch.Tensor, parts, slices, dim: int = 0):
     Per-molecule NaN flags placed this way carry batch-global molecule indices."""
     for part, (_, _, lo, hi) in zip(parts, slices):
         out.narrow(dim, lo, hi - lo).copy_(part)
+    return out
+
+
+def plan_launches(sizes, nodes, max_molecules: int, keys=None):
+    """How `EDM.sample_many` packs requests into launches: [(request indices, N)], every request in exactly one launch and
+    never split, N the largest N_k of the launch (the others are padded to it). Requests share a launch only with requests of
+    the same key (`keys`: one hashable per request, None for all the same), so each group is planned on its own, groups in
+    the order of their first request. Within a group the requests are sorted by (N_k, index), which keeps the padding small,
+    and filled in that order into launches of at most `max_molecules` molecules; a request larger than that gets a launch
+    of its own. Deterministic: the same inputs give the same plan."""
+    if len(sizes) != len(nodes) or (keys is not None and len(keys) != len(sizes)):
+        raise ValueError("sizes, nodes and keys need one entry per request")
+    if max_molecules < 1:
+        raise ValueError(f"max_molecules must be >= 1 (got {max_molecules})")
+    groups = {}
+    for k in range(len(sizes)):
+        groups.setdefault(None if keys is None else keys[k], []).append(k)
+    launches = []
+    for members in groups.values():
+        current, total = [], 0
+        for k in sorted(members, key=lambda k: (nodes[k], k)):
+            if current and total + sizes[k] > max_molecules:
+                launches.append(current)
+                current, total = [], 0
+            current.append(k)
+            total += sizes[k]
+        launches.append(current)
+    return [(ks, max(nodes[k] for k in ks)) for ks in launches]
+
+
+def deal_launches(costs, n_slots: int):
+    """The slot (index into the listed devices) of every launch: the costliest launch first, each to the slot with the least
+    cost so far, the lowest slot on a tie. Each slot then runs its launches in launch order."""
+    load, out = [0] * n_slots, [None] * len(costs)
+    for i in sorted(range(len(costs)), key=lambda i: (-costs[i], i)):
+        s = min(range(n_slots), key=lambda s: (load[s], s))
+        out[i] = s
+        load[s] += costs[i]
+    return out
+
+
+def pack_requests(requests, n_nodes: int, fc: bool):
+    """One launch's inputs from several requests' keyword arguments of `EDM.sample_chain`: each request's tensors padded with
+    dead atoms (zeros) to `n_nodes`, then concatenated along B in request order. On FC graphs (`fc`) the flattened edge mask
+    becomes each molecule's (N, N) block padded with 0 and is returned as (B N N, 1), the datasets.collate layout; on
+    cut-off graphs the per-node batch ids are rebuilt for the launch (the engine does not read them)."""
+    out = {}
+    for name in requests[0]:
+        vals = [r[name] for r in requests]
+        if all(v is None for v in vals):
+            out[name] = None
+        elif any(v is None for v in vals):
+            raise ValueError(f"some requests give {name} and others do not")
+        elif name != 'edge_mask':
+            out[name] = torch.cat([torch.cat([v, v.new_zeros((v.shape[0], n_nodes - v.shape[1]) + tuple(v.shape[2:]))], dim=1)
+                                   for v in vals])
+        elif fc:
+            blocks = []
+            for v, r in zip(vals, requests):
+                B, N = r['x'].shape[:2]
+                blocks.append(torch.nn.functional.pad(v.reshape(B, N, N), (0, n_nodes - N, 0, n_nodes - N)))
+            out[name] = torch.cat(blocks).reshape(-1, 1)
+        else:
+            B = sum(r['x'].shape[0] for r in requests)
+            out[name] = torch.arange(B, device=vals[0].device).repeat_interleave(n_nodes).to(vals[0].dtype)
+    return out
+
+
+def unpack_rows(t: torch.Tensor, sizes, nodes, dim: int = 0):
+    """The inverse of pack_requests for a launch's result `t`: request k's rows (along `dim`, in request order) and, when
+    `nodes` is given, its first N_k atoms (the dimension after `dim`), each as a contiguous tensor."""
+    out, lo = [], 0
+    for k, b in enumerate(sizes):
+        part = t.narrow(dim, lo, b)
+        if nodes is not None:
+            part = part.narrow(dim + 1, 0, nodes[k])
+        out.append(part.contiguous())
+        lo += b
     return out
 
 

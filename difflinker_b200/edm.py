@@ -15,7 +15,8 @@ import torch
 import torch.nn.functional as F
 
 from . import _native
-from .distributed import device_slices, place_rows, resolve_devices, slice_sampler_inputs
+from .distributed import (deal_launches, device_slices, pack_requests, place_rows, plan_launches, resolve_devices,
+                          slice_sampler_inputs, unpack_rows)
 from .noise import PredefinedNoiseSchedule
 from .utils import FoundNaNException, nan_exception_class
 
@@ -175,6 +176,9 @@ class EDM(torch.nn.Module):
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
+        # sample_many: per request, what last_seeds / last_attempts / last_connected hold after its own sample_chain call;
+        # per launch, (device, the requests it held, loop ms)
+        self.last_seeds_many = self.last_attempts_many = self.last_connected_many = self.last_loop_ms_many = None
 
     @property
     def devices(self):
@@ -238,11 +242,13 @@ class EDM(torch.nn.Module):
         """(T+1) rows of dl_step_coef: row r is reverse step s = T-1-r (edm.py:146-163, 178-208); row T is the
         final p(x,h|z_0) step (edm.py:210-235).  Evaluated on (n_samples,1) fp32 CPU tensors exactly as the
         reference does: torch's CPU transcendental kernels round differently for different tensor sizes, so this
-        is what makes the scalars bit-identical to the reference's for the same batch size. Cached."""
+        is what makes the scalars bit-identical to the reference's for the same batch size. Cached for the last few batch
+        sizes (sample_many needs one table per request size)."""
         T = self.T
         key = (T, keep_frames, n_samples, self.gamma.gamma._version, self.gamma.gamma.data_ptr())
-        if getattr(self, '_coef_cache', None) is not None and self._coef_cache[0] == key:
-            return self._coef_cache[1]
+        cache = self.__dict__.setdefault('_coef_cache', {})
+        if key in cache:
+            return cache[key]
         gamma = self._cpu_gamma()
         rows = (_native.DLStepCoef * (T + 1))()
         for r in range(T):
@@ -265,7 +271,9 @@ class EDM(torch.nn.Module):
         inv_alpha0 = 1. / self.alpha(g0)
         rows[T] = _native.DLStepCoef(0.0, float(inv_alpha0[0]), float(self.sigma(g0)[0]),
                                      float(self.SNR(-0.5 * g0)[0]), -1, self._final_qa(g0), 0.0, 0.0)
-        self._coef_cache = (key, rows)
+        if len(cache) >= 8:
+            cache.pop(next(iter(cache)))
+        cache[key] = rows
         return rows
 
     def draw_noise(self, n_draws, n_samples, n_nodes, device, generator=None):
@@ -465,9 +473,8 @@ class EDM(torch.nn.Module):
         else:
             assert keep_frames <= self.T
         lib = _native.load_library()
-        n_samples, n_nodes = x.size(0), x.size(1)
+        n_samples = x.size(0)
         dev = x.device
-        d = self.n_dims + self.in_node_nf
         self.last_attempts = None
         self.last_connected = None
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
@@ -495,7 +502,217 @@ class EDM(torch.nn.Module):
             seed, offset = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF, gen.get_offset()
             b0, b_full = (0, n_samples) if batch_slice is None else map(int, batch_slice)
         engines = self.dynamics.engines([(dev_i, replica) for dev_i, replica, _, _ in slices])
-        coef = self.step_coefficients(keep_frames, n_samples)
+        places = [torch.device('cuda', dev_i) for dev_i, *_ in slices] if split else [dev]
+        calls, finish = self._enqueue_batch(lib, full, keep_frames, self.step_coefficients(keep_frames, n_samples), slices,
+                                            engines, places, dev, noise=noise, dev_seeds=dev_seeds,
+                                            rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check)
+        by_device = {}
+        for dev_i, c in calls:
+            by_device.setdefault(dev_i, []).append(c)
+        try:
+            if len(slices) == 1:            # on the caller's thread
+                with torch.cuda.device(slices[0][0]):
+                    calls[0][1]()
+            else:
+                _run_per_device(by_device)
+        except BaseException:
+            for dev_i in by_device:         # let the loops that were enqueued finish before their inputs are released
+                try:
+                    torch.cuda.synchronize(dev_i)
+                except Exception:
+                    pass
+            raise
+        out = finish()
+        if on_device:
+            assert len(set(out['consumed'])) == 1, out['consumed']
+            gen.set_offset(offset + out['consumed'][0])
+        loop_ms = []
+        for (dev_i, _, lo, hi), eng in zip(slices, engines):
+            with torch.cuda.device(dev_i):
+                loop_ms.append((dev_i, lo, hi, float(lib.dl_last_elapsed_ms(eng))))
+        self.last_loop_ms = max(ms for *_, ms in loop_ms)
+        self.last_slice_loop_ms = loop_ms if split else None
+        if recover:
+            self.last_seeds, self.last_attempts = out['used'].cpu(), out['attempts'].cpu()
+        if check:
+            self.last_connected = out['connected'].cpu() != 0
+        if out['bad']:
+            exc = nan_exception_class()(flags=out['flags'].cpu().tolist())
+            if recover:
+                exc.chain = out['chain']    # the rows that did not fail, or were recovered, are good molecules
+            raise exc
+        return out['chain']
+
+    # the keyword arguments of sample_chain that make up one request of sample_many
+    _REQUEST_INPUTS = ('x', 'h', 'node_mask', 'fragment_mask', 'linker_mask', 'edge_mask', 'context')
+
+    @torch.no_grad()
+    def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
+                    max_molecules=256):
+        """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
+        edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
+        (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
+        sample_chain(**requests[k], keep_frames=keep_frames, seeds=seeds[k], nan_retries=..., require_connected=...): always
+        on the SIMT edge path, and on the tensor-core path while no node tile rescales its fp16 operands (DESIGN.md
+        section 6). It needs per-molecule streams: `seeds`, one list of B_k seeds per request, or noise_mode='per_molecule',
+        which draws them with one draw_seeds(B_k) per request in request order -- the results and the generator's final
+        offset are then those of the sequence of sample_chain calls.
+        Launches (distributed.plan_launches): whole requests, at most `max_molecules` molecules each unless one request is
+        larger, padded to the largest N_k in the launch. Requests share a launch only when sample_chain would give them the
+        same step coefficients (torch's CPU kernels round them differently for some batch sizes) and, with
+        aggregation_method='mean' on FC graphs, where the reference divides by the padded N, only with requests of the same
+        N. With `devices` set, whole launches are dealt to the listed devices by their cost (distributed.deal_launches), and
+        each device runs its launches in order, from a host thread of its own; a launch is never split.
+        `nan_retries` and `require_connected` run their rounds inside each launch, over its rows. Rows still diverging after
+        the last round raise once, after every launch: the FoundNaNException of the first such request, its index sets
+        local to that request, with `request` = k and `results` = every request's chain (and `chain` = its own when rounds
+        ran, as in sample_chain). `last_seeds_many`, `last_attempts_many` and `last_connected_many` hold per request what
+        last_seeds, last_attempts and last_connected would hold after its own call; `last_loop_ms_many` holds (device,
+        requests, loop ms) per launch. The single-call attributes are left as they were.
+        Raises ValueError for an empty list, the batch stream (its draws depend on B and N), noise= or a replaced draw
+        function, host inputs, requests on different devices or of different feature or context widths, and seeds that do
+        not match the requests."""
+        if keep_frames is None:
+            keep_frames = self.T
+        else:
+            assert keep_frames <= self.T
+        requests = list(requests)
+        if not requests:
+            raise ValueError("sample_many needs at least one request")
+        for k, r in enumerate(requests):
+            if 'noise' in r or 'batch_slice' in r:
+                raise ValueError(f"request {k} passes noise= or batch_slice=: sample_many samples per-molecule streams, "
+                                 "which need neither")
+            if set(r) != set(self._REQUEST_INPUTS):
+                raise ValueError(f"request {k} must hold exactly the inputs {self._REQUEST_INPUTS} (got {sorted(r)})")
+        if self._draws_replaced():
+            raise ValueError("sample_many needs the device-side per-molecule stream, but this model's draw function is replaced")
+        if seeds is None and self.noise_mode != 'per_molecule':
+            raise ValueError("sample_many needs per-molecule streams: pass seeds= or set noise_mode='per_molecule' (the batch "
+                             f"stream, noise_mode={self.noise_mode!r}, draws depending on B and N, so packing would change them)")
+        if seeds is not None and len(seeds) != len(requests):
+            raise ValueError(f"seeds holds {len(seeds)} lists for {len(requests)} requests")
+        x0 = requests[0]['x']
+        ctx_nf = self.dynamics.context_node_nf
+        for k, r in enumerate(requests):
+            x, h, ctx = r['x'], r['h'], r['context']
+            if x.device != x0.device:
+                raise ValueError(f"requests 0 and {k} are on different devices ({x0.device}, {x.device})")
+            if x.dim() != 3 or x.shape[0] < 1 or x.shape[2] != self.n_dims or h.shape[:2] != x.shape[:2]:
+                raise ValueError(f"request {k}: x must be (B, N, {self.n_dims}) with B >= 1 and h (B, N, F) "
+                                 f"(got {tuple(x.shape)} and {tuple(h.shape)})")
+            if h.shape[-1] != self.in_node_nf or h.shape[-1] != requests[0]['h'].shape[-1]:
+                raise ValueError(f"request {k} has {h.shape[-1]} atom features; the model and request 0 have "
+                                 f"{self.in_node_nf} and {requests[0]['h'].shape[-1]}")
+            if (ctx is None) != (requests[0]['context'] is None) or (ctx is not None and ctx.shape[-1] != ctx_nf):
+                raise ValueError(f"request {k}'s context is {None if ctx is None else ctx.shape[-1]} wide; the model takes "
+                                 f"{ctx_nf} columns and every request must give them")
+        sizes = [r['x'].shape[0] for r in requests]
+        nodes = [r['x'].shape[1] for r in requests]
+        if seeds is not None:
+            cpu_seeds = []
+            for k, (s, b) in enumerate(zip(seeds, sizes)):
+                try:
+                    cpu_seeds.append(seeds_tensor(s, b))
+                except ValueError as e:
+                    raise ValueError(f"request {k}: {e}") from None
+        dev = x0.device
+        if dev.type != 'cuda':
+            raise ValueError(f"sample_many needs CUDA inputs (got {dev})")
+        retries = self._nan_retries(nan_retries, seeds, None, None, x0)
+        check = self._require_connected(require_connected, seeds, None, None, x0)
+        recover = retries > 0 or check
+        self.dynamics._check_graph_type()
+        if seeds is None:
+            with torch.cuda.device(dev):    # one draw per request, in request order, as the sample_chain calls draw them
+                cpu_seeds = list(torch.cat([draw_seeds(b, dev) for b in sizes]).cpu().split(sizes))
+        coefs = {b: self.step_coefficients(keep_frames, b) for b in sorted(set(sizes))}
+        fc = self.dynamics.graph_type == 'FC'
+        same_n = fc and self.dynamics.aggregation_method == 'mean'
+        keys = [(bytes(coefs[b]), n if same_n else None) for b, n in zip(sizes, nodes)]
+        launches = plan_launches(sizes, nodes, max_molecules, keys)
+        if fc:                              # edges of the launch's padded molecules
+            costs = [sum(sizes[k] for k in ks) * n * n for ks, n in launches]
+        else:                               # live atoms, a proxy for the cut-off graph's edges
+            live = torch.stack([r['node_mask'].reshape(b, n).ne(0).sum() for r, b, n in zip(requests, sizes, nodes)]).tolist()
+            costs = [sum(live[k] for k in ks) for ks, _ in launches]
+        devices = [self.dynamics._device_index(x0)] if self.devices is None else self.devices
+        slots = [(d, replica) for d, replica, _, _ in device_slices(len(devices), devices)]
+        slot_of = deal_launches(costs, len(slots))
+        busy = sorted(set(slot_of))
+        engine_of = dict(zip(busy, self.dynamics.engines([slots[s] for s in busy])))
+        lib = _native.load_library()
+        finishes, by_device, loop_ms = [], {}, [None] * len(launches)
+
+        def timed(i, call, eng, dev_i, stream):
+            call()
+            stream.synchronize()            # the loop's events are read before the engine's next launch records them again
+            with torch.cuda.device(dev_i):
+                loop_ms[i] = float(lib.dl_last_elapsed_ms(eng))
+        for i, (ks, n) in enumerate(launches):
+            dev_i, replica = slots[slot_of[i]]
+            b = sum(sizes[k] for k in ks)
+            full = self._sampler_tensors(**pack_requests([requests[k] for k in ks], n, fc))
+            dev_seeds = torch.cat([cpu_seeds[k] for k in ks]).to(dev)
+            where = torch.device('cuda', dev_i)
+            eng = engine_of[slot_of[i]]
+            [(_, call)], finish = self._enqueue_batch(lib, full, keep_frames, coefs[sizes[ks[0]]], [(dev_i, replica, 0, b)], [eng],
+                                                      [where], dev, dev_seeds=dev_seeds, retries=retries, check=check)
+            finishes.append(finish)
+            by_device.setdefault(dev_i, []).append(
+                functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
+        try:
+            _run_per_device(by_device)
+        except BaseException:
+            for dev_i in by_device:         # let the loops that were enqueued finish before their inputs are released
+                try:
+                    torch.cuda.synchronize(dev_i)
+                except Exception:
+                    pass
+            raise
+        results, flags = [None] * len(requests), [None] * len(requests)
+        seeds_many, attempts_many, connected_many = list(cpu_seeds), [None] * len(requests), [None] * len(requests)
+        for (ks, _), finish in zip(launches, finishes):
+            out = finish()
+            rows = [sizes[k] for k in ks]
+            parts = {'chain': unpack_rows(out['chain'], rows, [nodes[k] for k in ks], dim=1),
+                     'flags': unpack_rows(out['flags'].cpu(), rows, None)}
+            if recover:
+                parts['used'] = unpack_rows(out['used'].cpu(), rows, None)
+                parts['attempts'] = unpack_rows(out['attempts'].cpu(), rows, None)
+            if check:
+                parts['connected'] = unpack_rows(out['connected'].cpu() != 0, rows, None)
+            for j, k in enumerate(ks):
+                results[k], flags[k] = parts['chain'][j], parts['flags'][j]
+                if recover:
+                    seeds_many[k], attempts_many[k] = parts['used'][j], parts['attempts'][j]
+                if check:
+                    connected_many[k] = parts['connected'][j]
+        self.last_seeds_many, self.last_attempts_many, self.last_connected_many = seeds_many, attempts_many, connected_many
+        self.last_loop_ms_many = [(slots[slot_of[i]][0], sorted(ks), loop_ms[i]) for i, (ks, _) in enumerate(launches)]
+        for k, f in enumerate(flags):
+            if f.any():
+                exc = nan_exception_class()(flags=f.tolist())
+                exc.request, exc.results = k, results
+                if recover:
+                    exc.chain = results[k]
+                raise exc
+        return results
+
+    def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
+                       retries=0, check=False):
+        """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
+        inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
+        replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
+        covers the batch where it is. The draws are the per-molecule `dev_seeds`, the batch stream `rng` = (seed, offset,
+        b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _require_connected.
+        Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
+        (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
+        back and returns dict(chain, flags, used, attempts, connected, bad, consumed) on `dev`. `bad` reads the flags: one
+        synchronisation, after every loop and copy."""
+        n_samples, n_nodes = full['x'].shape[:2]
+        d = self.n_dims + self.in_node_nf
+        recover = retries > 0 or check
         norm = self._norm()
         chain = torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32)
         flags = torch.zeros(n_samples, dtype=torch.int32, device=dev)
@@ -505,9 +722,8 @@ class EDM(torch.nn.Module):
         # connectivity: every row's flag, and the bond table on each slice's device
         connected = torch.empty(n_samples, dtype=torch.int32, device=dev) if check else None
         thr1 = self._bond_table() if check else None
-        places = [torch.device('cuda', dev_i) for dev_i, *_ in slices] if split else [dev]
         whole = places == [dev]             # one slice, the whole batch where it is: it samples the caller's tensors
-        results, calls, parts = [], {}, []  # (status, consumed) of every slice; each device's calls; every slice's tensors
+        results, calls, parts = [], [], []  # (status, consumed) of every slice; every slice's call; every slice's tensors
 
         def call(*args):
             results.append(_sample_slice(lib, *args))
@@ -528,54 +744,27 @@ class EDM(torch.nn.Module):
             parts.append(part)              # alive until the flags have been read below
             t, nz, sd, chain_i, flags_i, used_i, attempts_i, connected_i, thr1_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
-            calls.setdefault(dev_i, []).append(functools.partial(
+            rng_i = None if rng is None else (rng[0], rng[1], rng[2] + lo, rng[3])
+            calls.append((dev_i, functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
-                stream, nz, sd, (seed, offset, b0 + lo, b_full) if on_device else None,
-                (retries, used_i, attempts_i, (thr1_i, connected_i) if check else None) if recover else None))
-        try:
-            if len(slices) == 1:            # on the caller's thread
-                with torch.cuda.device(slices[0][0]):
-                    calls[slices[0][0]][0]()
-            else:
-                _run_per_device(calls)
-        except BaseException:
-            for dev_i in calls:             # let the loops that were enqueued finish before their inputs are released
-                try:
-                    torch.cuda.synchronize(dev_i)
-                except Exception:
-                    pass
-            raise
-        if on_device:
-            consumed = [used for _, used in results]
-            assert len(set(consumed)) == 1, consumed
-            gen.set_offset(offset + consumed[0])
-        if not whole:
-            place_rows(chain, [p[3] for p in parts], slices, dim=1)
-            place_rows(flags, [p[4] for p in parts], slices)
-            if recover:
-                place_rows(used, [p[5] for p in parts], slices)
-                place_rows(attempts, [p[6] for p in parts], slices)
-            if check:
-                place_rows(connected, [p[7] for p in parts], slices)
-        # the host sampler reports NaNs in its status; on the device, one sync per chain instead of one per step
-        # (egnn.py:441), after every slice's loop and copy
-        bad = _native.DL_NAN_DETECTED in [st for st, _ in results] or bool(flags.any().item())
-        loop_ms = []
-        for (dev_i, _, lo, hi), eng in zip(slices, engines):
-            with torch.cuda.device(dev_i):
-                loop_ms.append((dev_i, lo, hi, float(lib.dl_last_elapsed_ms(eng))))
-        self.last_loop_ms = max(ms for *_, ms in loop_ms)
-        self.last_slice_loop_ms = loop_ms if split else None
-        if recover:
-            self.last_seeds, self.last_attempts = used.cpu(), attempts.cpu()
-        if check:
-            self.last_connected = connected.cpu() != 0
-        if bad:
-            exc = nan_exception_class()(flags=flags.cpu().tolist())
-            if recover:
-                exc.chain = chain           # the rows that did not fail, or were recovered, are good molecules
-            raise exc
-        return chain
+                stream, nz, sd, rng_i,
+                (retries, used_i, attempts_i, (thr1_i, connected_i) if check else None) if recover else None)))
+
+        def finish():
+            if not whole:
+                place_rows(chain, [p[3] for p in parts], slices, dim=1)
+                place_rows(flags, [p[4] for p in parts], slices)
+                if recover:
+                    place_rows(used, [p[5] for p in parts], slices)
+                    place_rows(attempts, [p[6] for p in parts], slices)
+                if check:
+                    place_rows(connected, [p[7] for p in parts], slices)
+            # the host sampler reports NaNs in its status; on the device, one sync per chain instead of one per step
+            # (egnn.py:441), after every slice's loop and copy
+            bad = _native.DL_NAN_DETECTED in [st for st, _ in results] or bool(flags.any().item())
+            return dict(chain=chain, flags=flags, used=used, attempts=attempts, connected=connected, bad=bad,
+                        consumed=[c for _, c in results])
+        return calls, finish
 
 
 class InpaintingEDM(EDM):
