@@ -287,13 +287,89 @@ def masked_noise(noise_fn: NoiseFn, B: int, N: int, n_dims: int, F_: int, mask: 
     return torch.cat([zx, zh], dim=2)
 
 
+def step_scalars(gamma: Tensor, s: int, T: int, B: int, table_timesteps: int) -> Dict[str, Tensor]:
+    """The fp32 (B,1) scalars of reverse step s (edm.py:146-150, 196-205, 655-668), evaluated by the reference's ops in the
+    reference's order on (B,1) tensors: t, a = alpha_t|s, b = sigma2_t|s / alpha_t|s / sigma_t, c = sigma_t|s * sigma_s /
+    sigma_t and the q(z_s|z_t,x) pair qa = alpha_t|s sigma_s^2 / sigma_t^2, qb = alpha_s sigma2_t|s / sigma_t^2.
+    s = -1 is the final p(x,h|z_0) step (edm.py:210-242, 700-716): inv_alpha0 = 1/alpha_0, sigma0, snr0 = SNR(-0.5 g_0) and
+    qa0 = sigma_0 / alpha_0.  These are the rows of EDM.step_coefficients: row r is step s = T-1-r."""
+    if s < 0:
+        g0 = gamma_lookup(gamma, torch.zeros((B, 1)), table_timesteps)
+        return dict(inv_alpha0=1.0 / _alpha(g0), sigma0=_sigma(g0), snr0=torch.exp(-(-0.5 * g0)),   # edm.py:216,377-379
+                    qa0=_sigma(g0) / _alpha(g0))
+    s_arr = torch.full((B, 1), fill_value=s)
+    t_arr = (s_arr + 1) / T
+    s_arr = s_arr / T
+    g_s = gamma_lookup(gamma, s_arr, table_timesteps)
+    g_t = gamma_lookup(gamma, t_arr, table_timesteps)
+    sig2_ts, sig_ts, a_ts = _sigma_alpha_t_given_s(g_t, g_s)
+    sig_s, sig_t, al_s = _sigma(g_s), _sigma(g_t), _alpha(g_s)
+    return dict(t=t_arr, a=a_ts, b=sig2_ts / a_ts / sig_t, c=sig_ts * sig_s / sig_t,
+                qa=a_ts * (sig_s ** 2) / (sig_t ** 2), qb=al_s * sig2_ts / (sig_t ** 2))
+
+
+def _sc(scalars: Dict[str, Tensor], key: str, like: Tensor) -> Tensor:
+    """A (B,1) step scalar as a (B,1,1) tensor of `like`'s dtype and device (fp32 scalars promoted exactly)."""
+    return _bcast(scalars[key]).to(dtype=like.dtype, device=like.device)
+
+
+def linker_step(z, eps, scalars, draw, fm, lm):
+    """One reverse step of the linker sampler, sample_p_zs_given_zt_only_linker (edm.py:178-208), in z's dtype: `eps` is
+    the raw dynamics output and `draw` the step's standard-normal draw, both masked here by the linker mask."""
+    a, b, c = (_sc(scalars, k, z) for k in ("a", "b", "c"))
+    eps = eps * lm                                                        # edm.py:196
+    mu = z / a - b * eps                                                  # edm.py:199
+    z_s = mu + c * (draw * lm)                                            # edm.py:202-205, utils.py:189-192
+    return z * fm + z_s * lm                                              # edm.py:206
+
+
+def linker_final(z, eps, scalars, draw, fm, lm):
+    """sample_p_xh_given_z0_only_linker (edm.py:210-235) up to the unnormalisation: the final normalised (x,h)."""
+    inv_a0, sig0, snr0 = (_sc(scalars, k, z) for k in ("inv_alpha0", "sigma0", "snr0"))
+    eps = eps * lm
+    mu_x = inv_a0 * (z - sig0 * eps)                                      # edm.py:237-242
+    out = mu_x + snr0 * (draw * lm)                                       # edm.py:228
+    return z * fm + out * lm                                              # edm.py:229
+
+
+def inpaint_step(z, eps, scalars, draw_p, draw_q, xh, nm, fm, lm, n_dims=3):
+    """One reverse step of InpaintingEDM.sample_chain (edm.py:575-594) in z's dtype: p(z_s|z_t) on every atom from the
+    (centred) dynamics output `eps` and the prepared draw `draw_p`, q(z_s|z_t,x) on the fragment atoms from the normalised
+    data `xh` and `draw_q`, recombination and the centre-of-mass projection over the node mask. The draws are masked and
+    centre-of-mass free as com_free_noise makes them."""
+    a, b, c, qa, qb = (_sc(scalars, k, z) for k in ("a", "b", "c", "qa", "qb"))
+    mu = z / a - b * eps                                                  # edm.py:634-642
+    z_lin = mu + c * draw_p                                               # edm.py:645
+    mu_q = qa * z + qb * (xh * fm)                                        # edm.py:655-664
+    z_frag = mu_q + c * draw_q                                            # edm.py:669
+    z = z_lin * lm + z_frag * fm                                          # edm.py:589
+    return torch.cat([remove_mean(z[:, :, :n_dims], nm), z[:, :, n_dims:]], dim=2)   # edm.py:592-594
+
+
+def inpaint_final(z, eps, scalars, draw_p, draw_q):
+    """The two final variants of InpaintingEDM (edm.py:689-716) up to the unnormalisation: sample_p_xh_given_z0 with
+    `draw_p` and sample_q_xh_given_z0_and_x with `draw_q`, both normalised (x,h) on every atom."""
+    inv_a0, sig0, snr0, qa0 = (_sc(scalars, k, z) for k in ("inv_alpha0", "sigma0", "snr0", "qa0"))
+    out_l = inv_a0 * (z - sig0 * eps) + snr0 * draw_p                     # edm.py:689-690, 237-242
+    out_f = inv_a0 * z - qa0 * draw_q                                     # edm.py:706-716
+    return out_l, out_f
+
+
+def final_frame(out, node_mask, n_dims=3, norm_values=(1.0, 4.0, 10.0), norm_biases=(None, 0.0, 0.0)):
+    """chain[0] of a final (x,h): unnormalised coordinates and one_hot(argmax(h)) * node_mask (edm.py:231-233)."""
+    xo = out[:, :, :n_dims] * norm_values[0]
+    ho = out[:, :, n_dims:] * norm_values[1] + norm_biases[1]
+    ho = F.one_hot(torch.argmax(ho, dim=2), ho.shape[2]) * node_mask
+    return torch.cat([xo, ho], dim=2)
+
+
 def edm_sample_chain(sd, cfg: OracleConfig, gamma: Tensor, T: int, x, h, node_mask, fragment_mask, linker_mask,
                      edge_mask, context, keep_frames=None, norm_values=(1.0, 4.0, 10.0),
                      norm_biases=(None, 0.0, 0.0), noise_fn: Optional[NoiseFn] = None,
                      table_timesteps: Optional[int] = None):
     """EDM.sample_chain (edm.py:126-176) with sample_p_zs_given_zt_only_linker (178-208) and
-    sample_p_xh_given_z0_only_linker (210-235) inlined.  `gamma` is the fp32 table; `T` is edm.T (may have
-    been overridden by --n_steps, generate.py:103-104) while `table_timesteps` is the table's own length-1."""
+    sample_p_xh_given_z0_only_linker (210-235) as linker_step / linker_final.  `gamma` is the fp32 table; `T` is edm.T
+    (may have been overridden by --n_steps, generate.py:103-104) while `table_timesteps` is the table's own length-1."""
     if noise_fn is None:
         noise_fn = lambda shape: torch.randn(shape)
     if table_timesteps is None:
@@ -314,31 +390,16 @@ def edm_sample_chain(sd, cfg: OracleConfig, gamma: Tensor, T: int, x, h, node_ma
         return torch.cat([zz[:, :, :nd] * norm_values[0], zz[:, :, nd:] * norm_values[1] + norm_biases[1]], dim=2)
 
     for s in reversed(range(T)):
-        s_arr = torch.full((B, 1), fill_value=s)
-        t_arr = (s_arr + 1) / T
-        s_arr = s_arr / T
-        g_s = gamma_lookup(gamma, s_arr, table_timesteps)
-        g_t = gamma_lookup(gamma, t_arr, table_timesteps)
-        sig2_ts, sig_ts, a_ts = _sigma_alpha_t_given_s(g_t, g_s)
-        sig_s, sig_t = _sigma(g_s), _sigma(g_t)
-        eps = dynamics_forward(sd, cfg, t_arr, z, node_mask, linker_mask, edge_mask, context) * linker_mask
-        mu = z / _bcast(a_ts) - (_bcast(sig2_ts) / _bcast(a_ts) / _bcast(sig_t)) * eps      # edm.py:199
-        sigma = _bcast(sig_ts) * _bcast(sig_s) / _bcast(sig_t)                               # edm.py:202
-        z_s = mu + sigma * masked_noise(noise_fn, B, N, nd, F_, linker_mask)                 # edm.py:205
-        z = z * fragment_mask + z_s * linker_mask
+        sc = step_scalars(gamma, s, T, B, table_timesteps)
+        eps = dynamics_forward(sd, cfg, sc["t"], z, node_mask, linker_mask, edge_mask, context)
+        z = linker_step(z, eps, sc, masked_noise(noise_fn, B, N, nd, F_, linker_mask), fragment_mask, linker_mask)
         chain[(s * keep_frames) // T] = unnorm(z)
 
     zeros = torch.zeros((B, 1))
-    g0 = gamma_lookup(gamma, zeros, table_timesteps)
-    sigma_x = torch.exp(-(-0.5 * g0)).unsqueeze(1)                        # SNR(-0.5*g0), edm.py:216,377-379
-    eps = dynamics_forward(sd, cfg, zeros, z, node_mask, linker_mask, edge_mask, context) * linker_mask
-    mu_x = 1.0 / _bcast(_alpha(g0)) * (z - _bcast(_sigma(g0)) * eps)       # edm.py:237-242
-    out = mu_x + sigma_x * masked_noise(noise_fn, B, N, nd, F_, linker_mask)
-    out = z * fragment_mask + out * linker_mask
-    xo = out[:, :, :nd] * norm_values[0]
-    ho = out[:, :, nd:] * norm_values[1] + norm_biases[1]
-    ho = F.one_hot(torch.argmax(ho, dim=2), F_) * node_mask               # edm.py:233
-    chain[0] = torch.cat([xo, ho], dim=2)
+    eps = dynamics_forward(sd, cfg, zeros, z, node_mask, linker_mask, edge_mask, context)
+    out = linker_final(z, eps, step_scalars(gamma, -1, T, B, table_timesteps),
+                       masked_noise(noise_fn, B, N, nd, F_, linker_mask), fragment_mask, linker_mask)
+    chain[0] = final_frame(out, node_mask, nd, norm_values, norm_biases)
     return chain
 
 
@@ -382,37 +443,20 @@ def inpainting_sample_chain(sd, cfg: OracleConfig, gamma: Tensor, T: int, x, h, 
         return torch.cat([zz[:, :, :nd] * norm_values[0], zz[:, :, nd:] * norm_values[1] + norm_biases[1]], dim=2)
 
     for s in reversed(range(T)):
-        s_arr = torch.full((B, 1), fill_value=s)
-        t_arr = (s_arr + 1) / T
-        s_arr = s_arr / T
-        g_s = gamma_lookup(gamma, s_arr, table_timesteps)
-        g_t = gamma_lookup(gamma, t_arr, table_timesteps)
-        sig2_ts, sig_ts, a_ts = _sigma_alpha_t_given_s(g_t, g_s)
-        sig_s, sig_t, al_s = _sigma(g_s), _sigma(g_t), _alpha(g_s)
-        eps = dynamics_forward(sd, cfg, t_arr, z, node_mask, None, edge_mask, context)               # edm.py:626-633
-        mu = z / _bcast(a_ts) - (_bcast(sig2_ts) / _bcast(a_ts) / _bcast(sig_t)) * eps
-        sigma = _bcast(sig_ts) * _bcast(sig_s) / _bcast(sig_t)
-        z_lin = mu + sigma * com_free_noise(noise_fn, B, N, nd, F_, nmf)                             # edm.py:645
-        xf = xh * fragment_mask
-        mu_q = _bcast(a_ts) * (_bcast(sig_s) ** 2) / (_bcast(sig_t) ** 2) * z + _bcast(al_s) * _bcast(sig2_ts) / (_bcast(sig_t) ** 2) * xf
-        z_frag = mu_q + sigma * com_free_noise(noise_fn, B, N, nd, F_, fragment_mask)                # edm.py:669
-        z = z_lin * linker_mask + z_frag * fragment_mask                                              # edm.py:589
-        z = torch.cat([remove_mean(z[:, :, :nd], nmf), z[:, :, nd:]], dim=2)                          # edm.py:592-594
+        sc = step_scalars(gamma, s, T, B, table_timesteps)
+        eps = dynamics_forward(sd, cfg, sc["t"], z, node_mask, None, edge_mask, context)             # edm.py:626-633
+        draw_p = com_free_noise(noise_fn, B, N, nd, F_, nmf)                                          # edm.py:645
+        draw_q = com_free_noise(noise_fn, B, N, nd, F_, fragment_mask)                                # edm.py:669
+        z = inpaint_step(z, eps, sc, draw_p, draw_q, xh, nmf, fragment_mask, linker_mask, nd)
         chain[(s * keep_frames) // T] = unnorm(z)
 
     zeros = torch.zeros((B, 1))
-    g0 = gamma_lookup(gamma, zeros, table_timesteps)
-    sigma_x = torch.exp(-(-0.5 * g0)).unsqueeze(1)
     eps = dynamics_forward(sd, cfg, zeros, z, node_mask, None, edge_mask, context)
-    mu_x = 1.0 / _bcast(_alpha(g0)) * (z - _bcast(_sigma(g0)) * eps)
-    out_l = mu_x + sigma_x * com_free_noise(noise_fn, B, N, nd, F_, nmf)                              # edm.py:689-690
-    xl = out_l[:, :, :nd] * norm_values[0]
-    hl = F.one_hot(torch.argmax(out_l[:, :, nd:] * norm_values[1] + norm_biases[1], dim=2), F_) * node_mask
-    e2 = com_free_noise(noise_fn, B, N, nd, F_, nmf)                                                  # edm.py:706
-    out_f = (1 / _bcast(_alpha(g0))) * z - (_bcast(_sigma(g0)) / _bcast(_alpha(g0))) * e2
-    xf2 = out_f[:, :, :nd] * norm_values[0]
-    hf2 = F.one_hot(torch.argmax(out_f[:, :, nd:] * norm_values[1] + norm_biases[1], dim=2), F_) * node_mask
-    chain[0] = torch.cat([xl, hl], dim=2) * linker_mask + torch.cat([xf2, hf2], dim=2) * fragment_mask   # edm.py:603-608
+    draw_p = com_free_noise(noise_fn, B, N, nd, F_, nmf)                                              # edm.py:689-690
+    draw_q = com_free_noise(noise_fn, B, N, nd, F_, nmf)                                              # edm.py:706
+    out_l, out_f = inpaint_final(z, eps, step_scalars(gamma, -1, T, B, table_timesteps), draw_p, draw_q)
+    chain[0] = (final_frame(out_l, node_mask, nd, norm_values, norm_biases) * linker_mask
+                + final_frame(out_f, node_mask, nd, norm_values, norm_biases) * fragment_mask)        # edm.py:603-608
     return chain
 
 
