@@ -117,6 +117,9 @@ struct dl_engine {
   int num_sms = 0;
   int max_threads_per_sm = 2048;
   int slice_B_full = 0, slice_b0 = 0;   // dl_set_noise_slice: this engine samples rows [b0, b0 + B) of a B_full batch
+  // dl_set_start_step: the linker sampler starts at step start_step from q(z_t0 | x) with these scalars; -1: from noise at T
+  int start_step = -1;
+  float start_alpha = 0.f, start_sigma = 0.f;
   bool finalized = false;
   std::map<std::string, std::vector<float>> raw;
   float* wblob = nullptr;      // packed fp32 weights
@@ -673,6 +676,10 @@ dl_status check_sampler(const dl_engine* e, int sampler, int T, int keep_frames,
 // standard-normal draws of one chain: init + one per step + final (linker), or their masked pairs (inpainting)
 uint64_t sampler_draws(int sampler, int T) { return sampler == DL_SAMPLER_INPAINT ? (uint64_t)2 * T + 3 : (uint64_t)T + 2; }
 
+// Reverse steps of a call before the final one: the start step when one is set (dl_set_start_step), else T. The loop then
+// runs the last loop_steps + 1 rows of the coefficient table as a chain of that length, so it also sets the draws.
+int loop_steps(const dl_engine* e, int T) { return e && e->start_step >= 0 ? e->start_step : T; }
+
 // While alive, the engine's loop runs on the sub-batch workspace and records its loop time on the ev_r* events: the
 // full batch's workspace, the first loop's dl_last_elapsed_ms and the forward state dl_time_edge_kernel replays stay put.
 struct SubBatchScope {
@@ -935,7 +942,7 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
   if (s != DL_OK) return s;
   if (offset % 4 != 0) { set_err("philox offset must be a multiple of 4 (torch.Generator.get_offset())"); return DL_ERR_INVALID; }
   const NoiseRng q = make_rng(e, B, N, seed, offset);
-  if (offset_consumed) *offset_consumed = sampler_draws(sampler, T) * q.per_draw;
+  if (offset_consumed) *offset_consumed = sampler_draws(sampler, loop_steps(e, T)) * q.per_draw;
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, nullptr,
                            &q, coef, norm, chain, nan_flags, stream);
 }
@@ -958,6 +965,14 @@ dl_status dl_set_noise_slice(dl_engine* e, int32_t B_full, int32_t b0) {
   if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
   if (B_full < 0 || b0 < 0 || (B_full > 0 && b0 >= B_full)) { set_err("bad batch slice (%d of %d)", b0, B_full); return DL_ERR_INVALID; }
   e->slice_B_full = B_full; e->slice_b0 = B_full > 0 ? b0 : 0;
+  return DL_OK;
+}
+
+dl_status dl_set_start_step(dl_engine* e, int32_t t0, float alpha_t0, float sigma_t0) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  if (t0 < 0) { e->start_step = -1; e->start_alpha = e->start_sigma = 0.f; return DL_OK; }
+  if (!std::isfinite(alpha_t0) || !std::isfinite(sigma_t0)) { set_err("alpha_t0 and sigma_t0 must be finite"); return DL_ERR_INVALID; }
+  e->start_step = t0; e->start_alpha = alpha_t0; e->start_sigma = sigma_t0;
   return DL_OK;
 }
 
@@ -1002,6 +1017,13 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
                                     fragment_mask, linker_mask, context, coef, norm, chain);
   if (s != DL_OK) return s;
   const bool inpaint = sampler == DL_SAMPLER_INPAINT;
+  const bool partial = e->start_step >= 0;
+  if (partial && inpaint) { set_err("the inpainting sampler takes no start step (dl_set_start_step)"); return DL_ERR_INVALID; }
+  if (partial && e->start_step > T) { set_err("start step %d exceeds T = %d", e->start_step, T); return DL_ERR_INVALID; }
+  // A start step t0 runs the table's last t0 + 1 rows -- steps t0-1 .. 0, then the final one -- as a loop of Tl = t0 steps:
+  // loop step r reads row r of the copied rows and draw r + 1, so the draws are eps, one per step and the final one.
+  const int Tl = loop_steps(e, T);
+  coef += T - Tl;
   static_assert(sizeof(dl_step_coef) == 32, "dl_step_coef layout");
   CK(cudaSetDevice(e->cfg.device));
   cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
@@ -1012,18 +1034,18 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   const double tc0 = time_chain ? now_ms() : 0.0;
   double tc_plan = 0, tc_capture = 0, tc_inst = 0, tc_launch = 0;
   if ((s = ensure_workspace(e, B, N)) != DL_OK) return s;
-  if (e->coef_cap < T + 1) {
+  if (e->coef_cap < Tl + 1) {
     if (e->coef_dev) cudaFree(e->coef_dev);
     e->coef_dev = nullptr;
-    CK(cudaMalloc((void**)&e->coef_dev, (size_t)(T + 1) * sizeof(dl_step_coef)));
-    e->coef_cap = T + 1;
+    CK(cudaMalloc((void**)&e->coef_dev, (size_t)(Tl + 1) * sizeof(dl_step_coef)));
+    e->coef_cap = Tl + 1;
   }
   // order the private loop stream after the caller's stream (the legacy default stream cannot be captured)
   if (user != st) {
     CK(cudaEventRecord(e->ev_in, user));
     CK(cudaStreamWaitEvent(st, e->ev_in, 0));
   }
-  CK(cudaMemcpyAsync(e->coef_dev, coef, (size_t)(T + 1) * sizeof(dl_step_coef), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(e->coef_dev, coef, (size_t)(Tl + 1) * sizeof(dl_step_coef), cudaMemcpyHostToDevice, st));
   NoiseRng q = rng ? *rng : NoiseRng{};
   if (per_mol) {
     // the captured step reads the engine's copy: the caller's seeds buffer is free once the call has been enqueued
@@ -1033,7 +1055,8 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   CK(cudaMemsetAsync(e->step_ctr, 0, 2 * sizeof(int), st));
   if (nan_flags) CK(cudaMemsetAsync(nan_flags, 0, B * sizeof(int32_t), st));
   const int n = B * N, xd = 3 + e->cfg.in_node_nf;
-  // frames that no reverse step is the last writer of stay zero, as torch.zeros in edm.py:143
+  // frames that no reverse step is the last writer of stay zero, as torch.zeros in edm.py:143 -- with a start step also
+  // every frame whose steps all lie at or above it
   CK(cudaMemsetAsync(chain, 0, (size_t)keep_frames * n * xd * sizeof(float), st));
   if (inpaint && rng) {
     // z_T = COM-free masked noise on every atom (edm.py:565): draw 0 of the device-side stream
@@ -1044,6 +1067,12 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   } else if (inpaint) {
     // the caller's slab 0 is already masked and projected
     CK(cudaMemcpyAsync(e->ws.z, noise, (size_t)n * xd * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  } else if (partial) {
+    const float al = e->start_alpha, sg = e->start_sigma;
+    if (per_mol) k_init_z_partial<true><<<(n * xd + 255) / 256, 256, 0, st>>>(n, xd, xh, fragment_mask, linker_mask, noise, q, al, sg, e->ws.z);
+    else k_init_z_partial<false><<<(n * xd + 255) / 256, 256, 0, st>>>(n, xd, xh, fragment_mask, linker_mask, noise, q, al, sg, e->ws.z);
+    LAUNCH_CHECK();
+    e->launches += 1;
   } else {
     if (per_mol) k_init_z<true><<<(n * xd + 255) / 256, 256, 0, st>>>(n, xd, xh, fragment_mask, linker_mask, noise, q, e->ws.z);
     else k_init_z<false><<<(n * xd + 255) / 256, 256, 0, st>>>(n, xd, xh, fragment_mask, linker_mask, noise, q, e->ws.z);
@@ -1059,9 +1088,9 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   io.node_mask = node_mask; io.linker_mask = inpaint ? nullptr : linker_mask; io.edge_mask = edge_mask;
   io.context = context; io.nan_flags = nan_flags; io.fragment_mask = fragment_mask; io.noise = noise;
   io.rng = q;
-  io.chain = chain; io.T = T; io.norm0 = norm[0]; io.norm1 = norm[1]; io.bias1 = norm[2];
+  io.chain = chain; io.T = Tl; io.norm0 = norm[0]; io.norm1 = norm[1]; io.bias1 = norm[2];
 
-  // capture ONE reverse step; the step index lives on the device, so the same graph serves all T+1 steps
+  // capture ONE reverse step; the step index lives on the device, so the same graph serves all Tl+1 steps
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t exec = nullptr;
   const int64_t before = e->launches;
@@ -1078,7 +1107,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   if (time_chain) tc_inst = now_ms();
   if (ge == cudaSuccess) ge = cudaEventRecord(e->ev_t0, st);
   int failed_step = -1;
-  for (int r = 0; ge == cudaSuccess && r <= T; ++r) {
+  for (int r = 0; ge == cudaSuccess && r <= Tl; ++r) {
     ge = cudaGraphLaunch(exec, st);
     if (ge != cudaSuccess) failed_step = r;
   }
@@ -1089,7 +1118,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     const double tc_done = now_ms();
     float loop = 0.f; cudaEventElapsedTime(&loop, e->ev_t0, e->ev_t1);
     fprintf(stderr, "[dl chain] setup+plan %.2f ms | capture %.2f | instantiate %.2f | %d graph launches enqueued in %.2f | wait for the GPU %.2f | device loop %.2f\n",
-            tc_plan - tc0, tc_capture - tc_plan, tc_inst - tc_capture, T + 1, tc_launch - tc_inst, tc_done - tc_launch, loop);
+            tc_plan - tc0, tc_capture - tc_plan, tc_inst - tc_capture, Tl + 1, tc_launch - tc_inst, tc_done - tc_launch, loop);
   }
   if (ge == cudaSuccess && user != st) {
     ge = cudaEventRecord(e->ev_out, st);
@@ -1102,7 +1131,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     else set_err("%s:%d reverse-loop graph -> %s", __FILE__, __LINE__, cudaGetErrorString(ge));
     return DL_ERR_CUDA;
   }
-  e->launches = before + per_step * (T + 1);
+  e->launches = before + per_step * (Tl + 1);
   return DL_OK;
 }
 
@@ -1121,7 +1150,7 @@ dl_status dl_sample_chain_host(dl_engine* e, int32_t sampler, int32_t B, int32_t
   StageLayout sl;
   const int i_xh = sl.in(xh, frame_bytes), i_nm = sl.in(node_mask, n), i_fm = sl.in(fragment_mask, n * 4),
             i_lm = sl.in(linker_mask, n * 4), i_em = sl.in(fc_em ? edge_mask : nullptr, n * N),
-            i_ctx = sl.in(context, n * e->cfg.context_node_nf * 4), i_nz = sl.in(noise, sampler_draws(sampler, T) * frame_bytes),
+            i_ctx = sl.in(context, n * e->cfg.context_node_nf * 4), i_nz = sl.in(noise, sampler_draws(sampler, loop_steps(e, T)) * frame_bytes),
             i_ch = sl.out(keep_frames * frame_bytes), i_fl = sl.out(B * 4);
   cudaStream_t st = e->loop_stream;
   if ((s = stage_inputs(e->stage, sl, st)) != DL_OK) return s;

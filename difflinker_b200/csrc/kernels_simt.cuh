@@ -1187,6 +1187,22 @@ __global__ void k_init_z(int n_total, int xd, const float* __restrict__ xh, cons
   z[idx] = xh[idx] * fm[g] + (nz * l) * l;
 }
 
+// Partial diffusion: z_t0 ~ q(z_t0 | x) on the linker, the input on the fragments, as EDM.forward noises (edm.py:69-74):
+//   eps = noise[0]*linker_mask;  z_t0 = alpha_t0*xh + sigma_t0*eps;  z = xh*fragment_mask + z_t0*linker_mask
+// Every product and sum is rounded on its own, as torch's elementwise ops round them (no contraction into FMAs).
+template <bool PER_MOL = false>
+__global__ void k_init_z_partial(int n_total, int xd, const float* __restrict__ xh, const float* __restrict__ fm,
+                                 const float* __restrict__ lm, const float* __restrict__ noise, NoiseRng rng, float alpha,
+                                 float sigma, float* __restrict__ z) {
+  int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_total * xd) return;
+  int g = idx / xd;
+  const float l = lm[g], v = xh[idx];
+  const float nz = rng.on ? noise_draw<PER_MOL>(rng, 0, g, idx - g * xd) : noise[idx];
+  const float zt = __fadd_rn(__fmul_rn(alpha, v), __fmul_rn(sigma, __fmul_rn(nz, l)));
+  z[idx] = __fadd_rn(__fmul_rn(v, fm[g]), __fmul_rn(zt, l));
+}
+
 // Debug / test helper: the (n_draws, n_total, 3+F) tensor the device-side stream stands for.
 __global__ void k_noise_fill(int n_draws, int n_total, int xd, NoiseRng rng, float* __restrict__ out) {
   const long long total = (long long)n_draws * n_total * xd;

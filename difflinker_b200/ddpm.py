@@ -51,9 +51,26 @@ def _build_edm(hp: dict, edge_impl='auto', is_geom=None):
                norm_values=hp['normalize_factors'], is_geom=_is_geom(hp) if is_geom is None else bool(is_geom))
 
 
-def sampler_inputs(model, data, sample_fn=None):
+def _keep_linker(data, template):
+    """The template's positions and one-hot with the linker rows of `data` filled in, for partial diffusion, which varies
+    the linker the batch holds. create_templates_for_linker_generation puts a molecule's fragment atoms first and its
+    linker after them; a batch whose linker rows lie elsewhere raises ValueError."""
+    lm = template['linker_mask']
+    n = lm.shape[1]
+    same = (data['linker_mask'].shape[1] >= n and torch.equal(data['linker_mask'][:, :n].to(lm.dtype), lm)
+            and not data['linker_mask'][:, n:].any())
+    if not same:
+        raise ValueError("start_step varies the batch's linker, so each molecule's linker rows must follow its fragment "
+                         "rows, where the sampling template puts them")
+    keep = lm.bool()
+    return (torch.where(keep, data['positions'][:, :n], template['positions']),
+            torch.where(keep, data['one_hot'][:, :n], template['one_hot']))
+
+
+def sampler_inputs(model, data, sample_fn=None, keep_linker=False):
     """What DDPM.sample_chain hands to EDM.sample_chain (lightning.py:405-452): the template batch, the context
-    columns and the centred coordinates, as the keyword arguments of `edm.sample_chain`.
+    columns and the centred coordinates, as the keyword arguments of `edm.sample_chain`. `keep_linker` (partial diffusion)
+    fills the template's linker rows with the batch's own linker before the coordinates are centred.
     `model` needs .inpainting, .anchors_context, .train_data_prefix, .center_of_mass, .val_dataset."""
     if sample_fn is None:
         linker_sizes = data['linker_mask'].sum(1).view(-1).int()
@@ -61,6 +78,8 @@ def sampler_inputs(model, data, sample_fn=None):
         linker_sizes = sample_fn(data)
     template = data if model.inpainting else create_templates_for_linker_generation(data, linker_sizes)
     x, h = template['positions'], template['one_hot']
+    if keep_linker and not model.inpainting:
+        x, h = _keep_linker(data, template)
     node_mask, edge_mask = template['atom_mask'], template['edge_mask']
     anchors, fragment_mask, linker_mask = template['anchors'], template['fragment_mask'], template['linker_mask']
     pocket = '.' in model.train_data_prefix
@@ -86,34 +105,48 @@ def sampler_inputs(model, data, sample_fn=None):
                 linker_mask=linker_mask, context=context)
 
 
-def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None):
+def _check_start(sample_fn, start_step):
+    if sample_fn is not None and start_step is not None:
+        raise ValueError("start_step varies the batch's own linker, so its size is the batch's: pass no sample_fn")
+
+
+def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
+                 start_step=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
     `nan_retries`: rounds that resample only the diverged molecules (EDM.sample_chain; None uses `model.edm.nan_retries`).
-    `require_connected`: the rounds also resample the disconnected molecules (None uses `model.edm.require_connected`)."""
-    kw = sampler_inputs(model, data, sample_fn)
+    `require_connected`: the rounds also resample the disconnected molecules (None uses `model.edm.require_connected`).
+    `start_step` = t0 (partial diffusion, EDM.sample_chain): the template of sample_fn=None with the batch's own linker
+    positions and atom types on its linker rows, sampled from step t0; ValueError with a sample_fn, or when the batch's
+    linker rows do not directly follow its fragment rows."""
+    _check_start(sample_fn, start_step)
+    kw = sampler_inputs(model, data, sample_fn, keep_linker=start_step is not None)
     extra = {} if seeds is None else {'seeds': seeds}
     if nan_retries is not None:
         extra['nan_retries'] = nan_retries
     if require_connected is not None:
         extra['require_connected'] = require_connected
+    if start_step is not None:
+        extra['start_step'] = start_step
     chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **extra)
     return chain, kw['node_mask']
 
 
 def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                max_molecules=256):
+                max_molecules=256, start_step=None):
     """The body of sample_chain for many batches `datas` at once, sampled in shared launches by EDM.sample_many: returns
     [(chain_k, node_mask_k)] in the order of `datas`, each equal to what sample_chain(model, datas[k], ...) returns (with
     seeds[k]) in the sense of EDM.sample_many. `model` as for sample_chain, so accelerated reference modules take it too.
     `sample_fn`, and with noise_mode='per_molecule' and no `seeds` draw_seeds, are called once per batch, in the order the
-    sequential sample_chain calls call them: linker sizes, seeds and the generator's final state are theirs."""
+    sequential sample_chain calls call them: linker sizes, seeds and the generator's final state are theirs. `start_step`,
+    one for every batch, as in sample_chain."""
+    _check_start(sample_fn, start_step)
     edm = model.edm
     derive = seeds is None and edm.noise_mode == 'per_molecule'
     requests, drawn = [], []
     for data in datas:
-        kw = sampler_inputs(model, data, sample_fn)
+        kw = sampler_inputs(model, data, sample_fn, keep_linker=start_step is not None)
         requests.append(kw)
         x = kw['x']
         if derive and x.is_cuda:                # a host batch is refused by EDM.sample_many
@@ -124,6 +157,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
     extra = {} if nan_retries is None else {'nan_retries': nan_retries}
     if require_connected is not None:
         extra['require_connected'] = require_connected
+    if start_step is not None:
+        extra['start_step'] = start_step
     chains = edm.sample_many(requests, keep_frames=keep_frames, seeds=seeds, max_molecules=max_molecules, **extra)
     return [(chain, kw['node_mask']) for chain, kw in zip(chains, requests)]
 
@@ -163,14 +198,15 @@ class DDPM(nn.Module):
         self.edm = _build_edm(self.hparams, edge_impl=edge_impl)
         self.edm.devices = devices          # EDM.devices: split each sampling batch over these CUDA devices
 
-    def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None):
+    def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
+                     start_step=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
-                            require_connected=require_connected)
+                            require_connected=require_connected, start_step=start_step)
 
     def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                    max_molecules=256):
+                    max_molecules=256, start_step=None):
         return sample_many(self, datas, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
-                           require_connected=require_connected, max_molecules=max_molecules)
+                           require_connected=require_connected, max_molecules=max_molecules, start_step=start_step)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

@@ -25,14 +25,26 @@ def _generator_of(dev):
     return torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
 
 
-def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None):
+def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
     samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, conn) resamples
     the molecules that diverged (dl_sample_chain_seeded_retry, which blocks until its rounds are done) and, with `conn` =
-    (thr1, connected), those that are not connected (dl_sample_chain_seeded_retry_connected). Returns (status, what the
-    batch stream consumed)."""
+    (thr1, connected), those that are not connected (dl_sample_chain_seeded_retry_connected). `start` = (t0, alpha_t0,
+    sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of the call
+    (dl_set_start_step). Returns (status, what the batch stream consumed)."""
+    if start is not None:
+        _native.check(lib.dl_set_start_step(eng, *start), "dl_set_start_step")
+    try:
+        return _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry)
+    finally:
+        if start is not None:
+            lib.dl_set_start_step(eng, -1, 0.0, 0.0)
+
+
+def _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry):
+    """_sample_slice's call of the entry point that matches its draws."""
     if stream is None:
         return _native.check(lib.dl_sample_chain_host(eng, *head, noise.data_ptr(), *tail), "dl_sample_chain_host"), 0
     if retry is not None:
@@ -323,19 +335,51 @@ class EDM(torch.nn.Module):
                     fragment_mask=prep(fragment_mask.reshape(n_samples, n_nodes), torch.float32),
                     linker_mask=prep(linker_mask.reshape(n_samples, n_nodes), torch.float32), edge_mask=em, context=ctx)
 
-    def _noise(self, noise, x, node_mask, fragment_mask):
+    def _noise(self, noise, x, node_mask, fragment_mask, start_step=None):
         """(on_device, noise): the device-side stream unless a tensor is injected (tests), the draw function is replaced, or
-        another mode is set; otherwise the whole batch's draws on x's device."""
+        another mode is set; otherwise the whole batch's draws on x's device -- t0 + 2 of them from a start step t0."""
         n_samples, n_nodes = x.size(0), x.size(1)
         dev = x.device
         on_device = (noise is None and dev.type == 'cuda' and self.noise_mode == 'reference_stream'
                      and not self._draws_replaced())
+        n_draws = self._n_draws() if start_step is None else start_step + 2
         if not on_device:
             if noise is None:
-                noise = self._draw_tensor(n_samples, n_nodes, dev, node_mask, fragment_mask)
+                noise = (self._draw_tensor(n_samples, n_nodes, dev, node_mask, fragment_mask) if start_step is None
+                         else self.draw_noise(n_draws, n_samples, n_nodes, dev))
             noise = noise.to(device=dev, dtype=torch.float32).contiguous()
-            assert noise.shape == (self._n_draws(), n_samples, n_nodes, self.n_dims + self.in_node_nf), noise.shape
+            assert noise.shape == (n_draws, n_samples, n_nodes, self.n_dims + self.in_node_nf), noise.shape
         return on_device, noise
+
+    def start_scalars(self, t0, n_samples=1):
+        """(alpha_t0, sigma_t0) of q(z_t0 | x) as EDM.forward evaluates them (edm.py:50-65): t = t0 / T on an (n_samples, 1)
+        fp32 CPU tensor, gamma(t), then sqrt(sigmoid(-gamma)) and sqrt(sigmoid(gamma)). Like step_coefficients, the values
+        are those of torch's CPU kernels at this batch size."""
+        g = self._cpu_gamma()(torch.full((n_samples, 1), fill_value=float(t0)) / self.T)
+        return float(self.alpha(g)[0]), float(self.sigma(g)[0])
+
+    def _start(self, start_step, n_samples):
+        """(t0, alpha_t0, sigma_t0) of a call that starts at step `start_step`, or None for one that starts from noise at T.
+        Raises ValueError unless start_step is an int with 0 <= start_step <= T."""
+        if start_step is None:
+            return None
+        try:
+            if isinstance(start_step, bool):
+                raise TypeError
+            t0 = operator.index(start_step)
+        except TypeError:
+            raise ValueError(f"start_step is an integer step (got {start_step!r})") from None
+        if not 0 <= t0 <= self.T:
+            raise ValueError(f"start_step must lie in [0, T = {self.T}] (got {t0})")
+        return (t0,) + self.start_scalars(t0, n_samples)
+
+    def _nan_exception(self, flags, start):
+        """The FoundNaNException of (B,) NaN flags. The engine tags a flag with the row of the loop it ran; from a start step
+        t0 that loop begins at row T - t0 of the table, so the tag is moved there and first_step names the table's row."""
+        flags = flags.cpu().tolist()
+        if start is not None:
+            flags = [f + ((self.T - start[0]) << 8) if f >> 8 else f for f in flags]
+        return nan_exception_class()(flags=flags)
 
     def _per_molecule_seeds(self, seeds, noise, batch_slice, x):
         """The (B,) int64 seeds on x's device when this call samples the per-molecule stream -- `seeds` are given, or
@@ -436,9 +480,17 @@ class EDM(torch.nn.Module):
 
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None):
+                     noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
+        `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
+        the linker_mask rows of x, h is varied instead of sampled from noise. The loop starts from q(z_t0 | x) as EDM.forward
+        draws it (edm.py:67-74) -- eps drawn as z_T is drawn today, z = xh * fragment_mask + (alpha_t0 xh + sigma_t0 eps) *
+        linker_mask with the scalars of start_scalars -- and runs steps t0-1 .. 0 and the final step as the plain loop runs
+        them. The draws are eps, one per step and the final draw: t0 + 2 (noise= holds t0 + 2 slabs; the batch stream
+        advances by t0 + 2 draws; per-molecule streams use their draws 0 .. t0+1). Frames that no step below t0 writes are
+        zero. t0 bounds how far a sample may move from its input; t0 = T is not the plain sampler (z_T keeps alpha_T xh).
+        Everything below -- seeds, recovery rounds, devices, batch_slice -- applies unchanged.
         `batch_slice=(b0, B_full)`: the inputs are rows [b0, b0+B) of a batch of B_full molecules (strong scaling,
         distributed.sample_chain_sharded); the device-side noise is then those rows of the full batch's draws.
         `seeds` (B ints, or an integer tensor; CUDA inputs): molecule b draws exactly what the reference draws for it
@@ -477,12 +529,14 @@ class EDM(torch.nn.Module):
         dev = x.device
         self.last_attempts = None
         self.last_connected = None
+        start = self._start(start_step, n_samples)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
         check = self._require_connected(require_connected, seeds, noise, batch_slice, x)
         recover = retries > 0 or check      # the recovery entry point: seeds used and attempts come back
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
         full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
-        on_device, noise = (False, None) if dev_seeds is not None else self._noise(noise, x, node_mask, fragment_mask)
+        on_device, noise = ((False, None) if dev_seeds is not None
+                            else self._noise(noise, x, node_mask, fragment_mask, None if start is None else start[0]))
         if batch_slice is not None and not on_device:
             raise ValueError("batch_slice needs the device-side noise stream (CUDA tensors, noise_mode='reference_stream')")
         self.dynamics._check_graph_type()
@@ -505,7 +559,8 @@ class EDM(torch.nn.Module):
         places = [torch.device('cuda', dev_i) for dev_i, *_ in slices] if split else [dev]
         calls, finish = self._enqueue_batch(lib, full, keep_frames, self.step_coefficients(keep_frames, n_samples), slices,
                                             engines, places, dev, noise=noise, dev_seeds=dev_seeds,
-                                            rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check)
+                                            rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check,
+                                            start=start)
         by_device = {}
         for dev_i, c in calls:
             by_device.setdefault(dev_i, []).append(c)
@@ -537,7 +592,7 @@ class EDM(torch.nn.Module):
         if check:
             self.last_connected = out['connected'].cpu() != 0
         if out['bad']:
-            exc = nan_exception_class()(flags=out['flags'].cpu().tolist())
+            exc = self._nan_exception(out['flags'], start)
             if recover:
                 exc.chain = out['chain']    # the rows that did not fail, or were recovered, are good molecules
             raise exc
@@ -548,18 +603,20 @@ class EDM(torch.nn.Module):
 
     @torch.no_grad()
     def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                    max_molecules=256):
+                    max_molecules=256, start_step=None):
         """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
         edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
         (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
-        sample_chain(**requests[k], keep_frames=keep_frames, seeds=seeds[k], nan_retries=..., require_connected=...): always
+        sample_chain(**requests[k], keep_frames=keep_frames, seeds=seeds[k], nan_retries=..., require_connected=...,
+        start_step=start_step): always
         on the SIMT edge path, and on the tensor-core path while no node tile rescales its fp16 operands (DESIGN.md
         section 6). It needs per-molecule streams: `seeds`, one list of B_k seeds per request, or noise_mode='per_molecule',
         which draws them with one draw_seeds(B_k) per request in request order -- the results and the generator's final
         offset are then those of the sequence of sample_chain calls.
         Launches (distributed.plan_launches): whole requests, at most `max_molecules` molecules each unless one request is
         larger, padded to the largest N_k in the launch. Requests share a launch only when sample_chain would give them the
-        same step coefficients (torch's CPU kernels round them differently for some batch sizes) and, with
+        same step coefficients (torch's CPU kernels round them differently for some batch sizes) -- with a `start_step`, one
+        for the whole call, also the same start_scalars, which depend on the batch size the same way -- and, with
         aggregation_method='mean' on FC graphs, where the reference divides by the padded N, only with requests of the same
         N. With `devices` set, whole launches are dealt to the listed devices by their cost (distributed.deal_launches), and
         each device runs its launches in order, from a host thread of its own; a launch is never split.
@@ -579,6 +636,7 @@ class EDM(torch.nn.Module):
         requests = list(requests)
         if not requests:
             raise ValueError("sample_many needs at least one request")
+        self._start(start_step, 1)          # validates it before anything else is checked
         for k, r in enumerate(requests):
             if 'noise' in r or 'batch_slice' in r:
                 raise ValueError(f"request {k} passes noise= or batch_slice=: sample_many samples per-molecule streams, "
@@ -626,10 +684,8 @@ class EDM(torch.nn.Module):
         if seeds is None:
             with torch.cuda.device(dev):    # one draw per request, in request order, as the sample_chain calls draw them
                 cpu_seeds = list(torch.cat([draw_seeds(b, dev) for b in sizes]).cpu().split(sizes))
-        coefs = {b: self.step_coefficients(keep_frames, b) for b in sorted(set(sizes))}
+        coefs, starts, keys = self._launch_keys(sizes, nodes, keep_frames, start_step)
         fc = self.dynamics.graph_type == 'FC'
-        same_n = fc and self.dynamics.aggregation_method == 'mean'
-        keys = [(bytes(coefs[b]), n if same_n else None) for b, n in zip(sizes, nodes)]
         launches = plan_launches(sizes, nodes, max_molecules, keys)
         if fc:                              # edges of the launch's padded molecules
             costs = [sum(sizes[k] for k in ks) * n * n for ks, n in launches]
@@ -657,7 +713,8 @@ class EDM(torch.nn.Module):
             where = torch.device('cuda', dev_i)
             eng = engine_of[slot_of[i]]
             [(_, call)], finish = self._enqueue_batch(lib, full, keep_frames, coefs[sizes[ks[0]]], [(dev_i, replica, 0, b)], [eng],
-                                                      [where], dev, dev_seeds=dev_seeds, retries=retries, check=check)
+                                                      [where], dev, dev_seeds=dev_seeds, retries=retries, check=check,
+                                                      start=starts[sizes[ks[0]]])
             finishes.append(finish)
             by_device.setdefault(dev_i, []).append(
                 functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
@@ -692,20 +749,31 @@ class EDM(torch.nn.Module):
         self.last_loop_ms_many = [(slots[slot_of[i]][0], sorted(ks), loop_ms[i]) for i, (ks, _) in enumerate(launches)]
         for k, f in enumerate(flags):
             if f.any():
-                exc = nan_exception_class()(flags=f.tolist())
+                exc = self._nan_exception(f, starts[sizes[k]])
                 exc.request, exc.results = k, results
                 if recover:
                     exc.chain = results[k]
                 raise exc
         return results
 
+    def _launch_keys(self, sizes, nodes, keep_frames, start_step):
+        """({B: step coefficients}, {B: _start}, the plan_launches key of every request) of sample_many's requests of sizes
+        B_k and N_k: requests share a launch only where sample_chain would give them the same coefficient table and start
+        scalars and, with mean aggregation on FC graphs, the same N."""
+        coefs = {b: self.step_coefficients(keep_frames, b) for b in sorted(set(sizes))}
+        starts = {b: self._start(start_step, b) for b in sorted(set(sizes))}
+        same_n = self.dynamics.graph_type == 'FC' and self.dynamics.aggregation_method == 'mean'
+        keys = [(bytes(coefs[b]), starts[b], n if same_n else None) for b, n in zip(sizes, nodes)]
+        return coefs, starts, keys
+
     def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
-                       retries=0, check=False):
+                       retries=0, check=False, start=None):
         """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
         inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
         replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
         covers the batch where it is. The draws are the per-molecule `dev_seeds`, the batch stream `rng` = (seed, offset,
-        b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _require_connected.
+        b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _require_connected; `start`
+        as returned by _start.
         Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
         (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
         back and returns dict(chain, flags, used, attempts, connected, bad, consumed) on `dev`. `bad` reads the flags: one
@@ -748,7 +816,7 @@ class EDM(torch.nn.Module):
             calls.append((dev_i, functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
-                (retries, used_i, attempts_i, (thr1_i, connected_i) if check else None) if recover else None)))
+                (retries, used_i, attempts_i, (thr1_i, connected_i) if check else None) if recover else None, start)))
 
         def finish():
             if not whole:
@@ -811,8 +879,15 @@ class InpaintingEDM(EDM):
         """draw_noise_inpaint replaced on the instance, in a subclass or on the class supplies the draws."""
         return 'draw_noise_inpaint' in self.__dict__ or type(self).draw_noise_inpaint is not _DRAW_NOISE_INPAINT
 
+    def _start(self, start_step, n_samples):
+        """Partial diffusion noises the linker from the data with EDM.forward's q(z_t | x); this class noises the whole
+        molecule without a centre of mass, which has no such start."""
+        if start_step is not None:
+            raise ValueError("InpaintingEDM does not take start_step: partial diffusion starts the linker sampler (EDM) only")
+        return None
+
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None):
+                     noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -820,11 +895,11 @@ class InpaintingEDM(EDM):
         in which case the replacement draws them. `batch_slice=(b0, B_full)` and `seeds` as in EDM.sample_chain: with
         seeds, molecule b's 2T+3 raw draws are those of the molecule sampled alone after torch.cuda.manual_seed(seeds[b]),
         masked and projected per molecule as always. `nan_retries` and `require_connected` as in EDM.sample_chain; the
-        connectivity check covers every atom of the molecule."""
+        connectivity check covers every atom of the molecule. `start_step` raises ValueError unless None."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
-                                    require_connected=require_connected)
+                                    require_connected=require_connected, start_step=start_step)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

@@ -18,6 +18,8 @@
  *     sample_p_xh_given_z0_only_linker  edm.py:210-235
  *   InpaintingEDM.sample_chain   src/edm.py:549-612      dl_sample_chain (+ _rng) with DL_SAMPLER_INPAINT
  *   either, one seed per molecule (no reference API)     dl_sample_chain_seeded
+ *   EDM, from q(z_t0 | x) of a known linker (edm.py:67-74) dl_set_start_step, then any dl_sample_chain* entry point
+ *     at step t0 (partial diffusion, no reference API)
  *   either, resampling only the molecules that diverged  dl_sample_chain_seeded_retry, dl_retry_seed, dl_last_retry_ms
  *     (the reference's callers resample the whole batch, generate.py:153-161)
  *   either, also resampling the disconnected molecules  dl_sample_chain_seeded_retry_connected, dl_molecule_connected
@@ -299,6 +301,23 @@ float dl_last_retry_ms(dl_engine* e);
  * GEMM to rescale a tile's fp16 operands (tiles span molecules, so the split moves them; DESIGN.md section 6). B_full = 0
  * switches it off. */
 dl_status dl_set_noise_slice(dl_engine* e, int32_t B_full, int32_t b0);
+/*
+ * Partial diffusion (no reference API; the `optimize` mode of DiffSBDD): the following dl_sample_chain* calls of this engine,
+ * the recovery rounds of dl_sample_chain_seeded_retry(_connected) included, vary the linker the caller's xh holds on its
+ * linker_mask rows instead of sampling one from pure noise. With 0 <= t0 <= T:
+ *   z     = xh * fragment_mask + (alpha_t0 * xh + sigma_t0 * eps) * linker_mask,   eps = draw 0 * linker_mask
+ *           -- q(z_t0 | x) as EDM.forward draws it (edm.py:67-74), each product and sum rounded on its own; alpha_t0 and
+ *           sigma_t0 are sqrt(sigmoid(-gamma)) and sqrt(sigmoid(gamma)) of gamma(t0 / T), evaluated as the caller evaluates
+ *           the coefficient table;
+ *   steps s = t0-1 .. 0 with rows T-1-s of `coef` (time feature (s+1)/T), then the final step with row T.
+ * The draws are eps, one per step and the final draw: t0 + 2, in the order of dl_sample_chain_rng -- a noise tensor holds t0 + 2
+ * slabs, offset_consumed is (t0 + 2) * per_draw, and a per-molecule stream uses its draws 0 .. t0+1. Frames with no step
+ * below t0 stay zero; chain[0] is the final sample. The NaN flags' row tag counts the loop's rows from the start step: row
+ * j is step t0-1-j. t0 = T is not the plain sampler: z_T keeps alpha_T * xh. DL_SAMPLER_INPAINT with a start step set, or
+ * t0 > T, is DL_ERR_INVALID at the sampling call. A negative t0 clears the start step (the default). Non-finite alpha_t0 or
+ * sigma_t0 is DL_ERR_INVALID.
+ */
+dl_status dl_set_start_step(dl_engine* e, int32_t t0, float alpha_t0, float sigma_t0);
 /* The (n_draws,B,N,3+F) tensor the device-side stream of dl_sample_chain_rng stands for (tests, debugging). DEVICE out. */
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream);
