@@ -10,6 +10,7 @@ GRAPH_TYPES = {"FC": 0, "4A": 1, "FC-4A": 2, "FC-10A-4A": 3}
 EDGE_IMPLS = {"auto": 0, "simt": 1, "wgmma": 2}
 SAMPLER_LINKER, SAMPLER_INPAINT = 0, 1
 AGGREGATIONS = {"sum": 0, "mean": 1}
+CHECK_CONNECTED, CHECK_VALENCE = 1, 2   # DL_CHECK_*
 COORDS_RANGE = 15.0   # EGNN hands its own coords_range=15 to every EquivariantBlock (src/egnn.py:183,209)
 
 
@@ -32,6 +33,17 @@ class DLEgnnOptions(C.Structure):
 class DLSizeGNNConfig(C.Structure):
     _fields_ = [("in_node_nf", C.c_int32), ("hidden_nf", C.c_int32), ("out_node_nf", C.c_int32),
                 ("n_layers", C.c_int32), ("device", C.c_int32)]
+
+
+class DLMoleculeChecks(C.Structure):
+    _fields_ = [("require", C.c_int32), ("n_types", C.c_int32), ("thr1", C.c_void_p), ("thr2", C.c_void_p),
+                ("thr3", C.c_void_p), ("max_valence", C.c_void_p)]
+
+    @classmethod
+    def of(cls, require, tables):
+        """The struct over `tables` = [thr1] or [thr1, thr2, thr3, max_valence], device tensors the caller keeps alive."""
+        ptrs = [t.data_ptr() for t in tables] + [None] * (4 - len(tables))
+        return cls(require, tables[0].shape[0], *ptrs)
 
 
 class DLStepCoef(C.Structure):
@@ -62,6 +74,9 @@ SYMBOLS = {
     "dl_sample_chain_seeded_retry_connected": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                                       _P, _I32, _P, _P, _I32, _P, _P, _P]),
     "dl_molecule_connected": (_I32, [_I32, _I32, _I32, _P, _I32, _P, _P, _I32, _I32, _P, _P, _P]),
+    "dl_sample_chain_seeded_retry_checked": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                                    _P, _I32, _P, _P, C.POINTER(DLMoleculeChecks), _P, _P]),
+    "dl_molecule_check": (_I32, [_I32, _I32, C.POINTER(DLMoleculeChecks), _P, _I32, _P, _P, _I32, _I32, _P, _P, _P]),
     "dl_last_retry_ms": (_F, [_P]),
     "dl_set_noise_slice": (_I32, [_P, _I32, _I32]),
     "dl_set_start_step": (_I32, [_P, _I32, _F, _F]),

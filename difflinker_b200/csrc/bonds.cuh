@@ -1,6 +1,6 @@
-// The bond predicate of molecule_builder.get_bond_order (src/molecule_builder.py:77-102), shared by dl_bond_orders
-// (output_stage.cu) and the connectivity check of the recovery rounds (kernels_retry.cuh), so both decide "bonded" with
-// the same arithmetic.
+// The bond predicate and the bond order of molecule_builder.get_bond_order (src/molecule_builder.py:77-102), shared by
+// dl_bond_orders (output_stage.cu) and the connectivity and valence checks of the recovery rounds (kernels_retry.cuh), so
+// all of them decide "bonded" and "the order of a pair" with the same arithmetic.
 #pragma once
 
 namespace dl {
@@ -18,6 +18,19 @@ __device__ __forceinline__ int bond_pair(float3 xi, float3 xj, int ti, int tj, i
   if (a < 0 || c >= T) return -1;
   const float t1 = thr1[a * T + c];
   return (t1 >= 0.f && dist < t1) ? a * T + c : -1;
+}
+
+// get_bond_order(...) itself: 0 when the atoms do not bond (bond_pair), else 1, 2 or 3 -- double when the distance is also
+// below the pair's thr2 entry and that entry exists, triple when it is below thr3 as well.
+__device__ __forceinline__ int bond_order_pair(float3 xi, float3 xj, int ti, int tj, int T, const float* __restrict__ thr1,
+                                               const float* __restrict__ thr2, const float* __restrict__ thr3) {
+  float dist;
+  const int k = bond_pair(xi, xj, ti, tj, T, thr1, &dist);
+  if (k < 0) return 0;
+  const float t2 = thr2[k];
+  if (!(t2 >= 0.f && dist < t2)) return 1;
+  const float t3 = thr3[k];
+  return (t3 >= 0.f && dist < t3) ? 3 : 2;
 }
 
 }  // namespace dl

@@ -1167,30 +1167,47 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt) { return retry_seed(seed,
 
 namespace {
 
-// The connectivity check of dl_sample_chain_seeded_retry_connected: the bond table and the (B) flags it writes.
-struct ConnCheck {
-  int n_types;
-  const float* thr1;
-  int32_t* connected;
-};
+static_assert(CHECK_CONNECTED == DL_CHECK_CONNECTED && CHECK_VALENCE == DL_CHECK_VALENCE, "kernels_retry.cuh vs header");
 
-// k_connected over frame 0 of a (B, N) chain of this engine's model: ligand rows only on cut-off (pocket) graphs.
-ConnArgs conn_args(const dl_engine* e, const ConnCheck& cc, const float* chain, int N, const int8_t* node_mask,
-                   const float* context, int32_t* connected) {
-  ConnArgs ca{};
-  ca.xh = chain; ca.N = N; ca.row_stride = 3 + e->cfg.in_node_nf; ca.n_types = cc.n_types; ca.thr1 = cc.thr1;
-  ca.node_mask = node_mask; ca.C = e->cfg.context_node_nf; ca.context = context;
-  ca.drop_pocket = e->cfg.graph_type != DL_GRAPH_FC; ca.connected = connected;
+// What is wrong with a caller's dl_molecule_checks for molecules of N rows whose h holds at most max_types type columns, or
+// null.
+const char* checks_error(const dl_molecule_checks* ck, int N, int max_types) {
+  if (!ck) return "null checks";
+  if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE)))
+    return "checks->require must be DL_CHECK_CONNECTED, DL_CHECK_VALENCE or both";
+  if (ck->n_types < 1 || ck->n_types > max_types) return "checks->n_types must be in [1, the width of the atom features]";
+  if (!ck->thr1) return "null checks->thr1";
+  if ((ck->require & DL_CHECK_VALENCE) && (!ck->thr2 || !ck->thr3 || !ck->max_valence))
+    return "DL_CHECK_VALENCE needs checks->thr2, thr3 and max_valence";
+  if (N > CONN_MAX_N) return "the molecule checks take N <= 8192";
+  return nullptr;
+}
+
+// k_molecule_check over (B, N) molecules with the caller's tables.
+CheckArgs check_args(const dl_molecule_checks& ck, const float* xh, int N, int row_stride, const int8_t* node_mask,
+                     const float* context, int C, bool drop_pocket, int32_t* passed) {
+  CheckArgs ca{};
+  ca.xh = xh; ca.N = N; ca.row_stride = row_stride; ca.n_types = ck.n_types;
+  ca.thr1 = ck.thr1; ca.thr2 = ck.thr2; ca.thr3 = ck.thr3; ca.max_valence = ck.max_valence;
+  ca.node_mask = node_mask; ca.C = C; ca.context = context; ca.drop_pocket = drop_pocket; ca.passed = passed;
   return ca;
 }
 
-// dl_sample_chain_seeded_retry, and with `cc` its connectivity check: a row then fails if its NaN flag is set or it is not
-// connected, and a resampled row replaces the caller's unless the caller's row is finite and the new one diverged.
+// ... over frame 0 of a (B, N) chain of this engine's model: ligand rows only on cut-off (pocket) graphs.
+CheckArgs check_args(const dl_engine* e, const dl_molecule_checks& ck, const float* chain, int N, const int8_t* node_mask,
+                     const float* context, int32_t* passed) {
+  return check_args(ck, chain, N, 3 + e->cfg.in_node_nf, node_mask, context, e->cfg.context_node_nf,
+                    e->cfg.graph_type != DL_GRAPH_FC, passed);
+}
+
+// dl_sample_chain_seeded_retry, and with `ck` its molecule checks, whose verdicts go to `passed`: a row then fails if its NaN
+// flag is set or a required bit is missing, and a resampled row replaces the caller's unless the caller's row is finite and
+// the new one diverged.
 dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames, const float* xh,
                        const int8_t* node_mask, const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
                        const float* context, const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
-                       int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts, const ConnCheck* cc,
-                       void* stream) {
+                       int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
+                       const dl_molecule_checks* ck, int32_t* passed, void* stream) {
   e->retry_ms = 0.f;
   dl_status s = dl_sample_chain_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask,
                                        context, seeds, coef, norm, chain, nan_flags, stream);
@@ -1198,11 +1215,12 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CK(cudaMemcpyAsync(seeds_used, seeds, (size_t)B * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(attempts, 0, (size_t)B * sizeof(int32_t), st));
-  std::vector<int32_t> flags(B), conn(B, 1);
-  if (cc) {
-    CK(launch_connected(conn_args(e, *cc, chain, N, node_mask, context, cc->connected), B, st));
+  const int require = ck ? ck->require : 0;
+  std::vector<int32_t> flags(B), pass(B, require);
+  if (ck) {
+    CK(launch_molecule_check(require, check_args(e, *ck, chain, N, node_mask, context, passed), B, st));
     e->launches += 1;
-    CK(cudaMemcpyAsync(conn.data(), cc->connected, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(pass.data(), passed, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   }
   CK(cudaMemcpyAsync(flags.data(), nan_flags, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -1211,7 +1229,7 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
   const int xd = 3 + e->cfg.in_node_nf, C = e->cfg.context_node_nf;
   for (int a = 1; a <= max_retries; ++a) {
     std::vector<int32_t> rows;
-    for (int b = 0; b < B; ++b) if (flags[b] != 0 || conn[b] == 0) rows.push_back(b);
+    for (int b = 0; b < B; ++b) if (flags[b] != 0 || pass[b] != require) rows.push_back(b);
     if (rows.empty()) break;
     const int Bs = (int)rows.size();
     const size_t n = (size_t)Bs * N;
@@ -1220,7 +1238,7 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
               i_fm = sl.out(n * 4), i_lm = sl.out(n * 4), i_em = sl.add(nullptr, n * N, fc_em),
               i_ctx = sl.add(nullptr, n * C * 4, context != nullptr && C > 0), i_sd = sl.out((size_t)Bs * 8),
               i_ch = sl.out((size_t)keep_frames * n * xd * 4), i_fl = sl.out((size_t)Bs * 4),
-              i_cn = sl.add(nullptr, (size_t)Bs * 4, cc != nullptr), i_tk = sl.add(nullptr, (size_t)Bs * 4, cc != nullptr);
+              i_ps = sl.add(nullptr, (size_t)Bs * 4, ck != nullptr), i_tk = sl.add(nullptr, (size_t)Bs * 4, ck != nullptr);
     if ((s = stage_inputs(e->sub_rows, sl, st)) != DL_OK) return s;   // the row list goes to the device once per round
     CK(cudaEventRecord(e->ev_g0, st));
     RowGatherArgs ga{};
@@ -1246,12 +1264,12 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     sa.s_chain = sl.at<float>(i_ch); sa.s_flags = sl.at<int32_t>(i_fl); sa.s_seeds = ga.s_seeds;
     sa.chain = chain; sa.flags = nan_flags; sa.seeds_used = reinterpret_cast<unsigned long long*>(seeds_used);
     sa.attempts = attempts;
-    if (cc) {
-      ConnArgs ca = conn_args(e, *cc, sa.s_chain, N, ga.s_node_mask, ga.s_context, sl.at<int32_t>(i_cn));
+    if (ck) {
+      CheckArgs ca = check_args(e, *ck, sa.s_chain, N, ga.s_node_mask, ga.s_context, sl.at<int32_t>(i_ps));
       ca.rows = ga.rows; ca.flags = nan_flags; ca.s_flags = sa.s_flags; ca.take = sl.at<int32_t>(i_tk);
-      CK(launch_connected(ca, Bs, st));
+      CK(launch_molecule_check(require, ca, Bs, st));
       e->launches += 1;
-      sa.take = ca.take; sa.s_connected = ca.connected; sa.connected = cc->connected;
+      sa.take = ca.take; sa.s_passed = ca.passed; sa.passed = passed;
       k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
     } else {
       k_scatter_rows<false><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
@@ -1259,10 +1277,10 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     LAUNCH_CHECK();
     e->launches += 1;
     CK(cudaEventRecord(e->ev_g1, st));
-    std::vector<int32_t> sub_flags(Bs), sub_conn(Bs, 1), take(Bs, 1);
+    std::vector<int32_t> sub_flags(Bs), sub_pass(Bs, require), take(Bs, 1);
     CK(cudaMemcpyAsync(sub_flags.data(), sa.s_flags, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    if (cc) {
-      CK(cudaMemcpyAsync(sub_conn.data(), sa.s_connected, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (ck) {
+      CK(cudaMemcpyAsync(sub_pass.data(), sa.s_passed, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
       CK(cudaMemcpyAsync(take.data(), sa.take, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     }
     CK(cudaStreamSynchronize(st));
@@ -1270,7 +1288,7 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     CK(cudaEventElapsedTime(&ms, e->ev_g0, e->ev_g1));
     e->retry_ms += ms;
     for (int i = 0; i < Bs; ++i)
-      if (take[i]) { flags[rows[i]] = sub_flags[i]; conn[rows[i]] = sub_conn[i]; }
+      if (take[i]) { flags[rows[i]] = sub_flags[i]; pass[rows[i]] = sub_pass[i]; }
   }
   for (int b = 0; b < B; ++b) if (flags[b] != 0) return DL_NAN_DETECTED;
   return DL_OK;
@@ -1290,7 +1308,7 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
   if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
   if (!nan_flags || !seeds_used || !attempts) { set_err("null argument (nan_flags, seeds_used or attempts)"); return DL_ERR_INVALID; }
   return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
-                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, nullptr, stream);
+                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, nullptr, nullptr, stream);
 }
 
 dl_status dl_sample_chain_seeded_retry_connected(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
@@ -1311,9 +1329,30 @@ dl_status dl_sample_chain_seeded_retry_connected(dl_engine* e, int32_t sampler, 
     return DL_ERR_INVALID;
   }
   if (N > CONN_MAX_N) { set_err("the connectivity check takes N <= %d (got %d)", CONN_MAX_N, N); return DL_ERR_INVALID; }
-  const ConnCheck cc{n_types, thr1, connected};
+  const dl_molecule_checks ck{DL_CHECK_CONNECTED, n_types, thr1, nullptr, nullptr, nullptr};
   return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
-                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, &cc, stream);
+                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, &ck, connected, stream);
+}
+
+dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
+                                               int32_t keep_frames, const float* xh, const int8_t* node_mask,
+                                               const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
+                                               const float* context, const uint64_t* seeds, const dl_step_coef* coef,
+                                               const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries,
+                                               uint64_t* seeds_used, int32_t* attempts, const dl_molecule_checks* checks,
+                                               int32_t* passed, void* stream) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
+  if (!nan_flags || !seeds_used || !attempts || !passed) {
+    set_err("null argument (nan_flags, seeds_used, attempts or passed)");
+    return DL_ERR_INVALID;
+  }
+  if (const char* why = checks_error(checks, N, e->cfg.in_node_nf)) {
+    set_err("dl_sample_chain_seeded_retry_checked: %s", why);
+    return DL_ERR_INVALID;
+  }
+  return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
+                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, passed, stream);
 }
 
 dl_status dl_molecule_connected(int32_t B, int32_t N, int32_t n_types, const float* xh, int32_t xh_row_stride,
@@ -1324,10 +1363,25 @@ dl_status dl_molecule_connected(int32_t B, int32_t N, int32_t n_types, const flo
     set_err("dl_molecule_connected: invalid argument");
     return DL_ERR_INVALID;
   }
-  ConnArgs ca{};
-  ca.xh = xh; ca.N = N; ca.row_stride = xh_row_stride; ca.n_types = n_types; ca.thr1 = thr1; ca.node_mask = node_mask;
-  ca.context = context; ca.C = context_nf; ca.drop_pocket = drop_pocket != 0; ca.connected = connected;
-  CK(launch_connected(ca, B, reinterpret_cast<cudaStream_t>(stream)));
+  const dl_molecule_checks ck{DL_CHECK_CONNECTED, n_types, thr1, nullptr, nullptr, nullptr};
+  CK(launch_molecule_check(ck.require, check_args(ck, xh, N, xh_row_stride, node_mask, context, context_nf, drop_pocket != 0,
+                                                  connected), B, reinterpret_cast<cudaStream_t>(stream)));
+  return DL_OK;
+}
+
+dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
+                            const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
+                            int32_t* passed, int32_t* valence, void* stream) {
+  const char* why = checks_error(checks, N, xh_row_stride - 3);
+  if (!why && (B <= 0 || N <= 0 || !xh || !node_mask || !passed || (drop_pocket && (!context || context_nf < 1))))
+    why = "invalid argument";
+  if (!why && valence && !(checks->require & DL_CHECK_VALENCE)) why = "valence needs DL_CHECK_VALENCE";
+  if (why) { set_err("dl_molecule_check: %s", why); return DL_ERR_INVALID; }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CheckArgs ca = check_args(*checks, xh, N, xh_row_stride, node_mask, context, context_nf, drop_pocket != 0, passed);
+  ca.valence = valence;
+  if (valence) CK(cudaMemsetAsync(valence, 0, (size_t)B * N * sizeof(int32_t), st));   // the rows that are not checked
+  CK(launch_molecule_check(checks->require, ca, B, st));
   return DL_OK;
 }
 

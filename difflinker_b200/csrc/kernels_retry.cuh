@@ -57,19 +57,19 @@ struct RowScatterArgs {
   int32_t* flags;
   unsigned long long* seeds_used;
   int32_t* attempts;
-  // CONN rounds only: take[i] (k_connected) says whether sub-batch row i replaces the caller's row; s_connected / connected
-  // are the sub-batch's and the caller's connectivity flags
-  const int32_t *take, *s_connected;
-  int32_t* connected;
+  // CHECKED rounds only: take[i] (k_molecule_check) says whether sub-batch row i replaces the caller's row; s_passed /
+  // passed are the sub-batch's and the caller's check verdicts
+  const int32_t *take, *s_passed;
+  int32_t* passed;
 };
 
 // grid (Bs, keep_frames): CTA (i, f) writes frame f of sub-batch row i over row rows[i] of the caller's chain; the f = 0
-// CTAs also write the molecule's flags, the seed that produced the row and the attempt. CONN: only rows with take[i] set,
-// and their connectivity flag with them.
-template <bool CONN>
+// CTAs also write the molecule's flags, the seed that produced the row and the attempt. CHECKED: only rows with take[i]
+// set, and their check verdicts with them.
+template <bool CHECKED>
 __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a) {
   const int i = blockIdx.x, f = blockIdx.y;
-  if (CONN && !a.take[i]) return;
+  if (CHECKED && !a.take[i]) return;
   const size_t b = a.rows[i], row = (size_t)a.N * a.xd;
   const float* src = a.s_chain + ((size_t)f * a.Bs + i) * row;
   float* dst = a.chain + ((size_t)f * a.B + b) * row;
@@ -78,25 +78,33 @@ __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a) {
     a.flags[b] = a.s_flags[i];
     a.seeds_used[b] = a.s_seeds[i];
     a.attempts[b] = a.attempt;
-    if (CONN) a.connected[b] = a.s_connected[i];
+    if (CHECKED) a.passed[b] = a.s_passed[i];
   }
 }
 
-// ---- connectivity: is the final molecule in one piece? ---------------------------------------------------------------
+// ---- molecule checks: is the final molecule in one piece, and is every atom within its valence? -----------------------
 // The atoms of molecule b are its rows n with node_mask != 0, minus the pocket atoms (context column C - 1 set) when
-// drop_pocket; atoms i and j bond iff bond_pair (get_bond_order > 0) with types argmax(h[:n_types]). connected[b] = 1 iff
-// that graph has exactly one component (a single atom is connected, no atom is not): len(Chem.GetMolFrags(mol)) == 1 for
-// the molecule build_molecule makes of them (lightning.py:364-377, metrics.py:20-27).
+// drop_pocket, with types argmax(h[:n_types]).
+// CHECK_CONNECTED: atoms i and j bond iff bond_pair (get_bond_order > 0); the bit is set iff that graph has exactly one
+// component (a single atom is connected, no atom is not): len(Chem.GetMolFrags(mol)) == 1 for the molecule build_molecule
+// makes of them (lightning.py:364-377, metrics.py:20-27).
+// CHECK_VALENCE: an atom's valence is the sum of bond_order_pair (get_bond_order) over the other checked atoms; the bit is
+// set iff every atom's valence is <= max_valence[its type] (no atom: set). The predicate is stated in full at
+// dl_molecule_checks in the header.
+constexpr int CHECK_CONNECTED = 1, CHECK_VALENCE = 2;                // DL_CHECK_* of the header
 constexpr int CONN_MAX_N = 8192;                                     // rows per molecule: 20 bytes of shared memory each
 constexpr int CONN_SMEM_MAX = CONN_MAX_N * (int)(sizeof(float4) + sizeof(int));
 
-struct ConnArgs {
+struct CheckArgs {
   const float* xh;                       // (B, N, row_stride): x at columns 0..2, h from column 3 -- chain[0]
   int N, row_stride, n_types, C, drop_pocket;
-  const float* thr1;                     // (n_types, n_types) single-bond thresholds in pm, [min type][max type]
+  const float *thr1, *thr2, *thr3;       // (n_types, n_types) bond thresholds in pm, [min type][max type]; thr2, thr3 and
+  const int32_t* max_valence;            // max_valence (n_types) are read by CHECK_VALENCE only
   const int8_t* node_mask;               // (B, N)
   const float* context;                  // (B, N, C); read only when drop_pocket
-  int32_t* connected;                    // (B) out
+  int32_t* passed;                       // (B) out: OR of the CHECK_* bits the molecule satisfies, among those checked
+  int32_t* valence;                      // (B, N) or null: the valence of every checked row (CHECK_VALENCE; other rows are
+                                         // not written)
   // recovery rounds (rows != null): the molecules are sub-batch rows; take[i] = whether row i replaces the caller's row
   // rows[i] -- always, unless the caller's row is finite (flags == 0) and the resampled one diverged
   const int* rows;
@@ -105,13 +113,17 @@ struct ConnArgs {
 };
 
 // One CTA per molecule. The checked atoms are compacted, in row order, into shared memory (coordinates and type; padded
-// and pocket rows are never read beyond their masks). Components are then found by min-label hooking: every bonded pair
-// whose trees differ hooks the larger root under the smaller (atomicMin), trees are flattened, and this repeats until a
-// pass over all pairs hooks nothing. Labels only ever decrease and each root is its tree's smallest atom, so the final
-// labels -- every atom's component minimum -- and the flag do not depend on the order the threads hook in.
-__global__ void __launch_bounds__(256) k_connected(ConnArgs a) {
+// and pocket rows are never read beyond their masks).
+// Valence: a warp per atom sums the integer bond orders of its pairs with every other atom, so the sums do not depend on
+// the order the lanes add in.
+// Components are found by min-label hooking: every bonded pair whose trees differ hooks the larger root under the smaller
+// (atomicMin), trees are flattened, and this repeats until a pass over all pairs hooks nothing. Labels only ever decrease
+// and each root is its tree's smallest atom, so the final labels -- every atom's component minimum -- and the flag do not
+// depend on the order the threads hook in.
+template <int CHECKS>
+__global__ void __launch_bounds__(256) k_molecule_check(CheckArgs a) {
   extern __shared__ float4 s_at[];                    // [n]: x, y, z, type (int bits)
-  int* s_lab = reinterpret_cast<int*>(s_at + a.N);    // [n]: parent pointers
+  int* s_lab = reinterpret_cast<int*>(s_at + a.N);    // [n]: the atoms' rows (valence), then parent pointers (components)
   __shared__ int s_warp[8], s_n, s_changed;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = blockIdx.x;
@@ -135,63 +147,101 @@ __global__ void __launch_bounds__(256) k_connected(ConnArgs a) {
         if (v > cur || (isnan(v) && !isnan(cur))) best = k;
       }
       s_at[off] = make_float4(row[0], row[1], row[2], __int_as_float(best));
-      s_lab[off] = off;
+      s_lab[off] = (CHECKS & CHECK_VALENCE) ? r : off;
     }
     __syncthreads();
     if (tid == 0) s_n += total;
     __syncthreads();
   }
   const int n = s_n;
-  volatile int* lab = s_lab;
-  for (;;) {
-    if (tid == 0) s_changed = 0;
-    __syncthreads();
-    for (int i = warp; i < n; i += 8) {               // warp per row i, lanes over the pairs (i, j < i)
+  int verdict = 0;
+  if (CHECKS & CHECK_VALENCE) {
+    int over = 0;
+    for (int i = warp; i < n; i += 8) {               // warp per atom i, lanes over its partners j != i
       const float4 pi = s_at[i];
-      for (int j = lane; j < i; j += 32) {
+      int v = 0;
+      for (int j = lane; j < n; j += 32) {
         const float4 pj = s_at[j];
-        float dist;
-        if (bond_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
-                      __float_as_int(pj.w), a.n_types, a.thr1, &dist) < 0)
-          continue;
-        int ri = i, rj = j;
-        while (lab[ri] != ri) ri = lab[ri];
-        while (lab[rj] != rj) rj = lab[rj];
-        if (ri != rj) {
-          atomicMin(&s_lab[max(ri, rj)], min(ri, rj));
-          s_changed = 1;
-        }
+        if (j != i)
+          v += bond_order_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
+                               __float_as_int(pj.w), a.n_types, a.thr1, a.thr2, a.thr3);
+      }
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == 0) {
+        over |= v > a.max_valence[__float_as_int(pi.w)];
+        if (a.valence) a.valence[g0 + s_lab[i]] = v;
       }
     }
-    __syncthreads();
-    const int changed = s_changed;
-    for (int i = tid; i < n; i += 256) {              // flatten: every atom points at its root
-      int r = i;
-      while (lab[r] != r) r = lab[r];
-      lab[i] = r;
+    if (!__syncthreads_or(over)) verdict |= CHECK_VALENCE;
+    if (CHECKS & CHECK_CONNECTED) {
+      for (int i = tid; i < n; i += 256) s_lab[i] = i;
+      __syncthreads();
     }
-    __syncthreads();
-    if (!changed) break;
   }
-  int roots = 0;
-  for (int i0 = 0; i0 < n; i0 += 256) roots += __syncthreads_count(i0 + tid < n && lab[i0 + tid] == i0 + tid);
+  if (CHECKS & CHECK_CONNECTED) {
+    volatile int* lab = s_lab;
+    for (;;) {
+      if (tid == 0) s_changed = 0;
+      __syncthreads();
+      for (int i = warp; i < n; i += 8) {             // warp per row i, lanes over the pairs (i, j < i)
+        const float4 pi = s_at[i];
+        for (int j = lane; j < i; j += 32) {
+          const float4 pj = s_at[j];
+          float dist;
+          if (bond_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
+                        __float_as_int(pj.w), a.n_types, a.thr1, &dist) < 0)
+            continue;
+          int ri = i, rj = j;
+          while (lab[ri] != ri) ri = lab[ri];
+          while (lab[rj] != rj) rj = lab[rj];
+          if (ri != rj) {
+            atomicMin(&s_lab[max(ri, rj)], min(ri, rj));
+            s_changed = 1;
+          }
+        }
+      }
+      __syncthreads();
+      const int changed = s_changed;
+      for (int i = tid; i < n; i += 256) {            // flatten: every atom points at its root
+        int r = i;
+        while (lab[r] != r) r = lab[r];
+        lab[i] = r;
+      }
+      __syncthreads();
+      if (!changed) break;
+    }
+    int roots = 0;
+    for (int i0 = 0; i0 < n; i0 += 256) roots += __syncthreads_count(i0 + tid < n && lab[i0 + tid] == i0 + tid);
+    if (roots == 1) verdict |= CHECK_CONNECTED;
+  }
   if (tid == 0) {
-    const int conn = roots == 1;
-    a.connected[b] = conn;
+    a.passed[b] = verdict;
     if (a.rows) a.take[b] = !(a.flags[a.rows[b]] == 0 && a.s_flags[b] != 0);
   }
 }
 
-// Launches k_connected over B molecules; N <= CONN_MAX_N. The shared-memory limit is raised to its one maximum the first
-// time a molecule needs more than the default, so concurrent callers never lower it under each other.
-inline cudaError_t launch_connected(const ConnArgs& a, int B, cudaStream_t st) {
+template <int CHECKS>
+cudaError_t launch_molecule_check_as(const CheckArgs& a, int B, cudaStream_t st) {
   const size_t smem = (size_t)a.N * (sizeof(float4) + sizeof(int));
   if (smem > 48 * 1024) {
-    const cudaError_t err = cudaFuncSetAttribute(k_connected, cudaFuncAttributeMaxDynamicSharedMemorySize, CONN_SMEM_MAX);
+    const cudaError_t err =
+        cudaFuncSetAttribute(k_molecule_check<CHECKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, CONN_SMEM_MAX);
     if (err != cudaSuccess) return err;
   }
-  k_connected<<<B, 256, smem, st>>>(a);
+  k_molecule_check<CHECKS><<<B, 256, smem, st>>>(a);
   return cudaGetLastError();
+}
+
+// Launches k_molecule_check<checks> over B molecules; checks is CHECK_CONNECTED, CHECK_VALENCE or both, N <= CONN_MAX_N.
+// The shared-memory limit is raised to its one maximum the first time a molecule needs more than the default, so
+// concurrent callers never lower it under each other.
+inline cudaError_t launch_molecule_check(int checks, const CheckArgs& a, int B, cudaStream_t st) {
+  switch (checks) {
+    case CHECK_CONNECTED: return launch_molecule_check_as<CHECK_CONNECTED>(a, B, st);
+    case CHECK_VALENCE: return launch_molecule_check_as<CHECK_VALENCE>(a, B, st);
+    case CHECK_CONNECTED | CHECK_VALENCE: return launch_molecule_check_as<CHECK_CONNECTED | CHECK_VALENCE>(a, B, st);
+    default: return cudaErrorInvalidValue;
+  }
 }
 
 }  // namespace dl

@@ -134,17 +134,8 @@ __global__ void __launch_bounds__(256) k_bond_orders(int N, int T, const float* 
     if (j < i && node_mask[g0 + i] && node_mask[g0 + j]) {
       const float* xi = x + (g0 + i) * x_stride;
       const float* xj = x + (g0 + j) * x_stride;
-      float dist;
-      const int k = dl::bond_pair(make_float3(xi[0], xi[1], xi[2]), make_float3(xj[0], xj[1], xj[2]), types[g0 + i],
-                                  types[g0 + j], T, thr1, &dist);
-      if (k >= 0) {
-        const float t2 = thr2[k], t3 = thr3[k];
-        order = 1;
-        if (t2 >= 0.f && dist < t2) {
-          order = 2;
-          if (t3 >= 0.f && dist < t3) order = 3;
-        }
-      }
+      order = (int8_t)dl::bond_order_pair(make_float3(xi[0], xi[1], xi[2]), make_float3(xj[0], xj[1], xj[2]), types[g0 + i],
+                                          types[g0 + j], T, thr1, thr2, thr3);
     }
     E[g0 * N + idx] = order;
   }

@@ -31,7 +31,9 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
     samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, conn) resamples
     the molecules that diverged (dl_sample_chain_seeded_retry, which blocks until its rounds are done) and, with `conn` =
-    (thr1, connected), those that are not connected (dl_sample_chain_seeded_retry_connected). `start` = (t0, alpha_t0,
+    (require, tables, passed), those that miss a required check: `require` = CHECK_CONNECTED with tables [thr1]
+    (dl_sample_chain_seeded_retry_connected), or any checks with [thr1, thr2, thr3, max_valence]
+    (dl_sample_chain_seeded_retry_checked). `start` = (t0, alpha_t0,
     sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of the call
     (dl_set_start_step). Returns (status, what the batch stream consumed)."""
     if start is not None:
@@ -50,10 +52,16 @@ def _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry):
     if retry is not None:
         max_retries, used, attempts, conn = retry
         if conn is not None:
-            thr1, connected = conn
-            return _native.check(lib.dl_sample_chain_seeded_retry_connected(
-                eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr(), thr1.shape[0],
-                thr1.data_ptr(), connected.data_ptr(), stream), "dl_sample_chain_seeded_retry_connected"), 0
+            require, tables, passed = conn
+            if require == _native.CHECK_CONNECTED:
+                thr1 = tables[0]
+                return _native.check(lib.dl_sample_chain_seeded_retry_connected(
+                    eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr(), thr1.shape[0],
+                    thr1.data_ptr(), passed.data_ptr(), stream), "dl_sample_chain_seeded_retry_connected"), 0
+            return _native.check(lib.dl_sample_chain_seeded_retry_checked(
+                eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr(),
+                _native.DLMoleculeChecks.of(require, tables), passed.data_ptr(), stream),
+                "dl_sample_chain_seeded_retry_checked"), 0
         return _native.check(lib.dl_sample_chain_seeded_retry(eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(),
                                                               attempts.data_ptr(), stream), "dl_sample_chain_seeded_retry"), 0
     if seeds is not None:
@@ -185,12 +193,19 @@ class EDM(torch.nn.Module):
         self.is_geom = is_geom
         self.require_connected = False
         self.last_connected = None             # calls with require_connected: the (B,) CPU bool connectivity of every row
+        # Valence: likewise for the molecules with an atom whose bond orders sum to more than its element allows
+        # (molecule_builder.max_valence_table; dl_sample_chain_seeded_retry_checked). With require_connected it is the
+        # reference's validity_and_connectivity, as far as "explicit valence within the table" is RDKit's sanitization
+        # (not verified, see molecule_builder.valence_ok). Same needs; False, the default, checks nothing.
+        self.require_valid = False
+        self.last_valid = None                 # calls with require_valid: the (B,) CPU bool valence verdict of every row
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
-        # sample_many: per request, what last_seeds / last_attempts / last_connected hold after its own sample_chain call;
-        # per launch, (device, the requests it held, loop ms)
+        # sample_many: per request, what last_seeds / last_attempts / last_connected / last_valid hold after its own
+        # sample_chain call; per launch, (device, the requests it held, loop ms)
         self.last_seeds_many = self.last_attempts_many = self.last_connected_many = self.last_loop_ms_many = None
+        self.last_valid_many = None
 
     @property
     def devices(self):
@@ -437,38 +452,52 @@ class EDM(torch.nn.Module):
             raise ValueError(f"nan_retries needs CUDA inputs (got {x.device})")
         return n
 
-    def _require_connected(self, require_connected, seeds, noise, batch_slice, x):
-        """Whether a call checks connectivity: `require_connected`, or the `require_connected` attribute when None. True
-        needs what nan_retries > 0 needs -- the per-molecule stream on CUDA inputs, no noise tensor, replaced draw function
-        or batch_slice -- and the bond tables of `is_geom`."""
-        c = self.require_connected if require_connected is None else require_connected
+    def _require_check(self, name, value, seeds, noise, batch_slice, x):
+        """Whether a call runs the molecule check `name` (require_connected or require_valid): `value`, or the attribute of
+        that name when None. True needs what nan_retries > 0 needs -- the per-molecule stream on CUDA inputs, no noise
+        tensor, replaced draw function or batch_slice -- and the bond tables of `is_geom`."""
+        c = getattr(self, name) if value is None else value
         if not isinstance(c, bool):
-            raise ValueError(f"require_connected is True or False (got {c!r})")
+            raise ValueError(f"{name} is True or False (got {c!r})")
         if not c:
             return False
         if noise is not None:
-            raise ValueError("require_connected resamples disconnected molecules with new seeds; an injected noise= tensor has "
-                             "no new draws")
+            raise ValueError(f"{name} resamples the failing molecules with new seeds; an injected noise= tensor has no new "
+                             "draws")
         if self._draws_replaced():
-            raise ValueError("require_connected needs the device-side per-molecule stream, but this model's draw function is "
-                             "replaced")
+            raise ValueError(f"{name} needs the device-side per-molecule stream, but this model's draw function is replaced")
         if batch_slice is not None:
-            raise ValueError("require_connected does not take batch_slice: pass each slice its rows of the seeds instead")
+            raise ValueError(f"{name} does not take batch_slice: pass each slice its rows of the seeds instead")
         if seeds is None and self.noise_mode != 'per_molecule':
-            raise ValueError("require_connected needs per-molecule streams: pass seeds= or set noise_mode='per_molecule' (the "
+            raise ValueError(f"{name} needs per-molecule streams: pass seeds= or set noise_mode='per_molecule' (the "
                              f"batch stream, noise_mode={self.noise_mode!r}, cannot give one molecule new draws)")
         if self.is_geom is None:
-            raise ValueError("require_connected needs the bond tables: build the EDM with is_geom=True (GEOM / MOAD atom "
+            raise ValueError(f"{name} needs the bond tables: build the EDM with is_geom=True (GEOM / MOAD atom "
                              "types) or False (ZINC), or set edm.is_geom")
         if x.device.type != 'cuda':
-            raise ValueError(f"require_connected needs CUDA inputs (got {x.device})")
+            raise ValueError(f"{name} needs CUDA inputs (got {x.device})")
         return True
+
+    def _checks(self, require_connected, require_valid, seeds, noise, batch_slice, x):
+        """The molecule checks of a call as the OR of _native.CHECK_*; 0 checks nothing."""
+        return ((_native.CHECK_CONNECTED if self._require_check('require_connected', require_connected, seeds, noise,
+                                                                batch_slice, x) else 0) |
+                (_native.CHECK_VALENCE if self._require_check('require_valid', require_valid, seeds, noise, batch_slice, x)
+                 else 0))
 
     def _bond_table(self):
         """The (T,T) fp32 single-bond thresholds of `is_geom` (molecule_builder.threshold_tables), the table that decides
         whether two atoms bond."""
         from .molecule_builder import threshold_tables
         return threshold_tables(bool(self.is_geom))[0].contiguous()
+
+    def _check_tables(self, check):
+        """The tables the checks `check` read: [thr1], and with CHECK_VALENCE [thr1, thr2, thr3, max_valence]
+        (molecule_builder.threshold_tables, max_valence_table)."""
+        if not check & _native.CHECK_VALENCE:
+            return [self._bond_table()]
+        from .molecule_builder import max_valence_table, threshold_tables
+        return [t.contiguous() for t in threshold_tables(bool(self.is_geom))] + [max_valence_table(bool(self.is_geom))]
 
     def _head(self, n_samples, n_nodes, keep_frames, t):
         ptr = lambda v: None if v is None else v.data_ptr()
@@ -480,7 +509,8 @@ class EDM(torch.nn.Module):
 
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None):
+                     noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
+                     require_valid=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -516,6 +546,13 @@ class EDM(torch.nn.Module):
         A resampled row replaces the old one unless the old one was finite and the new one diverged. Rows that are still
         disconnected after the last round are returned; `last_connected` (B,) CPU bool tells which rows are connected. It
         raises ValueError where nan_retries does, and without `is_geom`.
+        `require_valid` (None: the `require_valid` attribute, default False) adds a third, in the same rounds and with the
+        same refusals: some atom of that molecule carries more bond order -- the sum of get_bond_order over its pairs -- than
+        molecule_builder.max_valence_table allows its element (dl_sample_chain_seeded_retry_checked; both checks share one
+        launch). `last_valid` (B,) CPU bool tells which rows pass. This is "explicit valence within the table", how
+        build_molecule's molecules are expected to fail RDKit's sanitization; that has not been verified against RDKit.
+        A row whose fragments alone break the rule cannot be repaired by a new linker: it is resampled every round and
+        comes back flagged, so vet inputs with molecule_builder.valence_ok. Either flag alone or both.
         The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
         and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
         device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
@@ -528,11 +565,11 @@ class EDM(torch.nn.Module):
         n_samples = x.size(0)
         dev = x.device
         self.last_attempts = None
-        self.last_connected = None
+        self.last_connected = self.last_valid = None
         start = self._start(start_step, n_samples)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
-        check = self._require_connected(require_connected, seeds, noise, batch_slice, x)
-        recover = retries > 0 or check      # the recovery entry point: seeds used and attempts come back
+        check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x)
+        recover = retries > 0 or check != 0 # the recovery entry point: seeds used and attempts come back
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
         full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
         on_device, noise = ((False, None) if dev_seeds is not None
@@ -589,8 +626,10 @@ class EDM(torch.nn.Module):
         self.last_slice_loop_ms = loop_ms if split else None
         if recover:
             self.last_seeds, self.last_attempts = out['used'].cpu(), out['attempts'].cpu()
-        if check:
-            self.last_connected = out['connected'].cpu() != 0
+        if check & _native.CHECK_CONNECTED:
+            self.last_connected = (out['passed'].cpu() & _native.CHECK_CONNECTED) != 0
+        if check & _native.CHECK_VALENCE:
+            self.last_valid = (out['passed'].cpu() & _native.CHECK_VALENCE) != 0
         if out['bad']:
             exc = self._nan_exception(out['flags'], start)
             if recover:
@@ -603,12 +642,12 @@ class EDM(torch.nn.Module):
 
     @torch.no_grad()
     def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                    max_molecules=256, start_step=None):
+                    max_molecules=256, start_step=None, require_valid=None):
         """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
         edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
         (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
         sample_chain(**requests[k], keep_frames=keep_frames, seeds=seeds[k], nan_retries=..., require_connected=...,
-        start_step=start_step): always
+        require_valid=..., start_step=start_step): always
         on the SIMT edge path, and on the tensor-core path while no node tile rescales its fp16 operands (DESIGN.md
         section 6). It needs per-molecule streams: `seeds`, one list of B_k seeds per request, or noise_mode='per_molecule',
         which draws them with one draw_seeds(B_k) per request in request order -- the results and the generator's final
@@ -620,11 +659,11 @@ class EDM(torch.nn.Module):
         aggregation_method='mean' on FC graphs, where the reference divides by the padded N, only with requests of the same
         N. With `devices` set, whole launches are dealt to the listed devices by their cost (distributed.deal_launches), and
         each device runs its launches in order, from a host thread of its own; a launch is never split.
-        `nan_retries` and `require_connected` run their rounds inside each launch, over its rows. Rows still diverging after
+        `nan_retries`, `require_connected` and `require_valid` run their rounds inside each launch, over its rows. Rows still diverging after
         the last round raise once, after every launch: the FoundNaNException of the first such request, its index sets
         local to that request, with `request` = k and `results` = every request's chain (and `chain` = its own when rounds
-        ran, as in sample_chain). `last_seeds_many`, `last_attempts_many` and `last_connected_many` hold per request what
-        last_seeds, last_attempts and last_connected would hold after its own call; `last_loop_ms_many` holds (device,
+        ran, as in sample_chain). `last_seeds_many`, `last_attempts_many`, `last_connected_many` and `last_valid_many` hold per
+        request what last_seeds, last_attempts, last_connected and last_valid would hold after its own call; `last_loop_ms_many` holds (device,
         requests, loop ms) per launch. The single-call attributes are left as they were.
         Raises ValueError for an empty list, the batch stream (its draws depend on B and N), noise= or a replaced draw
         function, host inputs, requests on different devices or of different feature or context widths, and seeds that do
@@ -678,8 +717,8 @@ class EDM(torch.nn.Module):
         if dev.type != 'cuda':
             raise ValueError(f"sample_many needs CUDA inputs (got {dev})")
         retries = self._nan_retries(nan_retries, seeds, None, None, x0)
-        check = self._require_connected(require_connected, seeds, None, None, x0)
-        recover = retries > 0 or check
+        check = self._checks(require_connected, require_valid, seeds, None, None, x0)
+        recover = retries > 0 or check != 0
         self.dynamics._check_graph_type()
         if seeds is None:
             with torch.cuda.device(dev):    # one draw per request, in request order, as the sample_chain calls draw them
@@ -728,7 +767,8 @@ class EDM(torch.nn.Module):
                     pass
             raise
         results, flags = [None] * len(requests), [None] * len(requests)
-        seeds_many, attempts_many, connected_many = list(cpu_seeds), [None] * len(requests), [None] * len(requests)
+        seeds_many, attempts_many = list(cpu_seeds), [None] * len(requests)
+        connected_many, valid_many = [None] * len(requests), [None] * len(requests)
         for (ks, _), finish in zip(launches, finishes):
             out = finish()
             rows = [sizes[k] for k in ks]
@@ -738,14 +778,17 @@ class EDM(torch.nn.Module):
                 parts['used'] = unpack_rows(out['used'].cpu(), rows, None)
                 parts['attempts'] = unpack_rows(out['attempts'].cpu(), rows, None)
             if check:
-                parts['connected'] = unpack_rows(out['connected'].cpu() != 0, rows, None)
+                parts['passed'] = unpack_rows(out['passed'].cpu(), rows, None)
             for j, k in enumerate(ks):
                 results[k], flags[k] = parts['chain'][j], parts['flags'][j]
                 if recover:
                     seeds_many[k], attempts_many[k] = parts['used'][j], parts['attempts'][j]
-                if check:
-                    connected_many[k] = parts['connected'][j]
+                if check & _native.CHECK_CONNECTED:
+                    connected_many[k] = (parts['passed'][j] & _native.CHECK_CONNECTED) != 0
+                if check & _native.CHECK_VALENCE:
+                    valid_many[k] = (parts['passed'][j] & _native.CHECK_VALENCE) != 0
         self.last_seeds_many, self.last_attempts_many, self.last_connected_many = seeds_many, attempts_many, connected_many
+        self.last_valid_many = valid_many
         self.last_loop_ms_many = [(slots[slot_of[i]][0], sorted(ks), loop_ms[i]) for i, (ks, _) in enumerate(launches)]
         for k, f in enumerate(flags):
             if f.any():
@@ -767,29 +810,30 @@ class EDM(torch.nn.Module):
         return coefs, starts, keys
 
     def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
-                       retries=0, check=False, start=None):
+                       retries=0, check=0, start=None):
         """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
         inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
         replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
         covers the batch where it is. The draws are the per-molecule `dev_seeds`, the batch stream `rng` = (seed, offset,
-        b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _require_connected; `start`
-        as returned by _start.
+        b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _checks; `start` as
+        returned by _start.
         Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
         (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
-        back and returns dict(chain, flags, used, attempts, connected, bad, consumed) on `dev`. `bad` reads the flags: one
+        back and returns dict(chain, flags, used, attempts, passed, bad, consumed) on `dev`; `passed` holds
+        every row's _native.CHECK_* verdict bits. `bad` reads the flags: one
         synchronisation, after every loop and copy."""
         n_samples, n_nodes = full['x'].shape[:2]
         d = self.n_dims + self.in_node_nf
-        recover = retries > 0 or check
+        recover = retries > 0 or check != 0
         norm = self._norm()
         chain = torch.empty((keep_frames, n_samples, n_nodes, d), device=dev, dtype=torch.float32)
         flags = torch.zeros(n_samples, dtype=torch.int32, device=dev)
         # recovery: the seed that produced every row and its attempt
         used, attempts = ((torch.empty(n_samples, dtype=torch.int64, device=dev), torch.empty(n_samples, dtype=torch.int32, device=dev))
                           if recover else (None, None))
-        # connectivity: every row's flag, and the bond table on each slice's device
-        connected = torch.empty(n_samples, dtype=torch.int32, device=dev) if check else None
-        thr1 = self._bond_table() if check else None
+        # molecule checks: every row's verdict bits, and the tables they read on each slice's device
+        passed = torch.empty(n_samples, dtype=torch.int32, device=dev) if check else None
+        tables = self._check_tables(check) if check else None
         whole = places == [dev]             # one slice, the whole batch where it is: it samples the caller's tensors
         results, calls, parts = [], [], []  # (status, consumed) of every slice; every slice's call; every slice's tensors
 
@@ -797,7 +841,7 @@ class EDM(torch.nn.Module):
             results.append(_sample_slice(lib, *args))
         for (dev_i, _, lo, hi), eng, where in zip(slices, engines, places):
             if whole:
-                part = (full, noise, dev_seeds, chain, flags, used, attempts, connected)
+                part = (full, noise, dev_seeds, chain, flags, used, attempts, passed)
             else:
                 to = lambda v: None if v is None else v.to(where).contiguous()
                 with torch.cuda.device(where):
@@ -808,15 +852,15 @@ class EDM(torch.nn.Module):
                             *((torch.empty(hi - lo, dtype=torch.int64, device=where),
                                torch.empty(hi - lo, dtype=torch.int32, device=where)) if recover else (None, None)),
                             torch.empty(hi - lo, dtype=torch.int32, device=where) if check else None)
-            part = part + (None if thr1 is None else thr1.to(where),)
+            part = part + (None if tables is None else [t.to(where) for t in tables],)
             parts.append(part)              # alive until the flags have been read below
-            t, nz, sd, chain_i, flags_i, used_i, attempts_i, connected_i, thr1_i = part
+            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, tables_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
             rng_i = None if rng is None else (rng[0], rng[1], rng[2] + lo, rng[3])
             calls.append((dev_i, functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
-                (retries, used_i, attempts_i, (thr1_i, connected_i) if check else None) if recover else None, start)))
+                (retries, used_i, attempts_i, (check, tables_i, passed_i) if check else None) if recover else None, start)))
 
         def finish():
             if not whole:
@@ -826,11 +870,11 @@ class EDM(torch.nn.Module):
                     place_rows(used, [p[5] for p in parts], slices)
                     place_rows(attempts, [p[6] for p in parts], slices)
                 if check:
-                    place_rows(connected, [p[7] for p in parts], slices)
+                    place_rows(passed, [p[7] for p in parts], slices)
             # the host sampler reports NaNs in its status; on the device, one sync per chain instead of one per step
             # (egnn.py:441), after every slice's loop and copy
             bad = _native.DL_NAN_DETECTED in [st for st, _ in results] or bool(flags.any().item())
-            return dict(chain=chain, flags=flags, used=used, attempts=attempts, connected=connected, bad=bad,
+            return dict(chain=chain, flags=flags, used=used, attempts=attempts, passed=passed, bad=bad,
                         consumed=[c for _, c in results])
         return calls, finish
 
@@ -887,19 +931,20 @@ class InpaintingEDM(EDM):
         return None
 
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
-                     noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None):
+                     noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
+                     require_valid=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
         (dl_sample_chain_rng), unless `draw_noise_inpaint` is replaced -- on the instance, in a subclass or on the class --
         in which case the replacement draws them. `batch_slice=(b0, B_full)` and `seeds` as in EDM.sample_chain: with
         seeds, molecule b's 2T+3 raw draws are those of the molecule sampled alone after torch.cuda.manual_seed(seeds[b]),
-        masked and projected per molecule as always. `nan_retries` and `require_connected` as in EDM.sample_chain; the
-        connectivity check covers every atom of the molecule. `start_step` raises ValueError unless None."""
+        masked and projected per molecule as always. `nan_retries`, `require_connected` and `require_valid` as in EDM.sample_chain;
+        the checks cover every atom of the molecule. `start_step` raises ValueError unless None."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
-                                    require_connected=require_connected, start_step=start_step)
+                                    require_connected=require_connected, start_step=start_step, require_valid=require_valid)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

@@ -1,7 +1,8 @@
 """Bond inference: `src/molecule_builder.py::build_xae_molecule` / `get_bond_order` (lines 44-102) for whole batches on the
 GPU (`dl_bond_orders`) instead of an O(n^2) Python loop with one `.item()` per atom pair.
 RDKit molecule construction (`build_molecule`, molecule_builder.py:29-42) stays with the caller: RDKit is not part of
-the path (SURVEY.md section 8(f) rank 4).
+the path (SURVEY.md section 8(f) rank 4). `connected` and `valence_ok` decide on the device what the reference's
+`validity_and_connectivity` asks of those molecules, the latter as "explicit valence within a table".
 """
 import torch
 
@@ -22,6 +23,9 @@ DOUBLE = {('C', 'C'): 134, ('C', 'O'): 120, ('C', 'N'): 129, ('C', 'S'): 160, ('
           ('O', 'P'): 150, ('N', 'N'): 125, ('S', 'P'): 186}
 TRIPLE = {('C', 'C'): 120, ('C', 'O'): 113, ('C', 'N'): 116, ('N', 'N'): 110}
 MARGINS_EDM = [10, 5, 2]                                                                   # src/const.py:180
+# The most bond order an atom of each element may carry in valences / valence_ok: the largest entry of RDKit's default
+# valence list for the element.
+MAX_VALENCE = {'C': 4, 'N': 3, 'O': 2, 'F': 1, 'S': 6, 'Cl': 1, 'Br': 1, 'I': 5, 'P': 7}
 
 
 def threshold_tables(is_geom, margins=MARGINS_EDM):
@@ -38,6 +42,12 @@ def threshold_tables(is_geom, margins=MARGINS_EDM):
                     t[a, c] = float(v + margin)
         out.append(t)
     return out
+
+
+def max_valence_table(is_geom):
+    """(T,) int32: MAX_VALENCE by atom type index (IDX2ATOM, or GEOM_IDX2ATOM with is_geom)."""
+    idx2atom = GEOM_IDX2ATOM if is_geom else IDX2ATOM
+    return torch.tensor([MAX_VALENCE[idx2atom[t]] for t in range(len(idx2atom))], dtype=torch.int32)
 
 
 @torch.no_grad()
@@ -84,6 +94,49 @@ def connected(xh, node_mask, is_geom, pocket_only=None):
                                                 None if po is None else po.data_ptr(), 1, int(po is not None),
                                                 t1.data_ptr(), out.data_ptr(), st), "dl_molecule_connected")
     return out != 0
+
+
+@torch.no_grad()
+def _molecule_check(xh, node_mask, is_geom, pocket_only, max_valence, require, want_valence):
+    """dl_molecule_check on a chain[0]-style batch: ((B,) int32 verdict bits, (B,N) int32 valences or None)."""
+    dev = xh.device
+    if dev.type != 'cuda':
+        raise RuntimeError("the molecule checks run on the GPU (no CPU fallback); move the tensors to the device")
+    B, N = xh.shape[:2]
+    xs = xh.float().contiguous()
+    nm = (node_mask.reshape(B, N) != 0).to(torch.int8).contiguous()
+    po = None if pocket_only is None else pocket_only.reshape(B, N, 1).float().contiguous()
+    mv = max_valence_table(is_geom) if max_valence is None else torch.as_tensor(max_valence).to(torch.int32)
+    tables = [t.to(dev).contiguous() for t in threshold_tables(is_geom)] + [mv.to(dev).contiguous()]
+    if tables[3].shape != (tables[0].shape[0],):
+        raise ValueError(f"max_valence holds one entry per atom type, {tables[0].shape[0]} (got shape {tuple(tables[3].shape)})")
+    checks = _native.DLMoleculeChecks.of(require, tables)
+    passed = torch.empty(B, dtype=torch.int32, device=dev)
+    valence = torch.empty((B, N), dtype=torch.int32, device=dev) if want_valence else None
+    lib = _native.load_library()
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream().cuda_stream
+        _native.check(lib.dl_molecule_check(B, N, checks, xs.data_ptr(), xs.shape[2], nm.data_ptr(),
+                                            None if po is None else po.data_ptr(), 1, int(po is not None), passed.data_ptr(),
+                                            None if valence is None else valence.data_ptr(), st), "dl_molecule_check")
+    return passed, valence
+
+
+def valences(xh, node_mask, is_geom, pocket_only=None, max_valence=None):
+    """(B,N) int32 on the device: every checked atom's valence -- the sum of get_bond_order over its pairs with the other
+    checked atoms, i.e. the row-plus-column sum of bond_orders' E -- and 0 on the other rows (dl_molecule_check, the check
+    behind sample_chain(require_valid=True)). `xh`, `node_mask`, `pocket_only` and the checked atoms as in connected()."""
+    return _molecule_check(xh, node_mask, is_geom, pocket_only, max_valence, _native.CHECK_VALENCE, True)[1]
+
+
+def valence_ok(xh, node_mask, is_geom, pocket_only=None, max_valence=None):
+    """(B,) bool on the device: whether every checked atom of a molecule has valence <= max_valence[its type]; a molecule
+    without atoms passes. `max_valence` is a (T,) integer table by atom type index, by default max_valence_table(is_geom).
+    This is "explicit valence within the table" on bond_orders' own orders. The molecules build_molecule makes carry single,
+    double and triple bonds only, no aromatic flags and no formal charges, so it is how they are expected to fail
+    Chem.SanitizeMol; that equivalence has not been verified against RDKit."""
+    passed, _ = _molecule_check(xh, node_mask, is_geom, pocket_only, max_valence, _native.CHECK_VALENCE, False)
+    return (passed & _native.CHECK_VALENCE) != 0
 
 
 def build_xae_molecule(positions, atom_types, is_geom, margins=MARGINS_EDM):
