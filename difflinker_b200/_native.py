@@ -71,9 +71,6 @@ SYMBOLS = {
     "dl_retry_seed": (C.c_uint64, [C.c_uint64, _I32]),
     "dl_sample_chain_seeded_retry": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32,
                                             _P, _P, _P]),
-    "dl_sample_chain_seeded_retry_connected": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
-                                                      _P, _I32, _P, _P, _I32, _P, _P, _P]),
-    "dl_molecule_connected": (_I32, [_I32, _I32, _I32, _P, _I32, _P, _P, _I32, _I32, _P, _P, _P]),
     "dl_sample_chain_seeded_retry_checked": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                                     _P, _I32, _P, _P, C.POINTER(DLMoleculeChecks), _P, _P]),
     "dl_molecule_check": (_I32, [_I32, _I32, C.POINTER(DLMoleculeChecks), _P, _I32, _P, _P, _I32, _I32, _P, _P, _P]),

@@ -1311,29 +1311,6 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
                       coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, nullptr, nullptr, stream);
 }
 
-dl_status dl_sample_chain_seeded_retry_connected(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
-                                                 int32_t keep_frames, const float* xh, const int8_t* node_mask,
-                                                 const float* fragment_mask, const float* linker_mask,
-                                                 const int8_t* edge_mask, const float* context, const uint64_t* seeds,
-                                                 const dl_step_coef* coef, const float* norm, float* chain, int32_t* nan_flags,
-                                                 int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
-                                                 int32_t n_types, const float* thr1, int32_t* connected, void* stream) {
-  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
-  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
-  if (!nan_flags || !seeds_used || !attempts || !thr1 || !connected) {
-    set_err("null argument (nan_flags, seeds_used, attempts, thr1 or connected)");
-    return DL_ERR_INVALID;
-  }
-  if (n_types < 1 || n_types > e->cfg.in_node_nf) {
-    set_err("n_types must be in [1, in_node_nf = %d] (got %d)", e->cfg.in_node_nf, n_types);
-    return DL_ERR_INVALID;
-  }
-  if (N > CONN_MAX_N) { set_err("the connectivity check takes N <= %d (got %d)", CONN_MAX_N, N); return DL_ERR_INVALID; }
-  const dl_molecule_checks ck{DL_CHECK_CONNECTED, n_types, thr1, nullptr, nullptr, nullptr};
-  return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
-                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, &ck, connected, stream);
-}
-
 dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
                                                int32_t keep_frames, const float* xh, const int8_t* node_mask,
                                                const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
@@ -1353,20 +1330,6 @@ dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, in
   }
   return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
                       coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, passed, stream);
-}
-
-dl_status dl_molecule_connected(int32_t B, int32_t N, int32_t n_types, const float* xh, int32_t xh_row_stride,
-                                const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
-                                const float* thr1, int32_t* connected, void* stream) {
-  if (B <= 0 || N <= 0 || N > CONN_MAX_N || n_types < 1 || xh_row_stride < 3 + n_types || !xh || !node_mask || !thr1 ||
-      !connected || (drop_pocket && (!context || context_nf < 1))) {
-    set_err("dl_molecule_connected: invalid argument");
-    return DL_ERR_INVALID;
-  }
-  const dl_molecule_checks ck{DL_CHECK_CONNECTED, n_types, thr1, nullptr, nullptr, nullptr};
-  CK(launch_molecule_check(ck.require, check_args(ck, xh, N, xh_row_stride, node_mask, context, context_nf, drop_pocket != 0,
-                                                  connected), B, reinterpret_cast<cudaStream_t>(stream)));
-  return DL_OK;
 }
 
 dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,

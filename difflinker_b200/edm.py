@@ -17,6 +17,7 @@ import torch.nn.functional as F
 from . import _native
 from .distributed import (deal_launches, device_slices, pack_requests, place_rows, plan_launches, resolve_devices,
                           slice_sampler_inputs, unpack_rows)
+from .molecule_builder import check_tables
 from .noise import PredefinedNoiseSchedule
 from .utils import FoundNaNException, nan_exception_class
 
@@ -29,13 +30,12 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
-    samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, conn) resamples
-    the molecules that diverged (dl_sample_chain_seeded_retry, which blocks until its rounds are done) and, with `conn` =
-    (require, tables, passed), those that miss a required check: `require` = CHECK_CONNECTED with tables [thr1]
-    (dl_sample_chain_seeded_retry_connected), or any checks with [thr1, thr2, thr3, max_valence]
-    (dl_sample_chain_seeded_retry_checked). `start` = (t0, alpha_t0,
-    sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of the call
-    (dl_set_start_step). Returns (status, what the batch stream consumed)."""
+    samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, require, tables,
+    passed) resamples the molecules that diverged (dl_sample_chain_seeded_retry, which blocks until its rounds are done)
+    and, with `require` != 0, those that miss a required check, whose verdict bits go to `passed`
+    (dl_sample_chain_seeded_retry_checked; `tables` as molecule_builder.check_tables returns them, on the slice's device).
+    `start` = (t0, alpha_t0, sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of
+    the call (dl_set_start_step). Returns (status, what the batch stream consumed)."""
     if start is not None:
         _native.check(lib.dl_set_start_step(eng, *start), "dl_set_start_step")
     try:
@@ -50,20 +50,13 @@ def _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry):
     if stream is None:
         return _native.check(lib.dl_sample_chain_host(eng, *head, noise.data_ptr(), *tail), "dl_sample_chain_host"), 0
     if retry is not None:
-        max_retries, used, attempts, conn = retry
-        if conn is not None:
-            require, tables, passed = conn
-            if require == _native.CHECK_CONNECTED:
-                thr1 = tables[0]
-                return _native.check(lib.dl_sample_chain_seeded_retry_connected(
-                    eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr(), thr1.shape[0],
-                    thr1.data_ptr(), passed.data_ptr(), stream), "dl_sample_chain_seeded_retry_connected"), 0
-            return _native.check(lib.dl_sample_chain_seeded_retry_checked(
-                eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr(),
-                _native.DLMoleculeChecks.of(require, tables), passed.data_ptr(), stream),
-                "dl_sample_chain_seeded_retry_checked"), 0
-        return _native.check(lib.dl_sample_chain_seeded_retry(eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(),
-                                                              attempts.data_ptr(), stream), "dl_sample_chain_seeded_retry"), 0
+        max_retries, used, attempts, require, tables, passed = retry
+        args = (eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr())
+        if not require:
+            return _native.check(lib.dl_sample_chain_seeded_retry(*args, stream), "dl_sample_chain_seeded_retry"), 0
+        return _native.check(lib.dl_sample_chain_seeded_retry_checked(
+            *args, _native.DLMoleculeChecks.of(require, tables), passed.data_ptr(), stream),
+            "dl_sample_chain_seeded_retry_checked"), 0
     if seeds is not None:
         return _native.check(lib.dl_sample_chain_seeded(eng, *head, seeds.data_ptr(), *tail, stream),
                              "dl_sample_chain_seeded"), 0
@@ -187,14 +180,14 @@ class EDM(torch.nn.Module):
         self.nan_retries = 0
         self.last_attempts = None              # calls with nan_retries > 0: the (B,) CPU int32 attempt of every row, else None
         # Connectivity: sample_chain also resamples, in the nan_retries rounds, the molecules whose final molecule is in more
-        # than one piece (dl_sample_chain_seeded_retry_connected); needs per-molecule streams and the bond tables of
+        # than one piece (dl_sample_chain_seeded_retry_checked); needs per-molecule streams and the bond tables of
         # `is_geom` (the ZINC or the GEOM / MOAD atom types, molecule_builder.threshold_tables), which DDPM, accelerate and
         # load_from_checkpoint set from the model's training data. False, the default, checks nothing.
         self.is_geom = is_geom
         self.require_connected = False
         self.last_connected = None             # calls with require_connected: the (B,) CPU bool connectivity of every row
         # Valence: likewise for the molecules with an atom whose bond orders sum to more than its element allows
-        # (molecule_builder.max_valence_table; dl_sample_chain_seeded_retry_checked). With require_connected it is the
+        # (molecule_builder.max_valence_table), in the same check launch. With require_connected it is the
         # reference's validity_and_connectivity, as far as "explicit valence within the table" is RDKit's sanitization
         # (not verified, see molecule_builder.valence_ok). Same needs; False, the default, checks nothing.
         self.require_valid = False
@@ -439,18 +432,23 @@ class EDM(torch.nn.Module):
             raise ValueError(f"nan_retries {n} does not fit an int32")
         if n == 0:
             return 0
-        if noise is not None:
-            raise ValueError("nan_retries resamples diverged molecules with new seeds; an injected noise= tensor has no new draws")
-        if self._draws_replaced():
-            raise ValueError("nan_retries needs the device-side per-molecule stream, but this model's draw function is replaced")
-        if batch_slice is not None:
-            raise ValueError("nan_retries does not take batch_slice: pass each slice its rows of the seeds instead")
-        if seeds is None and self.noise_mode != 'per_molecule':
-            raise ValueError("nan_retries needs per-molecule streams: pass seeds= or set noise_mode='per_molecule' (the batch "
-                             f"stream, noise_mode={self.noise_mode!r}, cannot give one molecule new draws)")
+        self._refuse_without_new_draws('nan_retries', seeds, noise, batch_slice)
         if x.device.type != 'cuda':
             raise ValueError(f"nan_retries needs CUDA inputs (got {x.device})")
         return n
+
+    def _refuse_without_new_draws(self, name, seeds, noise, batch_slice):
+        """Raises ValueError when the option `name` (nan_retries, require_connected or require_valid) could not give one
+        molecule new draws: it needs the per-molecule stream, and no noise tensor, replaced draw function or batch_slice."""
+        if noise is not None:
+            raise ValueError(f"{name} resamples molecules with new seeds; an injected noise= tensor has no new draws")
+        if self._draws_replaced():
+            raise ValueError(f"{name} needs the device-side per-molecule stream, but this model's draw function is replaced")
+        if batch_slice is not None:
+            raise ValueError(f"{name} does not take batch_slice: pass each slice its rows of the seeds instead")
+        if seeds is None and self.noise_mode != 'per_molecule':
+            raise ValueError(f"{name} needs per-molecule streams: pass seeds= or set noise_mode='per_molecule' (the "
+                             f"batch stream, noise_mode={self.noise_mode!r}, cannot give one molecule new draws)")
 
     def _require_check(self, name, value, seeds, noise, batch_slice, x):
         """Whether a call runs the molecule check `name` (require_connected or require_valid): `value`, or the attribute of
@@ -461,16 +459,7 @@ class EDM(torch.nn.Module):
             raise ValueError(f"{name} is True or False (got {c!r})")
         if not c:
             return False
-        if noise is not None:
-            raise ValueError(f"{name} resamples the failing molecules with new seeds; an injected noise= tensor has no new "
-                             "draws")
-        if self._draws_replaced():
-            raise ValueError(f"{name} needs the device-side per-molecule stream, but this model's draw function is replaced")
-        if batch_slice is not None:
-            raise ValueError(f"{name} does not take batch_slice: pass each slice its rows of the seeds instead")
-        if seeds is None and self.noise_mode != 'per_molecule':
-            raise ValueError(f"{name} needs per-molecule streams: pass seeds= or set noise_mode='per_molecule' (the "
-                             f"batch stream, noise_mode={self.noise_mode!r}, cannot give one molecule new draws)")
+        self._refuse_without_new_draws(name, seeds, noise, batch_slice)
         if self.is_geom is None:
             raise ValueError(f"{name} needs the bond tables: build the EDM with is_geom=True (GEOM / MOAD atom "
                              "types) or False (ZINC), or set edm.is_geom")
@@ -485,19 +474,9 @@ class EDM(torch.nn.Module):
                 (_native.CHECK_VALENCE if self._require_check('require_valid', require_valid, seeds, noise, batch_slice, x)
                  else 0))
 
-    def _bond_table(self):
-        """The (T,T) fp32 single-bond thresholds of `is_geom` (molecule_builder.threshold_tables), the table that decides
-        whether two atoms bond."""
-        from .molecule_builder import threshold_tables
-        return threshold_tables(bool(self.is_geom))[0].contiguous()
-
     def _check_tables(self, check):
-        """The tables the checks `check` read: [thr1], and with CHECK_VALENCE [thr1, thr2, thr3, max_valence]
-        (molecule_builder.threshold_tables, max_valence_table)."""
-        if not check & _native.CHECK_VALENCE:
-            return [self._bond_table()]
-        from .molecule_builder import max_valence_table, threshold_tables
-        return [t.contiguous() for t in threshold_tables(bool(self.is_geom))] + [max_valence_table(bool(self.is_geom))]
+        """The CPU tables the checks `check` read with this model's atom types (molecule_builder.check_tables)."""
+        return check_tables(self.is_geom, check)
 
     def _head(self, n_samples, n_nodes, keep_frames, t):
         ptr = lambda v: None if v is None else v.data_ptr()
@@ -541,15 +520,14 @@ class EDM(torch.nn.Module):
         round raise FoundNaNException with their batch-global indices only; its `chain` attribute holds the recovered chain.
         `require_connected` (None: the `require_connected` attribute, default False) adds a second reason to resample a row:
         its final molecule -- chain[0]'s atoms, without the pocket on cut-off graphs, bonded where get_bond_order > 0 with
-        the tables of `is_geom` -- is in more than one piece (dl_sample_chain_seeded_retry_connected). The check runs on the
+        the tables of `is_geom` -- is in more than one piece (dl_sample_chain_seeded_retry_checked). The check runs on the
         device after the loop and after every round; the rounds are the nan_retries rounds, so nan_retries=0 only reports.
         A resampled row replaces the old one unless the old one was finite and the new one diverged. Rows that are still
         disconnected after the last round are returned; `last_connected` (B,) CPU bool tells which rows are connected. It
         raises ValueError where nan_retries does, and without `is_geom`.
         `require_valid` (None: the `require_valid` attribute, default False) adds a third, in the same rounds and with the
         same refusals: some atom of that molecule carries more bond order -- the sum of get_bond_order over its pairs -- than
-        molecule_builder.max_valence_table allows its element (dl_sample_chain_seeded_retry_checked; both checks share one
-        launch). `last_valid` (B,) CPU bool tells which rows pass. This is "explicit valence within the table", how
+        molecule_builder.max_valence_table allows its element (both checks share one launch). `last_valid` (B,) CPU bool tells which rows pass. This is "explicit valence within the table", how
         build_molecule's molecules are expected to fail RDKit's sanitization; that has not been verified against RDKit.
         A row whose fragments alone break the rule cannot be repaired by a new linker: it is resampled every round and
         comes back flagged, so vet inputs with molecule_builder.valence_ok. Either flag alone or both.
@@ -860,7 +838,7 @@ class EDM(torch.nn.Module):
             calls.append((dev_i, functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
-                (retries, used_i, attempts_i, (check, tables_i, passed_i) if check else None) if recover else None, start)))
+                (retries, used_i, attempts_i, check, tables_i, passed_i) if recover else None, start)))
 
         def finish():
             if not whole:

@@ -50,6 +50,19 @@ def max_valence_table(is_geom):
     return torch.tensor([MAX_VALENCE[idx2atom[t]] for t in range(len(idx2atom))], dtype=torch.int32)
 
 
+def check_tables(is_geom, require, max_valence=None):
+    """The CPU tables the molecule checks `require` (an OR of _native.CHECK_*) read: [thr1] for connectivity alone, and
+    [thr1, thr2, thr3, max_valence] once CHECK_VALENCE is required (threshold_tables; `max_valence` a (T,) integer table by
+    atom type index, by default max_valence_table(is_geom))."""
+    thr = threshold_tables(is_geom)
+    if not require & _native.CHECK_VALENCE:
+        return thr[:1]
+    mv = max_valence_table(is_geom) if max_valence is None else torch.as_tensor(max_valence).to(torch.int32).contiguous()
+    if mv.shape != (thr[0].shape[0],):
+        raise ValueError(f"max_valence holds one entry per atom type, {thr[0].shape[0]} (got shape {tuple(mv.shape)})")
+    return thr + [mv]
+
+
 @torch.no_grad()
 def bond_orders(one_hot, x, node_mask, is_geom, margins=MARGINS_EDM):
     """Batched E of build_xae_molecule: (B,N,N) int8 on the inputs' device, E[b,i,j] (i > j) = bond order, else 0.
@@ -73,27 +86,13 @@ def bond_orders(one_hot, x, node_mask, is_geom, margins=MARGINS_EDM):
 
 @torch.no_grad()
 def connected(xh, node_mask, is_geom, pocket_only=None):
-    """(B,) bool on the device: whether each molecule is in one piece (dl_molecule_connected, the check behind
-    sample_chain(require_connected=True)). Its atoms are the rows with node_mask != 0, minus those with pocket_only != 0
-    when given; atoms i and j bond iff get_bond_order > 0, i.e. E[i, j] != 0 of bond_orders. `xh` is chain[0]-style
-    (B,N,3+F): the atom types are argmax of its first T feature columns (T = 9 with is_geom, else 8). One atom is
-    connected, none is not."""
-    dev = xh.device
-    if dev.type != 'cuda':
-        raise RuntimeError("connected runs on the GPU (no CPU fallback); move the tensors to the device")
-    B, N = xh.shape[:2]
-    xs = xh.float().contiguous()
-    nm = (node_mask.reshape(B, N) != 0).to(torch.int8).contiguous()
-    po = None if pocket_only is None else pocket_only.reshape(B, N, 1).float().contiguous()
-    t1 = threshold_tables(is_geom)[0].to(dev).contiguous()
-    out = torch.empty(B, dtype=torch.int32, device=dev)
-    lib = _native.load_library()
-    with torch.cuda.device(dev):
-        st = torch.cuda.current_stream().cuda_stream
-        _native.check(lib.dl_molecule_connected(B, N, t1.shape[0], xs.data_ptr(), xs.shape[2], nm.data_ptr(),
-                                                None if po is None else po.data_ptr(), 1, int(po is not None),
-                                                t1.data_ptr(), out.data_ptr(), st), "dl_molecule_connected")
-    return out != 0
+    """(B,) bool on the device: whether each molecule is in one piece (dl_molecule_check with CHECK_CONNECTED, the check
+    behind sample_chain(require_connected=True)). Its atoms are the rows with node_mask != 0, minus those with
+    pocket_only != 0 when given; atoms i and j bond iff get_bond_order > 0, i.e. E[i, j] != 0 of bond_orders. `xh` is
+    chain[0]-style (B,N,3+F): the atom types are argmax of its first T feature columns (T = 9 with is_geom, else 8). One
+    atom is connected, none is not."""
+    passed, _ = _molecule_check(xh, node_mask, is_geom, pocket_only, None, _native.CHECK_CONNECTED, False)
+    return (passed & _native.CHECK_CONNECTED) != 0
 
 
 @torch.no_grad()
@@ -106,10 +105,7 @@ def _molecule_check(xh, node_mask, is_geom, pocket_only, max_valence, require, w
     xs = xh.float().contiguous()
     nm = (node_mask.reshape(B, N) != 0).to(torch.int8).contiguous()
     po = None if pocket_only is None else pocket_only.reshape(B, N, 1).float().contiguous()
-    mv = max_valence_table(is_geom) if max_valence is None else torch.as_tensor(max_valence).to(torch.int32)
-    tables = [t.to(dev).contiguous() for t in threshold_tables(is_geom)] + [mv.to(dev).contiguous()]
-    if tables[3].shape != (tables[0].shape[0],):
-        raise ValueError(f"max_valence holds one entry per atom type, {tables[0].shape[0]} (got shape {tuple(tables[3].shape)})")
+    tables = [t.to(dev) for t in check_tables(is_geom, require, max_valence)]
     checks = _native.DLMoleculeChecks.of(require, tables)
     passed = torch.empty(B, dtype=torch.int32, device=dev)
     valence = torch.empty((B, N), dtype=torch.int32, device=dev) if want_valence else None

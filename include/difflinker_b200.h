@@ -22,9 +22,8 @@
  *     at step t0 (partial diffusion, no reference API)
  *   either, resampling only the molecules that diverged  dl_sample_chain_seeded_retry, dl_retry_seed, dl_last_retry_ms
  *     (the reference's callers resample the whole batch, generate.py:153-161)
- *   either, also resampling the disconnected molecules  dl_sample_chain_seeded_retry_connected, dl_molecule_connected
- *     (is_connected, src/metrics.py:20-27, on the molecules of src/lightning.py:364-377)
- *   either, also resampling the molecules with an atom   dl_sample_chain_seeded_retry_checked, dl_molecule_check
+ *   either, also resampling the molecules that are      dl_sample_chain_seeded_retry_checked, dl_molecule_check
+ *     disconnected (is_connected, src/metrics.py:20-27, on the molecules of src/lightning.py:364-377) or have an atom
  *     beyond its valence (the explicit-valence part of validity, src/metrics.py:12-17; see dl_molecule_checks)
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   build_xae_molecule           src/molecule_builder.py:44-102       dl_bond_orders
@@ -250,61 +249,24 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
                                        int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
                                        void* stream);
 /*
- * dl_sample_chain_seeded_retry that also resamples the molecules whose final molecule is in more than one piece -- the
- * reference's `is_connected` (src/metrics.py:20-27) on what src/lightning.py:364-377 builds from chain[0]:
- *   atoms     molecule b's rows with node_mask != 0; on cut-off (pocket) graphs, graph_type != DL_GRAPH_FC, minus the pocket
- *             atoms, the rows whose last context column (pocket_only, src/egnn.py:486-487) is non-zero (lightning.py:372-374).
- *             Inpainting models are checked over all their atoms.
- *   bonds     atoms i and j bond iff get_bond_order(...) > 0 (src/molecule_builder.py:77-102): with the types t = argmax of
- *             the first n_types columns of h (the first maximum), 100 |x_i - x_j| < thr1[min t][max t] and that entry
- *             >= 0 -- the arithmetic of dl_bond_orders, whose E != 0 is exactly this relation.
- *   connected the graph of those atoms and bonds has exactly one component (one atom is connected; no atom is not), i.e.
- *             len(Chem.GetMolFrags(mol)) == 1 for build_molecule's molecule. The AtomValenceException branch of
- *             is_connected, which needs RDKit's valence model, is not reproduced; the reference applies is_connected to
- *             sanitized molecules only (metrics.py:103-104), and for those the two agree. DL_CHECK_VALENCE of
- *             dl_molecule_checks is the explicit-valence test on the same atoms and bonds.
- * The check runs on the device after the seeded loop and after each round. A row fails if its NaN flag is set or it is not
- * connected; rounds gather, resample and write back failing rows as dl_sample_chain_seeded_retry does, except that a
- * resampled row does not replace a finite row with one that diverged. Rows that are only disconnected after the last round
- * are valid samples: they are returned with connected[b] = 0 and do not make the call fail. DL_NAN_DETECTED means, as there,
- * that some row still diverges. max_retries = 0 only reports connectivity.
- *   n_types    columns of h that hold the atom type (the one-hot width without charges); 1 <= n_types <= in_node_nf
- *   thr1       (n_types,n_types) fp32 DEVICE: single-bond thresholds in pm, [min type][max type], negative = no bond
- *              (dl_bond_orders' thr1; molecule_builder.threshold_tables)
- *   connected  (B) int32 DEVICE out: 1 if row b's returned molecule is connected, else 0
- * N <= 8192.
- */
-dl_status dl_sample_chain_seeded_retry_connected(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
-                                                 int32_t keep_frames, const float* xh, const int8_t* node_mask,
-                                                 const float* fragment_mask, const float* linker_mask,
-                                                 const int8_t* edge_mask, const float* context, const uint64_t* seeds,
-                                                 const dl_step_coef* coef, const float* norm, float* chain, int32_t* nan_flags,
-                                                 int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
-                                                 int32_t n_types, const float* thr1, int32_t* connected, void* stream);
-/*
- * The connectivity check of dl_sample_chain_seeded_retry_connected alone, on any (B,N) batch: connected[b] = 1 iff the
- * atoms of molecule b form one component under the bond relation above. DEVICE buffers, enqueued on `stream`.
- *   xh          (B,N,>=3+n_types) fp32, row stride xh_row_stride: x at columns 0..2, the atom-type one-hot from column 3
- *   node_mask   (B,N) int8
- *   context     (B,N,context_nf) fp32; with drop_pocket != 0 the rows whose column context_nf - 1 is non-zero are not atoms
- *               (read only then; may be NULL otherwise)
- *   thr1, n_types, connected as above. 1 <= N <= 8192.
- */
-dl_status dl_molecule_connected(int32_t B, int32_t N, int32_t n_types, const float* xh, int32_t xh_row_stride,
-                                const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
-                                const float* thr1, int32_t* connected, void* stream);
-/*
- * The checks a molecule can be put to, as data: connectivity (above) and valence. Both are evaluated on the device, on the
- * same atoms and with the arithmetic of dl_bond_orders.
- *   atoms      exactly those of the connectivity check: molecule b's rows with node_mask != 0; on cut-off (pocket) graphs minus
- *              the rows whose last context column (pocket_only) is non-zero; inpainting models over all their atoms. Types
- *              are the first argmax of the first n_types feature columns, NaN winning.
+ * The checks a molecule can be put to, as data: connectivity and valence. Both are evaluated on the device, on the same atoms
+ * and with the arithmetic of dl_bond_orders, on what src/lightning.py:364-377 builds from chain[0].
+ *   atoms      molecule b's rows with node_mask != 0; on cut-off (pocket) graphs, graph_type != DL_GRAPH_FC, minus the pocket
+ *              atoms, the rows whose last context column (pocket_only, src/egnn.py:486-487) is non-zero (lightning.py:372-374);
+ *              inpainting models over all their atoms. Types are the first argmax of the first n_types feature columns, NaN
+ *              winning.
  *   bond order of a pair: get_bond_order (src/molecule_builder.py:77-102) as dl_bond_orders evaluates it: 0, or 1 / 2 / 3 by
  *              100 |x_i - x_j| against thr1, thr2, thr3 [min type][max type] (a negative entry: the pair has no such bond).
+ *              Atoms i and j bond iff the order is > 0, i.e. 100 |x_i - x_j| < thr1[min t][max t] and that entry >= 0:
+ *              dl_bond_orders' E != 0 is exactly this relation.
  *   valence    of atom i: the integer sum of its pairs' bond orders over the other checked atoms. Pocket atoms are not
  *              partners either: src/lightning.py:372-374 drops them before the molecule is built.
+ *   DL_CHECK_CONNECTED holds iff the graph of the atoms and their bonds has exactly one component (one atom is connected; no
+ *              atom is not), i.e. len(Chem.GetMolFrags(mol)) == 1 for build_molecule's molecule: the reference's
+ *              `is_connected` (src/metrics.py:20-27). Its AtomValenceException branch, which needs RDKit's valence model, is
+ *              not reproduced; the reference applies is_connected to sanitized molecules only (metrics.py:103-104), and for
+ *              those the two agree.
  *   DL_CHECK_VALENCE holds iff every checked atom has valence <= max_valence[type]. A molecule with no checked atom passes.
- *   DL_CHECK_CONNECTED holds iff the molecule is connected as dl_sample_chain_seeded_retry_connected defines it.
  * What is certain about DL_CHECK_VALENCE is just that: explicit valence within the caller's table, on dl_bond_orders' own
  * orders. build_molecule's molecules carry single, double and triple bonds only, no aromatic flags and no formal charges, so
  * an atom beyond its element's largest allowed valence is how Chem.SanitizeMol (is_valid, src/metrics.py:12-17) is expected
@@ -321,14 +283,13 @@ typedef struct dl_molecule_checks {
   const int32_t* max_valence;  /* (n_types) int32 DEVICE; DL_CHECK_VALENCE only */
 } dl_molecule_checks;
 /*
- * dl_sample_chain_seeded_retry whose rounds also resample the rows that miss a required check; with require =
- * DL_CHECK_CONNECTED it is dl_sample_chain_seeded_retry_connected. The checks run in one launch after the seeded loop and,
- * on the sub-batch, after each round. A row fails if its NaN flag is set or a required bit is missing; a resampled row
- * replaces the caller's row unless the caller's row is finite and the resample diverged. Rows that merely miss a check after
- * the last round are valid samples: they are returned with their bits cleared and do not make the call fail. DL_NAN_DETECTED
- * means that some row still diverges. max_retries = 0 only reports. A row whose fragments alone break the valence rule cannot
- * be repaired by a new linker: it is resampled every round and comes back with the bit cleared (vet inputs with
- * dl_molecule_check).
+ * dl_sample_chain_seeded_retry whose rounds also resample the rows that miss a required check. The checks run in one launch
+ * after the seeded loop and, on the sub-batch, after each round. A row fails if its NaN flag is set or a required bit is
+ * missing; a resampled row replaces the caller's row unless the caller's row is finite and the resample diverged. Rows that
+ * merely miss a check after the last round are valid samples: they are returned with their bits cleared and do not make the
+ * call fail. DL_NAN_DETECTED means that some row still diverges. max_retries = 0 only reports. A row whose fragments alone
+ * break the valence rule cannot be repaired by a new linker: it is resampled every round and comes back with the bit cleared
+ * (vet inputs with dl_molecule_check).
  *   passed   (B) int32 DEVICE out: the OR of the DL_CHECK_* bits row b's returned molecule satisfies, among those required
  * The other arguments are those of dl_sample_chain_seeded_retry. 1 <= n_types <= in_node_nf, N <= 8192.
  */
@@ -340,19 +301,22 @@ dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, in
                                                uint64_t* seeds_used, int32_t* attempts, const dl_molecule_checks* checks,
                                                int32_t* passed, void* stream);
 /*
- * The checks alone, on any (B,N) batch; xh, node_mask, context, context_nf and drop_pocket as dl_molecule_connected takes
- * them. DEVICE buffers, enqueued on `stream`.
- *   passed   (B) int32 out, as above
- *   valence  (B,N) int32 out or NULL; needs DL_CHECK_VALENCE: each checked atom's valence, 0 on every other row (for a hand-off
- *            to RDKit, and for tests)
+ * The checks alone, on any (B,N) batch. DEVICE buffers, enqueued on `stream`.
+ *   xh        (B,N,>=3+n_types) fp32, row stride xh_row_stride: x at columns 0..2, the atom-type one-hot from column 3
+ *   node_mask (B,N) int8
+ *   context   (B,N,context_nf) fp32; with drop_pocket != 0 the rows whose column context_nf - 1 is non-zero are not atoms
+ *             (read only then; may be NULL otherwise)
+ *   passed    (B) int32 out, as above
+ *   valence   (B,N) int32 out or NULL; needs DL_CHECK_VALENCE: each checked atom's valence, 0 on every other row (for a
+ *             hand-off to RDKit, and for tests)
  * 1 <= N <= 8192.
  */
 dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
                             const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
                             int32_t* passed, int32_t* valence, void* stream);
-/* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_seeded_retry(_connected, _checked), each from its row gather
- * to its row scatter -- including the wait for the host to capture the sub-batch's step graph -- summed over the rounds; 0
- * when no round ran. */
+/* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_seeded_retry(_checked), each from its
+ * row gather to its row scatter -- including the wait for the host to capture the sub-batch's step graph -- summed over the
+ * rounds; 0 when no round ran. */
 float dl_last_retry_ms(dl_engine* e);
 /* Strong scaling (SURVEY 8(e)): this engine samples molecules [b0, b0 + B) of a batch of B_full. The device-side noise of
  * the following dl_sample_chain_rng / dl_noise_fill / dl_noise_fill_inpaint calls is then the slice's ROWS of the
@@ -363,7 +327,7 @@ float dl_last_retry_ms(dl_engine* e);
 dl_status dl_set_noise_slice(dl_engine* e, int32_t B_full, int32_t b0);
 /*
  * Partial diffusion (no reference API; the `optimize` mode of DiffSBDD): the following dl_sample_chain* calls of this engine,
- * the recovery rounds of dl_sample_chain_seeded_retry(_connected) included, vary the linker the caller's xh holds on its
+ * the recovery rounds of dl_sample_chain_seeded_retry(_checked) included, vary the linker the caller's xh holds on its
  * linker_mask rows instead of sampling one from pure noise. With 0 <= t0 <= T:
  *   z     = xh * fragment_mask + (alpha_t0 * xh + sigma_t0 * eps) * linker_mask,   eps = draw 0 * linker_mask
  *           -- q(z_t0 | x) as EDM.forward draws it (edm.py:67-74), each product and sum rounded on its own; alpha_t0 and

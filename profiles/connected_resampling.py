@@ -1,8 +1,9 @@
 """Connectivity in the recovery rounds: the cost of the device-side check and of the rounds that resample the disconnected
-molecules (`sample_chain(..., require_connected=True)`, dl_sample_chain_seeded_retry_connected).
+molecules (`sample_chain(..., require_connected=True)`, dl_sample_chain_seeded_retry_checked).
 
 Per workload (synthetic weights, seeds 0..B-1, keep_frames=1) it prints:
-  * the device time of the check alone (dl_molecule_connected, CUDA events, median of --reps calls) on the sampled chain[0];
+  * the device time of the check alone (dl_molecule_check with DL_CHECK_CONNECTED, CUDA events, median of --reps calls) on
+    the sampled chain[0];
   * the fraction of rows that are disconnected after the first loop (round 0);
   * the device time of each recovery round (dl_last_retry_ms of runs with 1, 2, ... rounds, differenced: row gather, the
     wait for the host to capture the sub-batch's step graph, the sub-batch loop, its check, row scatter) next to the
@@ -37,10 +38,12 @@ def card():
 
 
 def check_ms(edm, chain0, node_mask, pocket_only, reps):
-    """Median device time of dl_molecule_connected over the batch, as the engine launches it."""
+    """Median device time of dl_molecule_check with connectivity alone over the batch, as the engine launches it."""
     lib = _native.load_library()
     B, N = chain0.shape[:2]
-    thr1 = edm._bond_table().to(chain0.device)
+    require = _native.CHECK_CONNECTED
+    tables = [t.to(chain0.device) for t in edm._check_tables(require)]
+    checks = _native.DLMoleculeChecks.of(require, tables)
     nm = (node_mask.reshape(B, N) != 0).to(torch.int8).contiguous()
     ctx = None if pocket_only is None else pocket_only.reshape(B, N, 1).float().contiguous()
     out = torch.empty(B, dtype=torch.int32, device=chain0.device)
@@ -49,9 +52,9 @@ def check_ms(edm, chain0, node_mask, pocket_only, reps):
     times = []
     for _ in range(reps + 3):
         ev0.record(st)
-        _native.check(lib.dl_molecule_connected(B, N, thr1.shape[0], chain0.data_ptr(), chain0.shape[2], nm.data_ptr(),
-                                                None if ctx is None else ctx.data_ptr(), 1, int(ctx is not None),
-                                                thr1.data_ptr(), out.data_ptr(), st.cuda_stream), "dl_molecule_connected")
+        _native.check(lib.dl_molecule_check(B, N, checks, chain0.data_ptr(), chain0.shape[2], nm.data_ptr(),
+                                            None if ctx is None else ctx.data_ptr(), 1, int(ctx is not None), out.data_ptr(),
+                                            None, st.cuda_stream), "dl_molecule_check")
         ev1.record(st)
         ev1.synchronize()
         times.append(ev0.elapsed_time(ev1))

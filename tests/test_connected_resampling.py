@@ -1,5 +1,5 @@
-"""Connectivity in the recovery rounds: `sample_chain(..., require_connected=True)`, dl_sample_chain_seeded_retry_connected
-and dl_molecule_connected.
+"""Connectivity in the recovery rounds: `sample_chain(..., require_connected=True)`, and dl_sample_chain_seeded_retry_checked
+and dl_molecule_check with DL_CHECK_CONNECTED.
 
 A molecule is connected when the atoms of chain[0] -- without the pocket on cut-off graphs -- form one component under
 get_bond_order > 0 (what `is_connected` of the reference's metrics counts for the molecule build_molecule makes). The oracle
@@ -126,7 +126,9 @@ def test_models_hand_the_edm_their_bond_tables():
     assert EDM(dynamics=None, in_node_nf=9, n_dims=3, noise_schedule='polynomial_2', timesteps=10, is_geom=True).is_geom
 
 
-def test_header_compiles_as_c99_with_the_connectivity_entries(tmp_path):
+def test_header_compiles_as_c99_with_a_connectivity_only_check(tmp_path):
+    """dl_molecule_check with DL_CHECK_CONNECTED alone refuses N beyond the check's limit, naming itself and the limit.
+    (A null engine is refused as test_valid_resampling's header test checks.)"""
     gcc = shutil.which("gcc")
     if gcc is None:
         pytest.skip("gcc not available")
@@ -136,12 +138,10 @@ def test_header_compiles_as_c99_with_the_connectivity_entries(tmp_path):
     src.write_text(
         '#include <stdio.h>\n#include "difflinker_b200.h"\n'
         "int main(void) {\n"
-        "  uint64_t used[2]; int32_t attempts[2], flags[2], conn[2];\n"
-        "  dl_status a = dl_sample_chain_seeded_retry_connected(NULL, DL_SAMPLER_LINKER, 2, 4, 10, 1, NULL, NULL, NULL, NULL,\n"
-        "                                                       NULL, NULL, NULL, NULL, NULL, NULL, flags, 3, used, attempts,\n"
-        "                                                       8, NULL, conn, NULL);\n"
-        '  printf("%d|%s|", (int)a, dl_last_error());\n'
-        "  dl_status b = dl_molecule_connected(2, 9000, 8, NULL, 11, NULL, NULL, 0, 0, NULL, conn, NULL);\n"
+        "  int32_t conn[2];\n"
+        "  float thr1[64] = {0};\n"
+        "  dl_molecule_checks ck = {DL_CHECK_CONNECTED, 8, thr1, NULL, NULL, NULL};\n"
+        "  dl_status b = dl_molecule_check(2, 9000, &ck, NULL, 11, NULL, NULL, 0, 0, conn, NULL, NULL);\n"
         '  printf("%d|%s\\n", (int)b, dl_last_error());\n'
         "  return 0;\n}\n")
     exe = tmp_path / "connected_abi"
@@ -150,9 +150,8 @@ def test_header_compiles_as_c99_with_the_connectivity_entries(tmp_path):
                     f"-Wl,-rpath,{os.path.dirname(lib)}"], check=True, capture_output=True)
     res = subprocess.run([str(exe)], capture_output=True, text=True)
     assert res.returncode == 0, (res.stdout, res.stderr)
-    a, err_a, b, err_b = res.stdout.strip().split("|", 3)
-    assert int(a) == -1 and "null engine" in err_a
-    assert int(b) == -1 and "dl_molecule_connected" in err_b
+    b, err_b = res.stdout.strip().split("|", 1)
+    assert int(b) == -1 and "dl_molecule_check" in err_b and "8192" in err_b
 
 
 # ---- GPU: the kernel, molecule by molecule ------------------------------------------------------------------------------

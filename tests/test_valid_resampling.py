@@ -153,6 +153,8 @@ def test_models_pass_the_keyword_and_the_tables_to_the_edm():
 def test_native_binds_the_check_entries():
     lib = _native.load_library()
     assert "dl_sample_chain_seeded_retry_checked" in _native.SYMBOLS and "dl_molecule_check" in _native.SYMBOLS
+    for gone in ("dl_sample_chain_seeded_retry_connected", "dl_molecule_connected"):   # connectivity alone runs through them too
+        assert gone not in _native.SYMBOLS and not hasattr(lib, gone)
     assert lib.dl_molecule_check.argtypes[2]._type_ is _native.DLMoleculeChecks
     assert (_native.CHECK_CONNECTED, _native.CHECK_VALENCE) == (1, 2)
     assert _native.DLMoleculeChecks.of(3, [torch.zeros(8, 8)]).n_types == 8
@@ -247,7 +249,7 @@ def run_check(xh, nm, is_geom, po=None, require=BOTH, max_valence=None):
 
 
 def assert_matches_oracle(xh, nm, is_geom, po=None):
-    """Both verdict bits and every valence equal the oracle's, the connected bit also dl_molecule_connected's, and each
+    """Both verdict bits and every valence equal the oracle's, the connected bit also molecule_builder.connected's, and each
     check alone gives its own bit."""
     d = tcr.dev()
     T = 9 if is_geom else 8
@@ -541,33 +543,6 @@ def test_each_flag_alone_and_both_resample_their_own_rows(impl):
     n0 = launches(ddpm)
     edm.sample_chain(**kw, keep_frames=2, seeds=SEEDS, require_valid=True)
     assert with_conn == plain + 1 and launches(ddpm) - n0 == plain + 1
-
-
-@pytest.mark.gpu
-def test_the_checked_entry_with_connectivity_alone_is_the_connected_entry():
-    """dl_sample_chain_seeded_retry_checked with require = DL_CHECK_CONNECTED returns, bit for bit, what
-    dl_sample_chain_seeded_retry_connected returns: chain, flags, seeds, attempts and the connected output."""
-    ddpm, kw, _ = build("fc", "simt")
-    edm = ddpm.edm
-    want = edm.sample_chain(**kw, keep_frames=2, seeds=SEEDS, nan_retries=2, require_connected=True)
-    conn, attempts, used = edm.last_connected, edm.last_attempts, edm.last_seeds
-    from difflinker_b200 import edm as edm_mod
-    real = edm_mod._sample_slice_draws
-
-    def through_checked(lib, eng, head, tail, stream, noise, seeds, rng, retry):
-        max_retries, u, a, (require, tables, passed) = retry
-        assert require == _native.CHECK_CONNECTED
-        st = lib.dl_sample_chain_seeded_retry_checked(eng, *head, seeds.data_ptr(), *tail, max_retries, u.data_ptr(),
-                                                      a.data_ptr(), _native.DLMoleculeChecks.of(require, tables),
-                                                      passed.data_ptr(), stream)
-        return _native.check(st, "dl_sample_chain_seeded_retry_checked"), 0
-    edm_mod._sample_slice_draws = through_checked
-    try:
-        got = edm.sample_chain(**kw, keep_frames=2, seeds=SEEDS, nan_retries=2, require_connected=True)
-    finally:
-        edm_mod._sample_slice_draws = real
-    assert torch.equal(got, want) and torch.equal(edm.last_connected, conn)
-    assert torch.equal(edm.last_attempts, attempts) and torch.equal(edm.last_seeds, used)
 
 
 @pytest.mark.gpu
