@@ -10,7 +10,7 @@ GRAPH_TYPES = {"FC": 0, "4A": 1, "FC-4A": 2, "FC-10A-4A": 3}
 EDGE_IMPLS = {"auto": 0, "simt": 1, "wgmma": 2}
 SAMPLER_LINKER, SAMPLER_INPAINT = 0, 1
 AGGREGATIONS = {"sum": 0, "mean": 1}
-CHECK_CONNECTED, CHECK_VALENCE = 1, 2   # DL_CHECK_*
+CHECK_CONNECTED, CHECK_VALENCE, CHECK_CLASH = 1, 2, 4   # DL_CHECK_*
 COORDS_RANGE = 15.0   # EGNN hands its own coords_range=15 to every EquivariantBlock (src/egnn.py:183,209)
 
 
@@ -74,6 +74,8 @@ SYMBOLS = {
     "dl_sample_chain_seeded_retry_checked": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                                     _P, _I32, _P, _P, C.POINTER(DLMoleculeChecks), _P, _P]),
     "dl_molecule_check": (_I32, [_I32, _I32, C.POINTER(DLMoleculeChecks), _P, _I32, _P, _P, _I32, _I32, _P, _P, _P]),
+    "dl_set_clash_table": (_I32, [_P, _P]),
+    "dl_clash_check": (_I32, [_I32, _I32, _I32, _P, _P, _I32, _P, _P, _P, _I32, _P, _P, _P]),
     "dl_last_retry_ms": (_F, [_P]),
     "dl_set_noise_slice": (_I32, [_P, _I32, _I32]),
     "dl_set_start_step": (_I32, [_P, _I32, _F, _F]),

@@ -120,6 +120,8 @@ struct dl_engine {
   // dl_set_start_step: the linker sampler starts at step start_step from q(z_t0 | x) with these scalars; -1: from noise at T
   int start_step = -1;
   float start_alpha = 0.f, start_sigma = 0.f;
+  // dl_set_clash_table: the caller's (n_types, n_types) clash distances for DL_CHECK_CLASH; null: none set
+  const float* clash_table = nullptr;
   bool finalized = false;
   std::map<std::string, std::vector<float>> raw;
   float* wblob = nullptr;      // packed fp32 weights
@@ -976,6 +978,12 @@ dl_status dl_set_start_step(dl_engine* e, int32_t t0, float alpha_t0, float sigm
   return DL_OK;
 }
 
+dl_status dl_set_clash_table(dl_engine* e, const float* clash) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  e->clash_table = clash;
+  return DL_OK;
+}
+
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream) {
   dl_status s = check_shapes(e, B, N);
@@ -1167,16 +1175,22 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt) { return retry_seed(seed,
 
 namespace {
 
-static_assert(CHECK_CONNECTED == DL_CHECK_CONNECTED && CHECK_VALENCE == DL_CHECK_VALENCE, "kernels_retry.cuh vs header");
+static_assert(CHECK_CONNECTED == DL_CHECK_CONNECTED && CHECK_VALENCE == DL_CHECK_VALENCE && CHECK_CLASH == DL_CHECK_CLASH,
+              "kernels_retry.cuh vs header");
 
 // What is wrong with a caller's dl_molecule_checks for molecules of N rows whose h holds at most max_types type columns, or
-// null.
-const char* checks_error(const dl_molecule_checks* ck, int N, int max_types) {
+// null. The sampler takes every check; dl_molecule_check the bond checks only (the clash check has dl_clash_check).
+const char* checks_error(const dl_molecule_checks* ck, int N, int max_types, bool clash_allowed) {
   if (!ck) return "null checks";
-  if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE)))
-    return "checks->require must be DL_CHECK_CONNECTED, DL_CHECK_VALENCE or both";
+  if (clash_allowed) {
+    if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE | DL_CHECK_CLASH)))
+      return "checks->require must be a non-empty OR of DL_CHECK_CONNECTED, DL_CHECK_VALENCE and DL_CHECK_CLASH";
+  } else if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE))) {
+    return "checks->require must be DL_CHECK_CONNECTED, DL_CHECK_VALENCE or both (the clash check runs through "
+           "dl_clash_check)";
+  }
   if (ck->n_types < 1 || ck->n_types > max_types) return "checks->n_types must be in [1, the width of the atom features]";
-  if (!ck->thr1) return "null checks->thr1";
+  if ((ck->require & (DL_CHECK_CONNECTED | DL_CHECK_VALENCE)) && !ck->thr1) return "null checks->thr1";
   if ((ck->require & DL_CHECK_VALENCE) && (!ck->thr2 || !ck->thr3 || !ck->max_valence))
     return "DL_CHECK_VALENCE needs checks->thr2, thr3 and max_valence";
   if (N > CONN_MAX_N) return "the molecule checks take N <= 8192";
@@ -1218,7 +1232,8 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
   const int require = ck ? ck->require : 0;
   std::vector<int32_t> flags(B), pass(B, require);
   if (ck) {
-    CK(launch_molecule_check(require, check_args(e, *ck, chain, N, node_mask, context, passed), B, st));
+    const ClashArgs cl{linker_mask, e->clash_table, nullptr};   // the clash check's linker rows and table
+    CK(launch_molecule_check(require, check_args(e, *ck, chain, N, node_mask, context, passed), cl, B, st));
     e->launches += 1;
     CK(cudaMemcpyAsync(pass.data(), passed, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   }
@@ -1267,7 +1282,7 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     if (ck) {
       CheckArgs ca = check_args(e, *ck, sa.s_chain, N, ga.s_node_mask, ga.s_context, sl.at<int32_t>(i_ps));
       ca.rows = ga.rows; ca.flags = nan_flags; ca.s_flags = sa.s_flags; ca.take = sl.at<int32_t>(i_tk);
-      CK(launch_molecule_check(require, ca, Bs, st));
+      CK(launch_molecule_check(require, ca, ClashArgs{ga.s_linker_mask, e->clash_table, nullptr}, Bs, st));
       e->launches += 1;
       sa.take = ca.take; sa.s_passed = ca.passed; sa.passed = passed;
       k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
@@ -1324,7 +1339,13 @@ dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, in
     set_err("null argument (nan_flags, seeds_used, attempts or passed)");
     return DL_ERR_INVALID;
   }
-  if (const char* why = checks_error(checks, N, e->cfg.in_node_nf)) {
+  const char* why = checks_error(checks, N, e->cfg.in_node_nf, true);
+  if (!why && (checks->require & DL_CHECK_CLASH)) {
+    if (!e->clash_table) why = "DL_CHECK_CLASH needs a clash table (dl_set_clash_table)";
+    else if (e->cfg.graph_type == DL_GRAPH_FC) why = "DL_CHECK_CLASH needs a pocket: DL_GRAPH_FC graphs have none";
+    else if (sampler == DL_SAMPLER_INPAINT) why = "DL_CHECK_CLASH does not take DL_SAMPLER_INPAINT, which re-noises the pocket";
+  }
+  if (why) {
     set_err("dl_sample_chain_seeded_retry_checked: %s", why);
     return DL_ERR_INVALID;
   }
@@ -1335,7 +1356,7 @@ dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, in
 dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
                             const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
                             int32_t* passed, int32_t* valence, void* stream) {
-  const char* why = checks_error(checks, N, xh_row_stride - 3);
+  const char* why = checks_error(checks, N, xh_row_stride - 3, false);
   if (!why && (B <= 0 || N <= 0 || !xh || !node_mask || !passed || (drop_pocket && (!context || context_nf < 1))))
     why = "invalid argument";
   if (!why && valence && !(checks->require & DL_CHECK_VALENCE)) why = "valence needs DL_CHECK_VALENCE";
@@ -1344,7 +1365,26 @@ dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* chec
   CheckArgs ca = check_args(*checks, xh, N, xh_row_stride, node_mask, context, context_nf, drop_pocket != 0, passed);
   ca.valence = valence;
   if (valence) CK(cudaMemsetAsync(valence, 0, (size_t)B * N * sizeof(int32_t), st));   // the rows that are not checked
-  CK(launch_molecule_check(checks->require, ca, B, st));
+  CK(launch_molecule_check(checks->require, ca, ClashArgs{}, B, st));
+  return DL_OK;
+}
+
+dl_status dl_clash_check(int32_t B, int32_t N, int32_t n_types, const float* clash, const float* xh, int32_t xh_row_stride,
+                         const int8_t* node_mask, const float* linker_mask, const float* context, int32_t context_nf,
+                         int32_t* passed, int32_t* clashes, void* stream) {
+  const char* why = nullptr;
+  if (B <= 0 || N <= 0) why = "B and N must be >= 1";
+  else if (N > CONN_MAX_N) why = "the molecule checks take N <= 8192";
+  else if (n_types < 1 || n_types > xh_row_stride - 3) why = "n_types must be in [1, xh_row_stride - 3]";
+  else if (!clash) why = "null clash table";
+  else if (!xh || !node_mask || !linker_mask || !context || context_nf < 1 || !passed) why = "invalid argument";
+  if (why) { set_err("dl_clash_check: %s", why); return DL_ERR_INVALID; }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CheckArgs ca{};
+  ca.xh = xh; ca.N = N; ca.row_stride = xh_row_stride; ca.n_types = n_types;
+  ca.node_mask = node_mask; ca.C = context_nf; ca.context = context; ca.drop_pocket = 1; ca.passed = passed;
+  if (clashes) CK(cudaMemsetAsync(clashes, 0, (size_t)B * N * sizeof(int32_t), st));   // the rows that are not linker atoms
+  CK(launch_molecule_check(CHECK_CLASH, ca, ClashArgs{linker_mask, clash, clashes}, B, st));
   return DL_OK;
 }
 

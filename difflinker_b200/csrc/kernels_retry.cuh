@@ -89,9 +89,11 @@ __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a) {
 // component (a single atom is connected, no atom is not): len(Chem.GetMolFrags(mol)) == 1 for the molecule build_molecule
 // makes of them (lightning.py:364-377, metrics.py:20-27).
 // CHECK_VALENCE: an atom's valence is the sum of bond_order_pair (get_bond_order) over the other checked atoms; the bit is
-// set iff every atom's valence is <= max_valence[its type] (no atom: set). The predicate is stated in full at
-// dl_molecule_checks in the header.
-constexpr int CHECK_CONNECTED = 1, CHECK_VALENCE = 2;                // DL_CHECK_* of the header
+// set iff every atom's valence is <= max_valence[its type] (no atom: set).
+// CHECK_CLASH (always with drop_pocket): the linker atoms are the checked atoms with linker_mask != 0, the pocket atoms the
+// rows with node_mask != 0 and context column C - 1 != 0; the bit is set iff no linker atom clashes (clash_pair) with any
+// pocket atom (no linker or no pocket atom: set). The predicates are stated in full at dl_molecule_checks in the header.
+constexpr int CHECK_CONNECTED = 1, CHECK_VALENCE = 2, CHECK_CLASH = 4;   // DL_CHECK_* of the header
 constexpr int CONN_MAX_N = 8192;                                     // rows per molecule: 20 bytes of shared memory each
 constexpr int CONN_SMEM_MAX = CONN_MAX_N * (int)(sizeof(float4) + sizeof(int));
 
@@ -112,6 +114,16 @@ struct CheckArgs {
   int32_t* take;
 };
 
+// What CHECK_CLASH reads and writes besides CheckArgs. It is a kernel parameter of its own, passed to the instantiations
+// with the clash bit only: CheckArgs is 128 bytes, and any field appended to it changes the code ptxas generates for the
+// other instantiations.
+struct ClashArgs {
+  const float* linker_mask;              // (B, N): the checked atoms with linker_mask != 0 are the linker atoms
+  const float* clash;                    // (n_types, n_types) clash distances in pm, [min type][max type]
+  int32_t* clashes;                      // (B, N) or null: every linker atom's count of pocket atoms it clashes with (other
+                                         // rows are not written)
+};
+
 // One CTA per molecule. The checked atoms are compacted, in row order, into shared memory (coordinates and type; padded
 // and pocket rows are never read beyond their masks).
 // Valence: a warp per atom sums the integer bond orders of its pairs with every other atom, so the sums do not depend on
@@ -120,41 +132,111 @@ struct CheckArgs {
 // (atomicMin), trees are flattened, and this repeats until a pass over all pairs hooks nothing. Labels only ever decrease
 // and each root is its tree's smallest atom, so the final labels -- every atom's component minimum -- and the flag do not
 // depend on the order the threads hook in.
+// Clash: the pocket atoms are compacted into the same buffer from its back, s_at[N - 1 - k] (the checked atoms and the
+// pocket atoms are disjoint rows, so the two never meet), and s_lab[i] holds atom i's row with bit 31 set for a linker
+// atom until the clash pass is done. A warp per linker atom counts, in integers, the pocket atoms it clashes with; the
+// count and the verdict do not depend on the order the lanes add in.
+// The body of both k_molecule_check kernels below; cl is read with CHECK_CLASH only.
 template <int CHECKS>
-__global__ void __launch_bounds__(256) k_molecule_check(CheckArgs a) {
+__device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashArgs& cl) {
   extern __shared__ float4 s_at[];                    // [n]: x, y, z, type (int bits)
   int* s_lab = reinterpret_cast<int*>(s_at + a.N);    // [n]: the atoms' rows (valence), then parent pointers (components)
   __shared__ int s_warp[8], s_n, s_changed;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = blockIdx.x;
   const size_t g0 = (size_t)b * a.N;
-  if (tid == 0) s_n = 0;
-  __syncthreads();
-  for (int r0 = 0; r0 < a.N; r0 += 256) {
-    const int r = r0 + tid;
-    bool ok = r < a.N && a.node_mask[g0 + r] != 0;
-    if (ok && a.drop_pocket) ok = a.context[(g0 + r) * a.C + a.C - 1] == 0.f;
-    const unsigned m = __ballot_sync(0xffffffffu, ok);
-    if (lane == 0) s_warp[warp] = __popc(m);
+  int n_pocket = 0;
+  if constexpr ((CHECKS & CHECK_CLASH) != 0) {
+    __shared__ int s_pwarp[8], s_np;
+    if (tid == 0) s_n = s_np = 0;
     __syncthreads();
-    int off = s_n + __popc(m & ((1u << lane) - 1u)), total = 0;
-    for (int w = 0; w < 8; ++w) { off += w < warp ? s_warp[w] : 0; total += s_warp[w]; }
-    if (ok) {
-      const float* row = a.xh + (g0 + r) * a.row_stride;
-      int best = 0;                                   // torch.argmax: the first maximum; NaN wins
-      for (int k = 1; k < a.n_types; ++k) {
-        const float v = row[3 + k], cur = row[3 + best];
-        if (v > cur || (isnan(v) && !isnan(cur))) best = k;
+    for (int r0 = 0; r0 < a.N; r0 += 256) {
+      const int r = r0 + tid;
+      const bool live = r < a.N && a.node_mask[g0 + r] != 0;
+      const bool ok = live && a.context[(g0 + r) * a.C + a.C - 1] == 0.f, pocket = live && !ok;
+      const bool linker = ok && cl.linker_mask[g0 + r] != 0.f;
+      const unsigned m = __ballot_sync(0xffffffffu, ok), mp = __ballot_sync(0xffffffffu, pocket);
+      if (lane == 0) { s_warp[warp] = __popc(m); s_pwarp[warp] = __popc(mp); }
+      __syncthreads();
+      const unsigned below = (1u << lane) - 1u;
+      int off = s_n + __popc(m & below), poff = s_np + __popc(mp & below), total = 0, ptotal = 0;
+      for (int w = 0; w < 8; ++w) {
+        off += w < warp ? s_warp[w] : 0; total += s_warp[w];
+        poff += w < warp ? s_pwarp[w] : 0; ptotal += s_pwarp[w];
       }
-      s_at[off] = make_float4(row[0], row[1], row[2], __int_as_float(best));
-      s_lab[off] = (CHECKS & CHECK_VALENCE) ? r : off;
+      if (ok || pocket) {
+        const float* row = a.xh + (g0 + r) * a.row_stride;
+        int best = 0;                                 // torch.argmax: the first maximum; NaN wins
+        for (int k = 1; k < a.n_types; ++k) {
+          const float v = row[3 + k], cur = row[3 + best];
+          if (v > cur || (isnan(v) && !isnan(cur))) best = k;
+        }
+        const float4 at = make_float4(row[0], row[1], row[2], __int_as_float(best));
+        if (ok) {
+          s_at[off] = at;
+          s_lab[off] = r | (linker ? (int)0x80000000u : 0);
+        } else {
+          s_at[a.N - 1 - poff] = at;
+        }
+      }
+      __syncthreads();
+      if (tid == 0) { s_n += total; s_np += ptotal; }
+      __syncthreads();
     }
+    n_pocket = s_np;
+  } else {
+    if (tid == 0) s_n = 0;
     __syncthreads();
-    if (tid == 0) s_n += total;
-    __syncthreads();
+    for (int r0 = 0; r0 < a.N; r0 += 256) {
+      const int r = r0 + tid;
+      bool ok = r < a.N && a.node_mask[g0 + r] != 0;
+      if (ok && a.drop_pocket) ok = a.context[(g0 + r) * a.C + a.C - 1] == 0.f;
+      const unsigned m = __ballot_sync(0xffffffffu, ok);
+      if (lane == 0) s_warp[warp] = __popc(m);
+      __syncthreads();
+      int off = s_n + __popc(m & ((1u << lane) - 1u)), total = 0;
+      for (int w = 0; w < 8; ++w) { off += w < warp ? s_warp[w] : 0; total += s_warp[w]; }
+      if (ok) {
+        const float* row = a.xh + (g0 + r) * a.row_stride;
+        int best = 0;                                 // torch.argmax: the first maximum; NaN wins
+        for (int k = 1; k < a.n_types; ++k) {
+          const float v = row[3 + k], cur = row[3 + best];
+          if (v > cur || (isnan(v) && !isnan(cur))) best = k;
+        }
+        s_at[off] = make_float4(row[0], row[1], row[2], __int_as_float(best));
+        s_lab[off] = (CHECKS & CHECK_VALENCE) ? r : off;
+      }
+      __syncthreads();
+      if (tid == 0) s_n += total;
+      __syncthreads();
+    }
   }
   const int n = s_n;
   int verdict = 0;
+  if constexpr ((CHECKS & CHECK_CLASH) != 0) {
+    int hit = 0;
+    for (int i = warp; i < n; i += 8) {               // warp per linker atom i, lanes over the pocket atoms
+      const int tag = s_lab[i];
+      if (tag >= 0) continue;                         // not a linker atom: bit 31 clear
+      const float4 pi = s_at[i];
+      int c = 0;
+      for (int j = lane; j < n_pocket; j += 32) {
+        const float4 pj = s_at[a.N - 1 - j];
+        c += clash_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
+                        __float_as_int(pj.w), a.n_types, cl.clash);
+      }
+      for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+      if (lane == 0) {
+        hit |= c > 0;
+        if (cl.clashes) cl.clashes[g0 + (tag & 0x7fffffff)] = c;
+      }
+    }
+    if (!__syncthreads_or(hit)) verdict |= CHECK_CLASH;
+    if (CHECKS & (CHECK_CONNECTED | CHECK_VALENCE)) {   // what the other checks expect: rows (valence) or labels
+      for (int i = tid; i < n; i += 256) s_lab[i] = (CHECKS & CHECK_VALENCE) ? (s_lab[i] & 0x7fffffff) : i;
+      __syncthreads();
+    }
+  }
   if (CHECKS & CHECK_VALENCE) {
     int over = 0;
     for (int i = warp; i < n; i += 8) {               // warp per atom i, lanes over its partners j != i
@@ -220,26 +302,55 @@ __global__ void __launch_bounds__(256) k_molecule_check(CheckArgs a) {
   }
 }
 
+// The instantiations without the clash bit, and with it.
 template <int CHECKS>
-cudaError_t launch_molecule_check_as(const CheckArgs& a, int B, cudaStream_t st) {
+__global__ void __launch_bounds__(256) k_molecule_check(CheckArgs a) {
+  static_assert((CHECKS & CHECK_CLASH) == 0, "the clash check takes ClashArgs");
+  molecule_check<CHECKS>(a, ClashArgs{});
+}
+
+// (With __launch_bounds__(256) alone ptxas fits <6> into 32 registers and spills; a minimum of one CTA per SM lets it take
+// the 38-39 it needs.)
+template <int CHECKS>
+__global__ void __launch_bounds__(256, 1) k_molecule_check(CheckArgs a, ClashArgs k) {
+  static_assert((CHECKS & CHECK_CLASH) != 0, "only the clash check takes ClashArgs");
+  molecule_check<CHECKS>(a, k);
+}
+
+template <int CHECKS>
+cudaError_t launch_molecule_check_as(const CheckArgs& a, const ClashArgs& k, int B, cudaStream_t st) {
   const size_t smem = (size_t)a.N * (sizeof(float4) + sizeof(int));
-  if (smem > 48 * 1024) {
-    const cudaError_t err =
-        cudaFuncSetAttribute(k_molecule_check<CHECKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, CONN_SMEM_MAX);
-    if (err != cudaSuccess) return err;
+  if constexpr ((CHECKS & CHECK_CLASH) != 0) {
+    void (*kernel)(CheckArgs, ClashArgs) = k_molecule_check<CHECKS>;
+    if (smem > 48 * 1024) {
+      const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CONN_SMEM_MAX);
+      if (err != cudaSuccess) return err;
+    }
+    kernel<<<B, 256, smem, st>>>(a, k);
+  } else {
+    void (*kernel)(CheckArgs) = k_molecule_check<CHECKS>;
+    if (smem > 48 * 1024) {
+      const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CONN_SMEM_MAX);
+      if (err != cudaSuccess) return err;
+    }
+    kernel<<<B, 256, smem, st>>>(a);
   }
-  k_molecule_check<CHECKS><<<B, 256, smem, st>>>(a);
   return cudaGetLastError();
 }
 
-// Launches k_molecule_check<checks> over B molecules; checks is CHECK_CONNECTED, CHECK_VALENCE or both, N <= CONN_MAX_N.
+// Launches k_molecule_check<checks> over B molecules; checks is a non-empty OR of CHECK_*, N <= CONN_MAX_N.
 // The shared-memory limit is raised to its one maximum the first time a molecule needs more than the default, so
 // concurrent callers never lower it under each other.
-inline cudaError_t launch_molecule_check(int checks, const CheckArgs& a, int B, cudaStream_t st) {
+inline cudaError_t launch_molecule_check(int checks, const CheckArgs& a, const ClashArgs& k, int B, cudaStream_t st) {
+  constexpr int CV = CHECK_CONNECTED | CHECK_VALENCE;
   switch (checks) {
-    case CHECK_CONNECTED: return launch_molecule_check_as<CHECK_CONNECTED>(a, B, st);
-    case CHECK_VALENCE: return launch_molecule_check_as<CHECK_VALENCE>(a, B, st);
-    case CHECK_CONNECTED | CHECK_VALENCE: return launch_molecule_check_as<CHECK_CONNECTED | CHECK_VALENCE>(a, B, st);
+    case CHECK_CONNECTED: return launch_molecule_check_as<CHECK_CONNECTED>(a, k, B, st);
+    case CHECK_VALENCE: return launch_molecule_check_as<CHECK_VALENCE>(a, k, B, st);
+    case CHECK_CONNECTED | CHECK_VALENCE: return launch_molecule_check_as<CHECK_CONNECTED | CHECK_VALENCE>(a, k, B, st);
+    case CHECK_CLASH: return launch_molecule_check_as<CHECK_CLASH>(a, k, B, st);
+    case CHECK_CLASH | CHECK_CONNECTED: return launch_molecule_check_as<CHECK_CLASH | CHECK_CONNECTED>(a, k, B, st);
+    case CHECK_CLASH | CHECK_VALENCE: return launch_molecule_check_as<CHECK_CLASH | CHECK_VALENCE>(a, k, B, st);
+    case CHECK_CLASH | CV: return launch_molecule_check_as<CHECK_CLASH | CV>(a, k, B, st);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -111,13 +111,15 @@ def _check_start(sample_fn, start_step):
 
 
 def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                 start_step=None, require_valid=None):
+                 start_step=None, require_valid=None, require_clash_free=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
     `nan_retries`: rounds that resample only the diverged molecules (EDM.sample_chain; None uses `model.edm.nan_retries`).
     `require_connected`: the rounds also resample the disconnected molecules (None uses `model.edm.require_connected`).
     `require_valid`: ... and the molecules with an atom beyond its valence (None uses `model.edm.require_valid`).
+    `require_clash_free`: ... and, on pocket graphs, the molecules whose linker clashes with the pocket (None uses
+    `model.edm.require_clash_free`).
     `start_step` = t0 (partial diffusion, EDM.sample_chain): the template of sample_fn=None with the batch's own linker
     positions and atom types on its linker rows, sampled from step t0; ValueError with a sample_fn, or when the batch's
     linker rows do not directly follow its fragment rows."""
@@ -130,6 +132,8 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['require_connected'] = require_connected
     if require_valid is not None:
         extra['require_valid'] = require_valid
+    if require_clash_free is not None:
+        extra['require_clash_free'] = require_clash_free
     if start_step is not None:
         extra['start_step'] = start_step
     chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **extra)
@@ -137,7 +141,7 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
 
 
 def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                max_molecules=256, start_step=None, require_valid=None):
+                max_molecules=256, start_step=None, require_valid=None, require_clash_free=None):
     """The body of sample_chain for many batches `datas` at once, sampled in shared launches by EDM.sample_many: returns
     [(chain_k, node_mask_k)] in the order of `datas`, each equal to what sample_chain(model, datas[k], ...) returns (with
     seeds[k]) in the sense of EDM.sample_many. `model` as for sample_chain, so accelerated reference modules take it too.
@@ -162,6 +166,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['require_connected'] = require_connected
     if require_valid is not None:
         extra['require_valid'] = require_valid
+    if require_clash_free is not None:
+        extra['require_clash_free'] = require_clash_free
     if start_step is not None:
         extra['start_step'] = start_step
     chains = edm.sample_many(requests, keep_frames=keep_frames, seeds=seeds, max_molecules=max_molecules, **extra)
@@ -204,15 +210,16 @@ class DDPM(nn.Module):
         self.edm.devices = devices          # EDM.devices: split each sampling batch over these CUDA devices
 
     def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                     start_step=None, require_valid=None):
+                     start_step=None, require_valid=None, require_clash_free=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
-                            require_connected=require_connected, start_step=start_step, require_valid=require_valid)
+                            require_connected=require_connected, start_step=start_step, require_valid=require_valid,
+                            require_clash_free=require_clash_free)
 
     def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                    max_molecules=256, start_step=None, require_valid=None):
+                    max_molecules=256, start_step=None, require_valid=None, require_clash_free=None):
         return sample_many(self, datas, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                            require_connected=require_connected, max_molecules=max_molecules, start_step=start_step,
-                           require_valid=require_valid)
+                           require_valid=require_valid, require_clash_free=require_clash_free)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

@@ -17,7 +17,7 @@ import torch.nn.functional as F
 from . import _native
 from .distributed import (deal_launches, device_slices, pack_requests, place_rows, plan_launches, resolve_devices,
                           slice_sampler_inputs, unpack_rows)
-from .molecule_builder import check_tables
+from .molecule_builder import check_tables, clash_table
 from .noise import PredefinedNoiseSchedule
 from .utils import FoundNaNException, nan_exception_class
 
@@ -26,7 +26,7 @@ def _generator_of(dev):
     return torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
 
 
-def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None):
+def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None, clash=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
@@ -35,12 +35,18 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     and, with `require` != 0, those that miss a required check, whose verdict bits go to `passed`
     (dl_sample_chain_seeded_retry_checked; `tables` as molecule_builder.check_tables returns them, on the slice's device).
     `start` = (t0, alpha_t0, sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of
-    the call (dl_set_start_step). Returns (status, what the batch stream consumed)."""
+    the call (dl_set_start_step). `clash`, a (T,T) table on the slice's device, is the engine's clash table for the duration
+    of the call (dl_set_clash_table), which a `require` with CHECK_CLASH reads. Returns (status, what the batch stream
+    consumed)."""
     if start is not None:
         _native.check(lib.dl_set_start_step(eng, *start), "dl_set_start_step")
     try:
+        if clash is not None:
+            _native.check(lib.dl_set_clash_table(eng, clash.data_ptr()), "dl_set_clash_table")
         return _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry)
     finally:
+        if clash is not None:
+            lib.dl_set_clash_table(eng, None)
         if start is not None:
             lib.dl_set_start_step(eng, -1, 0.0, 0.0)
 
@@ -192,13 +198,18 @@ class EDM(torch.nn.Module):
         # (not verified, see molecule_builder.valence_ok). Same needs; False, the default, checks nothing.
         self.require_valid = False
         self.last_valid = None                 # calls with require_valid: the (B,) CPU bool valence verdict of every row
+        # Pocket clashes (cut-off graphs only): likewise for the molecules with a linker atom closer to a pocket atom than
+        # molecule_builder.clash_table(is_geom) allows, in the same check launch. Same needs; False, the default, checks
+        # nothing.
+        self.require_clash_free = False
+        self.last_clash_free = None            # calls with require_clash_free: the (B,) CPU bool clash verdict of every row
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
         # sample_many: per request, what last_seeds / last_attempts / last_connected / last_valid hold after its own
         # sample_chain call; per launch, (device, the requests it held, loop ms)
         self.last_seeds_many = self.last_attempts_many = self.last_connected_many = self.last_loop_ms_many = None
-        self.last_valid_many = None
+        self.last_valid_many = self.last_clash_free_many = None
 
     @property
     def devices(self):
@@ -467,12 +478,24 @@ class EDM(torch.nn.Module):
             raise ValueError(f"{name} needs CUDA inputs (got {x.device})")
         return True
 
-    def _checks(self, require_connected, require_valid, seeds, noise, batch_slice, x):
+    def _checks(self, require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free=None):
         """The molecule checks of a call as the OR of _native.CHECK_*; 0 checks nothing."""
         return ((_native.CHECK_CONNECTED if self._require_check('require_connected', require_connected, seeds, noise,
                                                                 batch_slice, x) else 0) |
                 (_native.CHECK_VALENCE if self._require_check('require_valid', require_valid, seeds, noise, batch_slice, x)
-                 else 0))
+                 else 0) |
+                (_native.CHECK_CLASH if self._require_clash_free(require_clash_free, seeds, noise, batch_slice, x) else 0))
+
+    def _require_clash_free(self, value, seeds, noise, batch_slice, x):
+        """_require_check for require_clash_free, which also needs a pocket that stays put: a cut-off (pocket) graph and the
+        linker sampler -- the inpainting sampler re-noises the pocket."""
+        if (self.require_clash_free if value is None else value) is True:
+            if self._SAMPLER == _native.SAMPLER_INPAINT:
+                raise ValueError("require_clash_free does not take InpaintingEDM: its loop re-noises the pocket")
+            if self.dynamics.graph_type == 'FC':
+                raise ValueError("require_clash_free needs a pocket: FC graphs have no pocket rows (use a pocket model on a "
+                                 "cut-off graph such as '4A' or 'FC-10A-4A')")
+        return self._require_check('require_clash_free', value, seeds, noise, batch_slice, x)
 
     def _check_tables(self, check):
         """The CPU tables the checks `check` read with this model's atom types (molecule_builder.check_tables)."""
@@ -489,7 +512,7 @@ class EDM(torch.nn.Module):
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
-                     require_valid=None):
+                     require_valid=None, require_clash_free=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -531,6 +554,11 @@ class EDM(torch.nn.Module):
         build_molecule's molecules are expected to fail RDKit's sanitization; that has not been verified against RDKit.
         A row whose fragments alone break the rule cannot be repaired by a new linker: it is resampled every round and
         comes back flagged, so vet inputs with molecule_builder.valence_ok. Either flag alone or both.
+        `require_clash_free` (None: the `require_clash_free` attribute, default False) adds a fourth, on cut-off (pocket)
+        graphs, in the same rounds and launch: some linker atom of chain[0] lies closer to a pocket atom than
+        molecule_builder.clash_table(is_geom) allows for the two atom types (this project's own predicate, stated at
+        dl_molecule_checks in the header; fragment atoms are not checked). `last_clash_free` (B,) CPU bool tells which rows
+        pass. Refusals as for require_valid, plus ValueError on FC graphs and for InpaintingEDM.
         The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
         and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
         device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
@@ -543,10 +571,10 @@ class EDM(torch.nn.Module):
         n_samples = x.size(0)
         dev = x.device
         self.last_attempts = None
-        self.last_connected = self.last_valid = None
+        self.last_connected = self.last_valid = self.last_clash_free = None
         start = self._start(start_step, n_samples)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
-        check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x)
+        check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free)
         recover = retries > 0 or check != 0 # the recovery entry point: seeds used and attempts come back
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
         full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
@@ -608,6 +636,8 @@ class EDM(torch.nn.Module):
             self.last_connected = (out['passed'].cpu() & _native.CHECK_CONNECTED) != 0
         if check & _native.CHECK_VALENCE:
             self.last_valid = (out['passed'].cpu() & _native.CHECK_VALENCE) != 0
+        if check & _native.CHECK_CLASH:
+            self.last_clash_free = (out['passed'].cpu() & _native.CHECK_CLASH) != 0
         if out['bad']:
             exc = self._nan_exception(out['flags'], start)
             if recover:
@@ -620,7 +650,7 @@ class EDM(torch.nn.Module):
 
     @torch.no_grad()
     def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                    max_molecules=256, start_step=None, require_valid=None):
+                    max_molecules=256, start_step=None, require_valid=None, require_clash_free=None):
         """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
         edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
         (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
@@ -637,10 +667,11 @@ class EDM(torch.nn.Module):
         aggregation_method='mean' on FC graphs, where the reference divides by the padded N, only with requests of the same
         N. With `devices` set, whole launches are dealt to the listed devices by their cost (distributed.deal_launches), and
         each device runs its launches in order, from a host thread of its own; a launch is never split.
-        `nan_retries`, `require_connected` and `require_valid` run their rounds inside each launch, over its rows. Rows still diverging after
+        `nan_retries`, `require_connected`, `require_valid` and `require_clash_free` run their rounds inside each launch, over its rows. Rows still diverging after
         the last round raise once, after every launch: the FoundNaNException of the first such request, its index sets
         local to that request, with `request` = k and `results` = every request's chain (and `chain` = its own when rounds
-        ran, as in sample_chain). `last_seeds_many`, `last_attempts_many`, `last_connected_many` and `last_valid_many` hold per
+        ran, as in sample_chain). `last_seeds_many`, `last_attempts_many`, `last_connected_many`, `last_valid_many` and
+        `last_clash_free_many` hold per
         request what last_seeds, last_attempts, last_connected and last_valid would hold after its own call; `last_loop_ms_many` holds (device,
         requests, loop ms) per launch. The single-call attributes are left as they were.
         Raises ValueError for an empty list, the batch stream (its draws depend on B and N), noise= or a replaced draw
@@ -695,7 +726,7 @@ class EDM(torch.nn.Module):
         if dev.type != 'cuda':
             raise ValueError(f"sample_many needs CUDA inputs (got {dev})")
         retries = self._nan_retries(nan_retries, seeds, None, None, x0)
-        check = self._checks(require_connected, require_valid, seeds, None, None, x0)
+        check = self._checks(require_connected, require_valid, seeds, None, None, x0, require_clash_free)
         recover = retries > 0 or check != 0
         self.dynamics._check_graph_type()
         if seeds is None:
@@ -746,7 +777,7 @@ class EDM(torch.nn.Module):
             raise
         results, flags = [None] * len(requests), [None] * len(requests)
         seeds_many, attempts_many = list(cpu_seeds), [None] * len(requests)
-        connected_many, valid_many = [None] * len(requests), [None] * len(requests)
+        connected_many, valid_many, clash_free_many = [None] * len(requests), [None] * len(requests), [None] * len(requests)
         for (ks, _), finish in zip(launches, finishes):
             out = finish()
             rows = [sizes[k] for k in ks]
@@ -765,8 +796,10 @@ class EDM(torch.nn.Module):
                     connected_many[k] = (parts['passed'][j] & _native.CHECK_CONNECTED) != 0
                 if check & _native.CHECK_VALENCE:
                     valid_many[k] = (parts['passed'][j] & _native.CHECK_VALENCE) != 0
+                if check & _native.CHECK_CLASH:
+                    clash_free_many[k] = (parts['passed'][j] & _native.CHECK_CLASH) != 0
         self.last_seeds_many, self.last_attempts_many, self.last_connected_many = seeds_many, attempts_many, connected_many
-        self.last_valid_many = valid_many
+        self.last_valid_many, self.last_clash_free_many = valid_many, clash_free_many
         self.last_loop_ms_many = [(slots[slot_of[i]][0], sorted(ks), loop_ms[i]) for i, (ks, _) in enumerate(launches)]
         for k, f in enumerate(flags):
             if f.any():
@@ -812,6 +845,7 @@ class EDM(torch.nn.Module):
         # molecule checks: every row's verdict bits, and the tables they read on each slice's device
         passed = torch.empty(n_samples, dtype=torch.int32, device=dev) if check else None
         tables = self._check_tables(check) if check else None
+        clash = clash_table(self.is_geom) if check & _native.CHECK_CLASH else None
         whole = places == [dev]             # one slice, the whole batch where it is: it samples the caller's tensors
         results, calls, parts = [], [], []  # (status, consumed) of every slice; every slice's call; every slice's tensors
 
@@ -830,15 +864,16 @@ class EDM(torch.nn.Module):
                             *((torch.empty(hi - lo, dtype=torch.int64, device=where),
                                torch.empty(hi - lo, dtype=torch.int32, device=where)) if recover else (None, None)),
                             torch.empty(hi - lo, dtype=torch.int32, device=where) if check else None)
-            part = part + (None if tables is None else [t.to(where) for t in tables],)
+            part = part + (None if tables is None else [t.to(where) for t in tables],
+                           None if clash is None else clash.to(where))
             parts.append(part)              # alive until the flags have been read below
-            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, tables_i = part
+            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, tables_i, clash_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
             rng_i = None if rng is None else (rng[0], rng[1], rng[2] + lo, rng[3])
             calls.append((dev_i, functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
-                (retries, used_i, attempts_i, check, tables_i, passed_i) if recover else None, start)))
+                (retries, used_i, attempts_i, check, tables_i, passed_i) if recover else None, start, clash_i)))
 
         def finish():
             if not whole:
@@ -910,7 +945,7 @@ class InpaintingEDM(EDM):
 
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
-                     require_valid=None):
+                     require_valid=None, require_clash_free=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -918,11 +953,13 @@ class InpaintingEDM(EDM):
         in which case the replacement draws them. `batch_slice=(b0, B_full)` and `seeds` as in EDM.sample_chain: with
         seeds, molecule b's 2T+3 raw draws are those of the molecule sampled alone after torch.cuda.manual_seed(seeds[b]),
         masked and projected per molecule as always. `nan_retries`, `require_connected` and `require_valid` as in EDM.sample_chain;
-        the checks cover every atom of the molecule. `start_step` raises ValueError unless None."""
+        the checks cover every atom of the molecule. `start_step` raises ValueError unless None, and `require_clash_free`
+        unless None or False: this loop re-noises the pocket."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
-                                    require_connected=require_connected, start_step=start_step, require_valid=require_valid)
+                                    require_connected=require_connected, start_step=start_step, require_valid=require_valid,
+                                    require_clash_free=require_clash_free)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

@@ -2,7 +2,8 @@
 GPU (`dl_bond_orders`) instead of an O(n^2) Python loop with one `.item()` per atom pair.
 RDKit molecule construction (`build_molecule`, molecule_builder.py:29-42) stays with the caller: RDKit is not part of
 the path (SURVEY.md section 8(f) rank 4). `connected` and `valence_ok` decide on the device what the reference's
-`validity_and_connectivity` asks of those molecules, the latter as "explicit valence within a table".
+`validity_and_connectivity` asks of those molecules, the latter as "explicit valence within a table". `clash_free` is this
+project's own check, with no reference counterpart: whether a linker runs into the pocket.
 """
 import torch
 
@@ -26,6 +27,8 @@ MARGINS_EDM = [10, 5, 2]                                                        
 # The most bond order an atom of each element may carry in valences / valence_ok: the largest entry of RDKit's default
 # valence list for the element.
 MAX_VALENCE = {'C': 4, 'N': 3, 'O': 2, 'F': 1, 'S': 6, 'Cl': 1, 'Br': 1, 'I': 5, 'P': 7}
+# Bondi van der Waals radii in Angstrom (J. Phys. Chem. 68, 441 (1964)), for the pocket-clash check's default table.
+VDW_RADII = {'C': 1.70, 'N': 1.55, 'O': 1.52, 'F': 1.47, 'P': 1.80, 'S': 1.80, 'Cl': 1.75, 'Br': 1.85, 'I': 1.98}
 
 
 def threshold_tables(is_geom, margins=MARGINS_EDM):
@@ -61,6 +64,19 @@ def check_tables(is_geom, require, max_valence=None):
     if mv.shape != (thr[0].shape[0],):
         raise ValueError(f"max_valence holds one entry per atom type, {thr[0].shape[0]} (got shape {tuple(mv.shape)})")
     return thr + [mv]
+
+
+def clash_table(is_geom, scale=0.75):
+    """(T,T) fp32 clash distances in pm for the pocket-clash check (sample_chain(require_clash_free=True), clash_free): entry
+    [a][b] = fp32(100 * scale * (R_a + R_b)), evaluated in double, with R the VDW_RADII of the two atom types (IDX2ATOM, or
+    GEOM_IDX2ATOM with is_geom). Symmetric; the check reads [min type][max type]. A linker atom closer than that to a pocket
+    atom clashes with it. The default scale, 0.75, is a common protein-ligand contact tolerance (C-C 2.55 A, N-O 2.30 A, below
+    hydrogen-bond distances); it is a default, not validated against any docking tool. A caller may set entries negative
+    to exempt a pair (e.g. a covalent warhead's element)."""
+    idx2atom = GEOM_IDX2ATOM if is_geom else IDX2ATOM
+    T = len(idx2atom)
+    r = [VDW_RADII[idx2atom[t]] for t in range(T)]
+    return torch.tensor([[100.0 * scale * (r[a] + r[b]) for b in range(T)] for a in range(T)], dtype=torch.float32)
 
 
 @torch.no_grad()
@@ -133,6 +149,51 @@ def valence_ok(xh, node_mask, is_geom, pocket_only=None, max_valence=None):
     Chem.SanitizeMol; that equivalence has not been verified against RDKit."""
     passed, _ = _molecule_check(xh, node_mask, is_geom, pocket_only, max_valence, _native.CHECK_VALENCE, False)
     return (passed & _native.CHECK_VALENCE) != 0
+
+
+@torch.no_grad()
+def pocket_clashes(xh, node_mask, linker_mask, pocket_only, is_geom, clash=None):
+    """(B,N) int32 on the device (dl_clash_check, the check behind sample_chain(require_clash_free=True)): for each linker
+    atom -- node_mask != 0, linker_mask != 0, pocket_only == 0 -- the number of pocket atoms (node_mask != 0, pocket_only !=
+    0) it clashes with, and 0 on every other row. Two atoms clash when 100 |x_i - x_j| in pm is below clash[min type][max
+    type] and that entry is >= 0; `clash` is a (T,T) table, by default clash_table(is_geom). `xh` is chain[0]-style
+    (B,N,3+F) and the atom types are argmax of its first T feature columns, as in connected(). A NaN coordinate clashes with
+    nothing. To vet inputs, pass the fragment rows as `linker_mask`."""
+    return _clash_check(xh, node_mask, linker_mask, pocket_only, is_geom, clash, True)[1]
+
+
+def clash_free(xh, node_mask, linker_mask, pocket_only, is_geom, clash=None):
+    """(B,) bool on the device: whether no linker atom of a molecule clashes with a pocket atom (pocket_clashes); a molecule
+    without linker or pocket atoms passes."""
+    passed, _ = _clash_check(xh, node_mask, linker_mask, pocket_only, is_geom, clash, False)
+    return (passed & _native.CHECK_CLASH) != 0
+
+
+@torch.no_grad()
+def _clash_check(xh, node_mask, linker_mask, pocket_only, is_geom, clash, want_counts):
+    """dl_clash_check on a chain[0]-style batch: ((B,) int32 verdict bits, (B,N) int32 counts or None)."""
+    dev = xh.device
+    if dev.type != 'cuda':
+        raise RuntimeError("the molecule checks run on the GPU (no CPU fallback); move the tensors to the device")
+    B, N = xh.shape[:2]
+    T = len(GEOM_IDX2ATOM if is_geom else IDX2ATOM)
+    table = clash_table(is_geom) if clash is None else torch.as_tensor(clash, dtype=torch.float32)
+    if table.shape != (T, T):
+        raise ValueError(f"clash is a ({T}, {T}) table, one row and column per atom type (got shape {tuple(table.shape)})")
+    table = table.to(dev).contiguous()
+    xs = xh.float().contiguous()
+    nm = (node_mask.reshape(B, N) != 0).to(torch.int8).contiguous()
+    lm = linker_mask.reshape(B, N).float().contiguous()
+    po = pocket_only.reshape(B, N, 1).float().contiguous()
+    passed = torch.empty(B, dtype=torch.int32, device=dev)
+    counts = torch.empty((B, N), dtype=torch.int32, device=dev) if want_counts else None
+    lib = _native.load_library()
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream().cuda_stream
+        _native.check(lib.dl_clash_check(B, N, T, table.data_ptr(), xs.data_ptr(), xs.shape[2], nm.data_ptr(),
+                                         lm.data_ptr(), po.data_ptr(), 1, passed.data_ptr(),
+                                         None if counts is None else counts.data_ptr(), st), "dl_clash_check")
+    return passed, counts
 
 
 def build_xae_molecule(positions, atom_types, is_geom, margins=MARGINS_EDM):

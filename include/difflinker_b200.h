@@ -25,6 +25,8 @@
  *   either, also resampling the molecules that are      dl_sample_chain_seeded_retry_checked, dl_molecule_check
  *     disconnected (is_connected, src/metrics.py:20-27, on the molecules of src/lightning.py:364-377) or have an atom
  *     beyond its valence (the explicit-valence part of validity, src/metrics.py:12-17; see dl_molecule_checks)
+ *   either on pocket graphs, also resampling the        dl_set_clash_table, DL_CHECK_CLASH, dl_clash_check
+ *     molecules whose linker clashes with the pocket (no reference API; see dl_molecule_checks)
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   build_xae_molecule           src/molecule_builder.py:44-102       dl_bond_orders
  *   frame restore + .xyz text    generate.py:163-171, src/visualizer.py:14-31   dl_restore_frame, dl_format_xyz
@@ -272,12 +274,24 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
  * an atom beyond its element's largest allowed valence is how Chem.SanitizeMol (is_valid, src/metrics.py:12-17) is expected
  * to reject them; that "SanitizeMol fails iff this check fails" has NOT been verified against RDKit. A caller with stricter
  * or looser chemistry passes their own table.
+ *   DL_CHECK_CLASH (this library's own predicate; the reference has no clash test) holds iff no linker atom clashes with a
+ *              pocket atom. Cut-off (pocket) graphs only, evaluated on chain[0] with the types above:
+ *     linker atoms  rows with node_mask != 0, linker_mask != 0 and the last context column == 0. Fragment atoms are not
+ *                   checked: they are inputs, which no resample moves.
+ *     pocket atoms  rows with node_mask != 0 and the last context column != 0.
+ *     clash         100 |x_i - x_j| in pm, with dl_bond_orders' arithmetic, is below clash[min t][max t] of the caller's
+ *                   (n_types,n_types) table and that entry is >= 0; a negative entry means the pair never clashes (e.g. a
+ *                   covalent warhead's element against the residue it binds).
+ *   A molecule with no linker atom or no pocket atom passes. A NaN coordinate compares false and clashes with nothing
+ *   (divergence is the NaN flag's business). The table travels outside this struct, through dl_set_clash_table and
+ *   dl_clash_check; molecule_builder.clash_table builds a default, 75% of the sum of the two elements' Bondi van der Waals
+ *   radii, a common protein-ligand contact tolerance that has not been validated against any docking tool.
  */
-enum { DL_CHECK_CONNECTED = 1, DL_CHECK_VALENCE = 2 };
+enum { DL_CHECK_CONNECTED = 1, DL_CHECK_VALENCE = 2, DL_CHECK_CLASH = 4 };
 typedef struct dl_molecule_checks {
   int32_t require;             /* OR of DL_CHECK_*, at least one: which verdicts make a row fail and be resampled */
   int32_t n_types;             /* columns of h that hold the atom type */
-  const float* thr1;           /* (n_types,n_types) fp32 DEVICE, as dl_bond_orders */
+  const float* thr1;           /* (n_types,n_types) fp32 DEVICE, as dl_bond_orders; needed unless DL_CHECK_CLASH alone */
   const float* thr2;           /* needed for DL_CHECK_VALENCE only */
   const float* thr3;
   const int32_t* max_valence;  /* (n_types) int32 DEVICE; DL_CHECK_VALENCE only */
@@ -291,7 +305,9 @@ typedef struct dl_molecule_checks {
  * break the valence rule cannot be repaired by a new linker: it is resampled every round and comes back with the bit cleared
  * (vet inputs with dl_molecule_check).
  *   passed   (B) int32 DEVICE out: the OR of the DL_CHECK_* bits row b's returned molecule satisfies, among those required
- * The other arguments are those of dl_sample_chain_seeded_retry. 1 <= n_types <= in_node_nf, N <= 8192.
+ * The other arguments are those of dl_sample_chain_seeded_retry. 1 <= n_types <= in_node_nf, N <= 8192. DL_CHECK_CLASH reads
+ * the linker rows of linker_mask (of the sub-batch in the rounds) and the engine's clash table; it is DL_ERR_INVALID without
+ * a table (dl_set_clash_table), on DL_GRAPH_FC (no pocket rows) and with DL_SAMPLER_INPAINT (whose loop re-noises the pocket).
  */
 dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
                                                int32_t keep_frames, const float* xh, const int8_t* node_mask,
@@ -309,11 +325,32 @@ dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, in
  *   passed    (B) int32 out, as above
  *   valence   (B,N) int32 out or NULL; needs DL_CHECK_VALENCE: each checked atom's valence, 0 on every other row (for a
  *             hand-off to RDKit, and for tests)
- * 1 <= N <= 8192.
+ * 1 <= N <= 8192. require takes DL_CHECK_CONNECTED and DL_CHECK_VALENCE only; the clash check alone is dl_clash_check.
  */
 dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
                             const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
                             int32_t* passed, int32_t* valence, void* stream);
+/*
+ * The clash table of the following dl_sample_chain_seeded_retry_checked calls of this engine that require DL_CHECK_CLASH:
+ * (checks->n_types)^2 fp32 DEVICE, in pm, [min type][max type] (see dl_molecule_checks), read by those calls and kept alive
+ * by the caller while they run. Sticky, like dl_set_start_step; NULL clears it (the default).
+ */
+dl_status dl_set_clash_table(dl_engine* e, const float* clash);
+/*
+ * DL_CHECK_CLASH alone, on any (B,N) batch, without an engine. DEVICE buffers, enqueued on `stream`.
+ *   clash       (n_types,n_types) fp32, in pm, as dl_set_clash_table
+ *   xh          (B,N,>=3+n_types) fp32, row stride xh_row_stride, as dl_molecule_check
+ *   node_mask   (B,N) int8
+ *   linker_mask (B,N) fp32: the rows checked against the pocket (to vet a fragment, pass the fragment rows here)
+ *   context     (B,N,context_nf) fp32, context_nf >= 1: column context_nf - 1 marks the pocket rows
+ *   passed      (B) int32 out: DL_CHECK_CLASH or 0
+ *   clashes     (B,N) int32 out or NULL: for each linker atom, the number of pocket atoms it clashes with; 0 on every
+ *               other row
+ * 1 <= n_types <= xh_row_stride - 3, 1 <= N <= 8192.
+ */
+dl_status dl_clash_check(int32_t B, int32_t N, int32_t n_types, const float* clash, const float* xh, int32_t xh_row_stride,
+                         const int8_t* node_mask, const float* linker_mask, const float* context, int32_t context_nf,
+                         int32_t* passed, int32_t* clashes, void* stream);
 /* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_seeded_retry(_checked), each from its
  * row gather to its row scatter -- including the wait for the host to capture the sub-batch's step graph -- summed over the
  * rounds; 0 when no round ran. */
