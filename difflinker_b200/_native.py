@@ -46,6 +46,11 @@ class DLMoleculeChecks(C.Structure):
         return cls(require, tables[0].shape[0], *ptrs)
 
 
+class DLSizeRedraw(C.Structure):
+    _fields_ = [("C", C.c_int32), ("logits_row_stride", C.c_int32), ("logits", C.c_void_p), ("sizes", C.c_void_p),
+                ("n_frag", C.c_void_p), ("linker_x", C.c_void_p)]
+
+
 class DLStepCoef(C.Structure):
     _fields_ = [("t", C.c_float), ("a", C.c_float), ("b", C.c_float), ("c", C.c_float), ("frame", C.c_int32),
                 ("qa", C.c_float), ("qb", C.c_float), ("pad", C.c_float)]
@@ -73,6 +78,11 @@ SYMBOLS = {
                                             _P, _P, _P]),
     "dl_sample_chain_seeded_retry_checked": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                                     _P, _I32, _P, _P, C.POINTER(DLMoleculeChecks), _P, _P]),
+    "dl_sample_chain_seeded_retry_sized": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                                  _P, _I32, _P, _P, C.POINTER(DLMoleculeChecks), _P,
+                                                  C.POINTER(DLSizeRedraw), _P, _P]),
+    "dl_size_draw": (_I32, [_I32, _I32, _P, _I32, _P, _P, _I32, _P, _P]),
+    "dl_size_uniform": (C.c_double, [C.c_uint64]),
     "dl_molecule_check": (_I32, [_I32, _I32, C.POINTER(DLMoleculeChecks), _P, _I32, _P, _P, _I32, _I32, _P, _P, _P]),
     "dl_set_clash_table": (_I32, [_P, _P]),
     "dl_clash_check": (_I32, [_I32, _I32, _I32, _P, _P, _I32, _P, _P, _P, _I32, _P, _P, _P]),

@@ -50,11 +50,12 @@ def collate(batch):
     return _add_masks(_stack_and_pad(batch), "pocket_mask" in batch[0])
 
 
-def create_templates_for_linker_generation(data, linker_sizes):
+def create_templates_for_linker_generation(data, linker_sizes, n_nodes=None):
     """Keep the fragment rows of every padded attribute and append `linker_size` template rows (ones for linker_mask,
     zeros elsewhere), then re-collate (datasets.py:483-512). Batched: the reference decouples the batch into one dict per
     molecule and collates again (a few thousand tiny ops per call on the GPU); the same tensors come out of a handful of
-    masked selects on the padded batch -- one host sync for the new padded length."""
+    masked selects on the padded batch -- one host sync for the new padded length. `n_nodes` pads the template to that
+    many rows instead of the largest molecule's (it must not be smaller)."""
     fm = data["fragment_mask"]
     dev = fm.device
     bs, n_old = fm.shape[0], fm.shape[1]
@@ -62,6 +63,10 @@ def create_templates_for_linker_generation(data, linker_sizes):
     sizes = torch.as_tensor(linker_sizes, device=dev).reshape(-1).long()
     n_tot = n_frag + sizes
     n_new = int(n_tot.max())
+    if n_nodes is not None:
+        if n_nodes < n_new:
+            raise ValueError(f"n_nodes = {n_nodes} is fewer rows than the largest template's {n_new}")
+        n_new = n_nodes
     idx = torch.arange(n_new, device=dev)[None, :]
     is_frag = (idx < n_frag[:, None])[:, :, None]
     is_link = ((idx >= n_frag[:, None]) & (idx < n_tot[:, None]))[:, :, None]

@@ -1214,6 +1214,40 @@ CheckArgs check_args(const dl_engine* e, const dl_molecule_checks& ck, const flo
                     e->cfg.graph_type != DL_GRAPH_FC, passed);
 }
 
+// What is wrong with the checks of a dl_sample_chain_seeded_retry_checked / _sized call, or null.
+const char* checked_error(const dl_engine* e, int32_t sampler, int N, const dl_molecule_checks* checks) {
+  const char* why = checks_error(checks, N, e->cfg.in_node_nf, true);
+  if (!why && (checks->require & DL_CHECK_CLASH)) {
+    if (!e->clash_table) why = "DL_CHECK_CLASH needs a clash table (dl_set_clash_table)";
+    else if (e->cfg.graph_type == DL_GRAPH_FC) why = "DL_CHECK_CLASH needs a pocket: DL_GRAPH_FC graphs have none";
+    else if (sampler == DL_SAMPLER_INPAINT) why = "DL_CHECK_CLASH does not take DL_SAMPLER_INPAINT, which re-noises the pocket";
+  }
+  return why;
+}
+
+// What is wrong with a dl_size_redraw for B molecules of N rows, or null. Copies the size table and n_frag to the host
+// through `st` (the call blocks anyway) to check that every redrawn template fits N rows.
+const char* redraw_error(int32_t sampler, int B, int N, const dl_size_redraw* rz, cudaStream_t st) {
+  if (sampler == DL_SAMPLER_INPAINT) return "DL_SAMPLER_INPAINT samples every atom of the batch: it has no linker size to redraw";
+  if (rz->C < 1 || rz->logits_row_stride < rz->C) return "redraw->C must be >= 1 and redraw->logits_row_stride >= C";
+  if (!rz->logits || !rz->sizes || !rz->n_frag || !rz->linker_x) return "null redraw->logits, sizes, n_frag or linker_x";
+  if (B < 1 || N < 1) return "B and N must be >= 1";
+  std::vector<int32_t> sizes(rz->C), n_frag(B);
+  if (cudaMemcpyAsync(sizes.data(), rz->sizes, sizes.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+      cudaMemcpyAsync(n_frag.data(), rz->n_frag, n_frag.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+      cudaStreamSynchronize(st) != cudaSuccess) {
+    cudaGetLastError();
+    return "redraw->sizes and n_frag must be DEVICE buffers";
+  }
+  const int32_t max_size = *std::max_element(sizes.begin(), sizes.end());
+  if (*std::min_element(sizes.begin(), sizes.end()) < 0) return "redraw->sizes must be >= 0";
+  for (int b = 0; b < B; ++b) {
+    if (n_frag[b] < 0) return "redraw->n_frag must be >= 0";
+    if ((int64_t)n_frag[b] + max_size > N) return "N < n_frag[b] + max(sizes) for some b: pad the batch to its capacity";
+  }
+  return nullptr;
+}
+
 // dl_sample_chain_seeded_retry, and with `ck` its molecule checks, whose verdicts go to `passed`: a row then fails if its NaN
 // flag is set or a required bit is missing, and a resampled row replaces the caller's unless the caller's row is finite and
 // the new one diverged.
@@ -1221,7 +1255,8 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
                        const int8_t* node_mask, const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
                        const float* context, const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
                        int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
-                       const dl_molecule_checks* ck, int32_t* passed, void* stream) {
+                       const dl_molecule_checks* ck, int32_t* passed, const dl_size_redraw* rz, int32_t* sizes_used,
+                       void* stream) {
   e->retry_ms = 0.f;
   dl_status s = dl_sample_chain_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask,
                                        context, seeds, coef, norm, chain, nan_flags, stream);
@@ -1253,7 +1288,8 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
               i_fm = sl.out(n * 4), i_lm = sl.out(n * 4), i_em = sl.add(nullptr, n * N, fc_em),
               i_ctx = sl.add(nullptr, n * C * 4, context != nullptr && C > 0), i_sd = sl.out((size_t)Bs * 8),
               i_ch = sl.out((size_t)keep_frames * n * xd * 4), i_fl = sl.out((size_t)Bs * 4),
-              i_ps = sl.add(nullptr, (size_t)Bs * 4, ck != nullptr), i_tk = sl.add(nullptr, (size_t)Bs * 4, ck != nullptr);
+              i_ps = sl.add(nullptr, (size_t)Bs * 4, ck != nullptr), i_tk = sl.add(nullptr, (size_t)Bs * 4, ck != nullptr),
+              i_sz = sl.add(nullptr, (size_t)Bs * 4, rz != nullptr);
     if ((s = stage_inputs(e->sub_rows, sl, st)) != DL_OK) return s;   // the row list goes to the device once per round
     CK(cudaEventRecord(e->ev_g0, st));
     RowGatherArgs ga{};
@@ -1264,7 +1300,14 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     ga.s_xh = sl.at<float>(i_xh); ga.s_fragment_mask = sl.at<float>(i_fm); ga.s_linker_mask = sl.at<float>(i_lm);
     ga.s_context = sl.at<float>(i_ctx); ga.s_node_mask = sl.at<int8_t>(i_nm); ga.s_edge_mask = sl.at<int8_t>(i_em);
     ga.s_seeds = sl.at<unsigned long long>(i_sd);
-    k_gather_rows<<<Bs, 256, 0, st>>>(ga);
+    const RowSizeArgs za{sl.at<int32_t>(i_sz), sizes_used};
+    if (rz) {
+      const RowResizeArgs ra{SizeDrawArgs{rz->C, rz->logits_row_stride, rz->logits, rz->sizes}, rz->n_frag, rz->linker_x,
+                             sl.at<int32_t>(i_sz)};
+      k_gather_rows<true><<<Bs, 256, 0, st>>>(ga, ra);
+    } else {
+      k_gather_rows<false><<<Bs, 256, 0, st>>>(ga);
+    }
     LAUNCH_CHECK();
     e->launches += 1;
     {
@@ -1285,7 +1328,10 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
       CK(launch_molecule_check(require, ca, ClashArgs{ga.s_linker_mask, e->clash_table, nullptr}, Bs, st));
       e->launches += 1;
       sa.take = ca.take; sa.s_passed = ca.passed; sa.passed = passed;
-      k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
+      if (rz) k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa, za);
+      else k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
+    } else if (rz) {
+      k_scatter_rows<false><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa, za);
     } else {
       k_scatter_rows<false><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
     }
@@ -1323,7 +1369,8 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
   if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
   if (!nan_flags || !seeds_used || !attempts) { set_err("null argument (nan_flags, seeds_used or attempts)"); return DL_ERR_INVALID; }
   return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
-                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, nullptr, nullptr, stream);
+                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, nullptr, nullptr, nullptr, nullptr,
+                      stream);
 }
 
 dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
@@ -1339,19 +1386,58 @@ dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, in
     set_err("null argument (nan_flags, seeds_used, attempts or passed)");
     return DL_ERR_INVALID;
   }
-  const char* why = checks_error(checks, N, e->cfg.in_node_nf, true);
-  if (!why && (checks->require & DL_CHECK_CLASH)) {
-    if (!e->clash_table) why = "DL_CHECK_CLASH needs a clash table (dl_set_clash_table)";
-    else if (e->cfg.graph_type == DL_GRAPH_FC) why = "DL_CHECK_CLASH needs a pocket: DL_GRAPH_FC graphs have none";
-    else if (sampler == DL_SAMPLER_INPAINT) why = "DL_CHECK_CLASH does not take DL_SAMPLER_INPAINT, which re-noises the pocket";
-  }
+  const char* why = checked_error(e, sampler, N, checks);
   if (why) {
     set_err("dl_sample_chain_seeded_retry_checked: %s", why);
     return DL_ERR_INVALID;
   }
   return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
-                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, passed, stream);
+                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, passed, nullptr, nullptr,
+                      stream);
 }
+
+dl_status dl_sample_chain_seeded_retry_sized(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
+                                             int32_t keep_frames, const float* xh, const int8_t* node_mask,
+                                             const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
+                                             const float* context, const uint64_t* seeds, const dl_step_coef* coef,
+                                             const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries,
+                                             uint64_t* seeds_used, int32_t* attempts, const dl_molecule_checks* checks,
+                                             int32_t* passed, const dl_size_redraw* redraw, int32_t* sizes_used,
+                                             void* stream) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
+  if (!nan_flags || !seeds_used || !attempts || (checks && !passed) || !redraw || !sizes_used) {
+    set_err("dl_sample_chain_seeded_retry_sized: null argument (nan_flags, seeds_used, attempts, passed with checks, "
+            "redraw or sizes_used)");
+    return DL_ERR_INVALID;
+  }
+  const char* why = checks ? checked_error(e, sampler, N, checks) : nullptr;
+  if (!why && cudaSetDevice(e->cfg.device) != cudaSuccess) why = "cudaSetDevice failed";
+  if (!why) why = redraw_error(sampler, B, N, redraw, reinterpret_cast<cudaStream_t>(stream));
+  if (why) {
+    set_err("dl_sample_chain_seeded_retry_sized: %s", why);
+    return DL_ERR_INVALID;
+  }
+  return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
+                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, passed, redraw, sizes_used,
+                      stream);
+}
+
+dl_status dl_size_draw(int32_t B, int32_t C, const float* logits, int32_t logits_row_stride, const int32_t* sizes,
+                       const uint64_t* seeds, int32_t attempt, int32_t* out_sizes, void* stream) {
+  const char* why = nullptr;
+  if (B <= 0 || C <= 0) why = "B and C must be >= 1";
+  else if (logits_row_stride < C) why = "logits_row_stride must be >= C";
+  else if (!logits || !sizes || !seeds || !out_sizes) why = "null argument";
+  if (why) { set_err("dl_size_draw: %s", why); return DL_ERR_INVALID; }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  k_size_draw<<<(B + 7) / 8, 256, 0, st>>>(SizeDrawArgs{C, logits_row_stride, logits, sizes}, B,
+                                           reinterpret_cast<const unsigned long long*>(seeds), attempt, out_sizes);
+  CK(cudaGetLastError());
+  return DL_OK;
+}
+
+double dl_size_uniform(uint64_t seed) { return size_uniform(seed); }
 
 dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
                             const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,

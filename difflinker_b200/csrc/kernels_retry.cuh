@@ -17,6 +17,66 @@ __host__ __device__ inline unsigned long long retry_seed(unsigned long long seed
   return z ^ (z >> 31);
 }
 
+// dl_size_uniform: the uniform in [0, 1) that draws a molecule's linker size from `seed` -- the top 53 bits of the
+// splitmix64 finaliser of seed ^ SIZE_DRAW_TAG, times 2^-53. The tag keeps it apart from the Philox streams and from
+// retry_seed, which feed no finaliser with it.
+constexpr unsigned long long SIZE_DRAW_TAG = 0x6C696E6B65722D6Eull;   // "linker-n" in ASCII
+__host__ __device__ inline double size_uniform(unsigned long long seed) {
+  unsigned long long z = seed ^ SIZE_DRAW_TAG;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  z ^= z >> 31;
+  return (double)(z >> 11) * 0x1.0p-53;
+}
+
+// The index dl_size_draw draws from the C logits l (stated at dl_size_draw in the header): in fp64 and in index order,
+// m = max l, e_i = exp(l_i - m), S = sum e_i, c_i = e_0 + ... + e_i; the first i with u * S < c_i, else the last i with
+// e_i > 0. Warp-collective (all 32 lanes, converged); every lane returns the index. The sums run in index order on every
+// lane -- each lane adds the 32 values of a chunk one after another through shuffles -- so they are the sequential sums.
+__device__ inline int size_draw_index(const float* l, int C, double u) {
+  const int lane = threadIdx.x & 31;
+  double m = -INFINITY;
+  for (int i = lane; i < C; i += 32) m = fmax(m, (double)l[i]);
+  for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+  double S = 0.0;
+  int last = 0;
+  for (int i0 = 0; i0 < C; i0 += 32) {
+    const double e = i0 + lane < C ? exp((double)l[i0 + lane] - m) : 0.0;
+    for (int k = 0; k < 32 && i0 + k < C; ++k) S += __shfl_sync(0xffffffffu, e, k);
+    const unsigned pos = __ballot_sync(0xffffffffu, e > 0.0);
+    if (pos) last = i0 + 31 - __clz(pos);
+  }
+  const double t = u * S;
+  double c = 0.0;
+  for (int i0 = 0; i0 < C; i0 += 32) {
+    const double e = i0 + lane < C ? exp((double)l[i0 + lane] - m) : 0.0;
+    double mine = 0.0;
+    for (int k = 0; k < 32 && i0 + k < C; ++k) {
+      c += __shfl_sync(0xffffffffu, e, k);
+      if (k == lane) mine = c;
+    }
+    const unsigned hit = __ballot_sync(0xffffffffu, i0 + lane < C && t < mine);
+    if (hit) return i0 + __ffs(hit) - 1;
+  }
+  return last;
+}
+
+// The size tables of a redraw (dl_size_redraw of the header), as the kernels read them.
+struct SizeDrawArgs {
+  int C, logits_stride;
+  const float* logits;                   // (B, logits_stride): molecule b's C logits from column 0
+  const int32_t* sizes;                  // (C)
+};
+
+// dl_size_draw: one warp per molecule b writes sizes[index drawn with size_uniform(retry_seed(seeds[b], attempt))].
+__global__ void __launch_bounds__(256) k_size_draw(SizeDrawArgs a, int B, const unsigned long long* seeds, int attempt,
+                                                   int32_t* out) {
+  const int b = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (b >= B) return;                                 // whole warps leave together
+  const int i = size_draw_index(a.logits + (size_t)b * a.logits_stride, a.C, size_uniform(retry_seed(seeds[b], attempt)));
+  if ((threadIdx.x & 31) == 0) out[b] = a.sizes[i];
+}
+
 // One recovery round: the Bs failed molecules rows[i] (ascending batch rows) of the B-molecule batch. The src_* pointers
 // are the caller's full-batch inputs, the dst_* ones the sub-batch workspace, row i holding molecule rows[i].
 struct RowGatherArgs {
@@ -30,8 +90,23 @@ struct RowGatherArgs {
   unsigned long long* s_seeds;           // retry_seed(seeds[rows[i]], attempt)
 };
 
+// What a resizing round reads and writes besides RowGatherArgs / RowScatterArgs. Kernel parameters of their own, passed to
+// the resizing instantiations only, so the code of the fixed-size ones stays as it was.
+struct RowResizeArgs {
+  SizeDrawArgs draw;
+  const int32_t* n_frag;                 // (B) fragment rows of every molecule (pocket rows included)
+  const float* linker_x;                 // (B, 3) the xh coordinates of molecule b's linker rows in its template
+  int32_t* s_sizes;                      // (Bs) out: the size drawn for sub-batch row i
+};
+struct RowSizeArgs {
+  const int32_t* s_sizes;                // (Bs) the sub-batch's sizes
+  int32_t* sizes;                        // (B) the caller's sizes: written where a row is taken
+};
+
 // One CTA per failed molecule: copies its rows of every input, and derives its seed for this attempt.
+template <bool RESIZE>
 __global__ void __launch_bounds__(256) k_gather_rows(RowGatherArgs a) {
+  static_assert(!RESIZE, "the resizing gather takes RowResizeArgs");
   const int i = blockIdx.x;
   const size_t b = a.rows[i], N = a.N;
   for (size_t k = threadIdx.x; k < N * a.xd; k += blockDim.x) a.s_xh[i * N * a.xd + k] = a.xh[b * N * a.xd + k];
@@ -45,6 +120,48 @@ __global__ void __launch_bounds__(256) k_gather_rows(RowGatherArgs a) {
   if (a.edge_mask)
     for (size_t k = threadIdx.x; k < N * N; k += blockDim.x) a.s_edge_mask[i * N * N + k] = a.edge_mask[b * N * N + k];
   if (threadIdx.x == 0) a.s_seeds[i] = retry_seed(a.seeds[b], a.attempt);
+}
+
+// The resizing gather: warp 0 draws the molecule's size s' with this attempt's seed, then the CTA writes the template of
+// that size -- rows [0, n_frag) copied from the caller's input, rows [n_frag, n_frag + s') linker rows (node_mask 1,
+// linker_mask 1, fragment_mask 0, x = linker_x[b], h 0, context 0), every later row zero, and on FC graphs the edge-mask
+// block of batching._add_masks over the n_frag + s' live rows (-1 off the diagonal, -2 on it). The host guarantees
+// n_frag + s' <= N.
+template <bool RESIZE>
+__global__ void __launch_bounds__(256) k_gather_rows(RowGatherArgs a, RowResizeArgs r) {
+  static_assert(RESIZE, "only the resizing gather takes RowResizeArgs");
+  __shared__ int s_live;
+  const int i = blockIdx.x;
+  const size_t b = a.rows[i], N = a.N;
+  const unsigned long long seed = retry_seed(a.seeds[b], a.attempt);
+  if (threadIdx.x < 32) {
+    const int k = size_draw_index(r.draw.logits + b * r.draw.logits_stride, r.draw.C, size_uniform(seed));
+    if (threadIdx.x == 0) {
+      const int size = r.draw.sizes[k];
+      s_live = r.n_frag[b] + size;
+      r.s_sizes[i] = size;
+      a.s_seeds[i] = seed;
+    }
+  }
+  __syncthreads();
+  const size_t nf = r.n_frag[b], live = s_live;
+  for (size_t k = threadIdx.x; k < N * a.xd; k += blockDim.x) {
+    const size_t n = k / a.xd, c = k - n * a.xd;
+    a.s_xh[i * N * a.xd + k] = n < nf ? a.xh[b * N * a.xd + k] : (n < live && c < 3 ? r.linker_x[b * 3 + c] : 0.f);
+  }
+  for (size_t k = threadIdx.x; k < N; k += blockDim.x) {
+    a.s_node_mask[i * N + k] = k < nf ? a.node_mask[b * N + k] : (int8_t)(k < live);
+    a.s_fragment_mask[i * N + k] = k < nf ? a.fragment_mask[b * N + k] : 0.f;
+    a.s_linker_mask[i * N + k] = k < nf ? a.linker_mask[b * N + k] : (k < live ? 1.f : 0.f);
+  }
+  if (a.context)
+    for (size_t k = threadIdx.x; k < N * a.C; k += blockDim.x)
+      a.s_context[i * N * a.C + k] = k / a.C < nf ? a.context[b * N * a.C + k] : 0.f;
+  if (a.edge_mask)
+    for (size_t k = threadIdx.x; k < N * N; k += blockDim.x) {
+      const size_t p = k / N, q = k - p * N;
+      a.s_edge_mask[i * N * N + k] = p < live && q < live ? (p == q ? (int8_t)-2 : (int8_t)-1) : (int8_t)0;
+    }
 }
 
 struct RowScatterArgs {
@@ -66,8 +183,9 @@ struct RowScatterArgs {
 // grid (Bs, keep_frames): CTA (i, f) writes frame f of sub-batch row i over row rows[i] of the caller's chain; the f = 0
 // CTAs also write the molecule's flags, the seed that produced the row and the attempt. CHECKED: only rows with take[i]
 // set, and their check verdicts with them.
-template <bool CHECKED>
-__global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a) {
+// SIZED (resizing rounds, with RowSizeArgs): the f = 0 CTAs also write the row's size.
+template <bool CHECKED, bool SIZED>
+__device__ __forceinline__ void scatter_rows(const RowScatterArgs& a, const RowSizeArgs& z) {
   const int i = blockIdx.x, f = blockIdx.y;
   if (CHECKED && !a.take[i]) return;
   const size_t b = a.rows[i], row = (size_t)a.N * a.xd;
@@ -79,7 +197,18 @@ __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a) {
     a.seeds_used[b] = a.s_seeds[i];
     a.attempts[b] = a.attempt;
     if (CHECKED) a.passed[b] = a.s_passed[i];
+    if (SIZED) z.sizes[b] = z.s_sizes[i];
   }
+}
+
+template <bool CHECKED>
+__global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a) {
+  scatter_rows<CHECKED, false>(a, RowSizeArgs{});
+}
+
+template <bool CHECKED>
+__global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a, RowSizeArgs z) {
+  scatter_rows<CHECKED, true>(a, z);
 }
 
 // ---- molecule checks: is the final molecule in one piece, and is every atom within its valence? -----------------------

@@ -10,13 +10,16 @@ Two ways in:
 Both take `devices=[...]` (or 'all') to split every sampling batch over several local GPUs from one process.
 Training, datasets, metrics and visualisation are out of scope (SURVEY.md section 2).
 """
+import operator
+
 import torch
 import torch.nn as nn
 
 from . import utils
 from .batching import create_templates_for_linker_generation
-from .edm import EDM, InpaintingEDM, draw_seeds
+from .edm import EDM, InpaintingEDM, LinkerSizes, draw_seeds, seeds_tensor
 from .egnn import Dynamics, DynamicsWithPockets
+from .linker_size import SizeClassifier, draw_sizes
 
 
 def _is_geom(hp: dict):
@@ -76,7 +79,13 @@ def sampler_inputs(model, data, sample_fn=None, keep_linker=False):
         linker_sizes = data['linker_mask'].sum(1).view(-1).int()
     else:
         linker_sizes = sample_fn(data)
-    template = data if model.inpainting else create_templates_for_linker_generation(data, linker_sizes)
+    return _template_inputs(model, data, linker_sizes, keep_linker)[0]
+
+
+def _template_inputs(model, data, linker_sizes, keep_linker=False, n_nodes=None):
+    """(sampler_inputs of the template of `linker_sizes` padded to `n_nodes` rows, the centre of mass (B, 1, 3) that was
+    subtracted from its coordinates)."""
+    template = data if model.inpainting else create_templates_for_linker_generation(data, linker_sizes, n_nodes)
     x, h = template['positions'], template['one_hot']
     if keep_linker and not model.inpainting:
         x, h = _keep_linker(data, template)
@@ -100,9 +109,79 @@ def sampler_inputs(model, data, sample_fn=None, keep_linker=False):
         com_mask = anchors
     else:
         raise NotImplementedError(model.center_of_mass)
-    x = utils.remove_partial_mean_with_mask(x, node_mask, com_mask)
+    mean = utils.partial_mean(x, com_mask)                  # utils.remove_partial_mean_with_mask, with its mean kept
+    x = x - mean * node_mask
     return dict(x=x, h=h, node_mask=node_mask, edge_mask=edge_mask, fragment_mask=fragment_mask,
-                linker_mask=linker_mask, context=context)
+                linker_mask=linker_mask, context=context), mean
+
+
+def size_distribution(model, data, linker_sizes):
+    """(logits (B, C) fp32 on the batch's device, size table) of `linker_sizes` for the batch `data`: a SizeClassifier's
+    size_logits -- with_pocket and adjust_shape on pocket models, as generate_with_protein.py:182 calls it -- over its
+    linker_id2size; all-zero logits over lo..hi for a pair (lo, hi), as generate.py:76-84 draws with torch.randint; or
+    the one-entry table [n] for an int n."""
+    B = data['positions'].shape[0]
+    dev = data['positions'].device
+    if isinstance(linker_sizes, SizeClassifier):
+        pocket = '.' in (model.train_data_prefix or '')
+        logits = linker_sizes.size_logits(data, with_pocket=pocket, adjust_shape=pocket)
+        return logits.to(torch.float32), list(linker_sizes.linker_id2size)
+    try:
+        if isinstance(linker_sizes, bool):
+            raise TypeError
+        if isinstance(linker_sizes, (tuple, list)):
+            if len(linker_sizes) != 2 or any(isinstance(v, bool) for v in linker_sizes):
+                raise TypeError
+            lo, hi = (operator.index(v) for v in linker_sizes)
+        else:
+            lo = hi = operator.index(linker_sizes)
+    except TypeError:
+        raise ValueError("linker_sizes is a SizeClassifier, a pair (lo, hi) of ints or an int "
+                         f"(got {linker_sizes!r})") from None
+    if not 0 <= lo <= hi:
+        raise ValueError(f"linker_sizes needs 0 <= lo <= hi (got {lo}, {hi})")
+    return torch.zeros((B, hi - lo + 1), dtype=torch.float32, device=dev), list(range(lo, hi + 1))
+
+
+def _check_linker_sizes(model, sample_fn, start_step):
+    if sample_fn is not None:
+        raise ValueError("linker_sizes and sample_fn both choose the linker sizes: pass one of them")
+    if start_step is not None:
+        raise ValueError("linker_sizes does not take start_step: partial diffusion varies the batch's own linker")
+    if model.inpainting:
+        raise ValueError("linker_sizes does not take an inpainting model: it samples every atom, with no linker size")
+
+
+def _sized_inputs(model, data, linker_sizes, seeds):
+    """(sampler_inputs of the template at the sizes drawn from `seeds` (attempt 0) padded to its capacity N_cap =
+    max n_frag + max(sizes), the (B,) CPU int64 seeds, the edm.LinkerSizes of the call)."""
+    x = data['positions']
+    if x.device.type != 'cuda':
+        raise ValueError(f"linker_sizes needs CUDA inputs (got {x.device})")
+    edm = model.edm
+    B = x.shape[0]
+    if seeds is None:
+        if edm.noise_mode != 'per_molecule':
+            raise ValueError("linker_sizes needs per-molecule streams: pass seeds= or set noise_mode='per_molecule' (the "
+                             f"batch stream, noise_mode={edm.noise_mode!r}, cannot give one molecule new draws)")
+        with torch.cuda.device(x.device):
+            seeds = draw_seeds(B, x.device)
+    cpu_seeds = seeds_tensor(seeds, B)
+    logits, table = size_distribution(model, data, linker_sizes)
+    sizes = draw_sizes(logits, table, cpu_seeds)
+    fm = data['fragment_mask']
+    n_frag = fm.reshape(B, fm.shape[1]).sum(1).long()
+    n_cap = int(n_frag.max()) + max(table)
+    kw, mean = _template_inputs(model, data, sizes, n_nodes=n_cap)
+    linker_x = (torch.zeros_like(mean) - mean).reshape(B, 3)   # x - mean * node_mask of a linker row, whose x is 0
+    return kw, cpu_seeds, LinkerSizes(logits, table, n_frag, linker_x)
+
+
+def _final_node_mask(kw, linker_sizes, sizes):
+    """The template's atom mask at the returned sizes: rows [0, n_frag + size) of every molecule."""
+    n = kw['node_mask'].shape[1]
+    live = linker_sizes.n_frag.to(kw['node_mask'].device) + sizes.to(kw['node_mask'].device)
+    return (torch.arange(n, device=live.device)[None, :] < live[:, None]).to(kw['node_mask'].dtype)[:, :, None]
 
 
 def _check_start(sample_fn, start_step):
@@ -111,7 +190,7 @@ def _check_start(sample_fn, start_step):
 
 
 def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                 start_step=None, require_valid=None, require_clash_free=None):
+                 start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
@@ -122,10 +201,24 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     `model.edm.require_clash_free`).
     `start_step` = t0 (partial diffusion, EDM.sample_chain): the template of sample_fn=None with the batch's own linker
     positions and atom types on its linker rows, sampled from step t0; ValueError with a sample_fn, or when the batch's
-    linker rows do not directly follow its fragment rows."""
+    linker rows do not directly follow its fragment rows.
+    `linker_sizes` -- a SizeClassifier, a pair (lo, hi) or an int (size_distribution) -- draws molecule b's linker size from
+    its own seed (dl_size_draw; `seeds`, or draw_seeds with noise_mode='per_molecule'), builds the template at those sizes
+    padded to its capacity N_cap = max n_frag + max(sizes), and makes every recovery round redraw the size of each row it
+    resamples from that round's seed (EDM.sample_chain). A row's size and chain are then functions of `last_seeds[b]`:
+    molecule b alone, its input padded to the same number of rows (the size model mean-pools over the padding), with
+    seeds=[last_seeds[b]], gives the same size and row. `model.edm.last_sizes` holds the sizes, and the returned node_mask
+    is the template's at those sizes. ValueError with sample_fn, start_step, an inpainting model, host inputs, the batch
+    stream without seeds, and where EDM.sample_chain refuses it."""
     _check_start(sample_fn, start_step)
-    kw = sampler_inputs(model, data, sample_fn, keep_linker=start_step is not None)
+    if linker_sizes is not None:
+        _check_linker_sizes(model, sample_fn, start_step)
+        kw, seeds, sized = _sized_inputs(model, data, linker_sizes, seeds)
+    else:
+        kw, sized = sampler_inputs(model, data, sample_fn, keep_linker=start_step is not None), None
     extra = {} if seeds is None else {'seeds': seeds}
+    if sized is not None:
+        extra['linker_sizes'] = sized
     if nan_retries is not None:
         extra['nan_retries'] = nan_retries
     if require_connected is not None:
@@ -137,19 +230,39 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     if start_step is not None:
         extra['start_step'] = start_step
     chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **extra)
+    if sized is not None:
+        return chain, _final_node_mask(kw, sized, model.edm.last_sizes)
     return chain, kw['node_mask']
 
 
 def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                max_molecules=256, start_step=None, require_valid=None, require_clash_free=None):
+                max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None):
     """The body of sample_chain for many batches `datas` at once, sampled in shared launches by EDM.sample_many: returns
     [(chain_k, node_mask_k)] in the order of `datas`, each equal to what sample_chain(model, datas[k], ...) returns (with
     seeds[k]) in the sense of EDM.sample_many. `model` as for sample_chain, so accelerated reference modules take it too.
     `sample_fn`, and with noise_mode='per_molecule' and no `seeds` draw_seeds, are called once per batch, in the order the
     sequential sample_chain calls call them: linker sizes, seeds and the generator's final state are theirs. `start_step`,
-    one for every batch, as in sample_chain."""
+    one for every batch, as in sample_chain. `linker_sizes`, one for every batch, as in sample_chain: each batch's sizes
+    are drawn from its own seeds and its template padded to its own N_cap, so packing changes neither;
+    `edm.last_sizes_many` holds them."""
     _check_start(sample_fn, start_step)
     edm = model.edm
+    if linker_sizes is not None:
+        _check_linker_sizes(model, sample_fn, start_step)
+        if seeds is not None and len(seeds) != len(datas):
+            raise ValueError(f"seeds holds {len(seeds)} lists for {len(datas)} batches")
+        sized = [_sized_inputs(model, data, linker_sizes, None if seeds is None else seeds[k])
+                 for k, data in enumerate(datas)]
+        extra = {} if nan_retries is None else {'nan_retries': nan_retries}
+        for name, v in (('require_connected', require_connected), ('require_valid', require_valid),
+                        ('require_clash_free', require_clash_free)):
+            if v is not None:
+                extra[name] = v
+        requests = [kw for kw, _, _ in sized]
+        chains = edm.sample_many(requests, keep_frames=keep_frames, seeds=[s for _, s, _ in sized],
+                                 max_molecules=max_molecules, linker_sizes=[ls for _, _, ls in sized], **extra)
+        return [(chain, _final_node_mask(kw, ls, sizes))
+                for chain, (kw, _, ls), sizes in zip(chains, sized, edm.last_sizes_many)]
     derive = seeds is None and edm.noise_mode == 'per_molecule'
     requests, drawn = [], []
     for data in datas:
@@ -210,16 +323,16 @@ class DDPM(nn.Module):
         self.edm.devices = devices          # EDM.devices: split each sampling batch over these CUDA devices
 
     def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                     start_step=None, require_valid=None, require_clash_free=None):
+                     start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                             require_connected=require_connected, start_step=start_step, require_valid=require_valid,
-                            require_clash_free=require_clash_free)
+                            require_clash_free=require_clash_free, linker_sizes=linker_sizes)
 
     def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                    max_molecules=256, start_step=None, require_valid=None, require_clash_free=None):
+                    max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None):
         return sample_many(self, datas, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                            require_connected=require_connected, max_molecules=max_molecules, start_step=start_step,
-                           require_valid=require_valid, require_clash_free=require_clash_free)
+                           require_valid=require_valid, require_clash_free=require_clash_free, linker_sizes=linker_sizes)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

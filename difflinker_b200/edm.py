@@ -10,6 +10,7 @@ import ctypes as C
 import functools
 import operator
 import threading
+from typing import NamedTuple
 
 import torch
 import torch.nn.functional as F
@@ -26,14 +27,30 @@ def _generator_of(dev):
     return torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
 
 
+class LinkerSizes(NamedTuple):
+    """What EDM.sample_chain redraws linker sizes from in its recovery rounds (dl_sample_chain_seeded_retry_sized), for a
+    template built at the sizes dl_size_draw gives the call's seeds at attempt 0 and padded to at least
+    max(n_frag) + max(sizes) rows. ddpm.sample_chain(linker_sizes=...) builds it.
+      logits    (B, C) fp32 CUDA: every molecule's size logits
+      sizes     the C sizes of the table, ints >= 0
+      n_frag    (B) ints: every molecule's fragment rows (pocket rows included), which come first in the template
+      linker_x  (B, 3): the centred (not normalised) coordinates of every molecule's template linker rows"""
+    logits: torch.Tensor
+    sizes: list
+    n_frag: torch.Tensor
+    linker_x: torch.Tensor
+
+
 def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None, clash=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
     samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, require, tables,
-    passed) resamples the molecules that diverged (dl_sample_chain_seeded_retry, which blocks until its rounds are done)
-    and, with `require` != 0, those that miss a required check, whose verdict bits go to `passed`
+    passed, redraw) resamples the molecules that diverged (dl_sample_chain_seeded_retry, which blocks until its rounds are
+    done) and, with `require` != 0, those that miss a required check, whose verdict bits go to `passed`
     (dl_sample_chain_seeded_retry_checked; `tables` as molecule_builder.check_tables returns them, on the slice's device).
+    `redraw` = (logits, size table, n_frag, normalised linker_x, sizes_used), device tensors, redraws the resampled rows'
+    linker sizes (dl_sample_chain_seeded_retry_sized); None keeps them.
     `start` = (t0, alpha_t0, sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of
     the call (dl_set_start_step). `clash`, a (T,T) table on the slice's device, is the engine's clash table for the duration
     of the call (dl_set_clash_table), which a `require` with CHECK_CLASH reads. Returns (status, what the batch stream
@@ -56,8 +73,16 @@ def _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry):
     if stream is None:
         return _native.check(lib.dl_sample_chain_host(eng, *head, noise.data_ptr(), *tail), "dl_sample_chain_host"), 0
     if retry is not None:
-        max_retries, used, attempts, require, tables, passed = retry
+        max_retries, used, attempts, require, tables, passed, redraw = retry
         args = (eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr())
+        if redraw is not None:
+            logits, table, n_frag, linker_x, sizes = redraw
+            rz = _native.DLSizeRedraw(table.numel(), logits.stride(0), logits.data_ptr(), table.data_ptr(), n_frag.data_ptr(),
+                                      linker_x.data_ptr())
+            ck = _native.DLMoleculeChecks.of(require, tables) if require else None
+            return _native.check(lib.dl_sample_chain_seeded_retry_sized(
+                *args, ck, passed.data_ptr() if require else None, rz, sizes.data_ptr(), stream),
+                "dl_sample_chain_seeded_retry_sized"), 0
         if not require:
             return _native.check(lib.dl_sample_chain_seeded_retry(*args, stream), "dl_sample_chain_seeded_retry"), 0
         return _native.check(lib.dl_sample_chain_seeded_retry_checked(
@@ -203,13 +228,14 @@ class EDM(torch.nn.Module):
         # nothing.
         self.require_clash_free = False
         self.last_clash_free = None            # calls with require_clash_free: the (B,) CPU bool clash verdict of every row
+        self.last_sizes = None                 # calls with linker_sizes: the (B,) CPU int32 linker size of every returned row
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
         # sample_many: per request, what last_seeds / last_attempts / last_connected / last_valid hold after its own
         # sample_chain call; per launch, (device, the requests it held, loop ms)
         self.last_seeds_many = self.last_attempts_many = self.last_connected_many = self.last_loop_ms_many = None
-        self.last_valid_many = self.last_clash_free_many = None
+        self.last_valid_many = self.last_clash_free_many = self.last_sizes_many = None
 
     @property
     def devices(self):
@@ -497,6 +523,45 @@ class EDM(torch.nn.Module):
                                  "cut-off graph such as '4A' or 'FC-10A-4A')")
         return self._require_check('require_clash_free', value, seeds, noise, batch_slice, x)
 
+    def _linker_sizes(self, linker_sizes, seeds, noise, batch_slice, start_step, x, linker_mask):
+        """The device tensors (logits, size table, n_frag, normalised linker_x, attempt-0 sizes) of a call's `linker_sizes`
+        (a LinkerSizes for the (B, N) template x), or None without one. ValueError for what cannot redraw one molecule's
+        size: InpaintingEDM, start_step, no `seeds`, noise=, a replaced draw function, batch_slice, host inputs, and a
+        template of fewer rows than max(n_frag) + max(sizes)."""
+        if linker_sizes is None:
+            return None
+        if self._SAMPLER == _native.SAMPLER_INPAINT:
+            raise ValueError("linker_sizes does not take InpaintingEDM: it samples every atom and has no linker size")
+        if start_step is not None:
+            raise ValueError("linker_sizes does not take start_step: partial diffusion varies the batch's own linker, "
+                             "whose size is given")
+        self._refuse_without_new_draws('linker_sizes', seeds, noise, batch_slice)
+        if seeds is None:
+            raise ValueError("linker_sizes needs seeds=: the template's sizes are dl_size_draw's attempt-0 draws from them")
+        if x.device.type != 'cuda':
+            raise ValueError(f"linker_sizes needs CUDA inputs (got {x.device})")
+        if not isinstance(linker_sizes, LinkerSizes):
+            raise ValueError(f"linker_sizes is an edm.LinkerSizes at this level (got {type(linker_sizes).__name__}); "
+                             "ddpm.sample_chain resolves a size model, a range or an int")
+        B, N = x.shape[:2]
+        dev = x.device
+        table = torch.tensor([operator.index(v) for v in linker_sizes.sizes], dtype=torch.int32)
+        logits = linker_sizes.logits.detach().to(device=dev, dtype=torch.float32).contiguous()
+        n_frag = torch.as_tensor(linker_sizes.n_frag).detach().reshape(-1).to(device='cpu', dtype=torch.int32)
+        if table.numel() < 1 or (table < 0).any():
+            raise ValueError("linker_sizes.sizes must hold at least one size, each >= 0")
+        if tuple(logits.shape) != (B, table.numel()) or n_frag.numel() != B or linker_sizes.linker_x.numel() != 3 * B:
+            raise ValueError(f"linker_sizes must hold (B, C) logits, B n_frag and (B, 3) linker_x for B = {B} molecules and "
+                             f"C = {table.numel()} sizes (got {tuple(logits.shape)}, {n_frag.numel()} and "
+                             f"{tuple(linker_sizes.linker_x.shape)})")
+        need = int(n_frag.max()) + int(table.max())
+        if N < need:
+            raise ValueError(f"linker_sizes: the template has {N} rows, fewer than its capacity max(n_frag) + max(sizes) = "
+                             f"{need}, which every redrawn size must fit")
+        linker_x = linker_sizes.linker_x.detach().to(device=dev, dtype=torch.float32).reshape(B, 3) / self.norm_values[0]
+        sizes = linker_mask.detach().reshape(B, N).to(dev).sum(1).to(torch.int32)
+        return logits, table.to(dev), n_frag.to(dev), linker_x.contiguous(), sizes
+
     def _check_tables(self, check):
         """The CPU tables the checks `check` read with this model's atom types (molecule_builder.check_tables)."""
         return check_tables(self.is_geom, check)
@@ -512,7 +577,7 @@ class EDM(torch.nn.Module):
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
-                     require_valid=None, require_clash_free=None):
+                     require_valid=None, require_clash_free=None, linker_sizes=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -559,6 +624,11 @@ class EDM(torch.nn.Module):
         molecule_builder.clash_table(is_geom) allows for the two atom types (this project's own predicate, stated at
         dl_molecule_checks in the header; fragment atoms are not checked). `last_clash_free` (B,) CPU bool tells which rows
         pass. Refusals as for require_valid, plus ValueError on FC graphs and for InpaintingEDM.
+        `linker_sizes` (a LinkerSizes; ddpm.sample_chain builds it) makes every round redraw the linker size of the rows it
+        resamples, from the round's seed (dl_sample_chain_seeded_retry_sized), and rebuild their template rows at that size
+        inside the padded template. The inputs must be the template of the sizes dl_size_draw gives `seeds` at attempt 0,
+        padded to max(n_frag) + max(sizes) rows or more. `last_sizes` (B,) CPU int32 holds every returned row's size. It
+        needs `seeds` and raises ValueError where nan_retries does, with start_step and for InpaintingEDM.
         The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
         and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
         device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
@@ -571,8 +641,9 @@ class EDM(torch.nn.Module):
         n_samples = x.size(0)
         dev = x.device
         self.last_attempts = None
-        self.last_connected = self.last_valid = self.last_clash_free = None
+        self.last_connected = self.last_valid = self.last_clash_free = self.last_sizes = None
         start = self._start(start_step, n_samples)
+        redraw = self._linker_sizes(linker_sizes, seeds, noise, batch_slice, start_step, x, linker_mask)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
         check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free)
         recover = retries > 0 or check != 0 # the recovery entry point: seeds used and attempts come back
@@ -603,7 +674,7 @@ class EDM(torch.nn.Module):
         calls, finish = self._enqueue_batch(lib, full, keep_frames, self.step_coefficients(keep_frames, n_samples), slices,
                                             engines, places, dev, noise=noise, dev_seeds=dev_seeds,
                                             rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check,
-                                            start=start)
+                                            start=start, redraw=redraw)
         by_device = {}
         for dev_i, c in calls:
             by_device.setdefault(dev_i, []).append(c)
@@ -632,6 +703,8 @@ class EDM(torch.nn.Module):
         self.last_slice_loop_ms = loop_ms if split else None
         if recover:
             self.last_seeds, self.last_attempts = out['used'].cpu(), out['attempts'].cpu()
+        if redraw is not None:
+            self.last_sizes = (out['sizes'] if recover else redraw[4]).cpu()
         if check & _native.CHECK_CONNECTED:
             self.last_connected = (out['passed'].cpu() & _native.CHECK_CONNECTED) != 0
         if check & _native.CHECK_VALENCE:
@@ -650,7 +723,7 @@ class EDM(torch.nn.Module):
 
     @torch.no_grad()
     def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                    max_molecules=256, start_step=None, require_valid=None, require_clash_free=None):
+                    max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None):
         """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
         edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
         (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
@@ -674,6 +747,9 @@ class EDM(torch.nn.Module):
         `last_clash_free_many` hold per
         request what last_seeds, last_attempts, last_connected and last_valid would hold after its own call; `last_loop_ms_many` holds (device,
         requests, loop ms) per launch. The single-call attributes are left as they were.
+        `linker_sizes`, one LinkerSizes per request, all of one size table, redraws sizes in those rounds as in sample_chain
+        (it needs `seeds`); `last_sizes_many` holds every request's sizes. Each request's sizes come from its own seeds, so
+        packing does not change them.
         Raises ValueError for an empty list, the batch stream (its draws depend on B and N), noise= or a replaced draw
         function, host inputs, requests on different devices or of different feature or context widths, and seeds that do
         not match the requests."""
@@ -728,6 +804,14 @@ class EDM(torch.nn.Module):
         retries = self._nan_retries(nan_retries, seeds, None, None, x0)
         check = self._checks(require_connected, require_valid, seeds, None, None, x0, require_clash_free)
         recover = retries > 0 or check != 0
+        redraws = None
+        if linker_sizes is not None:
+            if len(linker_sizes) != len(requests):
+                raise ValueError(f"linker_sizes holds {len(linker_sizes)} entries for {len(requests)} requests")
+            redraws = [self._linker_sizes(ls, seeds, None, None, start_step, r['x'], r['linker_mask'])
+                       for ls, r in zip(linker_sizes, requests)]
+            if any(not torch.equal(rd[1], redraws[0][1]) for rd in redraws):
+                raise ValueError("linker_sizes: every request must draw from the same size table")
         self.dynamics._check_graph_type()
         if seeds is None:
             with torch.cuda.device(dev):    # one draw per request, in request order, as the sample_chain calls draw them
@@ -760,9 +844,12 @@ class EDM(torch.nn.Module):
             dev_seeds = torch.cat([cpu_seeds[k] for k in ks]).to(dev)
             where = torch.device('cuda', dev_i)
             eng = engine_of[slot_of[i]]
+            redraw = None
+            if redraws is not None:
+                redraw = tuple(redraws[ks[0]][1] if j == 1 else torch.cat([redraws[k][j] for k in ks]) for j in range(5))
             [(_, call)], finish = self._enqueue_batch(lib, full, keep_frames, coefs[sizes[ks[0]]], [(dev_i, replica, 0, b)], [eng],
                                                       [where], dev, dev_seeds=dev_seeds, retries=retries, check=check,
-                                                      start=starts[sizes[ks[0]]])
+                                                      start=starts[sizes[ks[0]]], redraw=redraw)
             finishes.append(finish)
             by_device.setdefault(dev_i, []).append(
                 functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
@@ -778,6 +865,7 @@ class EDM(torch.nn.Module):
         results, flags = [None] * len(requests), [None] * len(requests)
         seeds_many, attempts_many = list(cpu_seeds), [None] * len(requests)
         connected_many, valid_many, clash_free_many = [None] * len(requests), [None] * len(requests), [None] * len(requests)
+        sizes_many = [None] * len(requests) if redraws is None else [rd[4].cpu() for rd in redraws]
         for (ks, _), finish in zip(launches, finishes):
             out = finish()
             rows = [sizes[k] for k in ks]
@@ -788,10 +876,14 @@ class EDM(torch.nn.Module):
                 parts['attempts'] = unpack_rows(out['attempts'].cpu(), rows, None)
             if check:
                 parts['passed'] = unpack_rows(out['passed'].cpu(), rows, None)
+            if out['sizes'] is not None:
+                parts['sizes'] = unpack_rows(out['sizes'].cpu(), rows, None)
             for j, k in enumerate(ks):
                 results[k], flags[k] = parts['chain'][j], parts['flags'][j]
                 if recover:
                     seeds_many[k], attempts_many[k] = parts['used'][j], parts['attempts'][j]
+                if 'sizes' in parts:
+                    sizes_many[k] = parts['sizes'][j]
                 if check & _native.CHECK_CONNECTED:
                     connected_many[k] = (parts['passed'][j] & _native.CHECK_CONNECTED) != 0
                 if check & _native.CHECK_VALENCE:
@@ -799,7 +891,7 @@ class EDM(torch.nn.Module):
                 if check & _native.CHECK_CLASH:
                     clash_free_many[k] = (parts['passed'][j] & _native.CHECK_CLASH) != 0
         self.last_seeds_many, self.last_attempts_many, self.last_connected_many = seeds_many, attempts_many, connected_many
-        self.last_valid_many, self.last_clash_free_many = valid_many, clash_free_many
+        self.last_valid_many, self.last_clash_free_many, self.last_sizes_many = valid_many, clash_free_many, sizes_many
         self.last_loop_ms_many = [(slots[slot_of[i]][0], sorted(ks), loop_ms[i]) for i, (ks, _) in enumerate(launches)]
         for k, f in enumerate(flags):
             if f.any():
@@ -821,16 +913,16 @@ class EDM(torch.nn.Module):
         return coefs, starts, keys
 
     def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
-                       retries=0, check=0, start=None):
+                       retries=0, check=0, start=None, redraw=None):
         """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
         inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
         replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
         covers the batch where it is. The draws are the per-molecule `dev_seeds`, the batch stream `rng` = (seed, offset,
         b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _checks; `start` as
-        returned by _start.
+        returned by _start; `redraw` as returned by _linker_sizes (its rounds then redraw sizes, into `sizes`).
         Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
         (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
-        back and returns dict(chain, flags, used, attempts, passed, bad, consumed) on `dev`; `passed` holds
+        back and returns dict(chain, flags, used, attempts, passed, sizes, bad, consumed) on `dev`; `passed` holds
         every row's _native.CHECK_* verdict bits. `bad` reads the flags: one
         synchronisation, after every loop and copy."""
         n_samples, n_nodes = full['x'].shape[:2]
@@ -844,6 +936,9 @@ class EDM(torch.nn.Module):
                           if recover else (None, None))
         # molecule checks: every row's verdict bits, and the tables they read on each slice's device
         passed = torch.empty(n_samples, dtype=torch.int32, device=dev) if check else None
+        # size redraws: every row's size, the attempt-0 sizes on entry
+        redraw = redraw if recover else None
+        sizes = None if redraw is None else redraw[4].clone()
         tables = self._check_tables(check) if check else None
         clash = clash_table(self.is_geom) if check & _native.CHECK_CLASH else None
         whole = places == [dev]             # one slice, the whole batch where it is: it samples the caller's tensors
@@ -864,16 +959,22 @@ class EDM(torch.nn.Module):
                             *((torch.empty(hi - lo, dtype=torch.int64, device=where),
                                torch.empty(hi - lo, dtype=torch.int32, device=where)) if recover else (None, None)),
                             torch.empty(hi - lo, dtype=torch.int32, device=where) if check else None)
+            redraw_i = None
+            if redraw is not None:
+                logits, table, n_frag, linker_x, _ = redraw
+                redraw_i = ((logits, table, n_frag, linker_x, sizes) if whole else
+                            tuple(v.to(where).contiguous() for v in (logits[lo:hi], table, n_frag[lo:hi], linker_x[lo:hi],
+                                                                     sizes[lo:hi])))
             part = part + (None if tables is None else [t.to(where) for t in tables],
-                           None if clash is None else clash.to(where))
+                           None if clash is None else clash.to(where), redraw_i)
             parts.append(part)              # alive until the flags have been read below
-            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, tables_i, clash_i = part
+            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, tables_i, clash_i, redraw_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
             rng_i = None if rng is None else (rng[0], rng[1], rng[2] + lo, rng[3])
             calls.append((dev_i, functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
-                (retries, used_i, attempts_i, check, tables_i, passed_i) if recover else None, start, clash_i)))
+                (retries, used_i, attempts_i, check, tables_i, passed_i, redraw_i) if recover else None, start, clash_i)))
 
         def finish():
             if not whole:
@@ -884,10 +985,12 @@ class EDM(torch.nn.Module):
                     place_rows(attempts, [p[6] for p in parts], slices)
                 if check:
                     place_rows(passed, [p[7] for p in parts], slices)
+                if redraw is not None:
+                    place_rows(sizes, [p[10][4] for p in parts], slices)
             # the host sampler reports NaNs in its status; on the device, one sync per chain instead of one per step
             # (egnn.py:441), after every slice's loop and copy
             bad = _native.DL_NAN_DETECTED in [st for st, _ in results] or bool(flags.any().item())
-            return dict(chain=chain, flags=flags, used=used, attempts=attempts, passed=passed, bad=bad,
+            return dict(chain=chain, flags=flags, used=used, attempts=attempts, passed=passed, sizes=sizes, bad=bad,
                         consumed=[c for _, c in results])
         return calls, finish
 
@@ -945,7 +1048,7 @@ class InpaintingEDM(EDM):
 
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
-                     require_valid=None, require_clash_free=None):
+                     require_valid=None, require_clash_free=None, linker_sizes=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -954,12 +1057,12 @@ class InpaintingEDM(EDM):
         seeds, molecule b's 2T+3 raw draws are those of the molecule sampled alone after torch.cuda.manual_seed(seeds[b]),
         masked and projected per molecule as always. `nan_retries`, `require_connected` and `require_valid` as in EDM.sample_chain;
         the checks cover every atom of the molecule. `start_step` raises ValueError unless None, and `require_clash_free`
-        unless None or False: this loop re-noises the pocket."""
+        unless None or False: this loop re-noises the pocket; `linker_sizes` unless None: this model has no linker size."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
                                     require_connected=require_connected, start_step=start_step, require_valid=require_valid,
-                                    require_clash_free=require_clash_free)
+                                    require_clash_free=require_clash_free, linker_sizes=linker_sizes)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

@@ -4,6 +4,7 @@ runs as one native pass (`dl_sizegnn_forward`); parameter names and construction
 reference checkpoint's `state_dict` loads with `strict=True`. No CPU fallback.
 """
 import ctypes as C
+import operator
 
 import torch
 import torch.nn as nn
@@ -166,6 +167,11 @@ class SizeClassifier(nn.Module):
         self.gnn = SizeGNN(in_node_nf=in_node_nf, hidden_nf=hidden_nf, out_node_nf=out_node_nf, n_layers=n_layers,
                            normalization=normalization)
 
+    def size_logits(self, data, with_pocket=False, adjust_shape=False):
+        """(B, out_node_nf) fp32 logits over linker_id2size: forward(data, return_loss=False, ...)'s output. They mean-pool
+        over the padded rows of `data`, so they depend on its padding."""
+        return self.forward(data, return_loss=False, with_pocket=with_pocket, adjust_shape=adjust_shape)[0]
+
     def forward(self, data, return_loss=True, with_pocket=False, adjust_shape=False):
         h, x = data['one_hot'], data['positions']
         fragment_mask = data['fragment_only_mask'] if with_pocket else data['fragment_mask']
@@ -197,9 +203,41 @@ class SizeClassifier(nn.Module):
         return _load_lightning_checkpoint(cls, checkpoint_path, map_location, strict, overrides)
 
     @torch.no_grad()
-    def sample_sizes(self, data, generator=None):
-        """The `sample_fn` of generate.py:90-99: softmax -> Categorical -> linker sizes (int8, on the batch's device)."""
+    def sample_sizes(self, data, generator=None, seeds=None):
+        """The `sample_fn` of generate.py:90-99: softmax -> Categorical -> linker sizes (int8, on the batch's device).
+        With `seeds` (one per molecule), molecule b's size is instead draw_sizes' draw from seeds[b]: a function of its seed
+        and its logits alone; `generator` is then not read."""
         out, _ = self.forward(data, return_loss=False)
+        if seeds is not None:
+            return draw_sizes(out, self.linker_id2size, seeds).to(torch.int8)
         idx = torch.multinomial(torch.softmax(out, dim=1), 1, generator=generator).view(-1)
         table = torch.tensor(self.linker_id2size, device=idx.device)
         return table[idx].to(torch.int8)
+
+
+def size_uniform(seed):
+    """dl_size_uniform: the 53-bit uniform in [0, 1) a linker size is drawn with from `seed` (an int, reduced modulo 2^64)."""
+    return float(_native.load_library().dl_size_uniform(operator.index(seed) % (1 << 64)))
+
+
+@torch.no_grad()
+def draw_sizes(logits, sizes, seeds, attempt=0):
+    """dl_size_draw: molecule b's linker size drawn from its (C,) row of the (B, C) CUDA `logits` over the size table
+    `sizes` with the seed dl_retry_seed(seeds[b], attempt) -- the fp64 inverse-CDF rule stated in the header. Returns (B,)
+    int32 on the logits' device."""
+    from .edm import seeds_tensor
+    if not torch.is_tensor(logits) or logits.dim() != 2 or logits.device.type != 'cuda':
+        raise ValueError("draw_sizes takes (B, C) CUDA logits")
+    B, C = logits.shape
+    dev = logits.device
+    table = torch.tensor([operator.index(v) for v in sizes], dtype=torch.int32, device=dev)
+    if table.numel() != C:
+        raise ValueError(f"the size table holds {table.numel()} sizes for {C} logits")
+    lg = logits.detach().to(torch.float32).contiguous()
+    sd = seeds_tensor(seeds, B).to(dev)
+    out = torch.empty(B, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _native.check(_native.load_library().dl_size_draw(B, C, lg.data_ptr(), C, table.data_ptr(), sd.data_ptr(), attempt,
+                                                         out.data_ptr(), torch.cuda.current_stream().cuda_stream),
+                      "dl_size_draw")
+    return out

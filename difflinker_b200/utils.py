@@ -58,11 +58,15 @@ def remove_mean_with_mask(x, node_mask):
     return x - (torch.sum(x, dim=1, keepdim=True) / n) * node_mask
 
 
+def partial_mean(x, center_of_mass_mask):
+    """The (B, 1, 3) centre of mass of the `center_of_mass_mask` atoms that remove_partial_mean_with_mask subtracts."""
+    n = center_of_mass_mask.sum(1, keepdims=True)
+    return torch.sum(x * center_of_mass_mask, dim=1, keepdim=True) / n
+
+
 def remove_partial_mean_with_mask(x, node_mask, center_of_mass_mask):
     """src/utils.py:66-74: subtract the centre of mass of the `center_of_mass_mask` atoms from all atoms."""
-    n = center_of_mass_mask.sum(1, keepdims=True)
-    mean = torch.sum(x * center_of_mass_mask, dim=1, keepdim=True) / n
-    return x - mean * node_mask
+    return x - partial_mean(x, center_of_mass_mask) * node_mask
 
 
 def assert_correctly_masked(variable, node_mask):

@@ -28,6 +28,8 @@
  *   either on pocket graphs, also resampling the        dl_set_clash_table, DL_CHECK_CLASH, dl_clash_check
  *     molecules whose linker clashes with the pocket (no reference API; see dl_molecule_checks)
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
+ *   softmax + Categorical.sample of a size model (generate.py:88-99), from dl_size_draw, dl_size_uniform
+ *     the molecule's seed, and redrawn in the recovery rounds             dl_sample_chain_seeded_retry_sized
  *   build_xae_molecule           src/molecule_builder.py:44-102       dl_bond_orders
  *   frame restore + .xyz text    generate.py:163-171, src/visualizer.py:14-31   dl_restore_frame, dl_format_xyz
  *   utils.FoundNaNException      src/utils.py:274-289    DL_NAN_DETECTED + per-molecule nan_flags
@@ -316,6 +318,74 @@ dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, in
                                                const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries,
                                                uint64_t* seeds_used, int32_t* attempts, const dl_molecule_checks* checks,
                                                int32_t* passed, void* stream);
+/*
+ * Linker sizes drawn from a molecule's seed (no reference API; generate.py:88-99 draws them from one batch-level
+ * Categorical.sample). Molecule b's size distribution is a table sizes[0..C) of ints >= 0 with finite fp32 logits
+ * l_b[0..C): a SizeClassifier's output with sizes = its linker_id2size, all-zero logits over lo..hi for a uniform range, or
+ * the one-entry table [n]. The draw with seed s:
+ *   1. u = dl_size_uniform(s), a uniform in [0, 1) with 53 bits (below; a function of s alone, of no Philox draw);
+ *   2. in fp64 and in index order: m = max_i l_i, e_i = exp(l_i - m), S = sum_i e_i, c_i = e_0 + ... + e_i;
+ *   3. the drawn index is the first i with u * S < c_i, or, if rounding leaves none, the last i with e_i > 0; the size is
+ *      sizes[i].
+ * Attempt 0 uses the molecule's seed; recovery round a uses dl_retry_seed(seed, a), the seed of that round's noise, so the
+ * seed that produced a row (seeds_used) determines both its size and its chain. A SizeClassifier mean-pools over the padded
+ * rows of its input, so its logits -- and the size -- depend on the padding of the input batch: a molecule replays alone
+ * with its seed only when its input is padded to the same number of rows.
+ */
+/*
+ * dl_size_uniform(seed): the 53-bit uniform of the draw above. With the domain tag TAG = 0x6C696E6B65722D6E ("linker-n"):
+ *     z = seed ^ TAG;  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;  z = (z ^ (z >> 27)) * 0x94D049BB133111EB;
+ *     z = z ^ (z >> 31);  return (double)(z >> 11) * 2^-53;                      (all modulo 2^64)
+ * A pure host function.
+ */
+double dl_size_uniform(uint64_t seed);
+/*
+ * The draw above for B molecules, without an engine. DEVICE buffers, enqueued on `stream`.
+ *   logits     (B, logits_row_stride) fp32: molecule b's C logits from column 0; logits_row_stride >= C >= 1
+ *   sizes      (C) int32: the size table
+ *   seeds      (B) uint64: molecule b draws with dl_retry_seed(seeds[b], attempt) (attempt 0: seeds[b] itself)
+ *   out_sizes  (B) int32 out
+ */
+dl_status dl_size_draw(int32_t B, int32_t C, const float* logits, int32_t logits_row_stride, const int32_t* sizes,
+                       const uint64_t* seeds, int32_t attempt, int32_t* out_sizes, void* stream);
+/*
+ * What dl_sample_chain_seeded_retry_sized redraws sizes from. DEVICE buffers, read while the call runs.
+ */
+typedef struct dl_size_redraw {
+  int32_t C;                   /* entries of the size table, >= 1 */
+  int32_t logits_row_stride;   /* >= C */
+  const float* logits;         /* (B, logits_row_stride) fp32: molecule b's C logits */
+  const int32_t* sizes;        /* (C) int32 >= 0: the size table */
+  const int32_t* n_frag;       /* (B) int32: molecule b's fragment rows, pocket rows included, which come first */
+  const float* linker_x;       /* (B, 3) fp32: the (normalised) coordinates of molecule b's template linker rows, the
+                                  negated centre of mass of its template; given per molecule because a size-0 row has
+                                  no linker row to copy them from */
+} dl_size_redraw;
+/*
+ * dl_sample_chain_seeded_retry_checked (checks may be NULL: NaN recovery alone, passed is then not read) whose rounds
+ * redraw each resampled row's linker size. The inputs are the template of the attempt-0 sizes (dl_size_draw with attempt
+ * 0) padded to the capacity N >= max_b n_frag[b] + max(sizes), which every redrawn size fits. In round a, each failing row
+ * b draws size s' with dl_retry_seed(seeds[b], a) and is gathered as the template of that size:
+ *   rows [0, n_frag[b])                copied from the inputs;
+ *   rows [n_frag[b], n_frag[b] + s')   linker rows: node_mask 1, linker_mask 1, fragment_mask 0, x = linker_x[b], h 0,
+ *                                      context 0;
+ *   later rows                          zero; on DL_GRAPH_FC the edge-mask block is batching's int8 rule over the live rows
+ *                                      (-1 off the diagonal, -2 on it, 0 elsewhere).
+ * The take rule, the NaN flags and the verdicts are those of dl_sample_chain_seeded_retry_checked.
+ *   sizes_used  (B) int32 DEVICE in/out: the attempt-0 sizes on entry; on return, the size of every returned row (a row
+ *               that is not taken keeps its size)
+ * DL_ERR_INVALID with DL_SAMPLER_INPAINT (which has no linker size) and when N < n_frag[b] + max(sizes) for some b. Row b's
+ * size and chain are then those molecule b gets alone, padded to N, with seed seeds_used[b] -- subject to the padding rule
+ * of the size draw above and to the tensor-core caveat of dl_sample_chain_seeded_retry.
+ */
+dl_status dl_sample_chain_seeded_retry_sized(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
+                                             int32_t keep_frames, const float* xh, const int8_t* node_mask,
+                                             const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
+                                             const float* context, const uint64_t* seeds, const dl_step_coef* coef,
+                                             const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries,
+                                             uint64_t* seeds_used, int32_t* attempts, const dl_molecule_checks* checks,
+                                             int32_t* passed, const dl_size_redraw* redraw, int32_t* sizes_used,
+                                             void* stream);
 /*
  * The checks alone, on any (B,N) batch. DEVICE buffers, enqueued on `stream`.
  *   xh        (B,N,>=3+n_types) fp32, row stride xh_row_stride: x at columns 0..2, the atom-type one-hot from column 3
