@@ -346,8 +346,15 @@ Geom make_geom(const dl_engine* e, int B, int N) {
 
 // The work plan of ws (2 launches): live rows and columns of every molecule, then work items of at most tile_edges edges and
 // max_rows rows. Masks are constant over a whole sample_chain: the plan is built once per call.
+// k_plan_mol stages two ints per row in dynamic shared memory, which it gets without raising its attribute: N <= 6144.
+constexpr int PLAN_MAX_N = 48 * 1024 / (2 * (int)sizeof(int));
+
 dl_status build_plan(Workspace& ws, int B, int N, int graph_type, const int8_t* node_mask, const float* linker_mask,
                      const int8_t* edge_mask, int tile_edges, int max_rows, cudaStream_t st) {
+  if (N > PLAN_MAX_N) {
+    set_err("N = %d exceeds the work plan's limit of %d rows per molecule", N, PLAN_MAX_N);
+    return DL_ERR_UNSUPPORTED;
+  }
   CK(cudaMemsetAsync(ws.agg, 0, (size_t)B * N * H * sizeof(float), st));  // dead rows aggregate to exactly 0
   k_plan_mol<<<B, 256, 2 * N * sizeof(int), st>>>(N, graph_type, edge_mask, node_mask, linker_mask, ws.rowidx,
                                                   ws.colidx, ws.xrowidx, ws.nr, ws.nc, ws.nxr);

@@ -669,8 +669,10 @@ __global__ void __launch_bounds__(256, 1) k_edge_simt(Geom gm, EdgeArgs a) {
             d = dx * dx + dy * dy + dz * dz;
             float ex = yi[0] - yj[0], ey = yi[1] - yj[1], ez = yi[2] - yj[2];
             d0 = ex * ex + ey * ey + ez * ez;
-            if constexpr (EMB) {                          // the reference's rounding order for the sinusoid arguments
-              d = radial_rn(dx, dy, dz); d0 = radial_rn(ex, ey, ez);
+            // the reference's rounding order, not the contracted FMA form, where it decides something: the sinusoid
+            // arguments, and SizeGNN's edge set (radial < 6)
+            if constexpr (EMB || ACT == ACT_RELU) { d = radial_rn(dx, dy, dz); d0 = radial_rn(ex, ey, ez); }
+            if constexpr (EMB) {
 #pragma unroll
               for (int k = 0; k < N_SIN_FREQ; ++k) {
                 sincosf(sin_arg(d, k), &emb[k], &emb[N_SIN_FREQ + k]);

@@ -52,6 +52,28 @@ for _n in (32, 64, 128, 256, 512):
                                               T=10, seed=5)
 
 
+# Linker-size classifier batches: GEOM types without pockets, and a pocket batch on a 10-column one-hot whose pockets (140
+# atoms) give every pocket row more than 128 live columns once with_pocket moves them to the origin.
+SIZE_GNN_SPECS = {
+    "size_geom": WorkloadSpec("size_geom", B=5, N=40, n_min=15, l_min=2, l_max=10, F=9, L=2, T=10, seed=24),
+    "size_pocket_geom": WorkloadSpec("size_pocket_geom", B=3, N=160, n_min=150, l_min=4, l_max=8, F=10, L=2, T=10,
+                                     seed=23, pocket=140, graph_type='4A'),
+}
+
+
+def size_gnn_items(spec: WorkloadSpec, batch: int):
+    """make_items, and on pocket specs the fragment-only atoms of the last type moved to type 0: the last one-hot column
+    is then zero on every fragment-only row, as SizeClassifier.forward(adjust_shape=True) requires before dropping it."""
+    items = make_items(spec, batch=batch)
+    if spec.pocket:
+        for it in items:
+            oh = it['one_hot']
+            move = (it['fragment_only_mask'] != 0) & (oh[:, -1] != 0)
+            oh[move, -1] = 0.0
+            oh[move, 0] = 1.0
+    return items
+
+
 def model_hparams(spec: WorkloadSpec) -> dict:
     """DDPM hyper-parameters of the corresponding published config (configs/*.yml: nf 128, inv_sublayers 2,
     norm_constant 1e-6, normalization_factor 100, normalize_factors [1,4,10], polynomial_2, precision 1e-5)."""

@@ -554,7 +554,8 @@ dl_status dl_sizegnn_finalize_weights(dl_sizegnn* e);
  *   xh            (B,N,3+in_node_nf) fp32: [positions | one_hot] (the kernel applies fragment_mask to both)
  *   fragment_mask (B,N) int8 0/1       (data['fragment_mask'], or 'fragment_only_mask' with pockets)
  *   edge_mask     (B,N,N) int8, non-zero = live pair (datasets.collate_with_fragment_edges, datasets.py:396-402), or NULL
- *   out           (B,out_node_nf) fp32 logits */
+ *   out           (B,out_node_nf) fp32 logits
+ * N > 6144 is DL_ERR_UNSUPPORTED (the work plan's shared-memory staging; the same limit holds for every forward). */
 dl_status dl_sizegnn_forward(dl_sizegnn* e, int32_t B, int32_t N, const float* xh, const int8_t* fragment_mask,
                              const int8_t* edge_mask, float* out, void* stream);
 

@@ -469,14 +469,16 @@ def _bn_eval(sd, prefix, v, eps=1e-5):
         + sd[prefix + ".bias"]
 
 
-def size_gcl_forward(sd, prefix, h, row, col, edge_attr, node_mask, edge_mask, normalization):
+def size_gcl_forward(sd, prefix, h, edge_blocks, node_mask, normalization):
     """egnn.GCL with activation=ReLU, edges_in_d=1, normalization_factor=1, 'sum' (egnn.py:10-80 as built by
-    linker_size.py:53-83)."""
-    e_in = torch.cat([h.index_select(0, row), h.index_select(0, col), edge_attr], dim=1)
-    m = F.relu(_lin(sd, prefix + ".edge_mlp.0", e_in))
-    m = F.relu(_lin(sd, prefix + ".edge_mlp.2", m))
-    m = m * edge_mask
-    agg = segment_reduce(m, row, h.shape[0], 1, "sum")
+    linker_size.py:53-83), over the live edges only: a masked edge contributes m * 0 = 0 to the sum exactly, so leaving it
+    out changes nothing. `edge_blocks` holds (row, col, radial) blocks of live edges in the reference's edge order."""
+    agg = h.new_zeros(h.shape)
+    for row, col, radial in edge_blocks:
+        e_in = torch.cat([h.index_select(0, row), h.index_select(0, col), radial], dim=1)
+        m = F.relu(_lin(sd, prefix + ".edge_mlp.0", e_in))
+        m = F.relu(_lin(sd, prefix + ".edge_mlp.2", m))
+        agg.index_add_(0, row, m)
     n_in = torch.cat([h, agg], dim=1)
     if normalization is None:
         upd = _lin(sd, prefix + ".node_mlp.2", F.relu(_lin(sd, prefix + ".node_mlp.0", n_in)))
@@ -486,27 +488,56 @@ def size_gcl_forward(sd, prefix, h, row, col, edge_attr, node_mask, edge_mask, n
     return (h + upd) * node_mask
 
 
+def size_live_edges(x32, edge_mask, B, N, max_pairs=1 << 20):
+    """The size classifier's edges (linker_size_lightning.py:107-108): e = b*N*N + i*N + j is one when edge_mask[e] != 0
+    and the fp32 squared distance is < 6, with the squared distance in torch's rounding order, (dx^2 + dy^2) + dz^2 with
+    every term rounded. Returns (row, col) int64 blocks of global node indices, in edge order, each block from at most
+    `max_pairs` candidate pairs, so that the whole (B*N*N) edge list never exists at once."""
+    em = edge_mask.reshape(B, N, N)
+    xb = x32.reshape(B, N, 3)
+    rows = max(1, max_pairs // N)
+    out = []
+    for b in range(B):
+        for i0 in range(0, N, rows):
+            i1 = min(N, i0 + rows)
+            d = xb[b, i0:i1, None, :] - xb[b, None, :, :]                # (rows, N, 3) fp32
+            sq = d * d
+            radial = (sq[..., 0] + sq[..., 1]) + sq[..., 2]
+            ii, jj = torch.nonzero((em[b, i0:i1] != 0) & (radial < 6), as_tuple=True)
+            if ii.numel():
+                out.append((ii + (b * N + i0), jj + b * N))
+    return out
+
+
 def size_classifier_forward(sd, data, in_node_nf, n_layers, normalization=None, with_pocket=False, adjust_shape=False,
-                            prefix="gnn"):
+                            prefix="gnn", dtype=torch.float32):
     """SizeClassifier.forward(return_loss=False) (linker_size_lightning.py:83-110) with SizeGNN.forward inlined
-    (linker_size.py:85-91). `data` as produced by collate_with_fragment_edges. Returns the (B, classes) logits."""
-    h, x = data['one_hot'].float(), data['positions'].float()
+    (linker_size.py:85-91). `data` as produced by collate_with_fragment_edges (its `edges` list is not read). Returns the
+    (B, classes) logits in `dtype`, computed on the device of data['positions'].
+
+    The edge set is the reference's in any dtype: radial < 6 is evaluated on the fp32 radial in torch's rounding order.
+    The state dict, positions and one-hot are then cast to `dtype` before any arithmetic, and the edge MLP runs over the
+    live edges in blocks, so the peak memory stays a few GB up to N = 6144 in float64."""
+    dev = data['positions'].device
     fragment_mask = (data['fragment_only_mask'] if with_pocket else data['fragment_mask']).float()
-    x = x * fragment_mask
-    h = h * fragment_mask
+    x32 = data['positions'].float() * fragment_mask
+    B, N = x32.shape[0], x32.shape[1]
+    blocks = size_live_edges(x32.reshape(B * N, 3), data['edge_mask'].reshape(-1).to(dev), B, N)
+    sd = {k: v.to(device=dev, dtype=dtype) if v.is_floating_point() else v.to(dev) for k, v in sd.items()}
+    fragment_mask = fragment_mask.to(dtype)
+    x = (data['positions'].to(dtype) * fragment_mask).reshape(B * N, 3)
+    h = data['one_hot'].to(dtype) * fragment_mask
     if h.shape[-1] != in_node_nf and adjust_shape:
         h = h[..., :-1]
-    B, N = x.shape[0], x.shape[1]
     fm = fragment_mask.reshape(B * N, 1)
-    x = x.reshape(B * N, -1)
     h = h.reshape(B * N, -1)
-    row, col = fc_edge_index(N, B)                                        # datasets.py:405-412
-    radial, _ = pair_geometry(x, row, col)                                # coord2diff: SQUARED distance
-    em = (data['edge_mask'].reshape(-1, 1).bool() & (radial < 6)).long()  # linker_size_lightning.py:107-108
+    edge_blocks = []
+    for row, col in blocks:                                               # coord2diff: SQUARED distance, in `dtype`
+        edge_blocks.append((row, col, (x.index_select(0, row) - x.index_select(0, col)).pow(2).sum(1, keepdim=True)))
     h = _lin(sd, prefix + ".embedding_in", h)
-    h = size_gcl_forward(sd, prefix + ".gcl1", h, row, col, radial, fm, em, normalization)
+    h = size_gcl_forward(sd, prefix + ".gcl1", h, edge_blocks, fm, normalization)
     for l in range(n_layers - 1):
-        h = size_gcl_forward(sd, f"{prefix}.gcl_layers.{l}", h, row, col, radial, fm, em, normalization)
+        h = size_gcl_forward(sd, f"{prefix}.gcl_layers.{l}", h, edge_blocks, fm, normalization)
     out = _lin(sd, prefix + ".embedding_out", h)
     return out.view(B, N, -1).mean(1)
 

@@ -238,34 +238,53 @@ def golden_inpaint_chain(ns, name, spec, nb, seed, keep_frames):
 def golden_size_classifier(ns):
     """SizeClassifier.forward(return_loss=False) of the live reference (linker_size_lightning.py:83-110) on batches built by
     the reference's collate_with_fragment_edges; pins oracle.size_classifier_forward and the host mirror's parameter
-    layout / collate."""
+    layout / collate. size_gnn_pocket_geom takes the pocket branch (with_pocket, adjust_shape: the fragment-only rows' last
+    one-hot column is zero and is dropped) with every pocket atom at the origin, so its pocket rows have > 128 live columns."""
     import importlib
     from difflinker_b200 import linker_size as mine
     lsl = importlib.import_module("src.linker_size_lightning")
-    for name, spec, nb, normalization, seed in (("size_gnn_zinc", synthetic.SPECS["cfg1_plumbing"], 4, None, 5),
-                                                ("size_gnn_zinc_bn", synthetic.SPECS["cfg2_zinc_ragged"], 6, "batch_norm", 6)):
-        out_nf = len(ns.const.ZINC_TRAIN_LINKER_ID2SIZE)
+    zinc, geom = (ns.const.ZINC_TRAIN_LINKER_ID2SIZE, ns.const.ZINC_TRAIN_LINKER_SIZE2ID), \
+        (ns.const.GEOM_TRAIN_LINKER_ID2SIZE, ns.const.GEOM_TRAIN_LINKER_SIZE2ID)
+    cases = (  # name, spec, batch, normalization, seed, n_layers, table, in_node_nf, pocket
+        ("size_gnn_zinc", synthetic.SPECS["cfg1_plumbing"], 4, None, 5, 3, zinc, None, False),
+        ("size_gnn_zinc_bn", synthetic.SPECS["cfg2_zinc_ragged"], 6, "batch_norm", 6, 3, zinc, None, False),
+        ("size_gnn_pocket_geom", synthetic.SIZE_GNN_SPECS["size_pocket_geom"], 3, "batch_norm", 7, 3, geom, 9, True),
+        ("size_gnn_geom", synthetic.SIZE_GNN_SPECS["size_geom"], 5, None, 8, 2, geom, None, False),
+    )
+    for name, spec, nb, normalization, seed, n_layers, (id2size, size2id), in_nf, pocket in cases:
+        in_nf = in_nf or spec.F
+        out_nf = len(id2size)
         torch.manual_seed(seed)
-        ref = lsl.SizeClassifier(None, None, None, in_node_nf=spec.F, hidden_nf=128, out_node_nf=out_nf, n_layers=3,
-                                 batch_size=nb, lr=1e-3, torch_device='cpu', normalization=normalization)
+        ref = lsl.SizeClassifier(None, None, None, in_node_nf=in_nf, hidden_nf=128, out_node_nf=out_nf, n_layers=n_layers,
+                                 batch_size=nb, lr=1e-3, torch_device='cpu', normalization=normalization,
+                                 linker_size2id=size2id, linker_id2size=id2size)
         torch.manual_seed(seed)
-        host = mine.SizeClassifier(in_node_nf=spec.F, hidden_nf=128, out_node_nf=out_nf, n_layers=3, normalization=normalization)
+        host = mine.SizeClassifier(in_node_nf=in_nf, hidden_nf=128, out_node_nf=out_nf, n_layers=n_layers,
+                                   normalization=normalization, linker_size2id=size2id, linker_id2size=id2size)
         assert list(ref.state_dict().keys()) == list(host.state_dict().keys()), name
         for k, v in ref.state_dict().items():
             assert torch.equal(v, host.state_dict()[k]), (name, k)
         synthetic.init_size_gnn_like_trained(ref, seed)
         ref.eval()
-        items = synthetic.make_items(spec, batch=nb)
+        items = synthetic.size_gnn_items(spec, nb)
         data = ns.datasets.collate_with_fragment_edges(items)
         mydata = mine.collate_with_fragment_edges(items)
         assert torch.equal(data['edge_mask'], mydata['edge_mask']) and torch.equal(data['edges'][0], mydata['edges'][0]) \
             and torch.equal(data['edges'][1], mydata['edges'][1]), name
+        if pocket:
+            fo = data['fragment_only_mask'][..., 0]
+            assert data['one_hot'].shape[-1] == in_nf + 1 and (data['one_hot'][..., -1] * fo == 0).all()
+            assert (data['one_hot'][..., -1] * data['pocket_mask'][..., 0]).sum() > 0, "the dropped column is all zero"
+            live = (data['edge_mask'].view(nb, spec.N, spec.N) != 0).sum(-1)
+            assert int(live.max()) > 128, name
         with torch.no_grad():
-            out, loss = ref.forward(data, return_loss=False)
-            ora = orc.size_classifier_forward(ref.state_dict(), data, spec.F, 3, normalization)
+            out, loss = ref.forward(data, return_loss=False, with_pocket=pocket, adjust_shape=pocket)
+            ora = orc.size_classifier_forward(ref.state_dict(), data, in_nf, n_layers, normalization, with_pocket=pocket,
+                                              adjust_shape=pocket)
         err = (out - ora).abs().max().item()
         assert err <= 1e-6 * max(1.0, out.abs().max().item()), f"{name}: oracle vs reference {err}"
         save(name, dict(kind="size_gnn", spec=spec.name, batch=nb, seed=seed, normalization=normalization, out_nf=out_nf,
+                        n_layers=n_layers, in_node_nf=in_nf, with_pocket=pocket, adjust_shape=pocket,
                         sha=state_sha(ref.state_dict()), oracle_max_abs_err=err), logits=out)
 
 

@@ -24,7 +24,14 @@ for _gt in ("FC-10A-4A", "FC-4A", "4A"):
 
 
 def spec_by_name(name):
-    return synthetic.SPECS.get(name) or EXTRA_SPECS[name]
+    return synthetic.SPECS.get(name) or synthetic.SIZE_GNN_SPECS.get(name) or EXTRA_SPECS[name]
+
+
+def size_forward_kw(meta):
+    """The oracle arguments of a size_gnn fixture after (sd, data): in_node_nf, n_layers, normalization and the pocket flags."""
+    return dict(in_node_nf=meta.get("in_node_nf") or spec_by_name(meta["spec"]).F, n_layers=meta.get("n_layers", 3),
+                normalization=meta["normalization"], with_pocket=meta.get("with_pocket", False),
+                adjust_shape=meta.get("adjust_shape", False))
 
 
 def load_golden(name):
@@ -76,12 +83,16 @@ def build_size_classifier(meta):
     fixture's batch (collate_with_fragment_edges layout)."""
     from difflinker_b200 import linker_size
     spec = spec_by_name(meta["spec"])
+    kw = size_forward_kw(meta)
+    geom = meta["out_nf"] == len(linker_size.GEOM_TRAIN_LINKER_ID2SIZE)
+    tables = dict(linker_size2id=linker_size.GEOM_TRAIN_LINKER_SIZE2ID, linker_id2size=linker_size.GEOM_TRAIN_LINKER_ID2SIZE) \
+        if geom else {}
     torch.manual_seed(meta["seed"])
-    model = linker_size.SizeClassifier(in_node_nf=spec.F, hidden_nf=128, out_node_nf=meta["out_nf"], n_layers=3,
-                                       normalization=meta["normalization"])
+    model = linker_size.SizeClassifier(in_node_nf=kw["in_node_nf"], hidden_nf=128, out_node_nf=meta["out_nf"],
+                                       n_layers=kw["n_layers"], normalization=meta["normalization"], **tables)
     synthetic.init_size_gnn_like_trained(model, meta["seed"])
     model.eval()
-    data = linker_size.collate_with_fragment_edges(synthetic.make_items(spec, batch=meta["batch"]))
+    data = linker_size.collate_with_fragment_edges(synthetic.size_gnn_items(spec, meta["batch"]))
     return model, data
 
 

@@ -567,19 +567,25 @@ def test_restore_frame_with_sampled_linker_sizes():
     assert rel_err(got[..., :3], want) <= 1e-6 and torch.equal(got[..., 3:], chain0[..., 3:])
 
 
-@pytest.mark.parametrize("name", ["size_gnn_zinc", "size_gnn_zinc_bn"])
+@pytest.mark.parametrize("name", ["size_gnn_zinc", "size_gnn_zinc_bn", "size_gnn_pocket_geom", "size_gnn_geom"])
 def test_size_classifier_matches_reference_golden(name):
     """SizeClassifier.forward(return_loss=False) (linker_size_lightning.py:83-110): native logits vs the live reference's
-    (eval-mode batch norm folded on the host in the _bn case); then the sample_fn of generate.py:90-99."""
+    (eval-mode batch norm folded on the host in the _bn and pocket cases; the pocket case takes with_pocket and
+    adjust_shape); then the sample_fn of generate.py:90-99."""
     meta, a = helpers.load_golden(name)
     model, data = helpers.build_size_classifier(meta)
+    assert helpers.state_sha(model.state_dict()) == meta["sha"]
     d = dev()
     dd = {k: (v.to(d) if torch.is_tensor(v) else v) for k, v in data.items()}
-    out, loss = model.forward(dd, return_loss=False)
+    kw = helpers.size_forward_kw(meta)
+    pocket = dict(with_pocket=kw["with_pocket"], adjust_shape=kw["adjust_shape"])
+    out, loss = model.forward(dd, return_loss=False, **pocket)
     assert loss is None and out.shape == a["logits"].shape
     assert rel_err(out.cpu(), a["logits"]) <= 1e-5
-    out2, loss2 = model.forward(dd, return_loss=True)
+    out2, loss2 = model.forward(dd, return_loss=True, **pocket)
     assert torch.equal(out2, out) and torch.isfinite(loss2)
+    if kw["with_pocket"]:                                                 # sample_sizes is the non-pocket sample_fn
+        return
     sizes = model.sample_sizes(dd, generator=torch.Generator(device=d).manual_seed(0))
     assert sizes.dtype == torch.int8 and sizes.shape == (meta["batch"],)
     assert set(sizes.tolist()) <= set(model.linker_id2size)

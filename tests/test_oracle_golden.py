@@ -74,13 +74,13 @@ def test_oracle_inpainting_chain_matches_reference_golden():
     assert torch.equal(chain[0][:, :, 3:], a["chain"][0][:, :, 3:])
 
 
-@pytest.mark.parametrize("name", ["size_gnn_zinc", "size_gnn_zinc_bn"])
+@pytest.mark.parametrize("name", ["size_gnn_zinc", "size_gnn_zinc_bn", "size_gnn_pocket_geom", "size_gnn_geom"])
 def test_oracle_size_classifier_matches_reference_golden(name):
     meta, a = helpers.load_golden(name)
     model, data = helpers.build_size_classifier(meta)
     assert helpers.state_sha(model.state_dict()) == meta["sha"]
     with torch.no_grad():
-        out = orc.size_classifier_forward(model.state_dict(), data, model.in_node_nf, 3, meta["normalization"])
+        out = orc.size_classifier_forward(model.state_dict(), data, **helpers.size_forward_kw(meta))
     assert out.shape == a["logits"].shape                               # (B, classes)
     assert (out - a["logits"]).abs().max().item() <= 2e-6 * max(1.0, a["logits"].abs().max().item())
 
