@@ -37,13 +37,14 @@ class DLSizeGNNConfig(C.Structure):
 
 class DLMoleculeChecks(C.Structure):
     _fields_ = [("require", C.c_int32), ("n_types", C.c_int32), ("thr1", C.c_void_p), ("thr2", C.c_void_p),
-                ("thr3", C.c_void_p), ("max_valence", C.c_void_p)]
+                ("thr3", C.c_void_p), ("max_valence", C.c_void_p), ("clash", C.c_void_p)]
 
     @classmethod
-    def of(cls, require, tables):
-        """The struct over `tables` = [thr1] or [thr1, thr2, thr3, max_valence], device tensors the caller keeps alive."""
+    def of(cls, require, tables, clash=None):
+        """The struct over `tables` = [thr1] or [thr1, thr2, thr3, max_valence] and the (T,T) `clash` table (None: none),
+        device tensors the caller keeps alive."""
         ptrs = [t.data_ptr() for t in tables] + [None] * (4 - len(tables))
-        return cls(require, tables[0].shape[0], *ptrs)
+        return cls(require, tables[0].shape[0], *ptrs, None if clash is None else clash.data_ptr())
 
 
 class DLSizeRedraw(C.Structure):
@@ -74,17 +75,11 @@ SYMBOLS = {
                                    _P, _P]),
     "dl_sample_chain_seeded": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "dl_retry_seed": (C.c_uint64, [C.c_uint64, _I32]),
-    "dl_sample_chain_seeded_retry": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32,
-                                            _P, _P, _P]),
-    "dl_sample_chain_seeded_retry_checked": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
-                                                    _P, _I32, _P, _P, C.POINTER(DLMoleculeChecks), _P, _P]),
-    "dl_sample_chain_seeded_retry_sized": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
-                                                  _P, _I32, _P, _P, C.POINTER(DLMoleculeChecks), _P,
-                                                  C.POINTER(DLSizeRedraw), _P, _P]),
+    "dl_sample_chain_retry": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32, _P,
+                                     _P, C.POINTER(DLMoleculeChecks), _P, C.POINTER(DLSizeRedraw), _P, _P]),
     "dl_size_draw": (_I32, [_I32, _I32, _P, _I32, _P, _P, _I32, _P, _P]),
     "dl_size_uniform": (C.c_double, [C.c_uint64]),
     "dl_molecule_check": (_I32, [_I32, _I32, C.POINTER(DLMoleculeChecks), _P, _I32, _P, _P, _I32, _I32, _P, _P, _P]),
-    "dl_set_clash_table": (_I32, [_P, _P]),
     "dl_clash_check": (_I32, [_I32, _I32, _I32, _P, _P, _I32, _P, _P, _P, _I32, _P, _P, _P]),
     "dl_last_retry_ms": (_F, [_P]),
     "dl_set_noise_slice": (_I32, [_P, _I32, _I32]),

@@ -58,7 +58,7 @@ struct Workspace {
   std::vector<void*> allocs;
 };
 
-struct HostStage {  // device staging for the *_host entry points, and the sub-batch rows of dl_sample_chain_seeded_retry
+struct HostStage {  // device staging for the *_host entry points, and the sub-batch rows of dl_sample_chain_retry
   size_t cap = 0;
   char* buf = nullptr;
 };
@@ -120,8 +120,6 @@ struct dl_engine {
   // dl_set_start_step: the linker sampler starts at step start_step from q(z_t0 | x) with these scalars; -1: from noise at T
   int start_step = -1;
   float start_alpha = 0.f, start_sigma = 0.f;
-  // dl_set_clash_table: the caller's (n_types, n_types) clash distances for DL_CHECK_CLASH; null: none set
-  const float* clash_table = nullptr;
   bool finalized = false;
   std::map<std::string, std::vector<float>> raw;
   float* wblob = nullptr;      // packed fp32 weights
@@ -130,7 +128,7 @@ struct dl_engine {
   std::vector<EqW> eq;         // [L]
   const float *We_t = nullptr, *be = nullptr, *Wo = nullptr, *bo = nullptr;
   Workspace ws;
-  // dl_sample_chain_seeded_retry: the loop workspace of the failed molecules' sub-batch (cached by (B', N) like ws, which it
+  // dl_sample_chain_retry: the loop workspace of the failed molecules' sub-batch (cached by (B', N) like ws, which it
   // never frees or resizes), their gathered inputs and chain, and the events of the rounds (ev_r*: the sub-batch loop's
   // own, so ev_t0/ev_t1 keep timing the first loop; ev_g*: one round, gather to scatter)
   Workspace ws_sub;
@@ -985,12 +983,6 @@ dl_status dl_set_start_step(dl_engine* e, int32_t t0, float alpha_t0, float sigm
   return DL_OK;
 }
 
-dl_status dl_set_clash_table(dl_engine* e, const float* clash) {
-  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
-  e->clash_table = clash;
-  return DL_OK;
-}
-
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream) {
   dl_status s = check_shapes(e, B, N);
@@ -1221,11 +1213,11 @@ CheckArgs check_args(const dl_engine* e, const dl_molecule_checks& ck, const flo
                     e->cfg.graph_type != DL_GRAPH_FC, passed);
 }
 
-// What is wrong with the checks of a dl_sample_chain_seeded_retry_checked / _sized call, or null.
+// What is wrong with the checks of a dl_sample_chain_retry call, or null.
 const char* checked_error(const dl_engine* e, int32_t sampler, int N, const dl_molecule_checks* checks) {
   const char* why = checks_error(checks, N, e->cfg.in_node_nf, true);
   if (!why && (checks->require & DL_CHECK_CLASH)) {
-    if (!e->clash_table) why = "DL_CHECK_CLASH needs a clash table (dl_set_clash_table)";
+    if (!checks->clash) why = "DL_CHECK_CLASH needs a clash table (checks->clash)";
     else if (e->cfg.graph_type == DL_GRAPH_FC) why = "DL_CHECK_CLASH needs a pocket: DL_GRAPH_FC graphs have none";
     else if (sampler == DL_SAMPLER_INPAINT) why = "DL_CHECK_CLASH does not take DL_SAMPLER_INPAINT, which re-noises the pocket";
   }
@@ -1255,7 +1247,7 @@ const char* redraw_error(int32_t sampler, int B, int N, const dl_size_redraw* rz
   return nullptr;
 }
 
-// dl_sample_chain_seeded_retry, and with `ck` its molecule checks, whose verdicts go to `passed`: a row then fails if its NaN
+// dl_sample_chain_retry, and with `ck` its molecule checks, whose verdicts go to `passed`: a row then fails if its NaN
 // flag is set or a required bit is missing, and a resampled row replaces the caller's unless the caller's row is finite and
 // the new one diverged.
 dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames, const float* xh,
@@ -1274,7 +1266,7 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
   const int require = ck ? ck->require : 0;
   std::vector<int32_t> flags(B), pass(B, require);
   if (ck) {
-    const ClashArgs cl{linker_mask, e->clash_table, nullptr};   // the clash check's linker rows and table
+    const ClashArgs cl{linker_mask, ck->clash, nullptr};   // the clash check's linker rows and table
     CK(launch_molecule_check(require, check_args(e, *ck, chain, N, node_mask, context, passed), cl, B, st));
     e->launches += 1;
     CK(cudaMemcpyAsync(pass.data(), passed, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1332,7 +1324,7 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     if (ck) {
       CheckArgs ca = check_args(e, *ck, sa.s_chain, N, ga.s_node_mask, ga.s_context, sl.at<int32_t>(i_ps));
       ca.rows = ga.rows; ca.flags = nan_flags; ca.s_flags = sa.s_flags; ca.take = sl.at<int32_t>(i_tk);
-      CK(launch_molecule_check(require, ca, ClashArgs{ga.s_linker_mask, e->clash_table, nullptr}, Bs, st));
+      CK(launch_molecule_check(require, ca, ClashArgs{ga.s_linker_mask, ck->clash, nullptr}, Bs, st));
       e->launches += 1;
       sa.take = ca.take; sa.s_passed = ca.passed; sa.passed = passed;
       if (rz) k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa, za);
@@ -1366,63 +1358,26 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
 
 extern "C" {
 
-dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
-                                       const float* xh, const int8_t* node_mask, const float* fragment_mask,
-                                       const float* linker_mask, const int8_t* edge_mask, const float* context,
-                                       const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
-                                       int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
-                                       void* stream) {
+dl_status dl_sample_chain_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                                const float* xh, const int8_t* node_mask, const float* fragment_mask, const float* linker_mask,
+                                const int8_t* edge_mask, const float* context, const uint64_t* seeds, const dl_step_coef* coef,
+                                const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used,
+                                int32_t* attempts, const dl_molecule_checks* checks, int32_t* passed,
+                                const dl_size_redraw* redraw, int32_t* sizes_used, void* stream) {
   if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
   if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
-  if (!nan_flags || !seeds_used || !attempts) { set_err("null argument (nan_flags, seeds_used or attempts)"); return DL_ERR_INVALID; }
-  return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
-                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, nullptr, nullptr, nullptr, nullptr,
-                      stream);
-}
-
-dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
-                                               int32_t keep_frames, const float* xh, const int8_t* node_mask,
-                                               const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
-                                               const float* context, const uint64_t* seeds, const dl_step_coef* coef,
-                                               const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries,
-                                               uint64_t* seeds_used, int32_t* attempts, const dl_molecule_checks* checks,
-                                               int32_t* passed, void* stream) {
-  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
-  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
-  if (!nan_flags || !seeds_used || !attempts || !passed) {
-    set_err("null argument (nan_flags, seeds_used, attempts or passed)");
-    return DL_ERR_INVALID;
-  }
-  const char* why = checked_error(e, sampler, N, checks);
-  if (why) {
-    set_err("dl_sample_chain_seeded_retry_checked: %s", why);
-    return DL_ERR_INVALID;
-  }
-  return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
-                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, passed, nullptr, nullptr,
-                      stream);
-}
-
-dl_status dl_sample_chain_seeded_retry_sized(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
-                                             int32_t keep_frames, const float* xh, const int8_t* node_mask,
-                                             const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
-                                             const float* context, const uint64_t* seeds, const dl_step_coef* coef,
-                                             const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries,
-                                             uint64_t* seeds_used, int32_t* attempts, const dl_molecule_checks* checks,
-                                             int32_t* passed, const dl_size_redraw* redraw, int32_t* sizes_used,
-                                             void* stream) {
-  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
-  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
-  if (!nan_flags || !seeds_used || !attempts || (checks && !passed) || !redraw || !sizes_used) {
-    set_err("dl_sample_chain_seeded_retry_sized: null argument (nan_flags, seeds_used, attempts, passed with checks, "
-            "redraw or sizes_used)");
+  if (!nan_flags || !seeds_used || !attempts || (checks && !passed) || (redraw && !sizes_used)) {
+    set_err("dl_sample_chain_retry: null argument (nan_flags, seeds_used, attempts, passed with checks or sizes_used with "
+            "redraw)");
     return DL_ERR_INVALID;
   }
   const char* why = checks ? checked_error(e, sampler, N, checks) : nullptr;
-  if (!why && cudaSetDevice(e->cfg.device) != cudaSuccess) why = "cudaSetDevice failed";
-  if (!why) why = redraw_error(sampler, B, N, redraw, reinterpret_cast<cudaStream_t>(stream));
+  if (!why && redraw) {
+    if (cudaSetDevice(e->cfg.device) != cudaSuccess) why = "cudaSetDevice failed";
+    else why = redraw_error(sampler, B, N, redraw, reinterpret_cast<cudaStream_t>(stream));
+  }
   if (why) {
-    set_err("dl_sample_chain_seeded_retry_sized: %s", why);
+    set_err("dl_sample_chain_retry: %s", why);
     return DL_ERR_INVALID;
   }
   return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,

@@ -1,4 +1,4 @@
-// Per-molecule NaN recovery (dl_sample_chain_seeded_retry): the seed of a molecule's next attempt, and the row gather /
+// Per-molecule NaN recovery (dl_sample_chain_retry): the seed of a molecule's next attempt, and the row gather /
 // scatter between the caller's full batch and the sub-batch of the molecules that are sampled again.
 #pragma once
 #include <stdint.h>

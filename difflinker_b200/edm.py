@@ -28,7 +28,7 @@ def _generator_of(dev):
 
 
 class LinkerSizes(NamedTuple):
-    """What EDM.sample_chain redraws linker sizes from in its recovery rounds (dl_sample_chain_seeded_retry_sized), for a
+    """What EDM.sample_chain redraws linker sizes from in its recovery rounds (dl_sample_chain_retry), for a
     template built at the sizes dl_size_draw gives the call's seeds at attempt 0 and padded to at least
     max(n_frag) + max(sizes) rows. ddpm.sample_chain(linker_sizes=...) builds it.
       logits    (B, C) fp32 CUDA: every molecule's size logits
@@ -41,29 +41,23 @@ class LinkerSizes(NamedTuple):
     linker_x: torch.Tensor
 
 
-def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None, clash=None):
+def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
-    samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, require, tables,
-    passed, redraw) resamples the molecules that diverged (dl_sample_chain_seeded_retry, which blocks until its rounds are
-    done) and, with `require` != 0, those that miss a required check, whose verdict bits go to `passed`
-    (dl_sample_chain_seeded_retry_checked; `tables` as molecule_builder.check_tables returns them, on the slice's device).
+    samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, require, checks,
+    passed, redraw) resamples the molecules that diverged (dl_sample_chain_retry, which blocks until its rounds are done)
+    and, with `require` != 0, those that miss a required check, whose verdict bits go to `passed`; `checks` = (tables, clash)
+    on the slice's device, `tables` as molecule_builder.check_tables returns them and `clash` the (T,T) clash table or None.
     `redraw` = (logits, size table, n_frag, normalised linker_x, sizes_used), device tensors, redraws the resampled rows'
-    linker sizes (dl_sample_chain_seeded_retry_sized); None keeps them.
+    linker sizes; None keeps them.
     `start` = (t0, alpha_t0, sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of
-    the call (dl_set_start_step). `clash`, a (T,T) table on the slice's device, is the engine's clash table for the duration
-    of the call (dl_set_clash_table), which a `require` with CHECK_CLASH reads. Returns (status, what the batch stream
-    consumed)."""
+    the call (dl_set_start_step). Returns (status, what the batch stream consumed)."""
     if start is not None:
         _native.check(lib.dl_set_start_step(eng, *start), "dl_set_start_step")
     try:
-        if clash is not None:
-            _native.check(lib.dl_set_clash_table(eng, clash.data_ptr()), "dl_set_clash_table")
         return _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry)
     finally:
-        if clash is not None:
-            lib.dl_set_clash_table(eng, None)
         if start is not None:
             lib.dl_set_start_step(eng, -1, 0.0, 0.0)
 
@@ -73,21 +67,17 @@ def _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry):
     if stream is None:
         return _native.check(lib.dl_sample_chain_host(eng, *head, noise.data_ptr(), *tail), "dl_sample_chain_host"), 0
     if retry is not None:
-        max_retries, used, attempts, require, tables, passed, redraw = retry
-        args = (eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr())
+        max_retries, used, attempts, require, checks, passed, redraw = retry
+        ck = _native.DLMoleculeChecks.of(require, *checks) if require else None
+        rz = sizes = None
         if redraw is not None:
             logits, table, n_frag, linker_x, sizes = redraw
             rz = _native.DLSizeRedraw(table.numel(), logits.stride(0), logits.data_ptr(), table.data_ptr(), n_frag.data_ptr(),
                                       linker_x.data_ptr())
-            ck = _native.DLMoleculeChecks.of(require, tables) if require else None
-            return _native.check(lib.dl_sample_chain_seeded_retry_sized(
-                *args, ck, passed.data_ptr() if require else None, rz, sizes.data_ptr(), stream),
-                "dl_sample_chain_seeded_retry_sized"), 0
-        if not require:
-            return _native.check(lib.dl_sample_chain_seeded_retry(*args, stream), "dl_sample_chain_seeded_retry"), 0
-        return _native.check(lib.dl_sample_chain_seeded_retry_checked(
-            *args, _native.DLMoleculeChecks.of(require, tables), passed.data_ptr(), stream),
-            "dl_sample_chain_seeded_retry_checked"), 0
+        return _native.check(lib.dl_sample_chain_retry(
+            eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr(), ck,
+            passed.data_ptr() if require else None, rz, None if sizes is None else sizes.data_ptr(), stream),
+            "dl_sample_chain_retry"), 0
     if seeds is not None:
         return _native.check(lib.dl_sample_chain_seeded(eng, *head, seeds.data_ptr(), *tail, stream),
                              "dl_sample_chain_seeded"), 0
@@ -211,7 +201,7 @@ class EDM(torch.nn.Module):
         self.nan_retries = 0
         self.last_attempts = None              # calls with nan_retries > 0: the (B,) CPU int32 attempt of every row, else None
         # Connectivity: sample_chain also resamples, in the nan_retries rounds, the molecules whose final molecule is in more
-        # than one piece (dl_sample_chain_seeded_retry_checked); needs per-molecule streams and the bond tables of
+        # than one piece (dl_sample_chain_retry); needs per-molecule streams and the bond tables of
         # `is_geom` (the ZINC or the GEOM / MOAD atom types, molecule_builder.threshold_tables), which DDPM, accelerate and
         # load_from_checkpoint set from the model's training data. False, the default, checks nothing.
         self.is_geom = is_geom
@@ -600,7 +590,7 @@ class EDM(torch.nn.Module):
         reproduces its row, including a NaN divergence, so retry a diverged molecule with a new seed.
         `nan_retries` (None: the `nan_retries` attribute, default 0) does that on the device: after the loop, up to that many
         rounds resample only the molecules whose flags are set, as a sub-batch, with seeds dl_retry_seed(seed, round)
-        (dl_sample_chain_seeded_retry). It needs the per-molecule stream -- `seeds` or noise_mode='per_molecule' -- and raises
+        (dl_sample_chain_retry). It needs the per-molecule stream -- `seeds` or noise_mode='per_molecule' -- and raises
         ValueError with the batch stream, noise=, a replaced draw function, host inputs or batch_slice. Rows that did not fail
         are untouched, bit for bit; `last_seeds[b]` is then the seed that produced row b, so molecule b sampled alone with it
         reproduces the row -- bit for bit on the SIMT edge path, and on the tensor-core path while no node tile rescales
@@ -608,7 +598,7 @@ class EDM(torch.nn.Module):
         round raise FoundNaNException with their batch-global indices only; its `chain` attribute holds the recovered chain.
         `require_connected` (None: the `require_connected` attribute, default False) adds a second reason to resample a row:
         its final molecule -- chain[0]'s atoms, without the pocket on cut-off graphs, bonded where get_bond_order > 0 with
-        the tables of `is_geom` -- is in more than one piece (dl_sample_chain_seeded_retry_checked). The check runs on the
+        the tables of `is_geom` -- is in more than one piece (dl_sample_chain_retry's checks). The check runs on the
         device after the loop and after every round; the rounds are the nan_retries rounds, so nan_retries=0 only reports.
         A resampled row replaces the old one unless the old one was finite and the new one diverged. Rows that are still
         disconnected after the last round are returned; `last_connected` (B,) CPU bool tells which rows are connected. It
@@ -625,7 +615,7 @@ class EDM(torch.nn.Module):
         dl_molecule_checks in the header; fragment atoms are not checked). `last_clash_free` (B,) CPU bool tells which rows
         pass. Refusals as for require_valid, plus ValueError on FC graphs and for InpaintingEDM.
         `linker_sizes` (a LinkerSizes; ddpm.sample_chain builds it) makes every round redraw the linker size of the rows it
-        resamples, from the round's seed (dl_sample_chain_seeded_retry_sized), and rebuild their template rows at that size
+        resamples, from the round's seed (dl_sample_chain_retry's redraw), and rebuild their template rows at that size
         inside the padded template. The inputs must be the template of the sizes dl_size_draw gives `seeds` at attempt 0,
         padded to max(n_frag) + max(sizes) rows or more. `last_sizes` (B,) CPU int32 holds every returned row's size. It
         needs `seeds` and raises ValueError where nan_retries does, with start_step and for InpaintingEDM.
@@ -965,16 +955,16 @@ class EDM(torch.nn.Module):
                 redraw_i = ((logits, table, n_frag, linker_x, sizes) if whole else
                             tuple(v.to(where).contiguous() for v in (logits[lo:hi], table, n_frag[lo:hi], linker_x[lo:hi],
                                                                      sizes[lo:hi])))
-            part = part + (None if tables is None else [t.to(where) for t in tables],
-                           None if clash is None else clash.to(where), redraw_i)
+            checks_i = None if tables is None else ([t.to(where) for t in tables], None if clash is None else clash.to(where))
+            part = part + (checks_i, redraw_i)
             parts.append(part)              # alive until the flags have been read below
-            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, tables_i, clash_i, redraw_i = part
+            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, checks_i, redraw_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
             rng_i = None if rng is None else (rng[0], rng[1], rng[2] + lo, rng[3])
             calls.append((dev_i, functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
-                (retries, used_i, attempts_i, check, tables_i, passed_i, redraw_i) if recover else None, start, clash_i)))
+                (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i) if recover else None, start)))
 
         def finish():
             if not whole:
@@ -986,7 +976,7 @@ class EDM(torch.nn.Module):
                 if check:
                     place_rows(passed, [p[7] for p in parts], slices)
                 if redraw is not None:
-                    place_rows(sizes, [p[10][4] for p in parts], slices)
+                    place_rows(sizes, [p[9][4] for p in parts], slices)
             # the host sampler reports NaNs in its status; on the device, one sync per chain instead of one per step
             # (egnn.py:441), after every slice's loop and copy
             bad = _native.DL_NAN_DETECTED in [st for st, _ in results] or bool(flags.any().item())

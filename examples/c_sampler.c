@@ -13,7 +13,7 @@
  * dl_config) holds one uint64 seed per molecule instead of the pair and samples with dl_sample_chain_seeded: each molecule
  * then draws what it would draw sampled alone, so any molecule can be replayed from its seed.
  * out.bin: int32 status, uint64 philox offset consumed (0 for a seeded job), the (keep_frames, B, N, 3+F) chain,
- * B NaN flags. `--retries k` (seeded jobs only) samples with dl_sample_chain_seeded_retry instead: up to k rounds resample
+ * B NaN flags. `--retries k` (seeded jobs only) samples with dl_sample_chain_retry instead: up to k rounds resample
  * the molecules that diverged with new seeds (dl_retry_seed), and out.bin goes on with the B uint64 seeds that produced the
  * rows and the B int32 attempts (0 = the first draw); only rows that still fail keep their flags.
  *
@@ -140,15 +140,15 @@ int main(int argc, char** argv) {
   const int32_t sampler = cfg.centering ? DL_SAMPLER_INPAINT : DL_SAMPLER_LINKER;
   dl_status st;
   if (retries >= 0)   /* blocks until its rounds are done */
-    st = dl_sample_chain_seeded_retry(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, d_seeds, coef, norm,
-                                      d_chain, d_flags, retries, d_used, d_attempts, stream);
+    st = dl_sample_chain_retry(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, d_seeds, coef, norm, d_chain,
+                               d_flags, retries, d_used, d_attempts, NULL, NULL, NULL, NULL, stream);
   else if (seeded)
     st = dl_sample_chain_seeded(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, d_seeds, coef, norm, d_chain,
                                 d_flags, stream);
   else
     st = dl_sample_chain_rng(e, sampler, B, N, T, keep, d_xh, d_nm, d_fm, d_lm, d_em, d_ctx, rng[0], rng[1], &consumed, coef,
                              norm, d_chain, d_flags, stream);
-  if (st < 0) die(retries >= 0 ? "dl_sample_chain_seeded_retry" : seeded ? "dl_sample_chain_seeded" : "dl_sample_chain_rng");
+  if (st < 0) die(retries >= 0 ? "dl_sample_chain_retry" : seeded ? "dl_sample_chain_seeded" : "dl_sample_chain_rng");
   if (cudaStreamSynchronize(stream) != cudaSuccess) { fprintf(stderr, "c_sampler: the sampler's stream failed\n"); return 2; }
 
   float* chain = (float*)malloc(chain_bytes);

@@ -20,16 +20,16 @@
  *   either, one seed per molecule (no reference API)     dl_sample_chain_seeded
  *   EDM, from q(z_t0 | x) of a known linker (edm.py:67-74) dl_set_start_step, then any dl_sample_chain* entry point
  *     at step t0 (partial diffusion, no reference API)
- *   either, resampling only the molecules that diverged  dl_sample_chain_seeded_retry, dl_retry_seed, dl_last_retry_ms
+ *   either, resampling only the molecules that diverged  dl_sample_chain_retry, dl_retry_seed, dl_last_retry_ms
  *     (the reference's callers resample the whole batch, generate.py:153-161)
- *   either, also resampling the molecules that are      dl_sample_chain_seeded_retry_checked, dl_molecule_check
+ *   either, also resampling the molecules that are      dl_sample_chain_retry with dl_molecule_checks, dl_molecule_check
  *     disconnected (is_connected, src/metrics.py:20-27, on the molecules of src/lightning.py:364-377) or have an atom
  *     beyond its valence (the explicit-valence part of validity, src/metrics.py:12-17; see dl_molecule_checks)
- *   either on pocket graphs, also resampling the        dl_set_clash_table, DL_CHECK_CLASH, dl_clash_check
+ *   either on pocket graphs, also resampling the        dl_sample_chain_retry with DL_CHECK_CLASH, dl_clash_check
  *     molecules whose linker clashes with the pocket (no reference API; see dl_molecule_checks)
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   softmax + Categorical.sample of a size model (generate.py:88-99), from dl_size_draw, dl_size_uniform
- *     the molecule's seed, and redrawn in the recovery rounds             dl_sample_chain_seeded_retry_sized
+ *     the molecule's seed, and redrawn in the recovery rounds             dl_sample_chain_retry with dl_size_redraw
  *   build_xae_molecule           src/molecule_builder.py:44-102       dl_bond_orders
  *   frame restore + .xyz text    generate.py:163-171, src/visualizer.py:14-31   dl_restore_frame, dl_format_xyz
  *   utils.FoundNaNException      src/utils.py:274-289    DL_NAN_DETECTED + per-molecule nan_flags
@@ -223,35 +223,13 @@ dl_status dl_sample_chain_seeded(dl_engine* e, int32_t sampler, int32_t B, int32
                                  const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
                                  int32_t* nan_flags, void* stream);
 /*
- * The seed of attempt `attempt` of a molecule whose own seed is `seed` (dl_sample_chain_seeded_retry): attempt 0 (or below)
+ * The seed of attempt `attempt` of a molecule whose own seed is `seed` (dl_sample_chain_retry): attempt 0 (or below)
  * is `seed` itself; attempt a >= 1 is output a of a splitmix64 generator started from `seed`:
  *     z = seed + a * 0x9E3779B97F4A7C15;  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
  *     z = (z ^ (z >> 27)) * 0x94D049BB133111EB;  return z ^ (z >> 31);            (all modulo 2^64)
  * For one attempt distinct seeds give distinct retry seeds. A pure host function.
  */
 uint64_t dl_retry_seed(uint64_t seed, int32_t attempt);
-/*
- * dl_sample_chain_seeded that resamples only the molecules that diverged. BLOCKING, unlike the other sampling entries: it
- * runs the seeded loop, synchronises `stream` once and reads the B flags; then, for up to max_retries rounds, it gathers the
- * molecules whose flag is set into a sub-batch (B' molecules, same N), samples it with dl_retry_seed(seeds[b], a) in round
- * a, and writes its rows back over those molecules' rows of every one of the keep_frames frames of `chain` and of nan_flags.
- * Rows that did not fail are not touched. Molecule b's row is then what dl_sample_chain_seeded gives it alone with seed
- * seeds_used[b] -- bit for bit on the SIMT edge path; on the tensor-core path while no node tile rescales its fp16 operands,
- * and a sub-batch of diverging molecules is where that happens (DESIGN.md section 6). Both samplers, every graph type;
- * cut-off graphs never read edge_mask, so the sub-batch gets none.
- *   max_retries  >= 0 rounds (0: the seeded loop plus the synchronisation)
- *   nan_flags    (B) int32 DEVICE out, required: after the last round only the rows that still fail are set
- *   seeds_used   (B) uint64 DEVICE out: the seed that produced each returned row (its attempt's dl_retry_seed)
- *   attempts     (B) int32 DEVICE out: the attempt that produced each row, 0 = the first draw
- * Returns DL_NAN_DETECTED only if some row still fails after the last round. The sub-batch has a workspace of its own, cached
- * by (B', N); the full batch's is neither freed nor resized. dl_last_elapsed_ms keeps timing the first loop.
- */
-dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
-                                       const float* xh, const int8_t* node_mask, const float* fragment_mask,
-                                       const float* linker_mask, const int8_t* edge_mask, const float* context,
-                                       const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
-                                       int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
-                                       void* stream);
 /*
  * The checks a molecule can be put to, as data: connectivity and valence. Both are evaluated on the device, on the same atoms
  * and with the arithmetic of dl_bond_orders, on what src/lightning.py:364-377 builds from chain[0].
@@ -285,8 +263,8 @@ dl_status dl_sample_chain_seeded_retry(dl_engine* e, int32_t sampler, int32_t B,
  *                   (n_types,n_types) table and that entry is >= 0; a negative entry means the pair never clashes (e.g. a
  *                   covalent warhead's element against the residue it binds).
  *   A molecule with no linker atom or no pocket atom passes. A NaN coordinate compares false and clashes with nothing
- *   (divergence is the NaN flag's business). The table travels outside this struct, through dl_set_clash_table and
- *   dl_clash_check; molecule_builder.clash_table builds a default, 75% of the sum of the two elements' Bondi van der Waals
+ *   (divergence is the NaN flag's business). The table is the struct's `clash` field (dl_clash_check takes it as an
+ *   argument); molecule_builder.clash_table builds a default, 75% of the sum of the two elements' Bondi van der Waals
  *   radii, a common protein-ligand contact tolerance that has not been validated against any docking tool.
  */
 enum { DL_CHECK_CONNECTED = 1, DL_CHECK_VALENCE = 2, DL_CHECK_CLASH = 4 };
@@ -297,27 +275,8 @@ typedef struct dl_molecule_checks {
   const float* thr2;           /* needed for DL_CHECK_VALENCE only */
   const float* thr3;
   const int32_t* max_valence;  /* (n_types) int32 DEVICE; DL_CHECK_VALENCE only */
+  const float* clash;          /* (n_types,n_types) fp32 DEVICE, in pm, [min type][max type]; DL_CHECK_CLASH only */
 } dl_molecule_checks;
-/*
- * dl_sample_chain_seeded_retry whose rounds also resample the rows that miss a required check. The checks run in one launch
- * after the seeded loop and, on the sub-batch, after each round. A row fails if its NaN flag is set or a required bit is
- * missing; a resampled row replaces the caller's row unless the caller's row is finite and the resample diverged. Rows that
- * merely miss a check after the last round are valid samples: they are returned with their bits cleared and do not make the
- * call fail. DL_NAN_DETECTED means that some row still diverges. max_retries = 0 only reports. A row whose fragments alone
- * break the valence rule cannot be repaired by a new linker: it is resampled every round and comes back with the bit cleared
- * (vet inputs with dl_molecule_check).
- *   passed   (B) int32 DEVICE out: the OR of the DL_CHECK_* bits row b's returned molecule satisfies, among those required
- * The other arguments are those of dl_sample_chain_seeded_retry. 1 <= n_types <= in_node_nf, N <= 8192. DL_CHECK_CLASH reads
- * the linker rows of linker_mask (of the sub-batch in the rounds) and the engine's clash table; it is DL_ERR_INVALID without
- * a table (dl_set_clash_table), on DL_GRAPH_FC (no pocket rows) and with DL_SAMPLER_INPAINT (whose loop re-noises the pocket).
- */
-dl_status dl_sample_chain_seeded_retry_checked(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
-                                               int32_t keep_frames, const float* xh, const int8_t* node_mask,
-                                               const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
-                                               const float* context, const uint64_t* seeds, const dl_step_coef* coef,
-                                               const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries,
-                                               uint64_t* seeds_used, int32_t* attempts, const dl_molecule_checks* checks,
-                                               int32_t* passed, void* stream);
 /*
  * Linker sizes drawn from a molecule's seed (no reference API; generate.py:88-99 draws them from one batch-level
  * Categorical.sample). Molecule b's size distribution is a table sizes[0..C) of ints >= 0 with finite fp32 logits
@@ -349,7 +308,7 @@ double dl_size_uniform(uint64_t seed);
 dl_status dl_size_draw(int32_t B, int32_t C, const float* logits, int32_t logits_row_stride, const int32_t* sizes,
                        const uint64_t* seeds, int32_t attempt, int32_t* out_sizes, void* stream);
 /*
- * What dl_sample_chain_seeded_retry_sized redraws sizes from. DEVICE buffers, read while the call runs.
+ * What dl_sample_chain_retry redraws sizes from. DEVICE buffers, read while the call runs.
  */
 typedef struct dl_size_redraw {
   int32_t C;                   /* entries of the size table, >= 1 */
@@ -362,30 +321,55 @@ typedef struct dl_size_redraw {
                                   no linker row to copy them from */
 } dl_size_redraw;
 /*
- * dl_sample_chain_seeded_retry_checked (checks may be NULL: NaN recovery alone, passed is then not read) whose rounds
- * redraw each resampled row's linker size. The inputs are the template of the attempt-0 sizes (dl_size_draw with attempt
- * 0) padded to the capacity N >= max_b n_frag[b] + max(sizes), which every redrawn size fits. In round a, each failing row
- * b draws size s' with dl_retry_seed(seeds[b], a) and is gathered as the template of that size:
+ * dl_sample_chain_seeded that resamples only the molecules that fail: those that diverged and, with `checks`, those that
+ * miss a required check. BLOCKING, unlike the other sampling entries: it runs the seeded loop and the checks (one launch),
+ * synchronises `stream` once and reads the B flags and verdicts; then, for up to max_retries rounds, it gathers the failing
+ * molecules into a sub-batch (B' molecules, same N), samples it with dl_retry_seed(seeds[b], a) in round a, checks it, and
+ * writes the rows it takes back over those molecules' rows of every one of the keep_frames frames of `chain`, of nan_flags
+ * and of passed. A row fails if its NaN flag is set or a required bit is missing; a resampled row replaces the caller's row
+ * unless the caller's row is finite and the resample diverged. Rows that did not fail are not touched. Molecule b's row is
+ * then what dl_sample_chain_seeded gives it alone with seed seeds_used[b] -- bit for bit on the SIMT edge path; on the
+ * tensor-core path while no node tile rescales its fp16 operands, and a sub-batch of diverging molecules is where that
+ * happens (DESIGN.md section 6). Both samplers, every graph type; cut-off graphs never read edge_mask, so the sub-batch gets
+ * none.
+ *   max_retries  >= 0 rounds (0: the seeded loop, the checks and the synchronisation: it only reports)
+ *   nan_flags    (B) int32 DEVICE out, required: after the last round only the rows that still diverge are set
+ *   seeds_used   (B) uint64 DEVICE out: the seed that produced each returned row (its attempt's dl_retry_seed)
+ *   attempts     (B) int32 DEVICE out: the attempt that produced each row, 0 = the first draw
+ *   checks       the molecule checks (dl_molecule_checks), or NULL: NaN recovery alone, and `passed` is not read.
+ *                1 <= n_types <= in_node_nf, N <= 8192. DL_CHECK_CLASH reads the linker rows of linker_mask (of the
+ *                sub-batch in the rounds) and checks->clash; it is DL_ERR_INVALID without a table, on DL_GRAPH_FC (no pocket
+ *                rows) and with DL_SAMPLER_INPAINT (whose loop re-noises the pocket).
+ *   passed       (B) int32 DEVICE out, required with `checks`: the OR of the DL_CHECK_* bits row b's returned molecule
+ *                satisfies, among those required
+ *   redraw       the sizes to redraw each resampled row's linker size from (dl_size_redraw), or NULL: sizes stay fixed,
+ *                and `sizes_used` is not read
+ *   sizes_used   (B) int32 DEVICE in/out, required with `redraw`: the attempt-0 sizes on entry; on return, the size of every
+ *                returned row (a row that is not taken keeps its size)
+ * Rows that merely miss a check after the last round are valid samples: they are returned with their bits cleared and do not
+ * make the call fail. Returns DL_NAN_DETECTED only if some row still diverges after the last round. A row whose fragments
+ * alone break the valence rule cannot be repaired by a new linker: it is resampled every round and comes back with the bit
+ * cleared (vet inputs with dl_molecule_check).
+ * With `redraw`, the inputs are the template of the attempt-0 sizes (dl_size_draw with attempt 0) padded to the capacity
+ * N >= max_b n_frag[b] + max(sizes), which every redrawn size fits. In round a, each failing row b draws size s' with
+ * dl_retry_seed(seeds[b], a) and is gathered as the template of that size:
  *   rows [0, n_frag[b])                copied from the inputs;
  *   rows [n_frag[b], n_frag[b] + s')   linker rows: node_mask 1, linker_mask 1, fragment_mask 0, x = linker_x[b], h 0,
  *                                      context 0;
  *   later rows                          zero; on DL_GRAPH_FC the edge-mask block is batching's int8 rule over the live rows
  *                                      (-1 off the diagonal, -2 on it, 0 elsewhere).
- * The take rule, the NaN flags and the verdicts are those of dl_sample_chain_seeded_retry_checked.
- *   sizes_used  (B) int32 DEVICE in/out: the attempt-0 sizes on entry; on return, the size of every returned row (a row
- *               that is not taken keeps its size)
- * DL_ERR_INVALID with DL_SAMPLER_INPAINT (which has no linker size) and when N < n_frag[b] + max(sizes) for some b. Row b's
- * size and chain are then those molecule b gets alone, padded to N, with seed seeds_used[b] -- subject to the padding rule
- * of the size draw above and to the tensor-core caveat of dl_sample_chain_seeded_retry.
+ * It is DL_ERR_INVALID with DL_SAMPLER_INPAINT (which has no linker size) and when N < n_frag[b] + max(sizes) for some b.
+ * Row b's size and chain are then those molecule b gets alone, padded to N, with seed seeds_used[b] -- subject to the padding
+ * rule of the size draw above and to the tensor-core caveat above.
+ * The sub-batch has a workspace of its own, cached by (B', N); the full batch's is neither freed nor resized.
+ * dl_last_elapsed_ms keeps timing the first loop.
  */
-dl_status dl_sample_chain_seeded_retry_sized(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T,
-                                             int32_t keep_frames, const float* xh, const int8_t* node_mask,
-                                             const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
-                                             const float* context, const uint64_t* seeds, const dl_step_coef* coef,
-                                             const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries,
-                                             uint64_t* seeds_used, int32_t* attempts, const dl_molecule_checks* checks,
-                                             int32_t* passed, const dl_size_redraw* redraw, int32_t* sizes_used,
-                                             void* stream);
+dl_status dl_sample_chain_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                                const float* xh, const int8_t* node_mask, const float* fragment_mask, const float* linker_mask,
+                                const int8_t* edge_mask, const float* context, const uint64_t* seeds, const dl_step_coef* coef,
+                                const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used,
+                                int32_t* attempts, const dl_molecule_checks* checks, int32_t* passed,
+                                const dl_size_redraw* redraw, int32_t* sizes_used, void* stream);
 /*
  * The checks alone, on any (B,N) batch. DEVICE buffers, enqueued on `stream`.
  *   xh        (B,N,>=3+n_types) fp32, row stride xh_row_stride: x at columns 0..2, the atom-type one-hot from column 3
@@ -401,14 +385,8 @@ dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* chec
                             const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
                             int32_t* passed, int32_t* valence, void* stream);
 /*
- * The clash table of the following dl_sample_chain_seeded_retry_checked calls of this engine that require DL_CHECK_CLASH:
- * (checks->n_types)^2 fp32 DEVICE, in pm, [min type][max type] (see dl_molecule_checks), read by those calls and kept alive
- * by the caller while they run. Sticky, like dl_set_start_step; NULL clears it (the default).
- */
-dl_status dl_set_clash_table(dl_engine* e, const float* clash);
-/*
  * DL_CHECK_CLASH alone, on any (B,N) batch, without an engine. DEVICE buffers, enqueued on `stream`.
- *   clash       (n_types,n_types) fp32, in pm, as dl_set_clash_table
+ *   clash       (n_types,n_types) fp32, in pm, as dl_molecule_checks.clash
  *   xh          (B,N,>=3+n_types) fp32, row stride xh_row_stride, as dl_molecule_check
  *   node_mask   (B,N) int8
  *   linker_mask (B,N) fp32: the rows checked against the pocket (to vet a fragment, pass the fragment rows here)
@@ -421,9 +399,9 @@ dl_status dl_set_clash_table(dl_engine* e, const float* clash);
 dl_status dl_clash_check(int32_t B, int32_t N, int32_t n_types, const float* clash, const float* xh, int32_t xh_row_stride,
                          const int8_t* node_mask, const float* linker_mask, const float* context, int32_t context_nf,
                          int32_t* passed, int32_t* clashes, void* stream);
-/* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_seeded_retry(_checked), each from its
- * row gather to its row scatter -- including the wait for the host to capture the sub-batch's step graph -- summed over the
- * rounds; 0 when no round ran. */
+/* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_retry, each from its row gather to
+ * its row scatter -- including the wait for the host to capture the sub-batch's step graph -- summed over the rounds; 0 when
+ * no round ran. */
 float dl_last_retry_ms(dl_engine* e);
 /* Strong scaling (SURVEY 8(e)): this engine samples molecules [b0, b0 + B) of a batch of B_full. The device-side noise of
  * the following dl_sample_chain_rng / dl_noise_fill / dl_noise_fill_inpaint calls is then the slice's ROWS of the
@@ -434,8 +412,8 @@ float dl_last_retry_ms(dl_engine* e);
 dl_status dl_set_noise_slice(dl_engine* e, int32_t B_full, int32_t b0);
 /*
  * Partial diffusion (no reference API; the `optimize` mode of DiffSBDD): the following dl_sample_chain* calls of this engine,
- * the recovery rounds of dl_sample_chain_seeded_retry(_checked) included, vary the linker the caller's xh holds on its
- * linker_mask rows instead of sampling one from pure noise. With 0 <= t0 <= T:
+ * the recovery rounds of dl_sample_chain_retry included, vary the linker the caller's xh holds on its linker_mask rows
+ * instead of sampling one from pure noise. With 0 <= t0 <= T:
  *   z     = xh * fragment_mask + (alpha_t0 * xh + sigma_t0 * eps) * linker_mask,   eps = draw 0 * linker_mask
  *           -- q(z_t0 | x) as EDM.forward draws it (edm.py:67-74), each product and sum rounded on its own; alpha_t0 and
  *           sigma_t0 are sqrt(sigmoid(-gamma)) and sqrt(sigmoid(gamma)) of gamma(t0 / T), evaluated as the caller evaluates

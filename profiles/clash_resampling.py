@@ -1,5 +1,5 @@
 """Pocket clashes in the recovery rounds: the cost of the device-side clash check and of a round that resamples the molecules
-whose linker clashes with the pocket (`sample_chain(..., require_clash_free=True)`, dl_sample_chain_seeded_retry_checked).
+whose linker clashes with the pocket (`sample_chain(..., require_clash_free=True)`, dl_sample_chain_retry).
 
 It prints the card's name, power limit and maximum SM clock, read in this run, beside every number:
   * the clash check alone (dl_clash_check; CUDA events around --launches back-to-back launches after a warm-up, per launch)

@@ -1,5 +1,5 @@
 """Connectivity in the recovery rounds: the cost of the device-side check and of the rounds that resample the disconnected
-molecules (`sample_chain(..., require_connected=True)`, dl_sample_chain_seeded_retry_checked).
+molecules (`sample_chain(..., require_connected=True)`, dl_sample_chain_retry).
 
 Per workload (synthetic weights, seeds 0..B-1, keep_frames=1) it prints:
   * the device time of the check alone (dl_molecule_check with DL_CHECK_CONNECTED, CUDA events, median of --reps calls) on

@@ -1,4 +1,4 @@
-"""NaN recovery: the device time of one recovery round of dl_sample_chain_seeded_retry against a full-batch resample.
+"""NaN recovery: the device time of one recovery round of dl_sample_chain_retry against a full-batch resample.
 
 Samples a workload (synthetic weights, seeds 0..B-1, keep_frames=1) with `nan_retries=1` while k molecules carry a NaN
 fragment coordinate, so exactly those k fail the first loop and are resampled as one sub-batch of k (they fail again: the

@@ -67,7 +67,7 @@ chain, nm = ddpm3.sample_chain({k: mv(v) for k, v in b3.items()}, keep_frames=1,
 print("pocket connected rounds", ddpm3.edm.last_connected.tolist(), ddpm3.edm.last_attempts.tolist())
 
 # valence check, alone and with the connectivity check in the recovery rounds (dl_molecule_check,
-# dl_sample_chain_seeded_retry_checked)
+# dl_sample_chain_retry)
 print("valences", molecule_builder.valences(xh, sd['atom_mask'], False).sum(1).tolist(),
       molecule_builder.valence_ok(xh, sd['atom_mask'], False).tolist())
 chain, nm = ddpm.sample_chain(data, keep_frames=1, seeds=[1, 2, 3], nan_retries=2, require_connected=True, require_valid=True)

@@ -1,5 +1,5 @@
 """Valence in the recovery rounds: the cost of the device-side molecule checks and of the rounds that resample the molecules
-failing them (`sample_chain(..., require_valid=True, require_connected=True)`, dl_sample_chain_seeded_retry_checked).
+failing them (`sample_chain(..., require_valid=True, require_connected=True)`, dl_sample_chain_retry).
 
 It prints the card's name, power limit and maximum SM clock, read in this run, beside every number:
   * the check alone (dl_molecule_check: valence, connectivity, both; CUDA events around --launches back-to-back launches

@@ -1,5 +1,5 @@
-"""Pocket clashes in the recovery rounds: `sample_chain(..., require_clash_free=True)`, dl_sample_chain_seeded_retry_checked
-with DL_CHECK_CLASH, and dl_clash_check.
+"""Pocket clashes in the recovery rounds: `sample_chain(..., require_clash_free=True)`, dl_sample_chain_retry with
+DL_CHECK_CLASH, and dl_clash_check.
 
 A linker atom of chain[0] clashes with a pocket atom when 100 |x_i - x_j| in pm is below clash[min type][max type] and that
 entry is >= 0; a molecule passes when none of its linker atoms clashes with any pocket atom. This is the project's own
@@ -181,15 +181,16 @@ def test_models_pass_require_clash_free_to_the_edm():
     assert seen == [True, 'unset', False, True, 'unset', True]
 
 
-def test_native_binds_the_clash_entries():
+def test_native_binds_the_clash_check_and_the_retry_entry():
     lib = _native.load_library()
-    assert "dl_set_clash_table" in _native.SYMBOLS and "dl_clash_check" in _native.SYMBOLS
+    assert "dl_sample_chain_retry" in _native.SYMBOLS and "dl_clash_check" in _native.SYMBOLS
     assert _native.CHECK_CLASH == 4
     ck = _native.DLMoleculeChecks(_native.CHECK_CLASH, 8, 1, 1, 1, 1)   # the clash check alone runs through dl_clash_check
     assert lib.dl_molecule_check(1, 4, ck, 1, 11, 1, None, 0, 0, 1, None, None) == -1
     err = lib.dl_last_error()
     assert b"require" in err and b"dl_clash_check" in err
-    assert lib.dl_set_clash_table(None, None) == -1 and b"null engine" in lib.dl_last_error()
+    assert lib.dl_sample_chain_retry(None, 0, 2, 4, 10, 1, *[None] * 10, 1, 3, 1, 1, ck, 1, None, None, None) == -1
+    assert b"null engine" in lib.dl_last_error()
     # refusals before any pointer is read
     for args, why in (((0, 4, 8, 1, 1, 11, 1, 1, 1, 1, 1, None, None), b"B and N"),
                       ((1, 8193, 8, 1, 1, 11, 1, 1, 1, 1, 1, None, None), b"8192"),
@@ -200,7 +201,7 @@ def test_native_binds_the_clash_entries():
         assert why in lib.dl_last_error() and b"dl_clash_check" in lib.dl_last_error()
 
 
-def test_header_compiles_as_c99_with_the_clash_entries(tmp_path):
+def test_header_compiles_as_c99_with_the_clash_table_in_the_checks(tmp_path):
     gcc = shutil.which("gcc")
     if gcc is None:
         pytest.skip("gcc not available")
@@ -212,12 +213,15 @@ def test_header_compiles_as_c99_with_the_clash_entries(tmp_path):
         "int main(void) {\n"
         "  uint64_t used[2]; int32_t attempts[2], flags[2], passed[2];\n"
         "  float clash[64] = {0}, xh[22] = {0}, lm[2] = {0}, ctx[2] = {0}; int8_t nm[2] = {0};\n"
-        "  dl_molecule_checks ck = {DL_CHECK_CONNECTED | DL_CHECK_CLASH, 8, clash, NULL, NULL, NULL};\n"
-        "  dl_status a = dl_sample_chain_seeded_retry_checked(NULL, DL_SAMPLER_LINKER, 2, 4, 10, 1, NULL, NULL, NULL, NULL,\n"
-        "                                                     NULL, NULL, NULL, NULL, NULL, NULL, flags, 3, used, attempts,\n"
-        "                                                     &ck, passed, NULL);\n"
+        "  dl_molecule_checks ck = {DL_CHECK_CONNECTED | DL_CHECK_CLASH, 8, clash, NULL, NULL, NULL, clash};\n"
+        "  dl_molecule_checks clash_only = {DL_CHECK_CLASH, 8, NULL, NULL, NULL, NULL, clash};\n"
+        "  dl_status a = dl_sample_chain_retry(NULL, DL_SAMPLER_LINKER, 2, 4, 10, 1, NULL, NULL, NULL, NULL, NULL, NULL,\n"
+        "                                      NULL, NULL, NULL, NULL, flags, 3, used, attempts, &ck, passed, NULL, NULL,\n"
+        "                                      NULL);\n"
         '  printf("%d|%s|", (int)a, dl_last_error());\n'
-        "  dl_status b = dl_set_clash_table(NULL, clash);\n"
+        "  dl_status b = dl_sample_chain_retry(NULL, DL_SAMPLER_LINKER, 2, 4, 10, 1, NULL, NULL, NULL, NULL, NULL, NULL,\n"
+        "                                      NULL, NULL, NULL, NULL, flags, 3, used, attempts, &clash_only, passed, NULL,\n"
+        "                                      NULL, NULL);\n"
         '  printf("%d|%s|", (int)b, dl_last_error());\n'
         "  dl_status c = dl_clash_check(2, 8193, 8, clash, xh, 11, nm, lm, ctx, 1, passed, NULL, NULL);\n"
         '  printf("%d|%s|", (int)c, dl_last_error());\n'

@@ -1,4 +1,4 @@
-"""Connectivity in the recovery rounds: `sample_chain(..., require_connected=True)`, and dl_sample_chain_seeded_retry_checked
+"""Connectivity in the recovery rounds: `sample_chain(..., require_connected=True)`, and dl_sample_chain_retry
 and dl_molecule_check with DL_CHECK_CONNECTED.
 
 A molecule is connected when the atoms of chain[0] -- without the pocket on cut-off graphs -- form one component under
@@ -126,7 +126,7 @@ def test_models_hand_the_edm_their_bond_tables():
     assert EDM(dynamics=None, in_node_nf=9, n_dims=3, noise_schedule='polynomial_2', timesteps=10, is_geom=True).is_geom
 
 
-def test_header_compiles_as_c99_with_a_connectivity_only_check(tmp_path):
+def test_header_compiles_as_c99_with_a_connectivity_only_checks_struct(tmp_path):
     """dl_molecule_check with DL_CHECK_CONNECTED alone refuses N beyond the check's limit, naming itself and the limit.
     (A null engine is refused as test_valid_resampling's header test checks.)"""
     gcc = shutil.which("gcc")
@@ -140,7 +140,7 @@ def test_header_compiles_as_c99_with_a_connectivity_only_check(tmp_path):
         "int main(void) {\n"
         "  int32_t conn[2];\n"
         "  float thr1[64] = {0};\n"
-        "  dl_molecule_checks ck = {DL_CHECK_CONNECTED, 8, thr1, NULL, NULL, NULL};\n"
+        "  dl_molecule_checks ck = {DL_CHECK_CONNECTED, 8, thr1, NULL, NULL, NULL, NULL};\n"
         "  dl_status b = dl_molecule_check(2, 9000, &ck, NULL, 11, NULL, NULL, 0, 0, conn, NULL, NULL);\n"
         '  printf("%d|%s\\n", (int)b, dl_last_error());\n'
         "  return 0;\n}\n")

@@ -1,4 +1,4 @@
-"""NaN recovery: `sample_chain(..., nan_retries=)`, dl_sample_chain_seeded_retry, dl_retry_seed and `c_sampler --retries`.
+"""NaN recovery: `sample_chain(..., nan_retries=)`, dl_sample_chain_retry, dl_retry_seed and `c_sampler --retries`.
 
 With per-molecule seeds a molecule's chain does not depend on its batch, so resampling only the molecules that diverged,
 with seeds derived from their own, is itself an exact sample: the rows that did not fail stay bit for bit what they were,
@@ -117,7 +117,7 @@ def test_recovery_refuses_what_cannot_resample_one_molecule(inpainting):
     assert edm.last_attempts is None
 
 
-def test_header_compiles_as_c99_with_the_recovery_entries(tmp_path):
+def test_header_compiles_as_c99_with_the_one_recovery_entry(tmp_path):
     gcc = shutil.which("gcc")
     if gcc is None:
         pytest.skip("gcc not available")
@@ -128,8 +128,8 @@ def test_header_compiles_as_c99_with_the_recovery_entries(tmp_path):
         '#include <stdio.h>\n#include "difflinker_b200.h"\n'
         "int main(void) {\n"
         "  uint64_t used[2]; int32_t attempts[2], flags[2];\n"
-        "  dl_status st = dl_sample_chain_seeded_retry(NULL, DL_SAMPLER_LINKER, 2, 4, 10, 1, NULL, NULL, NULL, NULL, NULL, NULL,\n"
-        "                                              NULL, NULL, NULL, NULL, flags, 3, used, attempts, NULL);\n"
+        "  dl_status st = dl_sample_chain_retry(NULL, DL_SAMPLER_LINKER, 2, 4, 10, 1, NULL, NULL, NULL, NULL, NULL, NULL,\n"
+        "                                       NULL, NULL, NULL, NULL, flags, 3, used, attempts, NULL, NULL, NULL, NULL, NULL);\n"
         '  printf("%d|%llu|%llu|%.1f|%s\\n", (int)st, (unsigned long long)dl_retry_seed(0, 1),\n'
         "         (unsigned long long)dl_retry_seed(UINT64_MAX, 0), (double)dl_last_retry_ms(NULL), dl_last_error());\n"
         "  return 0;\n}\n")

@@ -1,4 +1,4 @@
-"""Linker sizes drawn from each molecule's seed: dl_size_uniform, dl_size_draw and dl_sample_chain_seeded_retry_sized, up to
+"""Linker sizes drawn from each molecule's seed: dl_size_uniform, dl_size_draw and dl_sample_chain_retry, up to
 `ddpm.sample_chain(data, linker_sizes=...)`.
 
 The oracle restates the draw of the header in numpy: u from a splitmix64 finaliser of seed ^ TAG, then the fp64 inverse CDF
@@ -133,11 +133,11 @@ def test_every_refusal_names_the_conflicting_argument():
         create_templates_for_linker_generation(data, [3, 3, 3], n_nodes=2)
 
 
-def test_header_declares_the_draw_and_a_c99_caller_compiles(tmp_path):
+def test_header_declares_the_draw_and_a_c99_retry_caller_compiles(tmp_path):
     with open(os.path.join(ROOT, "include", "difflinker_b200.h")) as f:
         header = f.read()
     assert "typedef struct dl_size_redraw" in header
-    for name in ("dl_size_uniform", "dl_size_draw", "dl_sample_chain_seeded_retry_sized"):
+    for name in ("dl_size_uniform", "dl_size_draw", "dl_sample_chain_retry"):
         assert f"{name}(" in header and name in _native.SYMBOLS, name
     gcc = shutil.which("gcc")
     if gcc is None:
@@ -150,7 +150,7 @@ def test_header_declares_the_draw_and_a_c99_caller_compiles(tmp_path):
         "int main(void) {\n"
         "  int32_t sizes[1] = {3}, used[2];\n"
         "  dl_size_redraw rz = {1, 1, NULL, sizes, NULL, NULL};\n"
-        "  dl_status a = dl_sample_chain_seeded_retry_sized(NULL, DL_SAMPLER_LINKER, 2, 20, 10, 1, NULL, NULL, NULL, NULL,\n"
+        "  dl_status a = dl_sample_chain_retry(NULL, DL_SAMPLER_LINKER, 2, 20, 10, 1, NULL, NULL, NULL, NULL,\n"
         "      NULL, NULL, NULL, NULL, NULL, NULL, NULL, 1, NULL, NULL, NULL, NULL, &rz, used, NULL);\n"
         '  printf("%d|%s\\n", (int)a, dl_last_error());\n'
         "  dl_status b = dl_size_draw(0, 1, NULL, 1, NULL, NULL, 0, NULL, NULL);\n"

@@ -1,4 +1,4 @@
-"""Valence in the recovery rounds: `sample_chain(..., require_valid=True)`, dl_sample_chain_seeded_retry_checked and
+"""Valence in the recovery rounds: `sample_chain(..., require_valid=True)`, dl_sample_chain_retry and
 dl_molecule_check.
 
 An atom's valence is the sum of get_bond_order over its pairs with the other checked atoms of chain[0] -- without the
@@ -150,10 +150,14 @@ def test_models_pass_the_keyword_and_the_tables_to_the_edm():
     assert seen == [True, 'unset', False, True, 'unset', True]
 
 
-def test_native_binds_the_check_entries():
+def test_native_binds_the_check_entry_and_the_one_retry_entry():
     lib = _native.load_library()
-    assert "dl_sample_chain_seeded_retry_checked" in _native.SYMBOLS and "dl_molecule_check" in _native.SYMBOLS
-    for gone in ("dl_sample_chain_seeded_retry_connected", "dl_molecule_connected"):   # connectivity alone runs through them too
+    assert "dl_sample_chain_retry" in _native.SYMBOLS and "dl_molecule_check" in _native.SYMBOLS
+    argtypes = lib.dl_sample_chain_retry.argtypes
+    assert argtypes[20]._type_ is _native.DLMoleculeChecks and argtypes[22]._type_ is _native.DLSizeRedraw
+    # connectivity alone, NaN recovery alone, checks, size redraws and the clash table all run through dl_sample_chain_retry
+    for gone in ("dl_sample_chain_seeded_retry_connected", "dl_molecule_connected", "dl_sample_chain_seeded_retry",
+                 "dl_sample_chain_seeded_retry_checked", "dl_sample_chain_seeded_retry_sized", "dl_set_clash_table"):
         assert gone not in _native.SYMBOLS and not hasattr(lib, gone)
     assert lib.dl_molecule_check.argtypes[2]._type_ is _native.DLMoleculeChecks
     assert (_native.CHECK_CONNECTED, _native.CHECK_VALENCE) == (1, 2)
@@ -164,7 +168,7 @@ def test_native_binds_the_check_entries():
         assert b"require" in lib.dl_last_error()
 
 
-def test_header_compiles_as_c99_with_the_check_entries(tmp_path):
+def test_header_compiles_as_c99_with_the_checks_of_the_retry_entry(tmp_path):
     gcc = shutil.which("gcc")
     if gcc is None:
         pytest.skip("gcc not available")
@@ -175,10 +179,10 @@ def test_header_compiles_as_c99_with_the_check_entries(tmp_path):
         '#include <stdio.h>\n#include "difflinker_b200.h"\n'
         "int main(void) {\n"
         "  uint64_t used[2]; int32_t attempts[2], flags[2], passed[2];\n"
-        "  dl_molecule_checks ck = {DL_CHECK_CONNECTED | DL_CHECK_VALENCE, 8, NULL, NULL, NULL, NULL};\n"
-        "  dl_status a = dl_sample_chain_seeded_retry_checked(NULL, DL_SAMPLER_LINKER, 2, 4, 10, 1, NULL, NULL, NULL, NULL,\n"
-        "                                                     NULL, NULL, NULL, NULL, NULL, NULL, flags, 3, used, attempts,\n"
-        "                                                     &ck, passed, NULL);\n"
+        "  dl_molecule_checks ck = {DL_CHECK_CONNECTED | DL_CHECK_VALENCE, 8, NULL, NULL, NULL, NULL, NULL};\n"
+        "  dl_status a = dl_sample_chain_retry(NULL, DL_SAMPLER_LINKER, 2, 4, 10, 1, NULL, NULL, NULL, NULL, NULL, NULL,\n"
+        "                                      NULL, NULL, NULL, NULL, flags, 3, used, attempts, &ck, passed, NULL, NULL,\n"
+        "                                      NULL);\n"
         '  printf("%d|%s|", (int)a, dl_last_error());\n'
         "  dl_status b = dl_molecule_check(2, 4, &ck, NULL, 11, NULL, NULL, 0, 0, passed, NULL, NULL);\n"
         '  printf("%d|%s|", (int)b, dl_last_error());\n'
