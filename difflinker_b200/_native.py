@@ -10,7 +10,7 @@ GRAPH_TYPES = {"FC": 0, "4A": 1, "FC-4A": 2, "FC-10A-4A": 3}
 EDGE_IMPLS = {"auto": 0, "simt": 1, "wgmma": 2}
 SAMPLER_LINKER, SAMPLER_INPAINT = 0, 1
 AGGREGATIONS = {"sum": 0, "mean": 1}
-CHECK_CONNECTED, CHECK_VALENCE, CHECK_CLASH = 1, 2, 4   # DL_CHECK_*
+CHECK_CONNECTED, CHECK_VALENCE, CHECK_CLASH, CHECK_UNIQUE = 1, 2, 4, 8   # DL_CHECK_*
 COORDS_RANGE = 15.0   # EGNN hands its own coords_range=15 to every EquivariantBlock (src/egnn.py:183,209)
 
 
@@ -41,8 +41,8 @@ class DLMoleculeChecks(C.Structure):
 
     @classmethod
     def of(cls, require, tables, clash=None):
-        """The struct over `tables` = [thr1] or [thr1, thr2, thr3, max_valence] and the (T,T) `clash` table (None: none),
-        device tensors the caller keeps alive."""
+        """The struct over `tables` = [thr1], [thr1, thr2, thr3] or [thr1, thr2, thr3, max_valence] and the (T,T) `clash`
+        table (None: none), device tensors the caller keeps alive."""
         ptrs = [t.data_ptr() for t in tables] + [None] * (4 - len(tables))
         return cls(require, tables[0].shape[0], *ptrs, None if clash is None else clash.data_ptr())
 
@@ -81,6 +81,7 @@ SYMBOLS = {
     "dl_size_uniform": (C.c_double, [C.c_uint64]),
     "dl_molecule_check": (_I32, [_I32, _I32, C.POINTER(DLMoleculeChecks), _P, _I32, _P, _P, _I32, _I32, _P, _P, _P]),
     "dl_clash_check": (_I32, [_I32, _I32, _I32, _P, _P, _I32, _P, _P, _P, _I32, _P, _P, _P]),
+    "dl_molecule_hash": (_I32, [_I32, _I32, C.POINTER(DLMoleculeChecks), _P, _I32, _P, _P, _I32, _I32, _P, _P]),
     "dl_last_retry_ms": (_F, [_P]),
     "dl_set_noise_slice": (_I32, [_P, _I32, _I32]),
     "dl_set_start_step": (_I32, [_P, _I32, _F, _F]),

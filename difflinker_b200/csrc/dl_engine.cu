@@ -133,6 +133,7 @@ struct dl_engine {
   // own, so ev_t0/ev_t1 keep timing the first loop; ev_g*: one round, gather to scatter)
   Workspace ws_sub;
   HostStage sub_rows;
+  HostStage hashes;            // DL_CHECK_UNIQUE: the full batch's graph hashes, (B) uint64, grown to the largest B
   cudaEvent_t ev_r0 = nullptr, ev_r1 = nullptr, ev_g0 = nullptr, ev_g1 = nullptr;
   float retry_ms = 0.f;
   cudaStream_t loop_stream = nullptr;
@@ -780,6 +781,7 @@ dl_status dl_destroy(dl_engine* e) {
   free_workspace(e->ws);
   free_workspace(e->ws_sub);
   if (e->sub_rows.buf) cudaFree(e->sub_rows.buf);
+  if (e->hashes.buf) cudaFree(e->hashes.buf);
   if (e->wblob) cudaFree(e->wblob);
   if (e->wblob_tc) cudaFree(e->wblob_tc);
   if (e->coef_dev) cudaFree(e->coef_dev);
@@ -1174,24 +1176,28 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt) { return retry_seed(seed,
 
 namespace {
 
-static_assert(CHECK_CONNECTED == DL_CHECK_CONNECTED && CHECK_VALENCE == DL_CHECK_VALENCE && CHECK_CLASH == DL_CHECK_CLASH,
-              "kernels_retry.cuh vs header");
+static_assert(CHECK_CONNECTED == DL_CHECK_CONNECTED && CHECK_VALENCE == DL_CHECK_VALENCE && CHECK_CLASH == DL_CHECK_CLASH &&
+              CHECK_UNIQUE == DL_CHECK_UNIQUE, "kernels_retry.cuh vs header");
 
 // What is wrong with a caller's dl_molecule_checks for molecules of N rows whose h holds at most max_types type columns, or
-// null. The sampler takes every check; dl_molecule_check the bond checks only (the clash check has dl_clash_check).
-const char* checks_error(const dl_molecule_checks* ck, int N, int max_types, bool clash_allowed) {
+// null. The sampler takes every check; dl_molecule_check the bond checks only (the clash check has dl_clash_check, and
+// DL_CHECK_UNIQUE compares the molecules of one sampling call with each other, which a per-molecule check cannot).
+const char* checks_error(const dl_molecule_checks* ck, int N, int max_types, bool sampler) {
   if (!ck) return "null checks";
-  if (clash_allowed) {
-    if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE | DL_CHECK_CLASH)))
-      return "checks->require must be a non-empty OR of DL_CHECK_CONNECTED, DL_CHECK_VALENCE and DL_CHECK_CLASH";
+  if (sampler) {
+    if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE | DL_CHECK_CLASH | DL_CHECK_UNIQUE)))
+      return "checks->require must be a non-empty OR of DL_CHECK_CONNECTED, DL_CHECK_VALENCE, DL_CHECK_CLASH and "
+             "DL_CHECK_UNIQUE";
   } else if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE))) {
     return "checks->require must be DL_CHECK_CONNECTED, DL_CHECK_VALENCE or both (the clash check runs through "
-           "dl_clash_check)";
+           "dl_clash_check; DL_CHECK_UNIQUE compares the molecules of a dl_sample_chain_retry call with each other, and "
+           "dl_molecule_hash gives their hashes)";
   }
   if (ck->n_types < 1 || ck->n_types > max_types) return "checks->n_types must be in [1, the width of the atom features]";
-  if ((ck->require & (DL_CHECK_CONNECTED | DL_CHECK_VALENCE)) && !ck->thr1) return "null checks->thr1";
+  if ((ck->require & (DL_CHECK_CONNECTED | DL_CHECK_VALENCE | DL_CHECK_UNIQUE)) && !ck->thr1) return "null checks->thr1";
   if ((ck->require & DL_CHECK_VALENCE) && (!ck->thr2 || !ck->thr3 || !ck->max_valence))
     return "DL_CHECK_VALENCE needs checks->thr2, thr3 and max_valence";
+  if ((ck->require & DL_CHECK_UNIQUE) && (!ck->thr2 || !ck->thr3)) return "DL_CHECK_UNIQUE needs checks->thr2 and thr3";
   if (N > CONN_MAX_N) return "the molecule checks take N <= 8192";
   return nullptr;
 }
@@ -1264,11 +1270,27 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
   CK(cudaMemcpyAsync(seeds_used, seeds, (size_t)B * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(attempts, 0, (size_t)B * sizeof(int32_t), st));
   const int require = ck ? ck->require : 0;
+  const bool unique = (require & DL_CHECK_UNIQUE) != 0;
   std::vector<int32_t> flags(B), pass(B, require);
+  unsigned long long* hash = nullptr;                      // DL_CHECK_UNIQUE: the full batch's graph hashes
+  if (unique) {
+    StageLayout hl;
+    hl.out((size_t)B * sizeof(uint64_t));
+    if ((s = stage_inputs(e->hashes, hl, st)) != DL_OK) return s;
+    hash = reinterpret_cast<unsigned long long*>(e->hashes.buf);
+  }
   if (ck) {
     const ClashArgs cl{linker_mask, ck->clash, nullptr};   // the clash check's linker rows and table
-    CK(launch_molecule_check(require, check_args(e, *ck, chain, N, node_mask, context, passed), cl, B, st));
+    CK(launch_molecule_check(require, check_args(e, *ck, chain, N, node_mask, context, passed), cl, HashArgs{hash, 0}, B,
+                             st));
     e->launches += 1;
+    if (unique) {                                          // every row is a candidate; there are no keepers yet
+      UniqueArgs u{};
+      u.B = B; u.require = require; u.hash = hash; u.flags = nan_flags; u.passed = passed;
+      k_unique_verdict<<<(B + 255) / 256, 256, 0, st>>>(u);
+      LAUNCH_CHECK();
+      e->launches += 1;
+    }
     CK(cudaMemcpyAsync(pass.data(), passed, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   }
   CK(cudaMemcpyAsync(flags.data(), nan_flags, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1288,7 +1310,7 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
               i_ctx = sl.add(nullptr, n * C * 4, context != nullptr && C > 0), i_sd = sl.out((size_t)Bs * 8),
               i_ch = sl.out((size_t)keep_frames * n * xd * 4), i_fl = sl.out((size_t)Bs * 4),
               i_ps = sl.add(nullptr, (size_t)Bs * 4, ck != nullptr), i_tk = sl.add(nullptr, (size_t)Bs * 4, ck != nullptr),
-              i_sz = sl.add(nullptr, (size_t)Bs * 4, rz != nullptr);
+              i_sz = sl.add(nullptr, (size_t)Bs * 4, rz != nullptr), i_sh = sl.add(nullptr, (size_t)Bs * 8, unique);
     if ((s = stage_inputs(e->sub_rows, sl, st)) != DL_OK) return s;   // the row list goes to the device once per round
     CK(cudaEventRecord(e->ev_g0, st));
     RowGatherArgs ga{};
@@ -1324,7 +1346,8 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     if (ck) {
       CheckArgs ca = check_args(e, *ck, sa.s_chain, N, ga.s_node_mask, ga.s_context, sl.at<int32_t>(i_ps));
       ca.rows = ga.rows; ca.flags = nan_flags; ca.s_flags = sa.s_flags; ca.take = sl.at<int32_t>(i_tk);
-      CK(launch_molecule_check(require, ca, ClashArgs{ga.s_linker_mask, ck->clash, nullptr}, Bs, st));
+      const HashArgs ha{sl.at<unsigned long long>(i_sh), 0};
+      CK(launch_molecule_check(require, ca, ClashArgs{ga.s_linker_mask, ck->clash, nullptr}, ha, Bs, st));
       e->launches += 1;
       sa.take = ca.take; sa.s_passed = ca.passed; sa.passed = passed;
       if (rz) k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa, za);
@@ -1336,6 +1359,14 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     }
     LAUNCH_CHECK();
     e->launches += 1;
+    if (unique) {                                          // the round's rows against the keepers and each other
+      UniqueArgs u{};
+      u.B = B; u.Bs = Bs; u.require = require; u.hash = hash; u.flags = nan_flags; u.passed = passed;
+      u.rows = ga.rows; u.take = sa.take; u.s_hash = sl.at<unsigned long long>(i_sh);
+      k_unique_verdict<<<(Bs + 255) / 256, 256, 0, st>>>(u);
+      LAUNCH_CHECK();
+      e->launches += 1;
+    }
     CK(cudaEventRecord(e->ev_g1, st));
     std::vector<int32_t> sub_flags(Bs), sub_pass(Bs, require), take(Bs, 1);
     CK(cudaMemcpyAsync(sub_flags.data(), sa.s_flags, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1343,12 +1374,14 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
       CK(cudaMemcpyAsync(sub_pass.data(), sa.s_passed, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
       CK(cudaMemcpyAsync(take.data(), sa.take, (size_t)Bs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     }
+    // the verdict may change the bit of rows that were not taken too: read every row's verdict
+    if (unique) CK(cudaMemcpyAsync(pass.data(), passed, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, e->ev_g0, e->ev_g1));
     e->retry_ms += ms;
     for (int i = 0; i < Bs; ++i)
-      if (take[i]) { flags[rows[i]] = sub_flags[i]; pass[rows[i]] = sub_pass[i]; }
+      if (take[i]) { flags[rows[i]] = sub_flags[i]; if (!unique) pass[rows[i]] = sub_pass[i]; }
   }
   for (int b = 0; b < B; ++b) if (flags[b] != 0) return DL_NAN_DETECTED;
   return DL_OK;
@@ -1413,7 +1446,24 @@ dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* chec
   CheckArgs ca = check_args(*checks, xh, N, xh_row_stride, node_mask, context, context_nf, drop_pocket != 0, passed);
   ca.valence = valence;
   if (valence) CK(cudaMemsetAsync(valence, 0, (size_t)B * N * sizeof(int32_t), st));   // the rows that are not checked
-  CK(launch_molecule_check(checks->require, ca, ClashArgs{}, B, st));
+  CK(launch_molecule_check(checks->require, ca, ClashArgs{}, HashArgs{}, B, st));
+  return DL_OK;
+}
+
+dl_status dl_molecule_hash(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
+                           const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
+                           uint64_t* hash, void* stream) {
+  const char* why = nullptr;
+  if (!checks) why = "null checks";
+  else if (B <= 0 || N <= 0) why = "B and N must be >= 1";
+  else if (N > CONN_MAX_N) why = "the molecule checks take N <= 8192";
+  else if (checks->n_types < 1 || checks->n_types > xh_row_stride - 3) why = "checks->n_types must be in [1, xh_row_stride - 3]";
+  else if (!checks->thr1 || !checks->thr2 || !checks->thr3) why = "the hash needs checks->thr1, thr2 and thr3";
+  else if (!xh || !node_mask || !hash || (drop_pocket && (!context || context_nf < 1))) why = "invalid argument";
+  if (why) { set_err("dl_molecule_hash: %s", why); return DL_ERR_INVALID; }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const CheckArgs ca = check_args(*checks, xh, N, xh_row_stride, node_mask, context, context_nf, drop_pocket != 0, nullptr);
+  CK(launch_molecule_check(CHECK_UNIQUE, ca, ClashArgs{}, HashArgs{reinterpret_cast<unsigned long long*>(hash), 0}, B, st));
   return DL_OK;
 }
 
@@ -1432,7 +1482,7 @@ dl_status dl_clash_check(int32_t B, int32_t N, int32_t n_types, const float* cla
   ca.xh = xh; ca.N = N; ca.row_stride = xh_row_stride; ca.n_types = n_types;
   ca.node_mask = node_mask; ca.C = context_nf; ca.context = context; ca.drop_pocket = 1; ca.passed = passed;
   if (clashes) CK(cudaMemsetAsync(clashes, 0, (size_t)B * N * sizeof(int32_t), st));   // the rows that are not linker atoms
-  CK(launch_molecule_check(CHECK_CLASH, ca, ClashArgs{linker_mask, clash, clashes}, B, st));
+  CK(launch_molecule_check(CHECK_CLASH, ca, ClashArgs{linker_mask, clash, clashes}, HashArgs{}, B, st));
   return DL_OK;
 }
 

@@ -3,6 +3,8 @@
 #pragma once
 #include <stdint.h>
 
+#include <algorithm>
+
 #include "bonds.cuh"
 
 namespace dl {
@@ -222,9 +224,31 @@ __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a, RowSizeA
 // CHECK_CLASH (always with drop_pocket): the linker atoms are the checked atoms with linker_mask != 0, the pocket atoms the
 // rows with node_mask != 0 and context column C - 1 != 0; the bit is set iff no linker atom clashes (clash_pair) with any
 // pocket atom (no linker or no pocket atom: set). The predicates are stated in full at dl_molecule_checks in the header.
-constexpr int CHECK_CONNECTED = 1, CHECK_VALENCE = 2, CHECK_CLASH = 4;   // DL_CHECK_* of the header
+// CHECK_UNIQUE: the kernel writes each molecule's graph hash (stated at DL_CHECK_UNIQUE in the header) and leaves the bit
+// clear; k_unique_verdict sets it, since it compares molecules with each other.
+constexpr int CHECK_CONNECTED = 1, CHECK_VALENCE = 2, CHECK_CLASH = 4, CHECK_UNIQUE = 8;   // DL_CHECK_* of the header
 constexpr int CONN_MAX_N = 8192;                                     // rows per molecule: 20 bytes of shared memory each
 constexpr int CONN_SMEM_MAX = CONN_MAX_N * (int)(sizeof(float4) + sizeof(int));
+// With CHECK_UNIQUE a molecule also takes 8 bytes per row (the atoms' rows and the CSR offsets) and 4 bytes per stored
+// directed bond: up to HASH_EDGES_PER_ROW per row, within the opt-in shared memory of a block on sm_90 (227 KB, less the
+// kernel's static shared memory).
+constexpr int HASH_SMEM_MAX = 226 * 1024;
+constexpr int HASH_EDGES_PER_ROW = 16;
+constexpr unsigned long long GRAPH_HASH_TAG = 0x67726170682D776Cull;   // "graph-wl" in ASCII
+constexpr unsigned long long GRAPH_HASH_ORDER = 0x9E3779B97F4A7C15ull;
+
+// mix() of the graph hash: the splitmix64 finaliser of size_uniform.
+__host__ __device__ inline unsigned long long hash_mix(unsigned long long z) {
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+// What CHECK_UNIQUE writes besides CheckArgs, a kernel parameter of the instantiations with the bit only.
+struct HashArgs {
+  unsigned long long* hash;              // (B) out: every molecule's graph hash
+  int edge_cap;                          // directed bonds the shared-memory CSR holds (set by launch_molecule_check_as)
+};
 
 struct CheckArgs {
   const float* xh;                       // (B, N, row_stride): x at columns 0..2, h from column 3 -- chain[0]
@@ -253,6 +277,128 @@ struct ClashArgs {
                                          // rows are not written)
 };
 
+// Row r of the molecule at g0 as the staging below makes its atom: x, y, z and the type (the first argmax, NaN winning) as
+// int bits. The graph hash reads the atoms whose bonds do not fit its shared-memory CSR this way.
+__device__ __forceinline__ float4 load_atom(const CheckArgs& a, size_t g0, int r) {
+  const float* row = a.xh + (g0 + r) * a.row_stride;
+  int best = 0;
+  for (int k = 1; k < a.n_types; ++k) {
+    const float v = row[3 + k], cur = row[3 + best];
+    if (v > cur || (isnan(v) && !isnan(cur))) best = k;
+  }
+  return make_float4(row[0], row[1], row[2], __int_as_float(best));
+}
+
+// The graph hash of the n staged atoms s_at[0, n) (rows s_row), stated at DL_CHECK_UNIQUE in the header: R = min(n, 64)
+// rounds of colour refinement c' (i) = mix(c(i) + sum over bonded j of mix(c(j) + o_ij * GRAPH_HASH_ORDER)), then
+// H = mix(n + sum_i c(i)). Block-collective; returns H on every thread.
+// The bonds are found once: a warp per atom counts them (all pairs, bond_pair), the counts are scanned into CSR offsets in
+// s_off, and a warp per atom writes its neighbours j | order << 16 in ascending j into s_edge. Atoms whose list would end
+// beyond edge_cap (a prefix of the atoms is stored, since the offsets ascend) rescan every atom in every round, reading the
+// rows from global memory (load_atom). The colours then live over s_at, two arrays of N, and the rounds add integers only:
+// the hash does not depend on the order the lanes add in.
+__device__ __forceinline__ unsigned long long graph_hash(const CheckArgs& a, const HashArgs& hk, size_t g0, int n,
+                                                        float4* s_at, int* s_off, const int* s_row, unsigned* s_edge) {
+  __shared__ int s_wsum[8], s_e;
+  __shared__ unsigned long long s_hsum[8];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int i = warp; i < n; i += 8) {                 // degrees
+    const float4 pi = s_at[i];
+    int d = 0;
+    for (int j = lane; j < n; j += 32) {
+      const float4 pj = s_at[j];
+      float dist;
+      d += j != i && bond_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
+                               __float_as_int(pj.w), a.n_types, a.thr1, &dist) >= 0;
+    }
+    for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+    if (lane == 0) s_off[i] = d;
+  }
+  if (tid == 0) s_e = 0;
+  __syncthreads();
+  for (int i0 = 0; i0 < n; i0 += 256) {               // exclusive scan of the degrees, 256 atoms at a time
+    const int i = i0 + tid;
+    const int v = i < n ? s_off[i] : 0;
+    int x = v;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, x, o);
+      if (lane >= o) x += y;
+    }
+    if (lane == 31) s_wsum[warp] = x;
+    __syncthreads();
+    int before = s_e, total = 0;
+    for (int w = 0; w < 8; ++w) { before += w < warp ? s_wsum[w] : 0; total += s_wsum[w]; }
+    if (i < n) s_off[i] = before + x - v;
+    __syncthreads();
+    if (tid == 0) s_e += total;
+    __syncthreads();
+  }
+  const int E = s_e;
+  auto end_of = [&](int i) { return i + 1 < n ? s_off[i + 1] : E; };
+  for (int i = warp; i < n; i += 8) {                 // the stored lists
+    const int start = s_off[i];
+    if (end_of(i) > hk.edge_cap) continue;
+    const float4 pi = s_at[i];
+    int at = start;
+    for (int j0 = 0; j0 < n; j0 += 32) {
+      const int j = j0 + lane;
+      int o = 0;
+      if (j < n && j != i) {
+        const float4 pj = s_at[j];
+        o = bond_order_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
+                            __float_as_int(pj.w), a.n_types, a.thr1, a.thr2, a.thr3);
+      }
+      const unsigned m = __ballot_sync(0xffffffffu, o > 0);
+      if (o > 0) s_edge[at + __popc(m & ((1u << lane) - 1u))] = (unsigned)j | ((unsigned)o << 16);
+      at += __popc(m);
+    }
+  }
+  __syncthreads();
+  unsigned long long* c = reinterpret_cast<unsigned long long*>(s_at);   // [N]: this round's colours
+  unsigned long long* c2 = c + a.N;                                        // [N]: the next round's
+  for (int i0 = 0; i0 < n; i0 += 256) {               // c_0, over the atoms of this chunk and the ones before it only
+    const int i = i0 + tid;
+    const int t = i < n ? __float_as_int(s_at[i].w) : 0;
+    __syncthreads();
+    if (i < n) c[i] = hash_mix(GRAPH_HASH_TAG ^ (unsigned long long)(t + 1));
+  }
+  __syncthreads();
+  const int R = min(n, 64);
+  for (int k = 0; k < R; ++k) {
+    for (int i = warp; i < n; i += 8) {
+      unsigned long long s = 0;
+      const int start = s_off[i], end = end_of(i);
+      if (end <= hk.edge_cap) {
+        for (int e = start + lane; e < end; e += 32) {
+          const unsigned v = s_edge[e];
+          s += hash_mix(c[v & 0xffffu] + (unsigned long long)(v >> 16) * GRAPH_HASH_ORDER);
+        }
+      } else {
+        const float4 pi = load_atom(a, g0, s_row[i]);
+        for (int j = lane; j < n; j += 32) {
+          if (j == i) continue;
+          const float4 pj = load_atom(a, g0, s_row[j]);
+          const int o = bond_order_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
+                                        __float_as_int(pj.w), a.n_types, a.thr1, a.thr2, a.thr3);
+          if (o > 0) s += hash_mix(c[j] + (unsigned long long)o * GRAPH_HASH_ORDER);
+        }
+      }
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      if (lane == 0) c2[i] = hash_mix(c[i] + s);
+    }
+    __syncthreads();
+    unsigned long long* t = c; c = c2; c2 = t;
+  }
+  unsigned long long s = 0;
+  for (int i = tid; i < n; i += 256) s += c[i];
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) s_hsum[warp] = s;
+  __syncthreads();
+  s = (unsigned long long)n;
+  for (int w = 0; w < 8; ++w) s += s_hsum[w];
+  return hash_mix(s);
+}
+
 // One CTA per molecule. The checked atoms are compacted, in row order, into shared memory (coordinates and type; padded
 // and pocket rows are never read beyond their masks).
 // Valence: a warp per atom sums the integer bond orders of its pairs with every other atom, so the sums do not depend on
@@ -265,11 +411,14 @@ struct ClashArgs {
 // pocket atoms are disjoint rows, so the two never meet), and s_lab[i] holds atom i's row with bit 31 set for a linker
 // atom until the clash pass is done. A warp per linker atom counts, in integers, the pocket atoms it clashes with; the
 // count and the verdict do not depend on the order the lanes add in.
-// The body of both k_molecule_check kernels below; cl is read with CHECK_CLASH only.
+// Hash (CHECK_UNIQUE): s_row[i] keeps atom i's row, and after the other checks graph_hash takes over the buffer: s_lab
+// holds the CSR offsets, the bonds follow s_row, and the colours overwrite s_at.
+// The body of the k_molecule_check kernels below; cl is read with CHECK_CLASH only, hk with CHECK_UNIQUE only.
 template <int CHECKS>
-__device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashArgs& cl) {
+__device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashArgs& cl, const HashArgs& hk) {
   extern __shared__ float4 s_at[];                    // [n]: x, y, z, type (int bits)
   int* s_lab = reinterpret_cast<int*>(s_at + a.N);    // [n]: the atoms' rows (valence), then parent pointers (components)
+  int* s_row = s_lab + a.N;                           // [n] (CHECK_UNIQUE): the atoms' rows
   __shared__ int s_warp[8], s_n, s_changed;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = blockIdx.x;
@@ -304,6 +453,7 @@ __device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashAr
         if (ok) {
           s_at[off] = at;
           s_lab[off] = r | (linker ? (int)0x80000000u : 0);
+          if (CHECKS & CHECK_UNIQUE) s_row[off] = r;
         } else {
           s_at[a.N - 1 - poff] = at;
         }
@@ -334,6 +484,7 @@ __device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashAr
         }
         s_at[off] = make_float4(row[0], row[1], row[2], __int_as_float(best));
         s_lab[off] = (CHECKS & CHECK_VALENCE) ? r : off;
+        if (CHECKS & CHECK_UNIQUE) s_row[off] = r;
       }
       __syncthreads();
       if (tid == 0) s_n += total;
@@ -425,31 +576,56 @@ __device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashAr
     for (int i0 = 0; i0 < n; i0 += 256) roots += __syncthreads_count(i0 + tid < n && lab[i0 + tid] == i0 + tid);
     if (roots == 1) verdict |= CHECK_CONNECTED;
   }
+  if constexpr ((CHECKS & CHECK_UNIQUE) != 0) {
+    __syncthreads();                                  // s_lab is read above until here
+    const unsigned long long h = graph_hash(a, hk, g0, n, s_at, s_lab, s_row, reinterpret_cast<unsigned*>(s_row + a.N));
+    if (tid == 0) hk.hash[b] = h;
+  }
   if (tid == 0) {
-    a.passed[b] = verdict;
+    if (!(CHECKS & CHECK_UNIQUE) || a.passed) a.passed[b] = verdict;   // dl_molecule_hash has no verdicts
     if (a.rows) a.take[b] = !(a.flags[a.rows[b]] == 0 && a.s_flags[b] != 0);
   }
 }
 
-// The instantiations without the clash bit, and with it.
+// The instantiations without the clash and hash bits, with the clash bit, and with the hash bit.
 template <int CHECKS>
 __global__ void __launch_bounds__(256) k_molecule_check(CheckArgs a) {
-  static_assert((CHECKS & CHECK_CLASH) == 0, "the clash check takes ClashArgs");
-  molecule_check<CHECKS>(a, ClashArgs{});
+  static_assert((CHECKS & (CHECK_CLASH | CHECK_UNIQUE)) == 0, "the clash check takes ClashArgs, the hash HashArgs");
+  molecule_check<CHECKS>(a, ClashArgs{}, HashArgs{});
 }
 
 // (With __launch_bounds__(256) alone ptxas fits <6> into 32 registers and spills; a minimum of one CTA per SM lets it take
 // the 38-39 it needs.)
 template <int CHECKS>
 __global__ void __launch_bounds__(256, 1) k_molecule_check(CheckArgs a, ClashArgs k) {
-  static_assert((CHECKS & CHECK_CLASH) != 0, "only the clash check takes ClashArgs");
-  molecule_check<CHECKS>(a, k);
+  static_assert((CHECKS & CHECK_CLASH) != 0 && (CHECKS & CHECK_UNIQUE) == 0, "only the clash check takes ClashArgs alone");
+  molecule_check<CHECKS>(a, k, HashArgs{});
 }
 
 template <int CHECKS>
-cudaError_t launch_molecule_check_as(const CheckArgs& a, const ClashArgs& k, int B, cudaStream_t st) {
+__global__ void __launch_bounds__(256, 1) k_molecule_check(CheckArgs a, ClashArgs k, HashArgs h) {
+  static_assert((CHECKS & CHECK_UNIQUE) != 0, "only the hash takes HashArgs");
+  molecule_check<CHECKS>(a, k, h);
+}
+
+template <int CHECKS>
+cudaError_t launch_molecule_check_as(const CheckArgs& a, const ClashArgs& k, const HashArgs& h, int B, cudaStream_t st) {
   const size_t smem = (size_t)a.N * (sizeof(float4) + sizeof(int));
-  if constexpr ((CHECKS & CHECK_CLASH) != 0) {
+  if constexpr ((CHECKS & CHECK_UNIQUE) != 0) {
+    // 8 more bytes per row, then the bonds: HASH_EDGES_PER_ROW per row or what HASH_SMEM_MAX leaves (512 at N = 8192;
+    // graph_hash rescans the atoms whose bonds do not fit)
+    const size_t base = smem + (size_t)a.N * 2 * sizeof(int);
+    const size_t cap = std::min((size_t)a.N * HASH_EDGES_PER_ROW, (HASH_SMEM_MAX - base) / sizeof(unsigned));
+    void (*kernel)(CheckArgs, ClashArgs, HashArgs) = k_molecule_check<CHECKS>;
+    const size_t total = base + cap * sizeof(unsigned);
+    if (total > 48 * 1024) {
+      const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HASH_SMEM_MAX);
+      if (err != cudaSuccess) return err;
+    }
+    HashArgs hh = h;
+    hh.edge_cap = (int)cap;
+    kernel<<<B, 256, total, st>>>(a, k, hh);
+  } else if constexpr ((CHECKS & CHECK_CLASH) != 0) {
     void (*kernel)(CheckArgs, ClashArgs) = k_molecule_check<CHECKS>;
     if (smem > 48 * 1024) {
       const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CONN_SMEM_MAX);
@@ -470,18 +646,69 @@ cudaError_t launch_molecule_check_as(const CheckArgs& a, const ClashArgs& k, int
 // Launches k_molecule_check<checks> over B molecules; checks is a non-empty OR of CHECK_*, N <= CONN_MAX_N.
 // The shared-memory limit is raised to its one maximum the first time a molecule needs more than the default, so
 // concurrent callers never lower it under each other.
-inline cudaError_t launch_molecule_check(int checks, const CheckArgs& a, const ClashArgs& k, int B, cudaStream_t st) {
-  constexpr int CV = CHECK_CONNECTED | CHECK_VALENCE;
+// CHECK_UNIQUE writes the hashes to h.hash.
+inline cudaError_t launch_molecule_check(int checks, const CheckArgs& a, const ClashArgs& k, const HashArgs& h, int B,
+                                         cudaStream_t st) {
+  constexpr int CV = CHECK_CONNECTED | CHECK_VALENCE, U = CHECK_UNIQUE;
   switch (checks) {
-    case CHECK_CONNECTED: return launch_molecule_check_as<CHECK_CONNECTED>(a, k, B, st);
-    case CHECK_VALENCE: return launch_molecule_check_as<CHECK_VALENCE>(a, k, B, st);
-    case CHECK_CONNECTED | CHECK_VALENCE: return launch_molecule_check_as<CHECK_CONNECTED | CHECK_VALENCE>(a, k, B, st);
-    case CHECK_CLASH: return launch_molecule_check_as<CHECK_CLASH>(a, k, B, st);
-    case CHECK_CLASH | CHECK_CONNECTED: return launch_molecule_check_as<CHECK_CLASH | CHECK_CONNECTED>(a, k, B, st);
-    case CHECK_CLASH | CHECK_VALENCE: return launch_molecule_check_as<CHECK_CLASH | CHECK_VALENCE>(a, k, B, st);
-    case CHECK_CLASH | CV: return launch_molecule_check_as<CHECK_CLASH | CV>(a, k, B, st);
+    case CHECK_CONNECTED: return launch_molecule_check_as<CHECK_CONNECTED>(a, k, h, B, st);
+    case CHECK_VALENCE: return launch_molecule_check_as<CHECK_VALENCE>(a, k, h, B, st);
+    case CHECK_CONNECTED | CHECK_VALENCE: return launch_molecule_check_as<CHECK_CONNECTED | CHECK_VALENCE>(a, k, h, B, st);
+    case CHECK_CLASH: return launch_molecule_check_as<CHECK_CLASH>(a, k, h, B, st);
+    case CHECK_CLASH | CHECK_CONNECTED: return launch_molecule_check_as<CHECK_CLASH | CHECK_CONNECTED>(a, k, h, B, st);
+    case CHECK_CLASH | CHECK_VALENCE: return launch_molecule_check_as<CHECK_CLASH | CHECK_VALENCE>(a, k, h, B, st);
+    case CHECK_CLASH | CV: return launch_molecule_check_as<CHECK_CLASH | CV>(a, k, h, B, st);
+    case U: return launch_molecule_check_as<U>(a, k, h, B, st);
+    case U | CHECK_CONNECTED: return launch_molecule_check_as<U | CHECK_CONNECTED>(a, k, h, B, st);
+    case U | CHECK_VALENCE: return launch_molecule_check_as<U | CHECK_VALENCE>(a, k, h, B, st);
+    case U | CV: return launch_molecule_check_as<U | CV>(a, k, h, B, st);
+    case U | CHECK_CLASH: return launch_molecule_check_as<U | CHECK_CLASH>(a, k, h, B, st);
+    case U | CHECK_CLASH | CHECK_CONNECTED: return launch_molecule_check_as<U | CHECK_CLASH | CHECK_CONNECTED>(a, k, h, B, st);
+    case U | CHECK_CLASH | CHECK_VALENCE: return launch_molecule_check_as<U | CHECK_CLASH | CHECK_VALENCE>(a, k, h, B, st);
+    case U | CHECK_CLASH | CV: return launch_molecule_check_as<U | CHECK_CLASH | CV>(a, k, h, B, st);
     default: return cudaErrorInvalidValue;
   }
+}
+
+// The uniqueness verdict over a batch of B molecules whose graph hashes are hash[b] (stated at DL_CHECK_UNIQUE in the
+// header). Candidates: every row (rows == null: the first loop), or the Bs rows rows[i] (ascending) of a recovery round,
+// whose hash is then s_hash[i] where take[i] is set and hash[rows[i]] where it is not. Keepers: the rows that are not
+// candidates and pass every bit of `require`. Eligible: a candidate with flags == 0 and every other bit of `require`.
+struct UniqueArgs {
+  int B, Bs, require;
+  unsigned long long* hash;              // (B); a round writes s_hash[i] to hash[rows[i]] where take[i] is set
+  const int32_t* flags;                  // (B)
+  int32_t* passed;                       // (B): DL_CHECK_UNIQUE set or cleared on the candidates
+  const int* rows;
+  const int32_t* take;
+  const unsigned long long* s_hash;      // (Bs)
+};
+
+// A thread per candidate: the bit iff its hash equals no keeper's and no eligible earlier candidate's. Each thread writes
+// only its own row's bit and hash; the bits and hashes other threads read are not among them (a keeper is never written,
+// and a candidate's other bits and its hash are read from where they do not change), so the verdict does not depend on
+// the order the threads run in.
+__global__ void __launch_bounds__(256) k_unique_verdict(UniqueArgs u) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int nc = u.rows ? u.Bs : u.B;
+  if (i >= nc) return;
+  const int other = u.require & ~CHECK_UNIQUE;
+  auto row = [&](int k) { return u.rows ? u.rows[k] : k; };
+  auto hash_of = [&](int k) { return u.rows && u.take[k] ? u.s_hash[k] : u.hash[row(k)]; };
+  const int b = row(i);
+  const unsigned long long h = hash_of(i);
+  bool dup = false;
+  if (u.rows)
+    for (int k = 0, p = 0; k < u.B && !dup; ++k) {   // keepers: the rows between the candidates
+      if (p < u.Bs && u.rows[p] == k) { ++p; continue; }
+      dup = u.flags[k] == 0 && (u.passed[k] & u.require) == u.require && u.hash[k] == h;
+    }
+  for (int k = 0; k < i && !dup; ++k) {
+    const int bk = row(k);
+    dup = u.flags[bk] == 0 && (u.passed[bk] & other) == other && hash_of(k) == h;
+  }
+  u.passed[b] = dup ? (u.passed[b] & ~CHECK_UNIQUE) : (u.passed[b] | CHECK_UNIQUE);
+  if (u.rows && u.take[i]) u.hash[b] = u.s_hash[i];
 }
 
 }  // namespace dl

@@ -190,7 +190,7 @@ def _check_start(sample_fn, start_step):
 
 
 def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                 start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None):
+                 start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
@@ -199,6 +199,7 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     `require_valid`: ... and the molecules with an atom beyond its valence (None uses `model.edm.require_valid`).
     `require_clash_free`: ... and, on pocket graphs, the molecules whose linker clashes with the pocket (None uses
     `model.edm.require_clash_free`).
+    `require_unique`: ... and the molecules whose bond graph repeats a batch-mate's (None uses `model.edm.require_unique`).
     `start_step` = t0 (partial diffusion, EDM.sample_chain): the template of sample_fn=None with the batch's own linker
     positions and atom types on its linker rows, sampled from step t0; ValueError with a sample_fn, or when the batch's
     linker rows do not directly follow its fragment rows.
@@ -227,6 +228,8 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['require_valid'] = require_valid
     if require_clash_free is not None:
         extra['require_clash_free'] = require_clash_free
+    if require_unique is not None:
+        extra['require_unique'] = require_unique
     if start_step is not None:
         extra['start_step'] = start_step
     chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **extra)
@@ -323,10 +326,10 @@ class DDPM(nn.Module):
         self.edm.devices = devices          # EDM.devices: split each sampling batch over these CUDA devices
 
     def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                     start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None):
+                     start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                             require_connected=require_connected, start_step=start_step, require_valid=require_valid,
-                            require_clash_free=require_clash_free, linker_sizes=linker_sizes)
+                            require_clash_free=require_clash_free, linker_sizes=linker_sizes, require_unique=require_unique)
 
     def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None):

@@ -18,7 +18,7 @@ import torch.nn.functional as F
 from . import _native
 from .distributed import (deal_launches, device_slices, pack_requests, place_rows, plan_launches, resolve_devices,
                           slice_sampler_inputs, unpack_rows)
-from .molecule_builder import check_tables, clash_table
+from .molecule_builder import check_tables, clash_table, graph_hashes
 from .noise import PredefinedNoiseSchedule
 from .utils import FoundNaNException, nan_exception_class
 
@@ -218,6 +218,12 @@ class EDM(torch.nn.Module):
         # nothing.
         self.require_clash_free = False
         self.last_clash_free = None            # calls with require_clash_free: the (B,) CPU bool clash verdict of every row
+        # Uniqueness: likewise for the molecules whose bond graph repeats a batch-mate's (molecule_builder.graph_hashes), in
+        # the same check launch and a verdict over the call's rows. Same needs, and one slice; False, the default, checks
+        # nothing.
+        self.require_unique = False
+        self.last_unique = None                # calls with require_unique: the (B,) CPU bool uniqueness verdict of every row
+        self.last_graph_hashes = None          # calls with require_unique: the (B,) CPU int64 graph hash of every row
         self.last_sizes = None                 # calls with linker_sizes: the (B,) CPU int32 linker size of every returned row
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
@@ -494,13 +500,16 @@ class EDM(torch.nn.Module):
             raise ValueError(f"{name} needs CUDA inputs (got {x.device})")
         return True
 
-    def _checks(self, require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free=None):
+    def _checks(self, require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free=None,
+                require_unique=None):
         """The molecule checks of a call as the OR of _native.CHECK_*; 0 checks nothing."""
         return ((_native.CHECK_CONNECTED if self._require_check('require_connected', require_connected, seeds, noise,
                                                                 batch_slice, x) else 0) |
                 (_native.CHECK_VALENCE if self._require_check('require_valid', require_valid, seeds, noise, batch_slice, x)
                  else 0) |
-                (_native.CHECK_CLASH if self._require_clash_free(require_clash_free, seeds, noise, batch_slice, x) else 0))
+                (_native.CHECK_CLASH if self._require_clash_free(require_clash_free, seeds, noise, batch_slice, x) else 0) |
+                (_native.CHECK_UNIQUE if self._require_check('require_unique', require_unique, seeds, noise, batch_slice, x)
+                 else 0))
 
     def _require_clash_free(self, value, seeds, noise, batch_slice, x):
         """_require_check for require_clash_free, which also needs a pocket that stays put: a cut-off (pocket) graph and the
@@ -567,7 +576,7 @@ class EDM(torch.nn.Module):
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
-                     require_valid=None, require_clash_free=None, linker_sizes=None):
+                     require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -614,6 +623,18 @@ class EDM(torch.nn.Module):
         molecule_builder.clash_table(is_geom) allows for the two atom types (this project's own predicate, stated at
         dl_molecule_checks in the header; fragment atoms are not checked). `last_clash_free` (B,) CPU bool tells which rows
         pass. Refusals as for require_valid, plus ValueError on FC graphs and for InpaintingEDM.
+        `require_unique` (None: the `require_unique` attribute, default False) adds a fifth, in the same rounds and launch:
+        the row's bond graph -- chain[0]'s checked atoms, types and get_bond_order orders -- repeats a batch-mate's, by the
+        graph hash of molecule_builder.graph_hashes. After the loop every row is a candidate; in a round, the rows it
+        resampled are. A candidate keeps the bit unless its hash equals that of a row outside the candidates that passes
+        every required check, or of an earlier candidate that is finite and passes every other required check. Rows that
+        pass are never resampled, and no two returned rows that pass every required check share a hash (a row failing
+        another check blocks no one, so two such rows may keep the bit with one hash). The group is this call: uniqueness
+        across calls is the caller's, with `last_graph_hashes` (B,) CPU int64 (one dl_molecule_hash of the returned
+        chain[0]). `last_unique` (B,) CPU bool tells which rows pass. Equal hashes mean isomorphic graphs up to the hash's
+        limits (1-WL-equivalent graphs and 64-bit collisions hash equal; stereochemistry is ignored; not verified against
+        RDKit canonical SMILES). Refusals as for require_valid, plus ValueError when `devices` splits the batch into more
+        than one slice: the slices recover on their engines independently, so no verdict sees the whole batch.
         `linker_sizes` (a LinkerSizes; ddpm.sample_chain builds it) makes every round redraw the linker size of the rows it
         resamples, from the round's seed (dl_sample_chain_retry's redraw), and rebuild their template rows at that size
         inside the padded template. The inputs must be the template of the sizes dl_size_draw gives `seeds` at attempt 0,
@@ -632,10 +653,12 @@ class EDM(torch.nn.Module):
         dev = x.device
         self.last_attempts = None
         self.last_connected = self.last_valid = self.last_clash_free = self.last_sizes = None
+        self.last_unique = self.last_graph_hashes = None
         start = self._start(start_step, n_samples)
         redraw = self._linker_sizes(linker_sizes, seeds, noise, batch_slice, start_step, x, linker_mask)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
-        check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free)
+        check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free,
+                             require_unique)
         recover = retries > 0 or check != 0 # the recovery entry point: seeds used and attempts come back
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
         full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
@@ -648,6 +671,10 @@ class EDM(torch.nn.Module):
         slices = device_slices(n_samples, self.devices) if split else [(self.dynamics._device_index(x), 0, 0, n_samples)]
         if not slices:
             raise ValueError("sample_chain needs at least one molecule")
+        if check & _native.CHECK_UNIQUE and len(slices) > 1:
+            raise ValueError(f"require_unique compares the rows of one engine call, but devices={self.devices!r} splits the "
+                             f"batch into {len(slices)} slices that recover independently; sample on one device, or "
+                             "deduplicate the slices with last_graph_hashes / molecule_builder.graph_hashes")
         if on_device:
             gen = _generator_of(dev)
             # the device-side stream reproduces torch's randn launch geometry, which depends on the device's SM count
@@ -701,12 +728,27 @@ class EDM(torch.nn.Module):
             self.last_valid = (out['passed'].cpu() & _native.CHECK_VALENCE) != 0
         if check & _native.CHECK_CLASH:
             self.last_clash_free = (out['passed'].cpu() & _native.CHECK_CLASH) != 0
+        if check & _native.CHECK_UNIQUE:
+            self.last_unique = (out['passed'].cpu() & _native.CHECK_UNIQUE) != 0
+            self.last_graph_hashes = self._graph_hashes(full, out['chain'][0], redraw, out['sizes']).cpu()
         if out['bad']:
             exc = self._nan_exception(out['flags'], start)
             if recover:
                 exc.chain = out['chain']    # the rows that did not fail, or were recovered, are good molecules
             raise exc
         return out['chain']
+
+    def _graph_hashes(self, full, chain0, redraw, sizes):
+        """graph_hashes of a returned chain[0] over the atoms the engine checked: the node mask of the inputs `full` or,
+        with a size redraw, of every row's template at its returned size (rows below n_frag as given, then `sizes` linker
+        rows); without the pocket on cut-off graphs."""
+        nm = full['node_mask']
+        if redraw is not None:
+            n_frag = redraw[2].to(torch.int64)[:, None]
+            rows = torch.arange(nm.shape[1], device=nm.device)[None, :]
+            nm = torch.where(rows < n_frag, nm, (rows < n_frag + sizes.to(torch.int64)[:, None]).to(nm.dtype))
+        pocket_only = full['context'][..., -1] if self.dynamics.graph_type != 'FC' else None
+        return graph_hashes(chain0, nm, self.is_geom, pocket_only)
 
     # the keyword arguments of sample_chain that make up one request of sample_many
     _REQUEST_INPUTS = ('x', 'h', 'node_mask', 'fragment_mask', 'linker_mask', 'edge_mask', 'context')
@@ -742,7 +784,8 @@ class EDM(torch.nn.Module):
         packing does not change them.
         Raises ValueError for an empty list, the batch stream (its draws depend on B and N), noise= or a replaced draw
         function, host inputs, requests on different devices or of different feature or context widths, and seeds that do
-        not match the requests."""
+        not match the requests. It takes no `require_unique`, and raises ValueError when the attribute is set: a launch packs
+        several requests, whose rows one verdict would compare with each other."""
         if keep_frames is None:
             keep_frames = self.T
         else:
@@ -750,6 +793,10 @@ class EDM(torch.nn.Module):
         requests = list(requests)
         if not requests:
             raise ValueError("sample_many needs at least one request")
+        if self.require_unique is not False:
+            raise ValueError("sample_many does not take require_unique: a launch packs several requests, so their rows would "
+                             "be compared with each other; call sample_chain per request, or deduplicate with "
+                             "molecule_builder.graph_hashes")
         self._start(start_step, 1)          # validates it before anything else is checked
         for k, r in enumerate(requests):
             if 'noise' in r or 'batch_slice' in r:
@@ -1038,21 +1085,22 @@ class InpaintingEDM(EDM):
 
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
-                     require_valid=None, require_clash_free=None, linker_sizes=None):
+                     require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
         (dl_sample_chain_rng), unless `draw_noise_inpaint` is replaced -- on the instance, in a subclass or on the class --
         in which case the replacement draws them. `batch_slice=(b0, B_full)` and `seeds` as in EDM.sample_chain: with
         seeds, molecule b's 2T+3 raw draws are those of the molecule sampled alone after torch.cuda.manual_seed(seeds[b]),
-        masked and projected per molecule as always. `nan_retries`, `require_connected` and `require_valid` as in EDM.sample_chain;
-        the checks cover every atom of the molecule. `start_step` raises ValueError unless None, and `require_clash_free`
+        masked and projected per molecule as always. `nan_retries`, `require_connected`, `require_valid` and `require_unique`
+        as in EDM.sample_chain; the checks and the hash cover every atom of the molecule. `start_step` raises ValueError unless None, and `require_clash_free`
         unless None or False: this loop re-noises the pocket; `linker_sizes` unless None: this model has no linker size."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
                                     require_connected=require_connected, start_step=start_step, require_valid=require_valid,
-                                    require_clash_free=require_clash_free, linker_sizes=linker_sizes)
+                                    require_clash_free=require_clash_free, linker_sizes=linker_sizes,
+                                    require_unique=require_unique)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

@@ -3,7 +3,8 @@ GPU (`dl_bond_orders`) instead of an O(n^2) Python loop with one `.item()` per a
 RDKit molecule construction (`build_molecule`, molecule_builder.py:29-42) stays with the caller: RDKit is not part of
 the path (SURVEY.md section 8(f) rank 4). `connected` and `valence_ok` decide on the device what the reference's
 `validity_and_connectivity` asks of those molecules, the latter as "explicit valence within a table". `clash_free` is this
-project's own check, with no reference counterpart: whether a linker runs into the pocket.
+project's own check, with no reference counterpart: whether a linker runs into the pocket. `graph_hashes` gives the hash
+behind uniqueness (compute_metrics.py's share of distinct molecules): equal for isomorphic bond graphs.
 """
 import torch
 
@@ -54,12 +55,13 @@ def max_valence_table(is_geom):
 
 
 def check_tables(is_geom, require, max_valence=None):
-    """The CPU tables the molecule checks `require` (an OR of _native.CHECK_*) read: [thr1] for connectivity alone, and
-    [thr1, thr2, thr3, max_valence] once CHECK_VALENCE is required (threshold_tables; `max_valence` a (T,) integer table by
-    atom type index, by default max_valence_table(is_geom))."""
+    """The CPU tables the molecule checks `require` (an OR of _native.CHECK_*) read: [thr1] for connectivity alone,
+    [thr1, thr2, thr3] for CHECK_UNIQUE (the bond orders of the graph hash), and [thr1, thr2, thr3, max_valence] once
+    CHECK_VALENCE is required (threshold_tables; `max_valence` a (T,) integer table by atom type index, by default
+    max_valence_table(is_geom))."""
     thr = threshold_tables(is_geom)
     if not require & _native.CHECK_VALENCE:
-        return thr[:1]
+        return thr if require & _native.CHECK_UNIQUE else thr[:1]
     mv = max_valence_table(is_geom) if max_valence is None else torch.as_tensor(max_valence).to(torch.int32).contiguous()
     if mv.shape != (thr[0].shape[0],):
         raise ValueError(f"max_valence holds one entry per atom type, {thr[0].shape[0]} (got shape {tuple(mv.shape)})")
@@ -149,6 +151,33 @@ def valence_ok(xh, node_mask, is_geom, pocket_only=None, max_valence=None):
     Chem.SanitizeMol; that equivalence has not been verified against RDKit."""
     passed, _ = _molecule_check(xh, node_mask, is_geom, pocket_only, max_valence, _native.CHECK_VALENCE, False)
     return (passed & _native.CHECK_VALENCE) != 0
+
+
+@torch.no_grad()
+def graph_hashes(xh, node_mask, is_geom, pocket_only=None):
+    """(B,) int64 on the device, holding the uint64 bits of every molecule's graph hash (dl_molecule_hash, the hash behind
+    sample_chain(require_unique=True)): Weisfeiler-Lehman colour refinement over the atoms, their types and bond_orders'
+    orders, stated at DL_CHECK_UNIQUE in the header. The atoms and types are those of connected(). Isomorphic graphs
+    always hash equal, whatever the row order, pose or padding; non-isomorphic graphs can collide (1-WL-equivalent pairs
+    always do, and a 64-bit collision is possible); stereochemistry is ignored, and equal hashes have not been verified to
+    mean equal RDKit canonical SMILES. Compare these to deduplicate across calls or devices."""
+    dev = xh.device
+    if dev.type != 'cuda':
+        raise RuntimeError("the molecule checks run on the GPU (no CPU fallback); move the tensors to the device")
+    B, N = xh.shape[:2]
+    xs = xh.float().contiguous()
+    nm = (node_mask.reshape(B, N) != 0).to(torch.int8).contiguous()
+    po = None if pocket_only is None else pocket_only.reshape(B, N, 1).float().contiguous()
+    tables = [t.to(dev) for t in check_tables(is_geom, _native.CHECK_UNIQUE)]
+    checks = _native.DLMoleculeChecks.of(_native.CHECK_UNIQUE, tables)
+    out = torch.empty(B, dtype=torch.int64, device=dev)
+    lib = _native.load_library()
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream().cuda_stream
+        _native.check(lib.dl_molecule_hash(B, N, checks, xs.data_ptr(), xs.shape[2], nm.data_ptr(),
+                                           None if po is None else po.data_ptr(), 1, int(po is not None), out.data_ptr(),
+                                           st), "dl_molecule_hash")
+    return out
 
 
 @torch.no_grad()

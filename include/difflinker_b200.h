@@ -27,6 +27,8 @@
  *     beyond its valence (the explicit-valence part of validity, src/metrics.py:12-17; see dl_molecule_checks)
  *   either on pocket graphs, also resampling the        dl_sample_chain_retry with DL_CHECK_CLASH, dl_clash_check
  *     molecules whose linker clashes with the pocket (no reference API; see dl_molecule_checks)
+ *   either, also resampling the molecules that repeat   dl_sample_chain_retry with DL_CHECK_UNIQUE, dl_molecule_hash
+ *     a batch-mate (uniqueness, compute_metrics.py; see DL_CHECK_UNIQUE)
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   softmax + Categorical.sample of a size model (generate.py:88-99), from dl_size_draw, dl_size_uniform
  *     the molecule's seed, and redrawn in the recovery rounds             dl_sample_chain_retry with dl_size_redraw
@@ -267,12 +269,40 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt);
  *   argument); molecule_builder.clash_table builds a default, 75% of the sum of the two elements' Bondi van der Waals
  *   radii, a common protein-ligand contact tolerance that has not been validated against any docking tool.
  */
-enum { DL_CHECK_CONNECTED = 1, DL_CHECK_VALENCE = 2, DL_CHECK_CLASH = 4 };
+/*
+ *   DL_CHECK_UNIQUE (uniqueness among the samples of one input, compute_metrics.py) compares molecules with each other,
+ *              by a graph hash of the atoms, types and bond orders above. With n atoms, t_i atom i's type, o_ij in {0,1,2,3}
+ *              the bond order of the pair, mix(z) the splitmix64 finaliser of dl_size_uniform (z ^= z >> 30;
+ *              z *= 0xBF58476D1CE4E5B9; z ^= z >> 27; z *= 0x94D049BB133111EB; z ^= z >> 31), TAG = 0x67726170682D776C
+ *              ("graph-wl") and all arithmetic modulo 2^64:
+ *                  c_0(i)     = mix(TAG ^ (t_i + 1))
+ *                  c_{k+1}(i) = mix(c_k(i) + sum over j != i with o_ij > 0 of mix(c_k(j) + o_ij * 0x9E3779B97F4A7C15))
+ *                  H          = mix(n + sum_i c_R(i)),   R = min(n, 64)          (no atom: H = mix(0) = 0)
+ *              i.e. Weisfeiler-Lehman colour refinement with order-free sums. What it promises and what it does not:
+ *                - isomorphic graphs (same elements, same bond orders) always hash equal, whatever the row order, pose
+ *                  or padding;
+ *                - non-isomorphic graphs can collide: 1-WL-equivalent pairs (e.g. decalin and bicyclopentyl) always do,
+ *                  and a 64-bit collision is possible. A false duplicate costs one needless resample, never a returned
+ *                  duplicate;
+ *                - stereochemistry is ignored;
+ *                - these are dl_bond_orders' graphs, not RDKit SMILES: two Kekule assignments of one aromatic ring are
+ *                  different graphs. "Equal hash iff equal canonical SMILES" has NOT been verified against RDKit.
+ *              The verdict, over the rows of one dl_sample_chain_retry call (the group is the whole call): after the first
+ *              loop every row is a candidate; in recovery round a, the rows of that round's sub-batch are, each as the
+ *              take rule left it. Keepers are the other rows that pass every required bit; eligible candidates are the
+ *              finite ones with every other required bit. Candidate b gets DL_CHECK_UNIQUE iff its hash equals no
+ *              keeper's and no eligible candidate b' < b has the same hash. Keepers never lose it, so rows that pass are
+ *              not touched, and no two rows the call returns passing every required bit share a hash. A row that
+ *              misses another bit blocks no one, so two such rows may both keep DL_CHECK_UNIQUE with one hash; they are
+ *              resampled for the other bit anyway. dl_molecule_check refuses the bit (it checks each molecule alone); dl_molecule_hash gives the hashes, to compare across calls or
+ *              devices.
+ */
+enum { DL_CHECK_CONNECTED = 1, DL_CHECK_VALENCE = 2, DL_CHECK_CLASH = 4, DL_CHECK_UNIQUE = 8 };
 typedef struct dl_molecule_checks {
   int32_t require;             /* OR of DL_CHECK_*, at least one: which verdicts make a row fail and be resampled */
   int32_t n_types;             /* columns of h that hold the atom type */
   const float* thr1;           /* (n_types,n_types) fp32 DEVICE, as dl_bond_orders; needed unless DL_CHECK_CLASH alone */
-  const float* thr2;           /* needed for DL_CHECK_VALENCE only */
+  const float* thr2;           /* needed for DL_CHECK_VALENCE and DL_CHECK_UNIQUE only */
   const float* thr3;
   const int32_t* max_valence;  /* (n_types) int32 DEVICE; DL_CHECK_VALENCE only */
   const float* clash;          /* (n_types,n_types) fp32 DEVICE, in pm, [min type][max type]; DL_CHECK_CLASH only */
@@ -341,7 +371,10 @@ typedef struct dl_size_redraw {
  *                sub-batch in the rounds) and checks->clash; it is DL_ERR_INVALID without a table, on DL_GRAPH_FC (no pocket
  *                rows) and with DL_SAMPLER_INPAINT (whose loop re-noises the pocket).
  *   passed       (B) int32 DEVICE out, required with `checks`: the OR of the DL_CHECK_* bits row b's returned molecule
- *                satisfies, among those required
+ *                satisfies, among those required. DL_CHECK_UNIQUE (needs thr1, thr2 and thr3) is the verdict stated at
+ *                DL_CHECK_UNIQUE above, over the rows of this call: it runs after the first loop's checks and after every
+ *                round's, on the device. Without it there is no extra launch or allocation; with it the full batch's hashes
+ *                live in the engine (cached by B), not in a caller buffer. Bits 16 and up are refused.
  *   redraw       the sizes to redraw each resampled row's linker size from (dl_size_redraw), or NULL: sizes stay fixed,
  *                and `sizes_used` is not read
  *   sizes_used   (B) int32 DEVICE in/out, required with `redraw`: the attempt-0 sizes on entry; on return, the size of every
@@ -379,7 +412,9 @@ dl_status dl_sample_chain_retry(dl_engine* e, int32_t sampler, int32_t B, int32_
  *   passed    (B) int32 out, as above
  *   valence   (B,N) int32 out or NULL; needs DL_CHECK_VALENCE: each checked atom's valence, 0 on every other row (for a
  *             hand-off to RDKit, and for tests)
- * 1 <= N <= 8192. require takes DL_CHECK_CONNECTED and DL_CHECK_VALENCE only; the clash check alone is dl_clash_check.
+ * 1 <= N <= 8192. require takes DL_CHECK_CONNECTED and DL_CHECK_VALENCE only; the clash check alone is dl_clash_check, and
+ * DL_CHECK_UNIQUE, a verdict on molecules compared with each other, has no per-molecule form: dl_molecule_hash gives the
+ * hashes it compares.
  */
 dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
                             const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
@@ -399,6 +434,16 @@ dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* chec
 dl_status dl_clash_check(int32_t B, int32_t N, int32_t n_types, const float* clash, const float* xh, int32_t xh_row_stride,
                          const int8_t* node_mask, const float* linker_mask, const float* context, int32_t context_nf,
                          int32_t* passed, int32_t* clashes, void* stream);
+/*
+ * The graph hash of DL_CHECK_UNIQUE alone, on any (B,N) batch, without an engine. DEVICE buffers, enqueued on `stream`.
+ *   checks    n_types, thr1, thr2 and thr3 are read; require, max_valence and clash are not
+ *   xh, node_mask, context, context_nf, drop_pocket   as dl_molecule_check: the atoms and types of dl_molecule_checks
+ *   hash      (B) uint64 out: molecule b's H
+ * 1 <= n_types <= xh_row_stride - 3, 1 <= N <= 8192.
+ */
+dl_status dl_molecule_hash(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
+                           const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
+                           uint64_t* hash, void* stream);
 /* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_retry, each from its row gather to
  * its row scatter -- including the wait for the host to capture the sub-batch's step graph -- summed over the rounds; 0 when
  * no round ran. */
