@@ -10,7 +10,7 @@ GRAPH_TYPES = {"FC": 0, "4A": 1, "FC-4A": 2, "FC-10A-4A": 3}
 EDGE_IMPLS = {"auto": 0, "simt": 1, "wgmma": 2}
 SAMPLER_LINKER, SAMPLER_INPAINT = 0, 1
 AGGREGATIONS = {"sum": 0, "mean": 1}
-CHECK_CONNECTED, CHECK_VALENCE, CHECK_CLASH, CHECK_UNIQUE = 1, 2, 4, 8   # DL_CHECK_*
+CHECK_CONNECTED, CHECK_VALENCE, CHECK_CLASH, CHECK_UNIQUE, CHECK_NOVEL = 1, 2, 4, 8, 16   # DL_CHECK_*
 COORDS_RANGE = 15.0   # EGNN hands its own coords_range=15 to every EquivariantBlock (src/egnn.py:183,209)
 
 
@@ -47,6 +47,17 @@ class DLMoleculeChecks(C.Structure):
         return cls(require, tables[0].shape[0], *ptrs, None if clash is None else clash.data_ptr())
 
 
+class DLHashSets(C.Structure):
+    _fields_ = [("known", C.c_void_p), ("n_known", C.c_int64), ("seen", C.c_void_p), ("n_seen", C.c_int64)]
+
+    @classmethod
+    def of(cls, known, seen):
+        """The struct over two 1-D int64 device tensors of uint64 bits in ascending unsigned order, or None (an empty set),
+        which the caller keeps alive."""
+        ptr = lambda t: (None, 0) if t is None else (t.data_ptr(), t.numel())
+        return cls(*ptr(known), *ptr(seen))
+
+
 class DLSizeRedraw(C.Structure):
     _fields_ = [("C", C.c_int32), ("logits_row_stride", C.c_int32), ("logits", C.c_void_p), ("sizes", C.c_void_p),
                 ("n_frag", C.c_void_p), ("linker_x", C.c_void_p)]
@@ -77,6 +88,11 @@ SYMBOLS = {
     "dl_retry_seed": (C.c_uint64, [C.c_uint64, _I32]),
     "dl_sample_chain_retry": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32, _P,
                                      _P, C.POINTER(DLMoleculeChecks), _P, C.POINTER(DLSizeRedraw), _P, _P]),
+    "dl_sample_chain_retry_sets": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32,
+                                          _P, _P, C.POINTER(DLMoleculeChecks), C.POINTER(DLHashSets), _P, _P,
+                                          C.POINTER(DLSizeRedraw), _P, _P]),
+    "dl_novel_check": (_I32, [_I32, _I32, C.POINTER(DLMoleculeChecks), C.POINTER(DLHashSets), _P, _I32, _P, _P, _P, _I32,
+                              _I32, _P, _P, _P, _P]),
     "dl_size_draw": (_I32, [_I32, _I32, _P, _I32, _P, _P, _I32, _P, _P]),
     "dl_size_uniform": (C.c_double, [C.c_uint64]),
     "dl_molecule_check": (_I32, [_I32, _I32, C.POINTER(DLMoleculeChecks), _P, _I32, _P, _P, _I32, _I32, _P, _P, _P]),

@@ -1177,27 +1177,32 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt) { return retry_seed(seed,
 namespace {
 
 static_assert(CHECK_CONNECTED == DL_CHECK_CONNECTED && CHECK_VALENCE == DL_CHECK_VALENCE && CHECK_CLASH == DL_CHECK_CLASH &&
-              CHECK_UNIQUE == DL_CHECK_UNIQUE, "kernels_retry.cuh vs header");
+              CHECK_UNIQUE == DL_CHECK_UNIQUE && CHECK_NOVEL == DL_CHECK_NOVEL, "kernels_retry.cuh vs header");
 
 // What is wrong with a caller's dl_molecule_checks for molecules of N rows whose h holds at most max_types type columns, or
-// null. The sampler takes every check; dl_molecule_check the bond checks only (the clash check has dl_clash_check, and
-// DL_CHECK_UNIQUE compares the molecules of one sampling call with each other, which a per-molecule check cannot).
+// null. The sampler takes every check; dl_molecule_check the bond checks only (the clash check has dl_clash_check,
+// DL_CHECK_UNIQUE compares the molecules of one sampling call with each other, which a per-molecule check cannot, and
+// DL_CHECK_NOVEL needs a linker_mask).
 const char* checks_error(const dl_molecule_checks* ck, int N, int max_types, bool sampler) {
   if (!ck) return "null checks";
+  constexpr int hashed = DL_CHECK_UNIQUE | DL_CHECK_NOVEL;
   if (sampler) {
-    if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE | DL_CHECK_CLASH | DL_CHECK_UNIQUE)))
-      return "checks->require must be a non-empty OR of DL_CHECK_CONNECTED, DL_CHECK_VALENCE, DL_CHECK_CLASH and "
-             "DL_CHECK_UNIQUE";
+    if (ck->require == 0 ||
+        (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE | DL_CHECK_CLASH | DL_CHECK_UNIQUE | DL_CHECK_NOVEL)))
+      return "checks->require must be a non-empty OR of DL_CHECK_CONNECTED, DL_CHECK_VALENCE, DL_CHECK_CLASH, "
+             "DL_CHECK_UNIQUE and DL_CHECK_NOVEL";
   } else if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE))) {
     return "checks->require must be DL_CHECK_CONNECTED, DL_CHECK_VALENCE or both (the clash check runs through "
            "dl_clash_check; DL_CHECK_UNIQUE compares the molecules of a dl_sample_chain_retry call with each other, and "
-           "dl_molecule_hash gives their hashes)";
+           "dl_molecule_hash gives their hashes; DL_CHECK_NOVEL needs a linker_mask, and its linker hashes are "
+           "dl_molecule_hash over node_mask AND linker_mask)";
   }
   if (ck->n_types < 1 || ck->n_types > max_types) return "checks->n_types must be in [1, the width of the atom features]";
-  if ((ck->require & (DL_CHECK_CONNECTED | DL_CHECK_VALENCE | DL_CHECK_UNIQUE)) && !ck->thr1) return "null checks->thr1";
+  if ((ck->require & (DL_CHECK_CONNECTED | DL_CHECK_VALENCE | hashed)) && !ck->thr1) return "null checks->thr1";
   if ((ck->require & DL_CHECK_VALENCE) && (!ck->thr2 || !ck->thr3 || !ck->max_valence))
     return "DL_CHECK_VALENCE needs checks->thr2, thr3 and max_valence";
   if ((ck->require & DL_CHECK_UNIQUE) && (!ck->thr2 || !ck->thr3)) return "DL_CHECK_UNIQUE needs checks->thr2 and thr3";
+  if ((ck->require & DL_CHECK_NOVEL) && (!ck->thr2 || !ck->thr3)) return "DL_CHECK_NOVEL needs checks->thr2 and thr3";
   if (N > CONN_MAX_N) return "the molecule checks take N <= 8192";
   return nullptr;
 }
@@ -1253,15 +1258,64 @@ const char* redraw_error(int32_t sampler, int B, int N, const dl_size_redraw* rz
   return nullptr;
 }
 
+// Whether p is device memory of `device` or managed memory, by cudaPointerGetAttributes: what a kernel on that device may
+// read. Host, unregistered and unknown pointers are not.
+bool device_readable(const void* p, int device) {
+  cudaPointerAttributes at{};
+  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return at.type == cudaMemoryTypeManaged || (at.type == cudaMemoryTypeDevice && at.device == device);
+}
+
+// What is wrong with the hash sets of a dl_sample_chain_retry_sets call whose checks require `require`, or null. Checks
+// through `st` (the call blocks anyway) that every set in use is ascending.
+const char* sets_error(dl_engine* e, int require, const dl_hash_sets* hs, cudaStream_t st) {
+  if (hs->n_known < 0 || hs->n_seen < 0) return "sets->n_known and n_seen must be >= 0";
+  const bool known = (require & DL_CHECK_NOVEL) && hs->n_known > 0, seen = (require & DL_CHECK_UNIQUE) && hs->n_seen > 0;
+  if ((known && !hs->known) || (seen && !hs->seen)) return "null sets->known or seen with a positive count";
+  if (!known && !seen) return nullptr;
+  if ((known && !device_readable(hs->known, e->cfg.device)) || (seen && !device_readable(hs->seen, e->cfg.device)))
+    return "sets->known and seen must be device (or managed) memory of the engine's device";
+  if (cudaSetDevice(e->cfg.device) != cudaSuccess) return "cudaSetDevice failed";
+  StageLayout sl;
+  const int i_bad = sl.out(2 * sizeof(int32_t));
+  if (stage_inputs(e->sub_rows, sl, st) != DL_OK) return "could not allocate the set check's flags";
+  int32_t* bad = sl.at<int32_t>(i_bad);
+  int32_t h_bad[2] = {0, 0};
+  bool ok = cudaMemsetAsync(bad, 0, 2 * sizeof(int32_t), st) == cudaSuccess;
+  const std::pair<const uint64_t*, int64_t> sets[2] = {{known ? hs->known : nullptr, hs->n_known},
+                                                       {seen ? hs->seen : nullptr, hs->n_seen}};
+  for (int k = 0; k < 2 && ok; ++k) {
+    if (!sets[k].first || sets[k].second < 2) continue;
+    const int64_t blocks = std::min<int64_t>((sets[k].second + 255) / 256, 1024);
+    k_sorted_check<<<(int)blocks, 256, 0, st>>>(reinterpret_cast<const unsigned long long*>(sets[k].first), sets[k].second,
+                                                bad + k);
+    ok = cudaGetLastError() == cudaSuccess;
+    e->launches += 1;
+  }
+  ok = ok && cudaMemcpyAsync(h_bad, bad, sizeof(h_bad), cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+       cudaStreamSynchronize(st) == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    return "the check of sets->known and seen failed";
+  }
+  if (h_bad[0]) return "sets->known is not in ascending unsigned order";
+  if (h_bad[1]) return "sets->seen is not in ascending unsigned order";
+  return nullptr;
+}
+
 // dl_sample_chain_retry, and with `ck` its molecule checks, whose verdicts go to `passed`: a row then fails if its NaN
 // flag is set or a required bit is missing, and a resampled row replaces the caller's unless the caller's row is finite and
-// the new one diverged.
+// the new one diverged. `hs` (or null) holds the known set of DL_CHECK_NOVEL and the seen set of DL_CHECK_UNIQUE;
+// `linker_hash` (or null) receives every returned row's linker hash with DL_CHECK_NOVEL.
 dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames, const float* xh,
                        const int8_t* node_mask, const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
                        const float* context, const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
                        int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
-                       const dl_molecule_checks* ck, int32_t* passed, const dl_size_redraw* rz, int32_t* sizes_used,
-                       void* stream) {
+                       const dl_molecule_checks* ck, const dl_hash_sets* hs, int32_t* passed, uint64_t* linker_hash,
+                       const dl_size_redraw* rz, int32_t* sizes_used, void* stream) {
   e->retry_ms = 0.f;
   dl_status s = dl_sample_chain_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask,
                                        context, seeds, coef, norm, chain, nan_flags, stream);
@@ -1271,6 +1325,12 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
   CK(cudaMemsetAsync(attempts, 0, (size_t)B * sizeof(int32_t), st));
   const int require = ck ? ck->require : 0;
   const bool unique = (require & DL_CHECK_UNIQUE) != 0;
+  const bool seen = unique && hs && hs->n_seen > 0;        // the verdict's seen set
+  const SeenArgs sn{seen ? reinterpret_cast<const unsigned long long*>(hs->seen) : nullptr, seen ? hs->n_seen : 0};
+  const bool known = (require & DL_CHECK_NOVEL) && hs && hs->n_known > 0;
+  const unsigned long long* kn = known ? reinterpret_cast<const unsigned long long*>(hs->known) : nullptr;
+  const long long n_known = known ? hs->n_known : 0;
+  unsigned long long* lh = (require & DL_CHECK_NOVEL) ? reinterpret_cast<unsigned long long*>(linker_hash) : nullptr;
   std::vector<int32_t> flags(B), pass(B, require);
   unsigned long long* hash = nullptr;                      // DL_CHECK_UNIQUE: the full batch's graph hashes
   if (unique) {
@@ -1282,12 +1342,13 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
   if (ck) {
     const ClashArgs cl{linker_mask, ck->clash, nullptr};   // the clash check's linker rows and table
     CK(launch_molecule_check(require, check_args(e, *ck, chain, N, node_mask, context, passed), cl, HashArgs{hash, 0}, B,
-                             st));
+                             st, NovelArgs{linker_mask, kn, n_known, lh}));
     e->launches += 1;
-    if (unique) {                                          // every row is a candidate; there are no keepers yet
+    if (unique) {                                          // every row is a candidate; the only keepers are the seen set
       UniqueArgs u{};
       u.B = B; u.require = require; u.hash = hash; u.flags = nan_flags; u.passed = passed;
-      k_unique_verdict<<<(B + 255) / 256, 256, 0, st>>>(u);
+      if (seen) k_unique_verdict<<<(B + 255) / 256, 256, 0, st>>>(u, sn);
+      else k_unique_verdict<<<(B + 255) / 256, 256, 0, st>>>(u);
       LAUNCH_CHECK();
       e->launches += 1;
     }
@@ -1347,7 +1408,8 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
       CheckArgs ca = check_args(e, *ck, sa.s_chain, N, ga.s_node_mask, ga.s_context, sl.at<int32_t>(i_ps));
       ca.rows = ga.rows; ca.flags = nan_flags; ca.s_flags = sa.s_flags; ca.take = sl.at<int32_t>(i_tk);
       const HashArgs ha{sl.at<unsigned long long>(i_sh), 0};
-      CK(launch_molecule_check(require, ca, ClashArgs{ga.s_linker_mask, ck->clash, nullptr}, ha, Bs, st));
+      CK(launch_molecule_check(require, ca, ClashArgs{ga.s_linker_mask, ck->clash, nullptr}, ha, Bs, st,
+                               NovelArgs{ga.s_linker_mask, kn, n_known, lh}));
       e->launches += 1;
       sa.take = ca.take; sa.s_passed = ca.passed; sa.passed = passed;
       if (rz) k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa, za);
@@ -1363,7 +1425,8 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
       UniqueArgs u{};
       u.B = B; u.Bs = Bs; u.require = require; u.hash = hash; u.flags = nan_flags; u.passed = passed;
       u.rows = ga.rows; u.take = sa.take; u.s_hash = sl.at<unsigned long long>(i_sh);
-      k_unique_verdict<<<(Bs + 255) / 256, 256, 0, st>>>(u);
+      if (seen) k_unique_verdict<<<(Bs + 255) / 256, 256, 0, st>>>(u, sn);
+      else k_unique_verdict<<<(Bs + 255) / 256, 256, 0, st>>>(u);
       LAUNCH_CHECK();
       e->launches += 1;
     }
@@ -1387,6 +1450,38 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
   return DL_OK;
 }
 
+// The argument checks of dl_sample_chain_retry(_sets) `name`, then seeded_retry.
+dl_status retry_entry(const char* name, dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                      const float* xh, const int8_t* node_mask, const float* fragment_mask, const float* linker_mask,
+                      const int8_t* edge_mask, const float* context, const uint64_t* seeds, const dl_step_coef* coef,
+                      const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used,
+                      int32_t* attempts, const dl_molecule_checks* checks, const dl_hash_sets* sets, int32_t* passed,
+                      uint64_t* linker_hash, const dl_size_redraw* redraw, int32_t* sizes_used, void* stream) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
+  if (!nan_flags || !seeds_used || !attempts || (checks && !passed) || (redraw && !sizes_used)) {
+    set_err("%s: null argument (nan_flags, seeds_used, attempts, passed with checks or sizes_used with redraw)", name);
+    return DL_ERR_INVALID;
+  }
+  const char* why = checks ? checked_error(e, sampler, N, checks) : nullptr;
+  if (!why && linker_hash && !(checks && (checks->require & DL_CHECK_NOVEL)))
+    why = "linker_hash needs checks with DL_CHECK_NOVEL";
+  if (!why && sets && !checks) why = "sets need checks: the known set is read with DL_CHECK_NOVEL, the seen set with "
+                                     "DL_CHECK_UNIQUE";
+  if (!why && redraw) {
+    if (cudaSetDevice(e->cfg.device) != cudaSuccess) why = "cudaSetDevice failed";
+    else why = redraw_error(sampler, B, N, redraw, reinterpret_cast<cudaStream_t>(stream));
+  }
+  if (!why && sets) why = sets_error(e, checks->require, sets, reinterpret_cast<cudaStream_t>(stream));
+  if (why) {
+    set_err("%s: %s", name, why);
+    return DL_ERR_INVALID;
+  }
+  return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
+                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, sets, passed, linker_hash,
+                      redraw, sizes_used, stream);
+}
+
 }  // namespace
 
 extern "C" {
@@ -1397,25 +1492,22 @@ dl_status dl_sample_chain_retry(dl_engine* e, int32_t sampler, int32_t B, int32_
                                 const float* norm, float* chain, int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used,
                                 int32_t* attempts, const dl_molecule_checks* checks, int32_t* passed,
                                 const dl_size_redraw* redraw, int32_t* sizes_used, void* stream) {
-  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
-  if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
-  if (!nan_flags || !seeds_used || !attempts || (checks && !passed) || (redraw && !sizes_used)) {
-    set_err("dl_sample_chain_retry: null argument (nan_flags, seeds_used, attempts, passed with checks or sizes_used with "
-            "redraw)");
-    return DL_ERR_INVALID;
-  }
-  const char* why = checks ? checked_error(e, sampler, N, checks) : nullptr;
-  if (!why && redraw) {
-    if (cudaSetDevice(e->cfg.device) != cudaSuccess) why = "cudaSetDevice failed";
-    else why = redraw_error(sampler, B, N, redraw, reinterpret_cast<cudaStream_t>(stream));
-  }
-  if (why) {
-    set_err("dl_sample_chain_retry: %s", why);
-    return DL_ERR_INVALID;
-  }
-  return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
-                      coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, passed, redraw, sizes_used,
-                      stream);
+  return retry_entry("dl_sample_chain_retry", e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask,
+                     edge_mask, context, seeds, coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks,
+                     nullptr, passed, nullptr, redraw, sizes_used, stream);
+}
+
+dl_status dl_sample_chain_retry_sets(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                                     const float* xh, const int8_t* node_mask, const float* fragment_mask,
+                                     const float* linker_mask, const int8_t* edge_mask, const float* context,
+                                     const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
+                                     int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
+                                     const dl_molecule_checks* checks, const dl_hash_sets* sets, int32_t* passed,
+                                     uint64_t* linker_hashes, const dl_size_redraw* redraw, int32_t* sizes_used,
+                                     void* stream) {
+  return retry_entry("dl_sample_chain_retry_sets", e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask,
+                     linker_mask, edge_mask, context, seeds, coef, norm, chain, nan_flags, max_retries, seeds_used, attempts,
+                     checks, sets, passed, linker_hashes, redraw, sizes_used, stream);
 }
 
 dl_status dl_size_draw(int32_t B, int32_t C, const float* logits, int32_t logits_row_stride, const int32_t* sizes,
@@ -1464,6 +1556,35 @@ dl_status dl_molecule_hash(int32_t B, int32_t N, const dl_molecule_checks* check
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const CheckArgs ca = check_args(*checks, xh, N, xh_row_stride, node_mask, context, context_nf, drop_pocket != 0, nullptr);
   CK(launch_molecule_check(CHECK_UNIQUE, ca, ClashArgs{}, HashArgs{reinterpret_cast<unsigned long long*>(hash), 0}, B, st));
+  return DL_OK;
+}
+
+dl_status dl_novel_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const dl_hash_sets* sets, const float* xh,
+                         int32_t xh_row_stride, const int8_t* node_mask, const float* linker_mask, const float* context,
+                         int32_t context_nf, int32_t drop_pocket, int32_t* passed, uint64_t* linker_hash, uint64_t* hash,
+                         void* stream) {
+  const char* why = checks_error(checks, N, xh_row_stride - 3, true);
+  const int require = checks ? checks->require : 0;
+  int dev = 0;
+  if (!why && !(require & DL_CHECK_NOVEL)) why = "checks->require must include DL_CHECK_NOVEL";
+  else if (!why && (B <= 0 || N <= 0 || !xh || !node_mask || !linker_mask || !passed ||
+                    (drop_pocket && (!context || context_nf < 1))))
+    why = "invalid argument";
+  else if (!why && (require & DL_CHECK_UNIQUE) && !hash) why = "DL_CHECK_UNIQUE needs `hash`";
+  else if (!why && (require & DL_CHECK_CLASH) && (!checks->clash || !drop_pocket))
+    why = "DL_CHECK_CLASH needs checks->clash and drop_pocket (the pocket rows)";
+  else if (!why && sets && sets->n_known < 0) why = "sets->n_known must be >= 0";
+  else if (!why && sets && sets->n_known > 0 &&
+           (!sets->known || cudaGetDevice(&dev) != cudaSuccess || !device_readable(sets->known, dev)))
+    why = "sets->known must be device (or managed) memory of the current device";
+  if (why) { set_err("dl_novel_check: %s", why); return DL_ERR_INVALID; }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const CheckArgs ca = check_args(*checks, xh, N, xh_row_stride, node_mask, context, context_nf, drop_pocket != 0, passed);
+  const bool known = sets && sets->n_known > 0;
+  const NovelArgs nv{linker_mask, known ? reinterpret_cast<const unsigned long long*>(sets->known) : nullptr,
+                     known ? sets->n_known : 0, reinterpret_cast<unsigned long long*>(linker_hash)};
+  CK(launch_molecule_check(require, ca, ClashArgs{linker_mask, checks->clash, nullptr},
+                           HashArgs{reinterpret_cast<unsigned long long*>(hash), 0}, B, st, nv));
   return DL_OK;
 }
 

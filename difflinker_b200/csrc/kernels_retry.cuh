@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include <algorithm>
+#include <utility>
 
 #include "bonds.cuh"
 
@@ -226,7 +227,10 @@ __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a, RowSizeA
 // pocket atom (no linker or no pocket atom: set). The predicates are stated in full at dl_molecule_checks in the header.
 // CHECK_UNIQUE: the kernel writes each molecule's graph hash (stated at DL_CHECK_UNIQUE in the header) and leaves the bit
 // clear; k_unique_verdict sets it, since it compares molecules with each other.
+// CHECK_NOVEL: the bit is set iff the linker hash L -- the graph hash of the checked atoms with linker_mask != 0 -- is not
+// in the caller's sorted set of known linker hashes (stated at DL_CHECK_NOVEL in the header).
 constexpr int CHECK_CONNECTED = 1, CHECK_VALENCE = 2, CHECK_CLASH = 4, CHECK_UNIQUE = 8;   // DL_CHECK_* of the header
+constexpr int CHECK_NOVEL = 16;
 constexpr int CONN_MAX_N = 8192;                                     // rows per molecule: 20 bytes of shared memory each
 constexpr int CONN_SMEM_MAX = CONN_MAX_N * (int)(sizeof(float4) + sizeof(int));
 // With CHECK_UNIQUE a molecule also takes 8 bytes per row (the atoms' rows and the CSR offsets) and 4 bytes per stored
@@ -276,6 +280,27 @@ struct ClashArgs {
   int32_t* clashes;                      // (B, N) or null: every linker atom's count of pocket atoms it clashes with (other
                                          // rows are not written)
 };
+
+// What CHECK_NOVEL reads besides CheckArgs, a kernel parameter of the instantiations with the bit only.
+struct NovelArgs {
+  const float* linker_mask;              // (B, N): the checked atoms with linker_mask != 0 are the linker atoms
+  const unsigned long long* known;       // (n_known) ascending, unsigned order: the known linker hashes
+  long long n_known;
+  unsigned long long* linker_hash;       // out or null: molecule b's L at row b, or in a recovery round (CheckArgs::rows)
+                                         // at the caller's row rows[b], where the row is taken
+};
+
+// Whether v is among s[0, n), ascending in unsigned order (duplicates allowed): a binary search for the first entry >= v,
+// with 64-bit indices and unsigned compares.
+__host__ __device__ inline bool sorted_contains(const unsigned long long* s, long long n, unsigned long long v) {
+  long long lo = 0, hi = n;
+  while (lo < hi) {
+    const long long mid = lo + ((hi - lo) >> 1);
+    if (s[mid] < v) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo < n && s[lo] == v;
+}
 
 // Row r of the molecule at g0 as the staging below makes its atom: x, y, z and the type (the first argmax, NaN winning) as
 // int bits. The graph hash reads the atoms whose bonds do not fit its shared-memory CSR this way.
@@ -413,9 +438,13 @@ __device__ __forceinline__ unsigned long long graph_hash(const CheckArgs& a, con
 // count and the verdict do not depend on the order the lanes add in.
 // Hash (CHECK_UNIQUE): s_row[i] keeps atom i's row, and after the other checks graph_hash takes over the buffer: s_lab
 // holds the CSR offsets, the bonds follow s_row, and the colours overwrite s_at.
-// The body of the k_molecule_check kernels below; cl is read with CHECK_CLASH only, hk with CHECK_UNIQUE only.
+// Linker hash (CHECK_NOVEL): last, the linker atoms are staged again from global memory, in row order, over whatever the
+// checks above left in the buffer, and graph_hash runs on them alone.
+// The body of the k_molecule_check kernels below; cl is read with CHECK_CLASH only, hk with CHECK_UNIQUE or CHECK_NOVEL
+// (its edge_cap) only, nv with CHECK_NOVEL only.
 template <int CHECKS>
-__device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashArgs& cl, const HashArgs& hk) {
+__device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashArgs& cl, const HashArgs& hk,
+                                               const NovelArgs& nv) {
   extern __shared__ float4 s_at[];                    // [n]: x, y, z, type (int bits)
   int* s_lab = reinterpret_cast<int*>(s_at + a.N);    // [n]: the atoms' rows (valence), then parent pointers (components)
   int* s_row = s_lab + a.N;                           // [n] (CHECK_UNIQUE): the atoms' rows
@@ -581,6 +610,38 @@ __device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashAr
     const unsigned long long h = graph_hash(a, hk, g0, n, s_at, s_lab, s_row, reinterpret_cast<unsigned*>(s_row + a.N));
     if (tid == 0) hk.hash[b] = h;
   }
+  if constexpr ((CHECKS & CHECK_NOVEL) != 0) {
+    __syncthreads();                                  // the buffer is read above until here
+    if (tid == 0) s_n = 0;
+    __syncthreads();
+    for (int r0 = 0; r0 < a.N; r0 += 256) {           // the linker atoms: checked atoms with linker_mask != 0
+      const int r = r0 + tid;
+      bool ok = r < a.N && a.node_mask[g0 + r] != 0 && nv.linker_mask[g0 + r] != 0.f;
+      if (ok && a.drop_pocket) ok = a.context[(g0 + r) * a.C + a.C - 1] == 0.f;
+      const unsigned m = __ballot_sync(0xffffffffu, ok);
+      if (lane == 0) s_warp[warp] = __popc(m);
+      __syncthreads();
+      int off = s_n + __popc(m & ((1u << lane) - 1u)), total = 0;
+      for (int w = 0; w < 8; ++w) { off += w < warp ? s_warp[w] : 0; total += s_warp[w]; }
+      if (ok) {
+        s_at[off] = load_atom(a, g0, r);
+        s_row[off] = r;
+      }
+      __syncthreads();
+      if (tid == 0) s_n += total;
+      __syncthreads();
+    }
+    const int n_linker = s_n;
+    const unsigned long long l = graph_hash(a, hk, g0, n_linker, s_at, s_lab, s_row,
+                                            reinterpret_cast<unsigned*>(s_row + a.N));
+    if (tid == 0) {
+      if (!sorted_contains(nv.known, nv.n_known, l)) verdict |= CHECK_NOVEL;
+      if (nv.linker_hash) {                           // the take rule of the end of this function
+        if (!a.rows) nv.linker_hash[b] = l;
+        else if (!(a.flags[a.rows[b]] == 0 && a.s_flags[b] != 0)) nv.linker_hash[a.rows[b]] = l;
+      }
+    }
+  }
   if (tid == 0) {
     if (!(CHECKS & CHECK_UNIQUE) || a.passed) a.passed[b] = verdict;   // dl_molecule_hash has no verdicts
     if (a.rows) a.take[b] = !(a.flags[a.rows[b]] == 0 && a.s_flags[b] != 0);
@@ -590,41 +651,59 @@ __device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashAr
 // The instantiations without the clash and hash bits, with the clash bit, and with the hash bit.
 template <int CHECKS>
 __global__ void __launch_bounds__(256) k_molecule_check(CheckArgs a) {
-  static_assert((CHECKS & (CHECK_CLASH | CHECK_UNIQUE)) == 0, "the clash check takes ClashArgs, the hash HashArgs");
-  molecule_check<CHECKS>(a, ClashArgs{}, HashArgs{});
+  static_assert((CHECKS & (CHECK_CLASH | CHECK_UNIQUE | CHECK_NOVEL)) == 0,
+                "the clash check takes ClashArgs, the hash HashArgs, the linker hash NovelArgs");
+  molecule_check<CHECKS>(a, ClashArgs{}, HashArgs{}, NovelArgs{});
 }
 
 // (With __launch_bounds__(256) alone ptxas fits <6> into 32 registers and spills; a minimum of one CTA per SM lets it take
 // the 38-39 it needs.)
 template <int CHECKS>
 __global__ void __launch_bounds__(256, 1) k_molecule_check(CheckArgs a, ClashArgs k) {
-  static_assert((CHECKS & CHECK_CLASH) != 0 && (CHECKS & CHECK_UNIQUE) == 0, "only the clash check takes ClashArgs alone");
-  molecule_check<CHECKS>(a, k, HashArgs{});
+  static_assert((CHECKS & CHECK_CLASH) != 0 && (CHECKS & (CHECK_UNIQUE | CHECK_NOVEL)) == 0,
+                "only the clash check takes ClashArgs alone");
+  molecule_check<CHECKS>(a, k, HashArgs{}, NovelArgs{});
 }
 
 template <int CHECKS>
 __global__ void __launch_bounds__(256, 1) k_molecule_check(CheckArgs a, ClashArgs k, HashArgs h) {
-  static_assert((CHECKS & CHECK_UNIQUE) != 0, "only the hash takes HashArgs");
-  molecule_check<CHECKS>(a, k, h);
+  static_assert((CHECKS & CHECK_UNIQUE) != 0 && (CHECKS & CHECK_NOVEL) == 0, "only the hash takes HashArgs alone");
+  molecule_check<CHECKS>(a, k, h, NovelArgs{});
 }
 
 template <int CHECKS>
-cudaError_t launch_molecule_check_as(const CheckArgs& a, const ClashArgs& k, const HashArgs& h, int B, cudaStream_t st) {
+__global__ void __launch_bounds__(256, 1) k_molecule_check(CheckArgs a, ClashArgs k, HashArgs h, NovelArgs v) {
+  static_assert((CHECKS & CHECK_NOVEL) != 0, "only the linker hash takes NovelArgs");
+  molecule_check<CHECKS>(a, k, h, v);
+}
+
+template <int CHECKS>
+cudaError_t launch_molecule_check_as(const CheckArgs& a, const ClashArgs& k, const HashArgs& h, const NovelArgs& v, int B,
+                                     cudaStream_t st) {
   const size_t smem = (size_t)a.N * (sizeof(float4) + sizeof(int));
-  if constexpr ((CHECKS & CHECK_UNIQUE) != 0) {
+  if constexpr ((CHECKS & (CHECK_UNIQUE | CHECK_NOVEL)) != 0) {
     // 8 more bytes per row, then the bonds: HASH_EDGES_PER_ROW per row or what HASH_SMEM_MAX leaves (512 at N = 8192;
     // graph_hash rescans the atoms whose bonds do not fit)
     const size_t base = smem + (size_t)a.N * 2 * sizeof(int);
     const size_t cap = std::min((size_t)a.N * HASH_EDGES_PER_ROW, (HASH_SMEM_MAX - base) / sizeof(unsigned));
-    void (*kernel)(CheckArgs, ClashArgs, HashArgs) = k_molecule_check<CHECKS>;
     const size_t total = base + cap * sizeof(unsigned);
-    if (total > 48 * 1024) {
-      const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HASH_SMEM_MAX);
-      if (err != cudaSuccess) return err;
-    }
     HashArgs hh = h;
     hh.edge_cap = (int)cap;
-    kernel<<<B, 256, total, st>>>(a, k, hh);
+    if constexpr ((CHECKS & CHECK_NOVEL) != 0) {
+      void (*kernel)(CheckArgs, ClashArgs, HashArgs, NovelArgs) = k_molecule_check<CHECKS>;
+      if (total > 48 * 1024) {
+        const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HASH_SMEM_MAX);
+        if (err != cudaSuccess) return err;
+      }
+      kernel<<<B, 256, total, st>>>(a, k, hh, v);
+    } else {
+      void (*kernel)(CheckArgs, ClashArgs, HashArgs) = k_molecule_check<CHECKS>;
+      if (total > 48 * 1024) {
+        const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HASH_SMEM_MAX);
+        if (err != cudaSuccess) return err;
+      }
+      kernel<<<B, 256, total, st>>>(a, k, hh);
+    }
   } else if constexpr ((CHECKS & CHECK_CLASH) != 0) {
     void (*kernel)(CheckArgs, ClashArgs) = k_molecule_check<CHECKS>;
     if (smem > 48 * 1024) {
@@ -643,31 +722,28 @@ cudaError_t launch_molecule_check_as(const CheckArgs& a, const ClashArgs& k, con
   return cudaGetLastError();
 }
 
+// launch_molecule_check_as<C> for the one C in {1, ..., sizeof...(C)} that equals checks.
+template <int... C>
+cudaError_t launch_molecule_check_of(int checks, const CheckArgs& a, const ClashArgs& k, const HashArgs& h,
+                                     const NovelArgs& v, int B, cudaStream_t st, std::integer_sequence<int, C...>) {
+  cudaError_t err = cudaErrorInvalidValue;
+  (void)((checks == C + 1 && ((err = launch_molecule_check_as<C + 1>(a, k, h, v, B, st)), true)) || ...);
+  return err;
+}
+
 // Launches k_molecule_check<checks> over B molecules; checks is a non-empty OR of CHECK_*, N <= CONN_MAX_N.
 // The shared-memory limit is raised to its one maximum the first time a molecule needs more than the default, so
 // concurrent callers never lower it under each other.
-// CHECK_UNIQUE writes the hashes to h.hash.
+// CHECK_UNIQUE writes the hashes to h.hash; CHECK_NOVEL reads v.
 inline cudaError_t launch_molecule_check(int checks, const CheckArgs& a, const ClashArgs& k, const HashArgs& h, int B,
-                                         cudaStream_t st) {
-  constexpr int CV = CHECK_CONNECTED | CHECK_VALENCE, U = CHECK_UNIQUE;
-  switch (checks) {
-    case CHECK_CONNECTED: return launch_molecule_check_as<CHECK_CONNECTED>(a, k, h, B, st);
-    case CHECK_VALENCE: return launch_molecule_check_as<CHECK_VALENCE>(a, k, h, B, st);
-    case CHECK_CONNECTED | CHECK_VALENCE: return launch_molecule_check_as<CHECK_CONNECTED | CHECK_VALENCE>(a, k, h, B, st);
-    case CHECK_CLASH: return launch_molecule_check_as<CHECK_CLASH>(a, k, h, B, st);
-    case CHECK_CLASH | CHECK_CONNECTED: return launch_molecule_check_as<CHECK_CLASH | CHECK_CONNECTED>(a, k, h, B, st);
-    case CHECK_CLASH | CHECK_VALENCE: return launch_molecule_check_as<CHECK_CLASH | CHECK_VALENCE>(a, k, h, B, st);
-    case CHECK_CLASH | CV: return launch_molecule_check_as<CHECK_CLASH | CV>(a, k, h, B, st);
-    case U: return launch_molecule_check_as<U>(a, k, h, B, st);
-    case U | CHECK_CONNECTED: return launch_molecule_check_as<U | CHECK_CONNECTED>(a, k, h, B, st);
-    case U | CHECK_VALENCE: return launch_molecule_check_as<U | CHECK_VALENCE>(a, k, h, B, st);
-    case U | CV: return launch_molecule_check_as<U | CV>(a, k, h, B, st);
-    case U | CHECK_CLASH: return launch_molecule_check_as<U | CHECK_CLASH>(a, k, h, B, st);
-    case U | CHECK_CLASH | CHECK_CONNECTED: return launch_molecule_check_as<U | CHECK_CLASH | CHECK_CONNECTED>(a, k, h, B, st);
-    case U | CHECK_CLASH | CHECK_VALENCE: return launch_molecule_check_as<U | CHECK_CLASH | CHECK_VALENCE>(a, k, h, B, st);
-    case U | CHECK_CLASH | CV: return launch_molecule_check_as<U | CHECK_CLASH | CV>(a, k, h, B, st);
-    default: return cudaErrorInvalidValue;
-  }
+                                         cudaStream_t st, const NovelArgs& v = NovelArgs{}) {
+  return launch_molecule_check_of(checks, a, k, h, v, B, st, std::make_integer_sequence<int, 2 * CHECK_NOVEL - 1>{});
+}
+
+// dl_sample_chain_retry's vetting of a caller's hash set: bad[0] = 1 if some s[i] > s[i + 1] in unsigned order.
+__global__ void __launch_bounds__(256) k_sorted_check(const unsigned long long* s, long long n, int32_t* bad) {
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i + 1 < n; i += (long long)gridDim.x * 256)
+    if (s[i] > s[i + 1]) *bad = 1;
 }
 
 // The uniqueness verdict over a batch of B molecules whose graph hashes are hash[b] (stated at DL_CHECK_UNIQUE in the
@@ -684,11 +760,18 @@ struct UniqueArgs {
   const unsigned long long* s_hash;      // (Bs)
 };
 
-// A thread per candidate: the bit iff its hash equals no keeper's and no eligible earlier candidate's. Each thread writes
-// only its own row's bit and hash; the bits and hashes other threads read are not among them (a keeper is never written,
-// and a candidate's other bits and its hash are read from where they do not change), so the verdict does not depend on
-// the order the threads run in.
-__global__ void __launch_bounds__(256) k_unique_verdict(UniqueArgs u) {
+// The hashes of a caller's seen set, which count as keepers: a kernel parameter of the verdict with a set only.
+struct SeenArgs {
+  const unsigned long long* seen;        // (n_seen) ascending, unsigned order
+  long long n_seen;
+};
+
+// A thread per candidate: the bit iff its hash equals no keeper's and no eligible earlier candidate's (SEEN: and is not in
+// the seen set). Each thread writes only its own row's bit and hash; the bits and hashes other threads read are not among
+// them (a keeper is never written, and a candidate's other bits and its hash are read from where they do not change), so
+// the verdict does not depend on the order the threads run in.
+template <bool SEEN>
+__device__ __forceinline__ void unique_verdict(const UniqueArgs& u, const SeenArgs& s) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int nc = u.rows ? u.Bs : u.B;
   if (i >= nc) return;
@@ -697,7 +780,7 @@ __global__ void __launch_bounds__(256) k_unique_verdict(UniqueArgs u) {
   auto hash_of = [&](int k) { return u.rows && u.take[k] ? u.s_hash[k] : u.hash[row(k)]; };
   const int b = row(i);
   const unsigned long long h = hash_of(i);
-  bool dup = false;
+  bool dup = SEEN && sorted_contains(s.seen, s.n_seen, h);
   if (u.rows)
     for (int k = 0, p = 0; k < u.B && !dup; ++k) {   // keepers: the rows between the candidates
       if (p < u.Bs && u.rows[p] == k) { ++p; continue; }
@@ -710,5 +793,9 @@ __global__ void __launch_bounds__(256) k_unique_verdict(UniqueArgs u) {
   u.passed[b] = dup ? (u.passed[b] & ~CHECK_UNIQUE) : (u.passed[b] | CHECK_UNIQUE);
   if (u.rows && u.take[i]) u.hash[b] = u.s_hash[i];
 }
+
+__global__ void __launch_bounds__(256) k_unique_verdict(UniqueArgs u) { unique_verdict<false>(u, SeenArgs{}); }
+
+__global__ void __launch_bounds__(256) k_unique_verdict(UniqueArgs u, SeenArgs s) { unique_verdict<true>(u, s); }
 
 }  // namespace dl

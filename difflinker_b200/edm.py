@@ -18,7 +18,7 @@ import torch.nn.functional as F
 from . import _native
 from .distributed import (deal_launches, device_slices, pack_requests, place_rows, plan_launches, resolve_devices,
                           slice_sampler_inputs, unpack_rows)
-from .molecule_builder import check_tables, clash_table, graph_hashes
+from .molecule_builder import check_tables, clash_table, graph_hashes, sort_unsigned
 from .noise import PredefinedNoiseSchedule
 from .utils import FoundNaNException, nan_exception_class
 
@@ -46,11 +46,13 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
     samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, require, checks,
-    passed, redraw) resamples the molecules that diverged (dl_sample_chain_retry, which blocks until its rounds are done)
-    and, with `require` != 0, those that miss a required check, whose verdict bits go to `passed`; `checks` = (tables, clash)
-    on the slice's device, `tables` as molecule_builder.check_tables returns them and `clash` the (T,T) clash table or None.
-    `redraw` = (logits, size table, n_frag, normalised linker_x, sizes_used), device tensors, redraws the resampled rows'
-    linker sizes; None keeps them.
+    passed, redraw, sets, linker_hashes) resamples the molecules that diverged (dl_sample_chain_retry_sets, which blocks until its rounds
+    are done) and, with `require` != 0, those that miss a required check, whose verdict bits go to `passed`; `checks` =
+    (tables, clash) on the slice's device, `tables` as molecule_builder.check_tables returns them and `clash` the (T,T) clash
+    table or None. `redraw` = (logits, size table, n_frag, normalised linker_x, sizes_used), device tensors, redraws the
+    resampled rows' linker sizes; None keeps them. `sets` = (known, seen), sorted int64 device tensors or None, are the
+    hash sets of CHECK_NOVEL and CHECK_UNIQUE; None is two empty sets. `linker_hashes`, an int64 device tensor or None,
+    receives every returned row's linker hash (CHECK_NOVEL).
     `start` = (t0, alpha_t0, sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of
     the call (dl_set_start_step). Returns (status, what the batch stream consumed)."""
     if start is not None:
@@ -67,17 +69,19 @@ def _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry):
     if stream is None:
         return _native.check(lib.dl_sample_chain_host(eng, *head, noise.data_ptr(), *tail), "dl_sample_chain_host"), 0
     if retry is not None:
-        max_retries, used, attempts, require, checks, passed, redraw = retry
+        max_retries, used, attempts, require, checks, passed, redraw, sets, linker_hashes = retry
         ck = _native.DLMoleculeChecks.of(require, *checks) if require else None
+        hs = None if sets is None else _native.DLHashSets.of(*sets)
         rz = sizes = None
         if redraw is not None:
             logits, table, n_frag, linker_x, sizes = redraw
             rz = _native.DLSizeRedraw(table.numel(), logits.stride(0), logits.data_ptr(), table.data_ptr(), n_frag.data_ptr(),
                                       linker_x.data_ptr())
-        return _native.check(lib.dl_sample_chain_retry(
-            eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr(), ck,
-            passed.data_ptr() if require else None, rz, None if sizes is None else sizes.data_ptr(), stream),
-            "dl_sample_chain_retry"), 0
+        return _native.check(lib.dl_sample_chain_retry_sets(
+            eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr(), ck, hs,
+            passed.data_ptr() if require else None, None if linker_hashes is None else linker_hashes.data_ptr(), rz,
+            None if sizes is None else sizes.data_ptr(), stream),
+            "dl_sample_chain_retry_sets"), 0
     if seeds is not None:
         return _native.check(lib.dl_sample_chain_seeded(eng, *head, seeds.data_ptr(), *tail, stream),
                              "dl_sample_chain_seeded"), 0
@@ -224,14 +228,21 @@ class EDM(torch.nn.Module):
         self.require_unique = False
         self.last_unique = None                # calls with require_unique: the (B,) CPU bool uniqueness verdict of every row
         self.last_graph_hashes = None          # calls with require_unique: the (B,) CPU int64 graph hash of every row
-        self.last_sizes = None                 # calls with linker_sizes: the (B,) CPU int32 linker size of every returned row
+        # Novelty: likewise for the molecules whose linker hash (molecule_builder.linker_hashes) is in `known_linkers`, a
+        # 1-D int64 tensor of uint64 hashes in any order (molecule_builder.known_linkers builds it from a dataset), in the
+        # same check launch. Same needs; False, the default, checks nothing.
+        self.require_novel = False
+        self.known_linkers = None
+        self.last_novel = None                 # calls with require_novel: the (B,) CPU bool novelty verdict of every row
+        self.last_linker_hashes = None         # calls with require_novel: the (B,) CPU int64 linker hash of every row
+        self.last_sizes = None                # calls with linker_sizes: the (B,) CPU int32 linker size of every returned row
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
         # sample_many: per request, what last_seeds / last_attempts / last_connected / last_valid hold after its own
         # sample_chain call; per launch, (device, the requests it held, loop ms)
         self.last_seeds_many = self.last_attempts_many = self.last_connected_many = self.last_loop_ms_many = None
-        self.last_valid_many = self.last_clash_free_many = self.last_sizes_many = None
+        self.last_valid_many = self.last_clash_free_many = self.last_sizes_many = self.last_novel_many = None
 
     @property
     def devices(self):
@@ -501,7 +512,7 @@ class EDM(torch.nn.Module):
         return True
 
     def _checks(self, require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free=None,
-                require_unique=None):
+                require_unique=None, require_novel=None):
         """The molecule checks of a call as the OR of _native.CHECK_*; 0 checks nothing."""
         return ((_native.CHECK_CONNECTED if self._require_check('require_connected', require_connected, seeds, noise,
                                                                 batch_slice, x) else 0) |
@@ -509,7 +520,30 @@ class EDM(torch.nn.Module):
                  else 0) |
                 (_native.CHECK_CLASH if self._require_clash_free(require_clash_free, seeds, noise, batch_slice, x) else 0) |
                 (_native.CHECK_UNIQUE if self._require_check('require_unique', require_unique, seeds, noise, batch_slice, x)
-                 else 0))
+                 else 0) |
+                (_native.CHECK_NOVEL if self._require_novel(require_novel, seeds, noise, batch_slice, x) else 0))
+
+    def _require_novel(self, value, seeds, noise, batch_slice, x):
+        """_require_check for require_novel, which also needs the `known_linkers` set."""
+        if (self.require_novel if value is None else value) is True and self.known_linkers is None:
+            raise ValueError("require_novel needs the known linker hashes: set edm.known_linkers (e.g. "
+                             "molecule_builder.known_linkers of the training set)")
+        return self._require_check('require_novel', value, seeds, noise, batch_slice, x)
+
+    def _hash_sets(self, check, exclude_hashes, dev):
+        """(known, seen) of a call with the checks `check`: `known_linkers` with CHECK_NOVEL and `exclude_hashes` (with
+        CHECK_UNIQUE only), each sorted in unsigned order on `dev` (molecule_builder.sort_unsigned), or None; None without
+        either."""
+        def sorted_set(name, t):
+            if not torch.is_tensor(t) or t.dim() != 1 or t.dtype != torch.int64:
+                raise ValueError(f"{name} is a 1-D int64 tensor of uint64 hash bits (got "
+                                 f"{type(t).__name__ if not torch.is_tensor(t) else f'{t.dtype} of shape {tuple(t.shape)}'})")
+            return sort_unsigned(t.detach().to(dev))
+        if exclude_hashes is not None and not check & _native.CHECK_UNIQUE:
+            raise ValueError("exclude_hashes feeds the uniqueness verdict: it needs require_unique=True")
+        known = sorted_set('known_linkers', self.known_linkers) if check & _native.CHECK_NOVEL else None
+        seen = None if exclude_hashes is None else sorted_set('exclude_hashes', exclude_hashes)
+        return None if known is None and seen is None else (known, seen)
 
     def _require_clash_free(self, value, seeds, noise, batch_slice, x):
         """_require_check for require_clash_free, which also needs a pocket that stays put: a cut-off (pocket) graph and the
@@ -576,7 +610,8 @@ class EDM(torch.nn.Module):
     @torch.no_grad()
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
-                     require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None):
+                     require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
+                     require_novel=None, exclude_hashes=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -635,6 +670,16 @@ class EDM(torch.nn.Module):
         limits (1-WL-equivalent graphs and 64-bit collisions hash equal; stereochemistry is ignored; not verified against
         RDKit canonical SMILES). Refusals as for require_valid, plus ValueError when `devices` splits the batch into more
         than one slice: the slices recover on their engines independently, so no verdict sees the whole batch.
+        `exclude_hashes` (a 1-D int64 tensor of graph hashes, e.g. an earlier call's `last_graph_hashes`; needs
+        require_unique) extends that group across calls: its hashes count as keepers, so no returned row that passes every
+        required check has a hash among them. It is sorted in unsigned order on the device for every call.
+        `require_novel` (None: the `require_novel` attribute, default False) adds a sixth, in the same rounds and launch: the
+        row's linker hash -- molecule_builder.linker_hashes of chain[0], the graph hash of its checked atoms on the
+        linker_mask rows (with a size redraw, the row's returned linker rows) -- is in `known_linkers`, a 1-D int64 tensor of
+        uint64 hashes in any order (molecule_builder.known_linkers of a training set), sorted in unsigned order on the
+        device for every call. `last_novel` (B,) CPU bool tells which rows pass, `last_linker_hashes` (B,) CPU int64 holds
+        every row's linker hash, as the check launch computed it for the bit. Novel means "by this hash, against linkers hashed the same way", with the hash's limits
+        above. Refusals as for require_valid, plus ValueError without `known_linkers`.
         `linker_sizes` (a LinkerSizes; ddpm.sample_chain builds it) makes every round redraw the linker size of the rows it
         resamples, from the round's seed (dl_sample_chain_retry's redraw), and rebuild their template rows at that size
         inside the padded template. The inputs must be the template of the sizes dl_size_draw gives `seeds` at attempt 0,
@@ -653,12 +698,13 @@ class EDM(torch.nn.Module):
         dev = x.device
         self.last_attempts = None
         self.last_connected = self.last_valid = self.last_clash_free = self.last_sizes = None
-        self.last_unique = self.last_graph_hashes = None
+        self.last_unique = self.last_graph_hashes = self.last_novel = self.last_linker_hashes = None
         start = self._start(start_step, n_samples)
         redraw = self._linker_sizes(linker_sizes, seeds, noise, batch_slice, start_step, x, linker_mask)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
         check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free,
-                             require_unique)
+                             require_unique, require_novel)
+        sets = self._hash_sets(check, exclude_hashes, dev)
         recover = retries > 0 or check != 0 # the recovery entry point: seeds used and attempts come back
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
         full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
@@ -691,7 +737,7 @@ class EDM(torch.nn.Module):
         calls, finish = self._enqueue_batch(lib, full, keep_frames, self.step_coefficients(keep_frames, n_samples), slices,
                                             engines, places, dev, noise=noise, dev_seeds=dev_seeds,
                                             rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check,
-                                            start=start, redraw=redraw)
+                                            start=start, redraw=redraw, sets=sets)
         by_device = {}
         for dev_i, c in calls:
             by_device.setdefault(dev_i, []).append(c)
@@ -731,6 +777,9 @@ class EDM(torch.nn.Module):
         if check & _native.CHECK_UNIQUE:
             self.last_unique = (out['passed'].cpu() & _native.CHECK_UNIQUE) != 0
             self.last_graph_hashes = self._graph_hashes(full, out['chain'][0], redraw, out['sizes']).cpu()
+        if check & _native.CHECK_NOVEL:
+            self.last_novel = (out['passed'].cpu() & _native.CHECK_NOVEL) != 0
+            self.last_linker_hashes = out['linker_hashes'].cpu()
         if out['bad']:
             exc = self._nan_exception(out['flags'], start)
             if recover:
@@ -755,7 +804,8 @@ class EDM(torch.nn.Module):
 
     @torch.no_grad()
     def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
-                    max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None):
+                    max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
+                    require_novel=None):
         """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
         edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
         (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
@@ -779,6 +829,7 @@ class EDM(torch.nn.Module):
         `last_clash_free_many` hold per
         request what last_seeds, last_attempts, last_connected and last_valid would hold after its own call; `last_loop_ms_many` holds (device,
         requests, loop ms) per launch. The single-call attributes are left as they were.
+        `require_novel` likewise, against `known_linkers`; `last_novel_many` holds every request's verdict.
         `linker_sizes`, one LinkerSizes per request, all of one size table, redraws sizes in those rounds as in sample_chain
         (it needs `seeds`); `last_sizes_many` holds every request's sizes. Each request's sizes come from its own seeds, so
         packing does not change them.
@@ -839,7 +890,9 @@ class EDM(torch.nn.Module):
         if dev.type != 'cuda':
             raise ValueError(f"sample_many needs CUDA inputs (got {dev})")
         retries = self._nan_retries(nan_retries, seeds, None, None, x0)
-        check = self._checks(require_connected, require_valid, seeds, None, None, x0, require_clash_free)
+        check = self._checks(require_connected, require_valid, seeds, None, None, x0, require_clash_free,
+                             require_novel=require_novel)
+        sets = self._hash_sets(check, None, dev)
         recover = retries > 0 or check != 0
         redraws = None
         if linker_sizes is not None:
@@ -886,7 +939,7 @@ class EDM(torch.nn.Module):
                 redraw = tuple(redraws[ks[0]][1] if j == 1 else torch.cat([redraws[k][j] for k in ks]) for j in range(5))
             [(_, call)], finish = self._enqueue_batch(lib, full, keep_frames, coefs[sizes[ks[0]]], [(dev_i, replica, 0, b)], [eng],
                                                       [where], dev, dev_seeds=dev_seeds, retries=retries, check=check,
-                                                      start=starts[sizes[ks[0]]], redraw=redraw)
+                                                      start=starts[sizes[ks[0]]], redraw=redraw, sets=sets)
             finishes.append(finish)
             by_device.setdefault(dev_i, []).append(
                 functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
@@ -902,6 +955,7 @@ class EDM(torch.nn.Module):
         results, flags = [None] * len(requests), [None] * len(requests)
         seeds_many, attempts_many = list(cpu_seeds), [None] * len(requests)
         connected_many, valid_many, clash_free_many = [None] * len(requests), [None] * len(requests), [None] * len(requests)
+        novel_many = [None] * len(requests)
         sizes_many = [None] * len(requests) if redraws is None else [rd[4].cpu() for rd in redraws]
         for (ks, _), finish in zip(launches, finishes):
             out = finish()
@@ -927,8 +981,11 @@ class EDM(torch.nn.Module):
                     valid_many[k] = (parts['passed'][j] & _native.CHECK_VALENCE) != 0
                 if check & _native.CHECK_CLASH:
                     clash_free_many[k] = (parts['passed'][j] & _native.CHECK_CLASH) != 0
+                if check & _native.CHECK_NOVEL:
+                    novel_many[k] = (parts['passed'][j] & _native.CHECK_NOVEL) != 0
         self.last_seeds_many, self.last_attempts_many, self.last_connected_many = seeds_many, attempts_many, connected_many
         self.last_valid_many, self.last_clash_free_many, self.last_sizes_many = valid_many, clash_free_many, sizes_many
+        self.last_novel_many = novel_many
         self.last_loop_ms_many = [(slots[slot_of[i]][0], sorted(ks), loop_ms[i]) for i, (ks, _) in enumerate(launches)]
         for k, f in enumerate(flags):
             if f.any():
@@ -950,13 +1007,14 @@ class EDM(torch.nn.Module):
         return coefs, starts, keys
 
     def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
-                       retries=0, check=0, start=None, redraw=None):
+                       retries=0, check=0, start=None, redraw=None, sets=None):
         """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
         inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
         replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
         covers the batch where it is. The draws are the per-molecule `dev_seeds`, the batch stream `rng` = (seed, offset,
         b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _checks; `start` as
-        returned by _start; `redraw` as returned by _linker_sizes (its rounds then redraw sizes, into `sizes`).
+        returned by _start; `redraw` as returned by _linker_sizes (its rounds then redraw sizes, into `sizes`); `sets` as
+        returned by _hash_sets, copied to each slice's device.
         Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
         (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
         back and returns dict(chain, flags, used, attempts, passed, sizes, bad, consumed) on `dev`; `passed` holds
@@ -973,6 +1031,9 @@ class EDM(torch.nn.Module):
                           if recover else (None, None))
         # molecule checks: every row's verdict bits, and the tables they read on each slice's device
         passed = torch.empty(n_samples, dtype=torch.int32, device=dev) if check else None
+        # CHECK_NOVEL: the linker hash the check decided every returned row's bit on
+        novel = bool(check & _native.CHECK_NOVEL)
+        linker_hashes = torch.empty(n_samples, dtype=torch.int64, device=dev) if novel else None
         # size redraws: every row's size, the attempt-0 sizes on entry
         redraw = redraw if recover else None
         sizes = None if redraw is None else redraw[4].clone()
@@ -1003,15 +1064,18 @@ class EDM(torch.nn.Module):
                             tuple(v.to(where).contiguous() for v in (logits[lo:hi], table, n_frag[lo:hi], linker_x[lo:hi],
                                                                      sizes[lo:hi])))
             checks_i = None if tables is None else ([t.to(where) for t in tables], None if clash is None else clash.to(where))
-            part = part + (checks_i, redraw_i)
+            sets_i = None if sets is None else tuple(None if s is None else s.to(where) for s in sets)
+            lh_i = linker_hashes if whole or not novel else torch.empty(hi - lo, dtype=torch.int64, device=where)
+            part = part + (checks_i, redraw_i, sets_i, lh_i)
             parts.append(part)              # alive until the flags have been read below
-            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, checks_i, redraw_i = part
+            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, checks_i, redraw_i, sets_i, lh_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
             rng_i = None if rng is None else (rng[0], rng[1], rng[2] + lo, rng[3])
             calls.append((dev_i, functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
-                (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i) if recover else None, start)))
+                (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i, sets_i, lh_i) if recover else None,
+                start)))
 
         def finish():
             if not whole:
@@ -1024,11 +1088,13 @@ class EDM(torch.nn.Module):
                     place_rows(passed, [p[7] for p in parts], slices)
                 if redraw is not None:
                     place_rows(sizes, [p[9][4] for p in parts], slices)
+                if novel:
+                    place_rows(linker_hashes, [p[11] for p in parts], slices)
             # the host sampler reports NaNs in its status; on the device, one sync per chain instead of one per step
             # (egnn.py:441), after every slice's loop and copy
             bad = _native.DL_NAN_DETECTED in [st for st, _ in results] or bool(flags.any().item())
-            return dict(chain=chain, flags=flags, used=used, attempts=attempts, passed=passed, sizes=sizes, bad=bad,
-                        consumed=[c for _, c in results])
+            return dict(chain=chain, flags=flags, used=used, attempts=attempts, passed=passed, sizes=sizes,
+                        linker_hashes=linker_hashes, bad=bad, consumed=[c for _, c in results])
         return calls, finish
 
 
@@ -1085,7 +1151,8 @@ class InpaintingEDM(EDM):
 
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
-                     require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None):
+                     require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
+                     require_novel=None, exclude_hashes=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -1093,14 +1160,16 @@ class InpaintingEDM(EDM):
         in which case the replacement draws them. `batch_slice=(b0, B_full)` and `seeds` as in EDM.sample_chain: with
         seeds, molecule b's 2T+3 raw draws are those of the molecule sampled alone after torch.cuda.manual_seed(seeds[b]),
         masked and projected per molecule as always. `nan_retries`, `require_connected`, `require_valid` and `require_unique`
-        as in EDM.sample_chain; the checks and the hash cover every atom of the molecule. `start_step` raises ValueError unless None, and `require_clash_free`
+        as in EDM.sample_chain; the checks and the hash cover every atom of the molecule. `require_novel` and
+        `exclude_hashes` as there; the linker hash covers the linker_mask rows. `start_step` raises ValueError unless None, and `require_clash_free`
         unless None or False: this loop re-noises the pocket; `linker_sizes` unless None: this model has no linker size."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
                                     require_connected=require_connected, start_step=start_step, require_valid=require_valid,
                                     require_clash_free=require_clash_free, linker_sizes=linker_sizes,
-                                    require_unique=require_unique)
+                                    require_unique=require_unique, require_novel=require_novel,
+                                    exclude_hashes=exclude_hashes)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

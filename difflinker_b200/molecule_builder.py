@@ -4,7 +4,8 @@ RDKit molecule construction (`build_molecule`, molecule_builder.py:29-42) stays 
 the path (SURVEY.md section 8(f) rank 4). `connected` and `valence_ok` decide on the device what the reference's
 `validity_and_connectivity` asks of those molecules, the latter as "explicit valence within a table". `clash_free` is this
 project's own check, with no reference counterpart: whether a linker runs into the pocket. `graph_hashes` gives the hash
-behind uniqueness (compute_metrics.py's share of distinct molecules): equal for isomorphic bond graphs.
+behind uniqueness (compute_metrics.py's share of distinct molecules): equal for isomorphic bond graphs. `linker_hashes`
+and `known_linkers` give the linker-scoped hash behind novelty (the share of linkers not in the training set).
 """
 import torch
 
@@ -56,12 +57,12 @@ def max_valence_table(is_geom):
 
 def check_tables(is_geom, require, max_valence=None):
     """The CPU tables the molecule checks `require` (an OR of _native.CHECK_*) read: [thr1] for connectivity alone,
-    [thr1, thr2, thr3] for CHECK_UNIQUE (the bond orders of the graph hash), and [thr1, thr2, thr3, max_valence] once
-    CHECK_VALENCE is required (threshold_tables; `max_valence` a (T,) integer table by atom type index, by default
-    max_valence_table(is_geom))."""
+    [thr1, thr2, thr3] for CHECK_UNIQUE or CHECK_NOVEL (the bond orders of the graph hash), and [thr1, thr2, thr3,
+    max_valence] once CHECK_VALENCE is required (threshold_tables; `max_valence` a (T,) integer table by atom type index, by
+    default max_valence_table(is_geom))."""
     thr = threshold_tables(is_geom)
     if not require & _native.CHECK_VALENCE:
-        return thr if require & _native.CHECK_UNIQUE else thr[:1]
+        return thr if require & (_native.CHECK_UNIQUE | _native.CHECK_NOVEL) else thr[:1]
     mv = max_valence_table(is_geom) if max_valence is None else torch.as_tensor(max_valence).to(torch.int32).contiguous()
     if mv.shape != (thr[0].shape[0],):
         raise ValueError(f"max_valence holds one entry per atom type, {thr[0].shape[0]} (got shape {tuple(mv.shape)})")
@@ -178,6 +179,48 @@ def graph_hashes(xh, node_mask, is_geom, pocket_only=None):
                                            None if po is None else po.data_ptr(), 1, int(po is not None), out.data_ptr(),
                                            st), "dl_molecule_hash")
     return out
+
+
+def linker_hashes(xh, node_mask, linker_mask, is_geom, pocket_only=None):
+    """(B,) int64 on the device: every molecule's linker hash (the L of DL_CHECK_NOVEL, the hash behind
+    sample_chain(require_novel=True)) -- graph_hashes over the rows with node_mask != 0 and linker_mask != 0, i.e. the graph
+    the linker atoms induce, as the reference's linker is the molecule with every fragment atom removed. A molecule without
+    linker atoms hashes to 0."""
+    B, N = xh.shape[:2]
+    nm = (node_mask.reshape(B, N) != 0) & (linker_mask.reshape(B, N).to(node_mask.device) != 0)
+    return graph_hashes(xh, nm, is_geom, pocket_only)
+
+
+def sort_unsigned(hashes):
+    """A 1-D int64 tensor of uint64 bits sorted in unsigned order, on its own device: the sign bit is flipped, the values
+    sorted as int64 and the bit flipped back (flipping the sign bit maps unsigned order onto signed order)."""
+    sign = torch.tensor(-(1 << 63), dtype=torch.int64, device=hashes.device)
+    return torch.sort(hashes.to(torch.int64) ^ sign).values ^ sign
+
+
+@torch.no_grad()
+def known_linkers(items, is_geom, batch_size=256, device=None):
+    """(K,) int64 on the device: the sorted (unsigned order), de-duplicated linker hashes of dataset items -- the dicts
+    ZincDataset / MOADDataset hold in .data, with 'positions' (n, 3) in Angstrom, 'one_hot' (n, F) and 'linker_mask' (n,)
+    (plus 'fragment_mask') -- for EDM.known_linkers. Items are collated with batching.collate, `batch_size` at a time, on
+    `device` (default: the current CUDA device), and hashed with linker_hashes. Saving the set is the caller's business."""
+    from .batching import collate
+    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.type != 'cuda':
+        raise RuntimeError("known_linkers hashes on the GPU (no CPU fallback); pass a CUDA device")
+    items = list(items)
+    keys = ('positions', 'one_hot', 'fragment_mask', 'linker_mask')
+    out = []
+    for b0 in range(0, len(items), batch_size):
+        batch = collate([{k: torch.as_tensor(it[k]).to(dev) for k in keys} for it in items[b0:b0 + batch_size]])
+        xh = torch.cat([batch['positions'].float(), batch['one_hot'].float()], dim=2)
+        out.append(linker_hashes(xh, batch['atom_mask'], batch['linker_mask'], is_geom))
+    if not out:
+        return torch.zeros(0, dtype=torch.int64, device=dev)
+    s = sort_unsigned(torch.cat(out))
+    keep = torch.ones_like(s, dtype=torch.bool)
+    keep[1:] = s[1:] != s[:-1]
+    return s[keep]
 
 
 @torch.no_grad()

@@ -29,6 +29,9 @@
  *     molecules whose linker clashes with the pocket (no reference API; see dl_molecule_checks)
  *   either, also resampling the molecules that repeat   dl_sample_chain_retry with DL_CHECK_UNIQUE, dl_molecule_hash
  *     a batch-mate (uniqueness, compute_metrics.py; see DL_CHECK_UNIQUE)
+ *   either, also resampling the molecules whose linker   dl_sample_chain_retry_sets with DL_CHECK_NOVEL (known set) or
+ *     is known, or that repeat an earlier call's          DL_CHECK_UNIQUE (seen set); dl_molecule_hash over the linker rows
+ *     (novelty, compute_metrics.py; see DL_CHECK_NOVEL)   and dl_novel_check
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   softmax + Categorical.sample of a size model (generate.py:88-99), from dl_size_draw, dl_size_uniform
  *     the molecule's seed, and redrawn in the recovery rounds             dl_sample_chain_retry with dl_size_redraw
@@ -296,17 +299,48 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt);
  *              misses another bit blocks no one, so two such rows may both keep DL_CHECK_UNIQUE with one hash; they are
  *              resampled for the other bit anyway. dl_molecule_check refuses the bit (it checks each molecule alone); dl_molecule_hash gives the hashes, to compare across calls or
  *              devices.
+ *              With a seen set (dl_hash_sets.seen: n_seen hashes in ascending unsigned order, duplicates allowed, e.g. the
+ *              hashes an earlier call returned) the seen hashes count as keepers too: a candidate also loses the bit when
+ *              its H is in the set. No returned row that passes every required bit then has a hash in the set, and no
+ *              two such rows share a hash. Everything else about the verdict is unchanged.
+ *   DL_CHECK_NOVEL (novelty, compute_metrics.py: the share of generated linkers that are not linkers of the training set)
+ *              compares a molecule's linker with a caller's set of known linkers. The linker atoms of molecule b are its
+ *              checked atoms (above) with linker_mask != 0; in the recovery rounds linker_mask is the sub-batch's, so a
+ *              redrawn size counts the redrawn linker rows, as DL_CHECK_CLASH does. Its linker hash L_b is exactly the H
+ *              of DL_CHECK_UNIQUE on the graph those atoms induce: the same types, the same dl_bond_orders orders, only
+ *              the bonds between linker atoms -- the reference's linker, the molecule with every fragment atom removed
+ *              (reformat_data_obabel.py). So L_b is dl_molecule_hash of the batch with node_mask replaced by
+ *              node_mask AND linker_mask; a molecule with no linker atom has L = mix(0) = 0. The bit holds iff L_b is not
+ *              in the caller's set (dl_hash_sets.known: n_known hashes in ascending unsigned order, duplicates allowed);
+ *              an empty set passes every row. The limits are the hash's: novel means "by this hash, against linkers hashed
+ *              the same way"; stereochemistry is ignored, there is no tautomer canonicalisation, 1-WL-equivalent graphs and
+ *              64-bit collisions hash equal, and the hash has NOT been verified against RDKit canonical SMILES. A false
+ *              "known" costs one needless resample and never returns a known linker. dl_molecule_check refuses the bit (it
+ *              takes no linker_mask); dl_novel_check runs it on any batch, and dl_molecule_hash over node_mask AND
+ *              linker_mask gives the same linker hashes.
  */
-enum { DL_CHECK_CONNECTED = 1, DL_CHECK_VALENCE = 2, DL_CHECK_CLASH = 4, DL_CHECK_UNIQUE = 8 };
+enum { DL_CHECK_CONNECTED = 1, DL_CHECK_VALENCE = 2, DL_CHECK_CLASH = 4, DL_CHECK_UNIQUE = 8, DL_CHECK_NOVEL = 16 };
 typedef struct dl_molecule_checks {
   int32_t require;             /* OR of DL_CHECK_*, at least one: which verdicts make a row fail and be resampled */
   int32_t n_types;             /* columns of h that hold the atom type */
   const float* thr1;           /* (n_types,n_types) fp32 DEVICE, as dl_bond_orders; needed unless DL_CHECK_CLASH alone */
-  const float* thr2;           /* needed for DL_CHECK_VALENCE and DL_CHECK_UNIQUE only */
+  const float* thr2;           /* needed for DL_CHECK_VALENCE, DL_CHECK_UNIQUE and DL_CHECK_NOVEL only */
   const float* thr3;
   const int32_t* max_valence;  /* (n_types) int32 DEVICE; DL_CHECK_VALENCE only */
   const float* clash;          /* (n_types,n_types) fp32 DEVICE, in pm, [min type][max type]; DL_CHECK_CLASH only */
 } dl_molecule_checks;
+/*
+ * The hash sets of dl_sample_chain_retry_sets. DEVICE buffers, each in ascending unsigned order (duplicates allowed), read
+ * while the call runs. A count of 0 is an empty set, whatever the pointer. It is a struct of its own rather than more fields
+ * of dl_molecule_checks, so that existing positional initialisers of that struct still compile warning-free.
+ */
+typedef struct dl_hash_sets {
+  const uint64_t* known;       /* (n_known): the known linker hashes of DL_CHECK_NOVEL; read with DL_CHECK_NOVEL only */
+  int64_t n_known;
+  const uint64_t* seen;        /* (n_seen): hashes that count as keepers in the DL_CHECK_UNIQUE verdict; read with
+                                  DL_CHECK_UNIQUE only */
+  int64_t n_seen;
+} dl_hash_sets;
 /*
  * Linker sizes drawn from a molecule's seed (no reference API; generate.py:88-99 draws them from one batch-level
  * Categorical.sample). Molecule b's size distribution is a table sizes[0..C) of ints >= 0 with finite fp32 logits
@@ -374,7 +408,10 @@ typedef struct dl_size_redraw {
  *                satisfies, among those required. DL_CHECK_UNIQUE (needs thr1, thr2 and thr3) is the verdict stated at
  *                DL_CHECK_UNIQUE above, over the rows of this call: it runs after the first loop's checks and after every
  *                round's, on the device. Without it there is no extra launch or allocation; with it the full batch's hashes
- *                live in the engine (cached by B), not in a caller buffer. Bits 16 and up are refused.
+ *                live in the engine (cached by B), not in a caller buffer. DL_CHECK_NOVEL (needs thr1, thr2 and thr3) reads
+ *                the linker rows of linker_mask (of the sub-batch in the rounds) and hashes them in the same launch as the
+ *                other checks; through this entry its known set is empty, so every row passes it (the set is an argument
+ *                of dl_sample_chain_retry_sets). Bits 32 and up are refused.
  *   redraw       the sizes to redraw each resampled row's linker size from (dl_size_redraw), or NULL: sizes stay fixed,
  *                and `sizes_used` is not read
  *   sizes_used   (B) int32 DEVICE in/out, required with `redraw`: the attempt-0 sizes on entry; on return, the size of every
@@ -404,6 +441,25 @@ dl_status dl_sample_chain_retry(dl_engine* e, int32_t sampler, int32_t B, int32_
                                 int32_t* attempts, const dl_molecule_checks* checks, int32_t* passed,
                                 const dl_size_redraw* redraw, int32_t* sizes_used, void* stream);
 /*
+ * dl_sample_chain_retry with the hash sets of DL_CHECK_NOVEL and DL_CHECK_UNIQUE (dl_hash_sets): `known` is the set
+ * DL_CHECK_NOVEL tests each row's linker hash against, `seen` the hashes that count as keepers in the DL_CHECK_UNIQUE
+ * verdict. sets == NULL, or both counts 0, is dl_sample_chain_retry itself: no extra launch. Before the first loop it
+ * checks, on `stream`, that every set in use (known with DL_CHECK_NOVEL, seen with DL_CHECK_UNIQUE, count > 0) is in
+ * ascending unsigned order; a set that is not, a pointer that is not device or managed memory of the engine's device, a NULL
+ * pointer with a positive count, a negative count or sets without `checks` is DL_ERR_INVALID.
+ *   linker_hashes  (B) uint64 DEVICE out or NULL; needs DL_CHECK_NOVEL: the linker hash L the check computed for every
+ *                  returned row -- the L its DL_CHECK_NOVEL bit was decided on.
+ * Everything else is dl_sample_chain_retry's.
+ */
+dl_status dl_sample_chain_retry_sets(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                                     const float* xh, const int8_t* node_mask, const float* fragment_mask,
+                                     const float* linker_mask, const int8_t* edge_mask, const float* context,
+                                     const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
+                                     int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
+                                     const dl_molecule_checks* checks, const dl_hash_sets* sets, int32_t* passed,
+                                     uint64_t* linker_hashes, const dl_size_redraw* redraw, int32_t* sizes_used,
+                                     void* stream);
+/*
  * The checks alone, on any (B,N) batch. DEVICE buffers, enqueued on `stream`.
  *   xh        (B,N,>=3+n_types) fp32, row stride xh_row_stride: x at columns 0..2, the atom-type one-hot from column 3
  *   node_mask (B,N) int8
@@ -414,11 +470,30 @@ dl_status dl_sample_chain_retry(dl_engine* e, int32_t sampler, int32_t B, int32_
  *             hand-off to RDKit, and for tests)
  * 1 <= N <= 8192. require takes DL_CHECK_CONNECTED and DL_CHECK_VALENCE only; the clash check alone is dl_clash_check, and
  * DL_CHECK_UNIQUE, a verdict on molecules compared with each other, has no per-molecule form: dl_molecule_hash gives the
- * hashes it compares.
+ * hashes it compares. DL_CHECK_NOVEL needs a linker_mask, which this entry does not take: the linker hashes are
+ * dl_molecule_hash over node_mask AND linker_mask.
  */
 dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
                             const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
                             int32_t* passed, int32_t* valence, void* stream);
+/*
+ * The checks with DL_CHECK_NOVEL, on any (B,N) batch, without an engine: the check launch of dl_sample_chain_retry_sets.
+ * DEVICE buffers, enqueued on `stream` of the current device.
+ *   checks       require includes DL_CHECK_NOVEL and may add DL_CHECK_CONNECTED, DL_CHECK_VALENCE, DL_CHECK_CLASH (needs
+ *                checks->clash and drop_pocket) and DL_CHECK_UNIQUE (needs `hash`; the bit itself is a verdict over a
+ *                call's rows and stays clear). Tables as for dl_sample_chain_retry.
+ *   sets         known (ascending unsigned order, not checked here) or NULL: an empty set; seen is not read
+ *   xh, node_mask, context, context_nf, drop_pocket   as dl_molecule_check
+ *   linker_mask  (B,N) fp32: the checked rows with linker_mask != 0 are the linker atoms
+ *   passed       (B) int32 out: the bits of require the molecule satisfies (DL_CHECK_UNIQUE clear)
+ *   linker_hash  (B) uint64 out or NULL: molecule b's L
+ *   hash         (B) uint64 out, with DL_CHECK_UNIQUE: molecule b's H
+ * 1 <= n_types <= xh_row_stride - 3, 1 <= N <= 8192.
+ */
+dl_status dl_novel_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const dl_hash_sets* sets, const float* xh,
+                         int32_t xh_row_stride, const int8_t* node_mask, const float* linker_mask, const float* context,
+                         int32_t context_nf, int32_t drop_pocket, int32_t* passed, uint64_t* linker_hash, uint64_t* hash,
+                         void* stream);
 /*
  * DL_CHECK_CLASH alone, on any (B,N) batch, without an engine. DEVICE buffers, enqueued on `stream`.
  *   clash       (n_types,n_types) fp32, in pm, as dl_molecule_checks.clash
