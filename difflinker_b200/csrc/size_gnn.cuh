@@ -8,6 +8,10 @@
 //   out[b] = mean over the N padded rows of embedding_out(h)
 // It is tiny next to the 500-step sampler (one pass over B*N^2 edges), so the fp32 SIMT kernels are the right tool.
 // normalization='batch_norm' (eval mode) is an affine map per channel: the host folds it into W3/b3 and W4/b4.
+// hidden_nf is 128 (the argparse default of train_size_gnn.py) or 256 (the reference README's recipe). The 256-wide model
+// runs its own kernels (kernels_size_wide.cuh: k_szw_prep -> [k_szw_edge -> k_szw_node] x n_layers -> k_szw_out) with the
+// same arithmetic, edge set and summation order; the 128-wide one runs the denoiser's SIMT kernels as before.
+#include "kernels_size_wide.cuh"
 
 struct dl_sizegnn {
   dl_sizegnn_config cfg{};
@@ -25,6 +29,7 @@ namespace {
 
 std::vector<ExpectedParam> sz_expected_params(const dl_sizegnn_config& c) {
   std::vector<ExpectedParam> v;
+  const int H = c.hidden_nf;
   v.push_back({"embedding_in.weight", (int64_t)H * c.in_node_nf});
   v.push_back({"embedding_in.bias", H});
   char buf[64];
@@ -50,6 +55,7 @@ dl_status sz_ensure_workspace(dl_sizegnn* e, int B, int N) {
   if (ws.B == B && ws.N == N) return DL_OK;
   free_workspace(ws);
   const size_t n = (size_t)B * N;
+  const int H = e->cfg.hidden_nf;
   dl_status s;
 #define WSA(field, cnt) if ((s = dev_alloc(ws, &ws.field, (cnt))) != DL_OK) return s
   WSA(nm, n); WSA(x0, n * 3); WSA(xa, n * 3); WSA(h, n * H); WSA(ABg, n * 2 * H); WSA(ABgmax, n * 2); WSA(agg, n * H);
@@ -60,13 +66,66 @@ dl_status sz_ensure_workspace(dl_sizegnn* e, int B, int N) {
   return DL_OK;
 }
 
+// k-major fp32 copies of one 256-wide GCL (prefix p ends in '.'): the edge MLP's first Linear over [h_i, h_j, radial]
+// split into W1a_t / W1b_t / b1 / wd, its second Linear W2_t / b2, and the node MLP W3_t ([h, agg] rows) / b3, W4_t / b4.
+void sz_pack_wide_gcl(Packer& pk, GclW& w, const RawWeights& raw, const std::string& p) {
+  constexpr int Hw = szw::W;
+  const auto& W1 = raw.at(p + "edge_mlp.0.weight");
+  pk.add(&w.W1a_t, transpose_block(W1, Hw, 2 * Hw + 1, 0, Hw));
+  pk.add(&w.W1b_t, transpose_block(W1, Hw, 2 * Hw + 1, Hw, Hw));
+  pk.add(&w.b1, raw.at(p + "edge_mlp.0.bias"));
+  pk.add(&w.wd, column(W1, Hw, 2 * Hw + 1, 2 * Hw));
+  pk.add(&w.W2_t, transpose_block(raw.at(p + "edge_mlp.2.weight"), Hw, Hw, 0, Hw));
+  pk.add(&w.b2, raw.at(p + "edge_mlp.2.bias"));
+  pk.add(&w.W3_t, transpose_block(raw.at(p + "node_mlp.0.weight"), Hw, 2 * Hw, 0, 2 * Hw));
+  pk.add(&w.b3, raw.at(p + "node_mlp.0.bias"));
+  pk.add(&w.W4_t, transpose_block(raw.at(p + "node_mlp.2.weight"), Hw, Hw, 0, Hw));
+  pk.add(&w.b4, raw.at(p + "node_mlp.2.bias"));
+}
+
+// The 256-wide forward after the work plan: the same launch sequence as the 128-wide one, on the wide kernels.
+dl_status sz_forward_wide(dl_sizegnn* e, const Geom& gm, const int8_t* fragment_mask, const float* xh, const int8_t* edge_mask,
+                          float* out, cudaStream_t st) {
+  Workspace& ws = e->ws;
+  const int n = gm.B * gm.N, L = e->cfg.n_layers;
+  // build_plan zeroes the first B*N*128 floats of agg; dead rows of the 256-wide aggregate must be exactly 0 as well
+  CK(cudaMemsetAsync(ws.agg, 0, (size_t)n * szw::W * sizeof(float), st));
+  const int node_blocks = (n + szw::TM - 1) / szw::TM;
+  szw::PrepArgsW pa{};
+  pa.xh = xh; pa.node_mask = fragment_mask; pa.We_t = e->We_t; pa.be = e->be; pa.proj = proj_of(e->layers[0]);
+  pa.nm = ws.nm; pa.x0 = ws.x0; pa.h = ws.h; pa.AB = ws.ABg;
+  szw::k_szw_prep<<<node_blocks, 256, 0, st>>>(gm, pa);
+  LAUNCH_CHECK();
+  const Plan plan = make_plan(ws);
+  for (int l = 0; l < L; ++l) {
+    const GclW& w = e->layers[l];
+    EdgeArgs ea{};
+    ea.AB = ws.ABg; ea.x0 = ws.x0; ea.edge_mask = edge_mask; ea.nm = ws.nm;
+    ea.W2_t = w.W2_t; ea.b2 = w.b2; ea.wd = w.wd; ea.plan = plan; ea.agg = ws.agg;
+    szw::k_szw_edge<<<2 * e->num_sms, 256, szw::EDGE_SMEM, st>>>(gm, ea);
+    LAUNCH_CHECK();
+    NodeArgs na{};
+    na.h = ws.h; na.agg = ws.agg; na.nm = ws.nm; na.W3_t = w.W3_t; na.b3 = w.b3; na.W4_t = w.W4_t; na.b4 = w.b4;
+    if (l + 1 < L) { na.proj1 = proj_of(e->layers[l + 1]); na.AB1 = ws.ABg; }
+    szw::k_szw_node<<<node_blocks, 256, szw::NODE_SMEM, st>>>(n, na);
+    LAUNCH_CHECK();
+  }
+  szw::k_szw_out<<<gm.B, 256, 0, st>>>(gm.N, e->cfg.out_node_nf, ws.h, e->Wo, e->bo, out);
+  LAUNCH_CHECK();
+  e->launches += 4 + 2 * L;
+  return DL_OK;
+}
+
 }  // namespace
 
 extern "C" {
 
 dl_status dl_sizegnn_create(const dl_sizegnn_config* cfg, dl_sizegnn** out) {
   if (!cfg || !out) { set_err("null argument"); return DL_ERR_INVALID; }
-  if (cfg->hidden_nf != H) { set_err("SizeGNN: hidden_nf must be %d (got %d)", H, cfg->hidden_nf); return DL_ERR_UNSUPPORTED; }
+  if (cfg->hidden_nf != H && cfg->hidden_nf != szw::W) {
+    set_err("SizeGNN: hidden_nf must be %d or %d (got %d)", H, szw::W, cfg->hidden_nf);
+    return DL_ERR_UNSUPPORTED;
+  }
   if (cfg->in_node_nf < 1 || cfg->in_node_nf > MAX_DIN || cfg->n_layers < 1 || cfg->out_node_nf < 1 ||
       cfg->out_node_nf > SZ_MAX_OUT) {
     set_err("SizeGNN: unsupported shape (in_node_nf %d, n_layers %d, out_node_nf %d)", cfg->in_node_nf, cfg->n_layers,
@@ -85,8 +144,13 @@ dl_status dl_sizegnn_create(const dl_sizegnn_config* cfg, dl_sizegnn** out) {
   dl_sizegnn* e = new dl_sizegnn();
   e->cfg = *cfg;
   e->num_sms = prop.multiProcessorCount;
-  CK(cudaFuncSetAttribute(k_node<ACT_RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * NODE_TM * LDX * sizeof(float)));
-  CK(cudaFuncSetAttribute(k_edge_simt<false, ACT_RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EDGE_SIMT_SMEM));
+  if (cfg->hidden_nf == szw::W) {
+    CK(cudaFuncSetAttribute(szw::k_szw_node, cudaFuncAttributeMaxDynamicSharedMemorySize, szw::NODE_SMEM));
+    CK(cudaFuncSetAttribute(szw::k_szw_edge, cudaFuncAttributeMaxDynamicSharedMemorySize, szw::EDGE_SMEM));
+  } else {
+    CK(cudaFuncSetAttribute(k_node<ACT_RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * NODE_TM * LDX * sizeof(float)));
+    CK(cudaFuncSetAttribute(k_edge_simt<false, ACT_RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EDGE_SIMT_SMEM));
+  }
   *out = e;
   return DL_OK;
 }
@@ -127,7 +191,8 @@ dl_status dl_sizegnn_finalize_weights(dl_sizegnn* e) {
   const RawWeights& raw = e->raw;
   Packer pk;
   e->layers.assign(L, GclW{});
-  pk.add(&e->We_t, transpose_block(raw.at("embedding_in.weight"), H, F_in, 0, F_in));
+  const bool wide = e->cfg.hidden_nf == szw::W;
+  pk.add(&e->We_t, transpose_block(raw.at("embedding_in.weight"), e->cfg.hidden_nf, F_in, 0, F_in));
   pk.add(&e->be, raw.at("embedding_in.bias"));
   pk.add(&e->Wo, raw.at("embedding_out.weight"));
   pk.add(&e->bo, raw.at("embedding_out.bias"));
@@ -135,6 +200,7 @@ dl_status dl_sizegnn_finalize_weights(dl_sizegnn* e) {
   for (int l = 0; l < L; ++l) {
     snprintf(buf, sizeof(buf), "layer%d.", l);
     GclW& w = e->layers[l];
+    if (wide) { sz_pack_wide_gcl(pk, w, raw, buf); continue; }
     pack_gcl(pk, w, raw, buf, 2 * H + 1);
     pk.add(&w.w0, std::vector<float>(H, 0.f));   // no input-distance column
   }
@@ -160,6 +226,7 @@ dl_status dl_sizegnn_forward(dl_sizegnn* e, int32_t B, int32_t N, const float* x
   gm.graph_type = 4; gm.norm_constant = 0.f; gm.normalization_factor = 1.f;
 
   if ((s = build_plan(ws, B, N, gm.graph_type, fragment_mask, nullptr, edge_mask, ET, MAXR, st)) != DL_OK) return s;
+  if (e->cfg.hidden_nf == szw::W) return sz_forward_wide(e, gm, fragment_mask, xh, edge_mask, out, st);
 
   const int node_blocks = (n + NODE_TM - 1) / NODE_TM;
   PrepArgs pa{};

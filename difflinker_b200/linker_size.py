@@ -18,6 +18,7 @@ ZINC_TRAIN_LINKER_SIZE2ID = {size: idx for idx, size in enumerate(ZINC_TRAIN_LIN
 GEOM_TRAIN_LINKER_ID2SIZE = [3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19,   # src/const.py:200-203
                              20, 21, 22, 23, 24, 25, 26, 27, 28, 29, 30, 31, 32, 36, 38, 41]
 GEOM_TRAIN_LINKER_SIZE2ID = {size: idx for idx, size in enumerate(GEOM_TRAIN_LINKER_ID2SIZE)}
+SIZE_GNN_WIDTHS = (128, 256)    # hidden_nf values the native SizeGNN has kernels for
 
 
 class _GCLParams(nn.Module):
@@ -50,8 +51,9 @@ class SizeGNN(nn.Module):
 
     def __init__(self, in_node_nf, hidden_nf, out_node_nf, n_layers, normalization, device='cpu'):
         super().__init__()
-        if hidden_nf != 128:
-            raise NotImplementedError("the native SizeGNN is specialised to hidden_nf = 128 (train_size_gnn.py:19)")
+        if hidden_nf not in SIZE_GNN_WIDTHS:
+            raise NotImplementedError(f"the native SizeGNN supports hidden_nf = 128 (train_size_gnn.py:19) or 256 (the "
+                                      f"README's size-model recipe), not {hidden_nf}")
         self.in_node_nf, self.hidden_nf, self.out_node_nf, self.n_layers = in_node_nf, hidden_nf, out_node_nf, n_layers
         self.normalization = normalization
         self.embedding_in = nn.Linear(in_node_nf, hidden_nf)

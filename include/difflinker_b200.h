@@ -639,7 +639,7 @@ dl_status dl_bond_orders(int32_t B, int32_t N, int32_t n_types, const float* x, 
 typedef struct dl_sizegnn dl_sizegnn; /* opaque */
 typedef struct dl_sizegnn_config {
   int32_t in_node_nf;   /* one-hot width the network was trained with */
-  int32_t hidden_nf;    /* 128 */
+  int32_t hidden_nf;    /* 128 (train_size_gnn.py's default) or 256 (the README's recipe); else DL_ERR_UNSUPPORTED */
   int32_t out_node_nf;  /* number of linker-size classes */
   int32_t n_layers;     /* GCLs (train_size_gnn.py:20: 3) */
   int32_t device;
