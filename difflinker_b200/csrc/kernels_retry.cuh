@@ -222,6 +222,8 @@ __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a, RowSizeA
 // makes of them (lightning.py:364-377, metrics.py:20-27).
 // CHECK_VALENCE: an atom's valence is the sum of bond_order_pair (get_bond_order) over the other checked atoms; the bit is
 // set iff every atom's valence is <= max_valence[its type] (no atom: set).
+// Both measure a pair as torch.cdist does over the n checked atoms, the later atom first (bonds.cuh): n counts the atoms
+// after drop_pocket, and the linker hash of CHECK_NOVEL measures over the linker atoms alone.
 // CHECK_CLASH (always with drop_pocket): the linker atoms are the checked atoms with linker_mask != 0, the pocket atoms the
 // rows with node_mask != 0 and context column C - 1 != 0; the bit is set iff no linker atom clashes (clash_pair) with any
 // pocket atom (no linker or no pocket atom: set). The predicates are stated in full at dl_molecule_checks in the header.
@@ -314,6 +316,21 @@ __device__ __forceinline__ float4 load_atom(const CheckArgs& a, size_t g0, int r
   return make_float4(row[0], row[1], row[2], __int_as_float(best));
 }
 
+// The staged atoms i != j (coordinates and type bits) of a molecule of n checked atoms, as a pair of bonds.cuh: the later
+// atom max(i, j) first, the orientation torch.cdist's matrix is read in (dists[i, j], i > j).
+__device__ __forceinline__ bool staged_bonded(const CheckArgs& a, int i, float4 pi, int j, float4 pj, int n) {
+  const float4 p = i > j ? pi : pj, q = i > j ? pj : pi;
+  float dist;
+  return bond_pair(make_float3(p.x, p.y, p.z), make_float3(q.x, q.y, q.z), __float_as_int(p.w), __float_as_int(q.w),
+                   a.n_types, a.thr1, n, &dist) >= 0;
+}
+
+__device__ __forceinline__ int staged_order(const CheckArgs& a, int i, float4 pi, int j, float4 pj, int n) {
+  const float4 p = i > j ? pi : pj, q = i > j ? pj : pi;
+  return bond_order_pair(make_float3(p.x, p.y, p.z), make_float3(q.x, q.y, q.z), __float_as_int(p.w), __float_as_int(q.w),
+                         a.n_types, a.thr1, a.thr2, a.thr3, n);
+}
+
 // The graph hash of the n staged atoms s_at[0, n) (rows s_row), stated at DL_CHECK_UNIQUE in the header: R = min(n, 64)
 // rounds of colour refinement c' (i) = mix(c(i) + sum over bonded j of mix(c(j) + o_ij * GRAPH_HASH_ORDER)), then
 // H = mix(n + sum_i c(i)). Block-collective; returns H on every thread.
@@ -332,9 +349,7 @@ __device__ __forceinline__ unsigned long long graph_hash(const CheckArgs& a, con
     int d = 0;
     for (int j = lane; j < n; j += 32) {
       const float4 pj = s_at[j];
-      float dist;
-      d += j != i && bond_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
-                               __float_as_int(pj.w), a.n_types, a.thr1, &dist) >= 0;
+      d += j != i && staged_bonded(a, i, pi, j, pj, n);
     }
     for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
     if (lane == 0) s_off[i] = d;
@@ -370,8 +385,7 @@ __device__ __forceinline__ unsigned long long graph_hash(const CheckArgs& a, con
       int o = 0;
       if (j < n && j != i) {
         const float4 pj = s_at[j];
-        o = bond_order_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
-                            __float_as_int(pj.w), a.n_types, a.thr1, a.thr2, a.thr3);
+        o = staged_order(a, i, pi, j, pj, n);
       }
       const unsigned m = __ballot_sync(0xffffffffu, o > 0);
       if (o > 0) s_edge[at + __popc(m & ((1u << lane) - 1u))] = (unsigned)j | ((unsigned)o << 16);
@@ -403,8 +417,7 @@ __device__ __forceinline__ unsigned long long graph_hash(const CheckArgs& a, con
         for (int j = lane; j < n; j += 32) {
           if (j == i) continue;
           const float4 pj = load_atom(a, g0, s_row[j]);
-          const int o = bond_order_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
-                                        __float_as_int(pj.w), a.n_types, a.thr1, a.thr2, a.thr3);
+          const int o = staged_order(a, i, pi, j, pj, n);
           if (o > 0) s += hash_mix(c[j] + (unsigned long long)o * GRAPH_HASH_ORDER);
         }
       }
@@ -553,9 +566,7 @@ __device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashAr
       int v = 0;
       for (int j = lane; j < n; j += 32) {
         const float4 pj = s_at[j];
-        if (j != i)
-          v += bond_order_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
-                               __float_as_int(pj.w), a.n_types, a.thr1, a.thr2, a.thr3);
+        if (j != i) v += staged_order(a, i, pi, j, pj, n);
       }
       for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
       if (lane == 0) {
@@ -578,10 +589,7 @@ __device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashAr
         const float4 pi = s_at[i];
         for (int j = lane; j < i; j += 32) {
           const float4 pj = s_at[j];
-          float dist;
-          if (bond_pair(make_float3(pi.x, pi.y, pi.z), make_float3(pj.x, pj.y, pj.z), __float_as_int(pi.w),
-                        __float_as_int(pj.w), a.n_types, a.thr1, &dist) < 0)
-            continue;
+          if (!staged_bonded(a, i, pi, j, pj, n)) continue;
           int ri = i, rj = j;
           while (lab[ri] != ri) ri = lab[ri];
           while (lab[rj] != rj) rj = lab[rj];

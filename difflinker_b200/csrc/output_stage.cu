@@ -119,6 +119,7 @@ extern "C" int64_t dl_format_xyz(int32_t B, int32_t N, int32_t F, const float* p
 // padded batch. E[b][i][j] (i > j, both atoms valid) = bond order 0..3 decided by the pair's distance in pm against the
 // tabulated single / double / triple bond lengths (+ margins) of the type pair ordered by type index
 // (`sorted([atom_types[i], atom_types[j]])`); the upper triangle and masked rows are 0 ("the graph is DIRECTED").
+// The distance is torch.cdist's over the molecule's n rows with node_mask != 0 (bonds.cuh): each block counts them.
 // thr1/thr2/thr3: (T x T) fp32 thresholds indexed [min type][max type]; a negative entry = pair absent from that table.
 // ------------------------------------------------------------------------------------------------------------------
 namespace {
@@ -128,6 +129,8 @@ __global__ void __launch_bounds__(256) k_bond_orders(int N, int T, const float* 
                                                      const float* __restrict__ thr3, int8_t* __restrict__ E) {
   const int b = blockIdx.y;
   const size_t g0 = (size_t)b * N;
+  int n = 0;
+  for (int r0 = 0; r0 < N; r0 += 256) n += __syncthreads_count(r0 + (int)threadIdx.x < N && node_mask[g0 + r0 + threadIdx.x]);
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < N * N; idx += gridDim.x * blockDim.x) {
     const int i = idx / N, j = idx - i * N;
     int8_t order = 0;
@@ -135,7 +138,7 @@ __global__ void __launch_bounds__(256) k_bond_orders(int N, int T, const float* 
       const float* xi = x + (g0 + i) * x_stride;
       const float* xj = x + (g0 + j) * x_stride;
       order = (int8_t)dl::bond_order_pair(make_float3(xi[0], xi[1], xi[2]), make_float3(xj[0], xj[1], xj[2]), types[g0 + i],
-                                          types[g0 + j], T, thr1, thr2, thr3);
+                                          types[g0 + j], T, thr1, thr2, thr3, n);
     }
     E[g0 * N + idx] = order;
   }

@@ -85,7 +85,11 @@ def clash_table(is_geom, scale=0.75):
 @torch.no_grad()
 def bond_orders(one_hot, x, node_mask, is_geom, margins=MARGINS_EDM):
     """Batched E of build_xae_molecule: (B,N,N) int8 on the inputs' device, E[b,i,j] (i > j) = bond order, else 0.
-    `x` may be (B,N,3) or chain[0]-style (B,N,3+F); atom types are argmax(one_hot) (molecule_builder.py:20)."""
+    `x` may be (B,N,3) or chain[0]-style (B,N,3+F); atom types are argmax(one_hot) (molecule_builder.py:20).
+    Distances are torch.cdist's on the CPU over each molecule's n rows with node_mask != 0, row i the later atom: the direct
+    form for n <= 25, the matmul form (_euclidean_dist) above, as stated at dl_molecule_checks in the header. torch's CPU
+    sqrt (MKL vsSqrt) is not always correctly rounded, so a pair within one ulp of a threshold can be decided the other way
+    by the reference; oracle/bond_rounding.py restates this arithmetic exactly."""
     dev = x.device
     if dev.type != 'cuda':
         raise RuntimeError("bond_orders runs on the GPU (no CPU fallback); move the tensors to the device")
@@ -107,7 +111,8 @@ def bond_orders(one_hot, x, node_mask, is_geom, margins=MARGINS_EDM):
 def connected(xh, node_mask, is_geom, pocket_only=None):
     """(B,) bool on the device: whether each molecule is in one piece (dl_molecule_check with CHECK_CONNECTED, the check
     behind sample_chain(require_connected=True)). Its atoms are the rows with node_mask != 0, minus those with
-    pocket_only != 0 when given; atoms i and j bond iff get_bond_order > 0, i.e. E[i, j] != 0 of bond_orders. `xh` is
+    pocket_only != 0 when given; atoms i and j bond iff get_bond_order > 0 on a distance measured as in bond_orders, over
+    these checked atoms (so dropping the pocket can change the form a pair is measured in). `xh` is
     chain[0]-style (B,N,3+F): the atom types are argmax of its first T feature columns (T = 9 with is_geom, else 8). One
     atom is connected, none is not."""
     passed, _ = _molecule_check(xh, node_mask, is_geom, pocket_only, None, _native.CHECK_CONNECTED, False)
@@ -140,7 +145,9 @@ def _molecule_check(xh, node_mask, is_geom, pocket_only, max_valence, require, w
 def valences(xh, node_mask, is_geom, pocket_only=None, max_valence=None):
     """(B,N) int32 on the device: every checked atom's valence -- the sum of get_bond_order over its pairs with the other
     checked atoms, i.e. the row-plus-column sum of bond_orders' E -- and 0 on the other rows (dl_molecule_check, the check
-    behind sample_chain(require_valid=True)). `xh`, `node_mask`, `pocket_only` and the checked atoms as in connected()."""
+    behind sample_chain(require_valid=True)). `xh`, `node_mask`, `pocket_only` and the checked atoms as in connected(). Each
+    pair is measured as torch.cdist measures it over the n checked atoms, the later atom as the row (bond_orders): with a
+    pocket dropped, n counts the atoms left."""
     return _molecule_check(xh, node_mask, is_geom, pocket_only, max_valence, _native.CHECK_VALENCE, True)[1]
 
 
@@ -161,7 +168,9 @@ def graph_hashes(xh, node_mask, is_geom, pocket_only=None):
     orders, stated at DL_CHECK_UNIQUE in the header. The atoms and types are those of connected(). Isomorphic graphs
     always hash equal, whatever the row order, pose or padding; non-isomorphic graphs can collide (1-WL-equivalent pairs
     always do, and a 64-bit collision is possible); stereochemistry is ignored, and equal hashes have not been verified to
-    mean equal RDKit canonical SMILES. Compare these to deduplicate across calls or devices."""
+    mean equal RDKit canonical SMILES. Compare these to deduplicate across calls or devices. The bond orders are
+    measured as torch.cdist measures them over the n hashed atoms, the later atom as the row (bond_orders): the direct form
+    for n <= 25, the matmul form above."""
     dev = xh.device
     if dev.type != 'cuda':
         raise RuntimeError("the molecule checks run on the GPU (no CPU fallback); move the tensors to the device")
@@ -185,7 +194,9 @@ def linker_hashes(xh, node_mask, linker_mask, is_geom, pocket_only=None):
     """(B,) int64 on the device: every molecule's linker hash (the L of DL_CHECK_NOVEL, the hash behind
     sample_chain(require_novel=True)) -- graph_hashes over the rows with node_mask != 0 and linker_mask != 0, i.e. the graph
     the linker atoms induce, as the reference's linker is the molecule with every fragment atom removed. A molecule without
-    linker atoms hashes to 0."""
+    linker atoms hashes to 0. The pairs are measured over the linker atoms alone (n is their count, bond_orders), so a
+    pair can be decided differently here than in graph_hashes of the whole molecule, as the reference decides it when it
+    builds the linker on its own."""
     B, N = xh.shape[:2]
     nm = (node_mask.reshape(B, N) != 0) & (linker_mask.reshape(B, N).to(node_mask.device) != 0)
     return graph_hashes(xh, nm, is_geom, pocket_only)

@@ -246,6 +246,17 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt);
  *              100 |x_i - x_j| against thr1, thr2, thr3 [min type][max type] (a negative entry: the pair has no such bond).
  *              Atoms i and j bond iff the order is > 0, i.e. 100 |x_i - x_j| < thr1[min t][max t] and that entry >= 0:
  *              dl_bond_orders' E != 0 is exactly this relation.
+ *   distance   |x_i - x_j| as torch.cdist measures it on the CPU over the n atoms the caller checks (the reference decides
+ *              bonds after .cpu()), with i the later atom of the pair in the molecule's compacted atom order (dists[i, j],
+ *              i > j). n <= 25: sqrt(fma(dz, dz, fma(dy, dy, dx * dx))). n > 25 (torch's _euclidean_dist):
+ *              c = ((((-2 x_i0) x_j0 + (-2 x_i1) x_j1) + (-2 x_i2) x_j2) + |x_i|^2) + |x_j|^2, the second and third
+ *              products fused, |x|^2 = (x0^2 + x1^2) + x2^2 rounded at each step; then a NaN-keeping clamp at 0 and a
+ *              correctly rounded sqrt. n counts the checked atoms: connectivity, valence and the graph hash H use the atoms
+ *              above, the linker hash L the linker atoms alone, dl_bond_orders the rows with node_mask != 0. So one pair can
+ *              be decided differently in H and in L, or with and without the pocket rows, as it is in the reference.
+ *              Residual: torch's CPU sqrt (MKL vsSqrt) rounds a fraction of a percent of its results one ulp away from the
+ *              correctly rounded root (torch 2.11, MKL 2024.2, AVX-512), so a pair within one ulp of a threshold can be
+ *              decided the other way there; the sgemm entries themselves matched this order bitwise.
  *   valence    of atom i: the integer sum of its pairs' bond orders over the other checked atoms. Pocket atoms are not
  *              partners either: src/lightning.py:372-374 drops them before the molecule is built.
  *   DL_CHECK_CONNECTED holds iff the graph of the atoms and their bonds has exactly one component (one atom is connected; no
@@ -264,8 +275,9 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt);
  *     linker atoms  rows with node_mask != 0, linker_mask != 0 and the last context column == 0. Fragment atoms are not
  *                   checked: they are inputs, which no resample moves.
  *     pocket atoms  rows with node_mask != 0 and the last context column != 0.
- *     clash         100 |x_i - x_j| in pm, with dl_bond_orders' arithmetic, is below clash[min t][max t] of the caller's
- *                   (n_types,n_types) table and that entry is >= 0; a negative entry means the pair never clashes (e.g. a
+ *     clash         100 |x_i - x_j| in pm, in the direct form sqrt(fma(dz, dz, fma(dy, dy, dx * dx))) at every
+ *                   atom count (the bond predicate's n <= 25 form, never torch.cdist's matmul form), is below
+ *                   clash[min t][max t] of the caller's (n_types,n_types) table and that entry is >= 0; a negative entry means the pair never clashes (e.g. a
  *                   covalent warhead's element against the residue it binds).
  *   A molecule with no linker atom or no pocket atom passes. A NaN coordinate compares false and clashes with nothing
  *   (divergence is the NaN flag's business). The table is the struct's `clash` field (dl_clash_check takes it as an
@@ -617,7 +629,8 @@ int64_t dl_format_xyz(int32_t B, int32_t N, int32_t F, const float* positions, i
  * dl_bond_orders -- molecule_builder.build_xae_molecule / get_bond_order (src/molecule_builder.py:44-102) for a padded
  * batch: E[b][i][j] (i > j, both atoms valid) = 0..3 from the pair distance in pm against single / double / triple bond
  * length thresholds (table value + margin, src/const.py:66-146,180) of the type pair ordered by type index; the upper
- * triangle and masked rows are 0.  DEVICE buffers, enqueued on `stream`.
+ * triangle and masked rows are 0. The distance is torch.cdist's over the molecule's n rows with node_mask != 0, the later
+ * row i first (stated at "distance" under dl_molecule_checks).  DEVICE buffers, enqueued on `stream`.
  *   x (B,N,>=3) fp32 with row stride x_row_stride; atom_types (B,N) int32; node_mask (B,N) int8
  *   thr1/thr2/thr3 (n_types,n_types) fp32 indexed [min type][max type]; negative = pair absent from that table
  *   E (B,N,N) int8 out

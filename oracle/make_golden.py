@@ -319,6 +319,34 @@ def golden_bonds(ns):
         save(name, dict(kind="bonds", is_geom=is_geom, counts=counts), positions=P, types=Ty, node_mask=M, E=Eb)
 
 
+def golden_bond_thresholds(ns):
+    """molecule_builder.build_xae_molecule of the live reference on the designed near-threshold molecules of
+    oracle/bond_rounding.py (golden_molecules, both tables): one pair per molecule whose bond decision differs between
+    torch.cdist's direct (n <= 25) and matmul (n > 25) forms, 25/26-atom twins, pocket designs with and without the pocket
+    rows and linker designs whole and alone. Molecules are stored end to end: positions / types by atom, with offsets, and
+    E as its lower triangle by molecule, with offsets. Pins the emulation and oracle.xae_molecule under the ambiguity rule
+    (tests/test_oracle_golden.py), since the BLAS and vector math that wrote it may not be the test host's."""
+    import importlib
+    from difflinker_b200 import molecule_builder as mb
+    from oracle import bond_rounding as br
+    ref = importlib.import_module("src.molecule_builder")
+    pos, types, tri, groups, geom, atom_off, tri_off = [], [], [], [], [], [0], [0]
+    for is_geom in (False, True):
+        thr = [t.numpy() for t in mb.threshold_tables(is_geom)]
+        for group, x, ty in br.golden_molecules(thr, seed=31 + int(is_geom)):
+            _, A, E = ref.build_xae_molecule(torch.from_numpy(x), torch.from_numpy(ty), is_geom=is_geom)
+            n = len(x)
+            lo = np.tril_indices(n, -1)
+            pos.append(x); types.append(ty); tri.append(E.numpy()[lo].astype(np.int8))
+            groups.append(group); geom.append(is_geom)
+            atom_off.append(atom_off[-1] + n); tri_off.append(tri_off[-1] + len(lo[0]))
+    names = sorted(set(groups))
+    save("bonds_thresholds", dict(kind="bonds_thresholds", groups=names, seeds=[31, 32]),
+         positions=np.concatenate(pos).astype(np.float32), types=np.concatenate(types).astype(np.int8),
+         atom_offsets=np.array(atom_off, np.int64), E_lower=np.concatenate(tri), E_offsets=np.array(tri_off, np.int64),
+         group=np.array([names.index(g) for g in groups], np.int8), is_geom=np.array(geom, np.int8))
+
+
 def golden_xyz(ns):
     """visualizer.save_xyz_file (visualizer.py:14-31) run for real into a temp dir; its files pin oracle.xyz_text."""
     import importlib
@@ -398,6 +426,7 @@ def main():
     golden_inpaint_chain(ns, "inpaint_chain_cfg1", S["cfg1_plumbing"], 4, seed=0, keep_frames=3)
     golden_xyz(ns)
     golden_bonds(ns)
+    golden_bond_thresholds(ns)
     golden_size_classifier(ns)
     golden_ddpm_layout(ns)
     print("all oracle / host-mirror checks against the reference passed")

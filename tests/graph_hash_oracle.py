@@ -1,10 +1,11 @@
 """A host restatement of the graph hash and the uniqueness verdict of DL_CHECK_UNIQUE (stated at DL_CHECK_UNIQUE in
 include/difflinker_b200.h), for the tests: Python ints masked to 64 bits, and bond orders from fp32 distances as
-dl_bond_orders computes them."""
+dl_bond_orders computes them: torch.cdist's arithmetic over the molecule's atoms (oracle/bond_rounding.py)."""
 import numpy as np
 import torch
 
 from difflinker_b200 import molecule_builder as mb
+from oracle import bond_rounding as br
 
 M64 = (1 << 64) - 1
 TAG = 0x67726170682D776C                      # "graph-wl"
@@ -34,28 +35,18 @@ def graph_hash(types, orders):
     return mix(n + sum(c))
 
 
-def dist_pm(xi, xj):
-    """100 |xi - xj| in fp32, each operation rounded on its own (pair_dist_pm)."""
-    d = np.asarray(xi, np.float32) - np.asarray(xj, np.float32)
-    return np.float32(100) * np.sqrt((d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2])
-
-
 def bond_order_matrix(x, types, thr):
     """(n, n) bond orders of get_bond_order with the (T, T) threshold tables thr = (thr1, thr2, thr3) read [min][max], and
-    the smallest |distance - threshold| over every existing threshold of every pair (for the near-threshold exclusion)."""
+    the smallest |distance - threshold| over every existing threshold of every pair. The pairs are measured as the
+    kernels measure them in a molecule of these n atoms (br.pair_dist_pm)."""
     x = np.asarray(x, np.float32)
     types = np.asarray(types)
     n = len(types)
     if n == 0:
         return np.zeros((0, 0), np.int64), np.inf
-    d = dist_pm(x[:, None, :], x[None, :, :])
-    lo, hi = np.minimum(types[:, None], types[None, :]), np.maximum(types[:, None], types[None, :])
-    t1, t2, t3 = [np.asarray(t, np.float32)[lo, hi] for t in thr]
-    b1 = (t1 >= 0) & (d < t1)
-    b2 = b1 & (t2 >= 0) & (d < t2)
-    b3 = b2 & (t3 >= 0) & (d < t3)
-    o = b1.astype(np.int64) + b2 + b3
-    np.fill_diagonal(o, 0)
+    d = br.pair_dist_pm(x)
+    t1, t2, t3 = br.threshold_lookup(types, thr)
+    o = br.orders_of(d, types, thr)
     near = np.inf
     off = ~np.eye(n, dtype=bool)
     for t in (t1, t2, t3):

@@ -18,6 +18,7 @@ from difflinker_b200 import _native, molecule_builder as mb, output, synthetic
 from difflinker_b200.batching import collate
 from difflinker_b200.ddpm import sampler_inputs
 from difflinker_b200.edm import retry_seed, seeds_tensor
+from oracle import bond_rounding as br
 import dl_helpers as helpers
 import test_connected_resampling as tcr
 
@@ -25,14 +26,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def dist_pm(xi, xj):
-    """100 |xi - xj| in fp32, each operation rounded on its own."""
-    d = np.asarray(xi, np.float32) - np.asarray(xj, np.float32)
-    return np.float32(100) * np.sqrt((d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2])
+    """100 |xi - xj| in fp32 in the direct form the clash check measures every pair in, at any atom count
+    (sqrt(fma(dz, dz, fma(dy, dy, dx * dx))), oracle/bond_rounding.py)."""
+    return br.direct_dist_pm(xi, xj)
 
 
 def oracle_clashes(x, types, node_mask, linker_mask, pocket_only, table):
-    """The oracle for one molecule: (N,) int64 counts of the pocket atoms each linker atom clashes with (0 elsewhere), and
-    the matrix of linker x pocket distances minus thresholds (for the near-threshold exclusion)."""
+    """The oracle for one molecule: (N,) int64 counts of the pocket atoms each linker atom clashes with (0 elsewhere)."""
     x = np.asarray(x, np.float32)
     types = np.asarray(types)
     live = np.asarray(node_mask) != 0
@@ -41,31 +41,27 @@ def oracle_clashes(x, types, node_mask, linker_mask, pocket_only, table):
     table = np.asarray(table, np.float32)
     li, pi = np.nonzero(linker)[0], np.nonzero(pocket)[0]
     counts = np.zeros(x.shape[0], np.int64)
-    margin = np.full((len(li), len(pi)), np.inf, np.float32)
     if len(li) and len(pi):
         d = dist_pm(x[li][:, None, :], x[pi][None, :, :])
         t = table[np.minimum(types[li][:, None], types[pi][None, :]), np.maximum(types[li][:, None], types[pi][None, :])]
         hit = (t >= 0) & (d < t)                                          # a NaN distance compares false
         counts[li] = hit.sum(1)
-        margin = np.where(t >= 0, np.abs(d - t), np.inf)
-    return counts, margin
+    return counts
 
 
 def oracle_batch(xh, nm, lm, po, is_geom, table=None):
-    """((B,N) counts, (B,) clash-free, (B,) min |distance - threshold|) of a chain[0]-style batch."""
+    """((B,N) counts, (B,) clash-free) of a chain[0]-style batch."""
     T = 9 if is_geom else 8
     table = mb.clash_table(is_geom) if table is None else table
     xh = xh.cpu()
     types = torch.argmax(xh[:, :, 3:3 + T], dim=2).numpy()
-    counts, ok, near = [], [], []
+    counts, ok = [], []
     for b in range(xh.shape[0]):
-        c, m = oracle_clashes(xh[b, :, :3].numpy(), types[b], nm[b].cpu().numpy(), lm[b].cpu().numpy(),
+        c = oracle_clashes(xh[b, :, :3].numpy(), types[b], nm[b].cpu().numpy(), lm[b].cpu().numpy(),
                               po[b].cpu().numpy(), table.numpy())
         counts.append(torch.from_numpy(c))
         ok.append(not c.any())
-        m = m[~np.isnan(m)]                                              # NaN distances: no clash, nothing near
-        near.append(float(m.min()) if m.size else np.inf)
-    return torch.stack(counts), torch.tensor(ok), near
+    return torch.stack(counts), torch.tensor(ok)
 
 
 # ---- CPU --------------------------------------------------------------------------------------------------------------
@@ -108,11 +104,11 @@ def test_oracle_on_pairs_either_side_of_every_threshold():
                     x = np.array([[0, 0, 0], [d, 0, 0]], np.float32)
                     # the linker atom may be either type of the pair: the table is read [min][max]
                     for types in ((a, b), (b, a)):
-                        c, _ = oracle_clashes(x, np.array(types), [1, 1], [1, 0], [0, 1], table)
+                        c = oracle_clashes(x, np.array(types), [1, 1], [1, 0], [0, 1], table)
                         assert c.tolist() == [int(inside), 0], (is_geom, a, b, inside)
     table = mb.clash_table(False).clone()
     table[0, 0] = -1.0                                                   # a negative entry: the pair never clashes
-    c, _ = oracle_clashes(np.zeros((2, 3), np.float32), np.array([0, 0]), [1, 1], [1, 0], [0, 1], table)
+    c = oracle_clashes(np.zeros((2, 3), np.float32), np.array([0, 0]), [1, 1], [1, 0], [0, 1], table)
     assert c.tolist() == [0, 0]
 
 
@@ -262,7 +258,7 @@ def run_clash(xh, nm, lm, po, is_geom, table=None):
 
 def assert_matches_oracle(xh, nm, lm, po, is_geom, table=None):
     ok, counts = run_clash(xh, nm, lm, po, is_geom, table)
-    want_counts, want_ok, _ = oracle_batch(xh, nm, lm, po, is_geom, table)
+    want_counts, want_ok = oracle_batch(xh, nm, lm, po, is_geom, table)
     assert torch.equal(counts.long(), want_counts)
     assert torch.equal(ok, want_ok)
     return ok, counts
@@ -378,8 +374,7 @@ def test_a_linker_in_a_whole_protein_pocket(N):
 @pytest.mark.gpu
 @pytest.mark.parametrize("is_geom", [False, True])
 def test_kernel_matches_the_oracle_on_random_batches(is_geom):
-    """Random ligands in random pockets; molecules with a pair within 0.01 pm of its threshold are left out of the
-    comparison (the device may contract the fp32 distance differently)."""
+    """Random ligands in random pockets, every molecule compared: the oracle measures in the kernel's direct form."""
     T = 9 if is_geom else 8
     g = torch.Generator().manual_seed(11)
     B, N = 128, 60
@@ -391,11 +386,9 @@ def test_kernel_matches_the_oracle_on_random_batches(is_geom):
     xh = torch.cat([torch.rand(B, N, 3, generator=g) * scale,
                     torch.nn.functional.one_hot(torch.randint(0, T, (B, N), generator=g), T).float()], 2)
     ok, counts = run_clash(xh, nm, lm, po, is_geom)
-    want_counts, want_ok, near = oracle_batch(xh, nm, lm, po, is_geom)
-    keep = [b for b in range(B) if near[b] > 0.01]
-    assert len(keep) > B * 0.9, len(keep)
-    assert torch.equal(counts[keep].long(), want_counts[keep]) and torch.equal(ok[keep], want_ok[keep])
-    assert 0 < int(want_ok[keep].sum()) < len(keep), int(want_ok.sum())  # both outcomes are exercised
+    want_counts, want_ok = oracle_batch(xh, nm, lm, po, is_geom)
+    assert torch.equal(counts.long(), want_counts) and torch.equal(ok, want_ok)
+    assert 0 < int(want_ok.sum()) < B, int(want_ok.sum())              # both outcomes are exercised
 
 
 # ---- GPU: the sampler, end to end ---------------------------------------------------------------------------------------
@@ -453,7 +446,7 @@ def oracle_rows(ddpm, kw, chain0):
     """(B,) clash-free of a returned chain[0], by the host oracle and by molecule_builder.clash_free (which must agree)."""
     B, N = chain0.shape[:2]
     nm, lm, po = kw['node_mask'].reshape(B, N), kw['linker_mask'].reshape(B, N), kw['context'][..., -1].reshape(B, N)
-    _, want, _ = oracle_batch(chain0, nm, lm, po, ddpm.edm.is_geom)
+    _, want = oracle_batch(chain0, nm, lm, po, ddpm.edm.is_geom)
     got = mb.clash_free(chain0, nm, lm, po, ddpm.edm.is_geom).cpu()
     assert torch.equal(got, want)
     return want

@@ -103,6 +103,78 @@ def test_oracle_bond_orders_match_reference_golden(name):
     assert (t1[lower] == -1).all()                                           # only the index-ordered direction is ever read
 
 
+def test_oracle_and_emulation_match_reference_threshold_golden():
+    """tests/golden/bonds_thresholds.npz: the live reference's build_xae_molecule on molecules built around one pair each
+    whose bond decision differs between torch.cdist's direct (n <= 25) and matmul (n > 25) forms. The emulation of the
+    kernels' arithmetic (oracle/bond_rounding.py) and oracle.xae_molecule (live torch.cdist, the reference's dists[i, j],
+    i > j, and strict '<' against the tables) must give the fixture's E on every pair except the ambiguous ones -- where
+    the emulation's decision differs from the fixture's, which the one-ulp CPU square root leaves -- and those stay below 1%
+    of the molecules. Up to 25 atoms nothing is ambiguous."""
+    from difflinker_b200 import molecule_builder as mb, output
+    from oracle import bond_rounding as br
+    meta, a = helpers.load_golden("bonds_thresholds")
+    ao, eo = a["atom_offsets"].numpy(), a["E_offsets"].numpy()
+    M = len(ao) - 1
+    counts = {}
+    amb_mols, bad = 0, []
+    for m in range(M):
+        is_geom = bool(a["is_geom"][m])
+        group = meta["groups"][int(a["group"][m])]
+        x = a["positions"][ao[m]:ao[m + 1]].numpy()
+        ty = a["types"][ao[m]:ao[m + 1]].numpy().astype(np.int64)
+        n = len(x)
+        lo = np.tril_indices(n, -1)
+        want = a["E_lower"][eo[m]:eo[m + 1]].numpy().astype(np.int64)
+        thr = [t.numpy() for t in mb.threshold_tables(is_geom)]
+        mine = br.bond_orders(x, ty, thr)[lo]
+        idx2atom = output.GEOM_IDX2ATOM if is_geom else output.IDX2ATOM
+        _, A, E = orc.xae_molecule(torch.from_numpy(x), torch.from_numpy(ty), idx2atom, mb.SINGLE, mb.DOUBLE, mb.TRIPLE,
+                                   mb.MARGINS_EDM)
+        live = E.numpy()[lo]
+        amb = mine != want
+        if n <= br.CDIST_MM_ROWS and amb.any():
+            bad.append(f"molecule {m} ({group}, n={n}): the direct form differs from the reference on {int(amb.sum())} pairs")
+        if (live != want)[~amb].any():
+            bad.append(f"molecule {m} ({group}, n={n}): oracle.xae_molecule differs from the reference off the ambiguous pairs")
+        amb_mols += bool(amb.any())
+        counts[group] = counts.get(group, 0) + 1
+    assert not bad, "\n".join(bad[:40])
+    print(f"bonds_thresholds: {M} molecules {counts}, {amb_mols} with an ambiguous pair")
+    assert counts["designed"] >= 700 and counts["twin25"] == counts["twin26"] > 0
+    assert amb_mols <= 0.01 * M
+
+
+def test_reference_decides_the_designed_pairs_by_atom_count():
+    """In the fixture, the reference's E of each 25-atom twin is the direct form's and differs from its 26-atom twin's; a
+    pocket design's ligand alone and with its pocket rows, and a linker design whole and alone, differ too."""
+    meta, a = helpers.load_golden("bonds_thresholds")
+    ao, eo, groups = a["atom_offsets"].numpy(), a["E_offsets"].numpy(), meta["groups"]
+    g = [groups[int(k)] for k in a["group"]]
+
+    def E(m, n_keep):
+        n = ao[m + 1] - ao[m]
+        full = np.zeros((n, n), np.int64)
+        full[np.tril_indices(n, -1)] = a["E_lower"][eo[m]:eo[m + 1]].numpy()
+        return full[:n_keep, :n_keep]
+
+    pairs = [(m, m + 1) for m in range(len(g) - 1) if g[m] == "twin25" and g[m + 1] == "twin26"]
+    pairs += [(m + 1, m) for m in range(len(g) - 1) if g[m] == "pocket_all" and g[m + 1] == "pocket_dropped"]
+    assert len(pairs) > 20
+    for small, big in pairs:
+        n = ao[small + 1] - ao[small]
+        assert not np.array_equal(E(small, n), E(big, n)), (g[small], small)
+    linker = [m for m in range(len(g) - 1) if g[m] == "linker_whole" and g[m + 1] == "linker_alone"]
+    assert linker
+    for m in linker:
+        n_alone = ao[m + 2] - ao[m + 1]
+        x_whole, x_alone = a["positions"][ao[m]:ao[m + 1]].numpy(), a["positions"][ao[m + 1]:ao[m + 2]].numpy()
+        rows = [int(np.flatnonzero((x_whole == r).all(1))[0]) for r in x_alone]
+        n = ao[m + 1] - ao[m]
+        full = np.zeros((n, n), np.int64)
+        full[np.tril_indices(n, -1)] = a["E_lower"][eo[m]:eo[m + 1]].numpy()
+        assert not np.array_equal(full[np.ix_(rows, rows)], E(m + 1, n_alone)), m
+
+
 def test_gamma_tables_match_reference_golden():
     _, a = helpers.load_golden("gamma_tables")
     for key, ref in a.items():
