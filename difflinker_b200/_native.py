@@ -101,10 +101,12 @@ SYMBOLS = {
     "dl_last_retry_ms": (_F, [_P]),
     "dl_set_noise_slice": (_I32, [_P, _I32, _I32]),
     "dl_set_start_step": (_I32, [_P, _I32, _F, _F]),
+    "dl_set_start_steps": (_I32, [_P, _I32, _P, _P, _P]),
     "dl_noise_fill": (_I32, [_P, _I32, _I32, _I32, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "dl_noise_fill_inpaint": (_I32, [_P, _I32, _I32, _I32, _P, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "dl_sample_chain_host": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "dl_launch_count": (_I64, [_P]),
+    "dl_last_molecule_steps": (_I64, [_P]),
     "dl_last_elapsed_ms": (_F, [_P]),
     "dl_time_edge_kernel": (_F, [_P, _I32]),
     "dl_selftest_tc": (_I32, [_P, C.POINTER(_F), C.POINTER(_F)]),

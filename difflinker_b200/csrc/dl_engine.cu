@@ -120,6 +120,11 @@ struct dl_engine {
   // dl_set_start_step: the linker sampler starts at step start_step from q(z_t0 | x) with these scalars; -1: from noise at T
   int start_step = -1;
   float start_alpha = 0.f, start_sigma = 0.f;
+  // dl_set_start_steps: molecule b of the following calls starts at step starts_t0[b] with its own scalars; empty: none
+  std::vector<int32_t> starts_t0;
+  std::vector<float> starts_alpha, starts_sigma;
+  HostStage start_rows;        // a per-molecule start-step call's row order, lags, scalars and gathered inputs
+  int64_t mol_steps = 0;       // dl_last_molecule_steps
   bool finalized = false;
   std::map<std::string, std::vector<float>> raw;
   float* wblob = nullptr;      // packed fp32 weights
@@ -384,6 +389,7 @@ struct FwdIO {
   const float* fragment_mask = nullptr; const float* noise = nullptr; float* chain = nullptr;
   NoiseRng rng{};
   int T = 0; float norm0 = 1.f, norm1 = 1.f, bias1 = 0.f;
+  RowStarts rows{};   // per-molecule start steps, or rows.lag = null
 };
 
 ProjW proj_of(const EdgeMlpW& w) { return ProjW{w.W1a_t, w.W1b_t, w.b1}; }
@@ -576,7 +582,7 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
   if (fused_update) {
     fa.z = ws.z; fa.fragment_mask = io.fragment_mask; fa.linker_mask = io.linker_mask; fa.noise = io.noise; fa.rng = io.rng;
     fa.coef = e->coef_dev; fa.step_fin = e->step_ctr + 1; fa.step_prep = e->step_ctr; fa.T = io.T;
-    fa.norm0 = io.norm0; fa.norm1 = io.norm1; fa.bias1 = io.bias1; fa.chain = io.chain;
+    fa.norm0 = io.norm0; fa.norm1 = io.norm1; fa.bias1 = io.bias1; fa.chain = io.chain; fa.rows = io.rows;
   } else if (io.sampler) {
     fa.tag_step = e->step_ctr + 1;
   }
@@ -686,7 +692,11 @@ uint64_t sampler_draws(int sampler, int T) { return sampler == DL_SAMPLER_INPAIN
 
 // Reverse steps of a call before the final one: the start step when one is set (dl_set_start_step), else T. The loop then
 // runs the last loop_steps + 1 rows of the coefficient table as a chain of that length, so it also sets the draws.
-int loop_steps(const dl_engine* e, int T) { return e && e->start_step >= 0 ? e->start_step : T; }
+// With per-molecule start steps (dl_set_start_steps) the loop runs from the largest.
+int loop_steps(const dl_engine* e, int T) {
+  if (e && !e->starts_t0.empty()) return *std::max_element(e->starts_t0.begin(), e->starts_t0.end());
+  return e && e->start_step >= 0 ? e->start_step : T;
+}
 
 // While alive, the engine's loop runs on the sub-batch workspace and records its loop time on the ev_r* events: the
 // full batch's workspace, the first loop's dl_last_elapsed_ms and the forward state dl_time_edge_kernel replays stay put.
@@ -695,14 +705,79 @@ struct SubBatchScope {
   const int8_t* edge_mask;
   const float* linker_mask;
   int B, N;
+  int64_t mol_steps;
   explicit SubBatchScope(dl_engine* e_)
-      : e(e_), edge_mask(e_->last_edge_mask), linker_mask(e_->last_linker_mask), B(e_->last_B), N(e_->last_N) { swap(); }
+      : e(e_), edge_mask(e_->last_edge_mask), linker_mask(e_->last_linker_mask), B(e_->last_B), N(e_->last_N),
+        mol_steps(e_->mol_steps) { swap(); }
   ~SubBatchScope() {
     swap();
     e->last_edge_mask = edge_mask; e->last_linker_mask = linker_mask; e->last_B = B; e->last_N = N;
+    e->mol_steps = mol_steps;
   }
   void swap() { std::swap(e->ws, e->ws_sub); std::swap(e->ev_t0, e->ev_r0); std::swap(e->ev_t1, e->ev_r1); }
 };
+
+// The rows of a call with per-molecule start steps (dl_set_start_steps) in the engine's order: the caller's rows stably
+// sorted by t0 descending, so that the rows a loop step computes -- those that have started -- are a prefix.
+struct RowOrder {
+  const float *xh, *fragment_mask, *linker_mask, *context, *alpha, *sigma;
+  const int8_t *node_mask, *edge_mask;
+  RowStarts rs;
+  std::vector<int> active;   // (Tl + 1) the length of the prefix loop step r computes
+};
+
+// Orders the B rows of a loop of Tl + 1 steps, stages the order, lags and scalars, and gathers the inputs (and with
+// per-molecule streams the seeds, into the workspace) in that order with the recovery rounds' gather.
+dl_status order_rows(dl_engine* e, int B, int N, int Tl, const float* xh, const int8_t* node_mask, const float* fragment_mask,
+                     const float* linker_mask, const int8_t* edge_mask, const float* context, const unsigned long long* seeds,
+                     cudaStream_t st, RowOrder& ro) {
+  const std::vector<int32_t>& t0 = e->starts_t0;
+  std::vector<int> order(B), lag(B);
+  std::vector<float> al(B), sg(B);
+  for (int b = 0; b < B; ++b) order[b] = b;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return t0[a] > t0[b]; });
+  for (int i = 0; i < B; ++i) {
+    lag[i] = Tl - t0[order[i]]; al[i] = e->starts_alpha[order[i]]; sg[i] = e->starts_sigma[order[i]];
+  }
+  // row i has started at loop step r (step Tl - 1 - r) once t0 > Tl - 1 - r, i.e. lag[i] <= r; lag ascends along the order
+  ro.active.resize(Tl + 1);
+  for (int r = 0; r <= Tl; ++r) ro.active[r] = (int)(std::upper_bound(lag.begin(), lag.end(), r) - lag.begin());
+  const bool fc_em = edge_mask && e->cfg.graph_type == DL_GRAPH_FC;
+  const int xd = 3 + e->cfg.in_node_nf, C = e->cfg.context_node_nf;
+  const size_t n = (size_t)B * N;
+  StageLayout sl;
+  const int i_src = sl.in(order.data(), B * sizeof(int)), i_lag = sl.in(lag.data(), B * sizeof(int)),
+            i_al = sl.in(al.data(), B * sizeof(float)), i_sg = sl.in(sg.data(), B * sizeof(float)), i_xh = sl.out(n * xd * 4),
+            i_nm = sl.out(n), i_fm = sl.out(n * 4), i_lm = sl.out(n * 4), i_em = sl.add(nullptr, n * N, fc_em),
+            i_ctx = sl.add(nullptr, n * C * 4, context != nullptr && C > 0);
+  dl_status s = stage_inputs(e->start_rows, sl, st);
+  if (s != DL_OK) return s;
+  RowGatherArgs ga{};
+  ga.rows = sl.at<const int>(i_src); ga.N = N; ga.xd = xd; ga.C = C; ga.attempt = 0;
+  ga.xh = xh; ga.fragment_mask = fragment_mask; ga.linker_mask = linker_mask; ga.context = sl.at<float>(i_ctx) ? context : nullptr;
+  ga.node_mask = node_mask; ga.edge_mask = fc_em ? edge_mask : nullptr; ga.seeds = seeds;
+  ga.s_xh = sl.at<float>(i_xh); ga.s_fragment_mask = sl.at<float>(i_fm); ga.s_linker_mask = sl.at<float>(i_lm);
+  ga.s_context = sl.at<float>(i_ctx); ga.s_node_mask = sl.at<int8_t>(i_nm); ga.s_edge_mask = sl.at<int8_t>(i_em);
+  ga.s_seeds = e->ws.seeds;
+  k_gather_rows<false><<<B, 256, 0, st>>>(ga);
+  LAUNCH_CHECK();
+  e->launches += 1;
+  ro.xh = ga.s_xh; ro.fragment_mask = ga.s_fragment_mask; ro.linker_mask = ga.s_linker_mask; ro.context = ga.s_context;
+  ro.node_mask = ga.s_node_mask; ro.edge_mask = ga.s_edge_mask;
+  ro.alpha = sl.at<const float>(i_al); ro.sigma = sl.at<const float>(i_sg);
+  ro.rs = RowStarts{sl.at<const int>(i_lag), sl.at<const int>(i_src), (int)n};
+  return DL_OK;
+}
+
+// Captures one reverse step over the first Bp rows of the workspace into *graph.
+dl_status capture_step(dl_engine* e, int Bp, int N, const FwdIO& io, cudaStream_t st, cudaGraph_t* graph) {
+  CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  const dl_status s = enqueue_forward(e, Bp, N, io, st);
+  const cudaError_t ce = cudaStreamEndCapture(st, graph);
+  if (s != DL_OK) { if (*graph) cudaGraphDestroy(*graph); *graph = nullptr; return s; }
+  if (ce != cudaSuccess) { set_err("cudaStreamEndCapture -> %s", cudaGetErrorString(ce)); return DL_ERR_CUDA; }
+  return DL_OK;
+}
 
 }  // namespace
 
@@ -781,6 +856,7 @@ dl_status dl_destroy(dl_engine* e) {
   free_workspace(e->ws);
   free_workspace(e->ws_sub);
   if (e->sub_rows.buf) cudaFree(e->sub_rows.buf);
+  if (e->start_rows.buf) cudaFree(e->start_rows.buf);
   if (e->hashes.buf) cudaFree(e->hashes.buf);
   if (e->wblob) cudaFree(e->wblob);
   if (e->wblob_tc) cudaFree(e->wblob_tc);
@@ -950,6 +1026,11 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
   if (s == DL_OK) s = check_slice(e, B);
   if (s != DL_OK) return s;
   if (offset % 4 != 0) { set_err("philox offset must be a multiple of 4 (torch.Generator.get_offset())"); return DL_ERR_INVALID; }
+  if (!e->starts_t0.empty()) {
+    set_err("dl_sample_chain_rng: the batch stream's draws are not per molecule, so it takes no per-molecule start steps "
+            "(dl_set_start_steps): use dl_sample_chain_seeded or a noise tensor");
+    return DL_ERR_INVALID;
+  }
   const NoiseRng q = make_rng(e, B, N, seed, offset);
   if (offset_consumed) *offset_consumed = sampler_draws(sampler, loop_steps(e, T)) * q.per_draw;
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, nullptr,
@@ -982,6 +1063,23 @@ dl_status dl_set_start_step(dl_engine* e, int32_t t0, float alpha_t0, float sigm
   if (t0 < 0) { e->start_step = -1; e->start_alpha = e->start_sigma = 0.f; return DL_OK; }
   if (!std::isfinite(alpha_t0) || !std::isfinite(sigma_t0)) { set_err("alpha_t0 and sigma_t0 must be finite"); return DL_ERR_INVALID; }
   e->start_step = t0; e->start_alpha = alpha_t0; e->start_sigma = sigma_t0;
+  e->starts_t0.clear(); e->starts_alpha.clear(); e->starts_sigma.clear();
+  return DL_OK;
+}
+
+dl_status dl_set_start_steps(dl_engine* e, int32_t B, const int32_t* t0, const float* alpha, const float* sigma) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  if (B < 0) { set_err("dl_set_start_steps: B must be >= 0 (got %d)", B); return DL_ERR_INVALID; }
+  if (B > 0 && (!t0 || !alpha || !sigma)) { set_err("dl_set_start_steps: null t0, alpha or sigma"); return DL_ERR_INVALID; }
+  for (int b = 0; b < B; ++b) {
+    if (t0[b] < 0) { set_err("dl_set_start_steps: t0[%d] = %d is negative", b, t0[b]); return DL_ERR_INVALID; }
+    if (!std::isfinite(alpha[b]) || !std::isfinite(sigma[b])) {
+      set_err("dl_set_start_steps: alpha[%d] and sigma[%d] must be finite", b, b);
+      return DL_ERR_INVALID;
+    }
+  }
+  e->starts_t0.assign(t0, t0 + B); e->starts_alpha.assign(alpha, alpha + B); e->starts_sigma.assign(sigma, sigma + B);
+  e->start_step = -1; e->start_alpha = e->start_sigma = 0.f;
   return DL_OK;
 }
 
@@ -1027,8 +1125,18 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   if (s != DL_OK) return s;
   const bool inpaint = sampler == DL_SAMPLER_INPAINT;
   const bool partial = e->start_step >= 0;
+  const bool per_row = !e->starts_t0.empty();   // per-molecule start steps (dl_set_start_steps)
   if (partial && inpaint) { set_err("the inpainting sampler takes no start step (dl_set_start_step)"); return DL_ERR_INVALID; }
   if (partial && e->start_step > T) { set_err("start step %d exceeds T = %d", e->start_step, T); return DL_ERR_INVALID; }
+  if (per_row) {
+    if ((int)e->starts_t0.size() != B) {
+      set_err("per-molecule start steps were set for %d molecules; the call samples %d", (int)e->starts_t0.size(), B);
+      return DL_ERR_INVALID;
+    }
+    if (inpaint) { set_err("the inpainting sampler takes no start steps (dl_set_start_steps)"); return DL_ERR_INVALID; }
+    if (rng && !per_mol) { set_err("the batch stream takes no per-molecule start steps"); return DL_ERR_INVALID; }
+    if (loop_steps(e, T) > T) { set_err("start step %d exceeds T = %d", loop_steps(e, T), T); return DL_ERR_INVALID; }
+  }
   // A start step t0 runs the table's last t0 + 1 rows -- steps t0-1 .. 0, then the final one -- as a loop of Tl = t0 steps:
   // loop step r reads row r of the copied rows and draw r + 1, so the draws are eps, one per step and the final one.
   const int Tl = loop_steps(e, T);
@@ -1056,9 +1164,19 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   }
   CK(cudaMemcpyAsync(e->coef_dev, coef, (size_t)(Tl + 1) * sizeof(dl_step_coef), cudaMemcpyHostToDevice, st));
   NoiseRng q = rng ? *rng : NoiseRng{};
+  // per-molecule start steps: the loop runs on the rows in start-step order, each loop step on those that have started
+  RowOrder ro{};
+  if (per_row) {
+    s = order_rows(e, B, N, Tl, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, per_mol ? rng->seeds : nullptr,
+                   st, ro);
+    if (s != DL_OK) return s;
+    xh = ro.xh; node_mask = ro.node_mask; fragment_mask = ro.fragment_mask; linker_mask = ro.linker_mask;
+    edge_mask = ro.edge_mask; context = ro.context;
+  }
   if (per_mol) {
     // the captured step reads the engine's copy: the caller's seeds buffer is free once the call has been enqueued
-    CK(cudaMemcpyAsync(e->ws.seeds, rng->seeds, (size_t)B * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
+    if (!per_row)
+      CK(cudaMemcpyAsync(e->ws.seeds, rng->seeds, (size_t)B * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
     q.seeds = e->ws.seeds;
   }
   CK(cudaMemsetAsync(e->step_ctr, 0, 2 * sizeof(int), st));
@@ -1076,6 +1194,11 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   } else if (inpaint) {
     // the caller's slab 0 is already masked and projected
     CK(cudaMemcpyAsync(e->ws.z, noise, (size_t)n * xd * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  } else if (per_row) {
+    if (per_mol) k_init_z_rows<true><<<(n * xd + 255) / 256, 256, 0, st>>>(n, N, xd, xh, fragment_mask, linker_mask, noise, q, ro.alpha, ro.sigma, ro.rs, e->ws.z);
+    else k_init_z_rows<false><<<(n * xd + 255) / 256, 256, 0, st>>>(n, N, xd, xh, fragment_mask, linker_mask, noise, q, ro.alpha, ro.sigma, ro.rs, e->ws.z);
+    LAUNCH_CHECK();
+    e->launches += 1;
   } else if (partial) {
     const float al = e->start_alpha, sg = e->start_sigma;
     if (per_mol) k_init_z_partial<true><<<(n * xd + 255) / 256, 256, 0, st>>>(n, xd, xh, fragment_mask, linker_mask, noise, q, al, sg, e->ws.z);
@@ -1089,7 +1212,8 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     e->launches += 1;
   }
   // inpainting: the dynamics see linker_mask=None (edm.py:632), so every live row gets a coordinate update
-  if ((s = build_forward_plan(e, B, N, node_mask, inpaint ? nullptr : linker_mask, edge_mask, st)) != DL_OK) return s;
+  int Bp = per_row ? ro.active[0] : B;   // the rows the current step graph computes
+  if ((s = build_forward_plan(e, Bp, N, node_mask, inpaint ? nullptr : linker_mask, edge_mask, st)) != DL_OK) return s;
 
   if (time_chain) { cudaStreamSynchronize(st); tc_plan = now_ms(); }
   FwdIO io;
@@ -1098,16 +1222,14 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   io.context = context; io.nan_flags = nan_flags; io.fragment_mask = fragment_mask; io.noise = noise;
   io.rng = q;
   io.chain = chain; io.T = Tl; io.norm0 = norm[0]; io.norm1 = norm[1]; io.bias1 = norm[2];
+  io.rows = per_row ? ro.rs : RowStarts{};
 
-  // capture ONE reverse step; the step index lives on the device, so the same graph serves all Tl+1 steps
+  // capture ONE reverse step; the step index lives on the device, so the same graph serves all Tl+1 steps -- with
+  // per-molecule start steps, all steps of one prefix length: the graph is recaptured whenever the prefix grows
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t exec = nullptr;
   const int64_t before = e->launches;
-  CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-  s = enqueue_forward(e, B, N, io, st);
-  cudaError_t ce = cudaStreamEndCapture(st, &graph);
-  if (s != DL_OK) { if (graph) cudaGraphDestroy(graph); return s; }
-  if (ce != cudaSuccess) { set_err("cudaStreamEndCapture -> %s", cudaGetErrorString(ce)); return DL_ERR_CUDA; }
+  if ((s = capture_step(e, Bp, N, io, st, &graph)) != DL_OK) return s;
   const int64_t per_step = e->launches - before;
   // every exit below releases the captured graph and its executable (destruction is deferred by the runtime until the
   // launched work has finished)
@@ -1116,9 +1238,30 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   if (time_chain) tc_inst = now_ms();
   if (ge == cudaSuccess) ge = cudaEventRecord(e->ev_t0, st);
   int failed_step = -1;
+  int64_t mol_steps = 0, replans = 0;
   for (int r = 0; ge == cudaSuccess && r <= Tl; ++r) {
+    if (per_row && ro.active[r] != Bp) {
+      // more rows have started: their plan and step graph, which replaces the executable's (or a new one)
+      Bp = ro.active[r];
+      ++replans;
+      cudaGraph_t next = nullptr;
+      s = build_forward_plan(e, Bp, N, node_mask, linker_mask, edge_mask, st);
+      if (s == DL_OK) s = capture_step(e, Bp, N, io, st, &next);
+      if (s != DL_OK) { cudaGraphExecDestroy(exec); cudaGraphDestroy(graph); return s; }
+      cudaGraphDestroy(graph);
+      graph = next;
+      cudaGraphExecUpdateResultInfo info;
+      if (cudaGraphExecUpdate(exec, graph, &info) != cudaSuccess) {
+        cudaGetLastError();
+        cudaGraphExecDestroy(exec);
+        exec = nullptr;
+        ge = cudaGraphInstantiate(&exec, graph, 0);
+        if (ge != cudaSuccess) break;
+      }
+    }
     ge = cudaGraphLaunch(exec, st);
     if (ge != cudaSuccess) failed_step = r;
+    mol_steps += Bp;
   }
   if (ge == cudaSuccess) ge = cudaEventRecord(e->ev_t1, st);
   if (time_chain) {
@@ -1140,7 +1283,8 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     else set_err("%s:%d reverse-loop graph -> %s", __FILE__, __LINE__, cudaGetErrorString(ge));
     return DL_ERR_CUDA;
   }
-  e->launches = before + per_step * (Tl + 1);
+  e->launches = before + per_step * (Tl + 1) + 2 * replans;
+  e->mol_steps = mol_steps;
   return DL_OK;
 }
 
@@ -1392,12 +1536,23 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     }
     LAUNCH_CHECK();
     e->launches += 1;
+    // with per-molecule start steps, the sub-batch carries each failing row's step and scalars
+    std::vector<int32_t> t0_all;
+    std::vector<float> alpha_all, sigma_all;
+    const bool per_row = !e->starts_t0.empty();
+    if (per_row) {
+      t0_all.swap(e->starts_t0); alpha_all.swap(e->starts_alpha); sigma_all.swap(e->starts_sigma);
+      for (int b : rows) {
+        e->starts_t0.push_back(t0_all[b]); e->starts_alpha.push_back(alpha_all[b]); e->starts_sigma.push_back(sigma_all[b]);
+      }
+    }
     {
       SubBatchScope sub(e);
       s = dl_sample_chain_seeded(e, sampler, Bs, N, T, keep_frames, ga.s_xh, ga.s_node_mask, ga.s_fragment_mask,
                                  ga.s_linker_mask, ga.s_edge_mask, ga.s_context, reinterpret_cast<const uint64_t*>(ga.s_seeds),
                                  coef, norm, sl.at<float>(i_ch), sl.at<int32_t>(i_fl), stream);
     }
+    if (per_row) { e->starts_t0.swap(t0_all); e->starts_alpha.swap(alpha_all); e->starts_sigma.swap(sigma_all); }
     if (s != DL_OK) return s;
     RowScatterArgs sa{};
     sa.rows = ga.rows; sa.B = B; sa.Bs = Bs; sa.N = N; sa.xd = xd; sa.attempt = a;
@@ -1468,6 +1623,8 @@ dl_status retry_entry(const char* name, dl_engine* e, int32_t sampler, int32_t B
     why = "linker_hash needs checks with DL_CHECK_NOVEL";
   if (!why && sets && !checks) why = "sets need checks: the known set is read with DL_CHECK_NOVEL, the seen set with "
                                      "DL_CHECK_UNIQUE";
+  if (!why && redraw && !e->starts_t0.empty())
+    why = "a size redraw takes no start steps: partial diffusion varies the batch's own linker, whose size is given";
   if (!why && redraw) {
     if (cudaSetDevice(e->cfg.device) != cudaSuccess) why = "cudaSetDevice failed";
     else why = redraw_error(sampler, B, N, redraw, reinterpret_cast<cudaStream_t>(stream));
@@ -1610,6 +1767,8 @@ dl_status dl_clash_check(int32_t B, int32_t N, int32_t n_types, const float* cla
 float dl_last_retry_ms(dl_engine* e) { return e ? e->retry_ms : -1.f; }
 
 int64_t dl_launch_count(const dl_engine* e) { return e ? e->launches : 0; }
+
+int64_t dl_last_molecule_steps(dl_engine* e) { return e ? e->mol_steps : 0; }
 
 float dl_last_elapsed_ms(dl_engine* e) {
   if (!e) return -1.f;

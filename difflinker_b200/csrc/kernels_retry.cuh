@@ -87,7 +87,7 @@ struct RowGatherArgs {
   int N, xd, C, attempt;
   const float *xh, *fragment_mask, *linker_mask, *context;
   const int8_t *node_mask, *edge_mask;   // edge_mask: FC graphs' (B,N,N) int8 blocks, or null (all ones / cut-off graphs)
-  const unsigned long long* seeds;       // the caller's base seeds
+  const unsigned long long* seeds;       // the caller's base seeds, or null: no seeds to gather
   float *s_xh, *s_fragment_mask, *s_linker_mask, *s_context;
   int8_t *s_node_mask, *s_edge_mask;
   unsigned long long* s_seeds;           // retry_seed(seeds[rows[i]], attempt)
@@ -122,7 +122,7 @@ __global__ void __launch_bounds__(256) k_gather_rows(RowGatherArgs a) {
     for (size_t k = threadIdx.x; k < N * a.C; k += blockDim.x) a.s_context[i * N * a.C + k] = a.context[b * N * a.C + k];
   if (a.edge_mask)
     for (size_t k = threadIdx.x; k < N * N; k += blockDim.x) a.s_edge_mask[i * N * N + k] = a.edge_mask[b * N * N + k];
-  if (threadIdx.x == 0) a.s_seeds[i] = retry_seed(a.seeds[b], a.attempt);
+  if (threadIdx.x == 0 && a.seeds) a.s_seeds[i] = retry_seed(a.seeds[b], a.attempt);
 }
 
 // The resizing gather: warp 0 draws the molecule's size s' with this attempt's seed, then the CTA writes the template of

@@ -875,6 +875,16 @@ __device__ __forceinline__ float noise_draw(const NoiseRng& q, int r, int g, int
   return philox_normal_elem(q.seed, base + q.cx, q.Sh, gg * q.F + (d - 3));
 }
 
+// Per-molecule start steps (dl_set_start_steps): the engine's rows are the caller's, ordered by start step t0 descending,
+// and loop step r computes the prefix of rows that have started. Row i is caller row src[i]; it started lag[i] = t0max - t0
+// steps after the loop did, so its own draw k is loop draw k + lag[i] and its NaN tag counts from its own start. The caller's
+// noise tensor, chain frames and NaN flags keep the caller's n_full = B * N node rows.
+struct RowStarts {
+  const int* lag;
+  const int* src;
+  int n_full;
+};
+
 struct FinishArgs {
   const float* h;        // (B*N,128) final hidden state
   const float* x;        // (B*N,3) final coordinates
@@ -895,6 +905,7 @@ struct FinishArgs {
   float norm0, norm1, bias1;
   float* chain;          // (keep,B*N,3+F)
   const int* tag_step;   // non-sampler mode inside the inpainting loop: step counter used to tag NaN flags (or null)
+  RowStarts rows;        // per-molecule start steps (dl_set_start_steps), or lag = null
 };
 
 template <bool PER_MOL = false>
@@ -923,6 +934,15 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
   } else if (a.tag_step != nullptr) {
     step = *a.tag_step;
   }
+  // this row's draw offset, and node g's row in the caller's noise, chain and flags
+  int lag = 0;
+  size_t gc = g, nc = n_total;
+  if (a.rows.lag != nullptr && g < n_total) {
+    const int b = g / gm.N;
+    lag = a.rows.lag[b];
+    gc = (size_t)a.rows.src[b] * gm.N + (g - b * gm.N);
+    nc = a.rows.n_full;
+  }
   for (int idx = tid; idx < 16 * (H / 4); idx += 256) {
     const int rr = idx / (H / 4), k4 = idx - rr * (H / 4);
     const int gg = blockIdx.x * 16 + rr;
@@ -949,8 +969,8 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
       // bit0: NaN in vel, bit1: NaN in h (utils.py:274-282); bits 8.. = 1 + index of the first failing
       // reverse step. Later steps do not add bits: the reference raises at the first failing step.
       const int bits = d < 3 ? 1 : 2;
-      const int tag = ((a.z != nullptr || a.tag_step != nullptr) ? step + 1 : 0) << 8;
-      int* p = a.nan_flags + g / gm.N;
+      const int tag = ((a.z != nullptr || a.tag_step != nullptr) ? step + 1 - lag : 0) << 8;
+      int* p = a.nan_flags + gc / gm.N;
       const int old = atomicCAS(p, 0, bits | tag);
       if (old != 0 && (old & ~0xff) == tag) atomicOr(p, bits);
     }
@@ -967,8 +987,8 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
     lm = a.linker_mask[g]; fm = a.fragment_mask[g];
     const float zt = a.z[(size_t)g * xd + d];
     const float eps = e * lm;                                                 // edm.py:196 / 225
-    const float nz = (a.rng.on ? noise_draw<PER_MOL>(a.rng, step + 1, g, d)
-                               : a.noise[((size_t)(step + 1) * n_total + g) * xd + d]) * lm;  // utils.py:189-192
+    const float nz = (a.rng.on ? noise_draw<PER_MOL>(a.rng, step + 1 - lag, g, d)
+                               : a.noise[((size_t)(step + 1 - lag) * nc + gc) * xd + d]) * lm;  // utils.py:189-192
     if (step < a.T) {
       float mu = zt / ca - cb * eps;                                          // edm.py:199
       float zs = mu + cc * nz;                                                // edm.py:205, 342-345
@@ -976,7 +996,7 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
       a.z[(size_t)g * xd + d] = znew;
       if (frame >= 0) {
         float o = d < 3 ? znew * a.norm0 : znew * a.norm1 + a.bias1;          // edm.py:352-361
-        a.chain[((size_t)frame * n_total + g) * xd + d] = o;
+        a.chain[((size_t)frame * nc + gc) * xd + d] = o;
       }
     } else {
       float mux = ca * (zt - cb * eps);                                       // edm.py:241 (ca = 1/alpha_0)
@@ -998,7 +1018,7 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
     }
     if (act) {
       float o = d < 3 ? znew * a.norm0 : ((d == best ? 1.f : 0.f) * a.nm[g]);
-      a.chain[(size_t)g * xd + d] = o;                                        // chain[0], edm.py:174
+      a.chain[gc * xd + d] = o;                                               // chain[0], edm.py:174
     }
   }
 }
@@ -1202,6 +1222,22 @@ __global__ void k_init_z_partial(int n_total, int xd, const float* __restrict__ 
   const float l = lm[g], v = xh[idx];
   const float nz = rng.on ? noise_draw<PER_MOL>(rng, 0, g, idx - g * xd) : noise[idx];
   const float zt = __fadd_rn(__fmul_rn(alpha, v), __fmul_rn(sigma, __fmul_rn(nz, l)));
+  z[idx] = __fadd_rn(__fmul_rn(v, fm[g]), __fmul_rn(zt, l));
+}
+
+// k_init_z_partial with per-molecule start steps (dl_set_start_steps): row b of the engine's order starts from its own
+// alpha[b] and sigma[b], and reads draw 0 of a noise tensor at its caller row rows.src[b].
+template <bool PER_MOL = false>
+__global__ void k_init_z_rows(int n_total, int N, int xd, const float* __restrict__ xh, const float* __restrict__ fm,
+                              const float* __restrict__ lm, const float* __restrict__ noise, NoiseRng rng,
+                              const float* __restrict__ alpha, const float* __restrict__ sigma, RowStarts rows,
+                              float* __restrict__ z) {
+  int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_total * xd) return;
+  const int g = idx / xd, b = g / N, d = idx - g * xd;
+  const float l = lm[g], v = xh[idx];
+  const float nz = rng.on ? noise_draw<PER_MOL>(rng, 0, g, d) : noise[((size_t)rows.src[b] * N + (g - b * N)) * xd + d];
+  const float zt = __fadd_rn(__fmul_rn(alpha[b], v), __fmul_rn(sigma[b], __fmul_rn(nz, l)));
   z[idx] = __fadd_rn(__fmul_rn(v, fm[g]), __fmul_rn(zt, l));
 }
 

@@ -205,8 +205,9 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     `require_novel`: ... and the molecules whose linker hash is in `model.edm.known_linkers` (None uses
     `model.edm.require_novel`).
     `start_step` = t0 (partial diffusion, EDM.sample_chain): the template of sample_fn=None with the batch's own linker
-    positions and atom types on its linker rows, sampled from step t0; ValueError with a sample_fn, or when the batch's
-    linker rows do not directly follow its fragment rows.
+    positions and atom types on its linker rows, sampled from step t0 -- or from one step per molecule, a 1-D sequence or
+    integer tensor (EDM.sample_chain); ValueError with a sample_fn, or when the batch's linker rows do not directly follow
+    its fragment rows.
     `linker_sizes` -- a SizeClassifier, a pair (lo, hi) or an int (size_distribution) -- draws molecule b's linker size from
     its own seed (dl_size_draw; `seeds`, or draw_seeds with noise_mode='per_molecule'), builds the template at those sizes
     padded to its capacity N_cap = max n_frag + max(sizes), and makes every recovery round redraw the size of each row it

@@ -41,6 +41,33 @@ class LinkerSizes(NamedTuple):
     linker_x: torch.Tensor
 
 
+class StartSteps(NamedTuple):
+    """Per-molecule start steps of a call (dl_set_start_steps): row b starts at step t0[b] with the scalars alpha[b],
+    sigma[b] of start_scalars(t0[b], B) at the call's own B."""
+    t0: list
+    alpha: list
+    sigma: list
+
+    def rows(self, lo, hi):
+        return StartSteps(self.t0[lo:hi], self.alpha[lo:hi], self.sigma[lo:hi])
+
+    @staticmethod
+    def cat(parts):
+        return StartSteps(*(sum((list(p[i]) for p in parts), []) for i in range(3)))
+
+    def set_on(self, lib, eng):
+        n = len(self.t0)
+        _native.check(lib.dl_set_start_steps(eng, n, (C.c_int32 * n)(*self.t0), (C.c_float * n)(*self.alpha),
+                                             (C.c_float * n)(*self.sigma)), "dl_set_start_steps")
+
+
+def _loop_steps(start):
+    """The step a call's loop starts from: t0 of a scalar start, the largest t0 of per-molecule ones, or None."""
+    if start is None:
+        return None
+    return max(start.t0) if isinstance(start, StartSteps) else start[0]
+
+
 def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
@@ -54,13 +81,19 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     hash sets of CHECK_NOVEL and CHECK_UNIQUE; None is two empty sets. `linker_hashes`, an int64 device tensor or None,
     receives every returned row's linker hash (CHECK_NOVEL).
     `start` = (t0, alpha_t0, sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of
-    the call (dl_set_start_step). Returns (status, what the batch stream consumed)."""
-    if start is not None:
+    the call (dl_set_start_step); a StartSteps starts each row at its own step (dl_set_start_steps). Returns (status, what
+    the batch stream consumed)."""
+    per_row = isinstance(start, StartSteps)
+    if per_row:
+        start.set_on(lib, eng)
+    elif start is not None:
         _native.check(lib.dl_set_start_step(eng, *start), "dl_set_start_step")
     try:
         return _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry)
     finally:
-        if start is not None:
+        if per_row:
+            lib.dl_set_start_steps(eng, 0, None, None, None)
+        elif start is not None:
             lib.dl_set_start_step(eng, -1, 0.0, 0.0)
 
 
@@ -411,25 +444,44 @@ class EDM(torch.nn.Module):
         return float(self.alpha(g)[0]), float(self.sigma(g)[0])
 
     def _start(self, start_step, n_samples):
-        """(t0, alpha_t0, sigma_t0) of a call that starts at step `start_step`, or None for one that starts from noise at T.
-        Raises ValueError unless start_step is an int with 0 <= start_step <= T."""
+        """(t0, alpha_t0, sigma_t0) of a call of n_samples molecules that starts at step `start_step`, or None for one that
+        starts from noise at T; for a 1-D sequence or integer tensor of one step per molecule, their StartSteps, every
+        scalar evaluated at n_samples. Raises ValueError unless every step is an int with 0 <= t0 <= T, and for a sequence
+        of another length."""
         if start_step is None:
             return None
+        if torch.is_tensor(start_step) and start_step.dim() == 1 or isinstance(start_step, (list, tuple, range)):
+            if torch.is_tensor(start_step):
+                if start_step.dtype.is_floating_point or start_step.dtype.is_complex or start_step.dtype == torch.bool:
+                    raise ValueError(f"start_step is a tensor of integer steps (got {start_step.dtype})")
+                start_step = start_step.tolist()
+            t0 = [self._start_step(v) for v in start_step]
+            if len(t0) != n_samples:
+                raise ValueError(f"start_step holds {len(t0)} steps for a batch of {n_samples} molecules")
+            scalars = {t: self.start_scalars(t, n_samples) for t in sorted(set(t0))}
+            return StartSteps(t0, [scalars[t][0] for t in t0], [scalars[t][1] for t in t0])
+        t0 = self._start_step(start_step)
+        return (t0,) + self.start_scalars(t0, n_samples)
+
+    def _start_step(self, v):
+        """v as a start step: an int in [0, T], else ValueError."""
         try:
-            if isinstance(start_step, bool):
+            if isinstance(v, bool):
                 raise TypeError
-            t0 = operator.index(start_step)
+            t0 = operator.index(v)
         except TypeError:
-            raise ValueError(f"start_step is an integer step (got {start_step!r})") from None
+            raise ValueError(f"start_step is an integer step (got {v!r})") from None
         if not 0 <= t0 <= self.T:
             raise ValueError(f"start_step must lie in [0, T = {self.T}] (got {t0})")
-        return (t0,) + self.start_scalars(t0, n_samples)
+        return t0
 
     def _nan_exception(self, flags, start):
         """The FoundNaNException of (B,) NaN flags. The engine tags a flag with the row of the loop it ran; from a start step
         t0 that loop begins at row T - t0 of the table, so the tag is moved there and first_step names the table's row."""
         flags = flags.cpu().tolist()
-        if start is not None:
+        if isinstance(start, StartSteps):
+            flags = [f + ((self.T - t0) << 8) if f >> 8 else f for f, t0 in zip(flags, start.t0)]
+        elif start is not None:
             flags = [f + ((self.T - start[0]) << 8) if f >> 8 else f for f in flags]
         return nan_exception_class()(flags=flags)
 
@@ -622,6 +674,14 @@ class EDM(torch.nn.Module):
         advances by t0 + 2 draws; per-molecule streams use their draws 0 .. t0+1). Frames that no step below t0 writes are
         zero. t0 bounds how far a sample may move from its input; t0 = T is not the plain sampler (z_T keeps alpha_T xh).
         Everything below -- seeds, recovery rounds, devices, batch_slice -- applies unchanged.
+        `start_step` may also be a 1-D sequence, or integer tensor, of one t0 per molecule (dl_set_start_steps): molecule b
+        is then sampled as the call with start_step=t0[b] samples it on the same batch, with the same seeds or noise rows
+        (scalars of start_scalars(t0[b], B)) -- bit for bit on the SIMT edge path, on the tensor-core path within the
+        per-molecule rule -- and an all-equal sequence is the int call bit for bit. noise= then holds max(t0) + 2 slabs, of
+        which row b reads 0 .. t0[b]+1. One launch computes only the molecules that have started: sum_b (t0[b] + 1)
+        molecule-steps. It needs per-molecule streams (seeds or noise_mode='per_molecule') or noise=, works with the
+        recovery rounds, every require_* and `devices`, and raises ValueError for a wrong length, an entry that is not an
+        int in [0, T], the batch stream, InpaintingEDM, sample_fn and linker_sizes.
         `batch_slice=(b0, B_full)`: the inputs are rows [b0, b0+B) of a batch of B_full molecules (strong scaling,
         distributed.sample_chain_sharded); the device-side noise is then those rows of the full batch's draws.
         `seeds` (B ints, or an integer tensor; CUDA inputs): molecule b draws exactly what the reference draws for it
@@ -709,7 +769,10 @@ class EDM(torch.nn.Module):
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
         full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
         on_device, noise = ((False, None) if dev_seeds is not None
-                            else self._noise(noise, x, node_mask, fragment_mask, None if start is None else start[0]))
+                            else self._noise(noise, x, node_mask, fragment_mask, _loop_steps(start)))
+        if isinstance(start, StartSteps) and on_device:
+            raise ValueError("per-molecule start steps need per-molecule streams (seeds= or noise_mode='per_molecule') or "
+                             f"noise=: the batch stream, noise_mode={self.noise_mode!r}, does not draw per molecule")
         if batch_slice is not None and not on_device:
             raise ValueError("batch_slice needs the device-side noise stream (CUDA tensors, noise_mode='reference_stream')")
         self.dynamics._check_graph_type()
@@ -833,6 +896,9 @@ class EDM(torch.nn.Module):
         `linker_sizes`, one LinkerSizes per request, all of one size table, redraws sizes in those rounds as in sample_chain
         (it needs `seeds`); `last_sizes_many` holds every request's sizes. Each request's sizes come from its own seeds, so
         packing does not change them.
+        `start_step` may also be a list with one entry per request, each an int or one step per molecule of that request:
+        results[k] then equals sample_chain with that request's steps (their scalars at its own B_k), and requests of
+        different steps share launches, since the steps travel per row.
         Raises ValueError for an empty list, the batch stream (its draws depend on B and N), noise= or a replaced draw
         function, host inputs, requests on different devices or of different feature or context widths, and seeds that do
         not match the requests. It takes no `require_unique`, and raises ValueError when the attribute is set: a launch packs
@@ -848,7 +914,11 @@ class EDM(torch.nn.Module):
             raise ValueError("sample_many does not take require_unique: a launch packs several requests, so their rows would "
                              "be compared with each other; call sample_chain per request, or deduplicate with "
                              "molecule_builder.graph_hashes")
-        self._start(start_step, 1)          # validates it before anything else is checked
+        per_request = isinstance(start_step, (list, tuple))
+        if per_request and len(start_step) != len(requests):
+            raise ValueError(f"start_step holds {len(start_step)} entries for {len(requests)} requests")
+        if not per_request:
+            self._start(start_step, 1)      # validates it before anything else is checked
         for k, r in enumerate(requests):
             if 'noise' in r or 'batch_slice' in r:
                 raise ValueError(f"request {k} passes noise= or batch_slice=: sample_many samples per-molecule streams, "
@@ -879,6 +949,12 @@ class EDM(torch.nn.Module):
                                  f"{ctx_nf} columns and every request must give them")
         sizes = [r['x'].shape[0] for r in requests]
         nodes = [r['x'].shape[1] for r in requests]
+        if per_request:                     # validates every request's steps before anything else is checked
+            for k, (s, b) in enumerate(zip(start_step, sizes)):
+                if s is None:
+                    raise ValueError(f"start_step[{k}] is None: a start_step list holds an int or one step per molecule "
+                                     "for every request")
+                self._start(s, b)
         if seeds is not None:
             cpu_seeds = []
             for k, (s, b) in enumerate(zip(seeds, sizes)):
@@ -937,9 +1013,10 @@ class EDM(torch.nn.Module):
             redraw = None
             if redraws is not None:
                 redraw = tuple(redraws[ks[0]][1] if j == 1 else torch.cat([redraws[k][j] for k in ks]) for j in range(5))
+            start = StartSteps.cat([starts[k] for k in ks]) if per_request else starts[sizes[ks[0]]]
             [(_, call)], finish = self._enqueue_batch(lib, full, keep_frames, coefs[sizes[ks[0]]], [(dev_i, replica, 0, b)], [eng],
                                                       [where], dev, dev_seeds=dev_seeds, retries=retries, check=check,
-                                                      start=starts[sizes[ks[0]]], redraw=redraw, sets=sets)
+                                                      start=start, redraw=redraw, sets=sets)
             finishes.append(finish)
             by_device.setdefault(dev_i, []).append(
                 functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
@@ -989,7 +1066,7 @@ class EDM(torch.nn.Module):
         self.last_loop_ms_many = [(slots[slot_of[i]][0], sorted(ks), loop_ms[i]) for i, (ks, _) in enumerate(launches)]
         for k, f in enumerate(flags):
             if f.any():
-                exc = self._nan_exception(f, starts[sizes[k]])
+                exc = self._nan_exception(f, starts[k] if per_request else starts[sizes[k]])
                 exc.request, exc.results = k, results
                 if recover:
                     exc.chain = results[k]
@@ -999,10 +1076,17 @@ class EDM(torch.nn.Module):
     def _launch_keys(self, sizes, nodes, keep_frames, start_step):
         """({B: step coefficients}, {B: _start}, the plan_launches key of every request) of sample_many's requests of sizes
         B_k and N_k: requests share a launch only where sample_chain would give them the same coefficient table and start
-        scalars and, with mean aggregation on FC graphs, the same N."""
+        scalars and, with mean aggregation on FC graphs, the same N. With a list `start_step`, one entry per request (an int
+        or one step per molecule), the starts are every request's StartSteps at its own B_k, which travel per row: the key
+        is then the coefficient table (and N) alone, so requests of different steps share launches."""
         coefs = {b: self.step_coefficients(keep_frames, b) for b in sorted(set(sizes))}
-        starts = {b: self._start(start_step, b) for b in sorted(set(sizes))}
         same_n = self.dynamics.graph_type == 'FC' and self.dynamics.aggregation_method == 'mean'
+        if isinstance(start_step, (list, tuple)):
+            starts = [self._start(s, b) for s, b in zip(start_step, sizes)]
+            starts = [s if isinstance(s, StartSteps) else StartSteps(*([v] * b for v in s)) for s, b in zip(starts, sizes)]
+            keys = [(bytes(coefs[b]), None, n if same_n else None) for b, n in zip(sizes, nodes)]
+            return coefs, starts, keys
+        starts = {b: self._start(start_step, b) for b in sorted(set(sizes))}
         keys = [(bytes(coefs[b]), starts[b], n if same_n else None) for b, n in zip(sizes, nodes)]
         return coefs, starts, keys
 
@@ -1075,7 +1159,7 @@ class EDM(torch.nn.Module):
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
                 (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i, sets_i, lh_i) if recover else None,
-                start)))
+                start.rows(lo, hi) if isinstance(start, StartSteps) else start)))
 
         def finish():
             if not whole:

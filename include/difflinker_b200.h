@@ -20,6 +20,7 @@
  *   either, one seed per molecule (no reference API)     dl_sample_chain_seeded
  *   EDM, from q(z_t0 | x) of a known linker (edm.py:67-74) dl_set_start_step, then any dl_sample_chain* entry point
  *     at step t0 (partial diffusion, no reference API)
+ *     ... at one step t0[b] per molecule                 dl_set_start_steps, then the per-row entry points
  *   either, resampling only the molecules that diverged  dl_sample_chain_retry, dl_retry_seed, dl_last_retry_ms
  *     (the reference's callers resample the whole batch, generate.py:153-161)
  *   either, also resampling the molecules that are      dl_sample_chain_retry with dl_molecule_checks, dl_molecule_check
@@ -559,6 +560,30 @@ dl_status dl_set_noise_slice(dl_engine* e, int32_t B_full, int32_t b0);
  * sigma_t0 is DL_ERR_INVALID.
  */
 dl_status dl_set_start_step(dl_engine* e, int32_t t0, float alpha_t0, float sigma_t0);
+/*
+ * Partial diffusion from per-molecule start steps (no reference API): with host arrays t0, alpha and sigma of B entries,
+ * 0 <= t0[b] <= T, molecule b of the following sampling calls of this engine -- the recovery rounds included -- is sampled
+ * exactly as dl_set_start_step(t0[b], alpha[b], sigma[b]) samples it, whatever the other rows' steps:
+ *   start  z_b = xh * fragment_mask + (alpha[b] * xh + sigma[b] * eps) * linker_mask; (alpha[b], sigma[b]) are the
+ *          scalars of t0[b] the caller evaluates at the call's own B (EDM.start_scalars(t0[b], B)), since they depend on it;
+ *   steps  t0[b]-1 .. 0 with rows T-1-s of `coef`, then the final row T;
+ *   draws  row b's draw k is its own k-th draw: draw 0 is eps, step s consumes draw t0[b] - s and the final step draw
+ *          t0[b] + 1. A noise tensor holds t0max + 2 slabs (t0max = max_b t0[b]) of which row b reads slabs 0 .. t0[b]+1
+ *          of its own row; per-molecule seeds use their stream's draws 0 .. t0[b]+1;
+ *   output frames with no step below t0[b] stay zero for row b; until row b starts, its z is held bit for bit; its NaN
+ *          flag ignores every forward it is not part of, and its row tag counts from its own start: tag row j is step
+ *          t0[b]-1-j.
+ * Row b of a call thus equals row b of the single-step call with t0[b] on the same batch, seeds or noise rows: bit for bit
+ * on the SIMT edge path, and on the tensor-core path within the per-molecule rule (node tiles span molecules, the caveat of
+ * batch slices and sub-batches). With every t0[b] equal, the call is the dl_set_start_step call, bit for bit on both paths.
+ * The engine orders the rows by t0 descending (stably), gathers their inputs in that order, and loop step r computes only
+ * the prefix of rows that have started, recapturing the step graph when the prefix grows: a call costs
+ * sum_b (t0[b] + 1) molecule-steps instead of B * (t0max + 1) (dl_last_molecule_steps).
+ * B = 0 clears them. Setting either this or dl_set_start_step clears the other. DL_ERR_INVALID: here, a negative t0[b] or a
+ * non-finite scalar; at the sampling call, a B other than the one set, t0[b] > T, DL_SAMPLER_INPAINT, dl_sample_chain_rng
+ * (the batch stream's draws are not per row) and a dl_size_redraw (linker sizes take no start step).
+ */
+dl_status dl_set_start_steps(dl_engine* e, int32_t B, const int32_t* t0, const float* alpha, const float* sigma);
 /* The (n_draws,B,N,3+F) tensor the device-side stream of dl_sample_chain_rng stands for (tests, debugging). DEVICE out. */
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream);
@@ -580,6 +605,9 @@ dl_status dl_sample_chain_host(dl_engine* e, int32_t sampler, int32_t B, int32_t
  * of the most recent dl_sample_chain loop / dl_dynamics_forward measured with CUDA events on `stream`
  * (valid after the stream has been synchronised). */
 int64_t dl_launch_count(const dl_engine* e);
+/* The molecule-steps the most recent sampling loop computed, summed over its steps: B * (t0 + 1) with one start step
+ * (B * (T + 1) without), sum_b (t0[b] + 1) with per-molecule ones. The recovery rounds keep the first loop's. */
+int64_t dl_last_molecule_steps(dl_engine* e);
 float dl_last_elapsed_ms(dl_engine* e);
 /* Average device time (ms, CUDA events on the engine's loop stream) of the dominant kernel -- the layer-0 GCL
  * edge kernel -- relaunched `reps` times on the engine's current workspace (state of the last call; the
