@@ -124,6 +124,11 @@ struct dl_engine {
   std::vector<int32_t> starts_t0;
   std::vector<float> starts_alpha, starts_sigma;
   HostStage start_rows;        // a per-molecule start-step call's row order, lags, scalars and gathered inputs
+  // dl_set_resamplings: the inpainting sampler runs `resamplings` passes per reverse step, for calls of T = resample_T,
+  // re-noising with the (T, 2) (alpha_t|s, sigma_t|s) of `jump`; 1: the plain loop. coef_passes: the device table's host copy.
+  int resamplings = 1, resample_T = 0;
+  std::vector<float> jump;
+  std::vector<dl_step_coef> coef_passes;
   int64_t mol_steps = 0;       // dl_last_molecule_steps
   bool finalized = false;
   std::map<std::string, std::vector<float>> raw;
@@ -144,8 +149,8 @@ struct dl_engine {
   cudaStream_t loop_stream = nullptr;
   cudaEvent_t ev_in = nullptr, ev_out = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
   float* coef_dev = nullptr;
-  int coef_cap = 0;
-  int* step_ctr = nullptr;     // [2]: step_prep, step_fin
+  int coef_cap = 0;            // bytes of coef_dev
+  int* step_ctr = nullptr;     // [3]: step_prep, step_fin, and with resampling the step k_finish tags NaN flags with
   int64_t launches = 0;
   HostStage stage;
   KernelTimes times;           // DL_TIME_KERNELS
@@ -390,6 +395,7 @@ struct FwdIO {
   NoiseRng rng{};
   int T = 0; float norm0 = 1.f, norm1 = 1.f, bias1 = 0.f;
   RowStarts rows{};   // per-molecule start steps, or rows.lag = null
+  int R = 1; const float* jump = nullptr;   // resampling passes per reverse step (dl_set_resamplings), T counting passes
 };
 
 ProjW proj_of(const EdgeMlpW& w) { return ProjW{w.W1a_t, w.W1b_t, w.b1}; }
@@ -584,7 +590,7 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     fa.coef = e->coef_dev; fa.step_fin = e->step_ctr + 1; fa.step_prep = e->step_ctr; fa.T = io.T;
     fa.norm0 = io.norm0; fa.norm1 = io.norm1; fa.bias1 = io.bias1; fa.chain = io.chain; fa.rows = io.rows;
   } else if (io.sampler) {
-    fa.tag_step = e->step_ctr + 1;
+    fa.tag_step = e->step_ctr + (io.R > 1 ? 2 : 1);   // with resampling the pass counter is not the step
   }
   const bool per_mol = io.rng.on == NOISE_PER_MOLECULE;
   TIMED("k_finish", st, (launch_chain(per_mol ? k_finish<true> : k_finish<false>, dim3((n + 15) / 16), dim3(256), 0, st, gm, fa)));
@@ -600,7 +606,11 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     ia.coef = e->coef_dev;
     ia.step_prep = e->step_ctr; ia.step_fin = e->step_ctr + 1; ia.T = io.T;
     ia.norm0 = io.norm0; ia.norm1 = io.norm1; ia.bias1 = io.bias1; ia.chain = io.chain;
-    if (per_mol) k_inpaint<true><<<B, 256, 0, st>>>(gm, ia);
+    ia.R = io.R; ia.jump = io.jump; ia.step_tag = e->step_ctr + 2;
+    if (io.R > 1) {
+      if (per_mol) k_inpaint<true, true><<<B, 256, 0, st>>>(gm, ia);
+      else k_inpaint<false, true><<<B, 256, 0, st>>>(gm, ia);
+    } else if (per_mol) k_inpaint<true><<<B, 256, 0, st>>>(gm, ia);
     else k_inpaint<false><<<B, 256, 0, st>>>(gm, ia);
     LAUNCH_CHECK();
     e->launches += 1;
@@ -687,8 +697,22 @@ dl_status check_sampler(const dl_engine* e, int sampler, int T, int keep_frames,
   return DL_OK;
 }
 
-// standard-normal draws of one chain: init + one per step + final (linker), or their masked pairs (inpainting)
-uint64_t sampler_draws(int sampler, int T) { return sampler == DL_SAMPLER_INPAINT ? (uint64_t)2 * T + 3 : (uint64_t)T + 2; }
+// standard-normal draws of one chain: init + one per step + final (linker), or their masked pairs (inpainting) -- with R
+// resampling passes per step, each pass's pair and, but on the last pass, the re-noise draw
+uint64_t sampler_draws(int sampler, int T, int R = 1) {
+  return sampler == DL_SAMPLER_INPAINT ? 1 + (uint64_t)T * (3 * R - 1) + 2 : (uint64_t)T + 2;
+}
+
+// The resampling passes of a call (dl_set_resamplings), or 0 with DL_ERR_INVALID set when the setting does not apply to it.
+int call_resamplings(const dl_engine* e, int sampler, int T) {
+  if (e->resamplings == 1) return 1;
+  if (sampler != DL_SAMPLER_INPAINT) { set_err("resampling (dl_set_resamplings) takes DL_SAMPLER_INPAINT only"); return 0; }
+  if (T != e->resample_T) {
+    set_err("dl_set_resamplings was given the jump coefficients of T = %d; the call samples T = %d", e->resample_T, T);
+    return 0;
+  }
+  return e->resamplings;
+}
 
 // Reverse steps of a call before the final one: the start step when one is set (dl_set_start_step), else T. The loop then
 // runs the last loop_steps + 1 rows of the coefficient table as a chain of that length, so it also sets the draws.
@@ -833,7 +857,7 @@ dl_status dl_create_ex(const dl_config* cfg, const dl_egnn_options* opts, dl_eng
   CK(cudaEventCreate(&e->ev_r1));
   CK(cudaEventCreate(&e->ev_g0));
   CK(cudaEventCreate(&e->ev_g1));
-  CK(cudaMalloc((void**)&e->step_ctr, 2 * sizeof(int)));
+  CK(cudaMalloc((void**)&e->step_ctr, 3 * sizeof(int)));
   CK(cudaFuncSetAttribute(k_node<ACT_SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * NODE_TM * LDX * sizeof(float)));
   CK(opt_in_edge_simt<true>());
   CK(opt_in_edge_simt<false>());
@@ -1031,8 +1055,10 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
             "(dl_set_start_steps): use dl_sample_chain_seeded or a noise tensor");
     return DL_ERR_INVALID;
   }
+  const int R = call_resamplings(e, sampler, T);
+  if (R < 1) return DL_ERR_INVALID;
   const NoiseRng q = make_rng(e, B, N, seed, offset);
-  if (offset_consumed) *offset_consumed = sampler_draws(sampler, loop_steps(e, T)) * q.per_draw;
+  if (offset_consumed) *offset_consumed = sampler_draws(sampler, loop_steps(e, T), R) * q.per_draw;
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, nullptr,
                            &q, coef, norm, chain, nan_flags, stream);
 }
@@ -1083,6 +1109,25 @@ dl_status dl_set_start_steps(dl_engine* e, int32_t B, const int32_t* t0, const f
   return DL_OK;
 }
 
+dl_status dl_set_resamplings(dl_engine* e, int32_t r, int32_t T, const float* jump) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  if (r < 1) { set_err("dl_set_resamplings: r must be >= 1 (got %d)", r); return DL_ERR_INVALID; }
+  if (r == 1) { e->resamplings = 1; e->resample_T = 0; e->jump.clear(); return DL_OK; }
+  if (!jump) { set_err("dl_set_resamplings: r = %d needs the jump coefficients", r); return DL_ERR_INVALID; }
+  if (T < 1) { set_err("dl_set_resamplings: T must be >= 1 (got %d)", T); return DL_ERR_INVALID; }
+  if ((int64_t)T * r > (1 << 24)) {   // the expanded coefficient table and the draw indices stay well inside int
+    set_err("dl_set_resamplings: T * r = %lld passes exceeds 2^24", (long long)T * r);
+    return DL_ERR_INVALID;
+  }
+  for (int i = 0; i < 2 * T; ++i)
+    if (!std::isfinite(jump[i])) {
+      set_err("dl_set_resamplings: jump[%d][%d] is not finite", i / 2, i % 2);
+      return DL_ERR_INVALID;
+    }
+  e->resamplings = r; e->resample_T = T; e->jump.assign(jump, jump + 2 * T);
+  return DL_OK;
+}
+
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream) {
   dl_status s = check_shapes(e, B, N);
@@ -1104,11 +1149,19 @@ dl_status dl_noise_fill_inpaint(dl_engine* e, int32_t T, int32_t B, int32_t N, c
   if (!node_mask || !fragment_mask || !out) { set_err("null argument"); return DL_ERR_INVALID; }
   if (T < 1 || 2 * T + 3 > 65535) { set_err("need 1 <= T <= 32766 (got %d)", T); return DL_ERR_INVALID; }
   if ((s = check_slice(e, B)) != DL_OK) return s;
+  const int R = call_resamplings(e, DL_SAMPLER_INPAINT, T);
+  if (R < 1) return DL_ERR_INVALID;
+  const uint64_t draws = sampler_draws(DL_SAMPLER_INPAINT, T, R);
+  if (draws > 65535) { set_err("%llu draws exceed the grid's 65535 rows", (unsigned long long)draws); return DL_ERR_INVALID; }
   CK(cudaSetDevice(e->cfg.device));
   const NoiseRng q = make_rng(e, B, N, seed, offset);
-  if (offset_consumed) *offset_consumed = (uint64_t)(2 * T + 3) * q.per_draw;
-  k_com_free_draws<false><<<dim3(B, 2 * T + 3), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      N, 3 + e->cfg.in_node_nf, T, q, node_mask, fragment_mask, out);
+  if (offset_consumed) *offset_consumed = draws * q.per_draw;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (R > 1)
+    k_com_free_draws<false, true><<<dim3(B, (unsigned)draws), 256, 0, st>>>(N, 3 + e->cfg.in_node_nf, T, q, node_mask,
+                                                                           fragment_mask, out, R);
+  else
+    k_com_free_draws<false><<<dim3(B, 2 * T + 3), 256, 0, st>>>(N, 3 + e->cfg.in_node_nf, T, q, node_mask, fragment_mask, out);
   LAUNCH_CHECK();
   return DL_OK;
 }
@@ -1137,11 +1190,26 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     if (rng && !per_mol) { set_err("the batch stream takes no per-molecule start steps"); return DL_ERR_INVALID; }
     if (loop_steps(e, T) > T) { set_err("start step %d exceeds T = %d", loop_steps(e, T), T); return DL_ERR_INVALID; }
   }
+  const int R = call_resamplings(e, sampler, T);
+  if (R < 1) return DL_ERR_INVALID;
   // A start step t0 runs the table's last t0 + 1 rows -- steps t0-1 .. 0, then the final one -- as a loop of Tl = t0 steps:
   // loop step r reads row r of the copied rows and draw r + 1, so the draws are eps, one per step and the final one.
   const int Tl = loop_steps(e, T);
   coef += T - Tl;
   static_assert(sizeof(dl_step_coef) == 32, "dl_step_coef layout");
+  // Resampling: the loop runs P = T*R passes and the final step. Pass k*R + u reads row k of the caller's table, whose frame
+  // only its last pass writes; the jump coefficients follow the table on the device.
+  const int P = Tl * R, rows = P + 1;
+  const size_t coef_bytes = (size_t)rows * sizeof(dl_step_coef) + (R > 1 ? e->jump.size() * sizeof(float) : 0);
+  if (R > 1) {
+    e->coef_passes.resize(rows);
+    for (int p = 0; p < P; ++p) {
+      e->coef_passes[p] = coef[p / R];
+      if (p % R != R - 1) e->coef_passes[p].frame = -1;
+    }
+    e->coef_passes[P] = coef[Tl];
+    coef = e->coef_passes.data();
+  }
   CK(cudaSetDevice(e->cfg.device));
   cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
   cudaStream_t st = e->loop_stream;
@@ -1151,18 +1219,22 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   const double tc0 = time_chain ? now_ms() : 0.0;
   double tc_plan = 0, tc_capture = 0, tc_inst = 0, tc_launch = 0;
   if ((s = ensure_workspace(e, B, N)) != DL_OK) return s;
-  if (e->coef_cap < Tl + 1) {
+  if ((size_t)e->coef_cap < coef_bytes) {
     if (e->coef_dev) cudaFree(e->coef_dev);
     e->coef_dev = nullptr;
-    CK(cudaMalloc((void**)&e->coef_dev, (size_t)(Tl + 1) * sizeof(dl_step_coef)));
-    e->coef_cap = Tl + 1;
+    CK(cudaMalloc((void**)&e->coef_dev, coef_bytes));
+    e->coef_cap = (int)coef_bytes;
   }
   // order the private loop stream after the caller's stream (the legacy default stream cannot be captured)
   if (user != st) {
     CK(cudaEventRecord(e->ev_in, user));
     CK(cudaStreamWaitEvent(st, e->ev_in, 0));
   }
-  CK(cudaMemcpyAsync(e->coef_dev, coef, (size_t)(Tl + 1) * sizeof(dl_step_coef), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(e->coef_dev, coef, (size_t)rows * sizeof(dl_step_coef), cudaMemcpyHostToDevice, st));
+  const float* jump_dev = R > 1 ? e->coef_dev + (size_t)rows * 8 : nullptr;
+  if (R > 1)
+    CK(cudaMemcpyAsync(const_cast<float*>(jump_dev), e->jump.data(), e->jump.size() * sizeof(float), cudaMemcpyHostToDevice,
+                       st));
   NoiseRng q = rng ? *rng : NoiseRng{};
   // per-molecule start steps: the loop runs on the rows in start-step order, each loop step on those that have started
   RowOrder ro{};
@@ -1179,7 +1251,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
       CK(cudaMemcpyAsync(e->ws.seeds, rng->seeds, (size_t)B * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
     q.seeds = e->ws.seeds;
   }
-  CK(cudaMemsetAsync(e->step_ctr, 0, 2 * sizeof(int), st));
+  CK(cudaMemsetAsync(e->step_ctr, 0, 3 * sizeof(int), st));
   if (nan_flags) CK(cudaMemsetAsync(nan_flags, 0, B * sizeof(int32_t), st));
   const int n = B * N, xd = 3 + e->cfg.in_node_nf;
   // frames that no reverse step is the last writer of stay zero, as torch.zeros in edm.py:143 -- with a start step also
@@ -1221,11 +1293,13 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   io.node_mask = node_mask; io.linker_mask = inpaint ? nullptr : linker_mask; io.edge_mask = edge_mask;
   io.context = context; io.nan_flags = nan_flags; io.fragment_mask = fragment_mask; io.noise = noise;
   io.rng = q;
-  io.chain = chain; io.T = Tl; io.norm0 = norm[0]; io.norm1 = norm[1]; io.bias1 = norm[2];
+  io.chain = chain; io.T = P; io.norm0 = norm[0]; io.norm1 = norm[1]; io.bias1 = norm[2];
   io.rows = per_row ? ro.rs : RowStarts{};
+  io.R = R; io.jump = jump_dev;
 
-  // capture ONE reverse step; the step index lives on the device, so the same graph serves all Tl+1 steps -- with
-  // per-molecule start steps, all steps of one prefix length: the graph is recaptured whenever the prefix grows
+  // capture ONE reverse step; the step index lives on the device, so the same graph serves all Tl+1 steps (all P+1 passes
+  // with resampling) -- with per-molecule start steps, all steps of one prefix length: the graph is recaptured whenever the
+  // prefix grows
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t exec = nullptr;
   const int64_t before = e->launches;
@@ -1239,7 +1313,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   if (ge == cudaSuccess) ge = cudaEventRecord(e->ev_t0, st);
   int failed_step = -1;
   int64_t mol_steps = 0, replans = 0;
-  for (int r = 0; ge == cudaSuccess && r <= Tl; ++r) {
+  for (int r = 0; ge == cudaSuccess && r <= P; ++r) {
     if (per_row && ro.active[r] != Bp) {
       // more rows have started: their plan and step graph, which replaces the executable's (or a new one)
       Bp = ro.active[r];
@@ -1270,7 +1344,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     const double tc_done = now_ms();
     float loop = 0.f; cudaEventElapsedTime(&loop, e->ev_t0, e->ev_t1);
     fprintf(stderr, "[dl chain] setup+plan %.2f ms | capture %.2f | instantiate %.2f | %d graph launches enqueued in %.2f | wait for the GPU %.2f | device loop %.2f\n",
-            tc_plan - tc0, tc_capture - tc_plan, tc_inst - tc_capture, Tl + 1, tc_launch - tc_inst, tc_done - tc_launch, loop);
+            tc_plan - tc0, tc_capture - tc_plan, tc_inst - tc_capture, P + 1, tc_launch - tc_inst, tc_done - tc_launch, loop);
   }
   if (ge == cudaSuccess && user != st) {
     ge = cudaEventRecord(e->ev_out, st);
@@ -1283,7 +1357,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     else set_err("%s:%d reverse-loop graph -> %s", __FILE__, __LINE__, cudaGetErrorString(ge));
     return DL_ERR_CUDA;
   }
-  e->launches = before + per_step * (Tl + 1) + 2 * replans;
+  e->launches = before + per_step * (P + 1) + 2 * replans;
   e->mol_steps = mol_steps;
   return DL_OK;
 }
@@ -1300,10 +1374,12 @@ dl_status dl_sample_chain_host(dl_engine* e, int32_t sampler, int32_t B, int32_t
   CK(cudaSetDevice(e->cfg.device));
   const size_t n = (size_t)B * N, frame_bytes = n * (3 + e->cfg.in_node_nf) * 4;
   const bool fc_em = edge_mask && e->cfg.graph_type == DL_GRAPH_FC;
+  const int R = std::max(call_resamplings(e, sampler, T), 1);   // a refused setting fails in dl_sample_chain below
   StageLayout sl;
   const int i_xh = sl.in(xh, frame_bytes), i_nm = sl.in(node_mask, n), i_fm = sl.in(fragment_mask, n * 4),
             i_lm = sl.in(linker_mask, n * 4), i_em = sl.in(fc_em ? edge_mask : nullptr, n * N),
-            i_ctx = sl.in(context, n * e->cfg.context_node_nf * 4), i_nz = sl.in(noise, sampler_draws(sampler, loop_steps(e, T)) * frame_bytes),
+            i_ctx = sl.in(context, n * e->cfg.context_node_nf * 4),
+            i_nz = sl.in(noise, sampler_draws(sampler, loop_steps(e, T), R) * frame_bytes),
             i_ch = sl.out(keep_frames * frame_bytes), i_fl = sl.out(B * 4);
   cudaStream_t st = e->loop_stream;
   if ((s = stage_inputs(e->stage, sl, st)) != DL_OK) return s;

@@ -1047,6 +1047,11 @@ struct InpaintArgs {
   int T;
   float norm0, norm1, bias1;
   float* chain;
+  // RePaint resampling (k_inpaint<PER_MOL, true>): R passes per reverse step. The step counters then count passes, and
+  // coef is the engine's table of T*R + 1 rows, row k*R + u being step k's row (frame -1 but on its last pass u = R-1).
+  int R;
+  const float* jump;        // (T, 2) (alpha_t|s, sigma_t|s) of step k, for the re-noise after every pass but the last
+  int* step_tag;            // written here: the step of the next pass, which k_finish tags NaN flags with
 };
 
 __device__ __forceinline__ float block_sum_256(float v, float* red) {
@@ -1076,6 +1081,12 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
 // 3+F columns for a global write and read of the whole draw. An empty mask gives 0/0 means, as in the tensor path.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool com_free_on_fragments(int r, int T) { return r >= 2 && r <= 2 * T && (r & 1) == 0; }
+// The same with R resampling passes per step (dl_set_resamplings): step k's draws are 1 + k(3R-1) + 3u + {0, 1, 2} for
+// pass u -- p(z_s|z_t), q(z_s|z_t,x) and, on every pass but the last, the re-noise draw -- so the fragment draws are those
+// at offset 1 mod 3 within a step's 3R - 1. R = 1 is the function above.
+__device__ __forceinline__ bool com_free_on_fragments(int r, int T, int R) {
+  return r >= 1 && r <= T * (3 * R - 1) && (r - 1) % (3 * R - 1) % 3 == 1;
+}
 
 template <bool PER_MOL, typename M>
 __device__ float3 com_free_means(const NoiseRng& q, int r, int b, int N, const M* __restrict__ mask, float* red) {
@@ -1100,10 +1111,14 @@ __device__ __forceinline__ float com_free_value(const NoiseRng& q, int r, int g,
   return __fsub_rn(xm, __fmul_rn(d == 0 ? mean.x : d == 1 ? mean.y : mean.z, m));
 }
 
-template <bool PER_MOL = false>
+// RES (RePaint, dl_set_resamplings): `step` counts passes, a.T = T*R of them before the final one. Pass u < R-1 of step k
+// ends with the re-noise z <- alpha_t|s * z + sigma_t|s * eps on every atom (eps: draw rC, COM-free on the node mask),
+// rounded op by op as the torch expression is, after the projection and instead of advancing to step k+1.
+template <bool PER_MOL = false, bool RES = false>
 __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
   __shared__ float red[8];
   __shared__ float means[4];
+  __shared__ float renoise[5];      // RES: the re-noise draw's means, alpha_t|s and sigma_t|s (shared: no registers held)
   const int b = blockIdx.x, tid = threadIdx.x, N = gm.N, xd = 3 + gm.F;
   const size_t g0 = (size_t)b * N;
   int step = 0;
@@ -1130,14 +1145,28 @@ __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
   const int frame = __float_as_int(cf[4]);
   const size_t slab = (size_t)gm.B * N * xd;
   // draw rA: p(z_s|z_t) on all atoms; draw rB: q(z_s|z_t,x) on the fragment atoms, or the final q draw on all atoms
-  const int rA = 1 + 2 * step, rB = rA + 1;
+  int rA = 1 + 2 * step, rC = -1;   // rC: the re-noise draw, or -1
+  if constexpr (RES) {
+    const int k = step / a.R, u = step - k * a.R;
+    rA = 1 + k * (3 * a.R - 1) + 3 * u;
+    if (step < a.T && u < a.R - 1) {
+      rC = rA + 2;
+      if (tid == 0) { renoise[3] = a.jump[2 * k]; renoise[4] = a.jump[2 * k + 1]; }   // read after the barriers below
+    }
+  }
+  const int rB = rA + 1;
   const float* nA = a.rng.on ? nullptr : a.noise + (size_t)rA * slab;
   const float* nB = a.rng.on ? nullptr : a.noise + (size_t)rB * slab;
+  const float* nC = a.rng.on || rC < 0 ? nullptr : a.noise + (size_t)rC * slab;
   float3 meanA{}, meanB{};
   if (a.rng.on) {
     meanA = com_free_means<PER_MOL>(a.rng, rA, b, N, a.nm, red);
-    meanB = com_free_on_fragments(rB, a.T) ? com_free_means<PER_MOL>(a.rng, rB, b, N, a.fragment_mask, red)
-                                           : com_free_means<PER_MOL>(a.rng, rB, b, N, a.nm, red);
+    meanB = (RES ? step < a.T : com_free_on_fragments(rB, a.T)) ? com_free_means<PER_MOL>(a.rng, rB, b, N, a.fragment_mask, red)
+                                                                : com_free_means<PER_MOL>(a.rng, rB, b, N, a.nm, red);
+    if (RES && rC >= 0) {                                                  // uniform over the CTA
+      const float3 mc = com_free_means<PER_MOL>(a.rng, rC, b, N, a.nm, red);
+      if (tid == 0) { renoise[0] = mc.x; renoise[1] = mc.y; renoise[2] = mc.z; }
+    }
   }
   if (step < a.T) {
     // pass 1: new latent before the centre-of-mass projection
@@ -1166,6 +1195,13 @@ __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
       float zn = a.z[gi];
       if (d < 3) { zn -= means[d] * a.nm[g0 + n]; a.z[gi] = zn; }                // edm.py:592, utils.py:56-63
       if (frame >= 0) a.chain[(size_t)frame * slab + gi] = d < 3 ? zn * a.norm0 : zn * a.norm1 + a.bias1;
+      if (RES && rC >= 0) {
+        const float m = a.nm[g0 + n];
+        const float ec = a.rng.on ? com_free_value<PER_MOL>(a.rng, rC, (int)(g0 + n), d, m,
+                                                            make_float3(renoise[0], renoise[1], renoise[2]))
+                                  : nC[gi];
+        a.z[gi] = __fadd_rn(__fmul_rn(renoise[3], zn), __fmul_rn(renoise[4], ec));
+      }
     }
   } else {
     // final step: thread per atom, both variants and their argmax (edm.py:689-721)
@@ -1194,7 +1230,10 @@ __global__ void __launch_bounds__(256) k_inpaint(Geom gm, InpaintArgs a) {
         a.chain[(g0 + n) * xd + d] = ((d == bl ? 1.f : 0.f) * m) * lm + ((d == bf ? 1.f : 0.f) * m) * fm;
     }
   }
-  if (tid == 0 && b == 0) *a.step_prep = step + 1;
+  if (tid == 0 && b == 0) {
+    *a.step_prep = step + 1;
+    if constexpr (RES) *a.step_tag = (step + 1) / a.R;
+  }
 }
 
 // z0 = xh*fragment_mask + (noise[0]*linker_mask)*linker_mask   (edm.py:136-137)
@@ -1253,13 +1292,14 @@ __global__ void k_noise_fill(int n_draws, int n_total, int xd, NoiseRng rng, flo
 
 // Draws [0, gridDim.y) of the inpainting sampler's stream, masked and COM-projected, one CTA per (molecule, draw):
 // out is (gridDim.y, B = gridDim.x, N, xd). All 2T+3 for dl_noise_fill_inpaint; draw 0 -- the initial z (edm.py:565) --
-// straight into the workspace when the sampler draws on the device.
-template <bool PER_MOL = false>
+// straight into the workspace when the sampler draws on the device. RES: the 1 + T(3R-1) + 2 draws of R resampling passes.
+template <bool PER_MOL = false, bool RES = false>
 __global__ void __launch_bounds__(256) k_com_free_draws(int N, int xd, int T, NoiseRng rng, const int8_t* __restrict__ node_mask,
-                                                        const float* __restrict__ fragment_mask, float* __restrict__ out) {
+                                                        const float* __restrict__ fragment_mask, float* __restrict__ out,
+                                                        int R = 1) {
   __shared__ float red[8];
   const int b = blockIdx.x, r = blockIdx.y;
-  const bool frag = com_free_on_fragments(r, T);
+  const bool frag = RES ? com_free_on_fragments(r, T, R) : com_free_on_fragments(r, T);
   const float3 mean = frag ? com_free_means<PER_MOL>(rng, r, b, N, fragment_mask, red)
                            : com_free_means<PER_MOL>(rng, r, b, N, node_mask, red);
   float* o = out + ((size_t)blockIdx.y * gridDim.x + b) * N * xd;

@@ -191,7 +191,7 @@ def _check_start(sample_fn, start_step):
 
 def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                  start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                 require_novel=None, exclude_hashes=None):
+                 require_novel=None, exclude_hashes=None, resamplings=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
@@ -215,7 +215,9 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     molecule b alone, its input padded to the same number of rows (the size model mean-pools over the padding), with
     seeds=[last_seeds[b]], gives the same size and row. `model.edm.last_sizes` holds the sizes, and the returned node_mask
     is the template's at those sizes. ValueError with sample_fn, start_step, an inpainting model, host inputs, the batch
-    stream without seeds, and where EDM.sample_chain refuses it."""
+    stream without seeds, and where EDM.sample_chain refuses it.
+    `resamplings` = r: r RePaint passes per reverse step of an inpainting model (InpaintingEDM.sample_chain; None uses
+    `model.edm.resamplings`)."""
     _check_start(sample_fn, start_step)
     if linker_sizes is not None:
         _check_linker_sizes(model, sample_fn, start_step)
@@ -241,6 +243,8 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['exclude_hashes'] = exclude_hashes
     if start_step is not None:
         extra['start_step'] = start_step
+    if resamplings is not None:
+        extra['resamplings'] = resamplings
     chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **extra)
     if sized is not None:
         return chain, _final_node_mask(kw, sized, model.edm.last_sizes)
@@ -249,7 +253,7 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
 
 def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                 max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                require_novel=None):
+                require_novel=None, resamplings=None):
     """The body of sample_chain for many batches `datas` at once, sampled in shared launches by EDM.sample_many: returns
     [(chain_k, node_mask_k)] in the order of `datas`, each equal to what sample_chain(model, datas[k], ...) returns (with
     seeds[k]) in the sense of EDM.sample_many. `model` as for sample_chain, so accelerated reference modules take it too.
@@ -257,7 +261,7 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
     sequential sample_chain calls call them: linker sizes, seeds and the generator's final state are theirs. `start_step`,
     one for every batch, as in sample_chain. `linker_sizes`, one for every batch, as in sample_chain: each batch's sizes
     are drawn from its own seeds and its template padded to its own N_cap, so packing changes neither;
-    `edm.last_sizes_many` holds them."""
+    `edm.last_sizes_many` holds them. `resamplings` as in sample_chain."""
     _check_start(sample_fn, start_step)
     edm = model.edm
     if linker_sizes is not None:
@@ -298,6 +302,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['require_novel'] = require_novel
     if start_step is not None:
         extra['start_step'] = start_step
+    if resamplings is not None:
+        extra['resamplings'] = resamplings
     chains = edm.sample_many(requests, keep_frames=keep_frames, seeds=seeds, max_molecules=max_molecules, **extra)
     return [(chain, kw['node_mask']) for chain, kw in zip(chains, requests)]
 
@@ -339,19 +345,19 @@ class DDPM(nn.Module):
 
     def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                      start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                     require_novel=None, exclude_hashes=None):
+                     require_novel=None, exclude_hashes=None, resamplings=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                             require_connected=require_connected, start_step=start_step, require_valid=require_valid,
                             require_clash_free=require_clash_free, linker_sizes=linker_sizes, require_unique=require_unique,
-                            require_novel=require_novel, exclude_hashes=exclude_hashes)
+                            require_novel=require_novel, exclude_hashes=exclude_hashes, resamplings=resamplings)
 
     def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                    require_novel=None):
+                    require_novel=None, resamplings=None):
         return sample_many(self, datas, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                            require_connected=require_connected, max_molecules=max_molecules, start_step=start_step,
                            require_valid=require_valid, require_clash_free=require_clash_free, linker_sizes=linker_sizes,
-                           require_novel=require_novel)
+                           require_novel=require_novel, resamplings=resamplings)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

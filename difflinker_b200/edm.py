@@ -68,7 +68,7 @@ def _loop_steps(start):
     return max(start.t0) if isinstance(start, StartSteps) else start[0]
 
 
-def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None):
+def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None, resample=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
@@ -81,16 +81,21 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     hash sets of CHECK_NOVEL and CHECK_UNIQUE; None is two empty sets. `linker_hashes`, an int64 device tensor or None,
     receives every returned row's linker hash (CHECK_NOVEL).
     `start` = (t0, alpha_t0, sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of
-    the call (dl_set_start_step); a StartSteps starts each row at its own step (dl_set_start_steps). Returns (status, what
-    the batch stream consumed)."""
+    the call (dl_set_start_step); a StartSteps starts each row at its own step (dl_set_start_steps). `resample` = (r, T,
+    jump) runs r RePaint passes per step, set on the engine for the duration of the call (dl_set_resamplings). Returns
+    (status, what the batch stream consumed)."""
     per_row = isinstance(start, StartSteps)
     if per_row:
         start.set_on(lib, eng)
     elif start is not None:
         _native.check(lib.dl_set_start_step(eng, *start), "dl_set_start_step")
     try:
+        if resample is not None:
+            _native.check(lib.dl_set_resamplings(eng, *resample), "dl_set_resamplings")
         return _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry)
     finally:
+        if resample is not None:
+            lib.dl_set_resamplings(eng, 1, 0, None)
         if per_row:
             lib.dl_set_start_steps(eng, 0, None, None, None)
         elif start is not None:
@@ -269,6 +274,9 @@ class EDM(torch.nn.Module):
         self.last_novel = None                 # calls with require_novel: the (B,) CPU bool novelty verdict of every row
         self.last_linker_hashes = None         # calls with require_novel: the (B,) CPU int64 linker hash of every row
         self.last_sizes = None                # calls with linker_sizes: the (B,) CPU int32 linker size of every returned row
+        # RePaint resampling (InpaintingEDM only): the passes of every reverse step when sample_chain / sample_many get no
+        # `resamplings`; 1, the default, is the plain loop
+        self.resamplings = 1
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
@@ -373,6 +381,50 @@ class EDM(torch.nn.Module):
         cache[key] = rows
         return rows
 
+    def jump_coefficients(self, n_samples=1):
+        """The (T, 2) jump coefficients of dl_set_resamplings as a flat ctypes float array: row r, in step_coefficients' row
+        order (step s = T-1-r), holds (alpha_t|s, sigma_t|s) of sigma_and_alpha_t_given_s(gamma(t), gamma(s)), t = (s+1)/T,
+        evaluated on (n_samples, 1) fp32 CPU tensors as step_coefficients evaluates its rows. Cached likewise."""
+        T = self.T
+        key = ('jump', T, n_samples, self.gamma.gamma._version, self.gamma.gamma.data_ptr())
+        cache = self.__dict__.setdefault('_coef_cache', {})
+        if key in cache:
+            return cache[key]
+        gamma = self._cpu_gamma()
+        out = (C.c_float * (2 * T))()
+        for r in range(T):
+            s_arr = torch.full((n_samples, 1), fill_value=T - 1 - r)
+            t_arr = (s_arr + 1) / T
+            _, sigma_ts, alpha_ts = self.sigma_and_alpha_t_given_s(gamma(t_arr), gamma(s_arr / T))
+            out[2 * r], out[2 * r + 1] = float(alpha_ts[0]), float(sigma_ts[0])
+        if len(cache) >= 8:
+            cache.pop(next(iter(cache)))
+        cache[key] = out
+        return out
+
+    def _resamplings(self, resamplings):
+        """The RePaint passes of a call: `resamplings`, or the `resamplings` attribute when None. ValueError unless an int
+        >= 1 (not a bool); the linker sampler, which does not inpaint, takes 1 only."""
+        r = self.resamplings if resamplings is None else resamplings
+        try:
+            if isinstance(r, bool):
+                raise TypeError
+            r = operator.index(r)
+        except TypeError:
+            raise ValueError(f"resamplings is a count of passes per step (got {r!r})") from None
+        if r < 1:
+            raise ValueError(f"resamplings must be >= 1 (got {r})")
+        if r >= 1 << 31:
+            raise ValueError(f"resamplings {r} does not fit an int32")
+        if r > 1 and self._SAMPLER != _native.SAMPLER_INPAINT:
+            raise ValueError("resamplings re-noises an inpainting step: EDM samples the linker alone and takes 1 only "
+                             "(use InpaintingEDM)")
+        return r
+
+    def _resample(self, r, n_samples):
+        """_sample_slice's `resample` of r passes at batch size n_samples, or None for the plain loop."""
+        return None if r == 1 else (r, self.T, self.jump_coefficients(n_samples))
+
     def draw_noise(self, n_draws, n_samples, n_nodes, device, generator=None):
         """(n_draws, B, N, 3+F) standard normal. 'reference_stream': the reference's call order -- for every
         draw randn(B,N,3) then randn(B,N,F) (edm.py:328-340, utils.py:189-192) -- so seeds line up."""
@@ -391,10 +443,10 @@ class EDM(torch.nn.Module):
     # ---- what the two samplers differ in: the device sampler, the number of draws and how a noise tensor is drawn ----
     _SAMPLER = _native.SAMPLER_LINKER
 
-    def _n_draws(self):
+    def _n_draws(self, resamplings=1):
         return self.T + 2
 
-    def _draw_tensor(self, n_samples, n_nodes, device, node_mask, fragment_mask):
+    def _draw_tensor(self, n_samples, n_nodes, device, node_mask, fragment_mask, resamplings=1):
         return self.draw_noise(self.T + 2, n_samples, n_nodes, device)
 
     def _draws_replaced(self):
@@ -420,17 +472,18 @@ class EDM(torch.nn.Module):
                     fragment_mask=prep(fragment_mask.reshape(n_samples, n_nodes), torch.float32),
                     linker_mask=prep(linker_mask.reshape(n_samples, n_nodes), torch.float32), edge_mask=em, context=ctx)
 
-    def _noise(self, noise, x, node_mask, fragment_mask, start_step=None):
+    def _noise(self, noise, x, node_mask, fragment_mask, start_step=None, resamplings=1):
         """(on_device, noise): the device-side stream unless a tensor is injected (tests), the draw function is replaced, or
-        another mode is set; otherwise the whole batch's draws on x's device -- t0 + 2 of them from a start step t0."""
+        another mode is set; otherwise the whole batch's draws on x's device -- t0 + 2 of them from a start step t0, those
+        of `resamplings` passes per step for the inpainting sampler."""
         n_samples, n_nodes = x.size(0), x.size(1)
         dev = x.device
         on_device = (noise is None and dev.type == 'cuda' and self.noise_mode == 'reference_stream'
                      and not self._draws_replaced())
-        n_draws = self._n_draws() if start_step is None else start_step + 2
+        n_draws = self._n_draws(resamplings) if start_step is None else start_step + 2
         if not on_device:
             if noise is None:
-                noise = (self._draw_tensor(n_samples, n_nodes, dev, node_mask, fragment_mask) if start_step is None
+                noise = (self._draw_tensor(n_samples, n_nodes, dev, node_mask, fragment_mask, resamplings) if start_step is None
                          else self.draw_noise(n_draws, n_samples, n_nodes, dev))
             noise = noise.to(device=dev, dtype=torch.float32).contiguous()
             assert noise.shape == (n_draws, n_samples, n_nodes, self.n_dims + self.in_node_nf), noise.shape
@@ -663,7 +716,7 @@ class EDM(torch.nn.Module):
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                     require_novel=None, exclude_hashes=None):
+                     require_novel=None, exclude_hashes=None, resamplings=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -745,6 +798,8 @@ class EDM(torch.nn.Module):
         inside the padded template. The inputs must be the template of the sizes dl_size_draw gives `seeds` at attempt 0,
         padded to max(n_frag) + max(sizes) rows or more. `last_sizes` (B,) CPU int32 holds every returned row's size. It
         needs `seeds` and raises ValueError where nan_retries does, with start_step and for InpaintingEDM.
+        `resamplings` (None: the `resamplings` attribute, default 1) is InpaintingEDM's; this class raises ValueError for
+        anything but 1 (or None), and for a value that is not an int >= 1.
         The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
         and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
         device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
@@ -760,6 +815,7 @@ class EDM(torch.nn.Module):
         self.last_connected = self.last_valid = self.last_clash_free = self.last_sizes = None
         self.last_unique = self.last_graph_hashes = self.last_novel = self.last_linker_hashes = None
         start = self._start(start_step, n_samples)
+        r = self._resamplings(resamplings)
         redraw = self._linker_sizes(linker_sizes, seeds, noise, batch_slice, start_step, x, linker_mask)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
         check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free,
@@ -769,7 +825,7 @@ class EDM(torch.nn.Module):
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
         full = self._sampler_tensors(x, h, node_mask, fragment_mask, linker_mask, edge_mask, context)
         on_device, noise = ((False, None) if dev_seeds is not None
-                            else self._noise(noise, x, node_mask, fragment_mask, _loop_steps(start)))
+                            else self._noise(noise, x, node_mask, fragment_mask, _loop_steps(start), r))
         if isinstance(start, StartSteps) and on_device:
             raise ValueError("per-molecule start steps need per-molecule streams (seeds= or noise_mode='per_molecule') or "
                              f"noise=: the batch stream, noise_mode={self.noise_mode!r}, does not draw per molecule")
@@ -800,7 +856,8 @@ class EDM(torch.nn.Module):
         calls, finish = self._enqueue_batch(lib, full, keep_frames, self.step_coefficients(keep_frames, n_samples), slices,
                                             engines, places, dev, noise=noise, dev_seeds=dev_seeds,
                                             rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check,
-                                            start=start, redraw=redraw, sets=sets)
+                                            start=start, redraw=redraw, sets=sets,
+                                            resample=self._resample(r, n_samples))
         by_device = {}
         for dev_i, c in calls:
             by_device.setdefault(dev_i, []).append(c)
@@ -868,7 +925,7 @@ class EDM(torch.nn.Module):
     @torch.no_grad()
     def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                    require_novel=None):
+                    require_novel=None, resamplings=None):
         """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
         edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
         (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
@@ -899,6 +956,8 @@ class EDM(torch.nn.Module):
         `start_step` may also be a list with one entry per request, each an int or one step per molecule of that request:
         results[k] then equals sample_chain with that request's steps (their scalars at its own B_k), and requests of
         different steps share launches, since the steps travel per row.
+        `resamplings` as in sample_chain, for every request; requests then also share a launch only where sample_chain
+        would give them the same jump coefficients (jump_coefficients, which depend on the batch size as the table does).
         Raises ValueError for an empty list, the batch stream (its draws depend on B and N), noise= or a replaced draw
         function, host inputs, requests on different devices or of different feature or context widths, and seeds that do
         not match the requests. It takes no `require_unique`, and raises ValueError when the attribute is set: a launch packs
@@ -919,6 +978,7 @@ class EDM(torch.nn.Module):
             raise ValueError(f"start_step holds {len(start_step)} entries for {len(requests)} requests")
         if not per_request:
             self._start(start_step, 1)      # validates it before anything else is checked
+        r_passes = self._resamplings(resamplings)
         for k, r in enumerate(requests):
             if 'noise' in r or 'batch_slice' in r:
                 raise ValueError(f"request {k} passes noise= or batch_slice=: sample_many samples per-molecule streams, "
@@ -983,6 +1043,8 @@ class EDM(torch.nn.Module):
             with torch.cuda.device(dev):    # one draw per request, in request order, as the sample_chain calls draw them
                 cpu_seeds = list(torch.cat([draw_seeds(b, dev) for b in sizes]).cpu().split(sizes))
         coefs, starts, keys = self._launch_keys(sizes, nodes, keep_frames, start_step)
+        if r_passes > 1:                    # the jump coefficients depend on the batch size as the table does
+            keys = [k + (bytes(self.jump_coefficients(b)),) for k, b in zip(keys, sizes)]
         fc = self.dynamics.graph_type == 'FC'
         launches = plan_launches(sizes, nodes, max_molecules, keys)
         if fc:                              # edges of the launch's padded molecules
@@ -1016,7 +1078,8 @@ class EDM(torch.nn.Module):
             start = StartSteps.cat([starts[k] for k in ks]) if per_request else starts[sizes[ks[0]]]
             [(_, call)], finish = self._enqueue_batch(lib, full, keep_frames, coefs[sizes[ks[0]]], [(dev_i, replica, 0, b)], [eng],
                                                       [where], dev, dev_seeds=dev_seeds, retries=retries, check=check,
-                                                      start=start, redraw=redraw, sets=sets)
+                                                      start=start, redraw=redraw, sets=sets,
+                                                      resample=self._resample(r_passes, sizes[ks[0]]))
             finishes.append(finish)
             by_device.setdefault(dev_i, []).append(
                 functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
@@ -1091,14 +1154,14 @@ class EDM(torch.nn.Module):
         return coefs, starts, keys
 
     def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
-                       retries=0, check=0, start=None, redraw=None, sets=None):
+                       retries=0, check=0, start=None, redraw=None, sets=None, resample=None):
         """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
         inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
         replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
         covers the batch where it is. The draws are the per-molecule `dev_seeds`, the batch stream `rng` = (seed, offset,
         b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _checks; `start` as
         returned by _start; `redraw` as returned by _linker_sizes (its rounds then redraw sizes, into `sizes`); `sets` as
-        returned by _hash_sets, copied to each slice's device.
+        returned by _hash_sets, copied to each slice's device; `resample` as returned by _resample.
         Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
         (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
         back and returns dict(chain, flags, used, attempts, passed, sizes, bad, consumed) on `dev`; `passed` holds
@@ -1159,7 +1222,7 @@ class EDM(torch.nn.Module):
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
                 (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i, sets_i, lh_i) if recover else None,
-                start.rows(lo, hi) if isinstance(start, StartSteps) else start)))
+                start.rows(lo, hi) if isinstance(start, StartSteps) else start, resample)))
 
         def finish():
             if not whole:
@@ -1195,11 +1258,14 @@ class InpaintingEDM(EDM):
         xm = x * mask
         return xm - (xm.sum(dim=-2, keepdim=True) / mask.sum(dim=-2, keepdim=True)) * mask
 
-    def draw_noise_inpaint(self, n_samples, n_nodes, device, node_mask, fragment_mask, generator=None):
+    def draw_noise_inpaint(self, n_samples, n_nodes, device, node_mask, fragment_mask, generator=None, resamplings=1):
         """(2T+3, B, N, 3+F): the reference's draws in call order, already masked and COM-projected:
-        init (all atoms); per step: p(z_s|z_t) on all atoms then q(z_s|z_t,x) on fragment atoms; final p and q draws."""
+        init (all atoms); per step: p(z_s|z_t) on all atoms then q(z_s|z_t,x) on fragment atoms; final p and q draws.
+        With r = `resamplings` passes per step, each pass draws the pair and, but on the last, the re-noise draw on all
+        atoms: (1 + T(3r-1) + 2, B, N, 3+F)."""
         T, nd, nf = self.T, self.n_dims, self.in_node_nf
-        masks = [node_mask] + [node_mask, fragment_mask] * T + [node_mask, node_mask]
+        step = [node_mask, fragment_mask, node_mask] * (resamplings - 1) + [node_mask, fragment_mask]
+        masks = [node_mask] + step * T + [node_mask, node_mask]
         out = torch.empty((len(masks), n_samples, n_nodes, nd + nf), device=device, dtype=torch.float32)
         for r, m in enumerate(masks):
             m = m.to(device=device, dtype=torch.float32)
@@ -1216,11 +1282,13 @@ class InpaintingEDM(EDM):
     def _final_qa(self, g0):
         return float((self.sigma(g0) / self.alpha(g0))[0])                         # edm.py:716
 
-    def _n_draws(self):
-        return 2 * self.T + 3
+    def _n_draws(self, resamplings=1):
+        return 1 + self.T * (3 * resamplings - 1) + 2
 
-    def _draw_tensor(self, n_samples, n_nodes, device, node_mask, fragment_mask):
-        return self.draw_noise_inpaint(n_samples, n_nodes, device, node_mask, fragment_mask)
+    def _draw_tensor(self, n_samples, n_nodes, device, node_mask, fragment_mask, resamplings=1):
+        if resamplings == 1:                # the plain loop: the draw function as it is called without resampling
+            return self.draw_noise_inpaint(n_samples, n_nodes, device, node_mask, fragment_mask)
+        return self.draw_noise_inpaint(n_samples, n_nodes, device, node_mask, fragment_mask, resamplings=resamplings)
 
     def _draws_replaced(self):
         """draw_noise_inpaint replaced on the instance, in a subclass or on the class supplies the draws."""
@@ -1236,7 +1304,7 @@ class InpaintingEDM(EDM):
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                     require_novel=None, exclude_hashes=None):
+                     require_novel=None, exclude_hashes=None, resamplings=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -1246,14 +1314,24 @@ class InpaintingEDM(EDM):
         masked and projected per molecule as always. `nan_retries`, `require_connected`, `require_valid` and `require_unique`
         as in EDM.sample_chain; the checks and the hash cover every atom of the molecule. `require_novel` and
         `exclude_hashes` as there; the linker hash covers the linker_mask rows. `start_step` raises ValueError unless None, and `require_clash_free`
-        unless None or False: this loop re-noises the pocket; `linker_sizes` unless None: this model has no linker size."""
+        unless None or False: this loop re-noises the pocket; `linker_sizes` unless None: this model has no linker size.
+        `resamplings` = r (None: the `resamplings` attribute, default 1) runs every reverse step as r RePaint passes
+        (Lugmayr et al., 2022; DiffSBDD's inpaint(..., resamplings=r); dl_set_resamplings): pass u denoises as the plain
+        step does, with time feature (s+1)/T, and every pass but the last then re-noises z <- alpha_t|s z + sigma_t|s eps
+        on every atom (eps COM-free on the node mask, as sample_combined_position_feature_noise draws it; the two scalars
+        are jump_coefficients'), so the generated atoms can adapt to the known ones. The frame of step s is written after
+        its last pass. The draws are z_T, per step and pass the p and q draws plus the re-noise draw for u < r-1, then the
+        two final draws: 1 + T(3r-1) + 2 (noise= holds that many prepared slabs, draw_noise_inpaint(resamplings=r) makes
+        them; the batch stream advances by as many draws; per-molecule streams use their draws in that order). r = 1 is
+        the plain sampler, bit for bit. A call costs about r times the loop. ValueError for a non-integer, a bool or
+        r < 1."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
                                     require_connected=require_connected, start_step=start_step, require_valid=require_valid,
                                     require_clash_free=require_clash_free, linker_sizes=linker_sizes,
                                     require_unique=require_unique, require_novel=require_novel,
-                                    exclude_hashes=exclude_hashes)
+                                    exclude_hashes=exclude_hashes, resamplings=resamplings)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

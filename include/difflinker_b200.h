@@ -21,6 +21,8 @@
  *   EDM, from q(z_t0 | x) of a known linker (edm.py:67-74) dl_set_start_step, then any dl_sample_chain* entry point
  *     at step t0 (partial diffusion, no reference API)
  *     ... at one step t0[b] per molecule                 dl_set_start_steps, then the per-row entry points
+ *   InpaintingEDM, r RePaint passes per step            dl_set_resamplings, then any dl_sample_chain* entry point
+ *     (DiffSBDD's inpaint(..., resamplings=r), no reference API)
  *   either, resampling only the molecules that diverged  dl_sample_chain_retry, dl_retry_seed, dl_last_retry_ms
  *     (the reference's callers resample the whole batch, generate.py:153-161)
  *   either, also resampling the molecules that are      dl_sample_chain_retry with dl_molecule_checks, dl_molecule_check
@@ -584,11 +586,31 @@ dl_status dl_set_start_step(dl_engine* e, int32_t t0, float alpha_t0, float sigm
  * (the batch stream's draws are not per row) and a dl_size_redraw (linker sizes take no start step).
  */
 dl_status dl_set_start_steps(dl_engine* e, int32_t B, const int32_t* t0, const float* alpha, const float* sigma);
+/*
+ * RePaint resampling (Lugmayr et al., 2022; DiffSBDD's inpaint(..., resamplings=r); no reference API) for DL_SAMPLER_INPAINT:
+ * with r >= 1, reverse step s = T-1 .. 0 of the following dl_sample_chain, _rng, _seeded, _retry and _retry_sets calls of
+ * this engine -- the recovery rounds included -- becomes r passes. Pass u = 0 .. r-1:
+ *   denoise   the plain inpainting step (row T-1-s of `coef`, time feature (s+1)/T on every pass): p(z_s | z_t) on all atoms,
+ *             q(z_s | z_t, x) on the fragment atoms, combined by the masks and projected to a zero centre of mass;
+ *   re-noise  for u < r-1: z <- alpha_t|s * z + sigma_t|s * eps on every atom, eps COM-free on the node mask (coordinates)
+ *             and masked (features) like the p draw; each product and the sum rounded on its own. No projection follows:
+ *             the next pass projects.
+ * The frame of step s is written after its last pass; the final p(x, h | z_0) step is unchanged. `jump` holds (T, 2) HOST
+ * floats, (alpha_t|s, sigma_t|s) of sigma_and_alpha_t_given_s(gamma_t, gamma_s) per row in dl_step_coef row order (row j is
+ * step T-1-j). The draws are z_T; then per step and pass the p and q draws and, for u < r-1, the re-noise draw; then the two
+ * final draws: 1 + T(3r-1) + 2 in that order, which a noise tensor holds as prepared slabs, offset_consumed counts and
+ * dl_noise_fill_inpaint writes. The NaN flags' row tag names the step, whatever the pass. r = 1 (the default) restores
+ * the plain loop, bit for bit and with the same launches. Sticky like dl_set_start_step. DL_ERR_INVALID: here, r < 1,
+ * r > 1 with a null jump, T < 1 or a non-finite jump value; at the sampling call, with r > 1, a T other than the one set
+ * and DL_SAMPLER_LINKER. A call costs about r times the plain loop (T*r + 1 forwards).
+ */
+dl_status dl_set_resamplings(dl_engine* e, int32_t r, int32_t T, const float* jump);
 /* The (n_draws,B,N,3+F) tensor the device-side stream of dl_sample_chain_rng stands for (tests, debugging). DEVICE out. */
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream);
 /* The (2T+3,B,N,3+F) prepared draws the device-side stream of dl_sample_chain_rng(DL_SAMPLER_INPAINT) stands for, computed by
- * the same device code (tests, debugging). node_mask (B,N) int8, fragment_mask (B,N) fp32, out: DEVICE. */
+ * the same device code (tests, debugging); with r resampling passes set (dl_set_resamplings), the 1 + T(3r-1) + 2 draws of
+ * that loop. node_mask (B,N) int8, fragment_mask (B,N) fp32, out: DEVICE. */
 dl_status dl_noise_fill_inpaint(dl_engine* e, int32_t T, int32_t B, int32_t N, const int8_t* node_mask,
                                 const float* fragment_mask, uint64_t seed, uint64_t offset, float* out,
                                 uint64_t* offset_consumed, void* stream);
@@ -606,7 +628,8 @@ dl_status dl_sample_chain_host(dl_engine* e, int32_t sampler, int32_t B, int32_t
  * (valid after the stream has been synchronised). */
 int64_t dl_launch_count(const dl_engine* e);
 /* The molecule-steps the most recent sampling loop computed, summed over its steps: B * (t0 + 1) with one start step
- * (B * (T + 1) without), sum_b (t0[b] + 1) with per-molecule ones. The recovery rounds keep the first loop's. */
+ * (B * (T + 1) without), sum_b (t0[b] + 1) with per-molecule ones, B * (T * r + 1) with r resampling passes (every pass
+ * counts). The recovery rounds keep the first loop's. */
 int64_t dl_last_molecule_steps(dl_engine* e);
 float dl_last_elapsed_ms(dl_engine* e);
 /* Average device time (ms, CUDA events on the engine's loop stream) of the dominant kernel -- the layer-0 GCL
