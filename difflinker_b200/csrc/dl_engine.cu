@@ -144,6 +144,12 @@ struct dl_engine {
   Workspace ws_sub;
   HostStage sub_rows;
   HostStage hashes;            // DL_CHECK_UNIQUE: the full batch's graph hashes, (B) uint64, grown to the largest B
+  // dl_set_ring_sizes: the ring sizes DL_CHECK_RINGS allows (ring_set: set at least once). ring_masks: the ring-size masks
+  // of the last dl_sample_chain_retry call's ring_B rows, grown to the largest B; ring_B = 0 when it did not require the bit
+  bool ring_set = false;
+  unsigned long long ring_allowed = 0;
+  HostStage ring_masks;
+  int ring_B = 0;
   cudaEvent_t ev_r0 = nullptr, ev_r1 = nullptr, ev_g0 = nullptr, ev_g1 = nullptr;
   float retry_ms = 0.f;
   cudaStream_t loop_stream = nullptr;
@@ -882,6 +888,7 @@ dl_status dl_destroy(dl_engine* e) {
   if (e->sub_rows.buf) cudaFree(e->sub_rows.buf);
   if (e->start_rows.buf) cudaFree(e->start_rows.buf);
   if (e->hashes.buf) cudaFree(e->hashes.buf);
+  if (e->ring_masks.buf) cudaFree(e->ring_masks.buf);
   if (e->wblob) cudaFree(e->wblob);
   if (e->wblob_tc) cudaFree(e->wblob_tc);
   if (e->coef_dev) cudaFree(e->coef_dev);
@@ -1125,6 +1132,18 @@ dl_status dl_set_resamplings(dl_engine* e, int32_t r, int32_t T, const float* ju
       return DL_ERR_INVALID;
     }
   e->resamplings = r; e->resample_T = T; e->jump.assign(jump, jump + 2 * T);
+  return DL_OK;
+}
+
+dl_status dl_set_ring_sizes(dl_engine* e, uint64_t allowed) {
+  if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  if (allowed & 7u) {
+    set_err("dl_set_ring_sizes: bits 0-2 of allowed must be clear (a ring has at least 3 atoms; got 0x%llx)",
+            (unsigned long long)allowed);
+    return DL_ERR_INVALID;
+  }
+  e->ring_allowed = allowed;
+  e->ring_set = true;
   return DL_OK;
 }
 
@@ -1397,28 +1416,30 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt) { return retry_seed(seed,
 namespace {
 
 static_assert(CHECK_CONNECTED == DL_CHECK_CONNECTED && CHECK_VALENCE == DL_CHECK_VALENCE && CHECK_CLASH == DL_CHECK_CLASH &&
-              CHECK_UNIQUE == DL_CHECK_UNIQUE && CHECK_NOVEL == DL_CHECK_NOVEL, "kernels_retry.cuh vs header");
+              CHECK_UNIQUE == DL_CHECK_UNIQUE && CHECK_NOVEL == DL_CHECK_NOVEL && CHECK_RINGS == DL_CHECK_RINGS,
+              "kernels_retry.cuh vs header");
 
 // What is wrong with a caller's dl_molecule_checks for molecules of N rows whose h holds at most max_types type columns, or
 // null. The sampler takes every check; dl_molecule_check the bond checks only (the clash check has dl_clash_check,
 // DL_CHECK_UNIQUE compares the molecules of one sampling call with each other, which a per-molecule check cannot, and
-// DL_CHECK_NOVEL needs a linker_mask).
+// DL_CHECK_NOVEL and DL_CHECK_RINGS need a linker_mask).
 const char* checks_error(const dl_molecule_checks* ck, int N, int max_types, bool sampler) {
   if (!ck) return "null checks";
   constexpr int hashed = DL_CHECK_UNIQUE | DL_CHECK_NOVEL;
   if (sampler) {
-    if (ck->require == 0 ||
-        (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE | DL_CHECK_CLASH | DL_CHECK_UNIQUE | DL_CHECK_NOVEL)))
+    if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE | DL_CHECK_CLASH | DL_CHECK_UNIQUE |
+                                             DL_CHECK_NOVEL | DL_CHECK_RINGS)))
       return "checks->require must be a non-empty OR of DL_CHECK_CONNECTED, DL_CHECK_VALENCE, DL_CHECK_CLASH, "
-             "DL_CHECK_UNIQUE and DL_CHECK_NOVEL";
+             "DL_CHECK_UNIQUE, DL_CHECK_NOVEL and DL_CHECK_RINGS";
   } else if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE))) {
     return "checks->require must be DL_CHECK_CONNECTED, DL_CHECK_VALENCE or both (the clash check runs through "
            "dl_clash_check; DL_CHECK_UNIQUE compares the molecules of a dl_sample_chain_retry call with each other, and "
            "dl_molecule_hash gives their hashes; DL_CHECK_NOVEL needs a linker_mask, and its linker hashes are "
-           "dl_molecule_hash over node_mask AND linker_mask)";
+           "dl_molecule_hash over node_mask AND linker_mask; DL_CHECK_RINGS runs through dl_ring_check)";
   }
   if (ck->n_types < 1 || ck->n_types > max_types) return "checks->n_types must be in [1, the width of the atom features]";
-  if ((ck->require & (DL_CHECK_CONNECTED | DL_CHECK_VALENCE | hashed)) && !ck->thr1) return "null checks->thr1";
+  if ((ck->require & (DL_CHECK_CONNECTED | DL_CHECK_VALENCE | hashed | DL_CHECK_RINGS)) && !ck->thr1)
+    return "null checks->thr1";
   if ((ck->require & DL_CHECK_VALENCE) && (!ck->thr2 || !ck->thr3 || !ck->max_valence))
     return "DL_CHECK_VALENCE needs checks->thr2, thr3 and max_valence";
   if ((ck->require & DL_CHECK_UNIQUE) && (!ck->thr2 || !ck->thr3)) return "DL_CHECK_UNIQUE needs checks->thr2 and thr3";
@@ -1452,6 +1473,8 @@ const char* checked_error(const dl_engine* e, int32_t sampler, int N, const dl_m
     else if (e->cfg.graph_type == DL_GRAPH_FC) why = "DL_CHECK_CLASH needs a pocket: DL_GRAPH_FC graphs have none";
     else if (sampler == DL_SAMPLER_INPAINT) why = "DL_CHECK_CLASH does not take DL_SAMPLER_INPAINT, which re-noises the pocket";
   }
+  if (!why && (checks->require & DL_CHECK_RINGS) && !e->ring_set)
+    why = "DL_CHECK_RINGS in checks->require needs the allowed ring sizes: call dl_set_ring_sizes first";
   return why;
 }
 
@@ -1537,6 +1560,7 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
                        const dl_molecule_checks* ck, const dl_hash_sets* hs, int32_t* passed, uint64_t* linker_hash,
                        const dl_size_redraw* rz, int32_t* sizes_used, void* stream) {
   e->retry_ms = 0.f;
+  e->ring_B = 0;
   dl_status s = dl_sample_chain_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask,
                                        context, seeds, coef, norm, chain, nan_flags, stream);
   if (s != DL_OK) return s;
@@ -1559,10 +1583,18 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     if ((s = stage_inputs(e->hashes, hl, st)) != DL_OK) return s;
     hash = reinterpret_cast<unsigned long long*>(e->hashes.buf);
   }
+  const bool rings = (require & DL_CHECK_RINGS) != 0;
+  unsigned long long* ring_masks = nullptr;                // DL_CHECK_RINGS: every returned row's mask (dl_last_ring_sizes)
+  if (rings) {
+    StageLayout rl;
+    rl.out((size_t)B * sizeof(uint64_t));
+    if ((s = stage_inputs(e->ring_masks, rl, st)) != DL_OK) return s;
+    ring_masks = reinterpret_cast<unsigned long long*>(e->ring_masks.buf);
+  }
   if (ck) {
     const ClashArgs cl{linker_mask, ck->clash, nullptr};   // the clash check's linker rows and table
     CK(launch_molecule_check(require, check_args(e, *ck, chain, N, node_mask, context, passed), cl, HashArgs{hash, 0}, B,
-                             st, NovelArgs{linker_mask, kn, n_known, lh}));
+                             st, NovelArgs{linker_mask, kn, n_known, lh}, e->ring_allowed, ring_masks));
     e->launches += 1;
     if (unique) {                                          // every row is a candidate; the only keepers are the seen set
       UniqueArgs u{};
@@ -1640,7 +1672,7 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
       ca.rows = ga.rows; ca.flags = nan_flags; ca.s_flags = sa.s_flags; ca.take = sl.at<int32_t>(i_tk);
       const HashArgs ha{sl.at<unsigned long long>(i_sh), 0};
       CK(launch_molecule_check(require, ca, ClashArgs{ga.s_linker_mask, ck->clash, nullptr}, ha, Bs, st,
-                               NovelArgs{ga.s_linker_mask, kn, n_known, lh}));
+                               NovelArgs{ga.s_linker_mask, kn, n_known, lh}, e->ring_allowed, ring_masks));
       e->launches += 1;
       sa.take = ca.take; sa.s_passed = ca.passed; sa.passed = passed;
       if (rz) k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa, za);
@@ -1677,6 +1709,7 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     for (int i = 0; i < Bs; ++i)
       if (take[i]) { flags[rows[i]] = sub_flags[i]; if (!unique) pass[rows[i]] = sub_pass[i]; }
   }
+  if (rings) e->ring_B = B;
   for (int b = 0; b < B; ++b) if (flags[b] != 0) return DL_NAN_DETECTED;
   return DL_OK;
 }
@@ -1799,7 +1832,9 @@ dl_status dl_novel_check(int32_t B, int32_t N, const dl_molecule_checks* checks,
   const char* why = checks_error(checks, N, xh_row_stride - 3, true);
   const int require = checks ? checks->require : 0;
   int dev = 0;
-  if (!why && !(require & DL_CHECK_NOVEL)) why = "checks->require must include DL_CHECK_NOVEL";
+  if (!why && (require & DL_CHECK_RINGS))
+    why = "checks->require must be an OR of DL_CHECK_NOVEL and the bits below (DL_CHECK_RINGS runs through dl_ring_check)";
+  else if (!why && !(require & DL_CHECK_NOVEL)) why = "checks->require must include DL_CHECK_NOVEL";
   else if (!why && (B <= 0 || N <= 0 || !xh || !node_mask || !linker_mask || !passed ||
                     (drop_pocket && (!context || context_nf < 1))))
     why = "invalid argument";
@@ -1837,6 +1872,37 @@ dl_status dl_clash_check(int32_t B, int32_t N, int32_t n_types, const float* cla
   ca.node_mask = node_mask; ca.C = context_nf; ca.context = context; ca.drop_pocket = 1; ca.passed = passed;
   if (clashes) CK(cudaMemsetAsync(clashes, 0, (size_t)B * N * sizeof(int32_t), st));   // the rows that are not linker atoms
   CK(launch_molecule_check(CHECK_CLASH, ca, ClashArgs{linker_mask, clash, clashes}, HashArgs{}, B, st));
+  return DL_OK;
+}
+
+dl_status dl_ring_check(int32_t B, int32_t N, int32_t n_types, const float* thr1, const float* xh, int32_t xh_row_stride,
+                        const int8_t* node_mask, const float* linker_mask, const float* context, int32_t context_nf,
+                        int32_t drop_pocket, uint64_t allowed, int32_t* passed, uint64_t* ring_sizes, void* stream) {
+  const char* why = nullptr;
+  if (B <= 0 || N <= 0) why = "B and N must be >= 1";
+  else if (N > CONN_MAX_N) why = "the molecule checks take N <= 8192";
+  else if (n_types < 1 || n_types > xh_row_stride - 3) why = "n_types must be in [1, xh_row_stride - 3]";
+  else if (allowed & 7u) why = "bits 0-2 of allowed must be clear (a ring has at least 3 atoms)";
+  else if (!thr1 || !xh || !node_mask || !linker_mask || !passed || (drop_pocket && (!context || context_nf < 1)))
+    why = "invalid argument";
+  if (why) { set_err("dl_ring_check: %s", why); return DL_ERR_INVALID; }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CheckArgs ca{};
+  ca.xh = xh; ca.N = N; ca.row_stride = xh_row_stride; ca.n_types = n_types; ca.thr1 = thr1;
+  ca.node_mask = node_mask; ca.C = context_nf; ca.context = context; ca.drop_pocket = drop_pocket != 0; ca.passed = passed;
+  CK(launch_molecule_check(CHECK_RINGS, ca, ClashArgs{}, HashArgs{}, B, st, NovelArgs{linker_mask, nullptr, 0, nullptr},
+                           allowed, reinterpret_cast<unsigned long long*>(ring_sizes)));
+  return DL_OK;
+}
+
+dl_status dl_last_ring_sizes(dl_engine* e, int32_t B, uint64_t* out, void* stream) {
+  const char* why = nullptr;
+  if (!e || !out) why = "null engine or out";
+  else if (e->ring_B == 0) why = "the last dl_sample_chain_retry call of this engine did not require DL_CHECK_RINGS";
+  else if (B != e->ring_B) why = "B differs from the last dl_sample_chain_retry call's";
+  if (why) { set_err("dl_last_ring_sizes: %s", why); return DL_ERR_INVALID; }
+  CK(cudaMemcpyAsync(out, e->ring_masks.buf, (size_t)B * sizeof(uint64_t), cudaMemcpyDeviceToDevice,
+                     reinterpret_cast<cudaStream_t>(stream)));
   return DL_OK;
 }
 

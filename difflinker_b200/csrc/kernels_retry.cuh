@@ -231,8 +231,10 @@ __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a, RowSizeA
 // clear; k_unique_verdict sets it, since it compares molecules with each other.
 // CHECK_NOVEL: the bit is set iff the linker hash L -- the graph hash of the checked atoms with linker_mask != 0 -- is not
 // in the caller's sorted set of known linker hashes (stated at DL_CHECK_NOVEL in the header).
+// CHECK_RINGS: the bit is set iff the molecule's ring-size mask -- the smallest ring of every bond with a linker end, over
+// the graph of all its checked atoms -- lies inside the caller's allowed mask (stated at DL_CHECK_RINGS in the header).
 constexpr int CHECK_CONNECTED = 1, CHECK_VALENCE = 2, CHECK_CLASH = 4, CHECK_UNIQUE = 8;   // DL_CHECK_* of the header
-constexpr int CHECK_NOVEL = 16;
+constexpr int CHECK_NOVEL = 16, CHECK_RINGS = 32;
 constexpr int CONN_MAX_N = 8192;                                     // rows per molecule: 20 bytes of shared memory each
 constexpr int CONN_SMEM_MAX = CONN_MAX_N * (int)(sizeof(float4) + sizeof(int));
 // With CHECK_UNIQUE a molecule also takes 8 bytes per row (the atoms' rows and the CSR offsets) and 4 bytes per stored
@@ -291,6 +293,17 @@ struct NovelArgs {
   unsigned long long* linker_hash;       // out or null: molecule b's L at row b, or in a recovery round (CheckArgs::rows)
                                          // at the caller's row rows[b], where the row is taken
 };
+
+// What CHECK_RINGS reads and writes besides CheckArgs: NovelArgs, whose linker_mask it shares, and its own fields. The
+// instantiations with the bit take it in place of NovelArgs, and molecule_check reads the fields below through its NovelArgs
+// reference, so that the other instantiations keep their code (their shared variables' names follow its signature).
+struct RingArgs : NovelArgs {
+  unsigned long long allowed;            // bit k set: a smallest ring of k atoms passes (bit 63: of 63 or more)
+  unsigned long long* ring_sizes;        // out or null: molecule b's mask at row b, or in a recovery round (CheckArgs::rows)
+                                         // at the caller's row rows[b], where the row is taken
+};
+// The ring stage's breadth-first searches keep three bitsets over the rows per warp: visited, frontier and next frontier.
+constexpr int RING_BITSETS = 3 * 8;
 
 // Whether v is among s[0, n), ascending in unsigned order (duplicates allowed): a binary search for the first entry >= v,
 // with 64-bit indices and unsigned compares.
@@ -437,6 +450,126 @@ __device__ __forceinline__ unsigned long long graph_hash(const CheckArgs& a, con
   return hash_mix(s);
 }
 
+// The ring-size mask of the n staged atoms s_at[0, n), s_link[i] != 0 for a linker atom (stated at DL_CHECK_RINGS in the
+// header). Block-collective; returns the mask on every thread.
+// The bonds are found once into a CSR of neighbour indices (s_off, s_edge), as graph_hash finds them: atoms whose list
+// would end beyond edge_cap find their neighbours by testing every staged atom instead. Then a warp per atom u takes each
+// bond (u, v > u) with a linker end and searches breadth-first from u, level by level, for v in the graph without that
+// bond: bottom-up, each lane asks whether an atom not yet reached has a neighbour on the frontier, and a ballot writes 32
+// atoms' answers as one word of the next frontier. v reached at level d closes a smallest ring of d + 1 atoms. Bits are only
+// ever ORed into a warp's own register and then over the warps, so the mask does not depend on the order the warps run in.
+__device__ __forceinline__ unsigned long long ring_mask(const CheckArgs& a, int edge_cap, int n, const float4* s_at,
+                                                        int* s_off, const int* s_link, unsigned* s_bits, int* s_edge) {
+  __shared__ int s_wsum[8], s_e;
+  __shared__ unsigned long long s_rmask[8];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int i = warp; i < n; i += 8) {                 // degrees
+    const float4 pi = s_at[i];
+    int d = 0;
+    for (int j = lane; j < n; j += 32) d += j != i && staged_bonded(a, i, pi, j, s_at[j], n);
+    for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+    if (lane == 0) s_off[i] = d;
+  }
+  if (tid == 0) s_e = 0;
+  __syncthreads();
+  for (int i0 = 0; i0 < n; i0 += 256) {               // exclusive scan of the degrees, 256 atoms at a time
+    const int i = i0 + tid;
+    const int v = i < n ? s_off[i] : 0;
+    int x = v;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, x, o);
+      if (lane >= o) x += y;
+    }
+    if (lane == 31) s_wsum[warp] = x;
+    __syncthreads();
+    int before = s_e, total = 0;
+    for (int w = 0; w < 8; ++w) { before += w < warp ? s_wsum[w] : 0; total += s_wsum[w]; }
+    if (i < n) s_off[i] = before + x - v;
+    __syncthreads();
+    if (tid == 0) s_e += total;
+    __syncthreads();
+  }
+  const int E = s_e;
+  auto end_of = [&](int i) { return i + 1 < n ? s_off[i + 1] : E; };
+  for (int i = warp; i < n; i += 8) {                 // the stored lists, ascending
+    if (end_of(i) > edge_cap) continue;
+    const float4 pi = s_at[i];
+    int at = s_off[i];
+    for (int j0 = 0; j0 < n; j0 += 32) {
+      const int j = j0 + lane;
+      const bool bonded = j < n && j != i && staged_bonded(a, i, pi, j, s_at[j], n);
+      const unsigned m = __ballot_sync(0xffffffffu, bonded);
+      if (bonded) s_edge[at + __popc(m & ((1u << lane) - 1u))] = j;
+      at += __popc(m);
+    }
+  }
+  __syncthreads();
+  const int W = (n + 31) >> 5, WN = (a.N + 31) >> 5;
+  unsigned* vis = s_bits + warp * 3 * WN;
+  unsigned long long mask = 0;
+  for (int u = warp; u < n; u += 8) {
+    const bool stored_u = end_of(u) <= edge_cap;
+    const float4 pu = s_at[u];
+    // the neighbours v > u of u, 32 candidates at a time: from its list, or by testing every later atom
+    for (int k0 = stored_u ? s_off[u] : u + 1, k_end = stored_u ? end_of(u) : n; k0 < k_end; k0 += 32) {
+      const int k = k0 + lane;
+      int v = -1;
+      if (k < k_end) {
+        if (stored_u) v = s_edge[k] > u ? s_edge[k] : -1;
+        else v = staged_bonded(a, u, pu, k, s_at[k], n) ? k : -1;
+      }
+      unsigned todo = __ballot_sync(0xffffffffu, v >= 0 && (s_link[u] != 0 || s_link[v] != 0));
+      while (todo) {                                  // one bond (u, v) at a time, the whole warp on it
+        const int src = __ffs(todo) - 1;
+        todo &= todo - 1;
+        const int vv = __shfl_sync(0xffffffffu, v, src);
+        unsigned *fr = vis + WN, *nx = fr + WN;
+        for (int w = lane; w < W; w += 32) {
+          const unsigned m = w == (u >> 5) ? 1u << (u & 31) : 0u;
+          vis[w] = m;
+          fr[w] = m;
+        }
+        __syncwarp();
+        int ring = 0;
+        for (int d = 1;; ++d) {                       // level d: the atoms at distance d from u
+          unsigned any = 0;
+          bool found = false;
+          for (int w = 0; w < W; ++w) {
+            const int j = (w << 5) + lane;
+            bool hit = false;
+            if (j < n && !((vis[w] >> lane) & 1u)) {
+              auto on_frontier = [&](int q) { return (j != vv || q != u) && ((fr[q >> 5] >> (q & 31)) & 1u); };
+              if (end_of(j) <= edge_cap) {
+                for (int e = s_off[j], e_end = end_of(j); e < e_end && !hit; ++e) hit = on_frontier(s_edge[e]);
+              } else {
+                const float4 pj = s_at[j];
+                for (int q = 0; q < n && !hit; ++q) hit = q != j && on_frontier(q) && staged_bonded(a, j, pj, q, s_at[q], n);
+              }
+            }
+            const unsigned m = __ballot_sync(0xffffffffu, hit);
+            if (lane == 0) nx[w] = m;
+            any |= m;
+            found |= w == (vv >> 5) && ((m >> (vv & 31)) & 1u);
+          }
+          if (found) { ring = d + 1; break; }
+          if (!any) break;
+          __syncwarp();
+          for (int w = lane; w < W; w += 32) vis[w] |= nx[w];
+          unsigned* t = fr; fr = nx; nx = t;
+          __syncwarp();
+        }
+        __syncwarp();                                 // the next bond's search resets the bitsets
+        if (ring) mask |= 1ull << min(ring, 63);
+      }
+    }
+  }
+  if (lane == 0) s_rmask[warp] = mask;
+  __syncthreads();
+  mask = 0;
+  for (int w = 0; w < 8; ++w) mask |= s_rmask[w];
+  return mask;
+}
+
 // One CTA per molecule. The checked atoms are compacted, in row order, into shared memory (coordinates and type; padded
 // and pocket rows are never read beyond their masks).
 // Valence: a warp per atom sums the integer bond orders of its pairs with every other atom, so the sums do not depend on
@@ -453,8 +586,10 @@ __device__ __forceinline__ unsigned long long graph_hash(const CheckArgs& a, con
 // holds the CSR offsets, the bonds follow s_row, and the colours overwrite s_at.
 // Linker hash (CHECK_NOVEL): last, the linker atoms are staged again from global memory, in row order, over whatever the
 // checks above left in the buffer, and graph_hash runs on them alone.
-// The body of the k_molecule_check kernels below; cl is read with CHECK_CLASH only, hk with CHECK_UNIQUE or CHECK_NOVEL
-// (its edge_cap) only, nv with CHECK_NOVEL only.
+// Rings (CHECK_RINGS): last, every checked atom is staged again from global memory, in row order, with its linker flag in
+// s_row; ring_mask builds its CSR over s_lab and the bitsets and bonds after s_row.
+// The body of the k_molecule_check kernels below; cl is read with CHECK_CLASH only, hk with CHECK_UNIQUE, CHECK_NOVEL or
+// CHECK_RINGS (its edge_cap) only, nv with CHECK_NOVEL or CHECK_RINGS only.
 template <int CHECKS>
 __device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashArgs& cl, const HashArgs& hk,
                                                const NovelArgs& nv) {
@@ -650,13 +785,47 @@ __device__ __forceinline__ void molecule_check(const CheckArgs& a, const ClashAr
       }
     }
   }
+  if constexpr ((CHECKS & CHECK_RINGS) != 0) {
+    const RingArgs& rg = static_cast<const RingArgs&>(nv);   // the kernel's parameter is a RingArgs
+    __syncthreads();                                  // the buffer is read above until here
+    if (tid == 0) s_n = 0;
+    __syncthreads();
+    for (int r0 = 0; r0 < a.N; r0 += 256) {           // every checked atom again, with its linker flag in s_row
+      const int r = r0 + tid;
+      bool ok = r < a.N && a.node_mask[g0 + r] != 0;
+      if (ok && a.drop_pocket) ok = a.context[(g0 + r) * a.C + a.C - 1] == 0.f;
+      const unsigned m = __ballot_sync(0xffffffffu, ok);
+      if (lane == 0) s_warp[warp] = __popc(m);
+      __syncthreads();
+      int off = s_n + __popc(m & ((1u << lane) - 1u)), total = 0;
+      for (int w = 0; w < 8; ++w) { off += w < warp ? s_warp[w] : 0; total += s_warp[w]; }
+      if (ok) {
+        s_at[off] = load_atom(a, g0, r);
+        s_row[off] = rg.linker_mask[g0 + r] != 0.f;
+      }
+      __syncthreads();
+      if (tid == 0) s_n += total;
+      __syncthreads();
+    }
+    unsigned* s_bits = reinterpret_cast<unsigned*>(s_row + a.N);
+    const unsigned long long mask = ring_mask(a, hk.edge_cap, s_n, s_at, s_lab, s_row, s_bits,
+                                              reinterpret_cast<int*>(s_bits + RING_BITSETS * ((a.N + 31) >> 5)));
+    if (tid == 0) {
+      if ((mask & ~rg.allowed) == 0) verdict |= CHECK_RINGS;
+      if (rg.ring_sizes) {                            // the take rule of the end of this function
+        if (!a.rows) rg.ring_sizes[b] = mask;
+        else if (!(a.flags[a.rows[b]] == 0 && a.s_flags[b] != 0)) rg.ring_sizes[a.rows[b]] = mask;
+      }
+    }
+  }
   if (tid == 0) {
     if (!(CHECKS & CHECK_UNIQUE) || a.passed) a.passed[b] = verdict;   // dl_molecule_hash has no verdicts
     if (a.rows) a.take[b] = !(a.flags[a.rows[b]] == 0 && a.s_flags[b] != 0);
   }
 }
 
-// The instantiations without the clash and hash bits, with the clash bit, and with the hash bit.
+// The instantiations without the clash and hash bits, with the clash bit, with the hash bit, with the linker hash bit, and
+// with the ring bit.
 template <int CHECKS>
 __global__ void __launch_bounds__(256) k_molecule_check(CheckArgs a) {
   static_assert((CHECKS & (CHECK_CLASH | CHECK_UNIQUE | CHECK_NOVEL)) == 0,
@@ -686,10 +855,31 @@ __global__ void __launch_bounds__(256, 1) k_molecule_check(CheckArgs a, ClashArg
 }
 
 template <int CHECKS>
-cudaError_t launch_molecule_check_as(const CheckArgs& a, const ClashArgs& k, const HashArgs& h, const NovelArgs& v, int B,
+__global__ void __launch_bounds__(256, 1) k_molecule_check(CheckArgs a, ClashArgs k, HashArgs h, RingArgs g) {
+  static_assert((CHECKS & CHECK_RINGS) != 0, "only the ring check takes RingArgs");
+  molecule_check<CHECKS>(a, k, h, g);
+}
+
+template <int CHECKS>
+cudaError_t launch_molecule_check_as(const CheckArgs& a, const ClashArgs& k, const HashArgs& h, const NovelArgs& v,
+                                     unsigned long long ring_allowed, unsigned long long* ring_sizes, int B,
                                      cudaStream_t st) {
   const size_t smem = (size_t)a.N * (sizeof(float4) + sizeof(int));
-  if constexpr ((CHECKS & (CHECK_UNIQUE | CHECK_NOVEL)) != 0) {
+  if constexpr ((CHECKS & CHECK_RINGS) != 0) {
+    // the hash's 24 bytes per row, the ring search's bitsets, then the bonds: HASH_EDGES_PER_ROW per row or what
+    // HASH_SMEM_MAX leaves (2560 at N = 8192). The hash stages, if any, store their bonds in the same room.
+    const size_t base = smem + (size_t)a.N * sizeof(int) + (size_t)RING_BITSETS * ((a.N + 31) / 32) * sizeof(unsigned);
+    const size_t cap = std::min((size_t)a.N * HASH_EDGES_PER_ROW, (HASH_SMEM_MAX - base) / sizeof(unsigned));
+    const size_t total = base + cap * sizeof(unsigned);
+    HashArgs hh = h;
+    hh.edge_cap = (int)cap;
+    void (*kernel)(CheckArgs, ClashArgs, HashArgs, RingArgs) = k_molecule_check<CHECKS>;
+    if (total > 48 * 1024) {
+      const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, HASH_SMEM_MAX);
+      if (err != cudaSuccess) return err;
+    }
+    kernel<<<B, 256, total, st>>>(a, k, hh, RingArgs{v, ring_allowed, ring_sizes});
+  } else if constexpr ((CHECKS & (CHECK_UNIQUE | CHECK_NOVEL)) != 0) {
     // 8 more bytes per row, then the bonds: HASH_EDGES_PER_ROW per row or what HASH_SMEM_MAX leaves (512 at N = 8192;
     // graph_hash rescans the atoms whose bonds do not fit)
     const size_t base = smem + (size_t)a.N * 2 * sizeof(int);
@@ -733,19 +923,24 @@ cudaError_t launch_molecule_check_as(const CheckArgs& a, const ClashArgs& k, con
 // launch_molecule_check_as<C> for the one C in {1, ..., sizeof...(C)} that equals checks.
 template <int... C>
 cudaError_t launch_molecule_check_of(int checks, const CheckArgs& a, const ClashArgs& k, const HashArgs& h,
-                                     const NovelArgs& v, int B, cudaStream_t st, std::integer_sequence<int, C...>) {
+                                     const NovelArgs& v, unsigned long long ring_allowed, unsigned long long* ring_sizes,
+                                     int B, cudaStream_t st, std::integer_sequence<int, C...>) {
   cudaError_t err = cudaErrorInvalidValue;
-  (void)((checks == C + 1 && ((err = launch_molecule_check_as<C + 1>(a, k, h, v, B, st)), true)) || ...);
+  (void)((checks == C + 1 &&
+          ((err = launch_molecule_check_as<C + 1>(a, k, h, v, ring_allowed, ring_sizes, B, st)), true)) || ...);
   return err;
 }
 
 // Launches k_molecule_check<checks> over B molecules; checks is a non-empty OR of CHECK_*, N <= CONN_MAX_N.
 // The shared-memory limit is raised to its one maximum the first time a molecule needs more than the default, so
 // concurrent callers never lower it under each other.
-// CHECK_UNIQUE writes the hashes to h.hash; CHECK_NOVEL reads v.
+// CHECK_UNIQUE writes the hashes to h.hash; CHECK_NOVEL reads v; CHECK_RINGS reads v.linker_mask and ring_allowed and
+// writes the masks to ring_sizes (or null).
 inline cudaError_t launch_molecule_check(int checks, const CheckArgs& a, const ClashArgs& k, const HashArgs& h, int B,
-                                         cudaStream_t st, const NovelArgs& v = NovelArgs{}) {
-  return launch_molecule_check_of(checks, a, k, h, v, B, st, std::make_integer_sequence<int, 2 * CHECK_NOVEL - 1>{});
+                                         cudaStream_t st, const NovelArgs& v = NovelArgs{},
+                                         unsigned long long ring_allowed = 0, unsigned long long* ring_sizes = nullptr) {
+  return launch_molecule_check_of(checks, a, k, h, v, ring_allowed, ring_sizes, B, st,
+                                  std::make_integer_sequence<int, 2 * CHECK_RINGS - 1>{});
 }
 
 // dl_sample_chain_retry's vetting of a caller's hash set: bad[0] = 1 if some s[i] > s[i + 1] in unsigned order.

@@ -191,7 +191,7 @@ def _check_start(sample_fn, start_step):
 
 def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                  start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                 require_novel=None, exclude_hashes=None, resamplings=None):
+                 require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
@@ -204,6 +204,8 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     `exclude_hashes` (with it) also counts those graph hashes as taken.
     `require_novel`: ... and the molecules whose linker hash is in `model.edm.known_linkers` (None uses
     `model.edm.require_novel`).
+    `require_ring_sizes`: ... and the molecules whose linker closes a smallest ring of a size not in
+    `model.edm.allowed_ring_sizes` (None uses `model.edm.require_ring_sizes`).
     `start_step` = t0 (partial diffusion, EDM.sample_chain): the template of sample_fn=None with the batch's own linker
     positions and atom types on its linker rows, sampled from step t0 -- or from one step per molecule, a 1-D sequence or
     integer tensor (EDM.sample_chain); ValueError with a sample_fn, or when the batch's linker rows do not directly follow
@@ -239,6 +241,8 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['require_unique'] = require_unique
     if require_novel is not None:
         extra['require_novel'] = require_novel
+    if require_ring_sizes is not None:
+        extra['require_ring_sizes'] = require_ring_sizes
     if exclude_hashes is not None:
         extra['exclude_hashes'] = exclude_hashes
     if start_step is not None:
@@ -253,7 +257,7 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
 
 def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                 max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                require_novel=None, resamplings=None):
+                require_novel=None, resamplings=None, require_ring_sizes=None):
     """The body of sample_chain for many batches `datas` at once, sampled in shared launches by EDM.sample_many: returns
     [(chain_k, node_mask_k)] in the order of `datas`, each equal to what sample_chain(model, datas[k], ...) returns (with
     seeds[k]) in the sense of EDM.sample_many. `model` as for sample_chain, so accelerated reference modules take it too.
@@ -272,7 +276,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
                  for k, data in enumerate(datas)]
         extra = {} if nan_retries is None else {'nan_retries': nan_retries}
         for name, v in (('require_connected', require_connected), ('require_valid', require_valid),
-                        ('require_clash_free', require_clash_free), ('require_novel', require_novel)):
+                        ('require_clash_free', require_clash_free), ('require_novel', require_novel),
+                        ('require_ring_sizes', require_ring_sizes)):
             if v is not None:
                 extra[name] = v
         requests = [kw for kw, _, _ in sized]
@@ -300,6 +305,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['require_clash_free'] = require_clash_free
     if require_novel is not None:
         extra['require_novel'] = require_novel
+    if require_ring_sizes is not None:
+        extra['require_ring_sizes'] = require_ring_sizes
     if start_step is not None:
         extra['start_step'] = start_step
     if resamplings is not None:
@@ -345,19 +352,20 @@ class DDPM(nn.Module):
 
     def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                      start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                     require_novel=None, exclude_hashes=None, resamplings=None):
+                     require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                             require_connected=require_connected, start_step=start_step, require_valid=require_valid,
                             require_clash_free=require_clash_free, linker_sizes=linker_sizes, require_unique=require_unique,
-                            require_novel=require_novel, exclude_hashes=exclude_hashes, resamplings=resamplings)
+                            require_novel=require_novel, exclude_hashes=exclude_hashes, resamplings=resamplings,
+                            require_ring_sizes=require_ring_sizes)
 
     def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                    require_novel=None, resamplings=None):
+                    require_novel=None, resamplings=None, require_ring_sizes=None):
         return sample_many(self, datas, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                            require_connected=require_connected, max_molecules=max_molecules, start_step=start_step,
                            require_valid=require_valid, require_clash_free=require_clash_free, linker_sizes=linker_sizes,
-                           require_novel=require_novel, resamplings=resamplings)
+                           require_novel=require_novel, resamplings=resamplings, require_ring_sizes=require_ring_sizes)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

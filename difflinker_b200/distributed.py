@@ -190,7 +190,7 @@ def slice_sampler_inputs(kw: dict, lo: int, hi: int):
 
 def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=True, seeds=None, nan_retries=None,
                          require_connected=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                         require_novel=None):
+                         require_novel=None, require_ring_sizes=None):
     """Strong scaling of ONE batch (SURVEY.md section 8(e)): the template batch is built once (so every rank pads to the same
     N), each rank runs the reverse loop for its contiguous slice of the molecules with the slice's rows of the full-batch
     noise, and the chains are gathered -- the result equals `model.sample_chain(data)` on one GPU bit for bit, for any
@@ -203,7 +203,8 @@ def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=T
     `require_connected` (with seeds): each rank also resamples its own disconnected molecules; `model.edm.last_connected`
     holds the rank's rows. `require_valid` likewise for the molecules with an atom beyond its valence (`last_valid`), and
     `require_clash_free` for those whose linker clashes with the pocket (`last_clash_free`), and `require_novel` for those
-    whose linker hash is in `model.edm.known_linkers` (`last_novel`). `linker_sizes` is refused
+    whose linker hash is in `model.edm.known_linkers` (`last_novel`), and `require_ring_sizes` for those whose linker closes
+    a ring of a size not in `model.edm.allowed_ring_sizes` (`last_ring_sizes_ok`). `linker_sizes` is refused
     (ValueError): sample the batch with ddpm.sample_chain(linker_sizes=...) and EDM.devices instead."""
     if linker_sizes is not None:
         raise ValueError("sample_chain_sharded does not take linker_sizes: use ddpm.sample_chain(linker_sizes=...), which "
@@ -225,6 +226,8 @@ def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=T
         extra['require_clash_free'] = require_clash_free
     if require_novel is not None:
         extra['require_novel'] = require_novel
+    if require_ring_sizes is not None:
+        extra['require_ring_sizes'] = require_ring_sizes
     if seeds is not None:
         chain = model.edm.sample_chain(**local, keep_frames=keep_frames, seeds=seeds_tensor(seeds, B)[lo:hi], **extra)
     else:

@@ -18,7 +18,7 @@ import torch.nn.functional as F
 from . import _native
 from .distributed import (deal_launches, device_slices, pack_requests, place_rows, plan_launches, resolve_devices,
                           slice_sampler_inputs, unpack_rows)
-from .molecule_builder import check_tables, clash_table, graph_hashes, sort_unsigned
+from .molecule_builder import check_tables, clash_table, graph_hashes, ring_size_mask, sort_unsigned
 from .noise import PredefinedNoiseSchedule
 from .utils import FoundNaNException, nan_exception_class
 
@@ -73,13 +73,15 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
     samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, require, checks,
-    passed, redraw, sets, linker_hashes) resamples the molecules that diverged (dl_sample_chain_retry_sets, which blocks until its rounds
+    passed, redraw, sets, linker_hashes, rings) resamples the molecules that diverged (dl_sample_chain_retry_sets, which blocks until its rounds
     are done) and, with `require` != 0, those that miss a required check, whose verdict bits go to `passed`; `checks` =
     (tables, clash) on the slice's device, `tables` as molecule_builder.check_tables returns them and `clash` the (T,T) clash
     table or None. `redraw` = (logits, size table, n_frag, normalised linker_x, sizes_used), device tensors, redraws the
     resampled rows' linker sizes; None keeps them. `sets` = (known, seen), sorted int64 device tensors or None, are the
     hash sets of CHECK_NOVEL and CHECK_UNIQUE; None is two empty sets. `linker_hashes`, an int64 device tensor or None,
-    receives every returned row's linker hash (CHECK_NOVEL).
+    receives every returned row's linker hash (CHECK_NOVEL). `rings` = (allowed mask, (B,) int64 device tensor), or None,
+    sets the ring sizes CHECK_RINGS allows on the engine (dl_set_ring_sizes) and receives every returned row's ring-size
+    mask (dl_last_ring_sizes).
     `start` = (t0, alpha_t0, sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of
     the call (dl_set_start_step); a StartSteps starts each row at its own step (dl_set_start_steps). `resample` = (r, T,
     jump) runs r RePaint passes per step, set on the engine for the duration of the call (dl_set_resamplings). Returns
@@ -107,19 +109,24 @@ def _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry):
     if stream is None:
         return _native.check(lib.dl_sample_chain_host(eng, *head, noise.data_ptr(), *tail), "dl_sample_chain_host"), 0
     if retry is not None:
-        max_retries, used, attempts, require, checks, passed, redraw, sets, linker_hashes = retry
+        max_retries, used, attempts, require, checks, passed, redraw, sets, linker_hashes, rings = retry
         ck = _native.DLMoleculeChecks.of(require, *checks) if require else None
+        if rings is not None:
+            _native.check(lib.dl_set_ring_sizes(eng, rings[0]), "dl_set_ring_sizes")
         hs = None if sets is None else _native.DLHashSets.of(*sets)
         rz = sizes = None
         if redraw is not None:
             logits, table, n_frag, linker_x, sizes = redraw
             rz = _native.DLSizeRedraw(table.numel(), logits.stride(0), logits.data_ptr(), table.data_ptr(), n_frag.data_ptr(),
                                       linker_x.data_ptr())
-        return _native.check(lib.dl_sample_chain_retry_sets(
+        st = _native.check(lib.dl_sample_chain_retry_sets(
             eng, *head, seeds.data_ptr(), *tail, max_retries, used.data_ptr(), attempts.data_ptr(), ck, hs,
             passed.data_ptr() if require else None, None if linker_hashes is None else linker_hashes.data_ptr(), rz,
             None if sizes is None else sizes.data_ptr(), stream),
-            "dl_sample_chain_retry_sets"), 0
+            "dl_sample_chain_retry_sets")
+        if rings is not None:
+            _native.check(lib.dl_last_ring_sizes(eng, head[1], rings[1].data_ptr(), stream), "dl_last_ring_sizes")
+        return st, 0
     if seeds is not None:
         return _native.check(lib.dl_sample_chain_seeded(eng, *head, seeds.data_ptr(), *tail, stream),
                              "dl_sample_chain_seeded"), 0
@@ -273,6 +280,13 @@ class EDM(torch.nn.Module):
         self.known_linkers = None
         self.last_novel = None                 # calls with require_novel: the (B,) CPU bool novelty verdict of every row
         self.last_linker_hashes = None         # calls with require_novel: the (B,) CPU int64 linker hash of every row
+        # Ring sizes: likewise for the molecules whose linker closes a smallest ring of a size not in `allowed_ring_sizes`,
+        # an iterable of ints >= 3 (63 meaning 63 or more atoms; molecule_builder.ring_sizes), in the same check launch.
+        # Which sizes to allow is the caller's policy: there is no default. Same needs; False, the default, checks nothing.
+        self.require_ring_sizes = False
+        self.allowed_ring_sizes = None
+        self.last_ring_sizes_ok = None         # calls with require_ring_sizes: the (B,) CPU bool ring verdict of every row
+        self.last_ring_sizes = None            # calls with require_ring_sizes: the (B,) CPU int64 ring-size mask of every row
         self.last_sizes = None                # calls with linker_sizes: the (B,) CPU int32 linker size of every returned row
         # RePaint resampling (InpaintingEDM only): the passes of every reverse step when sample_chain / sample_many get no
         # `resamplings`; 1, the default, is the plain loop
@@ -284,6 +298,7 @@ class EDM(torch.nn.Module):
         # sample_chain call; per launch, (device, the requests it held, loop ms)
         self.last_seeds_many = self.last_attempts_many = self.last_connected_many = self.last_loop_ms_many = None
         self.last_valid_many = self.last_clash_free_many = self.last_sizes_many = self.last_novel_many = None
+        self.last_ring_sizes_ok_many = self.last_ring_sizes_many = None
 
     @property
     def devices(self):
@@ -617,7 +632,7 @@ class EDM(torch.nn.Module):
         return True
 
     def _checks(self, require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free=None,
-                require_unique=None, require_novel=None):
+                require_unique=None, require_novel=None, require_ring_sizes=None):
         """The molecule checks of a call as the OR of _native.CHECK_*; 0 checks nothing."""
         return ((_native.CHECK_CONNECTED if self._require_check('require_connected', require_connected, seeds, noise,
                                                                 batch_slice, x) else 0) |
@@ -626,7 +641,17 @@ class EDM(torch.nn.Module):
                 (_native.CHECK_CLASH if self._require_clash_free(require_clash_free, seeds, noise, batch_slice, x) else 0) |
                 (_native.CHECK_UNIQUE if self._require_check('require_unique', require_unique, seeds, noise, batch_slice, x)
                  else 0) |
-                (_native.CHECK_NOVEL if self._require_novel(require_novel, seeds, noise, batch_slice, x) else 0))
+                (_native.CHECK_NOVEL if self._require_novel(require_novel, seeds, noise, batch_slice, x) else 0) |
+                (_native.CHECK_RINGS if self._require_ring_sizes(require_ring_sizes, seeds, noise, batch_slice, x) else 0))
+
+    def _require_ring_sizes(self, value, seeds, noise, batch_slice, x):
+        """_require_check for require_ring_sizes, which also needs the `allowed_ring_sizes` policy."""
+        if (self.require_ring_sizes if value is None else value) is True and self.allowed_ring_sizes is None:
+            raise ValueError("require_ring_sizes needs the ring sizes to allow: set edm.allowed_ring_sizes (ints >= 3, 63 "
+                             "meaning 63 or more atoms; e.g. range(5, 7) for five- and six-membered rings only)")
+        if (self.require_ring_sizes if value is None else value) is True:
+            ring_size_mask(self.allowed_ring_sizes)   # ValueError for anything but ints in [3, 63]
+        return self._require_check('require_ring_sizes', value, seeds, noise, batch_slice, x)
 
     def _require_novel(self, value, seeds, noise, batch_slice, x):
         """_require_check for require_novel, which also needs the `known_linkers` set."""
@@ -716,7 +741,7 @@ class EDM(torch.nn.Module):
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                     require_novel=None, exclude_hashes=None, resamplings=None):
+                     require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -793,6 +818,14 @@ class EDM(torch.nn.Module):
         device for every call. `last_novel` (B,) CPU bool tells which rows pass, `last_linker_hashes` (B,) CPU int64 holds
         every row's linker hash, as the check launch computed it for the bit. Novel means "by this hash, against linkers hashed the same way", with the hash's limits
         above. Refusals as for require_valid, plus ValueError without `known_linkers`.
+        `require_ring_sizes` (None: the `require_ring_sizes` attribute, default False) adds a seventh, in the same rounds
+        and launch: some bond of chain[0] with a linker end (a checked atom on the linker_mask rows, with a size redraw the
+        row's returned linker rows) has a smallest ring whose size is not in `allowed_ring_sizes`, an iterable of ints >= 3
+        where 63 stands for 63 or more atoms (molecule_builder.ring_sizes, stated at DL_CHECK_RINGS in the header). The
+        bonds are decided over all the checked atoms, so rings through the fragment count; rings of fragment atoms alone do
+        not. `last_ring_sizes_ok` (B,) CPU bool tells which rows pass, `last_ring_sizes` (B,) CPU int64 holds every row's
+        ring-size mask (bit k: a smallest ring of k atoms), the one its bit was decided on. These are rings of bond_orders'
+        graph, not RDKit's SSSR. Refusals as for require_valid, plus ValueError without `allowed_ring_sizes`.
         `linker_sizes` (a LinkerSizes; ddpm.sample_chain builds it) makes every round redraw the linker size of the rows it
         resamples, from the round's seed (dl_sample_chain_retry's redraw), and rebuild their template rows at that size
         inside the padded template. The inputs must be the template of the sizes dl_size_draw gives `seeds` at attempt 0,
@@ -814,12 +847,13 @@ class EDM(torch.nn.Module):
         self.last_attempts = None
         self.last_connected = self.last_valid = self.last_clash_free = self.last_sizes = None
         self.last_unique = self.last_graph_hashes = self.last_novel = self.last_linker_hashes = None
+        self.last_ring_sizes_ok = self.last_ring_sizes = None
         start = self._start(start_step, n_samples)
         r = self._resamplings(resamplings)
         redraw = self._linker_sizes(linker_sizes, seeds, noise, batch_slice, start_step, x, linker_mask)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
         check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free,
-                             require_unique, require_novel)
+                             require_unique, require_novel, require_ring_sizes)
         sets = self._hash_sets(check, exclude_hashes, dev)
         recover = retries > 0 or check != 0 # the recovery entry point: seeds used and attempts come back
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
@@ -900,6 +934,9 @@ class EDM(torch.nn.Module):
         if check & _native.CHECK_NOVEL:
             self.last_novel = (out['passed'].cpu() & _native.CHECK_NOVEL) != 0
             self.last_linker_hashes = out['linker_hashes'].cpu()
+        if check & _native.CHECK_RINGS:
+            self.last_ring_sizes_ok = (out['passed'].cpu() & _native.CHECK_RINGS) != 0
+            self.last_ring_sizes = out['ring_sizes'].cpu()
         if out['bad']:
             exc = self._nan_exception(out['flags'], start)
             if recover:
@@ -925,7 +962,7 @@ class EDM(torch.nn.Module):
     @torch.no_grad()
     def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                    require_novel=None, resamplings=None):
+                    require_novel=None, resamplings=None, require_ring_sizes=None):
         """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
         edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
         (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
@@ -950,6 +987,8 @@ class EDM(torch.nn.Module):
         request what last_seeds, last_attempts, last_connected and last_valid would hold after its own call; `last_loop_ms_many` holds (device,
         requests, loop ms) per launch. The single-call attributes are left as they were.
         `require_novel` likewise, against `known_linkers`; `last_novel_many` holds every request's verdict.
+        `require_ring_sizes` likewise, against `allowed_ring_sizes`; `last_ring_sizes_ok_many` and `last_ring_sizes_many`
+        hold every request's verdicts and masks.
         `linker_sizes`, one LinkerSizes per request, all of one size table, redraws sizes in those rounds as in sample_chain
         (it needs `seeds`); `last_sizes_many` holds every request's sizes. Each request's sizes come from its own seeds, so
         packing does not change them.
@@ -1027,7 +1066,7 @@ class EDM(torch.nn.Module):
             raise ValueError(f"sample_many needs CUDA inputs (got {dev})")
         retries = self._nan_retries(nan_retries, seeds, None, None, x0)
         check = self._checks(require_connected, require_valid, seeds, None, None, x0, require_clash_free,
-                             require_novel=require_novel)
+                             require_novel=require_novel, require_ring_sizes=require_ring_sizes)
         sets = self._hash_sets(check, None, dev)
         recover = retries > 0 or check != 0
         redraws = None
@@ -1096,6 +1135,7 @@ class EDM(torch.nn.Module):
         seeds_many, attempts_many = list(cpu_seeds), [None] * len(requests)
         connected_many, valid_many, clash_free_many = [None] * len(requests), [None] * len(requests), [None] * len(requests)
         novel_many = [None] * len(requests)
+        rings_ok_many, rings_many = [None] * len(requests), [None] * len(requests)
         sizes_many = [None] * len(requests) if redraws is None else [rd[4].cpu() for rd in redraws]
         for (ks, _), finish in zip(launches, finishes):
             out = finish()
@@ -1109,6 +1149,8 @@ class EDM(torch.nn.Module):
                 parts['passed'] = unpack_rows(out['passed'].cpu(), rows, None)
             if out['sizes'] is not None:
                 parts['sizes'] = unpack_rows(out['sizes'].cpu(), rows, None)
+            if check & _native.CHECK_RINGS:
+                parts['ring_sizes'] = unpack_rows(out['ring_sizes'].cpu(), rows, None)
             for j, k in enumerate(ks):
                 results[k], flags[k] = parts['chain'][j], parts['flags'][j]
                 if recover:
@@ -1123,9 +1165,13 @@ class EDM(torch.nn.Module):
                     clash_free_many[k] = (parts['passed'][j] & _native.CHECK_CLASH) != 0
                 if check & _native.CHECK_NOVEL:
                     novel_many[k] = (parts['passed'][j] & _native.CHECK_NOVEL) != 0
+                if check & _native.CHECK_RINGS:
+                    rings_ok_many[k] = (parts['passed'][j] & _native.CHECK_RINGS) != 0
+                    rings_many[k] = parts['ring_sizes'][j]
         self.last_seeds_many, self.last_attempts_many, self.last_connected_many = seeds_many, attempts_many, connected_many
         self.last_valid_many, self.last_clash_free_many, self.last_sizes_many = valid_many, clash_free_many, sizes_many
         self.last_novel_many = novel_many
+        self.last_ring_sizes_ok_many, self.last_ring_sizes_many = rings_ok_many, rings_many
         self.last_loop_ms_many = [(slots[slot_of[i]][0], sorted(ks), loop_ms[i]) for i, (ks, _) in enumerate(launches)]
         for k, f in enumerate(flags):
             if f.any():
@@ -1181,6 +1227,10 @@ class EDM(torch.nn.Module):
         # CHECK_NOVEL: the linker hash the check decided every returned row's bit on
         novel = bool(check & _native.CHECK_NOVEL)
         linker_hashes = torch.empty(n_samples, dtype=torch.int64, device=dev) if novel else None
+        # CHECK_RINGS: the allowed sizes, and the ring-size mask the check decided every returned row's bit on
+        rings = bool(check & _native.CHECK_RINGS)
+        allowed = ring_size_mask(self.allowed_ring_sizes) if rings else 0
+        ring_sizes = torch.empty(n_samples, dtype=torch.int64, device=dev) if rings else None
         # size redraws: every row's size, the attempt-0 sizes on entry
         redraw = redraw if recover else None
         sizes = None if redraw is None else redraw[4].clone()
@@ -1213,15 +1263,17 @@ class EDM(torch.nn.Module):
             checks_i = None if tables is None else ([t.to(where) for t in tables], None if clash is None else clash.to(where))
             sets_i = None if sets is None else tuple(None if s is None else s.to(where) for s in sets)
             lh_i = linker_hashes if whole or not novel else torch.empty(hi - lo, dtype=torch.int64, device=where)
-            part = part + (checks_i, redraw_i, sets_i, lh_i)
+            rs_i = ring_sizes if whole or not rings else torch.empty(hi - lo, dtype=torch.int64, device=where)
+            part = part + (checks_i, redraw_i, sets_i, lh_i, rs_i)
             parts.append(part)              # alive until the flags have been read below
-            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, checks_i, redraw_i, sets_i, lh_i = part
+            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, checks_i, redraw_i, sets_i, lh_i, rs_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
             rng_i = None if rng is None else (rng[0], rng[1], rng[2] + lo, rng[3])
             calls.append((dev_i, functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
-                (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i, sets_i, lh_i) if recover else None,
+                (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i, sets_i, lh_i,
+                 (allowed, rs_i) if rings else None) if recover else None,
                 start.rows(lo, hi) if isinstance(start, StartSteps) else start, resample)))
 
         def finish():
@@ -1237,11 +1289,13 @@ class EDM(torch.nn.Module):
                     place_rows(sizes, [p[9][4] for p in parts], slices)
                 if novel:
                     place_rows(linker_hashes, [p[11] for p in parts], slices)
+                if rings:
+                    place_rows(ring_sizes, [p[12] for p in parts], slices)
             # the host sampler reports NaNs in its status; on the device, one sync per chain instead of one per step
             # (egnn.py:441), after every slice's loop and copy
             bad = _native.DL_NAN_DETECTED in [st for st, _ in results] or bool(flags.any().item())
             return dict(chain=chain, flags=flags, used=used, attempts=attempts, passed=passed, sizes=sizes,
-                        linker_hashes=linker_hashes, bad=bad, consumed=[c for _, c in results])
+                        linker_hashes=linker_hashes, ring_sizes=ring_sizes, bad=bad, consumed=[c for _, c in results])
         return calls, finish
 
 
@@ -1304,7 +1358,7 @@ class InpaintingEDM(EDM):
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                     require_novel=None, exclude_hashes=None, resamplings=None):
+                     require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -1313,7 +1367,8 @@ class InpaintingEDM(EDM):
         seeds, molecule b's 2T+3 raw draws are those of the molecule sampled alone after torch.cuda.manual_seed(seeds[b]),
         masked and projected per molecule as always. `nan_retries`, `require_connected`, `require_valid` and `require_unique`
         as in EDM.sample_chain; the checks and the hash cover every atom of the molecule. `require_novel` and
-        `exclude_hashes` as there; the linker hash covers the linker_mask rows. `start_step` raises ValueError unless None, and `require_clash_free`
+        `exclude_hashes` as there; the linker hash covers the linker_mask rows. `require_ring_sizes` as there: the rings of
+        the bonds with an end on the linker_mask rows. `start_step` raises ValueError unless None, and `require_clash_free`
         unless None or False: this loop re-noises the pocket; `linker_sizes` unless None: this model has no linker size.
         `resamplings` = r (None: the `resamplings` attribute, default 1) runs every reverse step as r RePaint passes
         (Lugmayr et al., 2022; DiffSBDD's inpaint(..., resamplings=r); dl_set_resamplings): pass u denoises as the plain
@@ -1331,7 +1386,8 @@ class InpaintingEDM(EDM):
                                     require_connected=require_connected, start_step=start_step, require_valid=require_valid,
                                     require_clash_free=require_clash_free, linker_sizes=linker_sizes,
                                     require_unique=require_unique, require_novel=require_novel,
-                                    exclude_hashes=exclude_hashes, resamplings=resamplings)
+                                    exclude_hashes=exclude_hashes, resamplings=resamplings,
+                                    require_ring_sizes=require_ring_sizes)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

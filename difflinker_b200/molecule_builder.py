@@ -6,7 +6,10 @@ the path (SURVEY.md section 8(f) rank 4). `connected` and `valence_ok` decide on
 project's own check, with no reference counterpart: whether a linker runs into the pocket. `graph_hashes` gives the hash
 behind uniqueness (compute_metrics.py's share of distinct molecules): equal for isomorphic bond graphs. `linker_hashes`
 and `known_linkers` give the linker-scoped hash behind novelty (the share of linkers not in the training set).
+`ring_sizes` and `ring_sizes_ok` give the smallest rings the linker closes, for a ring-size rule.
 """
+import operator
+
 import torch
 
 from . import _native
@@ -277,6 +280,62 @@ def _clash_check(xh, node_mask, linker_mask, pocket_only, is_geom, clash, want_c
                                          lm.data_ptr(), po.data_ptr(), 1, passed.data_ptr(),
                                          None if counts is None else counts.data_ptr(), st), "dl_clash_check")
     return passed, counts
+
+
+def ring_size_mask(sizes):
+    """The uint64 ring-size mask of an iterable of ring sizes, as a Python int: bit k for each size k, an int in [3, 63],
+    where 63 stands for every ring of 63 or more atoms (stated at DL_CHECK_RINGS in the header)."""
+    mask = 0
+    for k in sizes:
+        if isinstance(k, bool):
+            raise ValueError(f"ring sizes are ints in [3, 63] (got {k!r})")
+        try:
+            k = operator.index(k)
+        except TypeError:
+            raise ValueError(f"ring sizes are ints in [3, 63] (got {k!r})") from None
+        if not 3 <= k <= 63:
+            raise ValueError(f"ring sizes are ints in [3, 63], 63 meaning 63 or more atoms (got {k})")
+        mask |= 1 << k
+    return mask
+
+
+def ring_sizes(xh, node_mask, linker_mask, is_geom, pocket_only=None):
+    """(B,) int64 on the device, holding the uint64 bits of every molecule's ring-size mask (dl_ring_check, the check behind
+    sample_chain(require_ring_sizes=True)): bit k is set iff some bond with a linker end -- a checked atom with linker_mask
+    != 0 -- has a smallest ring of k atoms (3 <= k <= 62; bit 63: 63 or more). The checked atoms and bonds are those of
+    connected(), over the whole molecule; rings of fragment atoms alone are not counted. These are rings of bond_orders'
+    graph, not RDKit's SSSR, as stated at DL_CHECK_RINGS in the header."""
+    return _ring_check(xh, node_mask, linker_mask, is_geom, pocket_only, 0)[1]
+
+
+def ring_sizes_ok(xh, node_mask, linker_mask, is_geom, allowed, pocket_only=None):
+    """(B,) bool on the device: whether every smallest ring of a molecule's linker bonds (ring_sizes) has a size in
+    `allowed`, an iterable of ints in [3, 63], 63 meaning 63 or more atoms. A linker on no ring passes."""
+    passed, _ = _ring_check(xh, node_mask, linker_mask, is_geom, pocket_only, ring_size_mask(allowed))
+    return (passed & _native.CHECK_RINGS) != 0
+
+
+@torch.no_grad()
+def _ring_check(xh, node_mask, linker_mask, is_geom, pocket_only, allowed):
+    """dl_ring_check on a chain[0]-style batch: ((B,) int32 verdict bits, (B,) int64 masks)."""
+    dev = xh.device
+    if dev.type != 'cuda':
+        raise RuntimeError("the molecule checks run on the GPU (no CPU fallback); move the tensors to the device")
+    B, N = xh.shape[:2]
+    xs = xh.float().contiguous()
+    nm = (node_mask.reshape(B, N) != 0).to(torch.int8).contiguous()
+    lm = linker_mask.reshape(B, N).float().contiguous()
+    po = None if pocket_only is None else pocket_only.reshape(B, N, 1).float().contiguous()
+    thr1 = threshold_tables(is_geom)[0].to(dev).contiguous()
+    passed = torch.empty(B, dtype=torch.int32, device=dev)
+    masks = torch.empty(B, dtype=torch.int64, device=dev)
+    lib = _native.load_library()
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream().cuda_stream
+        _native.check(lib.dl_ring_check(B, N, thr1.shape[0], thr1.data_ptr(), xs.data_ptr(), xs.shape[2], nm.data_ptr(),
+                                        lm.data_ptr(), None if po is None else po.data_ptr(), 1, int(po is not None),
+                                        allowed, passed.data_ptr(), masks.data_ptr(), st), "dl_ring_check")
+    return passed, masks
 
 
 def build_xae_molecule(positions, atom_types, is_geom, margins=MARGINS_EDM):

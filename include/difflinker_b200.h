@@ -35,6 +35,9 @@
  *   either, also resampling the molecules whose linker   dl_sample_chain_retry_sets with DL_CHECK_NOVEL (known set) or
  *     is known, or that repeat an earlier call's          DL_CHECK_UNIQUE (seen set); dl_molecule_hash over the linker rows
  *     (novelty, compute_metrics.py; see DL_CHECK_NOVEL)   and dl_novel_check
+ *   either, also resampling the molecules whose linker   dl_sample_chain_retry with DL_CHECK_RINGS, dl_set_ring_sizes,
+ *     closes a ring of a size not allowed (see            dl_last_ring_sizes, dl_ring_check
+ *     DL_CHECK_RINGS)
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   softmax + Categorical.sample of a size model (generate.py:88-99), from dl_size_draw, dl_size_uniform
  *     the molecule's seed, and redrawn in the recovery rounds             dl_sample_chain_retry with dl_size_redraw
@@ -333,8 +336,34 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt);
  *              "known" costs one needless resample and never returns a known linker. dl_molecule_check refuses the bit (it
  *              takes no linker_mask); dl_novel_check runs it on any batch, and dl_molecule_hash over node_mask AND
  *              linker_mask gives the same linker hashes.
+ *   DL_CHECK_RINGS (a ring-size rule on the linker; compute_metrics.py reports rings after sampling) judges the smallest
+ *              ring of every bond the linker takes part in:
+ *     graph      the atoms and bonds of the checks above: checked atoms are rows with node_mask != 0, minus the pocket rows
+ *                when drop_pocket applies; two atoms are bonded when dl_bond_orders gives an order > 0. Bonds are decided
+ *                over all of the molecule's checked atoms, the same n that connectivity, valence and the graph hash H use
+ *                (not the linker-only n of the linker hash L): the bond predicate switches form at n = 25, and rings
+ *                through fragment atoms need the whole graph.
+ *     linker atoms  checked atoms with linker_mask != 0; in the recovery rounds this is the sub-batch's linker_mask, as
+ *                DL_CHECK_NOVEL reads it.
+ *     smallest ring of a bond (u, v)  the number of atoms on a shortest cycle through that bond: 1 + the shortest-path
+ *                length from u to v in the graph with that one bond removed. A bond on no cycle has no ring.
+ *     ring-size mask of a molecule  a uint64: bit k is set iff some bond with at least one linker endpoint has a smallest
+ *                ring of k atoms, for 3 <= k <= 62; bit 63 stands for any such ring of 63 or more atoms. Rings made only of
+ *                fragment atoms are not judged: they are inputs, and no resample changes them (the reasoning of
+ *                DL_CHECK_CLASH). A ring closed through both fragment and linker atoms is judged. A molecule with no linker
+ *                bond on a cycle has mask 0.
+ *              DL_CHECK_RINGS holds iff mask & ~allowed == 0, with `allowed` the caller's uint64 (dl_set_ring_sizes, or
+ *              dl_ring_check's argument), whose bits 0-2 must be clear.
+ *              Limits: these are rings of dl_bond_orders' graph. They are not RDKit's SSSR on OpenBabel-perceived bonds
+ *              (reformat_data_obabel.py), and no claim is made that the result matches CalcNumRings or the reference's
+ *              ring filter. A pair with a NaN coordinate compares false, so it is not bonded, as in the other checks.
+ *              dl_molecule_check and dl_novel_check refuse the bit; dl_ring_check runs it on any batch.
+ * dl_molecule_checks and dl_hash_sets do not grow for it: a positional initialiser of either struct fails -Wextra -Werror
+ * once the struct gains a field, and existing C callers use such initialisers. The allowed sizes are engine state
+ * (dl_set_ring_sizes) and the masks are read back with dl_last_ring_sizes.
  */
-enum { DL_CHECK_CONNECTED = 1, DL_CHECK_VALENCE = 2, DL_CHECK_CLASH = 4, DL_CHECK_UNIQUE = 8, DL_CHECK_NOVEL = 16 };
+enum { DL_CHECK_CONNECTED = 1, DL_CHECK_VALENCE = 2, DL_CHECK_CLASH = 4, DL_CHECK_UNIQUE = 8, DL_CHECK_NOVEL = 16,
+       DL_CHECK_RINGS = 32 };
 typedef struct dl_molecule_checks {
   int32_t require;             /* OR of DL_CHECK_*, at least one: which verdicts make a row fail and be resampled */
   int32_t n_types;             /* columns of h that hold the atom type */
@@ -426,7 +455,9 @@ typedef struct dl_size_redraw {
  *                live in the engine (cached by B), not in a caller buffer. DL_CHECK_NOVEL (needs thr1, thr2 and thr3) reads
  *                the linker rows of linker_mask (of the sub-batch in the rounds) and hashes them in the same launch as the
  *                other checks; through this entry its known set is empty, so every row passes it (the set is an argument
- *                of dl_sample_chain_retry_sets). Bits 32 and up are refused.
+ *                of dl_sample_chain_retry_sets). DL_CHECK_RINGS (needs thr1) reads the linker rows of linker_mask (of the
+ *                sub-batch in the rounds) and the allowed sizes of dl_set_ring_sizes, and is DL_ERR_INVALID before that
+ *                has been called on the engine; dl_last_ring_sizes returns the masks. Bits 64 and up are refused.
  *   redraw       the sizes to redraw each resampled row's linker size from (dl_size_redraw), or NULL: sizes stay fixed,
  *                and `sizes_used` is not read
  *   sizes_used   (B) int32 DEVICE in/out, required with `redraw`: the attempt-0 sizes on entry; on return, the size of every
@@ -534,6 +565,31 @@ dl_status dl_clash_check(int32_t B, int32_t N, int32_t n_types, const float* cla
 dl_status dl_molecule_hash(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
                            const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
                            uint64_t* hash, void* stream);
+/*
+ * DL_CHECK_RINGS alone, on any (B,N) batch, without an engine. DEVICE buffers, enqueued on `stream`.
+ *   thr1        (n_types,n_types) fp32, as dl_molecule_checks.thr1: the bonds
+ *   xh, node_mask, context, context_nf, drop_pocket   as dl_molecule_check: the checked atoms
+ *   linker_mask (B,N) fp32: the checked rows with linker_mask != 0 are the linker atoms
+ *   allowed     the ring sizes that pass (bits 0-2 clear), as dl_set_ring_sizes
+ *   passed      (B) int32 out: DL_CHECK_RINGS or 0
+ *   ring_sizes  (B) uint64 out or NULL: molecule b's ring-size mask
+ * 1 <= n_types <= xh_row_stride - 3, 1 <= N <= 8192.
+ */
+dl_status dl_ring_check(int32_t B, int32_t N, int32_t n_types, const float* thr1, const float* xh, int32_t xh_row_stride,
+                        const int8_t* node_mask, const float* linker_mask, const float* context, int32_t context_nf,
+                        int32_t drop_pocket, uint64_t allowed, int32_t* passed, uint64_t* ring_sizes, void* stream);
+/*
+ * The ring sizes DL_CHECK_RINGS allows in the following dl_sample_chain_retry(_sets) calls: bit k set lets a smallest ring
+ * of k atoms pass, bit 63 one of 63 or more (stated at DL_CHECK_RINGS). Sticky like dl_set_start_step; read only by calls
+ * whose checks require the bit. DL_ERR_INVALID: bits 0-2 set.
+ */
+dl_status dl_set_ring_sizes(dl_engine* e, uint64_t allowed);
+/*
+ * The ring-size mask of every returned row of the engine's last dl_sample_chain_retry(_sets) call -- the mask its
+ * DL_CHECK_RINGS bit was decided on -- copied to out, (B) uint64 DEVICE, on `stream`. DL_ERR_INVALID when that call did not
+ * require DL_CHECK_RINGS (or failed before returning rows), or had another B.
+ */
+dl_status dl_last_ring_sizes(dl_engine* e, int32_t B, uint64_t* out, void* stream);
 /* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_retry, each from its row gather to
  * its row scatter -- including the wait for the host to capture the sub-batch's step graph -- summed over the rounds; 0 when
  * no round ran. */
