@@ -11,6 +11,7 @@ EDGE_IMPLS = {"auto": 0, "simt": 1, "wgmma": 2}
 SAMPLER_LINKER, SAMPLER_INPAINT = 0, 1
 AGGREGATIONS = {"sum": 0, "mean": 1}
 CHECK_CONNECTED, CHECK_VALENCE, CHECK_CLASH, CHECK_UNIQUE, CHECK_NOVEL, CHECK_RINGS = 1, 2, 4, 8, 16, 32   # DL_CHECK_*
+CHECK_ANCHORS = 64
 COORDS_RANGE = 15.0   # EGNN hands its own coords_range=15 to every EquivariantBlock (src/egnn.py:183,209)
 
 
@@ -100,6 +101,8 @@ SYMBOLS = {
     "dl_ring_check": (_I32, [_I32, _I32, _I32, _P, _P, _I32, _P, _P, _P, _I32, _I32, C.c_uint64, _P, _P, _P]),
     "dl_set_ring_sizes": (_I32, [_P, C.c_uint64]),
     "dl_last_ring_sizes": (_I32, [_P, _I32, _P, _P]),
+    "dl_anchor_check": (_I32, [_I32, _I32, _I32, _P, _P, _I32, _P, _P, _P, _P, _I32, _I32, _P, _P, _P]),
+    "dl_set_anchors": (_I32, [_P, _I32, _I32, _P, _P]),
     "dl_molecule_hash": (_I32, [_I32, _I32, C.POINTER(DLMoleculeChecks), _P, _I32, _P, _P, _I32, _I32, _P, _P]),
     "dl_last_retry_ms": (_F, [_P]),
     "dl_set_noise_slice": (_I32, [_P, _I32, _I32]),

@@ -150,6 +150,11 @@ struct dl_engine {
   unsigned long long ring_allowed = 0;
   HostStage ring_masks;
   int ring_B = 0;
+  // dl_set_anchors: the (anchors_B, anchors_N) int8 anchor flags of the next dl_sample_chain_retry call, which clears
+  // anchors_set; the buffer is kept, grown to the largest B * N
+  HostStage anchors;
+  bool anchors_set = false;
+  int anchors_B = 0, anchors_N = 0;
   cudaEvent_t ev_r0 = nullptr, ev_r1 = nullptr, ev_g0 = nullptr, ev_g1 = nullptr;
   float retry_ms = 0.f;
   cudaStream_t loop_stream = nullptr;
@@ -889,6 +894,7 @@ dl_status dl_destroy(dl_engine* e) {
   if (e->start_rows.buf) cudaFree(e->start_rows.buf);
   if (e->hashes.buf) cudaFree(e->hashes.buf);
   if (e->ring_masks.buf) cudaFree(e->ring_masks.buf);
+  if (e->anchors.buf) cudaFree(e->anchors.buf);
   if (e->wblob) cudaFree(e->wblob);
   if (e->wblob_tc) cudaFree(e->wblob_tc);
   if (e->coef_dev) cudaFree(e->coef_dev);
@@ -1144,6 +1150,26 @@ dl_status dl_set_ring_sizes(dl_engine* e, uint64_t allowed) {
   }
   e->ring_allowed = allowed;
   e->ring_set = true;
+  return DL_OK;
+}
+
+dl_status dl_set_anchors(dl_engine* e, int32_t B, int32_t N, const int8_t* anchors, void* stream) {
+  const char* why = nullptr;
+  if (!e) why = "null engine";
+  else if (B < 1 || N < 1) why = "B and N must be >= 1";
+  else if (!anchors) why = "null anchors";
+  if (why) { set_err("dl_set_anchors: %s", why); return DL_ERR_INVALID; }
+  CK(cudaSetDevice(e->cfg.device));
+  e->anchors_set = false;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  StageLayout al;
+  const int i_an = al.out((size_t)B * N);
+  dl_status s = stage_inputs(e->anchors, al, st);
+  if (s != DL_OK) return s;
+  CK(cudaMemcpyAsync(al.at<int8_t>(i_an), anchors, (size_t)B * N, cudaMemcpyDefault, st));
+  e->anchors_set = true;
+  e->anchors_B = B;
+  e->anchors_N = N;
   return DL_OK;
 }
 
@@ -1416,29 +1442,30 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt) { return retry_seed(seed,
 namespace {
 
 static_assert(CHECK_CONNECTED == DL_CHECK_CONNECTED && CHECK_VALENCE == DL_CHECK_VALENCE && CHECK_CLASH == DL_CHECK_CLASH &&
-              CHECK_UNIQUE == DL_CHECK_UNIQUE && CHECK_NOVEL == DL_CHECK_NOVEL && CHECK_RINGS == DL_CHECK_RINGS,
-              "kernels_retry.cuh vs header");
+              CHECK_UNIQUE == DL_CHECK_UNIQUE && CHECK_NOVEL == DL_CHECK_NOVEL && CHECK_RINGS == DL_CHECK_RINGS &&
+              CHECK_ANCHORS == DL_CHECK_ANCHORS, "kernels_retry.cuh vs header");
 
 // What is wrong with a caller's dl_molecule_checks for molecules of N rows whose h holds at most max_types type columns, or
 // null. The sampler takes every check; dl_molecule_check the bond checks only (the clash check has dl_clash_check,
 // DL_CHECK_UNIQUE compares the molecules of one sampling call with each other, which a per-molecule check cannot, and
-// DL_CHECK_NOVEL and DL_CHECK_RINGS need a linker_mask).
+// DL_CHECK_NOVEL, DL_CHECK_RINGS and DL_CHECK_ANCHORS need a linker_mask).
 const char* checks_error(const dl_molecule_checks* ck, int N, int max_types, bool sampler) {
   if (!ck) return "null checks";
   constexpr int hashed = DL_CHECK_UNIQUE | DL_CHECK_NOVEL;
   if (sampler) {
     if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE | DL_CHECK_CLASH | DL_CHECK_UNIQUE |
-                                             DL_CHECK_NOVEL | DL_CHECK_RINGS)))
+                                             DL_CHECK_NOVEL | DL_CHECK_RINGS | DL_CHECK_ANCHORS)))
       return "checks->require must be a non-empty OR of DL_CHECK_CONNECTED, DL_CHECK_VALENCE, DL_CHECK_CLASH, "
-             "DL_CHECK_UNIQUE, DL_CHECK_NOVEL and DL_CHECK_RINGS";
+             "DL_CHECK_UNIQUE, DL_CHECK_NOVEL, DL_CHECK_RINGS and DL_CHECK_ANCHORS";
   } else if (ck->require == 0 || (ck->require & ~(DL_CHECK_CONNECTED | DL_CHECK_VALENCE))) {
     return "checks->require must be DL_CHECK_CONNECTED, DL_CHECK_VALENCE or both (the clash check runs through "
            "dl_clash_check; DL_CHECK_UNIQUE compares the molecules of a dl_sample_chain_retry call with each other, and "
            "dl_molecule_hash gives their hashes; DL_CHECK_NOVEL needs a linker_mask, and its linker hashes are "
-           "dl_molecule_hash over node_mask AND linker_mask; DL_CHECK_RINGS runs through dl_ring_check)";
+           "dl_molecule_hash over node_mask AND linker_mask; DL_CHECK_RINGS runs through dl_ring_check and "
+           "DL_CHECK_ANCHORS through dl_anchor_check)";
   }
   if (ck->n_types < 1 || ck->n_types > max_types) return "checks->n_types must be in [1, the width of the atom features]";
-  if ((ck->require & (DL_CHECK_CONNECTED | DL_CHECK_VALENCE | hashed | DL_CHECK_RINGS)) && !ck->thr1)
+  if ((ck->require & (DL_CHECK_CONNECTED | DL_CHECK_VALENCE | hashed | DL_CHECK_RINGS | DL_CHECK_ANCHORS)) && !ck->thr1)
     return "null checks->thr1";
   if ((ck->require & DL_CHECK_VALENCE) && (!ck->thr2 || !ck->thr3 || !ck->max_valence))
     return "DL_CHECK_VALENCE needs checks->thr2, thr3 and max_valence";
@@ -1465,8 +1492,16 @@ CheckArgs check_args(const dl_engine* e, const dl_molecule_checks& ck, const flo
                     e->cfg.graph_type != DL_GRAPH_FC, passed);
 }
 
-// What is wrong with the checks of a dl_sample_chain_retry call, or null.
-const char* checked_error(const dl_engine* e, int32_t sampler, int N, const dl_molecule_checks* checks) {
+// The anchor flags of a dl_sample_chain_retry call: what dl_set_anchors set since the engine's previous call, or nothing.
+struct CallAnchors {
+  bool set = false;
+  int B = 0, N = 0;
+  const int8_t* flags = nullptr;
+};
+
+// What is wrong with the checks of a dl_sample_chain_retry call of B molecules, or null.
+const char* checked_error(const dl_engine* e, int32_t sampler, int B, int N, const dl_molecule_checks* checks,
+                          const CallAnchors& an) {
   const char* why = checks_error(checks, N, e->cfg.in_node_nf, true);
   if (!why && (checks->require & DL_CHECK_CLASH)) {
     if (!checks->clash) why = "DL_CHECK_CLASH needs a clash table (checks->clash)";
@@ -1475,6 +1510,10 @@ const char* checked_error(const dl_engine* e, int32_t sampler, int N, const dl_m
   }
   if (!why && (checks->require & DL_CHECK_RINGS) && !e->ring_set)
     why = "DL_CHECK_RINGS in checks->require needs the allowed ring sizes: call dl_set_ring_sizes first";
+  if (!why && (checks->require & DL_CHECK_ANCHORS)) {
+    if (!an.set) why = "DL_CHECK_ANCHORS in checks->require needs the anchor flags: call dl_set_anchors before every call";
+    else if (an.B != B || an.N != N) why = "DL_CHECK_ANCHORS: dl_set_anchors was called with another B or N";
+  }
   return why;
 }
 
@@ -1552,13 +1591,14 @@ const char* sets_error(dl_engine* e, int require, const dl_hash_sets* hs, cudaSt
 // dl_sample_chain_retry, and with `ck` its molecule checks, whose verdicts go to `passed`: a row then fails if its NaN
 // flag is set or a required bit is missing, and a resampled row replaces the caller's unless the caller's row is finite and
 // the new one diverged. `hs` (or null) holds the known set of DL_CHECK_NOVEL and the seen set of DL_CHECK_UNIQUE;
-// `linker_hash` (or null) receives every returned row's linker hash with DL_CHECK_NOVEL.
+// `linker_hash` (or null) receives every returned row's linker hash with DL_CHECK_NOVEL. `anchors` (B, N), read with
+// DL_CHECK_ANCHORS only, are the anchor flags, which k_anchor_check reads right after the check launch.
 dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames, const float* xh,
                        const int8_t* node_mask, const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
                        const float* context, const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
                        int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
                        const dl_molecule_checks* ck, const dl_hash_sets* hs, int32_t* passed, uint64_t* linker_hash,
-                       const dl_size_redraw* rz, int32_t* sizes_used, void* stream) {
+                       const dl_size_redraw* rz, int32_t* sizes_used, const int8_t* anchors, void* stream) {
   e->retry_ms = 0.f;
   e->ring_B = 0;
   dl_status s = dl_sample_chain_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask,
@@ -1591,11 +1631,22 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     if ((s = stage_inputs(e->ring_masks, rl, st)) != DL_OK) return s;
     ring_masks = reinterpret_cast<unsigned long long*>(e->ring_masks.buf);
   }
+  // DL_CHECK_ANCHORS has a launch of its own after the check launch (which takes the other bits, if any), before the
+  // uniqueness verdict, whose eligible candidates need every other required bit
+  const int mol = require & ~DL_CHECK_ANCHORS;
+  const bool anchored = (require & DL_CHECK_ANCHORS) != 0;
   if (ck) {
     const ClashArgs cl{linker_mask, ck->clash, nullptr};   // the clash check's linker rows and table
-    CK(launch_molecule_check(require, check_args(e, *ck, chain, N, node_mask, context, passed), cl, HashArgs{hash, 0}, B,
-                             st, NovelArgs{linker_mask, kn, n_known, lh}, e->ring_allowed, ring_masks));
-    e->launches += 1;
+    const CheckArgs ca = check_args(e, *ck, chain, N, node_mask, context, passed);
+    if (mol) {
+      CK(launch_molecule_check(mol, ca, cl, HashArgs{hash, 0}, B, st, NovelArgs{linker_mask, kn, n_known, lh},
+                               e->ring_allowed, ring_masks));
+      e->launches += 1;
+    }
+    if (anchored) {
+      CK(launch_anchor_check(ca, AnchorArgs{linker_mask, anchors, nullptr, mol != 0}, B, st));
+      e->launches += 1;
+    }
     if (unique) {                                          // every row is a candidate; the only keepers are the seen set
       UniqueArgs u{};
       u.B = B; u.require = require; u.hash = hash; u.flags = nan_flags; u.passed = passed;
@@ -1671,9 +1722,15 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
       CheckArgs ca = check_args(e, *ck, sa.s_chain, N, ga.s_node_mask, ga.s_context, sl.at<int32_t>(i_ps));
       ca.rows = ga.rows; ca.flags = nan_flags; ca.s_flags = sa.s_flags; ca.take = sl.at<int32_t>(i_tk);
       const HashArgs ha{sl.at<unsigned long long>(i_sh), 0};
-      CK(launch_molecule_check(require, ca, ClashArgs{ga.s_linker_mask, ck->clash, nullptr}, ha, Bs, st,
-                               NovelArgs{ga.s_linker_mask, kn, n_known, lh}, e->ring_allowed, ring_masks));
-      e->launches += 1;
+      if (mol) {
+        CK(launch_molecule_check(mol, ca, ClashArgs{ga.s_linker_mask, ck->clash, nullptr}, ha, Bs, st,
+                                 NovelArgs{ga.s_linker_mask, kn, n_known, lh}, e->ring_allowed, ring_masks));
+        e->launches += 1;
+      }
+      if (anchored) {                                      // the caller's row rows[i], row for row
+        CK(launch_anchor_check(ca, AnchorArgs{ga.s_linker_mask, anchors, nullptr, mol != 0}, Bs, st));
+        e->launches += 1;
+      }
       sa.take = ca.take; sa.s_passed = ca.passed; sa.passed = passed;
       if (rz) k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa, za);
       else k_scatter_rows<true><<<dim3(Bs, keep_frames), 256, 0, st>>>(sa);
@@ -1722,12 +1779,16 @@ dl_status retry_entry(const char* name, dl_engine* e, int32_t sampler, int32_t B
                       int32_t* attempts, const dl_molecule_checks* checks, const dl_hash_sets* sets, int32_t* passed,
                       uint64_t* linker_hash, const dl_size_redraw* redraw, int32_t* sizes_used, void* stream) {
   if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
+  CallAnchors an;                                          // read and cleared by every call, whatever it requires
+  an.set = e->anchors_set; an.B = e->anchors_B; an.N = e->anchors_N;
+  an.flags = reinterpret_cast<const int8_t*>(e->anchors.buf);
+  e->anchors_set = false;
   if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
   if (!nan_flags || !seeds_used || !attempts || (checks && !passed) || (redraw && !sizes_used)) {
     set_err("%s: null argument (nan_flags, seeds_used, attempts, passed with checks or sizes_used with redraw)", name);
     return DL_ERR_INVALID;
   }
-  const char* why = checks ? checked_error(e, sampler, N, checks) : nullptr;
+  const char* why = checks ? checked_error(e, sampler, B, N, checks, an) : nullptr;
   if (!why && linker_hash && !(checks && (checks->require & DL_CHECK_NOVEL)))
     why = "linker_hash needs checks with DL_CHECK_NOVEL";
   if (!why && sets && !checks) why = "sets need checks: the known set is read with DL_CHECK_NOVEL, the seen set with "
@@ -1745,7 +1806,7 @@ dl_status retry_entry(const char* name, dl_engine* e, int32_t sampler, int32_t B
   }
   return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
                       coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, sets, passed, linker_hash,
-                      redraw, sizes_used, stream);
+                      redraw, sizes_used, an.flags, stream);
 }
 
 }  // namespace
@@ -1832,8 +1893,9 @@ dl_status dl_novel_check(int32_t B, int32_t N, const dl_molecule_checks* checks,
   const char* why = checks_error(checks, N, xh_row_stride - 3, true);
   const int require = checks ? checks->require : 0;
   int dev = 0;
-  if (!why && (require & DL_CHECK_RINGS))
-    why = "checks->require must be an OR of DL_CHECK_NOVEL and the bits below (DL_CHECK_RINGS runs through dl_ring_check)";
+  if (!why && (require & (DL_CHECK_RINGS | DL_CHECK_ANCHORS)))
+    why = "checks->require must be an OR of DL_CHECK_NOVEL and the bits below (DL_CHECK_RINGS runs through dl_ring_check, "
+          "DL_CHECK_ANCHORS through dl_anchor_check)";
   else if (!why && !(require & DL_CHECK_NOVEL)) why = "checks->require must include DL_CHECK_NOVEL";
   else if (!why && (B <= 0 || N <= 0 || !xh || !node_mask || !linker_mask || !passed ||
                     (drop_pocket && (!context || context_nf < 1))))
@@ -1892,6 +1954,25 @@ dl_status dl_ring_check(int32_t B, int32_t N, int32_t n_types, const float* thr1
   ca.node_mask = node_mask; ca.C = context_nf; ca.context = context; ca.drop_pocket = drop_pocket != 0; ca.passed = passed;
   CK(launch_molecule_check(CHECK_RINGS, ca, ClashArgs{}, HashArgs{}, B, st, NovelArgs{linker_mask, nullptr, 0, nullptr},
                            allowed, reinterpret_cast<unsigned long long*>(ring_sizes)));
+  return DL_OK;
+}
+
+dl_status dl_anchor_check(int32_t B, int32_t N, int32_t n_types, const float* thr1, const float* xh, int32_t xh_row_stride,
+                          const int8_t* node_mask, const float* linker_mask, const int8_t* anchors, const float* context,
+                          int32_t context_nf, int32_t drop_pocket, int32_t* passed, int32_t* attachments, void* stream) {
+  const char* why = nullptr;
+  if (B <= 0 || N <= 0) why = "B and N must be >= 1";
+  else if (N > CONN_MAX_N) why = "the molecule checks take N <= 8192";
+  else if (n_types < 1 || n_types > xh_row_stride - 3) why = "n_types must be in [1, xh_row_stride - 3]";
+  else if (!thr1 || !xh || !node_mask || !linker_mask || !anchors || !passed ||
+           (drop_pocket && (!context || context_nf < 1)))
+    why = "invalid argument";
+  if (why) { set_err("dl_anchor_check: %s", why); return DL_ERR_INVALID; }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CheckArgs ca{};
+  ca.xh = xh; ca.N = N; ca.row_stride = xh_row_stride; ca.n_types = n_types; ca.thr1 = thr1;
+  ca.node_mask = node_mask; ca.C = context_nf; ca.context = context; ca.drop_pocket = drop_pocket != 0; ca.passed = passed;
+  CK(launch_anchor_check(ca, AnchorArgs{linker_mask, anchors, attachments, 0}, B, st));
   return DL_OK;
 }
 

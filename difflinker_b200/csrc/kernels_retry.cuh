@@ -233,8 +233,10 @@ __global__ void __launch_bounds__(256) k_scatter_rows(RowScatterArgs a, RowSizeA
 // in the caller's sorted set of known linker hashes (stated at DL_CHECK_NOVEL in the header).
 // CHECK_RINGS: the bit is set iff the molecule's ring-size mask -- the smallest ring of every bond with a linker end, over
 // the graph of all its checked atoms -- lies inside the caller's allowed mask (stated at DL_CHECK_RINGS in the header).
+// CHECK_ANCHORS: the bit is set iff the linker bonds to each anchor by exactly one bond and to no other fragment atom
+// (stated at DL_CHECK_ANCHORS in the header). It runs in k_anchor_check, a launch of its own after k_molecule_check.
 constexpr int CHECK_CONNECTED = 1, CHECK_VALENCE = 2, CHECK_CLASH = 4, CHECK_UNIQUE = 8;   // DL_CHECK_* of the header
-constexpr int CHECK_NOVEL = 16, CHECK_RINGS = 32;
+constexpr int CHECK_NOVEL = 16, CHECK_RINGS = 32, CHECK_ANCHORS = 64;
 constexpr int CONN_MAX_N = 8192;                                     // rows per molecule: 20 bytes of shared memory each
 constexpr int CONN_SMEM_MAX = CONN_MAX_N * (int)(sizeof(float4) + sizeof(int));
 // With CHECK_UNIQUE a molecule also takes 8 bytes per row (the atoms' rows and the CSR offsets) and 4 bytes per stored
@@ -941,6 +943,107 @@ inline cudaError_t launch_molecule_check(int checks, const CheckArgs& a, const C
                                          unsigned long long ring_allowed = 0, unsigned long long* ring_sizes = nullptr) {
   return launch_molecule_check_of(checks, a, k, h, v, ring_allowed, ring_sizes, B, st,
                                   std::make_integer_sequence<int, 2 * CHECK_RINGS - 1>{});
+}
+
+// What CHECK_ANCHORS reads and writes besides CheckArgs, whose xh, N, row_stride, n_types, thr1, node_mask, context, C,
+// drop_pocket and passed it reads, and in a recovery round rows, flags, s_flags and take.
+struct AnchorArgs {
+  const float* linker_mask;              // (B, N): the checked atoms with linker_mask != 0 are the linker atoms
+  const int8_t* anchors;                 // (B, N): the anchor flags of molecule b at row b, or in a recovery round at the
+                                         // caller's row rows[b] (the fragment rows keep their positions in the sub-batch)
+  int32_t* attachments;                  // (B, N) or null: a_i on every fragment atom, 0 on every other row; at row b, or in
+                                         // a recovery round at the caller's row rows[b], where the row is taken
+  int or_into;                           // 1: ORs the bit into passed[b], which k_molecule_check wrote; 0: writes passed[b]
+                                         // (and take[b] in a round), with no k_molecule_check launch before it
+};
+// Shared memory per row: the staged atom, its role (row, linker and anchor bits) and the linker atoms' list.
+constexpr int ANCHOR_SMEM_PER_ROW = (int)(sizeof(float4) + 2 * sizeof(int));
+constexpr int ANCHOR_LINKER = 1 << 30, ANCHOR_FLAG = 1 << 29, ANCHOR_ROW = (1 << 29) - 1;
+
+// One CTA per molecule. The checked atoms are compacted, in row order, into shared memory as k_molecule_check compacts them
+// (so the pair orientation and n of staged_bonded are the other bits'), with their role beside them; the linker atoms' staged
+// indices are listed in the same pass. A warp per fragment atom i then counts, lanes over the linker atoms, the bonds a_i
+// between i and the linker, and the counts are reduced by shuffles: no atomics, and neither a_i nor the verdict depends on
+// the order the lanes or warps run in. (As for k_molecule_check, a minimum of one CTA per SM lets ptxas take the registers
+// it needs without spilling.)
+__global__ void __launch_bounds__(256, 1) k_anchor_check(CheckArgs a, AnchorArgs g) {
+  extern __shared__ float4 s_at[];                    // [n]: x, y, z, type (int bits)
+  int* s_role = reinterpret_cast<int*>(s_at + a.N);   // [n]: row | ANCHOR_LINKER | ANCHOR_FLAG
+  int* s_lnk = s_role + a.N;                          // [n_linker]: the staged indices of the linker atoms, ascending
+  __shared__ int s_warp[8], s_lwarp[8], s_n, s_nl;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int b = blockIdx.x;
+  const size_t g0 = (size_t)b * a.N;
+  const bool take = !a.rows || !(a.flags[a.rows[b]] == 0 && a.s_flags[b] != 0);   // k_molecule_check's take rule
+  const size_t caller0 = (size_t)(a.rows ? a.rows[b] : b) * a.N;
+  int32_t* att = g.attachments && take ? g.attachments + caller0 : nullptr;
+  if (tid == 0) s_n = s_nl = 0;
+  __syncthreads();
+  for (int r0 = 0; r0 < a.N; r0 += 256) {
+    const int r = r0 + tid;
+    bool ok = r < a.N && a.node_mask[g0 + r] != 0;
+    if (ok && a.drop_pocket) ok = a.context[(g0 + r) * a.C + a.C - 1] == 0.f;
+    const bool linker = ok && g.linker_mask[g0 + r] != 0.f;
+    const unsigned m = __ballot_sync(0xffffffffu, ok), ml = __ballot_sync(0xffffffffu, linker);
+    if (lane == 0) { s_warp[warp] = __popc(m); s_lwarp[warp] = __popc(ml); }
+    __syncthreads();
+    const unsigned below = (1u << lane) - 1u;
+    int off = s_n + __popc(m & below), loff = s_nl + __popc(ml & below), total = 0, ltotal = 0;
+    for (int w = 0; w < 8; ++w) {
+      off += w < warp ? s_warp[w] : 0; total += s_warp[w];
+      loff += w < warp ? s_lwarp[w] : 0; ltotal += s_lwarp[w];
+    }
+    if (ok) {
+      s_at[off] = load_atom(a, g0, r);
+      s_role[off] = r | (linker ? ANCHOR_LINKER : 0) | (!linker && g.anchors[caller0 + r] != 0 ? ANCHOR_FLAG : 0);
+      if (linker) s_lnk[loff] = off;
+    }
+    if (att && r < a.N && (!ok || linker)) att[r] = 0;   // the fragment atoms' rows are written below
+    __syncthreads();
+    if (tid == 0) { s_n += total; s_nl += ltotal; }
+    __syncthreads();
+  }
+  const int n = s_n, n_linker = s_nl;
+  int bad = 0, anchored = 0;
+  for (int i = warp; i < n; i += 8) {                 // warp per fragment atom i, lanes over the linker atoms
+    const int role = s_role[i];
+    if (role & ANCHOR_LINKER) continue;
+    anchored |= role & ANCHOR_FLAG;
+    const float4 pi = s_at[i];
+    int c = 0;
+    for (int k = lane; k < n_linker; k += 32) {
+      const int j = s_lnk[k];
+      c += staged_bonded(a, i, pi, j, s_at[j], n);
+    }
+    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if (lane == 0) {
+      bad |= c != ((role & ANCHOR_FLAG) ? 1 : 0);
+      if (att) att[role & ANCHOR_ROW] = c;
+    }
+  }
+  const bool any_anchor = __syncthreads_or(anchored) != 0;
+  const bool ok = !any_anchor || !__syncthreads_or(bad);   // a molecule with no anchor passes
+  if (tid == 0) {
+    if (g.or_into) {
+      if (ok) a.passed[b] |= CHECK_ANCHORS;
+    } else {
+      a.passed[b] = ok ? CHECK_ANCHORS : 0;
+      if (a.rows) a.take[b] = take;
+    }
+  }
+}
+
+// Launches k_anchor_check over B molecules, N <= CONN_MAX_N. The shared-memory limit is raised to its one maximum the first
+// time a molecule needs more than the default, as launch_molecule_check raises it.
+inline cudaError_t launch_anchor_check(const CheckArgs& a, const AnchorArgs& g, int B, cudaStream_t st) {
+  const size_t smem = (size_t)a.N * ANCHOR_SMEM_PER_ROW;
+  if (smem > 48 * 1024) {
+    const cudaError_t err = cudaFuncSetAttribute(k_anchor_check, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 CONN_MAX_N * ANCHOR_SMEM_PER_ROW);
+    if (err != cudaSuccess) return err;
+  }
+  k_anchor_check<<<B, 256, smem, st>>>(a, g);
+  return cudaGetLastError();
 }
 
 // dl_sample_chain_retry's vetting of a caller's hash set: bad[0] = 1 if some s[i] > s[i + 1] in unsigned order.

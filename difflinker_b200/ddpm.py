@@ -184,6 +184,41 @@ def _final_node_mask(kw, linker_sizes, sizes):
     return (torch.arange(n, device=live.device)[None, :] < live[:, None]).to(kw['node_mask'].dtype)[:, :, None]
 
 
+def template_anchors(model, data, n_nodes):
+    """The (B, n_nodes) anchor flags of the sampling template of `data` padded to n_nodes rows: the batch's 'anchors' on
+    its fragment rows, which the template keeps in place (create_templates_for_linker_generation), and 0 on every other
+    row; an inpainting model samples the batch itself, so its flags are the batch's."""
+    anchors = data['anchors']
+    B, n_old = anchors.shape[:2]
+    anchors = anchors.reshape(B, n_old)
+    if model.inpainting:
+        return anchors
+    if n_nodes > n_old:
+        anchors = torch.cat([anchors, anchors.new_zeros((B, n_nodes - n_old))], dim=1)
+    anchors = anchors[:, :n_nodes]
+    fm = data['fragment_mask']
+    n_frag = fm.reshape(B, fm.shape[1]).sum(1).long()
+    keep = torch.arange(n_nodes, device=anchors.device)[None, :] < n_frag.to(anchors.device)[:, None]
+    return torch.where(keep, anchors, torch.zeros((), dtype=anchors.dtype, device=anchors.device))
+
+
+def _anchor_extra(model, data, n_nodes, require_anchors, extra):
+    """Adds `require_anchors` (when given) and, when the call requires the check, the template's anchors (template_anchors)
+    to the keyword arguments `extra` of edm.sample_chain."""
+    if require_anchors is not None:
+        extra['require_anchors'] = require_anchors
+    require = getattr(model.edm, 'require_anchors', False) if require_anchors is None else require_anchors
+    if require is True and 'anchors' in data:
+        extra['anchors'] = template_anchors(model, data, n_nodes)
+
+
+def _with_anchors(model, data, kw, require_anchors):
+    """The sample_many request `kw`, with the template's anchors added when the call requires the check."""
+    extra = {}
+    _anchor_extra(model, data, kw['x'].shape[1], require_anchors, extra)
+    return dict(kw, anchors=extra['anchors']) if 'anchors' in extra else kw
+
+
 def _check_start(sample_fn, start_step):
     if sample_fn is not None and start_step is not None:
         raise ValueError("start_step varies the batch's own linker, so its size is the batch's: pass no sample_fn")
@@ -191,7 +226,7 @@ def _check_start(sample_fn, start_step):
 
 def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                  start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                 require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None):
+                 require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None, require_anchors=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
@@ -206,6 +241,9 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     `model.edm.require_novel`).
     `require_ring_sizes`: ... and the molecules whose linker closes a smallest ring of a size not in
     `model.edm.allowed_ring_sizes` (None uses `model.edm.require_ring_sizes`).
+    `require_anchors`: ... and the molecules whose linker does not attach by exactly one bond at each anchor of
+    `data['anchors']` and nowhere else (None uses `model.edm.require_anchors`); the template's flags (template_anchors,
+    at the padded size with `linker_sizes`) are passed as EDM.sample_chain's `anchors`.
     `start_step` = t0 (partial diffusion, EDM.sample_chain): the template of sample_fn=None with the batch's own linker
     positions and atom types on its linker rows, sampled from step t0 -- or from one step per molecule, a 1-D sequence or
     integer tensor (EDM.sample_chain); ValueError with a sample_fn, or when the batch's linker rows do not directly follow
@@ -243,6 +281,7 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['require_novel'] = require_novel
     if require_ring_sizes is not None:
         extra['require_ring_sizes'] = require_ring_sizes
+    _anchor_extra(model, data, kw['x'].shape[1], require_anchors, extra)
     if exclude_hashes is not None:
         extra['exclude_hashes'] = exclude_hashes
     if start_step is not None:
@@ -257,7 +296,7 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
 
 def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                 max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                require_novel=None, resamplings=None, require_ring_sizes=None):
+                require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None):
     """The body of sample_chain for many batches `datas` at once, sampled in shared launches by EDM.sample_many: returns
     [(chain_k, node_mask_k)] in the order of `datas`, each equal to what sample_chain(model, datas[k], ...) returns (with
     seeds[k]) in the sense of EDM.sample_many. `model` as for sample_chain, so accelerated reference modules take it too.
@@ -265,7 +304,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
     sequential sample_chain calls call them: linker sizes, seeds and the generator's final state are theirs. `start_step`,
     one for every batch, as in sample_chain. `linker_sizes`, one for every batch, as in sample_chain: each batch's sizes
     are drawn from its own seeds and its template padded to its own N_cap, so packing changes neither;
-    `edm.last_sizes_many` holds them. `resamplings` as in sample_chain."""
+    `edm.last_sizes_many` holds them. `resamplings` and `require_anchors` as in sample_chain: each request then holds its
+    batch's template anchors."""
     _check_start(sample_fn, start_step)
     edm = model.edm
     if linker_sizes is not None:
@@ -280,7 +320,9 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
                         ('require_ring_sizes', require_ring_sizes)):
             if v is not None:
                 extra[name] = v
-        requests = [kw for kw, _, _ in sized]
+        requests = [_with_anchors(model, data, kw, require_anchors) for data, (kw, _, _) in zip(datas, sized)]
+        if require_anchors is not None:
+            extra['require_anchors'] = require_anchors
         chains = edm.sample_many(requests, keep_frames=keep_frames, seeds=[s for _, s, _ in sized],
                                  max_molecules=max_molecules, linker_sizes=[ls for _, _, ls in sized], **extra)
         return [(chain, _final_node_mask(kw, ls, sizes))
@@ -289,7 +331,7 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
     requests, drawn = [], []
     for data in datas:
         kw = sampler_inputs(model, data, sample_fn, keep_linker=start_step is not None)
-        requests.append(kw)
+        requests.append(_with_anchors(model, data, kw, require_anchors))
         x = kw['x']
         if derive and x.is_cuda:                # a host batch is refused by EDM.sample_many
             with torch.cuda.device(x.device):
@@ -307,6 +349,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['require_novel'] = require_novel
     if require_ring_sizes is not None:
         extra['require_ring_sizes'] = require_ring_sizes
+    if require_anchors is not None:
+        extra['require_anchors'] = require_anchors
     if start_step is not None:
         extra['start_step'] = start_step
     if resamplings is not None:
@@ -352,20 +396,22 @@ class DDPM(nn.Module):
 
     def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                      start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                     require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None):
+                     require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
+                     require_anchors=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                             require_connected=require_connected, start_step=start_step, require_valid=require_valid,
                             require_clash_free=require_clash_free, linker_sizes=linker_sizes, require_unique=require_unique,
                             require_novel=require_novel, exclude_hashes=exclude_hashes, resamplings=resamplings,
-                            require_ring_sizes=require_ring_sizes)
+                            require_ring_sizes=require_ring_sizes, require_anchors=require_anchors)
 
     def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                    require_novel=None, resamplings=None, require_ring_sizes=None):
+                    require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None):
         return sample_many(self, datas, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                            require_connected=require_connected, max_molecules=max_molecules, start_step=start_step,
                            require_valid=require_valid, require_clash_free=require_clash_free, linker_sizes=linker_sizes,
-                           require_novel=require_novel, resamplings=resamplings, require_ring_sizes=require_ring_sizes)
+                           require_novel=require_novel, resamplings=resamplings, require_ring_sizes=require_ring_sizes,
+                           require_anchors=require_anchors)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

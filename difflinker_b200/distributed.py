@@ -190,7 +190,7 @@ def slice_sampler_inputs(kw: dict, lo: int, hi: int):
 
 def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=True, seeds=None, nan_retries=None,
                          require_connected=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                         require_novel=None, require_ring_sizes=None):
+                         require_novel=None, require_ring_sizes=None, require_anchors=None):
     """Strong scaling of ONE batch (SURVEY.md section 8(e)): the template batch is built once (so every rank pads to the same
     N), each rank runs the reverse loop for its contiguous slice of the molecules with the slice's rows of the full-batch
     noise, and the chains are gathered -- the result equals `model.sample_chain(data)` on one GPU bit for bit, for any
@@ -204,12 +204,14 @@ def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=T
     holds the rank's rows. `require_valid` likewise for the molecules with an atom beyond its valence (`last_valid`), and
     `require_clash_free` for those whose linker clashes with the pocket (`last_clash_free`), and `require_novel` for those
     whose linker hash is in `model.edm.known_linkers` (`last_novel`), and `require_ring_sizes` for those whose linker closes
-    a ring of a size not in `model.edm.allowed_ring_sizes` (`last_ring_sizes_ok`). `linker_sizes` is refused
+    a ring of a size not in `model.edm.allowed_ring_sizes` (`last_ring_sizes_ok`), and `require_anchors` for those whose
+    linker does not attach at `data['anchors']` alone (`last_anchors_ok`; each rank takes its rows of the template's
+    anchors). `linker_sizes` is refused
     (ValueError): sample the batch with ddpm.sample_chain(linker_sizes=...) and EDM.devices instead."""
     if linker_sizes is not None:
         raise ValueError("sample_chain_sharded does not take linker_sizes: use ddpm.sample_chain(linker_sizes=...), which "
                          "EDM.devices splits over local GPUs")
-    from .ddpm import sampler_inputs
+    from .ddpm import _anchor_extra, sampler_inputs
     from .edm import seeds_tensor
     kw = sampler_inputs(model, data, sample_fn)
     B = kw['x'].shape[0]
@@ -228,6 +230,9 @@ def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=T
         extra['require_novel'] = require_novel
     if require_ring_sizes is not None:
         extra['require_ring_sizes'] = require_ring_sizes
+    _anchor_extra(model, data, kw['x'].shape[1], require_anchors, extra)
+    if 'anchors' in extra:
+        extra['anchors'] = extra['anchors'][lo:hi]
     if seeds is not None:
         chain = model.edm.sample_chain(**local, keep_frames=keep_frames, seeds=seeds_tensor(seeds, B)[lo:hi], **extra)
     else:

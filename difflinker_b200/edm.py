@@ -73,7 +73,7 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
     samples host inputs (dl_sample_chain_host). With `seeds`, `retry` = (max_retries, seeds_used, attempts, require, checks,
-    passed, redraw, sets, linker_hashes, rings) resamples the molecules that diverged (dl_sample_chain_retry_sets, which blocks until its rounds
+    passed, redraw, sets, linker_hashes, rings, anchors) resamples the molecules that diverged (dl_sample_chain_retry_sets, which blocks until its rounds
     are done) and, with `require` != 0, those that miss a required check, whose verdict bits go to `passed`; `checks` =
     (tables, clash) on the slice's device, `tables` as molecule_builder.check_tables returns them and `clash` the (T,T) clash
     table or None. `redraw` = (logits, size table, n_frag, normalised linker_x, sizes_used), device tensors, redraws the
@@ -81,7 +81,8 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     hash sets of CHECK_NOVEL and CHECK_UNIQUE; None is two empty sets. `linker_hashes`, an int64 device tensor or None,
     receives every returned row's linker hash (CHECK_NOVEL). `rings` = (allowed mask, (B,) int64 device tensor), or None,
     sets the ring sizes CHECK_RINGS allows on the engine (dl_set_ring_sizes) and receives every returned row's ring-size
-    mask (dl_last_ring_sizes).
+    mask (dl_last_ring_sizes). `anchors`, a (B, N) int8 device tensor or None, are the anchor flags CHECK_ANCHORS reads
+    (dl_set_anchors, right before the call, which clears them).
     `start` = (t0, alpha_t0, sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of
     the call (dl_set_start_step); a StartSteps starts each row at its own step (dl_set_start_steps). `resample` = (r, T,
     jump) runs r RePaint passes per step, set on the engine for the duration of the call (dl_set_resamplings). Returns
@@ -109,10 +110,12 @@ def _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry):
     if stream is None:
         return _native.check(lib.dl_sample_chain_host(eng, *head, noise.data_ptr(), *tail), "dl_sample_chain_host"), 0
     if retry is not None:
-        max_retries, used, attempts, require, checks, passed, redraw, sets, linker_hashes, rings = retry
+        max_retries, used, attempts, require, checks, passed, redraw, sets, linker_hashes, rings, anchors = retry
         ck = _native.DLMoleculeChecks.of(require, *checks) if require else None
         if rings is not None:
             _native.check(lib.dl_set_ring_sizes(eng, rings[0]), "dl_set_ring_sizes")
+        if anchors is not None:
+            _native.check(lib.dl_set_anchors(eng, head[1], head[2], anchors.data_ptr(), stream), "dl_set_anchors")
         hs = None if sets is None else _native.DLHashSets.of(*sets)
         rz = sizes = None
         if redraw is not None:
@@ -287,6 +290,11 @@ class EDM(torch.nn.Module):
         self.allowed_ring_sizes = None
         self.last_ring_sizes_ok = None         # calls with require_ring_sizes: the (B,) CPU bool ring verdict of every row
         self.last_ring_sizes = None            # calls with require_ring_sizes: the (B,) CPU int64 ring-size mask of every row
+        # Anchors: likewise for the molecules whose linker does not attach by exactly one bond at each anchor and nowhere
+        # else on the fragments (molecule_builder.attachments), in a launch right after the check launch. The anchors are
+        # per-call input (sample_chain's `anchors=`). Same needs; False, the default, checks nothing.
+        self.require_anchors = False
+        self.last_anchors_ok = None            # calls with require_anchors: the (B,) CPU bool anchor verdict of every row
         self.last_sizes = None                # calls with linker_sizes: the (B,) CPU int32 linker size of every returned row
         # RePaint resampling (InpaintingEDM only): the passes of every reverse step when sample_chain / sample_many get no
         # `resamplings`; 1, the default, is the plain loop
@@ -299,6 +307,7 @@ class EDM(torch.nn.Module):
         self.last_seeds_many = self.last_attempts_many = self.last_connected_many = self.last_loop_ms_many = None
         self.last_valid_many = self.last_clash_free_many = self.last_sizes_many = self.last_novel_many = None
         self.last_ring_sizes_ok_many = self.last_ring_sizes_many = None
+        self.last_anchors_ok_many = None
 
     @property
     def devices(self):
@@ -632,7 +641,7 @@ class EDM(torch.nn.Module):
         return True
 
     def _checks(self, require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free=None,
-                require_unique=None, require_novel=None, require_ring_sizes=None):
+                require_unique=None, require_novel=None, require_ring_sizes=None, require_anchors=None):
         """The molecule checks of a call as the OR of _native.CHECK_*; 0 checks nothing."""
         return ((_native.CHECK_CONNECTED if self._require_check('require_connected', require_connected, seeds, noise,
                                                                 batch_slice, x) else 0) |
@@ -642,7 +651,41 @@ class EDM(torch.nn.Module):
                 (_native.CHECK_UNIQUE if self._require_check('require_unique', require_unique, seeds, noise, batch_slice, x)
                  else 0) |
                 (_native.CHECK_NOVEL if self._require_novel(require_novel, seeds, noise, batch_slice, x) else 0) |
-                (_native.CHECK_RINGS if self._require_ring_sizes(require_ring_sizes, seeds, noise, batch_slice, x) else 0))
+                (_native.CHECK_RINGS if self._require_ring_sizes(require_ring_sizes, seeds, noise, batch_slice, x) else 0) |
+                (_native.CHECK_ANCHORS if self._require_check('require_anchors', require_anchors, seeds, noise, batch_slice, x)
+                 else 0))
+
+    def _anchors(self, check, anchors, x, node_mask, linker_mask, context, what="anchors"):
+        """The (B, N) int8 anchor flags on x's device of a call with the checks `check`, or None without CHECK_ANCHORS
+        (`anchors` is then not read). ValueError without `anchors`, for a shape other than (B, N) or (B, N, 1), for a flag
+        on a linker row or (on cut-off graphs) a pocket row, and for a molecule with no anchor on its atoms."""
+        if not check & _native.CHECK_ANCHORS:
+            return None
+        B, N = x.shape[:2]
+        if anchors is None:
+            raise ValueError("require_anchors needs the anchor flags: pass anchors=, a (B, N) or (B, N, 1) tensor that is "
+                             "non-zero on each molecule's anchor atoms (the batch's 'anchors', as generate.py --anchors "
+                             "sets them)")
+        if not torch.is_tensor(anchors) or tuple(anchors.shape) not in ((B, N), (B, N, 1)):
+            got = tuple(anchors.shape) if torch.is_tensor(anchors) else type(anchors).__name__
+            raise ValueError(f"{what} must be a (B, N) or (B, N, 1) tensor for B = {B}, N = {N} (got {got})")
+        flags = anchors.detach().reshape(B, N).to(x.device) != 0
+        on_linker = flags & (linker_mask.detach().reshape(B, N).to(x.device) != 0)
+        if on_linker.any():
+            b = int(on_linker.any(1).nonzero()[0])
+            raise ValueError(f"{what}: molecule {b} has an anchor flag on a linker row; anchors are fragment atoms")
+        if self.dynamics.graph_type != 'FC' and context is not None:
+            on_pocket = flags & (context.detach()[..., -1].reshape(B, N).to(x.device) != 0)
+            if on_pocket.any():
+                b = int(on_pocket.any(1).nonzero()[0])
+                raise ValueError(f"{what}: molecule {b} has an anchor flag on a pocket row; anchors are ligand fragment "
+                                 "atoms")
+        none = ~(flags & (node_mask.detach().reshape(B, N).to(x.device) != 0)).any(1)
+        if none.any():
+            b = int(none.nonzero()[0])
+            raise ValueError(f"{what}: molecule {b} has no anchor atom, so require_anchors asks nothing of it; a batch "
+                             "built without --anchors has none (set the anchors, or sample without require_anchors)")
+        return flags.to(torch.int8).contiguous()
 
     def _require_ring_sizes(self, value, seeds, noise, batch_slice, x):
         """_require_check for require_ring_sizes, which also needs the `allowed_ring_sizes` policy."""
@@ -741,7 +784,8 @@ class EDM(torch.nn.Module):
     def sample_chain(self, x, h, node_mask, fragment_mask, linker_mask, edge_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                     require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None):
+                     require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
+                     require_anchors=None, anchors=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -826,6 +870,14 @@ class EDM(torch.nn.Module):
         not. `last_ring_sizes_ok` (B,) CPU bool tells which rows pass, `last_ring_sizes` (B,) CPU int64 holds every row's
         ring-size mask (bit k: a smallest ring of k atoms), the one its bit was decided on. These are rings of bond_orders'
         graph, not RDKit's SSSR. Refusals as for require_valid, plus ValueError without `allowed_ring_sizes`.
+        `require_anchors` (None: the `require_anchors` attribute, default False) adds an eighth, in the same rounds, in a
+        launch right after the check launch: the linker of chain[0] does not attach by exactly one bond at each anchor and
+        nowhere else on the fragments (molecule_builder.attachments, stated at DL_CHECK_ANCHORS in the header). `anchors`
+        is a (B, N) or (B, N, 1) tensor, non-zero on each molecule's anchor atoms (the batch's 'anchors'; ddpm.sample_chain
+        passes them); a round reads row b's own flags, since its fragment rows keep their positions. The bonds are
+        bond_orders', over all the checked atoms. `last_anchors_ok` (B,) CPU bool tells which rows pass. Refusals as for
+        require_valid, plus ValueError without `anchors`, for a flag on a linker or pocket row, for a molecule with no
+        anchor (nothing would be asked of it) and for the wrong shape.
         `linker_sizes` (a LinkerSizes; ddpm.sample_chain builds it) makes every round redraw the linker size of the rows it
         resamples, from the round's seed (dl_sample_chain_retry's redraw), and rebuild their template rows at that size
         inside the padded template. The inputs must be the template of the sizes dl_size_draw gives `seeds` at attempt 0,
@@ -848,12 +900,14 @@ class EDM(torch.nn.Module):
         self.last_connected = self.last_valid = self.last_clash_free = self.last_sizes = None
         self.last_unique = self.last_graph_hashes = self.last_novel = self.last_linker_hashes = None
         self.last_ring_sizes_ok = self.last_ring_sizes = None
+        self.last_anchors_ok = None
         start = self._start(start_step, n_samples)
         r = self._resamplings(resamplings)
         redraw = self._linker_sizes(linker_sizes, seeds, noise, batch_slice, start_step, x, linker_mask)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
         check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free,
-                             require_unique, require_novel, require_ring_sizes)
+                             require_unique, require_novel, require_ring_sizes, require_anchors)
+        anchor_flags = self._anchors(check, anchors, x, node_mask, linker_mask, context)
         sets = self._hash_sets(check, exclude_hashes, dev)
         recover = retries > 0 or check != 0 # the recovery entry point: seeds used and attempts come back
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
@@ -891,7 +945,7 @@ class EDM(torch.nn.Module):
                                             engines, places, dev, noise=noise, dev_seeds=dev_seeds,
                                             rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check,
                                             start=start, redraw=redraw, sets=sets,
-                                            resample=self._resample(r, n_samples))
+                                            resample=self._resample(r, n_samples), anchors=anchor_flags)
         by_device = {}
         for dev_i, c in calls:
             by_device.setdefault(dev_i, []).append(c)
@@ -937,6 +991,8 @@ class EDM(torch.nn.Module):
         if check & _native.CHECK_RINGS:
             self.last_ring_sizes_ok = (out['passed'].cpu() & _native.CHECK_RINGS) != 0
             self.last_ring_sizes = out['ring_sizes'].cpu()
+        if check & _native.CHECK_ANCHORS:
+            self.last_anchors_ok = (out['passed'].cpu() & _native.CHECK_ANCHORS) != 0
         if out['bad']:
             exc = self._nan_exception(out['flags'], start)
             if recover:
@@ -962,7 +1018,7 @@ class EDM(torch.nn.Module):
     @torch.no_grad()
     def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                    require_novel=None, resamplings=None, require_ring_sizes=None):
+                    require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None):
         """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
         edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
         (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
@@ -989,6 +1045,9 @@ class EDM(torch.nn.Module):
         `require_novel` likewise, against `known_linkers`; `last_novel_many` holds every request's verdict.
         `require_ring_sizes` likewise, against `allowed_ring_sizes`; `last_ring_sizes_ok_many` and `last_ring_sizes_many`
         hold every request's verdicts and masks.
+        `require_anchors` likewise; each request then also holds `anchors`, its (B_k, N_k) or (B_k, N_k, 1) anchor flags (a
+        request may hold them without the check, which ignores them), and `last_anchors_ok_many` holds every request's
+        verdicts.
         `linker_sizes`, one LinkerSizes per request, all of one size table, redraws sizes in those rounds as in sample_chain
         (it needs `seeds`); `last_sizes_many` holds every request's sizes. Each request's sizes come from its own seeds, so
         packing does not change them.
@@ -1022,8 +1081,9 @@ class EDM(torch.nn.Module):
             if 'noise' in r or 'batch_slice' in r:
                 raise ValueError(f"request {k} passes noise= or batch_slice=: sample_many samples per-molecule streams, "
                                  "which need neither")
-            if set(r) != set(self._REQUEST_INPUTS):
-                raise ValueError(f"request {k} must hold exactly the inputs {self._REQUEST_INPUTS} (got {sorted(r)})")
+            if set(r) - {'anchors'} != set(self._REQUEST_INPUTS):
+                raise ValueError(f"request {k} must hold exactly the inputs {self._REQUEST_INPUTS}, and may hold "
+                                 f"'anchors' (got {sorted(r)})")
         if self._draws_replaced():
             raise ValueError("sample_many needs the device-side per-molecule stream, but this model's draw function is replaced")
         if seeds is None and self.noise_mode != 'per_molecule':
@@ -1066,7 +1126,10 @@ class EDM(torch.nn.Module):
             raise ValueError(f"sample_many needs CUDA inputs (got {dev})")
         retries = self._nan_retries(nan_retries, seeds, None, None, x0)
         check = self._checks(require_connected, require_valid, seeds, None, None, x0, require_clash_free,
-                             require_novel=require_novel, require_ring_sizes=require_ring_sizes)
+                             require_novel=require_novel, require_ring_sizes=require_ring_sizes,
+                             require_anchors=require_anchors)
+        anchors_many = [self._anchors(check, r.get('anchors'), r['x'], r['node_mask'], r['linker_mask'], r['context'],
+                                      f"request {k}'s anchors") for k, r in enumerate(requests)]
         sets = self._hash_sets(check, None, dev)
         recover = retries > 0 or check != 0
         redraws = None
@@ -1107,7 +1170,11 @@ class EDM(torch.nn.Module):
         for i, (ks, n) in enumerate(launches):
             dev_i, replica = slots[slot_of[i]]
             b = sum(sizes[k] for k in ks)
-            full = self._sampler_tensors(**pack_requests([requests[k] for k in ks], n, fc))
+            full = self._sampler_tensors(**pack_requests([{name: requests[k][name] for name in self._REQUEST_INPUTS}
+                                                          for k in ks], n, fc))
+            anchors = None
+            if check & _native.CHECK_ANCHORS:
+                anchors = torch.cat([torch.nn.functional.pad(anchors_many[k], (0, n - nodes[k])) for k in ks])
             dev_seeds = torch.cat([cpu_seeds[k] for k in ks]).to(dev)
             where = torch.device('cuda', dev_i)
             eng = engine_of[slot_of[i]]
@@ -1118,7 +1185,7 @@ class EDM(torch.nn.Module):
             [(_, call)], finish = self._enqueue_batch(lib, full, keep_frames, coefs[sizes[ks[0]]], [(dev_i, replica, 0, b)], [eng],
                                                       [where], dev, dev_seeds=dev_seeds, retries=retries, check=check,
                                                       start=start, redraw=redraw, sets=sets,
-                                                      resample=self._resample(r_passes, sizes[ks[0]]))
+                                                      resample=self._resample(r_passes, sizes[ks[0]]), anchors=anchors)
             finishes.append(finish)
             by_device.setdefault(dev_i, []).append(
                 functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
@@ -1136,6 +1203,7 @@ class EDM(torch.nn.Module):
         connected_many, valid_many, clash_free_many = [None] * len(requests), [None] * len(requests), [None] * len(requests)
         novel_many = [None] * len(requests)
         rings_ok_many, rings_many = [None] * len(requests), [None] * len(requests)
+        anchors_ok_many = [None] * len(requests)
         sizes_many = [None] * len(requests) if redraws is None else [rd[4].cpu() for rd in redraws]
         for (ks, _), finish in zip(launches, finishes):
             out = finish()
@@ -1168,10 +1236,13 @@ class EDM(torch.nn.Module):
                 if check & _native.CHECK_RINGS:
                     rings_ok_many[k] = (parts['passed'][j] & _native.CHECK_RINGS) != 0
                     rings_many[k] = parts['ring_sizes'][j]
+                if check & _native.CHECK_ANCHORS:
+                    anchors_ok_many[k] = (parts['passed'][j] & _native.CHECK_ANCHORS) != 0
         self.last_seeds_many, self.last_attempts_many, self.last_connected_many = seeds_many, attempts_many, connected_many
         self.last_valid_many, self.last_clash_free_many, self.last_sizes_many = valid_many, clash_free_many, sizes_many
         self.last_novel_many = novel_many
         self.last_ring_sizes_ok_many, self.last_ring_sizes_many = rings_ok_many, rings_many
+        self.last_anchors_ok_many = anchors_ok_many
         self.last_loop_ms_many = [(slots[slot_of[i]][0], sorted(ks), loop_ms[i]) for i, (ks, _) in enumerate(launches)]
         for k, f in enumerate(flags):
             if f.any():
@@ -1200,14 +1271,15 @@ class EDM(torch.nn.Module):
         return coefs, starts, keys
 
     def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
-                       retries=0, check=0, start=None, redraw=None, sets=None, resample=None):
+                       retries=0, check=0, start=None, redraw=None, sets=None, resample=None, anchors=None):
         """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
         inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
         replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
         covers the batch where it is. The draws are the per-molecule `dev_seeds`, the batch stream `rng` = (seed, offset,
         b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _checks; `start` as
         returned by _start; `redraw` as returned by _linker_sizes (its rounds then redraw sizes, into `sizes`); `sets` as
-        returned by _hash_sets, copied to each slice's device; `resample` as returned by _resample.
+        returned by _hash_sets, copied to each slice's device; `resample` as returned by _resample; `anchors` as returned
+        by _anchors, each slice's rows on its device.
         Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
         (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
         back and returns dict(chain, flags, used, attempts, passed, sizes, bad, consumed) on `dev`; `passed` holds
@@ -1264,16 +1336,17 @@ class EDM(torch.nn.Module):
             sets_i = None if sets is None else tuple(None if s is None else s.to(where) for s in sets)
             lh_i = linker_hashes if whole or not novel else torch.empty(hi - lo, dtype=torch.int64, device=where)
             rs_i = ring_sizes if whole or not rings else torch.empty(hi - lo, dtype=torch.int64, device=where)
-            part = part + (checks_i, redraw_i, sets_i, lh_i, rs_i)
+            an_i = anchors if whole or anchors is None else anchors[lo:hi].to(where).contiguous()
+            part = part + (checks_i, redraw_i, sets_i, lh_i, rs_i, an_i)
             parts.append(part)              # alive until the flags have been read below
-            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, checks_i, redraw_i, sets_i, lh_i, rs_i = part
+            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, checks_i, redraw_i, sets_i, lh_i, rs_i, an_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
             rng_i = None if rng is None else (rng[0], rng[1], rng[2] + lo, rng[3])
             calls.append((dev_i, functools.partial(
                 call, eng, self._head(hi - lo, n_nodes, keep_frames, t), (coef, norm, chain_i.data_ptr(), flags_i.data_ptr()),
                 stream, nz, sd, rng_i,
                 (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i, sets_i, lh_i,
-                 (allowed, rs_i) if rings else None) if recover else None,
+                 (allowed, rs_i) if rings else None, an_i) if recover else None,
                 start.rows(lo, hi) if isinstance(start, StartSteps) else start, resample)))
 
         def finish():
@@ -1358,7 +1431,8 @@ class InpaintingEDM(EDM):
     def sample_chain(self, x, h, node_mask, edge_mask, fragment_mask, linker_mask, context, keep_frames=None,
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
-                     require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None):
+                     require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
+                     require_anchors=None, anchors=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -1368,7 +1442,8 @@ class InpaintingEDM(EDM):
         masked and projected per molecule as always. `nan_retries`, `require_connected`, `require_valid` and `require_unique`
         as in EDM.sample_chain; the checks and the hash cover every atom of the molecule. `require_novel` and
         `exclude_hashes` as there; the linker hash covers the linker_mask rows. `require_ring_sizes` as there: the rings of
-        the bonds with an end on the linker_mask rows. `start_step` raises ValueError unless None, and `require_clash_free`
+        the bonds with an end on the linker_mask rows. `require_anchors` and `anchors` as there: the linker atoms are the
+        linker_mask rows, the fragment atoms every other atom. `start_step` raises ValueError unless None, and `require_clash_free`
         unless None or False: this loop re-noises the pocket; `linker_sizes` unless None: this model has no linker size.
         `resamplings` = r (None: the `resamplings` attribute, default 1) runs every reverse step as r RePaint passes
         (Lugmayr et al., 2022; DiffSBDD's inpaint(..., resamplings=r); dl_set_resamplings): pass u denoises as the plain
@@ -1387,7 +1462,8 @@ class InpaintingEDM(EDM):
                                     require_clash_free=require_clash_free, linker_sizes=linker_sizes,
                                     require_unique=require_unique, require_novel=require_novel,
                                     exclude_hashes=exclude_hashes, resamplings=resamplings,
-                                    require_ring_sizes=require_ring_sizes)
+                                    require_ring_sizes=require_ring_sizes, require_anchors=require_anchors,
+                                    anchors=anchors)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

@@ -6,7 +6,8 @@ the path (SURVEY.md section 8(f) rank 4). `connected` and `valence_ok` decide on
 project's own check, with no reference counterpart: whether a linker runs into the pocket. `graph_hashes` gives the hash
 behind uniqueness (compute_metrics.py's share of distinct molecules): equal for isomorphic bond graphs. `linker_hashes`
 and `known_linkers` give the linker-scoped hash behind novelty (the share of linkers not in the training set).
-`ring_sizes` and `ring_sizes_ok` give the smallest rings the linker closes, for a ring-size rule.
+`ring_sizes` and `ring_sizes_ok` give the smallest rings the linker closes, for a ring-size rule. `attachments` and
+`anchors_ok` give where the linker bonds to the fragments (compute_metrics.py's find_exit), for the anchors of --anchors.
 """
 import operator
 
@@ -336,6 +337,49 @@ def _ring_check(xh, node_mask, linker_mask, is_geom, pocket_only, allowed):
                                         lm.data_ptr(), None if po is None else po.data_ptr(), 1, int(po is not None),
                                         allowed, passed.data_ptr(), masks.data_ptr(), st), "dl_ring_check")
     return passed, masks
+
+
+def attachments(xh, node_mask, linker_mask, is_geom, pocket_only=None):
+    """(B, N) int32 on the device (dl_anchor_check, the check behind sample_chain(require_anchors=True)): a_i, the number
+    of bonds between fragment atom i -- a checked atom with linker_mask == 0 -- and the linker atoms (linker_mask != 0),
+    and 0 on every other row. The checked atoms and bonds are those of connected(), over the whole molecule, so the bond
+    predicate takes the same n. These are bond_orders' bonds, not OpenBabel's, as stated at DL_CHECK_ANCHORS in the header."""
+    B, N = xh.shape[:2]
+    anchors = torch.zeros((B, N), dtype=torch.int8, device=xh.device)
+    return _anchor_check(xh, node_mask, linker_mask, anchors, is_geom, pocket_only, True)[1]
+
+
+def anchors_ok(xh, node_mask, linker_mask, anchors, is_geom, pocket_only=None):
+    """(B,) bool on the device: whether the linker attaches by exactly one bond at each anchor -- a fragment atom whose
+    `anchors` flag, (B, N) or (B, N, 1), is non-zero -- and by none anywhere else on the fragments (attachments). Flags on
+    linker rows, pocket rows and rows that are not checked are ignored; a molecule with no anchor passes."""
+    passed, _ = _anchor_check(xh, node_mask, linker_mask, anchors, is_geom, pocket_only, False)
+    return (passed & _native.CHECK_ANCHORS) != 0
+
+
+@torch.no_grad()
+def _anchor_check(xh, node_mask, linker_mask, anchors, is_geom, pocket_only, want_attachments):
+    """dl_anchor_check on a chain[0]-style batch: ((B,) int32 verdict bits, (B, N) int32 attachments or None)."""
+    dev = xh.device
+    if dev.type != 'cuda':
+        raise RuntimeError("the molecule checks run on the GPU (no CPU fallback); move the tensors to the device")
+    B, N = xh.shape[:2]
+    xs = xh.float().contiguous()
+    nm = (node_mask.reshape(B, N) != 0).to(torch.int8).contiguous()
+    lm = linker_mask.reshape(B, N).float().contiguous()
+    an = (anchors.reshape(B, N) != 0).to(device=dev, dtype=torch.int8).contiguous()
+    po = None if pocket_only is None else pocket_only.reshape(B, N, 1).float().contiguous()
+    thr1 = threshold_tables(is_geom)[0].to(dev).contiguous()
+    passed = torch.empty(B, dtype=torch.int32, device=dev)
+    att = torch.empty((B, N), dtype=torch.int32, device=dev) if want_attachments else None
+    lib = _native.load_library()
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream().cuda_stream
+        _native.check(lib.dl_anchor_check(B, N, thr1.shape[0], thr1.data_ptr(), xs.data_ptr(), xs.shape[2], nm.data_ptr(),
+                                          lm.data_ptr(), an.data_ptr(), None if po is None else po.data_ptr(), 1,
+                                          int(po is not None), passed.data_ptr(), None if att is None else att.data_ptr(),
+                                          st), "dl_anchor_check")
+    return passed, att
 
 
 def build_xae_molecule(positions, atom_types, is_geom, margins=MARGINS_EDM):

@@ -38,6 +38,10 @@
  *   either, also resampling the molecules whose linker   dl_sample_chain_retry with DL_CHECK_RINGS, dl_set_ring_sizes,
  *     closes a ring of a size not allowed (see            dl_last_ring_sizes, dl_ring_check
  *     DL_CHECK_RINGS)
+ *   either, also resampling the molecules whose linker   dl_sample_chain_retry with DL_CHECK_ANCHORS, dl_set_anchors,
+ *     does not attach at the given anchors (--anchors,     dl_anchor_check
+ *     generate.py:130-140; find_exit, compute_metrics.py;
+ *     see DL_CHECK_ANCHORS)
  *   SizeClassifier.forward       src/linker_size_lightning.py:83-110  dl_sizegnn_create/.../dl_sizegnn_forward
  *   softmax + Categorical.sample of a size model (generate.py:88-99), from dl_size_draw, dl_size_uniform
  *     the molecule's seed, and redrawn in the recovery rounds             dl_sample_chain_retry with dl_size_redraw
@@ -358,12 +362,33 @@ uint64_t dl_retry_seed(uint64_t seed, int32_t attempt);
  *              (reformat_data_obabel.py), and no claim is made that the result matches CalcNumRings or the reference's
  *              ring filter. A pair with a NaN coordinate compares false, so it is not bonded, as in the other checks.
  *              dl_molecule_check and dl_novel_check refuse the bit; dl_ring_check runs it on any batch.
- * dl_molecule_checks and dl_hash_sets do not grow for it: a positional initialiser of either struct fails -Wextra -Werror
+ *   DL_CHECK_ANCHORS (the attachment points of generate.py's --anchors; compute_metrics.py's find_exit lists the fragment
+ *              atoms bonded to linker atoms) judges where the linker bonds to the fragments:
+ *     graph      the atoms and bonds of DL_CHECK_RINGS: checked atoms are rows with node_mask != 0, minus the pocket rows
+ *                when drop_pocket applies; two atoms are bonded when dl_bond_orders gives an order > 0, decided over all of
+ *                the molecule's checked atoms (the same n, so the n <= 25 and n > 25 forms switch where they do for the other
+ *                bits), the pair oriented by the compacted atom order.
+ *     roles      linker atoms: checked atoms with linker_mask != 0 (in the recovery rounds, the sub-batch's linker_mask, as
+ *                DL_CHECK_NOVEL reads it); fragment atoms: the other checked atoms; anchors: fragment atoms whose anchor flag
+ *                (dl_set_anchors, or dl_anchor_check's argument) is non-zero. Flags on linker rows, pocket rows and rows
+ *                that are not checked are ignored.
+ *     attachments  a_i of a fragment atom i: the number of bonds between i and a linker atom.
+ *              DL_CHECK_ANCHORS holds iff a_i == 1 for every anchor and a_i == 0 for every other fragment atom: the linker
+ *              attaches by exactly one bond at each anchor and nowhere else -- find_exit's list, repeats included, equals
+ *              the anchor set. A molecule with no anchor passes (nothing was asked of it).
+ *              Limits: these are dl_bond_orders' bonds, not OpenBabel's. An anchor that takes two linker bonds (a fused or
+ *              spiro attachment) fails by design: the training data attaches one linker bond per anchor. A pair with a NaN
+ *              coordinate compares false, so it is not bonded, as in the other checks.
+ *              The check runs in a launch of its own (k_anchor_check) right after the check launch, before the
+ *              DL_CHECK_UNIQUE verdict, which therefore sees the bit. dl_molecule_check and dl_novel_check refuse the bit;
+ *              dl_anchor_check runs it on any batch.
+ * dl_molecule_checks and dl_hash_sets do not grow for these: a positional initialiser of either struct fails -Wextra -Werror
  * once the struct gains a field, and existing C callers use such initialisers. The allowed sizes are engine state
- * (dl_set_ring_sizes) and the masks are read back with dl_last_ring_sizes.
+ * (dl_set_ring_sizes) and the masks are read back with dl_last_ring_sizes; the anchor flags are per-call engine input
+ * (dl_set_anchors).
  */
 enum { DL_CHECK_CONNECTED = 1, DL_CHECK_VALENCE = 2, DL_CHECK_CLASH = 4, DL_CHECK_UNIQUE = 8, DL_CHECK_NOVEL = 16,
-       DL_CHECK_RINGS = 32 };
+       DL_CHECK_RINGS = 32, DL_CHECK_ANCHORS = 64 };
 typedef struct dl_molecule_checks {
   int32_t require;             /* OR of DL_CHECK_*, at least one: which verdicts make a row fail and be resampled */
   int32_t n_types;             /* columns of h that hold the atom type */
@@ -457,7 +482,11 @@ typedef struct dl_size_redraw {
  *                other checks; through this entry its known set is empty, so every row passes it (the set is an argument
  *                of dl_sample_chain_retry_sets). DL_CHECK_RINGS (needs thr1) reads the linker rows of linker_mask (of the
  *                sub-batch in the rounds) and the allowed sizes of dl_set_ring_sizes, and is DL_ERR_INVALID before that
- *                has been called on the engine; dl_last_ring_sizes returns the masks. Bits 64 and up are refused.
+ *                has been called on the engine; dl_last_ring_sizes returns the masks. DL_CHECK_ANCHORS (needs thr1) reads
+ *                the linker rows of linker_mask (of the sub-batch in the rounds) and the anchor flags of dl_set_anchors (of
+ *                the caller's row, row for row, in the rounds), and is DL_ERR_INVALID unless dl_set_anchors was called with
+ *                this B and N since the engine's previous dl_sample_chain_retry(_sets) call. Without it there is no extra
+ *                launch or allocation. Bits 128 and up are refused.
  *   redraw       the sizes to redraw each resampled row's linker size from (dl_size_redraw), or NULL: sizes stay fixed,
  *                and `sizes_used` is not read
  *   sizes_used   (B) int32 DEVICE in/out, required with `redraw`: the attempt-0 sizes on entry; on return, the size of every
@@ -517,7 +546,8 @@ dl_status dl_sample_chain_retry_sets(dl_engine* e, int32_t sampler, int32_t B, i
  * 1 <= N <= 8192. require takes DL_CHECK_CONNECTED and DL_CHECK_VALENCE only; the clash check alone is dl_clash_check, and
  * DL_CHECK_UNIQUE, a verdict on molecules compared with each other, has no per-molecule form: dl_molecule_hash gives the
  * hashes it compares. DL_CHECK_NOVEL needs a linker_mask, which this entry does not take: the linker hashes are
- * dl_molecule_hash over node_mask AND linker_mask.
+ * dl_molecule_hash over node_mask AND linker_mask. DL_CHECK_RINGS runs through dl_ring_check and DL_CHECK_ANCHORS through
+ * dl_anchor_check.
  */
 dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* checks, const float* xh, int32_t xh_row_stride,
                             const int8_t* node_mask, const float* context, int32_t context_nf, int32_t drop_pocket,
@@ -527,7 +557,8 @@ dl_status dl_molecule_check(int32_t B, int32_t N, const dl_molecule_checks* chec
  * DEVICE buffers, enqueued on `stream` of the current device.
  *   checks       require includes DL_CHECK_NOVEL and may add DL_CHECK_CONNECTED, DL_CHECK_VALENCE, DL_CHECK_CLASH (needs
  *                checks->clash and drop_pocket) and DL_CHECK_UNIQUE (needs `hash`; the bit itself is a verdict over a
- *                call's rows and stays clear). Tables as for dl_sample_chain_retry.
+ *                call's rows and stays clear). Tables as for dl_sample_chain_retry. DL_CHECK_RINGS runs through
+ *                dl_ring_check and DL_CHECK_ANCHORS through dl_anchor_check.
  *   sets         known (ascending unsigned order, not checked here) or NULL: an empty set; seen is not read
  *   xh, node_mask, context, context_nf, drop_pocket   as dl_molecule_check
  *   linker_mask  (B,N) fp32: the checked rows with linker_mask != 0 are the linker atoms
@@ -573,7 +604,7 @@ dl_status dl_molecule_hash(int32_t B, int32_t N, const dl_molecule_checks* check
  *   allowed     the ring sizes that pass (bits 0-2 clear), as dl_set_ring_sizes
  *   passed      (B) int32 out: DL_CHECK_RINGS or 0
  *   ring_sizes  (B) uint64 out or NULL: molecule b's ring-size mask
- * 1 <= n_types <= xh_row_stride - 3, 1 <= N <= 8192.
+ * 1 <= n_types <= xh_row_stride - 3, 1 <= N <= 8192. It judges DL_CHECK_RINGS alone: DL_CHECK_ANCHORS is dl_anchor_check.
  */
 dl_status dl_ring_check(int32_t B, int32_t N, int32_t n_types, const float* thr1, const float* xh, int32_t xh_row_stride,
                         const int8_t* node_mask, const float* linker_mask, const float* context, int32_t context_nf,
@@ -590,6 +621,26 @@ dl_status dl_set_ring_sizes(dl_engine* e, uint64_t allowed);
  * require DL_CHECK_RINGS (or failed before returning rows), or had another B.
  */
 dl_status dl_last_ring_sizes(dl_engine* e, int32_t B, uint64_t* out, void* stream);
+/*
+ * DL_CHECK_ANCHORS alone, on any (B,N) batch, without an engine. DEVICE buffers, enqueued on `stream`.
+ *   thr1        (n_types,n_types) fp32, as dl_molecule_checks.thr1: the bonds
+ *   xh, node_mask, context, context_nf, drop_pocket   as dl_molecule_check: the checked atoms
+ *   linker_mask (B,N) fp32: the checked rows with linker_mask != 0 are the linker atoms
+ *   anchors     (B,N) int8: the anchor flags (stated at DL_CHECK_ANCHORS)
+ *   passed      (B) int32 out: DL_CHECK_ANCHORS or 0
+ *   attachments (B,N) int32 out or NULL: a_i on every fragment atom, 0 on every other row
+ * 1 <= n_types <= xh_row_stride - 3, 1 <= N <= 8192.
+ */
+dl_status dl_anchor_check(int32_t B, int32_t N, int32_t n_types, const float* thr1, const float* xh, int32_t xh_row_stride,
+                          const int8_t* node_mask, const float* linker_mask, const int8_t* anchors, const float* context,
+                          int32_t context_nf, int32_t drop_pocket, int32_t* passed, int32_t* attachments, void* stream);
+/*
+ * The anchor flags of the engine's next dl_sample_chain_retry(_sets) call: (B,N) int8 (host or DEVICE), row b's flags
+ * those of molecule b (stated at DL_CHECK_ANCHORS). Copied into an engine buffer, cached by (B,N), on `stream`. Not sticky:
+ * the next dl_sample_chain_retry(_sets) call on the engine reads the flags and clears them, whether or not its checks
+ * require DL_CHECK_ANCHORS, so per-row data never carries over to a later batch. DL_ERR_INVALID: B or N < 1, NULL anchors.
+ */
+dl_status dl_set_anchors(dl_engine* e, int32_t B, int32_t N, const int8_t* anchors, void* stream);
 /* Device time (ms, CUDA events) of the retry rounds of the most recent dl_sample_chain_retry, each from its row gather to
  * its row scatter -- including the wait for the host to capture the sub-batch's step graph -- summed over the rounds; 0 when
  * no round ran. */
