@@ -129,6 +129,14 @@ struct dl_engine {
   int resamplings = 1, resample_T = 0;
   std::vector<float> jump;
   std::vector<dl_step_coef> coef_passes;
+  // dl_set_clash_guidance: the linker sampler pushes linker atoms out of the pocket at its last guide_steps reverse steps
+  // with guide_scale, by the (guide_types, guide_types) table guide_table (pm); guide_steps = 0: off. Each sampling call
+  // uploads the table to guide_clash (guide_cap floats) on its loop stream, as it uploads its coefficient table.
+  float guide_scale = 0.f;
+  int guide_steps = 0, guide_types = 0;
+  std::vector<float> guide_table;
+  float* guide_clash = nullptr;
+  size_t guide_cap = 0;
   int64_t mol_steps = 0;       // dl_last_molecule_steps
   bool finalized = false;
   std::map<std::string, std::vector<float>> raw;
@@ -607,6 +615,19 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
   TIMED("k_finish", st, (launch_chain(per_mol ? k_finish<true> : k_finish<false>, dim3((n + 15) / 16), dim3(256), 0, st, gm, fa)));
   LAUNCH_CHECK();
   e->launches += 1;
+  if (fused_update && e->guide_steps > 0) {
+    // clash guidance (dl_set_clash_guidance): the step's z_s moved before anything reads it; the kernel returns at the
+    // steps it does not guide, so one graph serves every step
+    GuideArgs ga{};
+    ga.xh = ws.z; ga.N = N; ga.row_stride = 3 + e->cfg.in_node_nf; ga.n_types = e->guide_types; ga.C = e->cfg.context_node_nf;
+    ga.scale = e->guide_scale; ga.clash = e->guide_clash;
+    ga.node_mask = io.node_mask; ga.linker_mask = io.linker_mask; ga.context = io.context;
+    ga.step = e->step_ctr + 1; ga.T = io.T; ga.steps = e->guide_steps; ga.coef = e->coef_dev;
+    ga.chain = io.chain; ga.norm0 = io.norm0;
+    TIMED("k_clash_guide", st, (launch_clash_guide(ga, B, st)));
+    LAUNCH_CHECK();
+    e->launches += 1;
+  }
   if (e->cfg.centering || io.inpaint) {
     // per-molecule stage of inpainting models: centring of the velocity (egnn.py:444-445) and, in the sampler,
     // the whole reverse step incl. the centre-of-mass projection (edm.py:549-612)
@@ -899,6 +920,7 @@ dl_status dl_destroy(dl_engine* e) {
   if (e->wblob_tc) cudaFree(e->wblob_tc);
   if (e->coef_dev) cudaFree(e->coef_dev);
   if (e->step_ctr) cudaFree(e->step_ctr);
+  if (e->guide_clash) cudaFree(e->guide_clash);
   if (e->stage.buf) cudaFree(e->stage.buf);
   if (e->loop_stream) cudaStreamDestroy(e->loop_stream);
   if (e->ev_in) cudaEventDestroy(e->ev_in);
@@ -1141,6 +1163,20 @@ dl_status dl_set_resamplings(dl_engine* e, int32_t r, int32_t T, const float* ju
   return DL_OK;
 }
 
+dl_status dl_set_clash_guidance(dl_engine* e, float scale, int32_t steps, int32_t n_types, const float* clash) {
+  if (!e) { set_err("dl_set_clash_guidance: null engine"); return DL_ERR_INVALID; }
+  const char* why = nullptr;
+  if (!std::isfinite(scale) || scale < 0.f) why = "scale must be finite and >= 0";
+  else if (steps < 0) why = "steps must be >= 0";
+  if (why) { set_err("dl_set_clash_guidance: %s (got scale %g, steps %d)", why, (double)scale, steps); return DL_ERR_INVALID; }
+  if (steps == 0 || scale == 0.f) { e->guide_scale = 0.f; e->guide_steps = e->guide_types = 0; return DL_OK; }
+  if (n_types < 1 || !clash) { set_err("dl_set_clash_guidance: needs n_types >= 1 and a clash table"); return DL_ERR_INVALID; }
+  // a host copy: the calls already enqueued keep the table they uploaded, later calls upload this one
+  e->guide_table.assign(clash, clash + (size_t)n_types * n_types);
+  e->guide_scale = scale; e->guide_steps = steps; e->guide_types = n_types;
+  return DL_OK;
+}
+
 dl_status dl_set_ring_sizes(dl_engine* e, uint64_t allowed) {
   if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
   if (allowed & 7u) {
@@ -1237,6 +1273,20 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   }
   const int R = call_resamplings(e, sampler, T);
   if (R < 1) return DL_ERR_INVALID;
+  if (e->guide_steps > 0) {
+    const char* why = nullptr;
+    if (inpaint) why = "the inpainting sampler re-noises the pocket";
+    else if (partial || per_row) why = "it takes no start step (dl_set_start_step, dl_set_start_steps)";
+    else if (e->cfg.graph_type == DL_GRAPH_FC) why = "DL_GRAPH_FC has no pocket rows";
+    else if (e->guide_steps > T) why = "its steps exceed the call's T";
+    else if (e->guide_types > e->cfg.in_node_nf) why = "its table has more atom types than the model's features";
+    else if (N > CONN_MAX_N) why = "it takes N <= 8192";
+    else if (!context || e->cfg.context_node_nf < 1) why = "it needs the context's pocket column";
+    if (why) {
+      set_err("clash guidance (dl_set_clash_guidance): %s", why);
+      return DL_ERR_INVALID;
+    }
+  }
   // A start step t0 runs the table's last t0 + 1 rows -- steps t0-1 .. 0, then the final one -- as a loop of Tl = t0 steps:
   // loop step r reads row r of the copied rows and draw r + 1, so the draws are eps, one per step and the final one.
   const int Tl = loop_steps(e, T);
@@ -1270,12 +1320,22 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     CK(cudaMalloc((void**)&e->coef_dev, coef_bytes));
     e->coef_cap = (int)coef_bytes;
   }
+  if (e->guide_steps > 0 && e->guide_cap < e->guide_table.size()) {
+    if (e->guide_clash) cudaFree(e->guide_clash);
+    e->guide_clash = nullptr;
+    e->guide_cap = 0;
+    CK(cudaMalloc((void**)&e->guide_clash, e->guide_table.size() * sizeof(float)));
+    e->guide_cap = e->guide_table.size();
+  }
   // order the private loop stream after the caller's stream (the legacy default stream cannot be captured)
   if (user != st) {
     CK(cudaEventRecord(e->ev_in, user));
     CK(cudaStreamWaitEvent(st, e->ev_in, 0));
   }
   CK(cudaMemcpyAsync(e->coef_dev, coef, (size_t)rows * sizeof(dl_step_coef), cudaMemcpyHostToDevice, st));
+  if (e->guide_steps > 0)   // the clash-guidance table of this call, ordered on the loop stream like the coefficients
+    CK(cudaMemcpyAsync(e->guide_clash, e->guide_table.data(), e->guide_table.size() * sizeof(float), cudaMemcpyHostToDevice,
+                       st));
   const float* jump_dev = R > 1 ? e->coef_dev + (size_t)rows * 8 : nullptr;
   if (R > 1)
     CK(cudaMemcpyAsync(const_cast<float*>(jump_dev), e->jump.data(), e->jump.size() * sizeof(float), cudaMemcpyHostToDevice,
@@ -1333,6 +1393,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   if ((s = build_forward_plan(e, Bp, N, node_mask, inpaint ? nullptr : linker_mask, edge_mask, st)) != DL_OK) return s;
 
   if (time_chain) { cudaStreamSynchronize(st); tc_plan = now_ms(); }
+  if (e->guide_steps > 0) CK(clash_guide_opt_in());
   FwdIO io;
   io.sampler = true; io.inpaint = inpaint; io.xh0 = xh; io.upd_linker_mask = linker_mask;
   io.node_mask = node_mask; io.linker_mask = inpaint ? nullptr : linker_mask; io.edge_mask = edge_mask;
@@ -1934,6 +1995,27 @@ dl_status dl_clash_check(int32_t B, int32_t N, int32_t n_types, const float* cla
   ca.node_mask = node_mask; ca.C = context_nf; ca.context = context; ca.drop_pocket = 1; ca.passed = passed;
   if (clashes) CK(cudaMemsetAsync(clashes, 0, (size_t)B * N * sizeof(int32_t), st));   // the rows that are not linker atoms
   CK(launch_molecule_check(CHECK_CLASH, ca, ClashArgs{linker_mask, clash, clashes}, HashArgs{}, B, st));
+  return DL_OK;
+}
+
+dl_status dl_clash_guide(int32_t B, int32_t N, int32_t n_types, const float* clash, float scale, float* xh,
+                         int32_t xh_row_stride, const int8_t* node_mask, const float* linker_mask, const float* context,
+                         int32_t context_nf, void* stream) {
+  const char* why = nullptr;
+  if (B <= 0 || N <= 0) why = "B and N must be >= 1";
+  else if (N > CONN_MAX_N) why = "it takes N <= 8192";
+  else if (n_types < 1 || n_types > xh_row_stride - 3) why = "n_types must be in [1, xh_row_stride - 3]";
+  else if (!clash) why = "null clash table";
+  else if (!std::isfinite(scale) || scale < 0.f) why = "scale must be finite and >= 0";
+  else if (!xh || !node_mask || !linker_mask || !context || context_nf < 1) why = "invalid argument";
+  if (why) { set_err("dl_clash_guide: %s", why); return DL_ERR_INVALID; }
+  if (scale == 0.f) return DL_OK;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CK(clash_guide_opt_in());
+  GuideArgs ga{};
+  ga.xh = xh; ga.N = N; ga.row_stride = xh_row_stride; ga.n_types = n_types; ga.C = context_nf;
+  ga.scale = scale; ga.clash = clash; ga.node_mask = node_mask; ga.linker_mask = linker_mask; ga.context = context;
+  CK(launch_clash_guide(ga, B, st));
   return DL_OK;
 }
 

@@ -319,8 +319,21 @@ __host__ __device__ inline bool sorted_contains(const unsigned long long* s, lon
   return lo < n && s[lo] == v;
 }
 
-// Row r of the molecule at g0 as the staging below makes its atom: x, y, z and the type (the first argmax, NaN winning) as
-// int bits. The graph hash reads the atoms whose bonds do not fit its shared-memory CSR this way.
+// An atom's type, the rule of every check and of clash guidance: torch.argmax over the row's n_types type channels (from
+// column 3), i.e. the first maximum, NaN winning. k_clash_guide calls it. load_atom and molecule_check's two staging loops
+// spell the same loop out: routed through this function, all 65 k_molecule_check and k_anchor_check instantiations
+// compile to different SASS, so they keep their own copies, which must stay the same as this one.
+__device__ __forceinline__ int first_type(const float* row, int n_types) {
+  int best = 0;
+  for (int k = 1; k < n_types; ++k) {
+    const float v = row[3 + k], cur = row[3 + best];
+    if (v > cur || (isnan(v) && !isnan(cur))) best = k;
+  }
+  return best;
+}
+
+// Row r of the molecule at g0 as the staging below makes its atom: x, y, z and the type (first_type's rule) as int bits.
+// The graph hash reads the atoms whose bonds do not fit its shared-memory CSR this way.
 __device__ __forceinline__ float4 load_atom(const CheckArgs& a, size_t g0, int r) {
   const float* row = a.xh + (g0 + r) * a.row_stride;
   int best = 0;
@@ -1043,6 +1056,120 @@ inline cudaError_t launch_anchor_check(const CheckArgs& a, const AnchorArgs& g, 
     if (err != cudaSuccess) return err;
   }
   k_anchor_check<<<B, 256, smem, st>>>(a, g);
+  return cudaGetLastError();
+}
+
+// Clash guidance (dl_set_clash_guidance, dl_clash_guide; stated at dl_set_clash_guidance in the header): every linker atom
+// i of a molecule moves by scale * sum_k max(0, r_ik - d_ik) (p_i - p_k) / d_ik over its pocket atoms k, r_ik the clash
+// table's entry for the pair in Angstrom. The rows are those of CHECK_CLASH: linker atoms have node_mask, linker_mask and
+// context column C - 1 == 0; pocket atoms node_mask and column C - 1 != 0.
+struct GuideArgs {
+  float* xh;                             // (B, N, row_stride) in/out: x at columns 0..2 (the linker rows' are rewritten),
+                                         // the types' channels from column 3
+  int N, row_stride, n_types, C;
+  float scale;
+  const float* clash;                    // (n_types, n_types) clash distances in pm, [min type][max type]
+  const int8_t* node_mask;               // (B, N)
+  const float* linker_mask;              // (B, N)
+  const float* context;                  // (B, N, C)
+  // in the reverse loop (step != null): loop row *step is guided iff T - steps <= *step < T, and the frame of its
+  // dl_step_coef row (coef, 8 floats per row) receives the moved coordinates times norm0
+  const int* step;
+  int T, steps;
+  const float* coef;
+  float* chain;                          // (keep, B*N, row_stride)
+  float norm0;
+};
+// Shared memory per row: the staged pocket atom and the linker atoms' list.
+constexpr int GUIDE_SMEM_PER_ROW = (int)(sizeof(float4) + sizeof(int));
+
+// One CTA per molecule. The pocket atoms are compacted, in row order, into shared memory (coordinates and type) and the
+// linker rows listed beside them in the same pass. A warp per linker atom then sums its push, lanes over the pocket atoms
+// in a fixed assignment, and reduces the three sums with xor shuffles: no atomics, and the result depends neither on the
+// order the warps run in nor on the molecule's batch-mates. The pair's distance is the clash check's (pair_dist_pm, in pm),
+// so an atom moves iff the check counts a clash for it; (r - d) / d is taken in pm, where it is the same ratio. A pair at
+// d = 0 or with a NaN distance contributes nothing, and an atom with no contributing pair is not written.
+__global__ void __launch_bounds__(256) k_clash_guide(GuideArgs a) {
+  extern __shared__ float4 s_pk[];                    // [n_pocket]: x, y, z, type (int bits)
+  int* s_lnk = reinterpret_cast<int*>(s_pk + a.N);    // [n_linker]: the linker atoms' rows, ascending
+  __shared__ int s_warp[8], s_lwarp[8], s_np, s_nl;
+  int frame = -1;
+  if (a.step != nullptr) {
+    const int step = *a.step;                         // the same for every CTA: the whole grid returns or none does
+    if (step >= a.T || step < a.T - a.steps) return;
+    frame = __float_as_int(a.coef[(size_t)step * 8 + 4]);
+  }
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const size_t g0 = (size_t)blockIdx.x * a.N;
+  if (tid == 0) s_np = s_nl = 0;
+  __syncthreads();
+  for (int r0 = 0; r0 < a.N; r0 += 256) {
+    const int r = r0 + tid;
+    const bool live = r < a.N && a.node_mask[g0 + r] != 0;
+    const bool pocket = live && a.context[(g0 + r) * a.C + a.C - 1] != 0.f;
+    const bool linker = live && !pocket && a.linker_mask[g0 + r] != 0.f;
+    const unsigned mp = __ballot_sync(0xffffffffu, pocket), ml = __ballot_sync(0xffffffffu, linker);
+    if (lane == 0) { s_warp[warp] = __popc(mp); s_lwarp[warp] = __popc(ml); }
+    __syncthreads();
+    const unsigned below = (1u << lane) - 1u;
+    int poff = s_np + __popc(mp & below), loff = s_nl + __popc(ml & below), ptotal = 0, ltotal = 0;
+    for (int w = 0; w < 8; ++w) {
+      poff += w < warp ? s_warp[w] : 0; ptotal += s_warp[w];
+      loff += w < warp ? s_lwarp[w] : 0; ltotal += s_lwarp[w];
+    }
+    if (pocket) {
+      const float* row = a.xh + (g0 + r) * a.row_stride;
+      s_pk[poff] = make_float4(row[0], row[1], row[2], __int_as_float(first_type(row, a.n_types)));
+    }
+    if (linker) s_lnk[loff] = r;
+    __syncthreads();
+    if (tid == 0) { s_np += ptotal; s_nl += ltotal; }
+    __syncthreads();
+  }
+  const int n_pocket = s_np, n_linker = s_nl;
+  for (int i = warp; i < n_linker; i += 8) {          // warp per linker atom, lanes over the pocket atoms
+    const int r = s_lnk[i];
+    float* row = a.xh + (g0 + r) * a.row_stride;
+    const float3 pi = make_float3(row[0], row[1], row[2]);
+    const int ti = first_type(row, a.n_types);
+    float fx = 0.f, fy = 0.f, fz = 0.f;
+    int hits = 0;
+    for (int k = lane; k < n_pocket; k += 32) {
+      const float4 pk = s_pk[k];
+      const float3 pj = make_float3(pk.x, pk.y, pk.z);
+      const int tj = __float_as_int(pk.w);
+      const float d = pair_dist_pm(pi, pj);
+      const float t = a.clash[min(ti, tj) * a.n_types + max(ti, tj)];
+      if (t >= 0.f && d < t && d > 0.f) {             // false for a NaN distance
+        const float w = (t - d) / d;
+        fx = fmaf(w, pi.x - pj.x, fx); fy = fmaf(w, pi.y - pj.y, fy); fz = fmaf(w, pi.z - pj.z, fz);
+        ++hits;
+      }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      fx += __shfl_xor_sync(0xffffffffu, fx, o);
+      fy += __shfl_xor_sync(0xffffffffu, fy, o);
+      fz += __shfl_xor_sync(0xffffffffu, fz, o);
+      hits += __shfl_xor_sync(0xffffffffu, hits, o);
+    }
+    if (hits == 0 || lane >= 3) continue;
+    const float p = lane == 0 ? pi.x : lane == 1 ? pi.y : pi.z;
+    const float f = lane == 0 ? fx : lane == 1 ? fy : fz;
+    const float v = fmaf(a.scale, f, p);
+    row[lane] = v;
+    if (frame >= 0) a.chain[((size_t)frame * gridDim.x * a.N + g0 + r) * a.row_stride + lane] = v * a.norm0;
+  }
+}
+
+// Launches k_clash_guide over B molecules, N <= CONN_MAX_N. Every caller first raises the kernel's shared-memory limit to
+// its one maximum (clash_guide_opt_in), whatever N: the 48 KB default counts the static shared memory too. A reverse loop
+// raises it before it captures its step (the attribute is not a stream operation).
+inline cudaError_t clash_guide_opt_in() {
+  return cudaFuncSetAttribute(k_clash_guide, cudaFuncAttributeMaxDynamicSharedMemorySize, CONN_MAX_N * GUIDE_SMEM_PER_ROW);
+}
+inline cudaError_t launch_clash_guide(const GuideArgs& a, int B, cudaStream_t st) {
+  const size_t smem = (size_t)a.N * GUIDE_SMEM_PER_ROW;
+  k_clash_guide<<<B, 256, smem, st>>>(a);
   return cudaGetLastError();
 }
 

@@ -66,8 +66,9 @@ def place_rows(out: torch.Tensor, parts, slices, dim: int = 0):
 def plan_launches(sizes, nodes, max_molecules: int, keys=None):
     """How `EDM.sample_many` packs requests into launches: [(request indices, N)], every request in exactly one launch and
     never split, N the largest N_k of the launch (the others are padded to it). Requests share a launch only with requests of
-    the same key (`keys`: one hashable per request, None for all the same), so each group is planned on its own, groups in
-    the order of their first request. Within a group the requests are sorted by (N_k, index), which keeps the padding small,
+    the same key (`keys`: one hashable per request, None for all the same; EDM.sample_many's holds what sets how a launch
+    samples: step coefficients, start scalars, jump coefficients, clash guidance), so each group is planned on its own,
+    groups in the order of their first request. Within a group the requests are sorted by (N_k, index), which keeps the padding small,
     and filled in that order into launches of at most `max_molecules` molecules; a request larger than that gets a launch
     of its own. Deterministic: the same inputs give the same plan."""
     if len(sizes) != len(nodes) or (keys is not None and len(keys) != len(sizes)):

@@ -8,10 +8,13 @@ torch seed produces the same noise stream as the reference would on that device.
 """
 import ctypes as C
 import functools
+import math
+import numbers
 import operator
 import threading
 from typing import NamedTuple
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -68,7 +71,8 @@ def _loop_steps(start):
     return max(start.t0) if isinstance(start, StartSteps) else start[0]
 
 
-def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None, resample=None):
+def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None, resample=None,
+                  guide=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
@@ -85,8 +89,9 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     (dl_set_anchors, right before the call, which clears them).
     `start` = (t0, alpha_t0, sigma_t0) starts the loop at step t0 from q(z_t0 | x), set on the engine for the duration of
     the call (dl_set_start_step); a StartSteps starts each row at its own step (dl_set_start_steps). `resample` = (r, T,
-    jump) runs r RePaint passes per step, set on the engine for the duration of the call (dl_set_resamplings). Returns
-    (status, what the batch stream consumed)."""
+    jump) runs r RePaint passes per step, set on the engine for the duration of the call (dl_set_resamplings). `guide` =
+    (scale, steps, clash table) pushes the linker atoms out of the pocket at the last `steps` steps, set on the engine for
+    the duration of the call (dl_set_clash_guidance). Returns (status, what the batch stream consumed)."""
     per_row = isinstance(start, StartSteps)
     if per_row:
         start.set_on(lib, eng)
@@ -95,8 +100,14 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     try:
         if resample is not None:
             _native.check(lib.dl_set_resamplings(eng, *resample), "dl_set_resamplings")
+        if guide is not None:
+            scale, steps, table = guide
+            _native.check(lib.dl_set_clash_guidance(eng, scale, steps, table.shape[0], table.data_ptr()),
+                          "dl_set_clash_guidance")
         return _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry)
     finally:
+        if guide is not None:
+            lib.dl_set_clash_guidance(eng, 0.0, 0, 0, None)
         if resample is not None:
             lib.dl_set_resamplings(eng, 1, 0, None)
         if per_row:
@@ -299,6 +310,10 @@ class EDM(torch.nn.Module):
         # RePaint resampling (InpaintingEDM only): the passes of every reverse step when sample_chain / sample_many get no
         # `resamplings`; 1, the default, is the plain loop
         self.resamplings = 1
+        # Clash guidance (EDM on cut-off graphs only): (scale, steps) pushes the linker atoms that overlap pocket atoms back
+        # towards molecule_builder.clash_table(is_geom)'s distances at the last `steps` reverse steps, when sample_chain /
+        # sample_many get no `clash_guidance`; None, the default, guides nothing
+        self.clash_guidance = None
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
@@ -448,6 +463,44 @@ class EDM(torch.nn.Module):
     def _resample(self, r, n_samples):
         """_sample_slice's `resample` of r passes at batch size n_samples, or None for the plain loop."""
         return None if r == 1 else (r, self.T, self.jump_coefficients(n_samples))
+
+    def _clash_guidance(self, clash_guidance, start_step):
+        """_sample_slice's `guide` of a call: (scale, steps, clash table) from `clash_guidance`, or the `clash_guidance`
+        attribute when None; None when neither is set or when scale or steps is 0 (the plain loop). ValueError unless a
+        pair of a finite real scale >= 0 (a Python or numpy real or a 0-d floating tensor, not a bool) and an integer
+        0 <= steps <= T; and, for any setting given, even one that guides nothing, for InpaintingEDM, FC graphs and a
+        start_step (`start_step` as the call got it: an int, a sequence or None)."""
+        g = self.clash_guidance if clash_guidance is None else clash_guidance
+        if g is None:
+            return None
+        try:
+            scale, steps = g
+        except (TypeError, ValueError):
+            raise ValueError(f"clash_guidance is a pair (scale, steps) (got {g!r})") from None
+        if isinstance(scale, (bool, np.bool_)) or not isinstance(scale, numbers.Real) and not (
+                torch.is_tensor(scale) and scale.dim() == 0 and scale.dtype.is_floating_point):
+            raise ValueError(f"clash_guidance's scale is a real number (got {scale!r})")
+        scale = C.c_float(float(scale)).value   # the engine's fp32
+        if not math.isfinite(scale) or scale < 0:
+            raise ValueError(f"clash_guidance's scale must be finite and >= 0 in fp32 (got {g[0]!r})")
+        try:
+            if isinstance(steps, (bool, np.bool_)):
+                raise TypeError
+            steps = operator.index(steps)
+        except TypeError:
+            raise ValueError(f"clash_guidance's steps is a count of reverse steps (got {steps!r})") from None
+        if not 0 <= steps <= self.T:
+            raise ValueError(f"clash_guidance's steps must lie in [0, T = {self.T}] (got {steps})")
+        if self._SAMPLER == _native.SAMPLER_INPAINT:
+            raise ValueError("clash_guidance does not take InpaintingEDM: its loop re-noises the pocket")
+        if self.dynamics.graph_type == 'FC':
+            raise ValueError("clash_guidance needs a pocket: FC graphs have no pocket rows (use a pocket model on a cut-off "
+                             "graph)")
+        if start_step is not None:
+            raise ValueError("clash_guidance does not take start_step: guidance is a tool of the sampler from noise")
+        if scale == 0 or steps == 0:
+            return None
+        return scale, steps, clash_table(self.is_geom).contiguous()
 
     def draw_noise(self, n_draws, n_samples, n_nodes, device, generator=None):
         """(n_draws, B, N, 3+F) standard normal. 'reference_stream': the reference's call order -- for every
@@ -785,7 +838,7 @@ class EDM(torch.nn.Module):
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, anchors=None):
+                     require_anchors=None, anchors=None, clash_guidance=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -885,6 +938,14 @@ class EDM(torch.nn.Module):
         needs `seeds` and raises ValueError where nan_retries does, with start_step and for InpaintingEDM.
         `resamplings` (None: the `resamplings` attribute, default 1) is InpaintingEDM's; this class raises ValueError for
         anything but 1 (or None), and for a value that is not an int >= 1.
+        `clash_guidance` = (scale, steps) (None: the `clash_guidance` attribute, default None) steers the linker away from
+        the pocket while it is sampled (dl_set_clash_guidance): after each reverse step s < steps has produced z_s, every
+        linker atom i moves by scale * sum_k max(0, r_ik - d_ik) (p_i - p_k) / d_ik over the pocket atoms k, r_ik the
+        clash_table(is_geom) distance of the two atom types (argmax of z_s's type channels) in Angstrom, and the remaining
+        steps rebuild the linker around it (molecule_builder.clash_guide states the push). It draws nothing, so draws,
+        seeds and recovery rounds are as without it; the rounds are guided too. scale = 0 or steps = 0 is the plain call,
+        bit for bit. A sampler tool with no claim about chemistry. ValueError for a bool, negative or non-finite scale,
+        steps outside [0, T], FC graphs, start_step and InpaintingEDM.
         The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
         and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
         device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
@@ -903,6 +964,7 @@ class EDM(torch.nn.Module):
         self.last_anchors_ok = None
         start = self._start(start_step, n_samples)
         r = self._resamplings(resamplings)
+        guide = self._clash_guidance(clash_guidance, start_step)
         redraw = self._linker_sizes(linker_sizes, seeds, noise, batch_slice, start_step, x, linker_mask)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
         check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free,
@@ -945,7 +1007,7 @@ class EDM(torch.nn.Module):
                                             engines, places, dev, noise=noise, dev_seeds=dev_seeds,
                                             rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check,
                                             start=start, redraw=redraw, sets=sets,
-                                            resample=self._resample(r, n_samples), anchors=anchor_flags)
+                                            resample=self._resample(r, n_samples), anchors=anchor_flags, guide=guide)
         by_device = {}
         for dev_i, c in calls:
             by_device.setdefault(dev_i, []).append(c)
@@ -1018,7 +1080,8 @@ class EDM(torch.nn.Module):
     @torch.no_grad()
     def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                    require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None):
+                    require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None,
+                    clash_guidance=None):
         """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
         edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
         (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
@@ -1056,6 +1119,8 @@ class EDM(torch.nn.Module):
         different steps share launches, since the steps travel per row.
         `resamplings` as in sample_chain, for every request; requests then also share a launch only where sample_chain
         would give them the same jump coefficients (jump_coefficients, which depend on the batch size as the table does).
+        `clash_guidance` as in sample_chain, for every request; it is part of every launch's key, and it draws nothing, so
+        packing does not change a request's rows.
         Raises ValueError for an empty list, the batch stream (its draws depend on B and N), noise= or a replaced draw
         function, host inputs, requests on different devices or of different feature or context widths, and seeds that do
         not match the requests. It takes no `require_unique`, and raises ValueError when the attribute is set: a launch packs
@@ -1077,6 +1142,7 @@ class EDM(torch.nn.Module):
         if not per_request:
             self._start(start_step, 1)      # validates it before anything else is checked
         r_passes = self._resamplings(resamplings)
+        guide = self._clash_guidance(clash_guidance, start_step)
         for k, r in enumerate(requests):
             if 'noise' in r or 'batch_slice' in r:
                 raise ValueError(f"request {k} passes noise= or batch_slice=: sample_many samples per-molecule streams, "
@@ -1147,6 +1213,8 @@ class EDM(torch.nn.Module):
         coefs, starts, keys = self._launch_keys(sizes, nodes, keep_frames, start_step)
         if r_passes > 1:                    # the jump coefficients depend on the batch size as the table does
             keys = [k + (bytes(self.jump_coefficients(b)),) for k, b in zip(keys, sizes)]
+        if guide is not None:               # the same for every request of a call: launches are sampled as it says
+            keys = [k + (guide[:2],) for k in keys]
         fc = self.dynamics.graph_type == 'FC'
         launches = plan_launches(sizes, nodes, max_molecules, keys)
         if fc:                              # edges of the launch's padded molecules
@@ -1185,7 +1253,8 @@ class EDM(torch.nn.Module):
             [(_, call)], finish = self._enqueue_batch(lib, full, keep_frames, coefs[sizes[ks[0]]], [(dev_i, replica, 0, b)], [eng],
                                                       [where], dev, dev_seeds=dev_seeds, retries=retries, check=check,
                                                       start=start, redraw=redraw, sets=sets,
-                                                      resample=self._resample(r_passes, sizes[ks[0]]), anchors=anchors)
+                                                      resample=self._resample(r_passes, sizes[ks[0]]), anchors=anchors,
+                                                      guide=guide)
             finishes.append(finish)
             by_device.setdefault(dev_i, []).append(
                 functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
@@ -1271,7 +1340,7 @@ class EDM(torch.nn.Module):
         return coefs, starts, keys
 
     def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
-                       retries=0, check=0, start=None, redraw=None, sets=None, resample=None, anchors=None):
+                       retries=0, check=0, start=None, redraw=None, sets=None, resample=None, anchors=None, guide=None):
         """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
         inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
         replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
@@ -1279,7 +1348,7 @@ class EDM(torch.nn.Module):
         b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _checks; `start` as
         returned by _start; `redraw` as returned by _linker_sizes (its rounds then redraw sizes, into `sizes`); `sets` as
         returned by _hash_sets, copied to each slice's device; `resample` as returned by _resample; `anchors` as returned
-        by _anchors, each slice's rows on its device.
+        by _anchors, each slice's rows on its device; `guide` as returned by _clash_guidance.
         Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
         (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
         back and returns dict(chain, flags, used, attempts, passed, sizes, bad, consumed) on `dev`; `passed` holds
@@ -1347,7 +1416,7 @@ class EDM(torch.nn.Module):
                 stream, nz, sd, rng_i,
                 (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i, sets_i, lh_i,
                  (allowed, rs_i) if rings else None, an_i) if recover else None,
-                start.rows(lo, hi) if isinstance(start, StartSteps) else start, resample)))
+                start.rows(lo, hi) if isinstance(start, StartSteps) else start, resample, guide)))
 
         def finish():
             if not whole:
@@ -1432,7 +1501,7 @@ class InpaintingEDM(EDM):
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, anchors=None):
+                     require_anchors=None, anchors=None, clash_guidance=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -1454,7 +1523,7 @@ class InpaintingEDM(EDM):
         two final draws: 1 + T(3r-1) + 2 (noise= holds that many prepared slabs, draw_noise_inpaint(resamplings=r) makes
         them; the batch stream advances by as many draws; per-molecule streams use their draws in that order). r = 1 is
         the plain sampler, bit for bit. A call costs about r times the loop. ValueError for a non-integer, a bool or
-        r < 1."""
+        r < 1. `clash_guidance` raises ValueError unless None: this loop re-noises the pocket."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
@@ -1463,7 +1532,7 @@ class InpaintingEDM(EDM):
                                     require_unique=require_unique, require_novel=require_novel,
                                     exclude_hashes=exclude_hashes, resamplings=resamplings,
                                     require_ring_sizes=require_ring_sizes, require_anchors=require_anchors,
-                                    anchors=anchors)
+                                    anchors=anchors, clash_guidance=clash_guidance)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

@@ -257,6 +257,42 @@ def clash_free(xh, node_mask, linker_mask, pocket_only, is_geom, clash=None):
 
 
 @torch.no_grad()
+def clash_guide(xh, node_mask, linker_mask, pocket_only, is_geom, scale, clash=None):
+    """One clash-guidance push (sample_chain(clash_guidance=...), dl_clash_guide) stated on the host in fp64: a copy of
+    `xh` (B,N,3+F) in which every linker atom i -- the rows of pocket_clashes -- has moved to
+        p_i + scale * sum_k max(0, r_ik - d_ik) (p_i - p_k) / d_ik,   d_ik = |p_i - p_k|,
+    k over the pocket atoms, r_ik = clash[min type][max type] / 100 Angstrom (`clash` by default clash_table(is_geom); a
+    negative entry exempts the pair), an atom's type the argmax of its first T feature columns. Every term comes from the
+    input state; a pair at d_ik = 0 or with a NaN distance contributes nothing, and only linker coordinates change. With
+    scale = 1 a linker atom in contact with one pocket atom lands at r_ik from it. The engine evaluates the same push in
+    fp32 and leaves an atom with no contributing pair unwritten."""
+    B, N = xh.shape[:2]
+    T = len(GEOM_IDX2ATOM if is_geom else IDX2ATOM)
+    table = (clash_table(is_geom) if clash is None else torch.as_tensor(clash, dtype=torch.float32)).double().cpu()
+    if table.shape != (T, T):
+        raise ValueError(f"clash is a ({T}, {T}) table, one row and column per atom type (got shape {tuple(table.shape)})")
+    out = xh.detach().clone()
+    x = xh[..., :3].detach().double().cpu()
+    types = xh[..., 3:3 + T].detach().cpu().argmax(-1)
+    live = node_mask.reshape(B, N).cpu() != 0
+    pocket = live & (pocket_only.reshape(B, N).cpu() != 0)
+    linker = live & ~pocket & (linker_mask.reshape(B, N).cpu() != 0)
+    for b in range(B):
+        li, pk = linker[b].nonzero().flatten(), pocket[b].nonzero().flatten()
+        if len(li) == 0 or len(pk) == 0:
+            continue
+        diff = x[b][li][:, None, :] - x[b][pk][None, :, :]                 # (n_linker, n_pocket, 3): p_i - p_k
+        d = diff.norm(dim=-1)
+        ti, tk = types[b][li][:, None], types[b][pk][None, :]
+        r = table[torch.minimum(ti, tk), torch.maximum(ti, tk)] / 100.0
+        on = (r >= 0) & (d < r) & (d > 0)                                    # False for a NaN distance
+        w = torch.where(on, (r - d) / torch.where(on, d, torch.ones_like(d)), torch.zeros_like(d))
+        push = torch.where(on[..., None], w[..., None] * diff, torch.zeros_like(diff)).sum(1)
+        out[b, li, :3] = (x[b, li] + float(scale) * push).to(out.dtype).to(out.device)
+    return out
+
+
+@torch.no_grad()
 def _clash_check(xh, node_mask, linker_mask, pocket_only, is_geom, clash, want_counts):
     """dl_clash_check on a chain[0]-style batch: ((B,) int32 verdict bits, (B,N) int32 counts or None)."""
     dev = xh.device

@@ -30,6 +30,9 @@
  *     beyond its valence (the explicit-valence part of validity, src/metrics.py:12-17; see dl_molecule_checks)
  *   either on pocket graphs, also resampling the        dl_sample_chain_retry with DL_CHECK_CLASH, dl_clash_check
  *     molecules whose linker clashes with the pocket (no reference API; see dl_molecule_checks)
+ *   EDM on pocket graphs, pushing linker atoms out of     dl_set_clash_guidance, then any dl_sample_chain* entry point;
+ *     the pocket during the last K steps (no reference   dl_clash_guide
+ *     API; see dl_set_clash_guidance)
  *   either, also resampling the molecules that repeat   dl_sample_chain_retry with DL_CHECK_UNIQUE, dl_molecule_hash
  *     a batch-mate (uniqueness, compute_metrics.py; see DL_CHECK_UNIQUE)
  *   either, also resampling the molecules whose linker   dl_sample_chain_retry_sets with DL_CHECK_NOVEL (known set) or
@@ -587,6 +590,23 @@ dl_status dl_clash_check(int32_t B, int32_t N, int32_t n_types, const float* cla
                          const int8_t* node_mask, const float* linker_mask, const float* context, int32_t context_nf,
                          int32_t* passed, int32_t* clashes, void* stream);
 /*
+ * One clash-guidance push (stated at dl_set_clash_guidance) on any (B,N) batch, without an engine. DEVICE buffers, enqueued
+ * on `stream`.
+ *   clash       (n_types,n_types) fp32, in pm, as dl_molecule_checks.clash: r_ik = clash[min type][max type] / 100 Angstrom;
+ *               a negative entry exempts the pair
+ *   scale       lambda, finite and >= 0 (0: nothing is launched)
+ *   xh          (B,N,>=3+n_types) fp32 in/out, row stride xh_row_stride: x at columns 0..2, the type channels from column 3
+ *               (an atom's type is the first maximum of its first n_types channels). Only columns 0..2 of linker rows with a
+ *               contributing pair are written.
+ *   node_mask   (B,N) int8
+ *   linker_mask (B,N) fp32
+ *   context     (B,N,context_nf) fp32, context_nf >= 1: column context_nf - 1 marks the pocket rows
+ * The rows are dl_clash_check's. 1 <= n_types <= xh_row_stride - 3, 1 <= N <= 8192.
+ */
+dl_status dl_clash_guide(int32_t B, int32_t N, int32_t n_types, const float* clash, float scale, float* xh,
+                         int32_t xh_row_stride, const int8_t* node_mask, const float* linker_mask, const float* context,
+                         int32_t context_nf, void* stream);
+/*
  * The graph hash of DL_CHECK_UNIQUE alone, on any (B,N) batch, without an engine. DEVICE buffers, enqueued on `stream`.
  *   checks    n_types, thr1, thr2 and thr3 are read; require, max_valence and clash are not
  *   xh, node_mask, context, context_nf, drop_pocket   as dl_molecule_check: the atoms and types of dl_molecule_checks
@@ -712,6 +732,29 @@ dl_status dl_set_start_steps(dl_engine* e, int32_t B, const int32_t* t0, const f
  * and DL_SAMPLER_LINKER. A call costs about r times the plain loop (T*r + 1 forwards).
  */
 dl_status dl_set_resamplings(dl_engine* e, int32_t r, int32_t T, const float* jump);
+/*
+ * Clash guidance (no reference API; a sampler tool that makes no claim about chemistry) for DL_SAMPLER_LINKER on cut-off
+ * (pocket) graphs: in the following dl_sample_chain* calls of this engine -- the recovery rounds of dl_sample_chain_retry
+ * included -- after the reverse update has produced z_s at a step s < steps, and before anything reads it, every molecule's
+ * linker atoms are pushed away from its pocket atoms:
+ *   p_i <- p_i + scale * sum_k max(0, r_ik - d_ik) (p_i - p_k) / d_ik,   d_ik = |p_i - p_k|
+ * with p the coordinate columns of z_s, i over the linker atoms (node_mask, linker_mask != 0 and context column C - 1 == 0)
+ * and k over the pocket atoms (node_mask and column C - 1 != 0): the rows of DL_CHECK_CLASH. r_ik = clash[min type][max
+ * type] / 100 Angstrom of the (n_types,n_types) HOST table in pm; a negative entry exempts the pair. The table is copied
+ * into host memory here, and each following sampling call uploads that copy on the engine's loop stream, ordered after
+ * the calls enqueued before it: setting another table never changes a call already made, even one still running. An atom's
+ * type is the first maximum of its first n_types feature channels in z_s. Every term is taken from the state before the
+ * push; a pair at d_ik = 0 or with a NaN distance contributes nothing. Only the coordinates of linker rows change; the
+ * final p(x, h | z_0) step is never guided. A frame written at a guided step holds the guided state, and the next step's
+ * cut-off graph is built from it. Guidance draws no noise: draws and their count are unchanged. The sum over the pocket
+ * atoms has a fixed shape and no atomics, so a molecule's result depends neither on its batch-mates nor on the launch.
+ * One launch per step of the captured step graph decides on the device whether its step is guided.
+ * Sticky like dl_set_start_step. steps = 0 or scale = 0 switches it off: the calls then launch exactly what they launch
+ * without it. DL_ERR_INVALID: here, a non-finite or negative scale, steps < 0, and n_types < 1 or a NULL table while on; at
+ * the sampling call, steps > T, DL_SAMPLER_INPAINT, a start step (dl_set_start_step or dl_set_start_steps), DL_GRAPH_FC,
+ * n_types > F, N > 8192 and a NULL context.
+ */
+dl_status dl_set_clash_guidance(dl_engine* e, float scale, int32_t steps, int32_t n_types, const float* clash);
 /* The (n_draws,B,N,3+F) tensor the device-side stream of dl_sample_chain_rng stands for (tests, debugging). DEVICE out. */
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream);
