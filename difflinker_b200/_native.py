@@ -9,6 +9,7 @@ DL_OK, DL_NAN_DETECTED = 0, 1
 GRAPH_TYPES = {"FC": 0, "4A": 1, "FC-4A": 2, "FC-10A-4A": 3}
 EDGE_IMPLS = {"auto": 0, "simt": 1, "wgmma": 2}
 SAMPLER_LINKER, SAMPLER_INPAINT = 0, 1
+SOLVERS = {"ancestral": 0, "ddim": 1, "dpmpp_2m": 2}   # DL_SOLVER_*
 AGGREGATIONS = {"sum": 0, "mean": 1}
 CHECK_CONNECTED, CHECK_VALENCE, CHECK_CLASH, CHECK_UNIQUE, CHECK_NOVEL, CHECK_RINGS = 1, 2, 4, 8, 16, 32   # DL_CHECK_*
 CHECK_ANCHORS = 64
@@ -110,6 +111,7 @@ SYMBOLS = {
     "dl_set_start_steps": (_I32, [_P, _I32, _P, _P, _P]),
     "dl_set_resamplings": (_I32, [_P, _I32, _I32, _P]),
     "dl_set_clash_guidance": (_I32, [_P, C.c_float, _I32, _I32, _P]),
+    "dl_set_solver": (_I32, [_P, _I32, _I32, _P]),
     "dl_clash_guide": (_I32, [_I32, _I32, _I32, _P, C.c_float, _P, _I32, _P, _P, _P, _I32, _P]),
     "dl_noise_fill": (_I32, [_P, _I32, _I32, _I32, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "dl_noise_fill_inpaint": (_I32, [_P, _I32, _I32, _I32, _P, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),

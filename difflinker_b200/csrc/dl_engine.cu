@@ -137,7 +137,11 @@ struct dl_engine {
   std::vector<float> guide_table;
   float* guide_clash = nullptr;
   size_t guide_cap = 0;
-  int64_t mol_steps = 0;       // dl_last_molecule_steps
+  // dl_set_solver: the linker sampler's update for calls of T = solver_T, from the (solver_T + 1, 8) table solver_table
+  // (host copy), which each call uploads after its coefficient rows; DL_SOLVER_ANCESTRAL: the plain loop
+  int solver_kind = DL_SOLVER_ANCESTRAL, solver_T = 0;
+  std::vector<float> solver_table;
+  int64_t mol_steps = 0;      // dl_last_molecule_steps
   bool finalized = false;
   std::map<std::string, std::vector<float>> raw;
   float* wblob = nullptr;      // packed fp32 weights
@@ -415,6 +419,7 @@ struct FwdIO {
   int T = 0; float norm0 = 1.f, norm1 = 1.f, bias1 = 0.f;
   RowStarts rows{};   // per-molecule start steps, or rows.lag = null
   int R = 1; const float* jump = nullptr;   // resampling passes per reverse step (dl_set_resamplings), T counting passes
+  const float* ode = nullptr;               // the solver rows of the loop (dl_set_solver), or null: the ancestral update
 };
 
 ProjW proj_of(const EdgeMlpW& w) { return ProjW{w.W1a_t, w.W1b_t, w.b1}; }
@@ -608,11 +613,15 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     fa.z = ws.z; fa.fragment_mask = io.fragment_mask; fa.linker_mask = io.linker_mask; fa.noise = io.noise; fa.rng = io.rng;
     fa.coef = e->coef_dev; fa.step_fin = e->step_ctr + 1; fa.step_prep = e->step_ctr; fa.T = io.T;
     fa.norm0 = io.norm0; fa.norm1 = io.norm1; fa.bias1 = io.bias1; fa.chain = io.chain; fa.rows = io.rows;
+    // the 2M history lives in ws.eps, which the fused linker update never writes otherwise
+    fa.ode = io.ode; fa.hist = io.ode && e->solver_kind == DL_SOLVER_DPMPP_2M ? ws.eps : nullptr;
   } else if (io.sampler) {
     fa.tag_step = e->step_ctr + (io.R > 1 ? 2 : 1);   // with resampling the pass counter is not the step
   }
   const bool per_mol = io.rng.on == NOISE_PER_MOLECULE;
-  TIMED("k_finish", st, (launch_chain(per_mol ? k_finish<true> : k_finish<false>, dim3((n + 15) / 16), dim3(256), 0, st, gm, fa)));
+  auto* finish = fa.ode ? (per_mol ? k_finish<true, true> : k_finish<false, true>)
+                        : (per_mol ? k_finish<true> : k_finish<false>);
+  TIMED("k_finish", st, (launch_chain(finish, dim3((n + 15) / 16), dim3(256), 0, st, gm, fa)));
   LAUNCH_CHECK();
   e->launches += 1;
   if (fused_update && e->guide_steps > 0) {
@@ -1177,6 +1186,30 @@ dl_status dl_set_clash_guidance(dl_engine* e, float scale, int32_t steps, int32_
   return DL_OK;
 }
 
+dl_status dl_set_solver(dl_engine* e, int32_t kind, int32_t T, const float* table) {
+  if (!e) { set_err("dl_set_solver: null engine"); return DL_ERR_INVALID; }
+  if (kind != DL_SOLVER_ANCESTRAL && kind != DL_SOLVER_DDIM && kind != DL_SOLVER_DPMPP_2M) {
+    set_err("dl_set_solver: unknown kind %d", kind);
+    return DL_ERR_INVALID;
+  }
+  if (kind == DL_SOLVER_ANCESTRAL) { e->solver_kind = kind; e->solver_T = 0; e->solver_table.clear(); return DL_OK; }
+  if (!table) { set_err("dl_set_solver: kind %d needs its table", kind); return DL_ERR_INVALID; }
+  if (T < 1 || T > (1 << 24)) { set_err("dl_set_solver: T must lie in [1, 2^24] (got %d)", T); return DL_ERR_INVALID; }
+  for (int i = 0; i < 8 * (T + 1); ++i)
+    if (!std::isfinite(table[i])) {
+      set_err("dl_set_solver: table[%d][%d] is not finite", i / 8, i % 8);
+      return DL_ERR_INVALID;
+    }
+  for (int r = 0; r < T; ++r)
+    if (!(table[8 * r + 6] > 0.f)) {
+      set_err("dl_set_solver: row %d has h = %g <= 0 (a grid point repeats)", r, (double)table[8 * r + 6]);
+      return DL_ERR_INVALID;
+    }
+  // a host copy: the calls already enqueued keep the rows they uploaded, later calls upload this table
+  e->solver_kind = kind; e->solver_T = T; e->solver_table.assign(table, table + 8 * (size_t)(T + 1));
+  return DL_OK;
+}
+
 dl_status dl_set_ring_sizes(dl_engine* e, uint64_t allowed) {
   if (!e) { set_err("null engine"); return DL_ERR_INVALID; }
   if (allowed & 7u) {
@@ -1287,15 +1320,23 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
       return DL_ERR_INVALID;
     }
   }
+  const bool ode = e->solver_kind != DL_SOLVER_ANCESTRAL;
+  if (ode && (inpaint || T != e->solver_T)) {
+    if (inpaint) set_err("dl_set_solver takes DL_SAMPLER_LINKER only");
+    else set_err("dl_set_solver was given the table of T = %d; the call samples T = %d", e->solver_T, T);
+    return DL_ERR_INVALID;
+  }
   // A start step t0 runs the table's last t0 + 1 rows -- steps t0-1 .. 0, then the final one -- as a loop of Tl = t0 steps:
   // loop step r reads row r of the copied rows and draw r + 1, so the draws are eps, one per step and the final one.
   const int Tl = loop_steps(e, T);
   coef += T - Tl;
   static_assert(sizeof(dl_step_coef) == 32, "dl_step_coef layout");
   // Resampling: the loop runs P = T*R passes and the final step. Pass k*R + u reads row k of the caller's table, whose frame
-  // only its last pass writes; the jump coefficients follow the table on the device.
+  // only its last pass writes; the jump coefficients follow the table on the device. A solver (never with R > 1, which is
+  // the inpainting sampler's) puts the same rows of its table there instead.
   const int P = Tl * R, rows = P + 1;
-  const size_t coef_bytes = (size_t)rows * sizeof(dl_step_coef) + (R > 1 ? e->jump.size() * sizeof(float) : 0);
+  const size_t coef_bytes = (size_t)rows * sizeof(dl_step_coef) + (R > 1 ? e->jump.size() * sizeof(float) : 0) +
+                            (ode ? (size_t)rows * 8 * sizeof(float) : 0);
   if (R > 1) {
     e->coef_passes.resize(rows);
     for (int p = 0; p < P; ++p) {
@@ -1340,6 +1381,10 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   if (R > 1)
     CK(cudaMemcpyAsync(const_cast<float*>(jump_dev), e->jump.data(), e->jump.size() * sizeof(float), cudaMemcpyHostToDevice,
                        st));
+  const float* ode_dev = ode ? e->coef_dev + (size_t)rows * 8 : nullptr;
+  if (ode)
+    CK(cudaMemcpyAsync(const_cast<float*>(ode_dev), e->solver_table.data() + (size_t)(T - Tl) * 8,
+                       (size_t)rows * 8 * sizeof(float), cudaMemcpyHostToDevice, st));
   NoiseRng q = rng ? *rng : NoiseRng{};
   // per-molecule start steps: the loop runs on the rows in start-step order, each loop step on those that have started
   RowOrder ro{};
@@ -1401,7 +1446,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   io.rng = q;
   io.chain = chain; io.T = P; io.norm0 = norm[0]; io.norm1 = norm[1]; io.bias1 = norm[2];
   io.rows = per_row ? ro.rs : RowStarts{};
-  io.R = R; io.jump = jump_dev;
+  io.R = R; io.jump = jump_dev; io.ode = ode_dev;
 
   // capture ONE reverse step; the step index lives on the device, so the same graph serves all Tl+1 steps (all P+1 passes
   // with resampling) -- with per-molecule start steps, all steps of one prefix length: the graph is recaptured whenever the

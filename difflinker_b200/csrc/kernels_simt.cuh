@@ -906,9 +906,13 @@ struct FinishArgs {
   float* chain;          // (keep,B*N,3+F)
   const int* tag_step;   // non-sampler mode inside the inpainting loop: step counter used to tag NaN flags (or null)
   RowStarts rows;        // per-molecule start steps (dl_set_start_steps), or lag = null
+  // ODE solvers (dl_set_solver, k_finish<., true>): the solver table of the loop's rows, 8 floats per row in coef's row
+  // order, and the DPM-Solver++(2M) history -- every node's data prediction of its previous step -- or null (DDIM)
+  const float* ode;
+  float* hist;
 };
 
-template <bool PER_MOL = false>
+template <bool PER_MOL = false, bool ODE = false>
 __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
   const int tid = threadIdx.x;
   const int d = tid & 15, r = tid >> 4;
@@ -983,7 +987,33 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
   const int frame = __float_as_int(cf[4]);
   float znew = 0.f;
   float lm = 0.f, fm = 0.f;
-  if (act) {
+  if constexpr (ODE) {
+    // deterministic update from the solver row sv = (sigma_t, 1/alpha_t, sigma_s/sigma_t, c1, c2a, c2b, h, 0): the data
+    // prediction xhat = (z_t - sigma_t eps) / alpha_t, then z_s = (sigma_s/sigma_t) z_t + c1 xhat at a row's first step
+    // (DDIM always), + c2a xhat + c2b xhat' after it; the final row returns xhat. No draw is read.
+    if (act) {
+      lm = a.linker_mask[g]; fm = a.fragment_mask[g];
+      const size_t gi = (size_t)g * xd + d;
+      const float zt = a.z[gi];
+      const float eps = e * lm;
+      const float* sv = a.ode + (size_t)step * 8;
+      const float xhat = sv[1] * (zt - sv[0] * eps);
+      if (step < a.T) {
+        float zs;
+        if (a.hist != nullptr && step > lag) zs = sv[2] * zt + (sv[4] * xhat + sv[5] * a.hist[gi]);
+        else zs = sv[2] * zt + sv[3] * xhat;
+        if (a.hist != nullptr) a.hist[gi] = xhat;
+        znew = zt * fm + zs * lm;
+        a.z[gi] = znew;
+        if (frame >= 0) {
+          float o = d < 3 ? znew * a.norm0 : znew * a.norm1 + a.bias1;
+          a.chain[((size_t)frame * nc + gc) * xd + d] = o;
+        }
+      } else {
+        znew = zt * fm + xhat * lm;
+      }
+    }
+  } else if (act) {
     lm = a.linker_mask[g]; fm = a.fragment_mask[g];
     const float zt = a.z[(size_t)g * xd + d];
     const float eps = e * lm;                                                 // edm.py:196 / 225

@@ -227,7 +227,7 @@ def _check_start(sample_fn, start_step):
 def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                  start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                  require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None, require_anchors=None,
-                 clash_guidance=None):
+                 clash_guidance=None, solver=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
@@ -260,7 +260,8 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     `resamplings` = r: r RePaint passes per reverse step of an inpainting model (InpaintingEDM.sample_chain; None uses
     `model.edm.resamplings`).
     `clash_guidance` = (scale, steps): push the linker atoms out of the pocket at the last `steps` reverse steps
-    (EDM.sample_chain; None uses `model.edm.clash_guidance`)."""
+    (EDM.sample_chain; None uses `model.edm.clash_guidance`).
+    `solver` = 'ancestral', 'ddim' or 'dpmpp_2m': the reverse update (EDM.sample_chain; None uses `model.edm.solver`)."""
     _check_start(sample_fn, start_step)
     if linker_sizes is not None:
         _check_linker_sizes(model, sample_fn, start_step)
@@ -293,6 +294,8 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['resamplings'] = resamplings
     if clash_guidance is not None:
         extra['clash_guidance'] = clash_guidance
+    if solver is not None:
+        extra['solver'] = solver
     chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **extra)
     if sized is not None:
         return chain, _final_node_mask(kw, sized, model.edm.last_sizes)
@@ -301,7 +304,8 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
 
 def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                 max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None, clash_guidance=None):
+                require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None, clash_guidance=None,
+                solver=None):
     """The body of sample_chain for many batches `datas` at once, sampled in shared launches by EDM.sample_many: returns
     [(chain_k, node_mask_k)] in the order of `datas`, each equal to what sample_chain(model, datas[k], ...) returns (with
     seeds[k]) in the sense of EDM.sample_many. `model` as for sample_chain, so accelerated reference modules take it too.
@@ -310,7 +314,7 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
     one for every batch, as in sample_chain. `linker_sizes`, one for every batch, as in sample_chain: each batch's sizes
     are drawn from its own seeds and its template padded to its own N_cap, so packing changes neither;
     `edm.last_sizes_many` holds them. `resamplings` and `require_anchors` as in sample_chain: each request then holds its
-    batch's template anchors. `clash_guidance` as in sample_chain."""
+    batch's template anchors. `clash_guidance` and `solver` as in sample_chain."""
     _check_start(sample_fn, start_step)
     edm = model.edm
     if linker_sizes is not None:
@@ -322,7 +326,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra = {} if nan_retries is None else {'nan_retries': nan_retries}
         for name, v in (('require_connected', require_connected), ('require_valid', require_valid),
                         ('require_clash_free', require_clash_free), ('require_novel', require_novel),
-                        ('require_ring_sizes', require_ring_sizes), ('clash_guidance', clash_guidance)):
+                        ('require_ring_sizes', require_ring_sizes), ('clash_guidance', clash_guidance),
+                        ('solver', solver)):
             if v is not None:
                 extra[name] = v
         requests = [_with_anchors(model, data, kw, require_anchors) for data, (kw, _, _) in zip(datas, sized)]
@@ -362,6 +367,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['resamplings'] = resamplings
     if clash_guidance is not None:
         extra['clash_guidance'] = clash_guidance
+    if solver is not None:
+        extra['solver'] = solver
     chains = edm.sample_many(requests, keep_frames=keep_frames, seeds=seeds, max_molecules=max_molecules, **extra)
     return [(chain, kw['node_mask']) for chain, kw in zip(chains, requests)]
 
@@ -404,23 +411,23 @@ class DDPM(nn.Module):
     def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                      start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, clash_guidance=None):
+                     require_anchors=None, clash_guidance=None, solver=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                             require_connected=require_connected, start_step=start_step, require_valid=require_valid,
                             require_clash_free=require_clash_free, linker_sizes=linker_sizes, require_unique=require_unique,
                             require_novel=require_novel, exclude_hashes=exclude_hashes, resamplings=resamplings,
                             require_ring_sizes=require_ring_sizes, require_anchors=require_anchors,
-                            clash_guidance=clash_guidance)
+                            clash_guidance=clash_guidance, solver=solver)
 
     def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
                     require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None,
-                    clash_guidance=None):
+                    clash_guidance=None, solver=None):
         return sample_many(self, datas, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                            require_connected=require_connected, max_molecules=max_molecules, start_step=start_step,
                            require_valid=require_valid, require_clash_free=require_clash_free, linker_sizes=linker_sizes,
                            require_novel=require_novel, resamplings=resamplings, require_ring_sizes=require_ring_sizes,
-                           require_anchors=require_anchors, clash_guidance=clash_guidance)
+                           require_anchors=require_anchors, clash_guidance=clash_guidance, solver=solver)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

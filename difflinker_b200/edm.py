@@ -72,7 +72,7 @@ def _loop_steps(start):
 
 
 def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None, resample=None,
-                  guide=None):
+                  guide=None, solver=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
@@ -91,7 +91,9 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     the call (dl_set_start_step); a StartSteps starts each row at its own step (dl_set_start_steps). `resample` = (r, T,
     jump) runs r RePaint passes per step, set on the engine for the duration of the call (dl_set_resamplings). `guide` =
     (scale, steps, clash table) pushes the linker atoms out of the pocket at the last `steps` steps, set on the engine for
-    the duration of the call (dl_set_clash_guidance). Returns (status, what the batch stream consumed)."""
+    the duration of the call (dl_set_clash_guidance). `solver` = (kind, T, table) replaces the ancestral update by an ODE
+    solver's, set on the engine for the duration of the call (dl_set_solver). Returns (status, what the batch stream
+    consumed)."""
     per_row = isinstance(start, StartSteps)
     if per_row:
         start.set_on(lib, eng)
@@ -104,8 +106,12 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
             scale, steps, table = guide
             _native.check(lib.dl_set_clash_guidance(eng, scale, steps, table.shape[0], table.data_ptr()),
                           "dl_set_clash_guidance")
+        if solver is not None:
+            _native.check(lib.dl_set_solver(eng, *solver), "dl_set_solver")
         return _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry)
     finally:
+        if solver is not None:
+            lib.dl_set_solver(eng, _native.SOLVERS['ancestral'], 0, None)
         if guide is not None:
             lib.dl_set_clash_guidance(eng, 0.0, 0, 0, None)
         if resample is not None:
@@ -314,6 +320,10 @@ class EDM(torch.nn.Module):
         # towards molecule_builder.clash_table(is_geom)'s distances at the last `steps` reverse steps, when sample_chain /
         # sample_many get no `clash_guidance`; None, the default, guides nothing
         self.clash_guidance = None
+        # Reverse update (EDM only): 'ancestral' (the default) samples p(z_s | z_t) as the reference does; 'ddim' and
+        # 'dpmpp_2m' take deterministic steps of the probability-flow ODE (solver_coefficients), for calls that get no
+        # `solver`. Meant for a shortened loop: edm.T = 20; edm.solver = 'dpmpp_2m'
+        self.solver = 'ancestral'
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
@@ -463,6 +473,62 @@ class EDM(torch.nn.Module):
     def _resample(self, r, n_samples):
         """_sample_slice's `resample` of r passes at batch size n_samples, or None for the plain loop."""
         return None if r == 1 else (r, self.T, self.jump_coefficients(n_samples))
+
+    def solver_coefficients(self, kind):
+        """The (T+1, 8) table of dl_set_solver for the solver `kind` ('ddim' or 'dpmpp_2m') as a flat ctypes float array,
+        in step_coefficients' row order. gamma_t and gamma_s are the schedule's fp32 entries at t = (s+1)/T and s/T (looked up
+        as step_coefficients looks them up); alpha = sqrt(sigmoid(-gamma)), sigma = sqrt(sigmoid(gamma)), lambda = -gamma/2
+        and h = lambda_s - lambda_t. Row r < T (step s = T-1-r): sigma_t, 1/alpha_t, sigma_s/sigma_t, c1 = -alpha_s
+        expm1(-h), c2a = c1 (1 + 1/(2 rho)), c2b = -c1/(2 rho) with rho = h_{r-1}/h_r (DPM-Solver++(2M); c2a = c1 and c2b = 0
+        for 'ddim' and in row 0), h, 0. Row T: sigma_0, 1/alpha_0 and zeros. Every entry is evaluated in fp64 and rounded to
+        fp32 once; the table does not depend on the batch size. Cached like jump_coefficients. ValueError for another kind
+        and for T above the schedule's timesteps, where grid points repeat and h would be 0."""
+        if kind not in ('ddim', 'dpmpp_2m'):
+            raise ValueError(f"solver_coefficients takes 'ddim' or 'dpmpp_2m' (got {kind!r})")
+        T = self.T
+        if T > self.gamma.timesteps:
+            raise ValueError(f"the ODE solvers need T <= the schedule's timesteps ({self.gamma.timesteps}); T = {T} would "
+                             "repeat grid points")
+        key = ('solver', kind, T, self.gamma.gamma._version, self.gamma.gamma.data_ptr())
+        cache = self.__dict__.setdefault('_coef_cache', {})
+        if key in cache:
+            return cache[key]
+        gamma = self._cpu_gamma()
+        one = lambda v: float(gamma(torch.full((1, 1), fill_value=v) / T)[0, 0])   # exact: an fp32 table entry
+        g = [one(T - r) for r in range(T)] + [float(gamma(torch.zeros((1, 1)))[0, 0])]   # g[r] = gamma_t of row r
+        alpha = lambda v: math.sqrt(1.0 / (1.0 + math.exp(v)))
+        sigma = lambda v: math.sqrt(1.0 / (1.0 + math.exp(-v)))
+        out = (C.c_float * (8 * (T + 1)))()
+        h_prev = None
+        for r in range(T):
+            g_t, g_s = g[r], g[r + 1]
+            h = (g_t - g_s) / 2.0
+            c1 = -alpha(g_s) * math.expm1(-h)
+            c2a, c2b = c1, 0.0
+            if kind == 'dpmpp_2m' and r > 0:
+                rho = h_prev / h
+                c2a, c2b = c1 * (1.0 + 1.0 / (2.0 * rho)), -c1 / (2.0 * rho)
+            out[8 * r:8 * r + 8] = [sigma(g_t), 1.0 / alpha(g_t), sigma(g_s) / sigma(g_t), c1, c2a, c2b, h, 0.0]
+            h_prev = h
+        out[8 * T:8 * T + 8] = [sigma(g[T]), 1.0 / alpha(g[T])] + [0.0] * 6
+        if len(cache) >= 8:
+            cache.pop(next(iter(cache)))
+        cache[key] = out
+        return out
+
+    def _solver(self, solver):
+        """_sample_slice's `solver` of a call: (kind, T, table) from `solver`, or the `solver` attribute when None; None for
+        'ancestral'. ValueError for another name than 'ancestral', 'ddim' and 'dpmpp_2m', for an ODE solver on
+        InpaintingEDM, and where solver_coefficients raises."""
+        name = self.solver if solver is None else solver
+        if not isinstance(name, str) or name not in _native.SOLVERS:
+            raise ValueError(f"solver is one of {sorted(_native.SOLVERS)} (got {name!r})")
+        if name == 'ancestral':
+            return None
+        if self._SAMPLER == _native.SAMPLER_INPAINT:
+            raise ValueError(f"solver={name!r} takes the linker sampler (EDM) only: InpaintingEDM's q(z_s | z_t, x) and "
+                             "centre-of-mass projection have no deterministic counterpart here")
+        return _native.SOLVERS[name], self.T, self.solver_coefficients(name)
 
     def _clash_guidance(self, clash_guidance, start_step):
         """_sample_slice's `guide` of a call: (scale, steps, clash table) from `clash_guidance`, or the `clash_guidance`
@@ -838,7 +904,7 @@ class EDM(torch.nn.Module):
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, anchors=None, clash_guidance=None):
+                     require_anchors=None, anchors=None, clash_guidance=None, solver=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -946,6 +1012,16 @@ class EDM(torch.nn.Module):
         seeds and recovery rounds are as without it; the rounds are guided too. scale = 0 or steps = 0 is the plain call,
         bit for bit. A sampler tool with no claim about chemistry. ValueError for a bool, negative or non-finite scale,
         steps outside [0, T], FC graphs, start_step and InpaintingEDM.
+        `solver` (None: the `solver` attribute, default 'ancestral') picks the reverse update (dl_set_solver): 'ancestral'
+        is the reference's p(z_s | z_t); 'ddim' (first order) and 'dpmpp_2m' (DPM-Solver++(2M), second order from a row's
+        second step on) are deterministic steps of the probability-flow ODE with the same eps-network, meant for a loop
+        shortened with `T` (edm.T = 20, as the reference's --n_steps sets it). The final step returns the data prediction
+        with no noise, so a sample is a function of its z_T (or its q(z_t0 | x)) alone. The draws stay those of the
+        ancestral loop in count and order (only draw 0 is read), so seeds, noise=, the batch stream's offset, start_step in
+        both forms (a row's own start step is its first), the recovery rounds (which start their rows afresh),
+        linker_sizes, clash_guidance (which pushes z_s after the update) and `devices` work as without it. The effect on
+        a trained model's samples is not measured. ValueError for another name, for InpaintingEDM and for T above the
+        schedule's timesteps.
         The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
         and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
         device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
@@ -965,6 +1041,7 @@ class EDM(torch.nn.Module):
         start = self._start(start_step, n_samples)
         r = self._resamplings(resamplings)
         guide = self._clash_guidance(clash_guidance, start_step)
+        ode = self._solver(solver)
         redraw = self._linker_sizes(linker_sizes, seeds, noise, batch_slice, start_step, x, linker_mask)
         retries = self._nan_retries(nan_retries, seeds, noise, batch_slice, x)
         check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free,
@@ -1007,7 +1084,8 @@ class EDM(torch.nn.Module):
                                             engines, places, dev, noise=noise, dev_seeds=dev_seeds,
                                             rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check,
                                             start=start, redraw=redraw, sets=sets,
-                                            resample=self._resample(r, n_samples), anchors=anchor_flags, guide=guide)
+                                            resample=self._resample(r, n_samples), anchors=anchor_flags, guide=guide,
+                                            solver=ode)
         by_device = {}
         for dev_i, c in calls:
             by_device.setdefault(dev_i, []).append(c)
@@ -1081,7 +1159,7 @@ class EDM(torch.nn.Module):
     def sample_many(self, requests, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
                     require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None,
-                    clash_guidance=None):
+                    clash_guidance=None, solver=None):
         """Samples many requests -- each a dict of sample_chain's inputs (x, h, node_mask, fragment_mask, linker_mask,
         edge_mask, context) holding its own (B_k, N_k) batch on one CUDA device -- in a few shared launches, and returns their
         (keep_frames, B_k, N_k, 3+F) chains in request order on that device. results[k] equals, bit for bit,
@@ -1120,7 +1198,8 @@ class EDM(torch.nn.Module):
         `resamplings` as in sample_chain, for every request; requests then also share a launch only where sample_chain
         would give them the same jump coefficients (jump_coefficients, which depend on the batch size as the table does).
         `clash_guidance` as in sample_chain, for every request; it is part of every launch's key, and it draws nothing, so
-        packing does not change a request's rows.
+        packing does not change a request's rows. `solver` as in sample_chain, for every request: its table does not
+        depend on the batch size, so it adds nothing to the key.
         Raises ValueError for an empty list, the batch stream (its draws depend on B and N), noise= or a replaced draw
         function, host inputs, requests on different devices or of different feature or context widths, and seeds that do
         not match the requests. It takes no `require_unique`, and raises ValueError when the attribute is set: a launch packs
@@ -1143,6 +1222,7 @@ class EDM(torch.nn.Module):
             self._start(start_step, 1)      # validates it before anything else is checked
         r_passes = self._resamplings(resamplings)
         guide = self._clash_guidance(clash_guidance, start_step)
+        ode = self._solver(solver)
         for k, r in enumerate(requests):
             if 'noise' in r or 'batch_slice' in r:
                 raise ValueError(f"request {k} passes noise= or batch_slice=: sample_many samples per-molecule streams, "
@@ -1254,7 +1334,7 @@ class EDM(torch.nn.Module):
                                                       [where], dev, dev_seeds=dev_seeds, retries=retries, check=check,
                                                       start=start, redraw=redraw, sets=sets,
                                                       resample=self._resample(r_passes, sizes[ks[0]]), anchors=anchors,
-                                                      guide=guide)
+                                                      guide=guide, solver=ode)
             finishes.append(finish)
             by_device.setdefault(dev_i, []).append(
                 functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
@@ -1340,7 +1420,8 @@ class EDM(torch.nn.Module):
         return coefs, starts, keys
 
     def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
-                       retries=0, check=0, start=None, redraw=None, sets=None, resample=None, anchors=None, guide=None):
+                       retries=0, check=0, start=None, redraw=None, sets=None, resample=None, anchors=None, guide=None,
+                       solver=None):
         """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
         inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
         replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
@@ -1348,7 +1429,8 @@ class EDM(torch.nn.Module):
         b0, B_full) or the `noise` tensor; `retries` and `check` as returned by _nan_retries and _checks; `start` as
         returned by _start; `redraw` as returned by _linker_sizes (its rounds then redraw sizes, into `sizes`); `sets` as
         returned by _hash_sets, copied to each slice's device; `resample` as returned by _resample; `anchors` as returned
-        by _anchors, each slice's rows on its device; `guide` as returned by _clash_guidance.
+        by _anchors, each slice's rows on its device; `guide` as returned by _clash_guidance; `solver` as returned by
+        _solver.
         Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
         (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
         back and returns dict(chain, flags, used, attempts, passed, sizes, bad, consumed) on `dev`; `passed` holds
@@ -1416,7 +1498,7 @@ class EDM(torch.nn.Module):
                 stream, nz, sd, rng_i,
                 (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i, sets_i, lh_i,
                  (allowed, rs_i) if rings else None, an_i) if recover else None,
-                start.rows(lo, hi) if isinstance(start, StartSteps) else start, resample, guide)))
+                start.rows(lo, hi) if isinstance(start, StartSteps) else start, resample, guide, solver)))
 
         def finish():
             if not whole:
@@ -1501,7 +1583,7 @@ class InpaintingEDM(EDM):
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, anchors=None, clash_guidance=None):
+                     require_anchors=None, anchors=None, clash_guidance=None, solver=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -1523,7 +1605,8 @@ class InpaintingEDM(EDM):
         two final draws: 1 + T(3r-1) + 2 (noise= holds that many prepared slabs, draw_noise_inpaint(resamplings=r) makes
         them; the batch stream advances by as many draws; per-molecule streams use their draws in that order). r = 1 is
         the plain sampler, bit for bit. A call costs about r times the loop. ValueError for a non-integer, a bool or
-        r < 1. `clash_guidance` raises ValueError unless None: this loop re-noises the pocket."""
+        r < 1. `clash_guidance` raises ValueError unless None: this loop re-noises the pocket. `solver` unless None or
+        'ancestral': this sampler has no ODE update."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
@@ -1532,7 +1615,7 @@ class InpaintingEDM(EDM):
                                     require_unique=require_unique, require_novel=require_novel,
                                     exclude_hashes=exclude_hashes, resamplings=resamplings,
                                     require_ring_sizes=require_ring_sizes, require_anchors=require_anchors,
-                                    anchors=anchors, clash_guidance=clash_guidance)
+                                    anchors=anchors, clash_guidance=clash_guidance, solver=solver)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

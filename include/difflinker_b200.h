@@ -21,6 +21,8 @@
  *   EDM, from q(z_t0 | x) of a known linker (edm.py:67-74) dl_set_start_step, then any dl_sample_chain* entry point
  *     at step t0 (partial diffusion, no reference API)
  *     ... at one step t0[b] per molecule                 dl_set_start_steps, then the per-row entry points
+ *   EDM, deterministic DDIM or DPM-Solver++(2M) steps   dl_set_solver, then any dl_sample_chain* entry point
+ *     instead of p(z_s | z_t) (no reference API)
  *   InpaintingEDM, r RePaint passes per step            dl_set_resamplings, then any dl_sample_chain* entry point
  *     (DiffSBDD's inpaint(..., resamplings=r), no reference API)
  *   either, resampling only the molecules that diverged  dl_sample_chain_retry, dl_retry_seed, dl_last_retry_ms
@@ -80,6 +82,7 @@ enum { DL_GRAPH_FC = 0, DL_GRAPH_4A = 1, DL_GRAPH_FC_4A = 2, DL_GRAPH_FC_10A_4A 
 enum { DL_EDGE_AUTO = 0, DL_EDGE_SIMT = 1, DL_EDGE_WGMMA = 2 };
 enum { DL_SAMPLER_LINKER = 0, DL_SAMPLER_INPAINT = 1 };
 enum { DL_AGGR_SUM = 0, DL_AGGR_MEAN = 1 };
+enum { DL_SOLVER_ANCESTRAL = 0, DL_SOLVER_DDIM = 1, DL_SOLVER_DPMPP_2M = 2 };   /* dl_set_solver */
 
 /* Mirrors the kwargs of Dynamics.__init__ (src/egnn.py:324-329) that reach the hot path. */
 typedef struct dl_config {
@@ -755,6 +758,34 @@ dl_status dl_set_resamplings(dl_engine* e, int32_t r, int32_t T, const float* ju
  * n_types > F, N > 8192 and a NULL context.
  */
 dl_status dl_set_clash_guidance(dl_engine* e, float scale, int32_t steps, int32_t n_types, const float* clash);
+/*
+ * ODE solvers for DL_SAMPLER_LINKER (no reference API): the following dl_sample_chain* calls of this engine -- the recovery
+ * rounds of dl_sample_chain_retry included -- replace the ancestral update p(z_s | z_t) by a deterministic step of the
+ * probability-flow ODE, so a sample is a function of its z_T (or its q(z_t0 | x)) alone. With alpha = sqrt(sigmoid(-gamma)),
+ * sigma = sqrt(sigmoid(gamma)), lambda = -gamma / 2 at t = (s+1)/T and s/T, and h = lambda_s - lambda_t > 0, row r < T of
+ * the (T + 1, 8) HOST fp32 `table` (step s = T-1-r, dl_step_coef's row order) holds
+ *   [0] sigma_t   [1] 1/alpha_t   [2] sigma_s/sigma_t   [3] c1 = -alpha_s expm1(-h)
+ *   [4] c2a = c1 (1 + 1/(2 rho))   [5] c2b = -c1 / (2 rho)   [6] h   [7] 0,      rho = h_{r-1} / h_r
+ * and row T [0] sigma_0, [1] 1/alpha_0, the rest 0. EDM.solver_coefficients builds it, each entry evaluated in fp64 from the
+ * fp32 gamma table and rounded once; for DL_SOLVER_DDIM, and in row 0, c2a = c1 and c2b = 0. On linker rows, eps = the
+ * dynamics output times linker_mask and
+ *   xhat = [1] * (z_t - [0] * eps)                         (the data prediction)
+ *   z_s  = [2] * z_t + [3] * xhat                          (DDIM; DPM-Solver++(2M) at a row's first step)
+ *   z_s  = [2] * z_t + ([4] * xhat + [5] * xhat')          (DPM-Solver++(2M) after it; xhat' = the row's previous xhat)
+ *   final row: x = xhat, with no sigma_x noise, then unnormalised and one-hot as the ancestral sampler's final row.
+ * Fragment rows keep z_t bit for bit and padded rows stay 0, as in the ancestral loop. A row's first step is the loop's
+ * first (its start step with dl_set_start_step), or its own start step with dl_set_start_steps; a recovery round starts its
+ * rows afresh. The history lives in the engine's workspace. The draws are those of the ancestral loop, in count and order
+ * (T + 2, or t0 + 2), so the device streams advance as they do without a solver, but only draw 0 (z_T, or the eps of
+ * q(z_t0 | x)) is read. dl_step_coef keeps giving the time feature and the frames. Clash guidance (dl_set_clash_guidance)
+ * pushes z_s after the update and never the history.
+ * The table is copied into host memory here, and each following call uploads the rows it runs on the engine's loop stream,
+ * so a call already enqueued keeps its table. Sticky like dl_set_resamplings. kind = DL_SOLVER_ANCESTRAL switches it off
+ * (T and table are ignored): the calls then launch exactly what they launch without it. DL_ERR_INVALID: here, an unknown
+ * kind, and while on a NULL table, T outside [1, 2^24], a non-finite entry or a row r < T with h <= 0; at the sampling
+ * call, a T other than the one set and DL_SAMPLER_INPAINT.
+ */
+dl_status dl_set_solver(dl_engine* e, int32_t kind, int32_t T, const float* table);
 /* The (n_draws,B,N,3+F) tensor the device-side stream of dl_sample_chain_rng stands for (tests, debugging). DEVICE out. */
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream);
