@@ -167,6 +167,13 @@ struct dl_engine {
   HostStage anchors;
   bool anchors_set = false;
   int anchors_B = 0, anchors_N = 0;
+  // dl_set_fixed_atoms: the (fixed_B, fixed_N) int8 flags of the linker rows the next dl_sample_chain* call keeps (in the
+  // buffer, followed by two ints of the call's vetting) and the host copy of the (fixed_T + 1, 2) scalars; that call reads
+  // and clears fixed_set, and its recovery rounds gather the flags of their rows
+  HostStage fixed;
+  bool fixed_set = false;
+  int fixed_B = 0, fixed_N = 0, fixed_T = 0;
+  std::vector<float> fixed_scalars;
   cudaEvent_t ev_r0 = nullptr, ev_r1 = nullptr, ev_g0 = nullptr, ev_g1 = nullptr;
   float retry_ms = 0.f;
   cudaStream_t loop_stream = nullptr;
@@ -420,6 +427,8 @@ struct FwdIO {
   RowStarts rows{};   // per-molecule start steps, or rows.lag = null
   int R = 1; const float* jump = nullptr;   // resampling passes per reverse step (dl_set_resamplings), T counting passes
   const float* ode = nullptr;               // the solver rows of the loop (dl_set_solver), or null: the ancestral update
+  const int8_t* fixed = nullptr;            // fixed atoms (dl_set_fixed_atoms): the rows' flags, or null
+  const float* fix = nullptr;               // ... and the (alpha_s, sigma_s) rows of the loop
 };
 
 ProjW proj_of(const EdgeMlpW& w) { return ProjW{w.W1a_t, w.W1b_t, w.b1}; }
@@ -615,11 +624,14 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     fa.norm0 = io.norm0; fa.norm1 = io.norm1; fa.bias1 = io.bias1; fa.chain = io.chain; fa.rows = io.rows;
     // the 2M history lives in ws.eps, which the fused linker update never writes otherwise
     fa.ode = io.ode; fa.hist = io.ode && e->solver_kind == DL_SOLVER_DPMPP_2M ? ws.eps : nullptr;
+    fa.fixed = io.fixed; fa.xh0 = io.xh0; fa.fix = io.fix;
   } else if (io.sampler) {
     fa.tag_step = e->step_ctr + (io.R > 1 ? 2 : 1);   // with resampling the pass counter is not the step
   }
   const bool per_mol = io.rng.on == NOISE_PER_MOLECULE;
-  auto* finish = fa.ode ? (per_mol ? k_finish<true, true> : k_finish<false, true>)
+  auto* finish = fa.fixed ? (fa.ode ? (per_mol ? k_finish<true, true, true> : k_finish<false, true, true>)
+                                   : (per_mol ? k_finish<true, false, true> : k_finish<false, false, true>))
+               : fa.ode ? (per_mol ? k_finish<true, true> : k_finish<false, true>)
                         : (per_mol ? k_finish<true> : k_finish<false>);
   TIMED("k_finish", st, (launch_chain(finish, dim3((n + 15) / 16), dim3(256), 0, st, gm, fa)));
   LAUNCH_CHECK();
@@ -632,7 +644,7 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     ga.scale = e->guide_scale; ga.clash = e->guide_clash;
     ga.node_mask = io.node_mask; ga.linker_mask = io.linker_mask; ga.context = io.context;
     ga.step = e->step_ctr + 1; ga.T = io.T; ga.steps = e->guide_steps; ga.coef = e->coef_dev;
-    ga.chain = io.chain; ga.norm0 = io.norm0;
+    ga.chain = io.chain; ga.norm0 = io.norm0; ga.fixed = io.fixed;
     TIMED("k_clash_guide", st, (launch_clash_guide(ga, B, st)));
     LAUNCH_CHECK();
     e->launches += 1;
@@ -786,16 +798,17 @@ struct SubBatchScope {
 // sorted by t0 descending, so that the rows a loop step computes -- those that have started -- are a prefix.
 struct RowOrder {
   const float *xh, *fragment_mask, *linker_mask, *context, *alpha, *sigma;
-  const int8_t *node_mask, *edge_mask;
+  const int8_t *node_mask, *edge_mask, *fixed;
   RowStarts rs;
   std::vector<int> active;   // (Tl + 1) the length of the prefix loop step r computes
 };
 
 // Orders the B rows of a loop of Tl + 1 steps, stages the order, lags and scalars, and gathers the inputs (and with
-// per-molecule streams the seeds, into the workspace) in that order with the recovery rounds' gather.
+// per-molecule streams the seeds, into the workspace; with fixed atoms their flags) in that order with the recovery rounds'
+// gather.
 dl_status order_rows(dl_engine* e, int B, int N, int Tl, const float* xh, const int8_t* node_mask, const float* fragment_mask,
                      const float* linker_mask, const int8_t* edge_mask, const float* context, const unsigned long long* seeds,
-                     cudaStream_t st, RowOrder& ro) {
+                     const int8_t* fixed, cudaStream_t st, RowOrder& ro) {
   const std::vector<int32_t>& t0 = e->starts_t0;
   std::vector<int> order(B), lag(B);
   std::vector<float> al(B), sg(B);
@@ -814,7 +827,7 @@ dl_status order_rows(dl_engine* e, int B, int N, int Tl, const float* xh, const 
   const int i_src = sl.in(order.data(), B * sizeof(int)), i_lag = sl.in(lag.data(), B * sizeof(int)),
             i_al = sl.in(al.data(), B * sizeof(float)), i_sg = sl.in(sg.data(), B * sizeof(float)), i_xh = sl.out(n * xd * 4),
             i_nm = sl.out(n), i_fm = sl.out(n * 4), i_lm = sl.out(n * 4), i_em = sl.add(nullptr, n * N, fc_em),
-            i_ctx = sl.add(nullptr, n * C * 4, context != nullptr && C > 0);
+            i_ctx = sl.add(nullptr, n * C * 4, context != nullptr && C > 0), i_fx = sl.add(nullptr, n, fixed != nullptr);
   dl_status s = stage_inputs(e->start_rows, sl, st);
   if (s != DL_OK) return s;
   RowGatherArgs ga{};
@@ -824,14 +837,40 @@ dl_status order_rows(dl_engine* e, int B, int N, int Tl, const float* xh, const 
   ga.s_xh = sl.at<float>(i_xh); ga.s_fragment_mask = sl.at<float>(i_fm); ga.s_linker_mask = sl.at<float>(i_lm);
   ga.s_context = sl.at<float>(i_ctx); ga.s_node_mask = sl.at<int8_t>(i_nm); ga.s_edge_mask = sl.at<int8_t>(i_em);
   ga.s_seeds = e->ws.seeds;
-  k_gather_rows<false><<<B, 256, 0, st>>>(ga);
+  const RowFixedArgs fa{fixed, sl.at<int8_t>(i_fx)};
+  if (fixed) k_gather_rows<false><<<B, 256, 0, st>>>(ga, fa);
+  else k_gather_rows<false><<<B, 256, 0, st>>>(ga);
   LAUNCH_CHECK();
   e->launches += 1;
+  ro.fixed = fa.s_fixed;
   ro.xh = ga.s_xh; ro.fragment_mask = ga.s_fragment_mask; ro.linker_mask = ga.s_linker_mask; ro.context = ga.s_context;
   ro.node_mask = ga.s_node_mask; ro.edge_mask = ga.s_edge_mask;
   ro.alpha = sl.at<const float>(i_al); ro.sigma = sl.at<const float>(i_sg);
   ro.rs = RowStarts{sl.at<const int>(i_lag), sl.at<const int>(i_src), (int)n};
   return DL_OK;
+}
+
+// The fixed atoms of a sampling call (dl_set_fixed_atoms): the (B, N) flags on the device, B, N and T as set, and the
+// host copy of the (T + 1, 2) scalars; flags = null: none. `vetted`: the flags are a recovery round's, gathered from a call
+// whose flags were checked.
+struct CallFixed {
+  const int8_t* flags = nullptr;
+  int B = 0, N = 0, T = 0;
+  const float* scalars = nullptr;
+  bool vetted = false;
+  int* bad = nullptr;        // two ints of device memory for k_fixed_check, unless vetted
+};
+
+// What dl_set_fixed_atoms set since the engine's previous sampling call, which every call reads and clears.
+CallFixed take_fixed(dl_engine* e) {
+  CallFixed fx;
+  if (e && e->fixed_set) {
+    fx.flags = reinterpret_cast<const int8_t*>(e->fixed.buf);
+    fx.B = e->fixed_B; fx.N = e->fixed_N; fx.T = e->fixed_T; fx.scalars = e->fixed_scalars.data();
+    fx.bad = reinterpret_cast<int*>(e->fixed.buf + align256((size_t)fx.B * fx.N));
+  }
+  if (e) e->fixed_set = false;
+  return fx;
 }
 
 // Captures one reverse step over the first Bp rows of the workspace into *graph.
@@ -925,6 +964,7 @@ dl_status dl_destroy(dl_engine* e) {
   if (e->hashes.buf) cudaFree(e->hashes.buf);
   if (e->ring_masks.buf) cudaFree(e->ring_masks.buf);
   if (e->anchors.buf) cudaFree(e->anchors.buf);
+  if (e->fixed.buf) cudaFree(e->fixed.buf);
   if (e->wblob) cudaFree(e->wblob);
   if (e->wblob_tc) cudaFree(e->wblob_tc);
   if (e->coef_dev) cudaFree(e->coef_dev);
@@ -1073,16 +1113,17 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
                                    const float* xh, const int8_t* node_mask, const float* fragment_mask,
                                    const float* linker_mask, const int8_t* edge_mask, const float* context,
                                    const float* noise, const NoiseRng* rng, const dl_step_coef* coef, const float* norm,
-                                   float* chain, int32_t* nan_flags, void* stream);
+                                   float* chain, int32_t* nan_flags, void* stream, const CallFixed& fx);
 
 dl_status dl_sample_chain(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
                           const float* xh, const int8_t* node_mask, const float* fragment_mask,
                           const float* linker_mask, const int8_t* edge_mask, const float* context,
                           const float* noise, const dl_step_coef* coef, const float* norm, float* chain,
                           int32_t* nan_flags, void* stream) {
+  const CallFixed fx = take_fixed(e);
   if (!noise) { set_err("null argument (noise): use dl_sample_chain_rng to draw on the device"); return DL_ERR_INVALID; }
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, noise,
-                           nullptr, coef, norm, chain, nan_flags, stream);
+                           nullptr, coef, norm, chain, nan_flags, stream, fx);
 }
 
 dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
@@ -1090,6 +1131,7 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
                               const float* linker_mask, const int8_t* edge_mask, const float* context, uint64_t seed,
                               uint64_t offset, uint64_t* offset_consumed, const dl_step_coef* coef, const float* norm,
                               float* chain, int32_t* nan_flags, void* stream) {
+  const CallFixed fx = take_fixed(e);
   dl_status s = check_shapes(e, B, N);
   if (s == DL_OK) s = check_slice(e, B);
   if (s != DL_OK) return s;
@@ -1104,21 +1146,34 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
   const NoiseRng q = make_rng(e, B, N, seed, offset);
   if (offset_consumed) *offset_consumed = sampler_draws(sampler, loop_steps(e, T), R) * q.per_draw;
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, nullptr,
-                           &q, coef, norm, chain, nan_flags, stream);
+                           &q, coef, norm, chain, nan_flags, stream, fx);
 }
 
-dl_status dl_sample_chain_seeded(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
-                                 const float* xh, const int8_t* node_mask, const float* fragment_mask,
-                                 const float* linker_mask, const int8_t* edge_mask, const float* context,
-                                 const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
-                                 int32_t* nan_flags, void* stream) {
+}  // extern "C"
+
+// dl_sample_chain_seeded with the fixed atoms fx: the recovery rounds' entry, which passes their gathered flags.
+static dl_status sample_seeded(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                               const float* xh, const int8_t* node_mask, const float* fragment_mask, const float* linker_mask,
+                               const int8_t* edge_mask, const float* context, const uint64_t* seeds, const dl_step_coef* coef,
+                               const float* norm, float* chain, int32_t* nan_flags, void* stream, const CallFixed& fx) {
   // the seeds name the molecules, so the engine's batch slice does not apply; sample_chain_impl copies them into the
   // workspace and points the stream at that copy
   NoiseRng q{};
   q.seeds = reinterpret_cast<const unsigned long long*>(seeds);
   q.F = e ? e->cfg.in_node_nf : 0; q.N = N; q.on = NOISE_PER_MOLECULE;
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, nullptr,
-                           &q, coef, norm, chain, nan_flags, stream);
+                           &q, coef, norm, chain, nan_flags, stream, fx);
+}
+
+extern "C" {
+
+dl_status dl_sample_chain_seeded(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
+                                 const float* xh, const int8_t* node_mask, const float* fragment_mask,
+                                 const float* linker_mask, const int8_t* edge_mask, const float* context,
+                                 const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
+                                 int32_t* nan_flags, void* stream) {
+  return sample_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
+                       coef, norm, chain, nan_flags, stream, take_fixed(e));
 }
 
 dl_status dl_set_noise_slice(dl_engine* e, int32_t B_full, int32_t b0) {
@@ -1242,6 +1297,35 @@ dl_status dl_set_anchors(dl_engine* e, int32_t B, int32_t N, const int8_t* ancho
   return DL_OK;
 }
 
+dl_status dl_set_fixed_atoms(dl_engine* e, int32_t B, int32_t N, const int8_t* fixed, int32_t T, const float* scalars,
+                             void* stream) {
+  if (!e) { set_err("dl_set_fixed_atoms: null engine"); return DL_ERR_INVALID; }
+  e->fixed_set = false;
+  if (!fixed) return DL_OK;
+  const char* why = nullptr;
+  if (B < 1 || N < 1) why = "B and N must be >= 1";
+  else if (T < 1 || T > (1 << 24)) why = "T must lie in [1, 2^24]";
+  else if (!scalars) why = "null scalars";
+  if (why) { set_err("dl_set_fixed_atoms: %s", why); return DL_ERR_INVALID; }
+  for (int i = 0; i < 2 * (T + 1); ++i)
+    if (!std::isfinite(scalars[i])) {
+      set_err("dl_set_fixed_atoms: scalars[%d][%d] is not finite", i / 2, i % 2);
+      return DL_ERR_INVALID;
+    }
+  CK(cudaSetDevice(e->cfg.device));
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  StageLayout fl;
+  const int i_fx = fl.out((size_t)B * N);
+  fl.out(2 * sizeof(int));   // the call's vetting (k_fixed_check)
+  dl_status s = stage_inputs(e->fixed, fl, st);
+  if (s != DL_OK) return s;
+  CK(cudaMemcpyAsync(fl.at<int8_t>(i_fx), fixed, (size_t)B * N, cudaMemcpyDefault, st));
+  e->fixed_scalars.assign(scalars, scalars + 2 * (size_t)(T + 1));
+  e->fixed_set = true;
+  e->fixed_B = B; e->fixed_N = N; e->fixed_T = T;
+  return DL_OK;
+}
+
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream) {
   dl_status s = check_shapes(e, B, N);
@@ -1284,7 +1368,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
                                    const float* xh, const int8_t* node_mask, const float* fragment_mask,
                                    const float* linker_mask, const int8_t* edge_mask, const float* context,
                                    const float* noise, const NoiseRng* rng, const dl_step_coef* coef, const float* norm,
-                                   float* chain, int32_t* nan_flags, void* stream) {
+                                   float* chain, int32_t* nan_flags, void* stream, const CallFixed& fx) {
   const bool per_mol = rng && rng->on == NOISE_PER_MOLECULE;
   dl_status s = check_shapes(e, B, N);
   if (s == DL_OK) s = check_sampler(e, sampler, T, keep_frames, noise || (rng && (!per_mol || rng->seeds)), xh, node_mask,
@@ -1326,6 +1410,13 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     else set_err("dl_set_solver was given the table of T = %d; the call samples T = %d", e->solver_T, T);
     return DL_ERR_INVALID;
   }
+  const bool fix = fx.flags != nullptr;
+  if (fix && (inpaint || B != fx.B || N != fx.N || T != fx.T)) {
+    if (inpaint) set_err("dl_set_fixed_atoms takes DL_SAMPLER_LINKER only: the inpainting sampler re-noises every atom");
+    else set_err("dl_set_fixed_atoms was given B = %d, N = %d, T = %d; the call samples B = %d, N = %d, T = %d", fx.B, fx.N,
+                 fx.T, B, N, T);
+    return DL_ERR_INVALID;
+  }
   // A start step t0 runs the table's last t0 + 1 rows -- steps t0-1 .. 0, then the final one -- as a loop of Tl = t0 steps:
   // loop step r reads row r of the copied rows and draw r + 1, so the draws are eps, one per step and the final one.
   const int Tl = loop_steps(e, T);
@@ -1335,8 +1426,9 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   // only its last pass writes; the jump coefficients follow the table on the device. A solver (never with R > 1, which is
   // the inpainting sampler's) puts the same rows of its table there instead.
   const int P = Tl * R, rows = P + 1;
+  // Fixed atoms put the (alpha_s, sigma_s) of the loop's Tl steps after them.
   const size_t coef_bytes = (size_t)rows * sizeof(dl_step_coef) + (R > 1 ? e->jump.size() * sizeof(float) : 0) +
-                            (ode ? (size_t)rows * 8 * sizeof(float) : 0);
+                            (ode ? (size_t)rows * 8 * sizeof(float) : 0) + (fix ? (size_t)Tl * 2 * sizeof(float) : 0);
   if (R > 1) {
     e->coef_passes.resize(rows);
     for (int p = 0; p < P; ++p) {
@@ -1385,16 +1477,40 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   if (ode)
     CK(cudaMemcpyAsync(const_cast<float*>(ode_dev), e->solver_table.data() + (size_t)(T - Tl) * 8,
                        (size_t)rows * 8 * sizeof(float), cudaMemcpyHostToDevice, st));
+  const float* fix_dev = fix ? e->coef_dev + (size_t)rows * 8 + (ode ? (size_t)rows * 8 : 0) : nullptr;
+  if (fix) {
+    CK(cudaMemcpyAsync(const_cast<float*>(fix_dev), fx.scalars + (size_t)(T - Tl) * 2, (size_t)Tl * 2 * sizeof(float),
+                       cudaMemcpyHostToDevice, st));
+    if (!fx.vetted) {
+      // the flags against the masks and the kept types (a recovery round's rows come from a call that passed this)
+      int bad[2] = {0, 0};
+      CK(cudaMemsetAsync(fx.bad, 0, sizeof(bad), st));
+      k_fixed_check<<<(B * N + 255) / 256, 256, 0, st>>>(B * N, 3 + e->cfg.in_node_nf, fx.flags, node_mask, fragment_mask,
+                                                        linker_mask, xh, norm[1], norm[2], fx.bad);
+      LAUNCH_CHECK();
+      e->launches += 1;
+      CK(cudaMemcpyAsync(bad, fx.bad, sizeof(bad), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      if (bad[0] || bad[1]) {
+        const int g = (bad[0] ? bad[0] : bad[1]) - 1;
+        set_err("dl_set_fixed_atoms: row %d of molecule %d %s", g % N, g / N,
+                bad[0] ? "is flagged but is not a live linker row (node_mask and linker_mask set, fragment_mask 0)"
+                       : "is flagged but its type channels are not a one-hot");
+        return DL_ERR_INVALID;
+      }
+    }
+  }
   NoiseRng q = rng ? *rng : NoiseRng{};
   // per-molecule start steps: the loop runs on the rows in start-step order, each loop step on those that have started
   RowOrder ro{};
   if (per_row) {
     s = order_rows(e, B, N, Tl, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, per_mol ? rng->seeds : nullptr,
-                   st, ro);
+                   fx.flags, st, ro);
     if (s != DL_OK) return s;
     xh = ro.xh; node_mask = ro.node_mask; fragment_mask = ro.fragment_mask; linker_mask = ro.linker_mask;
     edge_mask = ro.edge_mask; context = ro.context;
   }
+  const int8_t* fixed = per_row ? ro.fixed : fx.flags;   // in the workspace's row order
   if (per_mol) {
     // the captured step reads the engine's copy: the caller's seeds buffer is free once the call has been enqueued
     if (!per_row)
@@ -1433,6 +1549,17 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     LAUNCH_CHECK();
     e->launches += 1;
   }
+  if (fix) {
+    // the kept rows start from q(z_t | x) at the call's start: T (the scalars' last row), t0, or each row's own t0
+    const float al = partial ? e->start_alpha : fx.scalars[2 * T], sg = partial ? e->start_sigma : fx.scalars[2 * T + 1];
+    const float* al_rows = per_row ? ro.alpha : nullptr;
+    const float* sg_rows = per_row ? ro.sigma : nullptr;
+    const RowStarts rs = per_row ? ro.rs : RowStarts{};
+    if (per_mol) k_init_z_fixed<true><<<(n * xd + 255) / 256, 256, 0, st>>>(n, N, xd, xh, fragment_mask, linker_mask, fixed, noise, q, al, sg, al_rows, sg_rows, rs, e->ws.z);
+    else k_init_z_fixed<false><<<(n * xd + 255) / 256, 256, 0, st>>>(n, N, xd, xh, fragment_mask, linker_mask, fixed, noise, q, al, sg, al_rows, sg_rows, rs, e->ws.z);
+    LAUNCH_CHECK();
+    e->launches += 1;
+  }
   // inpainting: the dynamics see linker_mask=None (edm.py:632), so every live row gets a coordinate update
   int Bp = per_row ? ro.active[0] : B;   // the rows the current step graph computes
   if ((s = build_forward_plan(e, Bp, N, node_mask, inpaint ? nullptr : linker_mask, edge_mask, st)) != DL_OK) return s;
@@ -1447,6 +1574,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   io.chain = chain; io.T = P; io.norm0 = norm[0]; io.norm1 = norm[1]; io.bias1 = norm[2];
   io.rows = per_row ? ro.rs : RowStarts{};
   io.R = R; io.jump = jump_dev; io.ode = ode_dev;
+  io.fixed = fixed; io.fix = fix_dev;
 
   // capture ONE reverse step; the step index lives on the device, so the same graph serves all Tl+1 steps (all P+1 passes
   // with resampling) -- with per-molecule start steps, all steps of one prefix length: the graph is recaptured whenever the
@@ -1698,17 +1826,19 @@ const char* sets_error(dl_engine* e, int require, const dl_hash_sets* hs, cudaSt
 // flag is set or a required bit is missing, and a resampled row replaces the caller's unless the caller's row is finite and
 // the new one diverged. `hs` (or null) holds the known set of DL_CHECK_NOVEL and the seen set of DL_CHECK_UNIQUE;
 // `linker_hash` (or null) receives every returned row's linker hash with DL_CHECK_NOVEL. `anchors` (B, N), read with
-// DL_CHECK_ANCHORS only, are the anchor flags, which k_anchor_check reads right after the check launch.
+// DL_CHECK_ANCHORS only, are the anchor flags, which k_anchor_check reads right after the check launch. `fx` are the call's
+// fixed atoms: every round gathers its rows' flags and keeps them.
 dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames, const float* xh,
                        const int8_t* node_mask, const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
                        const float* context, const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
                        int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
                        const dl_molecule_checks* ck, const dl_hash_sets* hs, int32_t* passed, uint64_t* linker_hash,
-                       const dl_size_redraw* rz, int32_t* sizes_used, const int8_t* anchors, void* stream) {
+                       const dl_size_redraw* rz, int32_t* sizes_used, const int8_t* anchors, const CallFixed& fx,
+                       void* stream) {
   e->retry_ms = 0.f;
   e->ring_B = 0;
-  dl_status s = dl_sample_chain_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask,
-                                       context, seeds, coef, norm, chain, nan_flags, stream);
+  dl_status s = sample_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context,
+                              seeds, coef, norm, chain, nan_flags, stream, fx);
   if (s != DL_OK) return s;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CK(cudaMemcpyAsync(seeds_used, seeds, (size_t)B * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
@@ -1780,7 +1910,8 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
               i_ctx = sl.add(nullptr, n * C * 4, context != nullptr && C > 0), i_sd = sl.out((size_t)Bs * 8),
               i_ch = sl.out((size_t)keep_frames * n * xd * 4), i_fl = sl.out((size_t)Bs * 4),
               i_ps = sl.add(nullptr, (size_t)Bs * 4, ck != nullptr), i_tk = sl.add(nullptr, (size_t)Bs * 4, ck != nullptr),
-              i_sz = sl.add(nullptr, (size_t)Bs * 4, rz != nullptr), i_sh = sl.add(nullptr, (size_t)Bs * 8, unique);
+              i_sz = sl.add(nullptr, (size_t)Bs * 4, rz != nullptr), i_sh = sl.add(nullptr, (size_t)Bs * 8, unique),
+              i_fx = sl.add(nullptr, n, fx.flags != nullptr);
     if ((s = stage_inputs(e->sub_rows, sl, st)) != DL_OK) return s;   // the row list goes to the device once per round
     CK(cudaEventRecord(e->ev_g0, st));
     RowGatherArgs ga{};
@@ -1791,11 +1922,14 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     ga.s_xh = sl.at<float>(i_xh); ga.s_fragment_mask = sl.at<float>(i_fm); ga.s_linker_mask = sl.at<float>(i_lm);
     ga.s_context = sl.at<float>(i_ctx); ga.s_node_mask = sl.at<int8_t>(i_nm); ga.s_edge_mask = sl.at<int8_t>(i_em);
     ga.s_seeds = sl.at<unsigned long long>(i_sd);
+    const RowFixedArgs fa{fx.flags, sl.at<int8_t>(i_fx)};
     const RowSizeArgs za{sl.at<int32_t>(i_sz), sizes_used};
     if (rz) {
       const RowResizeArgs ra{SizeDrawArgs{rz->C, rz->logits_row_stride, rz->logits, rz->sizes}, rz->n_frag, rz->linker_x,
                              sl.at<int32_t>(i_sz)};
       k_gather_rows<true><<<Bs, 256, 0, st>>>(ga, ra);
+    } else if (fx.flags) {
+      k_gather_rows<false><<<Bs, 256, 0, st>>>(ga, fa);
     } else {
       k_gather_rows<false><<<Bs, 256, 0, st>>>(ga);
     }
@@ -1813,9 +1947,14 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
     }
     {
       SubBatchScope sub(e);
-      s = dl_sample_chain_seeded(e, sampler, Bs, N, T, keep_frames, ga.s_xh, ga.s_node_mask, ga.s_fragment_mask,
-                                 ga.s_linker_mask, ga.s_edge_mask, ga.s_context, reinterpret_cast<const uint64_t*>(ga.s_seeds),
-                                 coef, norm, sl.at<float>(i_ch), sl.at<int32_t>(i_fl), stream);
+      CallFixed sub_fx;                                    // the round's rows keep their fixed atoms
+      if (fx.flags) {
+        sub_fx = fx;
+        sub_fx.flags = fa.s_fixed; sub_fx.B = Bs; sub_fx.vetted = true;
+      }
+      s = sample_seeded(e, sampler, Bs, N, T, keep_frames, ga.s_xh, ga.s_node_mask, ga.s_fragment_mask, ga.s_linker_mask,
+                        ga.s_edge_mask, ga.s_context, reinterpret_cast<const uint64_t*>(ga.s_seeds), coef, norm,
+                        sl.at<float>(i_ch), sl.at<int32_t>(i_fl), stream, sub_fx);
     }
     if (per_row) { e->starts_t0.swap(t0_all); e->starts_alpha.swap(alpha_all); e->starts_sigma.swap(sigma_all); }
     if (s != DL_OK) return s;
@@ -1889,6 +2028,7 @@ dl_status retry_entry(const char* name, dl_engine* e, int32_t sampler, int32_t B
   an.set = e->anchors_set; an.B = e->anchors_B; an.N = e->anchors_N;
   an.flags = reinterpret_cast<const int8_t*>(e->anchors.buf);
   e->anchors_set = false;
+  const CallFixed fx = take_fixed(e);                      // likewise
   if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
   if (!nan_flags || !seeds_used || !attempts || (checks && !passed) || (redraw && !sizes_used)) {
     set_err("%s: null argument (nan_flags, seeds_used, attempts, passed with checks or sizes_used with redraw)", name);
@@ -1901,6 +2041,8 @@ dl_status retry_entry(const char* name, dl_engine* e, int32_t sampler, int32_t B
                                      "DL_CHECK_UNIQUE";
   if (!why && redraw && !e->starts_t0.empty())
     why = "a size redraw takes no start steps: partial diffusion varies the batch's own linker, whose size is given";
+  if (!why && redraw && fx.flags)
+    why = "a size redraw takes no fixed atoms (dl_set_fixed_atoms): it rebuilds the linker rows at new sizes";
   if (!why && redraw) {
     if (cudaSetDevice(e->cfg.device) != cudaSuccess) why = "cudaSetDevice failed";
     else why = redraw_error(sampler, B, N, redraw, reinterpret_cast<cudaStream_t>(stream));
@@ -1912,7 +2054,7 @@ dl_status retry_entry(const char* name, dl_engine* e, int32_t sampler, int32_t B
   }
   return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
                       coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, sets, passed, linker_hash,
-                      redraw, sizes_used, an.flags, stream);
+                      redraw, sizes_used, an.flags, fx, stream);
 }
 
 }  // namespace

@@ -106,10 +106,15 @@ struct RowSizeArgs {
   int32_t* sizes;                        // (B) the caller's sizes: written where a row is taken
 };
 
+// What the gather of a call with fixed atoms (dl_set_fixed_atoms) reads and writes besides RowGatherArgs: the caller's
+// (B, N) flags and the sub-batch's. A kernel parameter of its own, as RowResizeArgs is.
+struct RowFixedArgs {
+  const int8_t* fixed;
+  int8_t* s_fixed;
+};
+
 // One CTA per failed molecule: copies its rows of every input, and derives its seed for this attempt.
-template <bool RESIZE>
-__global__ void __launch_bounds__(256) k_gather_rows(RowGatherArgs a) {
-  static_assert(!RESIZE, "the resizing gather takes RowResizeArgs");
+__device__ __forceinline__ void gather_rows(const RowGatherArgs& a) {
   const int i = blockIdx.x;
   const size_t b = a.rows[i], N = a.N;
   for (size_t k = threadIdx.x; k < N * a.xd; k += blockDim.x) a.s_xh[i * N * a.xd + k] = a.xh[b * N * a.xd + k];
@@ -123,6 +128,19 @@ __global__ void __launch_bounds__(256) k_gather_rows(RowGatherArgs a) {
   if (a.edge_mask)
     for (size_t k = threadIdx.x; k < N * N; k += blockDim.x) a.s_edge_mask[i * N * N + k] = a.edge_mask[b * N * N + k];
   if (threadIdx.x == 0 && a.seeds) a.s_seeds[i] = retry_seed(a.seeds[b], a.attempt);
+}
+template <bool RESIZE>
+__global__ void __launch_bounds__(256) k_gather_rows(RowGatherArgs a) {
+  static_assert(!RESIZE, "the resizing gather takes RowResizeArgs");
+  gather_rows(a);
+}
+// ... and the molecule's fixed-atom flags.
+template <bool RESIZE>
+__global__ void __launch_bounds__(256) k_gather_rows(RowGatherArgs a, RowFixedArgs f) {
+  static_assert(!RESIZE, "a size redraw takes no fixed atoms");
+  gather_rows(a);
+  const size_t b = a.rows[blockIdx.x], N = a.N;
+  for (size_t k = threadIdx.x; k < N; k += blockDim.x) f.s_fixed[blockIdx.x * N + k] = f.fixed[b * N + k];
 }
 
 // The resizing gather: warp 0 draws the molecule's size s' with this attempt's seed, then the CTA writes the template of
@@ -1079,6 +1097,7 @@ struct GuideArgs {
   const float* coef;
   float* chain;                          // (keep, B*N, row_stride)
   float norm0;
+  const int8_t* fixed;                   // k_clash_guide<true>: (B, N) fixed-atom flags (dl_set_fixed_atoms), rows it never moves
 };
 // Shared memory per row: the staged pocket atom and the linker atoms' list.
 constexpr int GUIDE_SMEM_PER_ROW = (int)(sizeof(float4) + sizeof(int));
@@ -1088,7 +1107,9 @@ constexpr int GUIDE_SMEM_PER_ROW = (int)(sizeof(float4) + sizeof(int));
 // in a fixed assignment, and reduces the three sums with xor shuffles: no atomics, and the result depends neither on the
 // order the warps run in nor on the molecule's batch-mates. The pair's distance is the clash check's (pair_dist_pm, in pm),
 // so an atom moves iff the check counts a clash for it; (r - d) / d is taken in pm, where it is the same ratio. A pair at
-// d = 0 or with a NaN distance contributes nothing, and an atom with no contributing pair is not written.
+// d = 0 or with a NaN distance contributes nothing, and an atom with no contributing pair is not written. FIXED: the linker
+// rows flagged in a.fixed are not listed, so they neither move nor push (they are no pocket atoms either).
+template <bool FIXED = false>
 __global__ void __launch_bounds__(256) k_clash_guide(GuideArgs a) {
   extern __shared__ float4 s_pk[];                    // [n_pocket]: x, y, z, type (int bits)
   int* s_lnk = reinterpret_cast<int*>(s_pk + a.N);    // [n_linker]: the linker atoms' rows, ascending
@@ -1107,7 +1128,7 @@ __global__ void __launch_bounds__(256) k_clash_guide(GuideArgs a) {
     const int r = r0 + tid;
     const bool live = r < a.N && a.node_mask[g0 + r] != 0;
     const bool pocket = live && a.context[(g0 + r) * a.C + a.C - 1] != 0.f;
-    const bool linker = live && !pocket && a.linker_mask[g0 + r] != 0.f;
+    const bool linker = live && !pocket && a.linker_mask[g0 + r] != 0.f && (!FIXED || a.fixed[g0 + r] == 0);
     const unsigned mp = __ballot_sync(0xffffffffu, pocket), ml = __ballot_sync(0xffffffffu, linker);
     if (lane == 0) { s_warp[warp] = __popc(mp); s_lwarp[warp] = __popc(ml); }
     __syncthreads();
@@ -1165,11 +1186,16 @@ __global__ void __launch_bounds__(256) k_clash_guide(GuideArgs a) {
 // its one maximum (clash_guide_opt_in), whatever N: the 48 KB default counts the static shared memory too. A reverse loop
 // raises it before it captures its step (the attribute is not a stream operation).
 inline cudaError_t clash_guide_opt_in() {
-  return cudaFuncSetAttribute(k_clash_guide, cudaFuncAttributeMaxDynamicSharedMemorySize, CONN_MAX_N * GUIDE_SMEM_PER_ROW);
+  const cudaError_t err = cudaFuncSetAttribute(k_clash_guide<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               CONN_MAX_N * GUIDE_SMEM_PER_ROW);
+  if (err != cudaSuccess) return err;
+  return cudaFuncSetAttribute(k_clash_guide<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, CONN_MAX_N * GUIDE_SMEM_PER_ROW);
 }
+// a.fixed != null launches the instantiation that leaves the flagged rows in place
 inline cudaError_t launch_clash_guide(const GuideArgs& a, int B, cudaStream_t st) {
   const size_t smem = (size_t)a.N * GUIDE_SMEM_PER_ROW;
-  k_clash_guide<<<B, 256, smem, st>>>(a);
+  if (a.fixed != nullptr) k_clash_guide<true><<<B, 256, smem, st>>>(a);
+  else k_clash_guide<false><<<B, 256, smem, st>>>(a);
   return cudaGetLastError();
 }
 

@@ -910,9 +910,20 @@ struct FinishArgs {
   // order, and the DPM-Solver++(2M) history -- every node's data prediction of its previous step -- or null (DDIM)
   const float* ode;
   float* hist;
+  // fixed atoms (dl_set_fixed_atoms, k_finish<., ., true>): the linker rows to keep (B*N int8 in the workspace's row
+  // order), the normalised input xh they keep, and the (alpha_s, sigma_s) of the loop's rows, 2 floats per row in coef's
+  // row order
+  const int8_t* fixed;
+  const float* xh0;
+  const float* fix;
 };
 
-template <bool PER_MOL = false, bool ODE = false>
+// A kept row's z_s = alpha_s xh + sigma_s eps, every product and the sum rounded on their own as k_init_z_rows rounds them.
+__device__ __forceinline__ float fixed_state(const float* sc, float xh, float eps) {
+  return __fadd_rn(__fmul_rn(sc[0], xh), __fmul_rn(sc[1], eps));
+}
+
+template <bool PER_MOL = false, bool ODE = false, bool FIX = false>
 __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
   const int tid = threadIdx.x;
   const int d = tid & 15, r = tid >> 4;
@@ -991,6 +1002,7 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
     // deterministic update from the solver row sv = (sigma_t, 1/alpha_t, sigma_s/sigma_t, c1, c2a, c2b, h, 0): the data
     // prediction xhat = (z_t - sigma_t eps) / alpha_t, then z_s = (sigma_s/sigma_t) z_t + c1 xhat at a row's first step
     // (DDIM always), + c2a xhat + c2b xhat' after it; the final row returns xhat. No draw is read.
+    // FIX: a kept row then takes alpha_s xh + sigma_s eps_0 with its own draw 0 instead, so its history does not enter
     if (act) {
       lm = a.linker_mask[g]; fm = a.fragment_mask[g];
       const size_t gi = (size_t)g * xd + d;
@@ -998,10 +1010,15 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
       const float eps = e * lm;
       const float* sv = a.ode + (size_t)step * 8;
       const float xhat = sv[1] * (zt - sv[0] * eps);
+      const bool kept = FIX && a.fixed[g] != 0;
       if (step < a.T) {
         float zs;
         if (a.hist != nullptr && step > lag) zs = sv[2] * zt + (sv[4] * xhat + sv[5] * a.hist[gi]);
         else zs = sv[2] * zt + sv[3] * xhat;
+        if (kept) {
+          const float eps0 = a.rng.on ? noise_draw<PER_MOL>(a.rng, 0, g, d) : a.noise[gc * xd + d];
+          zs = fixed_state(a.fix + (size_t)step * 2, a.xh0[gi], eps0);
+        }
         if (a.hist != nullptr) a.hist[gi] = xhat;
         znew = zt * fm + zs * lm;
         a.z[gi] = znew;
@@ -1010,7 +1027,7 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
           a.chain[((size_t)frame * nc + gc) * xd + d] = o;
         }
       } else {
-        znew = zt * fm + xhat * lm;
+        znew = zt * fm + (kept ? a.xh0[gi] : xhat) * lm;
       }
     }
   } else if (act) {
@@ -1019,9 +1036,12 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
     const float eps = e * lm;                                                 // edm.py:196 / 225
     const float nz = (a.rng.on ? noise_draw<PER_MOL>(a.rng, step + 1 - lag, g, d)
                                : a.noise[((size_t)(step + 1 - lag) * nc + gc) * xd + d]) * lm;  // utils.py:189-192
+    // FIX: a kept row takes alpha_s xh + sigma_s nz_s from the draw the update reads, and the input at the final step
+    const bool kept = FIX && a.fixed[g] != 0;
     if (step < a.T) {
       float mu = zt / ca - cb * eps;                                          // edm.py:199
       float zs = mu + cc * nz;                                                // edm.py:205, 342-345
+      if (kept) zs = fixed_state(a.fix + (size_t)step * 2, a.xh0[(size_t)g * xd + d], nz);
       znew = zt * fm + zs * lm;                                               // edm.py:206
       a.z[(size_t)g * xd + d] = znew;
       if (frame >= 0) {
@@ -1031,6 +1051,7 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
     } else {
       float mux = ca * (zt - cb * eps);                                       // edm.py:241 (ca = 1/alpha_0)
       float xo = mux + cc * nz;                                               // edm.py:228
+      if (kept) xo = a.xh0[(size_t)g * xd + d];
       znew = zt * fm + xo * lm;                                               // edm.py:229
     }
   }
@@ -1308,6 +1329,46 @@ __global__ void k_init_z_rows(int n_total, int N, int xd, const float* __restric
   const float nz = rng.on ? noise_draw<PER_MOL>(rng, 0, g, d) : noise[((size_t)rows.src[b] * N + (g - b * N)) * xd + d];
   const float zt = __fadd_rn(__fmul_rn(alpha[b], v), __fmul_rn(sigma[b], __fmul_rn(nz, l)));
   z[idx] = __fadd_rn(__fmul_rn(v, fm[g]), __fmul_rn(zt, l));
+}
+
+// Fixed atoms (dl_set_fixed_atoms): after the start above, the kept linker rows start from q(z_t | x) of the input with the
+// formula of k_init_z_rows -- the scalars alpha, sigma of the call's start, or alpha_rows[b], sigma_rows[b] of each row's
+// own start step when given -- and the row's draw 0. Every other row keeps what the start wrote.
+template <bool PER_MOL = false>
+__global__ void k_init_z_fixed(int n_total, int N, int xd, const float* __restrict__ xh, const float* __restrict__ fm,
+                               const float* __restrict__ lm, const int8_t* __restrict__ fixed,
+                               const float* __restrict__ noise, NoiseRng rng, float alpha, float sigma,
+                               const float* __restrict__ alpha_rows, const float* __restrict__ sigma_rows, RowStarts rows,
+                               float* __restrict__ z) {
+  int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_total * xd) return;
+  const int g = idx / xd, b = g / N, d = idx - g * xd;
+  if (fixed[g] == 0) return;
+  const size_t gc = rows.src != nullptr ? (size_t)rows.src[b] * N + (g - b * N) : (size_t)g;
+  const float al = alpha_rows != nullptr ? alpha_rows[b] : alpha, sg = sigma_rows != nullptr ? sigma_rows[b] : sigma;
+  const float l = lm[g], v = xh[idx];
+  const float nz = rng.on ? noise_draw<PER_MOL>(rng, 0, g, d) : noise[gc * xd + d];
+  const float zt = __fadd_rn(__fmul_rn(al, v), __fmul_rn(sg, __fmul_rn(nz, l)));
+  z[idx] = __fadd_rn(__fmul_rn(v, fm[g]), __fmul_rn(zt, l));
+}
+
+// dl_set_fixed_atoms' vetting of a call's flags: bad[0] = 1 + a node row whose flag is set but which
+// is not a live linker row (node_mask, linker_mask != 0, fragment_mask == 0), bad[1] = 1 + a flagged row whose type channels are not a
+// one-hot as normalised: exactly one channel equal to (1 - bias1) / norm1 and every other to (0 - bias1) / norm1.
+__global__ void k_fixed_check(int n_total, int xd, const int8_t* __restrict__ fixed, const int8_t* __restrict__ node_mask,
+                              const float* __restrict__ fm, const float* __restrict__ lm, const float* __restrict__ xh,
+                              float norm1, float bias1, int* bad) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n_total || fixed[g] == 0) return;
+  if (node_mask[g] == 0 || lm[g] == 0.f || fm[g] != 0.f) atomicCAS(bad, 0, g + 1);
+  const float one = __fdiv_rn(__fsub_rn(1.f, bias1), norm1), zero = __fdiv_rn(__fsub_rn(0.f, bias1), norm1);
+  int ones = 0, others = 0;
+  for (int d = 3; d < xd; ++d) {
+    const float v = xh[(size_t)g * xd + d];
+    ones += v == one;
+    others += v != one && v != zero;
+  }
+  if (ones != 1 || others != 0) atomicCAS(bad + 1, 0, g + 1);
 }
 
 // Debug / test helper: the (n_draws, n_total, 3+F) tensor the device-side stream stands for.

@@ -54,7 +54,7 @@ def _build_edm(hp: dict, edge_impl='auto', is_geom=None):
                norm_values=hp['normalize_factors'], is_geom=_is_geom(hp) if is_geom is None else bool(is_geom))
 
 
-def _keep_linker(data, template):
+def _keep_linker(data, template, what="start_step varies the batch's linker"):
     """The template's positions and one-hot with the linker rows of `data` filled in, for partial diffusion, which varies
     the linker the batch holds. create_templates_for_linker_generation puts a molecule's fragment atoms first and its
     linker after them; a batch whose linker rows lie elsewhere raises ValueError."""
@@ -63,32 +63,33 @@ def _keep_linker(data, template):
     same = (data['linker_mask'].shape[1] >= n and torch.equal(data['linker_mask'][:, :n].to(lm.dtype), lm)
             and not data['linker_mask'][:, n:].any())
     if not same:
-        raise ValueError("start_step varies the batch's linker, so each molecule's linker rows must follow its fragment "
-                         "rows, where the sampling template puts them")
+        raise ValueError(f"{what}, so each molecule's linker rows must follow its fragment rows, where the sampling "
+                         "template puts them")
     keep = lm.bool()
     return (torch.where(keep, data['positions'][:, :n], template['positions']),
             torch.where(keep, data['one_hot'][:, :n], template['one_hot']))
 
 
-def sampler_inputs(model, data, sample_fn=None, keep_linker=False):
+def sampler_inputs(model, data, sample_fn=None, keep_linker=False, what="start_step varies the batch's linker"):
     """What DDPM.sample_chain hands to EDM.sample_chain (lightning.py:405-452): the template batch, the context
     columns and the centred coordinates, as the keyword arguments of `edm.sample_chain`. `keep_linker` (partial diffusion)
-    fills the template's linker rows with the batch's own linker before the coordinates are centred.
+    fills the template's linker rows with the batch's own linker before the coordinates are centred; `what` opens the
+    ValueError of a batch whose linker rows do not follow its fragment rows.
     `model` needs .inpainting, .anchors_context, .train_data_prefix, .center_of_mass, .val_dataset."""
     if sample_fn is None:
         linker_sizes = data['linker_mask'].sum(1).view(-1).int()
     else:
         linker_sizes = sample_fn(data)
-    return _template_inputs(model, data, linker_sizes, keep_linker)[0]
+    return _template_inputs(model, data, linker_sizes, keep_linker, what=what)[0]
 
 
-def _template_inputs(model, data, linker_sizes, keep_linker=False, n_nodes=None):
+def _template_inputs(model, data, linker_sizes, keep_linker=False, n_nodes=None, what="start_step varies the batch's linker"):
     """(sampler_inputs of the template of `linker_sizes` padded to `n_nodes` rows, the centre of mass (B, 1, 3) that was
     subtracted from its coordinates)."""
     template = data if model.inpainting else create_templates_for_linker_generation(data, linker_sizes, n_nodes)
     x, h = template['positions'], template['one_hot']
     if keep_linker and not model.inpainting:
-        x, h = _keep_linker(data, template)
+        x, h = _keep_linker(data, template, what)
     node_mask, edge_mask = template['atom_mask'], template['edge_mask']
     anchors, fragment_mask, linker_mask = template['anchors'], template['fragment_mask'], template['linker_mask']
     pocket = '.' in model.train_data_prefix
@@ -224,10 +225,36 @@ def _check_start(sample_fn, start_step):
         raise ValueError("start_step varies the batch's own linker, so its size is the batch's: pass no sample_fn")
 
 
+def _check_fixed(sample_fn, linker_sizes, fixed_atoms):
+    if fixed_atoms is None:
+        return
+    if sample_fn is not None:
+        raise ValueError("fixed_atoms keeps atoms of the batch's own linker rows, so its linker sizes are the batch's: pass "
+                         "no sample_fn")
+    if linker_sizes is not None:
+        raise ValueError("fixed_atoms does not take linker_sizes: a size redraw rebuilds the linker rows at new sizes")
+
+
+def _sampler_kw(model, data, sample_fn, start_step, fixed_atoms):
+    """sampler_inputs of a call, with the batch's own linker rows for start_step or fixed_atoms, and the latter as
+    EDM.sample_chain's `fixed_atoms` of the template's rows (the batch's linker rows keep their place in it)."""
+    if fixed_atoms is None:
+        return sampler_inputs(model, data, sample_fn, keep_linker=start_step is not None)
+    what = "start_step varies the batch's linker" if start_step is not None else "fixed_atoms keeps the batch's linker atoms"
+    kw = sampler_inputs(model, data, sample_fn, keep_linker=True, what=what)
+    B, n = kw['x'].shape[:2]
+    flags = fixed_atoms.detach().reshape(B, -1) if torch.is_tensor(fixed_atoms) else fixed_atoms
+    if torch.is_tensor(flags) and flags.shape[1] > n:
+        if flags[:, n:].any():
+            raise ValueError("fixed_atoms flags a row beyond the sampling template's, which holds the batch's linker rows")
+        flags = flags[:, :n]
+    return dict(kw, fixed_atoms=flags)
+
+
 def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                  start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                  require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None, require_anchors=None,
-                 clash_guidance=None, solver=None):
+                 clash_guidance=None, solver=None, fixed_atoms=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
@@ -261,13 +288,18 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     `model.edm.resamplings`).
     `clash_guidance` = (scale, steps): push the linker atoms out of the pocket at the last `steps` reverse steps
     (EDM.sample_chain; None uses `model.edm.clash_guidance`).
-    `solver` = 'ancestral', 'ddim' or 'dpmpp_2m': the reverse update (EDM.sample_chain; None uses `model.edm.solver`)."""
+    `solver` = 'ancestral', 'ddim' or 'dpmpp_2m': the reverse update (EDM.sample_chain; None uses `model.edm.solver`).
+    `fixed_atoms` ((B, N) or (B, N, 1), non-zero on the batch's linker atoms to keep): the template of sample_fn=None with
+    the batch's own linker rows, as for start_step, of which the flagged atoms are kept and the rest sampled around them
+    (EDM.sample_chain); ValueError with a sample_fn or linker_sizes, and when the batch's linker rows do not directly follow
+    its fragment rows."""
     _check_start(sample_fn, start_step)
+    _check_fixed(sample_fn, linker_sizes, fixed_atoms)
     if linker_sizes is not None:
         _check_linker_sizes(model, sample_fn, start_step)
         kw, seeds, sized = _sized_inputs(model, data, linker_sizes, seeds)
     else:
-        kw, sized = sampler_inputs(model, data, sample_fn, keep_linker=start_step is not None), None
+        kw, sized = _sampler_kw(model, data, sample_fn, start_step, fixed_atoms), None
     extra = {} if seeds is None else {'seeds': seeds}
     if sized is not None:
         extra['linker_sizes'] = sized
@@ -305,7 +337,7 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
 def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                 max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
                 require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None, clash_guidance=None,
-                solver=None):
+                solver=None, fixed_atoms=None):
     """The body of sample_chain for many batches `datas` at once, sampled in shared launches by EDM.sample_many: returns
     [(chain_k, node_mask_k)] in the order of `datas`, each equal to what sample_chain(model, datas[k], ...) returns (with
     seeds[k]) in the sense of EDM.sample_many. `model` as for sample_chain, so accelerated reference modules take it too.
@@ -314,8 +346,14 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
     one for every batch, as in sample_chain. `linker_sizes`, one for every batch, as in sample_chain: each batch's sizes
     are drawn from its own seeds and its template padded to its own N_cap, so packing changes neither;
     `edm.last_sizes_many` holds them. `resamplings` and `require_anchors` as in sample_chain: each request then holds its
-    batch's template anchors. `clash_guidance` and `solver` as in sample_chain."""
+    batch's template anchors. `clash_guidance` and `solver` as in sample_chain. `fixed_atoms`, one per batch (or None for a
+    batch that keeps none), as in sample_chain: each request then holds its batch's flags."""
     _check_start(sample_fn, start_step)
+    if fixed_atoms is not None:
+        if len(fixed_atoms) != len(datas):
+            raise ValueError(f"fixed_atoms holds {len(fixed_atoms)} entries for {len(datas)} batches")
+        for f in fixed_atoms:
+            _check_fixed(sample_fn, linker_sizes, f)
     edm = model.edm
     if linker_sizes is not None:
         _check_linker_sizes(model, sample_fn, start_step)
@@ -339,8 +377,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
                 for chain, (kw, _, ls), sizes in zip(chains, sized, edm.last_sizes_many)]
     derive = seeds is None and edm.noise_mode == 'per_molecule'
     requests, drawn = [], []
-    for data in datas:
-        kw = sampler_inputs(model, data, sample_fn, keep_linker=start_step is not None)
+    for k, data in enumerate(datas):
+        kw = _sampler_kw(model, data, sample_fn, start_step, None if fixed_atoms is None else fixed_atoms[k])
         requests.append(_with_anchors(model, data, kw, require_anchors))
         x = kw['x']
         if derive and x.is_cuda:                # a host batch is refused by EDM.sample_many
@@ -411,23 +449,24 @@ class DDPM(nn.Module):
     def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                      start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, clash_guidance=None, solver=None):
+                     require_anchors=None, clash_guidance=None, solver=None, fixed_atoms=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                             require_connected=require_connected, start_step=start_step, require_valid=require_valid,
                             require_clash_free=require_clash_free, linker_sizes=linker_sizes, require_unique=require_unique,
                             require_novel=require_novel, exclude_hashes=exclude_hashes, resamplings=resamplings,
                             require_ring_sizes=require_ring_sizes, require_anchors=require_anchors,
-                            clash_guidance=clash_guidance, solver=solver)
+                            clash_guidance=clash_guidance, solver=solver, fixed_atoms=fixed_atoms)
 
     def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
                     require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None,
-                    clash_guidance=None, solver=None):
+                    clash_guidance=None, solver=None, fixed_atoms=None):
         return sample_many(self, datas, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                            require_connected=require_connected, max_molecules=max_molecules, start_step=start_step,
                            require_valid=require_valid, require_clash_free=require_clash_free, linker_sizes=linker_sizes,
                            require_novel=require_novel, resamplings=resamplings, require_ring_sizes=require_ring_sizes,
-                           require_anchors=require_anchors, clash_guidance=clash_guidance, solver=solver)
+                           require_anchors=require_anchors, clash_guidance=clash_guidance, solver=solver,
+                           fixed_atoms=fixed_atoms)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

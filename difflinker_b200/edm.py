@@ -72,7 +72,7 @@ def _loop_steps(start):
 
 
 def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None, resample=None,
-                  guide=None, solver=None):
+                  guide=None, solver=None, fixed=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
@@ -92,8 +92,9 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     jump) runs r RePaint passes per step, set on the engine for the duration of the call (dl_set_resamplings). `guide` =
     (scale, steps, clash table) pushes the linker atoms out of the pocket at the last `steps` steps, set on the engine for
     the duration of the call (dl_set_clash_guidance). `solver` = (kind, T, table) replaces the ancestral update by an ODE
-    solver's, set on the engine for the duration of the call (dl_set_solver). Returns (status, what the batch stream
-    consumed)."""
+    solver's, set on the engine for the duration of the call (dl_set_solver). `fixed` = ((B, N) int8 flags on the slice's
+    device, or on the host with host inputs, T, scalars) keeps the flagged linker rows (dl_set_fixed_atoms, right before
+    the call, which clears it). Returns (status, what the batch stream consumed)."""
     per_row = isinstance(start, StartSteps)
     if per_row:
         start.set_on(lib, eng)
@@ -108,8 +109,14 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
                           "dl_set_clash_guidance")
         if solver is not None:
             _native.check(lib.dl_set_solver(eng, *solver), "dl_set_solver")
+        if fixed is not None:
+            flags, T, scalars = fixed
+            _native.check(lib.dl_set_fixed_atoms(eng, head[1], head[2], flags.data_ptr(), T, scalars, stream),
+                          "dl_set_fixed_atoms")
         return _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry)
     finally:
+        if fixed is not None:               # a call that failed before the engine read the flags
+            lib.dl_set_fixed_atoms(eng, 0, 0, None, 0, None, None)
         if solver is not None:
             lib.dl_set_solver(eng, _native.SOLVERS['ancestral'], 0, None)
         if guide is not None:
@@ -639,6 +646,61 @@ class EDM(torch.nn.Module):
         g = self._cpu_gamma()(torch.full((n_samples, 1), fill_value=float(t0)) / self.T)
         return float(self.alpha(g)[0]), float(self.sigma(g)[0])
 
+    def fixed_atom_scalars(self, n_samples=1):
+        """The (T + 1, 2) scalars of dl_set_fixed_atoms as a flat ctypes float array: row r < T, in step_coefficients' row
+        order (step s = T-1-r), holds start_scalars(s, n_samples) -- the (alpha_s, sigma_s) of q(z_s | x) a kept row is
+        drawn from at that step -- and row T holds start_scalars(T, n_samples), where a call from noise starts its kept
+        rows. A row that starts at t0 therefore sees the same scalars at its start and in the row of step t0. Cached like
+        step_coefficients."""
+        T = self.T
+        key = ('fixed', T, n_samples, self.gamma.gamma._version, self.gamma.gamma.data_ptr())
+        cache = self.__dict__.setdefault('_coef_cache', {})
+        if key in cache:
+            return cache[key]
+        out = (C.c_float * (2 * (T + 1)))()
+        for r in range(T + 1):
+            out[2 * r], out[2 * r + 1] = self.start_scalars(T - 1 - r if r < T else T, n_samples)
+        if len(cache) >= 8:
+            cache.pop(next(iter(cache)))
+        cache[key] = out
+        return out
+
+    def _fixed_atoms(self, fixed_atoms, x, h, node_mask, fragment_mask, linker_mask, context, what="fixed_atoms"):
+        """The (B, N) int8 flags on x's device of the linker rows a call keeps, or None without `fixed_atoms` or when it
+        flags no row (the plain call). ValueError for InpaintingEDM, a shape other than (B, N) or (B, N, 1), a flag on a
+        row that is not a live linker row (fragment, pocket or padding rows), and a flagged row whose types h are not a
+        one-hot."""
+        if fixed_atoms is None:
+            return None
+        if self._SAMPLER == _native.SAMPLER_INPAINT:
+            raise ValueError("fixed_atoms takes the linker sampler (EDM) only: InpaintingEDM samples every atom and "
+                             "re-noises the known ones itself")
+        B, N = x.shape[:2]
+        if not torch.is_tensor(fixed_atoms) or tuple(fixed_atoms.shape) not in ((B, N), (B, N, 1)):
+            got = tuple(fixed_atoms.shape) if torch.is_tensor(fixed_atoms) else type(fixed_atoms).__name__
+            raise ValueError(f"{what} must be a (B, N) or (B, N, 1) tensor for B = {B}, N = {N} (got {got})")
+        dev = x.device
+        flags = fixed_atoms.detach().reshape(B, N).to(dev) != 0
+        if not flags.any():
+            return None
+        live_linker = ((node_mask.detach().reshape(B, N).to(dev) != 0) & (linker_mask.detach().reshape(B, N).to(dev) != 0)
+                       & (fragment_mask.detach().reshape(B, N).to(dev) == 0))
+        if context is not None and self.dynamics.graph_type != 'FC':
+            live_linker &= context.detach()[..., -1].reshape(B, N).to(dev) == 0
+        off = flags & ~live_linker
+        if off.any():
+            b, n = (int(v) for v in off.nonzero()[0])
+            raise ValueError(f"{what}: row {n} of molecule {b} is flagged but is not a linker row; only linker atoms can be "
+                             "kept (fragment and pocket atoms are kept anyway, padding rows hold no atom)")
+        types = h.detach().reshape(B, N, -1).to(dev)[flags]
+        if not (((types == 0) | (types == 1)).all(dim=1) & (types == 1).sum(dim=1).eq(1)).all():
+            raise ValueError(f"{what}: a kept row's types h must be a one-hot, as it is decoded into chain[0]")
+        return flags.to(torch.int8).contiguous()
+
+    def _fixed(self, flags, n_samples):
+        """_enqueue_batch's `fixed` of flags returned by _fixed_atoms: (flags, scalars at n_samples), or None."""
+        return None if flags is None else (flags, self.fixed_atom_scalars(n_samples))
+
     def _start(self, start_step, n_samples):
         """(t0, alpha_t0, sigma_t0) of a call of n_samples molecules that starts at step `start_step`, or None for one that
         starts from noise at T; for a 1-D sequence or integer tensor of one step per molecule, their StartSteps, every
@@ -904,7 +966,7 @@ class EDM(torch.nn.Module):
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, anchors=None, clash_guidance=None, solver=None):
+                     require_anchors=None, anchors=None, clash_guidance=None, solver=None, fixed_atoms=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -1022,6 +1084,18 @@ class EDM(torch.nn.Module):
         linker_sizes, clash_guidance (which pushes z_s after the update) and `devices` work as without it. The effect on
         a trained model's samples is not measured. ValueError for another name, for InpaintingEDM and for T above the
         schedule's timesteps.
+        `fixed_atoms` (a (B, N) or (B, N, 1) tensor, non-zero on the linker rows to keep; None, the default, keeps none)
+        generates the rest of the linker around the kept atoms (dl_set_fixed_atoms): the kept rows are x's and h's linker
+        rows, as start_step reads them, and the other linker rows are sampled -- their inputs are ignored. The kept rows
+        stay noisy linker rows, replaced at every step by a draw of q(z_s | x) (replacement, as RePaint keeps known pixels,
+        without its re-noising passes): they start from alpha xh + sigma eps_0 at the call's start (T, or start_step in
+        either form), step s sets them to alpha_s xh + sigma_s nz_s with the draw the ancestral update reads for the row
+        (alpha_s xh + sigma_s eps_0 with an ODE `solver`), with the scalars of fixed_atom_scalars, and chain[0] holds their
+        input x and types. The draws are those of the call without it, so seeds, noise=, the batch stream, start_step, the
+        recovery rounds (resampled rows keep their kept atoms, which every check counts as linker atoms), clash_guidance
+        (which moves only the free linker atoms), `solver`, keep_frames, `devices` and batch_slice work as without it. A
+        mask that flags no row is the plain call, bit for bit. ValueError for a flag off the linker rows, a kept row whose
+        h is not a one-hot, the wrong shape, InpaintingEDM and linker_sizes.
         The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
         and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
         device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
@@ -1047,6 +1121,9 @@ class EDM(torch.nn.Module):
         check = self._checks(require_connected, require_valid, seeds, noise, batch_slice, x, require_clash_free,
                              require_unique, require_novel, require_ring_sizes, require_anchors)
         anchor_flags = self._anchors(check, anchors, x, node_mask, linker_mask, context)
+        fixed = self._fixed_atoms(fixed_atoms, x, h, node_mask, fragment_mask, linker_mask, context)
+        if fixed is not None and redraw is not None:
+            raise ValueError("fixed_atoms does not take linker_sizes: a size redraw rebuilds the linker rows at new sizes")
         sets = self._hash_sets(check, exclude_hashes, dev)
         recover = retries > 0 or check != 0 # the recovery entry point: seeds used and attempts come back
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
@@ -1085,7 +1162,7 @@ class EDM(torch.nn.Module):
                                             rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check,
                                             start=start, redraw=redraw, sets=sets,
                                             resample=self._resample(r, n_samples), anchors=anchor_flags, guide=guide,
-                                            solver=ode)
+                                            solver=ode, fixed=self._fixed(fixed, n_samples))
         by_device = {}
         for dev_i, c in calls:
             by_device.setdefault(dev_i, []).append(c)
@@ -1189,6 +1266,9 @@ class EDM(torch.nn.Module):
         `require_anchors` likewise; each request then also holds `anchors`, its (B_k, N_k) or (B_k, N_k, 1) anchor flags (a
         request may hold them without the check, which ignores them), and `last_anchors_ok_many` holds every request's
         verdicts.
+        `fixed_atoms` likewise: a request may hold its (B_k, N_k) or (B_k, N_k, 1) flags of the linker rows to keep, as
+        sample_chain's `fixed_atoms`. They travel per row, and requests then share a launch only where sample_chain would
+        give them the same fixed_atom_scalars.
         `linker_sizes`, one LinkerSizes per request, all of one size table, redraws sizes in those rounds as in sample_chain
         (it needs `seeds`); `last_sizes_many` holds every request's sizes. Each request's sizes come from its own seeds, so
         packing does not change them.
@@ -1227,9 +1307,9 @@ class EDM(torch.nn.Module):
             if 'noise' in r or 'batch_slice' in r:
                 raise ValueError(f"request {k} passes noise= or batch_slice=: sample_many samples per-molecule streams, "
                                  "which need neither")
-            if set(r) - {'anchors'} != set(self._REQUEST_INPUTS):
+            if set(r) - {'anchors', 'fixed_atoms'} != set(self._REQUEST_INPUTS):
                 raise ValueError(f"request {k} must hold exactly the inputs {self._REQUEST_INPUTS}, and may hold "
-                                 f"'anchors' (got {sorted(r)})")
+                                 f"'anchors' and 'fixed_atoms' (got {sorted(r)})")
         if self._draws_replaced():
             raise ValueError("sample_many needs the device-side per-molecule stream, but this model's draw function is replaced")
         if seeds is None and self.noise_mode != 'per_molecule':
@@ -1276,6 +1356,12 @@ class EDM(torch.nn.Module):
                              require_anchors=require_anchors)
         anchors_many = [self._anchors(check, r.get('anchors'), r['x'], r['node_mask'], r['linker_mask'], r['context'],
                                       f"request {k}'s anchors") for k, r in enumerate(requests)]
+        fixed_many = [self._fixed_atoms(r.get('fixed_atoms'), r['x'], r['h'], r['node_mask'], r['fragment_mask'],
+                                        r['linker_mask'], r['context'], f"request {k}'s fixed_atoms")
+                      for k, r in enumerate(requests)]
+        any_fixed = any(f is not None for f in fixed_many)
+        if any_fixed and linker_sizes is not None:
+            raise ValueError("fixed_atoms does not take linker_sizes: a size redraw rebuilds the linker rows at new sizes")
         sets = self._hash_sets(check, None, dev)
         recover = retries > 0 or check != 0
         redraws = None
@@ -1295,6 +1381,8 @@ class EDM(torch.nn.Module):
             keys = [k + (bytes(self.jump_coefficients(b)),) for k, b in zip(keys, sizes)]
         if guide is not None:               # the same for every request of a call: launches are sampled as it says
             keys = [k + (guide[:2],) for k in keys]
+        if any_fixed:                       # the kept rows' scalars depend on the batch size as the table does
+            keys = [k + (bytes(self.fixed_atom_scalars(b)),) for k, b in zip(keys, sizes)]
         fc = self.dynamics.graph_type == 'FC'
         launches = plan_launches(sizes, nodes, max_molecules, keys)
         if fc:                              # edges of the launch's padded molecules
@@ -1323,6 +1411,12 @@ class EDM(torch.nn.Module):
             anchors = None
             if check & _native.CHECK_ANCHORS:
                 anchors = torch.cat([torch.nn.functional.pad(anchors_many[k], (0, n - nodes[k])) for k in ks])
+            fixed = None
+            if any(fixed_many[k] is not None for k in ks):
+                fixed = self._fixed(torch.cat([torch.nn.functional.pad(
+                    fixed_many[k] if fixed_many[k] is not None else torch.zeros((sizes[k], nodes[k]), dtype=torch.int8,
+                                                                                device=dev), (0, n - nodes[k]))
+                    for k in ks]), sizes[ks[0]])
             dev_seeds = torch.cat([cpu_seeds[k] for k in ks]).to(dev)
             where = torch.device('cuda', dev_i)
             eng = engine_of[slot_of[i]]
@@ -1334,7 +1428,7 @@ class EDM(torch.nn.Module):
                                                       [where], dev, dev_seeds=dev_seeds, retries=retries, check=check,
                                                       start=start, redraw=redraw, sets=sets,
                                                       resample=self._resample(r_passes, sizes[ks[0]]), anchors=anchors,
-                                                      guide=guide, solver=ode)
+                                                      guide=guide, solver=ode, fixed=fixed)
             finishes.append(finish)
             by_device.setdefault(dev_i, []).append(
                 functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
@@ -1421,7 +1515,7 @@ class EDM(torch.nn.Module):
 
     def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
                        retries=0, check=0, start=None, redraw=None, sets=None, resample=None, anchors=None, guide=None,
-                       solver=None):
+                       solver=None, fixed=None):
         """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
         inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
         replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
@@ -1430,7 +1524,7 @@ class EDM(torch.nn.Module):
         returned by _start; `redraw` as returned by _linker_sizes (its rounds then redraw sizes, into `sizes`); `sets` as
         returned by _hash_sets, copied to each slice's device; `resample` as returned by _resample; `anchors` as returned
         by _anchors, each slice's rows on its device; `guide` as returned by _clash_guidance; `solver` as returned by
-        _solver.
+        _solver; `fixed` as returned by _fixed, each slice's rows of the flags on its device.
         Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
         (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
         back and returns dict(chain, flags, used, attempts, passed, sizes, bad, consumed) on `dev`; `passed` holds
@@ -1488,9 +1582,10 @@ class EDM(torch.nn.Module):
             lh_i = linker_hashes if whole or not novel else torch.empty(hi - lo, dtype=torch.int64, device=where)
             rs_i = ring_sizes if whole or not rings else torch.empty(hi - lo, dtype=torch.int64, device=where)
             an_i = anchors if whole or anchors is None else anchors[lo:hi].to(where).contiguous()
-            part = part + (checks_i, redraw_i, sets_i, lh_i, rs_i, an_i)
+            fx_i = None if fixed is None else (fixed[0] if whole else fixed[0][lo:hi].to(where).contiguous())
+            part = part + (checks_i, redraw_i, sets_i, lh_i, rs_i, an_i, fx_i)
             parts.append(part)              # alive until the flags have been read below
-            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, checks_i, redraw_i, sets_i, lh_i, rs_i, an_i = part
+            t, nz, sd, chain_i, flags_i, used_i, attempts_i, passed_i, checks_i, redraw_i, sets_i, lh_i, rs_i, an_i, fx_i = part
             stream = torch.cuda.current_stream(where).cuda_stream if where.type == 'cuda' else None
             rng_i = None if rng is None else (rng[0], rng[1], rng[2] + lo, rng[3])
             calls.append((dev_i, functools.partial(
@@ -1498,7 +1593,8 @@ class EDM(torch.nn.Module):
                 stream, nz, sd, rng_i,
                 (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i, sets_i, lh_i,
                  (allowed, rs_i) if rings else None, an_i) if recover else None,
-                start.rows(lo, hi) if isinstance(start, StartSteps) else start, resample, guide, solver)))
+                start.rows(lo, hi) if isinstance(start, StartSteps) else start, resample, guide, solver,
+                None if fixed is None else (fx_i, self.T, fixed[1]))))
 
         def finish():
             if not whole:
@@ -1583,7 +1679,7 @@ class InpaintingEDM(EDM):
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, anchors=None, clash_guidance=None, solver=None):
+                     require_anchors=None, anchors=None, clash_guidance=None, solver=None, fixed_atoms=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -1606,7 +1702,7 @@ class InpaintingEDM(EDM):
         them; the batch stream advances by as many draws; per-molecule streams use their draws in that order). r = 1 is
         the plain sampler, bit for bit. A call costs about r times the loop. ValueError for a non-integer, a bool or
         r < 1. `clash_guidance` raises ValueError unless None: this loop re-noises the pocket. `solver` unless None or
-        'ancestral': this sampler has no ODE update."""
+        'ancestral': this sampler has no ODE update. `fixed_atoms` unless None: this sampler keeps known atoms its own way."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
@@ -1615,7 +1711,7 @@ class InpaintingEDM(EDM):
                                     require_unique=require_unique, require_novel=require_novel,
                                     exclude_hashes=exclude_hashes, resamplings=resamplings,
                                     require_ring_sizes=require_ring_sizes, require_anchors=require_anchors,
-                                    anchors=anchors, clash_guidance=clash_guidance, solver=solver)
+                                    anchors=anchors, clash_guidance=clash_guidance, solver=solver, fixed_atoms=fixed_atoms)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

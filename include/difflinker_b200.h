@@ -23,6 +23,8 @@
  *     ... at one step t0[b] per molecule                 dl_set_start_steps, then the per-row entry points
  *   EDM, deterministic DDIM or DPM-Solver++(2M) steps   dl_set_solver, then any dl_sample_chain* entry point
  *     instead of p(z_s | z_t) (no reference API)
+ *   EDM, keeping given linker atoms and sampling the    dl_set_fixed_atoms before each dl_sample_chain* call
+ *     rest (replacement, RePaint without re-noising passes; no reference API)
  *   InpaintingEDM, r RePaint passes per step            dl_set_resamplings, then any dl_sample_chain* entry point
  *     (DiffSBDD's inpaint(..., resamplings=r), no reference API)
  *   either, resampling only the molecules that diverged  dl_sample_chain_retry, dl_retry_seed, dl_last_retry_ms
@@ -786,6 +788,38 @@ dl_status dl_set_clash_guidance(dl_engine* e, float scale, int32_t steps, int32_
  * call, a T other than the one set and DL_SAMPLER_INPAINT.
  */
 dl_status dl_set_solver(dl_engine* e, int32_t kind, int32_t T, const float* table);
+/*
+ * Fixed atoms for DL_SAMPLER_LINKER (scaffold-constrained generation by replacement, as RePaint replaces known pixels; no
+ * reference API): the engine's next dl_sample_chain* call -- and the recovery rounds of a dl_sample_chain_retry(_sets) call
+ * -- keeps the linker rows whose (B, N) int8 DEVICE flag `fixed` is non-zero at the coordinates and types of the call's
+ * xh, and samples the other linker rows around them. The kept rows stay noisy linker rows throughout, as the linker
+ * denoiser was trained to see them: with xh the row's normalised input, eps_0 its own draw 0, and (alpha_s, sigma_s) row
+ * r = T-1-s of the (T + 1, 2) HOST fp32 `scalars` (dl_step_coef's row order; row T holds (alpha_T, sigma_T)),
+ *   start                   alpha xh + sigma eps_0, as the partial-diffusion start forms it (k_init_z_rows), with the
+ *                           scalars of the call's start: row T from noise, dl_set_start_step's, or each row's own
+ *                           dl_set_start_steps scalars
+ *   step s < T, ancestral   alpha_s xh + sigma_s nz_s, nz_s the draw the update reads for the row and would otherwise
+ *                           scale by sigma; the draws stay those of the plain call in count and order, so seeds, offsets
+ *                           and noise tensors mean what they mean without this call
+ *   step s < T, dl_set_solver  alpha_s xh + sigma_s eps_0 (the probability-flow path of a known point); the 2M history of
+ *                           a kept row never enters it
+ *   final step              xh, so chain[0] holds the input's x times norm[0] (bit for bit when norm[0] is a power of two,
+ *                           as for every DiffLinker model) and the one-hot of its types
+ * Each product and the sum is rounded on its own. Frames hold the replaced state, unnormalised like every row. The network
+ * sees the kept rows as linker rows, and the molecule checks count them as linker atoms. Clash guidance
+ * (dl_set_clash_guidance) neither moves the kept rows nor lets them push. EDM.fixed_atom_scalars builds `scalars` as
+ * start_scalars(s, B) row by row (q(z_s | x)'s alpha and sigma as EDM.forward evaluates them at the call's batch size).
+ * Per-call input like dl_set_anchors: the flags are copied on `stream` (the call reads them while its loop runs), the
+ * scalars into host memory, uploaded on the loop stream by the call; every dl_sample_chain* call reads and clears the
+ * setting, whether or not it uses it. fixed = NULL switches it off (the other arguments are ignored): the calls then launch
+ * exactly what they launch without it. DL_ERR_INVALID: here, B or N < 1, T outside [1, 2^24], NULL scalars or a
+ * non-finite one; at the sampling call, which then blocks once to vet the flags, a B, N or T other than the ones set,
+ * DL_SAMPLER_INPAINT, a size redraw (dl_size_redraw), a flag on a row that is not a live linker row (node_mask and
+ * linker_mask non-zero, fragment_mask 0: fragment, pocket and padding rows), and a flagged row whose type channels are not
+ * a normalised one-hot (one channel (1 - norm[2]) / norm[1], the others (0 - norm[2]) / norm[1], in fp32).
+ */
+dl_status dl_set_fixed_atoms(dl_engine* e, int32_t B, int32_t N, const int8_t* fixed, int32_t T, const float* scalars,
+                             void* stream);
 /* The (n_draws,B,N,3+F) tensor the device-side stream of dl_sample_chain_rng stands for (tests, debugging). DEVICE out. */
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream);
