@@ -113,6 +113,7 @@ SYMBOLS = {
     "dl_set_clash_guidance": (_I32, [_P, C.c_float, _I32, _I32, _P]),
     "dl_set_solver": (_I32, [_P, _I32, _I32, _P]),
     "dl_set_fixed_atoms": (_I32, [_P, _I32, _I32, _P, _I32, _P, _P]),
+    "dl_set_linker_types": (_I32, [_P, _I32, _I32, _P, _I32, _P]),
     "dl_clash_guide": (_I32, [_I32, _I32, _I32, _P, C.c_float, _P, _I32, _P, _P, _P, _I32, _P]),
     "dl_noise_fill": (_I32, [_P, _I32, _I32, _I32, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "dl_noise_fill_inpaint": (_I32, [_P, _I32, _I32, _I32, _P, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),

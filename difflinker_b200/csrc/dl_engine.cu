@@ -174,6 +174,12 @@ struct dl_engine {
   bool fixed_set = false;
   int fixed_B = 0, fixed_N = 0, fixed_T = 0;
   std::vector<float> fixed_scalars;
+  // dl_set_linker_types: host copies of the (types_B) masks of allowed type channels and the (types_T + 1, 2) scalars; the
+  // next dl_sample_chain* call reads and clears types_set and uploads them, and its recovery rounds take their rows' masks
+  bool types_set = false;
+  int types_B = 0, types_T = 0;
+  std::vector<uint32_t> types_masks;
+  std::vector<float> types_scalars;
   cudaEvent_t ev_r0 = nullptr, ev_r1 = nullptr, ev_g0 = nullptr, ev_g1 = nullptr;
   float retry_ms = 0.f;
   cudaStream_t loop_stream = nullptr;
@@ -429,7 +435,16 @@ struct FwdIO {
   const float* ode = nullptr;               // the solver rows of the loop (dl_set_solver), or null: the ancestral update
   const int8_t* fixed = nullptr;            // fixed atoms (dl_set_fixed_atoms): the rows' flags, or null
   const float* fix = nullptr;               // ... and the (alpha_s, sigma_s) rows of the loop
+  const uint32_t* types = nullptr;          // linker types (dl_set_linker_types): the molecules' masks, or null
+  const float* tsc = nullptr;               // ... and the (alpha_t, sigma_t) rows of the loop
 };
+
+// The k_finish instantiation of a sampler step: per-molecule streams, an ODE solver, fixed atoms, linker types.
+template <bool FIX, bool TYPES>
+void (*finish_kernel(bool per_mol, bool ode))(Geom, FinishArgs) {
+  return ode ? (per_mol ? k_finish<true, true, FIX, TYPES> : k_finish<false, true, FIX, TYPES>)
+             : (per_mol ? k_finish<true, false, FIX, TYPES> : k_finish<false, false, FIX, TYPES>);
+}
 
 ProjW proj_of(const EdgeMlpW& w) { return ProjW{w.W1a_t, w.W1b_t, w.b1}; }
 
@@ -625,14 +640,13 @@ dl_status enqueue_forward(dl_engine* e, int B, int N, const FwdIO& io, cudaStrea
     // the 2M history lives in ws.eps, which the fused linker update never writes otherwise
     fa.ode = io.ode; fa.hist = io.ode && e->solver_kind == DL_SOLVER_DPMPP_2M ? ws.eps : nullptr;
     fa.fixed = io.fixed; fa.xh0 = io.xh0; fa.fix = io.fix;
+    fa.types = io.types; fa.tsc = io.tsc;
   } else if (io.sampler) {
     fa.tag_step = e->step_ctr + (io.R > 1 ? 2 : 1);   // with resampling the pass counter is not the step
   }
   const bool per_mol = io.rng.on == NOISE_PER_MOLECULE;
-  auto* finish = fa.fixed ? (fa.ode ? (per_mol ? k_finish<true, true, true> : k_finish<false, true, true>)
-                                   : (per_mol ? k_finish<true, false, true> : k_finish<false, false, true>))
-               : fa.ode ? (per_mol ? k_finish<true, true> : k_finish<false, true>)
-                        : (per_mol ? k_finish<true> : k_finish<false>);
+  auto* finish = fa.types ? (fa.fixed ? finish_kernel<true, true>(per_mol, fa.ode) : finish_kernel<false, true>(per_mol, fa.ode))
+                          : (fa.fixed ? finish_kernel<true, false>(per_mol, fa.ode) : finish_kernel<false, false>(per_mol, fa.ode));
   TIMED("k_finish", st, (launch_chain(finish, dim3((n + 15) / 16), dim3(256), 0, st, gm, fa)));
   LAUNCH_CHECK();
   e->launches += 1;
@@ -858,7 +872,7 @@ struct CallFixed {
   int B = 0, N = 0, T = 0;
   const float* scalars = nullptr;
   bool vetted = false;
-  int* bad = nullptr;        // two ints of device memory for k_fixed_check, unless vetted
+  int* bad = nullptr;        // three ints of device memory for k_fixed_check and k_kept_types_check, unless vetted
 };
 
 // What dl_set_fixed_atoms set since the engine's previous sampling call, which every call reads and clears.
@@ -871,6 +885,24 @@ CallFixed take_fixed(dl_engine* e) {
   }
   if (e) e->fixed_set = false;
   return fx;
+}
+
+// The linker types of a sampling call (dl_set_linker_types): the B masks and the (T + 1, 2) scalars, host memory, with B
+// and T as set; masks = null: none.
+struct CallTypes {
+  const uint32_t* masks = nullptr;
+  int B = 0, T = 0;
+  const float* scalars = nullptr;
+};
+
+// What dl_set_linker_types set since the engine's previous sampling call, which every call reads and clears.
+CallTypes take_types(dl_engine* e) {
+  CallTypes ty;
+  if (e && e->types_set) {
+    ty.masks = e->types_masks.data(); ty.B = e->types_B; ty.T = e->types_T; ty.scalars = e->types_scalars.data();
+  }
+  if (e) e->types_set = false;
+  return ty;
 }
 
 // Captures one reverse step over the first Bp rows of the workspace into *graph.
@@ -1113,7 +1145,8 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
                                    const float* xh, const int8_t* node_mask, const float* fragment_mask,
                                    const float* linker_mask, const int8_t* edge_mask, const float* context,
                                    const float* noise, const NoiseRng* rng, const dl_step_coef* coef, const float* norm,
-                                   float* chain, int32_t* nan_flags, void* stream, const CallFixed& fx);
+                                   float* chain, int32_t* nan_flags, void* stream, const CallFixed& fx,
+                                   const CallTypes& ty);
 
 dl_status dl_sample_chain(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
                           const float* xh, const int8_t* node_mask, const float* fragment_mask,
@@ -1121,9 +1154,10 @@ dl_status dl_sample_chain(dl_engine* e, int32_t sampler, int32_t B, int32_t N, i
                           const float* noise, const dl_step_coef* coef, const float* norm, float* chain,
                           int32_t* nan_flags, void* stream) {
   const CallFixed fx = take_fixed(e);
+  const CallTypes ty = take_types(e);
   if (!noise) { set_err("null argument (noise): use dl_sample_chain_rng to draw on the device"); return DL_ERR_INVALID; }
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, noise,
-                           nullptr, coef, norm, chain, nan_flags, stream, fx);
+                           nullptr, coef, norm, chain, nan_flags, stream, fx, ty);
 }
 
 dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
@@ -1132,6 +1166,7 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
                               uint64_t offset, uint64_t* offset_consumed, const dl_step_coef* coef, const float* norm,
                               float* chain, int32_t* nan_flags, void* stream) {
   const CallFixed fx = take_fixed(e);
+  const CallTypes ty = take_types(e);
   dl_status s = check_shapes(e, B, N);
   if (s == DL_OK) s = check_slice(e, B);
   if (s != DL_OK) return s;
@@ -1146,23 +1181,25 @@ dl_status dl_sample_chain_rng(dl_engine* e, int32_t sampler, int32_t B, int32_t 
   const NoiseRng q = make_rng(e, B, N, seed, offset);
   if (offset_consumed) *offset_consumed = sampler_draws(sampler, loop_steps(e, T), R) * q.per_draw;
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, nullptr,
-                           &q, coef, norm, chain, nan_flags, stream, fx);
+                           &q, coef, norm, chain, nan_flags, stream, fx, ty);
 }
 
 }  // extern "C"
 
-// dl_sample_chain_seeded with the fixed atoms fx: the recovery rounds' entry, which passes their gathered flags.
+// dl_sample_chain_seeded with the fixed atoms fx and the linker types ty: the recovery rounds' entry, which passes their
+// gathered flags and masks.
 static dl_status sample_seeded(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames,
                                const float* xh, const int8_t* node_mask, const float* fragment_mask, const float* linker_mask,
                                const int8_t* edge_mask, const float* context, const uint64_t* seeds, const dl_step_coef* coef,
-                               const float* norm, float* chain, int32_t* nan_flags, void* stream, const CallFixed& fx) {
+                               const float* norm, float* chain, int32_t* nan_flags, void* stream, const CallFixed& fx,
+                               const CallTypes& ty) {
   // the seeds name the molecules, so the engine's batch slice does not apply; sample_chain_impl copies them into the
   // workspace and points the stream at that copy
   NoiseRng q{};
   q.seeds = reinterpret_cast<const unsigned long long*>(seeds);
   q.F = e ? e->cfg.in_node_nf : 0; q.N = N; q.on = NOISE_PER_MOLECULE;
   return sample_chain_impl(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, nullptr,
-                           &q, coef, norm, chain, nan_flags, stream, fx);
+                           &q, coef, norm, chain, nan_flags, stream, fx, ty);
 }
 
 extern "C" {
@@ -1173,7 +1210,7 @@ dl_status dl_sample_chain_seeded(dl_engine* e, int32_t sampler, int32_t B, int32
                                  const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
                                  int32_t* nan_flags, void* stream) {
   return sample_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
-                       coef, norm, chain, nan_flags, stream, take_fixed(e));
+                       coef, norm, chain, nan_flags, stream, take_fixed(e), take_types(e));
 }
 
 dl_status dl_set_noise_slice(dl_engine* e, int32_t B_full, int32_t b0) {
@@ -1316,13 +1353,42 @@ dl_status dl_set_fixed_atoms(dl_engine* e, int32_t B, int32_t N, const int8_t* f
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   StageLayout fl;
   const int i_fx = fl.out((size_t)B * N);
-  fl.out(2 * sizeof(int));   // the call's vetting (k_fixed_check)
+  fl.out(3 * sizeof(int));   // the call's vetting (k_fixed_check, k_kept_types_check)
   dl_status s = stage_inputs(e->fixed, fl, st);
   if (s != DL_OK) return s;
   CK(cudaMemcpyAsync(fl.at<int8_t>(i_fx), fixed, (size_t)B * N, cudaMemcpyDefault, st));
   e->fixed_scalars.assign(scalars, scalars + 2 * (size_t)(T + 1));
   e->fixed_set = true;
   e->fixed_B = B; e->fixed_N = N; e->fixed_T = T;
+  return DL_OK;
+}
+
+dl_status dl_set_linker_types(dl_engine* e, int32_t B, int32_t F, const uint32_t* masks, int32_t T, const float* scalars) {
+  if (!e) { set_err("dl_set_linker_types: null engine"); return DL_ERR_INVALID; }
+  e->types_set = false;
+  if (!masks) return DL_OK;
+  const char* why = nullptr;
+  if (B < 1) why = "B must be >= 1";
+  else if (F != e->cfg.in_node_nf) why = "F must be the model's number of type channels (dl_config.in_node_nf)";
+  else if (T < 1 || T > (1 << 24)) why = "T must lie in [1, 2^24]";
+  else if (!scalars) why = "null scalars";
+  if (why) { set_err("dl_set_linker_types: %s", why); return DL_ERR_INVALID; }
+  for (int b = 0; b < B; ++b) {
+    if (masks[b] == 0 || (F < 32 && (masks[b] >> F) != 0)) {
+      set_err("dl_set_linker_types: the mask of molecule %d, 0x%x, %s", b, masks[b],
+              masks[b] == 0 ? "allows no type" : "has bits at or above F");
+      return DL_ERR_INVALID;
+    }
+  }
+  for (int i = 0; i < 2 * (T + 1); ++i)
+    if (!std::isfinite(scalars[i])) {
+      set_err("dl_set_linker_types: scalars[%d][%d] is not finite", i / 2, i % 2);
+      return DL_ERR_INVALID;
+    }
+  e->types_masks.assign(masks, masks + B);
+  e->types_scalars.assign(scalars, scalars + 2 * (size_t)(T + 1));
+  e->types_set = true;
+  e->types_B = B; e->types_T = T;
   return DL_OK;
 }
 
@@ -1368,7 +1434,8 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
                                    const float* xh, const int8_t* node_mask, const float* fragment_mask,
                                    const float* linker_mask, const int8_t* edge_mask, const float* context,
                                    const float* noise, const NoiseRng* rng, const dl_step_coef* coef, const float* norm,
-                                   float* chain, int32_t* nan_flags, void* stream, const CallFixed& fx) {
+                                   float* chain, int32_t* nan_flags, void* stream, const CallFixed& fx,
+                                   const CallTypes& ty) {
   const bool per_mol = rng && rng->on == NOISE_PER_MOLECULE;
   dl_status s = check_shapes(e, B, N);
   if (s == DL_OK) s = check_sampler(e, sampler, T, keep_frames, noise || (rng && (!per_mol || rng->seeds)), xh, node_mask,
@@ -1417,6 +1484,12 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
                  fx.T, B, N, T);
     return DL_ERR_INVALID;
   }
+  const bool types = ty.masks != nullptr;
+  if (types && (inpaint || B != ty.B || T != ty.T)) {
+    if (inpaint) set_err("dl_set_linker_types takes DL_SAMPLER_LINKER only: the inpainting sampler updates every atom");
+    else set_err("dl_set_linker_types was given B = %d, T = %d; the call samples B = %d, T = %d", ty.B, ty.T, B, T);
+    return DL_ERR_INVALID;
+  }
   // A start step t0 runs the table's last t0 + 1 rows -- steps t0-1 .. 0, then the final one -- as a loop of Tl = t0 steps:
   // loop step r reads row r of the copied rows and draw r + 1, so the draws are eps, one per step and the final one.
   const int Tl = loop_steps(e, T);
@@ -1426,9 +1499,11 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   // only its last pass writes; the jump coefficients follow the table on the device. A solver (never with R > 1, which is
   // the inpainting sampler's) puts the same rows of its table there instead.
   const int P = Tl * R, rows = P + 1;
-  // Fixed atoms put the (alpha_s, sigma_s) of the loop's Tl steps after them.
+  // Fixed atoms put the (alpha_s, sigma_s) of the loop's Tl steps after them, linker types the (alpha_t, sigma_t) of its
+  // rows and then the B masks.
   const size_t coef_bytes = (size_t)rows * sizeof(dl_step_coef) + (R > 1 ? e->jump.size() * sizeof(float) : 0) +
-                            (ode ? (size_t)rows * 8 * sizeof(float) : 0) + (fix ? (size_t)Tl * 2 * sizeof(float) : 0);
+                            (ode ? (size_t)rows * 8 * sizeof(float) : 0) + (fix ? (size_t)Tl * 2 * sizeof(float) : 0) +
+                            (types ? (size_t)rows * 2 * sizeof(float) + (size_t)B * sizeof(uint32_t) : 0);
   if (R > 1) {
     e->coef_passes.resize(rows);
     for (int p = 0; p < P; ++p) {
@@ -1478,24 +1553,46 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
     CK(cudaMemcpyAsync(const_cast<float*>(ode_dev), e->solver_table.data() + (size_t)(T - Tl) * 8,
                        (size_t)rows * 8 * sizeof(float), cudaMemcpyHostToDevice, st));
   const float* fix_dev = fix ? e->coef_dev + (size_t)rows * 8 + (ode ? (size_t)rows * 8 : 0) : nullptr;
+  const float* tsc_dev = types ? e->coef_dev + (size_t)rows * 8 + (ode ? (size_t)rows * 8 : 0) + (fix ? (size_t)Tl * 2 : 0)
+                               : nullptr;
+  const uint32_t* types_dev = types ? reinterpret_cast<const uint32_t*>(tsc_dev + (size_t)rows * 2) : nullptr;
+  if (types) {
+    // loop row r runs from t = Tl - r: the scalars' row of step t - 1 = T-1-(T-Tl+r-1), or row T where t = T
+    std::vector<float> tsc(2 * (size_t)rows);
+    for (int r = 0; r < rows; ++r) {
+      const int k = T - Tl + r, src = k > 0 ? k - 1 : T;
+      tsc[2 * r] = ty.scalars[2 * src]; tsc[2 * r + 1] = ty.scalars[2 * src + 1];
+    }
+    CK(cudaMemcpyAsync(const_cast<float*>(tsc_dev), tsc.data(), tsc.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(const_cast<uint32_t*>(types_dev), ty.masks, (size_t)B * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  }
   if (fix) {
     CK(cudaMemcpyAsync(const_cast<float*>(fix_dev), fx.scalars + (size_t)(T - Tl) * 2, (size_t)Tl * 2 * sizeof(float),
                        cudaMemcpyHostToDevice, st));
     if (!fx.vetted) {
       // the flags against the masks and the kept types (a recovery round's rows come from a call that passed this)
-      int bad[2] = {0, 0};
+      // with linker types, also the kept rows' types against their molecules' masks
+      int bad[3] = {0, 0, 0};
       CK(cudaMemsetAsync(fx.bad, 0, sizeof(bad), st));
       k_fixed_check<<<(B * N + 255) / 256, 256, 0, st>>>(B * N, 3 + e->cfg.in_node_nf, fx.flags, node_mask, fragment_mask,
                                                         linker_mask, xh, norm[1], norm[2], fx.bad);
       LAUNCH_CHECK();
       e->launches += 1;
+      if (types) {
+        k_kept_types_check<<<(B * N + 255) / 256, 256, 0, st>>>(B * N, N, 3 + e->cfg.in_node_nf, fx.flags, xh, types_dev,
+                                                               norm[1], norm[2], fx.bad + 2);
+        LAUNCH_CHECK();
+        e->launches += 1;
+      }
       CK(cudaMemcpyAsync(bad, fx.bad, sizeof(bad), cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
-      if (bad[0] || bad[1]) {
-        const int g = (bad[0] ? bad[0] : bad[1]) - 1;
-        set_err("dl_set_fixed_atoms: row %d of molecule %d %s", g % N, g / N,
-                bad[0] ? "is flagged but is not a live linker row (node_mask and linker_mask set, fragment_mask 0)"
-                       : "is flagged but its type channels are not a one-hot");
+      if (bad[0] || bad[1] || bad[2]) {
+        const int g = (bad[0] ? bad[0] : bad[1] ? bad[1] : bad[2]) - 1;
+        set_err("%s: row %d of molecule %d %s", bad[2] && !bad[0] && !bad[1] ? "dl_set_linker_types" : "dl_set_fixed_atoms",
+                g % N, g / N,
+                bad[0]   ? "is flagged but is not a live linker row (node_mask and linker_mask set, fragment_mask 0)"
+                : bad[1] ? "is flagged but its type channels are not a one-hot"
+                         : "is kept (dl_set_fixed_atoms) but its type is one its molecule's mask excludes");
         return DL_ERR_INVALID;
       }
     }
@@ -1575,6 +1672,7 @@ static dl_status sample_chain_impl(dl_engine* e, int32_t sampler, int32_t B, int
   io.rows = per_row ? ro.rs : RowStarts{};
   io.R = R; io.jump = jump_dev; io.ode = ode_dev;
   io.fixed = fixed; io.fix = fix_dev;
+  io.types = types_dev; io.tsc = tsc_dev;
 
   // capture ONE reverse step; the step index lives on the device, so the same graph serves all Tl+1 steps (all P+1 passes
   // with resampling) -- with per-molecule start steps, all steps of one prefix length: the graph is recaptured whenever the
@@ -1827,18 +1925,19 @@ const char* sets_error(dl_engine* e, int require, const dl_hash_sets* hs, cudaSt
 // the new one diverged. `hs` (or null) holds the known set of DL_CHECK_NOVEL and the seen set of DL_CHECK_UNIQUE;
 // `linker_hash` (or null) receives every returned row's linker hash with DL_CHECK_NOVEL. `anchors` (B, N), read with
 // DL_CHECK_ANCHORS only, are the anchor flags, which k_anchor_check reads right after the check launch. `fx` are the call's
-// fixed atoms: every round gathers its rows' flags and keeps them.
+// fixed atoms: every round gathers its rows' flags and keeps them. `ty` are the call's linker types: every round takes its
+// rows' masks.
 dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int32_t T, int32_t keep_frames, const float* xh,
                        const int8_t* node_mask, const float* fragment_mask, const float* linker_mask, const int8_t* edge_mask,
                        const float* context, const uint64_t* seeds, const dl_step_coef* coef, const float* norm, float* chain,
                        int32_t* nan_flags, int32_t max_retries, uint64_t* seeds_used, int32_t* attempts,
                        const dl_molecule_checks* ck, const dl_hash_sets* hs, int32_t* passed, uint64_t* linker_hash,
                        const dl_size_redraw* rz, int32_t* sizes_used, const int8_t* anchors, const CallFixed& fx,
-                       void* stream) {
+                       const CallTypes& ty, void* stream) {
   e->retry_ms = 0.f;
   e->ring_B = 0;
   dl_status s = sample_seeded(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context,
-                              seeds, coef, norm, chain, nan_flags, stream, fx);
+                              seeds, coef, norm, chain, nan_flags, stream, fx, ty);
   if (s != DL_OK) return s;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CK(cudaMemcpyAsync(seeds_used, seeds, (size_t)B * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
@@ -1952,9 +2051,16 @@ dl_status seeded_retry(dl_engine* e, int32_t sampler, int32_t B, int32_t N, int3
         sub_fx = fx;
         sub_fx.flags = fa.s_fixed; sub_fx.B = Bs; sub_fx.vetted = true;
       }
+      std::vector<uint32_t> sub_masks;                     // ... and their linker types
+      CallTypes sub_ty;
+      if (ty.masks) {
+        for (int b : rows) sub_masks.push_back(ty.masks[b]);
+        sub_ty = ty;
+        sub_ty.masks = sub_masks.data(); sub_ty.B = Bs;
+      }
       s = sample_seeded(e, sampler, Bs, N, T, keep_frames, ga.s_xh, ga.s_node_mask, ga.s_fragment_mask, ga.s_linker_mask,
                         ga.s_edge_mask, ga.s_context, reinterpret_cast<const uint64_t*>(ga.s_seeds), coef, norm,
-                        sl.at<float>(i_ch), sl.at<int32_t>(i_fl), stream, sub_fx);
+                        sl.at<float>(i_ch), sl.at<int32_t>(i_fl), stream, sub_fx, sub_ty);
     }
     if (per_row) { e->starts_t0.swap(t0_all); e->starts_alpha.swap(alpha_all); e->starts_sigma.swap(sigma_all); }
     if (s != DL_OK) return s;
@@ -2029,6 +2135,7 @@ dl_status retry_entry(const char* name, dl_engine* e, int32_t sampler, int32_t B
   an.flags = reinterpret_cast<const int8_t*>(e->anchors.buf);
   e->anchors_set = false;
   const CallFixed fx = take_fixed(e);                      // likewise
+  const CallTypes ty = take_types(e);                      // likewise
   if (max_retries < 0) { set_err("max_retries must be >= 0 (got %d)", max_retries); return DL_ERR_INVALID; }
   if (!nan_flags || !seeds_used || !attempts || (checks && !passed) || (redraw && !sizes_used)) {
     set_err("%s: null argument (nan_flags, seeds_used, attempts, passed with checks or sizes_used with redraw)", name);
@@ -2054,7 +2161,7 @@ dl_status retry_entry(const char* name, dl_engine* e, int32_t sampler, int32_t B
   }
   return seeded_retry(e, sampler, B, N, T, keep_frames, xh, node_mask, fragment_mask, linker_mask, edge_mask, context, seeds,
                       coef, norm, chain, nan_flags, max_retries, seeds_used, attempts, checks, sets, passed, linker_hash,
-                      redraw, sizes_used, an.flags, fx, stream);
+                      redraw, sizes_used, an.flags, fx, ty, stream);
 }
 
 }  // namespace

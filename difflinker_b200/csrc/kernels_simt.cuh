@@ -916,6 +916,11 @@ struct FinishArgs {
   const int8_t* fixed;
   const float* xh0;
   const float* fix;
+  // linker types (dl_set_linker_types, k_finish<., ., ., true>): one mask of allowed type channels per molecule (bit c:
+  // channel 3 + c), in the caller's row order (rows.src maps a workspace row to it), and the (alpha_t, sigma_t) of the
+  // loop's rows, 2 floats per row in coef's row order
+  const uint32_t* types;
+  const float* tsc;
 };
 
 // A kept row's z_s = alpha_s xh + sigma_s eps, every product and the sum rounded on their own as k_init_z_rows rounds them.
@@ -923,7 +928,10 @@ __device__ __forceinline__ float fixed_state(const float* sc, float xh, float ep
   return __fadd_rn(__fmul_rn(sc[0], xh), __fmul_rn(sc[1], eps));
 }
 
-template <bool PER_MOL = false, bool ODE = false, bool FIX = false>
+// TYPES: on a free linker row (linker_mask != 0, not kept), a type channel its molecule's mask excludes predicts the
+// one-hot's normalised "off" value, off = (0 - bias1) / norm1: the ODE update sets xhat = off, the ancestral update reads
+// eps = (z_t - alpha_t off) / sigma_t, which is the same, and the final decode takes the argmax over the allowed channels.
+template <bool PER_MOL = false, bool ODE = false, bool FIX = false, bool TYPES = false>
 __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
   const int tid = threadIdx.x;
   const int d = tid & 15, r = tid >> 4;
@@ -958,6 +966,7 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
     gc = (size_t)a.rows.src[b] * gm.N + (g - b * gm.N);
     nc = a.rows.n_full;
   }
+  const uint32_t allowed = TYPES && g < n_total ? a.types[gc / gm.N] : ~0u;   // the molecule's mask, in the caller's order
   for (int idx = tid; idx < 16 * (H / 4); idx += 256) {
     const int rr = idx / (H / 4), k4 = idx - rr * (H / 4);
     const int gg = blockIdx.x * 16 + rr;
@@ -998,6 +1007,7 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
   const int frame = __float_as_int(cf[4]);
   float znew = 0.f;
   float lm = 0.f, fm = 0.f;
+  bool excl = false;   // TYPES: channel d is an excluded type of a free linker row
   if constexpr (ODE) {
     // deterministic update from the solver row sv = (sigma_t, 1/alpha_t, sigma_s/sigma_t, c1, c2a, c2b, h, 0): the data
     // prediction xhat = (z_t - sigma_t eps) / alpha_t, then z_s = (sigma_s/sigma_t) z_t + c1 xhat at a row's first step
@@ -1009,8 +1019,10 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
       const float zt = a.z[gi];
       const float eps = e * lm;
       const float* sv = a.ode + (size_t)step * 8;
-      const float xhat = sv[1] * (zt - sv[0] * eps);
+      float xhat = sv[1] * (zt - sv[0] * eps);
       const bool kept = FIX && a.fixed[g] != 0;
+      excl = TYPES && d >= 3 && lm != 0.f && !kept && ((allowed >> (d - 3)) & 1u) == 0;
+      if (excl) xhat = __fdiv_rn(__fsub_rn(0.f, a.bias1), a.norm1);   // TYPES: the projected xhat, which the 2M history keeps
       if (step < a.T) {
         float zs;
         if (a.hist != nullptr && step > lag) zs = sv[2] * zt + (sv[4] * xhat + sv[5] * a.hist[gi]);
@@ -1033,11 +1045,17 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
   } else if (act) {
     lm = a.linker_mask[g]; fm = a.fragment_mask[g];
     const float zt = a.z[(size_t)g * xd + d];
-    const float eps = e * lm;                                                 // edm.py:196 / 225
+    float eps = e * lm;                                                       // edm.py:196 / 225
     const float nz = (a.rng.on ? noise_draw<PER_MOL>(a.rng, step + 1 - lag, g, d)
                                : a.noise[((size_t)(step + 1 - lag) * nc + gc) * xd + d]) * lm;  // utils.py:189-192
     // FIX: a kept row takes alpha_s xh + sigma_s nz_s from the draw the update reads, and the input at the final step
     const bool kept = FIX && a.fixed[g] != 0;
+    excl = TYPES && d >= 3 && lm != 0.f && !kept && ((allowed >> (d - 3)) & 1u) == 0;
+    if (excl) {   // TYPES: the eps of xhat = off, with the (alpha_t, sigma_t) of this row
+      const float* ts = a.tsc + (size_t)step * 2;
+      const float off = __fdiv_rn(__fsub_rn(0.f, a.bias1), a.norm1);
+      eps = __fdiv_rn(__fsub_rn(zt, __fmul_rn(ts[0], off)), ts[1]);
+    }
     if (step < a.T) {
       float mu = zt / ca - cb * eps;                                          // edm.py:199
       float zs = mu + cc * nz;                                                // edm.py:205, 342-345
@@ -1057,7 +1075,7 @@ __global__ void __launch_bounds__(256) k_finish(Geom gm, FinishArgs a) {
   }
   if (step >= a.T) {
     // edm.py:231-233: unnormalise, h = one_hot(argmax(h)) * node_mask. argmax over the 16-lane group.
-    float hv = (act && d >= 3) ? znew * a.norm1 + a.bias1 : -INFINITY;
+    float hv = (act && d >= 3 && !excl) ? znew * a.norm1 + a.bias1 : -INFINITY;   // TYPES: the allowed channels only
     int best = d;
     float bv = hv;
     const unsigned gmask = 0xffffffffu;
@@ -1369,6 +1387,18 @@ __global__ void k_fixed_check(int n_total, int xd, const int8_t* __restrict__ fi
     others += v != one && v != zero;
   }
   if (ones != 1 || others != 0) atomicCAS(bad + 1, 0, g + 1);
+}
+
+// dl_set_linker_types with dl_set_fixed_atoms: *bad = 1 + a flagged row whose type -- the channel equal to the normalised
+// one, (1 - bias1) / norm1 -- its molecule's mask excludes. k_fixed_check vets the one-hot itself.
+__global__ void k_kept_types_check(int n_total, int N, int xd, const int8_t* __restrict__ fixed, const float* __restrict__ xh,
+                                   const uint32_t* __restrict__ masks, float norm1, float bias1, int* bad) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n_total || fixed[g] == 0) return;
+  const float one = __fdiv_rn(__fsub_rn(1.f, bias1), norm1);
+  const uint32_t m = masks[g / N];
+  for (int d = 3; d < xd; ++d)
+    if (xh[(size_t)g * xd + d] == one && ((m >> (d - 3)) & 1u) == 0) atomicCAS(bad, 0, g + 1);
 }
 
 // Debug / test helper: the (n_draws, n_total, 3+F) tensor the device-side stream stands for.

@@ -20,6 +20,7 @@ from .batching import create_templates_for_linker_generation
 from .edm import EDM, InpaintingEDM, LinkerSizes, draw_seeds, seeds_tensor
 from .egnn import Dynamics, DynamicsWithPockets
 from .linker_size import SizeClassifier, draw_sizes
+from .output import GEOM_IDX2ATOM, IDX2ATOM
 
 
 def _is_geom(hp: dict):
@@ -235,6 +236,29 @@ def _check_fixed(sample_fn, linker_sizes, fixed_atoms):
         raise ValueError("fixed_atoms does not take linker_sizes: a size redraw rebuilds the linker rows at new sizes")
 
 
+def linker_types_mask(edm, linker_types):
+    """EDM.sample_chain's `linker_types` of `linker_types` as the DDPM level takes it: None; a (F,) or (B, F) bool tensor,
+    returned as it is; or element symbols (['C', 'N', 'O']), the (F,) bool set of their type channels in output.IDX2ATOM
+    (ZINC), or output.GEOM_IDX2ATOM with edm.is_geom (GEOM / MOAD), the tables molecule_builder reads types with.
+    ValueError for an unknown symbol, and for symbols when edm.is_geom is None."""
+    if linker_types is None or torch.is_tensor(linker_types):
+        return linker_types
+    symbols = [linker_types] if isinstance(linker_types, str) else list(linker_types)
+    if not all(isinstance(v, str) for v in symbols):
+        raise ValueError(f"linker_types is a bool tensor or a list of element symbols (got {linker_types!r})")
+    if edm.is_geom is None:
+        raise ValueError("linker_types by element symbol needs the atom types: build the EDM with is_geom=True (GEOM / MOAD) "
+                         "or False (ZINC), or set edm.is_geom")
+    idx2atom = GEOM_IDX2ATOM if edm.is_geom else IDX2ATOM
+    index = {a: i for i, a in idx2atom.items() if i < edm.in_node_nf}
+    mask = torch.zeros(edm.in_node_nf, dtype=torch.bool)
+    for a in symbols:
+        if a not in index:
+            raise ValueError(f"linker_types: unknown element {a!r}; this model's types are {sorted(index, key=index.get)}")
+        mask[index[a]] = True
+    return mask
+
+
 def _sampler_kw(model, data, sample_fn, start_step, fixed_atoms):
     """sampler_inputs of a call, with the batch's own linker rows for start_step or fixed_atoms, and the latter as
     EDM.sample_chain's `fixed_atoms` of the template's rows (the batch's linker rows keep their place in it)."""
@@ -254,7 +278,7 @@ def _sampler_kw(model, data, sample_fn, start_step, fixed_atoms):
 def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                  start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                  require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None, require_anchors=None,
-                 clash_guidance=None, solver=None, fixed_atoms=None):
+                 clash_guidance=None, solver=None, fixed_atoms=None, linker_types=None):
     """Body of DDPM.sample_chain (lightning.py:405-463), shared by `DDPM` below and by accelerated reference
     modules (`model` additionally needs .edm). `seeds`: one per molecule, see EDM.sample_chain. Linker sizes drawn by
     `sample_fn` still come from the batch's generator: to replay a molecule, keep its template or its linker size.
@@ -292,8 +316,11 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
     `fixed_atoms` ((B, N) or (B, N, 1), non-zero on the batch's linker atoms to keep): the template of sample_fn=None with
     the batch's own linker rows, as for start_step, of which the flagged atoms are kept and the rest sampled around them
     (EDM.sample_chain); ValueError with a sample_fn or linker_sizes, and when the batch's linker rows do not directly follow
-    its fragment rows."""
+    its fragment rows.
+    `linker_types`: the types the linker atoms may take (EDM.sample_chain; None uses `model.edm.linker_types`), also as
+    element symbols, ['C', 'N', 'O'] (linker_types_mask)."""
     _check_start(sample_fn, start_step)
+    linker_types = linker_types_mask(model.edm, linker_types)
     _check_fixed(sample_fn, linker_sizes, fixed_atoms)
     if linker_sizes is not None:
         _check_linker_sizes(model, sample_fn, start_step)
@@ -328,16 +355,23 @@ def sample_chain(model, data, sample_fn=None, keep_frames=None, seeds=None, nan_
         extra['clash_guidance'] = clash_guidance
     if solver is not None:
         extra['solver'] = solver
+    if linker_types is not None:
+        extra['linker_types'] = linker_types
     chain = model.edm.sample_chain(**kw, keep_frames=keep_frames, **extra)
     if sized is not None:
         return chain, _final_node_mask(kw, sized, model.edm.last_sizes)
     return chain, kw['node_mask']
 
 
+def _with_types(request, linker_types):
+    """The request with its `linker_types` key when it has a set."""
+    return request if linker_types is None else dict(request, linker_types=linker_types)
+
+
 def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                 max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
                 require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None, clash_guidance=None,
-                solver=None, fixed_atoms=None):
+                solver=None, fixed_atoms=None, linker_types=None):
     """The body of sample_chain for many batches `datas` at once, sampled in shared launches by EDM.sample_many: returns
     [(chain_k, node_mask_k)] in the order of `datas`, each equal to what sample_chain(model, datas[k], ...) returns (with
     seeds[k]) in the sense of EDM.sample_many. `model` as for sample_chain, so accelerated reference modules take it too.
@@ -347,8 +381,15 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
     are drawn from its own seeds and its template padded to its own N_cap, so packing changes neither;
     `edm.last_sizes_many` holds them. `resamplings` and `require_anchors` as in sample_chain: each request then holds its
     batch's template anchors. `clash_guidance` and `solver` as in sample_chain. `fixed_atoms`, one per batch (or None for a
-    batch that keeps none), as in sample_chain: each request then holds its batch's flags."""
+    batch that keeps none), as in sample_chain: each request then holds its batch's flags. `linker_types` as in
+    sample_chain, one set for every batch, or a list of one per batch (None for a batch that takes `edm.linker_types`):
+    each request then holds its batch's set."""
     _check_start(sample_fn, start_step)
+    per_batch = isinstance(linker_types, (list, tuple)) and not all(isinstance(v, str) for v in linker_types)
+    if per_batch and len(linker_types) != len(datas):
+        raise ValueError(f"linker_types holds {len(linker_types)} entries for {len(datas)} batches")
+    types = ([linker_types_mask(model.edm, v) for v in linker_types] if per_batch
+             else [linker_types_mask(model.edm, linker_types)] * len(datas))
     if fixed_atoms is not None:
         if len(fixed_atoms) != len(datas):
             raise ValueError(f"fixed_atoms holds {len(fixed_atoms)} entries for {len(datas)} batches")
@@ -368,7 +409,8 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
                         ('solver', solver)):
             if v is not None:
                 extra[name] = v
-        requests = [_with_anchors(model, data, kw, require_anchors) for data, (kw, _, _) in zip(datas, sized)]
+        requests = [_with_types(_with_anchors(model, data, kw, require_anchors), m) for data, (kw, _, _), m
+                    in zip(datas, sized, types)]
         if require_anchors is not None:
             extra['require_anchors'] = require_anchors
         chains = edm.sample_many(requests, keep_frames=keep_frames, seeds=[s for _, s, _ in sized],
@@ -379,7 +421,7 @@ def sample_many(model, datas, sample_fn=None, keep_frames=None, seeds=None, nan_
     requests, drawn = [], []
     for k, data in enumerate(datas):
         kw = _sampler_kw(model, data, sample_fn, start_step, None if fixed_atoms is None else fixed_atoms[k])
-        requests.append(_with_anchors(model, data, kw, require_anchors))
+        requests.append(_with_types(_with_anchors(model, data, kw, require_anchors), types[k]))
         x = kw['x']
         if derive and x.is_cuda:                # a host batch is refused by EDM.sample_many
             with torch.cuda.device(x.device):
@@ -449,24 +491,25 @@ class DDPM(nn.Module):
     def sample_chain(self, data, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                      start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, clash_guidance=None, solver=None, fixed_atoms=None):
+                     require_anchors=None, clash_guidance=None, solver=None, fixed_atoms=None, linker_types=None):
         return sample_chain(self, data, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                             require_connected=require_connected, start_step=start_step, require_valid=require_valid,
                             require_clash_free=require_clash_free, linker_sizes=linker_sizes, require_unique=require_unique,
                             require_novel=require_novel, exclude_hashes=exclude_hashes, resamplings=resamplings,
                             require_ring_sizes=require_ring_sizes, require_anchors=require_anchors,
-                            clash_guidance=clash_guidance, solver=solver, fixed_atoms=fixed_atoms)
+                            clash_guidance=clash_guidance, solver=solver, fixed_atoms=fixed_atoms,
+                            linker_types=linker_types)
 
     def sample_many(self, datas, sample_fn=None, keep_frames=None, seeds=None, nan_retries=None, require_connected=None,
                     max_molecules=256, start_step=None, require_valid=None, require_clash_free=None, linker_sizes=None,
                     require_novel=None, resamplings=None, require_ring_sizes=None, require_anchors=None,
-                    clash_guidance=None, solver=None, fixed_atoms=None):
+                    clash_guidance=None, solver=None, fixed_atoms=None, linker_types=None):
         return sample_many(self, datas, sample_fn=sample_fn, keep_frames=keep_frames, seeds=seeds, nan_retries=nan_retries,
                            require_connected=require_connected, max_molecules=max_molecules, start_step=start_step,
                            require_valid=require_valid, require_clash_free=require_clash_free, linker_sizes=linker_sizes,
                            require_novel=require_novel, resamplings=resamplings, require_ring_sizes=require_ring_sizes,
                            require_anchors=require_anchors, clash_guidance=clash_guidance, solver=solver,
-                           fixed_atoms=fixed_atoms)
+                           fixed_atoms=fixed_atoms, linker_types=linker_types)
 
     def forward(self, *a, **k):
         raise NotImplementedError("training is outside the difflinker_b200 hot path")

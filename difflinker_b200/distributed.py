@@ -191,7 +191,7 @@ def slice_sampler_inputs(kw: dict, lo: int, hi: int):
 
 def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=True, seeds=None, nan_retries=None,
                          require_connected=None, require_valid=None, require_clash_free=None, linker_sizes=None,
-                         require_novel=None, require_ring_sizes=None, require_anchors=None):
+                         require_novel=None, require_ring_sizes=None, require_anchors=None, linker_types=None):
     """Strong scaling of ONE batch (SURVEY.md section 8(e)): the template batch is built once (so every rank pads to the same
     N), each rank runs the reverse loop for its contiguous slice of the molecules with the slice's rows of the full-batch
     noise, and the chains are gathered -- the result equals `model.sample_chain(data)` on one GPU bit for bit, for any
@@ -207,12 +207,13 @@ def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=T
     whose linker hash is in `model.edm.known_linkers` (`last_novel`), and `require_ring_sizes` for those whose linker closes
     a ring of a size not in `model.edm.allowed_ring_sizes` (`last_ring_sizes_ok`), and `require_anchors` for those whose
     linker does not attach at `data['anchors']` alone (`last_anchors_ok`; each rank takes its rows of the template's
-    anchors). `linker_sizes` is refused
+    anchors). `linker_types` (or, when None, `model.edm.linker_types`) as in ddpm.sample_chain: a (B, F) set gives each
+    rank its rows. `linker_sizes` is refused
     (ValueError): sample the batch with ddpm.sample_chain(linker_sizes=...) and EDM.devices instead."""
     if linker_sizes is not None:
         raise ValueError("sample_chain_sharded does not take linker_sizes: use ddpm.sample_chain(linker_sizes=...), which "
                          "EDM.devices splits over local GPUs")
-    from .ddpm import _anchor_extra, sampler_inputs
+    from .ddpm import _anchor_extra, linker_types_mask, sampler_inputs
     from .edm import seeds_tensor
     kw = sampler_inputs(model, data, sample_fn)
     B = kw['x'].shape[0]
@@ -234,6 +235,11 @@ def sample_chain_sharded(model, data, sample_fn=None, keep_frames=None, gather=T
     _anchor_extra(model, data, kw['x'].shape[1], require_anchors, extra)
     if 'anchors' in extra:
         extra['anchors'] = extra['anchors'][lo:hi]
+    if linker_types is None:
+        linker_types = getattr(model.edm, 'linker_types', None)
+    types = linker_types_mask(model.edm, linker_types)
+    if types is not None:
+        extra['linker_types'] = types[lo:hi] if types.dim() == 2 else types
     if seeds is not None:
         chain = model.edm.sample_chain(**local, keep_frames=keep_frames, seeds=seeds_tensor(seeds, B)[lo:hi], **extra)
     else:

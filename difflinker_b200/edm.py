@@ -72,7 +72,7 @@ def _loop_steps(start):
 
 
 def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None, retry=None, start=None, resample=None,
-                  guide=None, solver=None, fixed=None):
+                  guide=None, solver=None, fixed=None, types=None):
     """One slice's reverse loop on its engine: dl_sample_chain_*(eng, *head, <draws>, *tail, stream). The draws are the
     per-molecule `seeds`, the batch stream `rng` = (seed, offset, b0, B_full) -- the call's B rows are rows [b0, b0 + B) of a
     B_full-molecule batch, set on the engine for the duration of the call -- or else the `noise` tensor. `stream` None
@@ -94,7 +94,8 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
     the duration of the call (dl_set_clash_guidance). `solver` = (kind, T, table) replaces the ancestral update by an ODE
     solver's, set on the engine for the duration of the call (dl_set_solver). `fixed` = ((B, N) int8 flags on the slice's
     device, or on the host with host inputs, T, scalars) keeps the flagged linker rows (dl_set_fixed_atoms, right before
-    the call, which clears it). Returns (status, what the batch stream consumed)."""
+    the call, which clears it). `types` = ((B,) int32 CPU masks, F, T, scalars) gives the linker atoms allowed types only
+    (dl_set_linker_types, right before the call, which clears it). Returns (status, what the batch stream consumed)."""
     per_row = isinstance(start, StartSteps)
     if per_row:
         start.set_on(lib, eng)
@@ -113,8 +114,14 @@ def _sample_slice(lib, eng, head, tail, stream, noise=None, seeds=None, rng=None
             flags, T, scalars = fixed
             _native.check(lib.dl_set_fixed_atoms(eng, head[1], head[2], flags.data_ptr(), T, scalars, stream),
                           "dl_set_fixed_atoms")
+        if types is not None:
+            masks, F, T, scalars = types
+            _native.check(lib.dl_set_linker_types(eng, head[1], F, masks.data_ptr(), T, scalars),
+                          "dl_set_linker_types")
         return _sample_slice_draws(lib, eng, head, tail, stream, noise, seeds, rng, retry)
     finally:
+        if types is not None:               # a call that failed before the engine read the masks
+            lib.dl_set_linker_types(eng, 0, 0, None, 0, None)
         if fixed is not None:               # a call that failed before the engine read the flags
             lib.dl_set_fixed_atoms(eng, 0, 0, None, 0, None, None)
         if solver is not None:
@@ -331,6 +338,9 @@ class EDM(torch.nn.Module):
         # 'dpmpp_2m' take deterministic steps of the probability-flow ODE (solver_coefficients), for calls that get no
         # `solver`. Meant for a shortened loop: edm.T = 20; edm.solver = 'dpmpp_2m'
         self.solver = 'ancestral'
+        # Linker types (EDM only): the allowed type channels of the linker atoms, a (F,) or (B, F) bool tensor, for calls
+        # that get no `linker_types` (sample_chain); None, the default, allows every type
+        self.linker_types = None
         self.devices = None
         self.last_loop_ms = None               # device time of the last reverse loop (CUDA events); the slowest slice's if split
         self.last_slice_loop_ms = None         # split calls: [(device, lo, hi, loop ms)] per slice of the batch
@@ -701,6 +711,42 @@ class EDM(torch.nn.Module):
         """_enqueue_batch's `fixed` of flags returned by _fixed_atoms: (flags, scalars at n_samples), or None."""
         return None if flags is None else (flags, self.fixed_atom_scalars(n_samples))
 
+    def _linker_types(self, linker_types, n_samples, fixed=None, h=None, what="linker_types"):
+        """The (B,) CPU int32 masks of the type channels a call's linker atoms may take (bit c: channel c), or None without
+        `linker_types` or when it allows every type (the plain call). `linker_types` is a (F,) bool tensor, one set for the
+        call, or (B, F), one per molecule; `fixed` (the flags of _fixed_atoms, or None) and the one-hot `h` are the kept rows,
+        whose types must be allowed. ValueError for InpaintingEDM, another shape or dtype, and a molecule that allows no
+        type."""
+        if linker_types is None:
+            return None
+        if self._SAMPLER == _native.SAMPLER_INPAINT:
+            raise ValueError("linker_types takes the linker sampler (EDM) only: InpaintingEDM generates its atoms in its own "
+                             "update")
+        F = self.in_node_nf
+        m = linker_types.detach() if torch.is_tensor(linker_types) else None
+        if m is None or m.dtype != torch.bool or tuple(m.shape) not in ((F,), (n_samples, F)):
+            got = (f"{m.dtype} of shape {tuple(m.shape)}" if m is not None else type(linker_types).__name__)
+            raise ValueError(f"{what} must be a bool tensor of shape (F,) or (B, F) for F = {F}, B = {n_samples} (got {got})")
+        m = m.cpu().expand(n_samples, F)
+        empty = (~m.any(dim=1)).nonzero()
+        if len(empty):
+            raise ValueError(f"{what}: molecule {int(empty[0])} allows no atom type")
+        if m.all():
+            return None
+        if fixed is not None:
+            kept = fixed.cpu() != 0
+            types = h.detach().reshape(n_samples, kept.shape[1], F).cpu().argmax(dim=2)
+            off = kept & ~torch.gather(m, 1, types)
+            if off.any():
+                b, n = (int(v) for v in off.nonzero()[0])
+                raise ValueError(f"{what}: row {n} of molecule {b} is kept (fixed_atoms) but its type {int(types[b, n])} "
+                                 "is one the molecule's set excludes")
+        return (m.to(torch.int64) << torch.arange(F)).sum(dim=1).to(torch.int32).contiguous()
+
+    def _types(self, masks, n_samples):
+        """_enqueue_batch's `types` of masks returned by _linker_types: (masks, F, scalars at n_samples), or None."""
+        return None if masks is None else (masks, self.in_node_nf, self.fixed_atom_scalars(n_samples))
+
     def _start(self, start_step, n_samples):
         """(t0, alpha_t0, sigma_t0) of a call of n_samples molecules that starts at step `start_step`, or None for one that
         starts from noise at T; for a 1-D sequence or integer tensor of one step per molecule, their StartSteps, every
@@ -966,7 +1012,8 @@ class EDM(torch.nn.Module):
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, anchors=None, clash_guidance=None, solver=None, fixed_atoms=None):
+                     require_anchors=None, anchors=None, clash_guidance=None, solver=None, fixed_atoms=None,
+                     linker_types=None):
         """Same contract as the reference (edm.py:126-176): returns (keep_frames, B, N, 3+F); chain[0] holds the
         final coordinates and one-hot atom types. `noise` optionally injects the (T+2,B,N,3+F) draws (tests).
         `start_step` = t0, an int in [0, T] (partial diffusion; None, the default, samples from noise at T): the linker on
@@ -1096,6 +1143,18 @@ class EDM(torch.nn.Module):
         (which moves only the free linker atoms), `solver`, keep_frames, `devices` and batch_slice work as without it. A
         mask that flags no row is the plain call, bit for bit. ValueError for a flag off the linker rows, a kept row whose
         h is not a one-hot, the wrong shape, InpaintingEDM and linker_sizes.
+        `linker_types` (a bool tensor, (F,) for one set of allowed type channels for the call or (B, F) for one per
+        molecule; None, the default, uses `edm.linker_types`) gives every linker atom of chain[0] an allowed type
+        (dl_set_linker_types): at every step, on every linker row that fixed_atoms does not keep, the data prediction
+        xhat = (z_t - sigma_t eps) / alpha_t of an excluded channel is set to the one-hot's normalised off value (0 - bias1)
+        / norm1 -- the ancestral update reads eps = (z_t - alpha_t off) / sigma_t instead, with the (alpha_t, sigma_t) of
+        fixed_atom_scalars, an ODE `solver` takes xhat itself, 2M history included -- and the final one-hot is the argmax
+        over the allowed channels. So the constraint holds by construction, including the rows of recovery rounds and NaN
+        retries; intermediate keep_frames frames are continuous states and carry no such guarantee. The draws are those
+        of the call without it, so seeds, noise=, the batch stream, start_step, the recovery rounds, linker_sizes,
+        clash_guidance, `solver`, keep_frames, `devices` and batch_slice work as without it. A set that allows every type
+        is the plain call, bit for bit. ValueError for a molecule that allows no type, the wrong shape or dtype,
+        InpaintingEDM, and a fixed_atoms row whose type is excluded.
         The batch is sampled in slices, each on an engine of its own: one covering it on x's device or, with `devices` set
         and no batch_slice, one per listed device (distributed.device_slices). Inputs and draws are prepared once on x's
         device; each slice samples its rows of them with the full batch's step coefficients, several slices from one host
@@ -1124,6 +1183,7 @@ class EDM(torch.nn.Module):
         fixed = self._fixed_atoms(fixed_atoms, x, h, node_mask, fragment_mask, linker_mask, context)
         if fixed is not None and redraw is not None:
             raise ValueError("fixed_atoms does not take linker_sizes: a size redraw rebuilds the linker rows at new sizes")
+        masks = self._linker_types(self.linker_types if linker_types is None else linker_types, n_samples, fixed, h)
         sets = self._hash_sets(check, exclude_hashes, dev)
         recover = retries > 0 or check != 0 # the recovery entry point: seeds used and attempts come back
         dev_seeds = self._per_molecule_seeds(seeds, noise, batch_slice, x)
@@ -1162,7 +1222,8 @@ class EDM(torch.nn.Module):
                                             rng=(seed, offset, b0, b_full) if on_device else None, retries=retries, check=check,
                                             start=start, redraw=redraw, sets=sets,
                                             resample=self._resample(r, n_samples), anchors=anchor_flags, guide=guide,
-                                            solver=ode, fixed=self._fixed(fixed, n_samples))
+                                            solver=ode, fixed=self._fixed(fixed, n_samples),
+                                            types=self._types(masks, n_samples))
         by_device = {}
         for dev_i, c in calls:
             by_device.setdefault(dev_i, []).append(c)
@@ -1269,6 +1330,10 @@ class EDM(torch.nn.Module):
         `fixed_atoms` likewise: a request may hold its (B_k, N_k) or (B_k, N_k, 1) flags of the linker rows to keep, as
         sample_chain's `fixed_atoms`. They travel per row, and requests then share a launch only where sample_chain would
         give them the same fixed_atom_scalars.
+        `linker_types` likewise: a request may hold its (F,) or (B_k, F) bool set of allowed types, as sample_chain's
+        `linker_types`; a request without one takes `edm.linker_types`. The masks travel per row, so requests with
+        different sets share a launch; a request whose set allows every type runs the plain update, as its own
+        sample_chain call does, and shares launches only with other such requests.
         `linker_sizes`, one LinkerSizes per request, all of one size table, redraws sizes in those rounds as in sample_chain
         (it needs `seeds`); `last_sizes_many` holds every request's sizes. Each request's sizes come from its own seeds, so
         packing does not change them.
@@ -1307,9 +1372,9 @@ class EDM(torch.nn.Module):
             if 'noise' in r or 'batch_slice' in r:
                 raise ValueError(f"request {k} passes noise= or batch_slice=: sample_many samples per-molecule streams, "
                                  "which need neither")
-            if set(r) - {'anchors', 'fixed_atoms'} != set(self._REQUEST_INPUTS):
+            if set(r) - {'anchors', 'fixed_atoms', 'linker_types'} != set(self._REQUEST_INPUTS):
                 raise ValueError(f"request {k} must hold exactly the inputs {self._REQUEST_INPUTS}, and may hold "
-                                 f"'anchors' and 'fixed_atoms' (got {sorted(r)})")
+                                 f"'anchors', 'fixed_atoms' and 'linker_types' (got {sorted(r)})")
         if self._draws_replaced():
             raise ValueError("sample_many needs the device-side per-molecule stream, but this model's draw function is replaced")
         if seeds is None and self.noise_mode != 'per_molecule':
@@ -1362,6 +1427,9 @@ class EDM(torch.nn.Module):
         any_fixed = any(f is not None for f in fixed_many)
         if any_fixed and linker_sizes is not None:
             raise ValueError("fixed_atoms does not take linker_sizes: a size redraw rebuilds the linker rows at new sizes")
+        types_many = [self._linker_types(r.get('linker_types', self.linker_types), r['x'].shape[0], fixed_many[k], r['h'],
+                                         f"request {k}'s linker_types") for k, r in enumerate(requests)]
+        any_types = any(m is not None for m in types_many)
         sets = self._hash_sets(check, None, dev)
         recover = retries > 0 or check != 0
         redraws = None
@@ -1381,8 +1449,10 @@ class EDM(torch.nn.Module):
             keys = [k + (bytes(self.jump_coefficients(b)),) for k, b in zip(keys, sizes)]
         if guide is not None:               # the same for every request of a call: launches are sampled as it says
             keys = [k + (guide[:2],) for k in keys]
-        if any_fixed:                       # the kept rows' scalars depend on the batch size as the table does
+        if any_fixed or any_types:          # the kept rows' scalars depend on the batch size as the table does
             keys = [k + (bytes(self.fixed_atom_scalars(b)),) for k, b in zip(keys, sizes)]
+        if any_types:                       # a request without a set runs the plain instantiation, as its own call does
+            keys = [k + (m is not None,) for k, m in zip(keys, types_many)]
         fc = self.dynamics.graph_type == 'FC'
         launches = plan_launches(sizes, nodes, max_molecules, keys)
         if fc:                              # edges of the launch's padded molecules
@@ -1417,6 +1487,9 @@ class EDM(torch.nn.Module):
                     fixed_many[k] if fixed_many[k] is not None else torch.zeros((sizes[k], nodes[k]), dtype=torch.int8,
                                                                                 device=dev), (0, n - nodes[k]))
                     for k in ks]), sizes[ks[0]])
+            types = None                    # the launch key keeps requests with and without a set apart
+            if types_many[ks[0]] is not None:
+                types = self._types(torch.cat([types_many[k] for k in ks]), sizes[ks[0]])
             dev_seeds = torch.cat([cpu_seeds[k] for k in ks]).to(dev)
             where = torch.device('cuda', dev_i)
             eng = engine_of[slot_of[i]]
@@ -1428,7 +1501,7 @@ class EDM(torch.nn.Module):
                                                       [where], dev, dev_seeds=dev_seeds, retries=retries, check=check,
                                                       start=start, redraw=redraw, sets=sets,
                                                       resample=self._resample(r_passes, sizes[ks[0]]), anchors=anchors,
-                                                      guide=guide, solver=ode, fixed=fixed)
+                                                      guide=guide, solver=ode, fixed=fixed, types=types)
             finishes.append(finish)
             by_device.setdefault(dev_i, []).append(
                 functools.partial(timed, i, call, eng, dev_i, torch.cuda.current_stream(where)))
@@ -1515,7 +1588,7 @@ class EDM(torch.nn.Module):
 
     def _enqueue_batch(self, lib, full, keep_frames, coef, slices, engines, places, dev, noise=None, dev_seeds=None, rng=None,
                        retries=0, check=0, start=None, redraw=None, sets=None, resample=None, anchors=None, guide=None,
-                       solver=None, fixed=None):
+                       solver=None, fixed=None, types=None):
         """The reverse loops of one batch, the single-launch path under sample_chain and sample_many: `full` (the prepared
         inputs of B molecules on `dev`, _sampler_tensors) sampled with the step coefficients `coef` in `slices` [(device,
         replica, lo, hi)], slice i on engines[i] with its inputs on places[i] -- the caller's tensors themselves when one slice
@@ -1524,7 +1597,8 @@ class EDM(torch.nn.Module):
         returned by _start; `redraw` as returned by _linker_sizes (its rounds then redraw sizes, into `sizes`); `sets` as
         returned by _hash_sets, copied to each slice's device; `resample` as returned by _resample; `anchors` as returned
         by _anchors, each slice's rows on its device; `guide` as returned by _clash_guidance; `solver` as returned by
-        _solver; `fixed` as returned by _fixed, each slice's rows of the flags on its device.
+        _solver; `fixed` as returned by _fixed, each slice's rows of the flags on its device; `types` as returned by _types,
+        each slice's rows of the masks.
         Allocates and copies on the calling thread and returns ([(device, call)], finish): each call runs one slice's loop
         (from a host thread of its device, in order per device), and finish(), after every call, copies the slices' rows
         back and returns dict(chain, flags, used, attempts, passed, sizes, bad, consumed) on `dev`; `passed` holds
@@ -1594,7 +1668,8 @@ class EDM(torch.nn.Module):
                 (retries, used_i, attempts_i, check, checks_i, passed_i, redraw_i, sets_i, lh_i,
                  (allowed, rs_i) if rings else None, an_i) if recover else None,
                 start.rows(lo, hi) if isinstance(start, StartSteps) else start, resample, guide, solver,
-                None if fixed is None else (fx_i, self.T, fixed[1]))))
+                None if fixed is None else (fx_i, self.T, fixed[1]),
+                None if types is None else (types[0][lo:hi].contiguous(), types[1], self.T, types[2]))))
 
         def finish():
             if not whole:
@@ -1679,7 +1754,8 @@ class InpaintingEDM(EDM):
                      noise=None, batch_slice=None, seeds=None, nan_retries=None, require_connected=None, start_step=None,
                      require_valid=None, require_clash_free=None, linker_sizes=None, require_unique=None,
                      require_novel=None, exclude_hashes=None, resamplings=None, require_ring_sizes=None,
-                     require_anchors=None, anchors=None, clash_guidance=None, solver=None, fixed_atoms=None):
+                     require_anchors=None, anchors=None, clash_guidance=None, solver=None, fixed_atoms=None,
+                     linker_types=None):
         """EDM.sample_chain in the reference's positional order for this class (edge_mask third). `noise` optionally
         injects the (2T+3,B,N,3+F) prepared draws of `draw_noise_inpaint` (tests). Without it, on CUDA and with noise_mode
         'reference_stream', the draws are made inside the kernels from the default generator's state
@@ -1702,7 +1778,8 @@ class InpaintingEDM(EDM):
         them; the batch stream advances by as many draws; per-molecule streams use their draws in that order). r = 1 is
         the plain sampler, bit for bit. A call costs about r times the loop. ValueError for a non-integer, a bool or
         r < 1. `clash_guidance` raises ValueError unless None: this loop re-noises the pocket. `solver` unless None or
-        'ancestral': this sampler has no ODE update. `fixed_atoms` unless None: this sampler keeps known atoms its own way."""
+        'ancestral': this sampler has no ODE update. `fixed_atoms` unless None: this sampler keeps known atoms its own way.
+        `linker_types` unless None: this sampler generates its atoms in its own update."""
         return super().sample_chain(x=x, h=h, node_mask=node_mask, fragment_mask=fragment_mask, linker_mask=linker_mask,
                                     edge_mask=edge_mask, context=context, keep_frames=keep_frames, noise=noise,
                                     batch_slice=batch_slice, seeds=seeds, nan_retries=nan_retries,
@@ -1711,7 +1788,8 @@ class InpaintingEDM(EDM):
                                     require_unique=require_unique, require_novel=require_novel,
                                     exclude_hashes=exclude_hashes, resamplings=resamplings,
                                     require_ring_sizes=require_ring_sizes, require_anchors=require_anchors,
-                                    anchors=anchors, clash_guidance=clash_guidance, solver=solver, fixed_atoms=fixed_atoms)
+                                    anchors=anchors, clash_guidance=clash_guidance, solver=solver, fixed_atoms=fixed_atoms,
+                                    linker_types=linker_types)
 
 
 # the draws the device-side stream reproduces; a replaced draw_noise_inpaint takes the tensor path

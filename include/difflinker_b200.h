@@ -25,6 +25,8 @@
  *     instead of p(z_s | z_t) (no reference API)
  *   EDM, keeping given linker atoms and sampling the    dl_set_fixed_atoms before each dl_sample_chain* call
  *     rest (replacement, RePaint without re-noising passes; no reference API)
+ *   EDM, with linker atoms of allowed elements only      dl_set_linker_types before each dl_sample_chain* call
+ *     (the data prediction projected; no reference API)
  *   InpaintingEDM, r RePaint passes per step            dl_set_resamplings, then any dl_sample_chain* entry point
  *     (DiffSBDD's inpaint(..., resamplings=r), no reference API)
  *   either, resampling only the molecules that diverged  dl_sample_chain_retry, dl_retry_seed, dl_last_retry_ms
@@ -820,6 +822,29 @@ dl_status dl_set_solver(dl_engine* e, int32_t kind, int32_t T, const float* tabl
  */
 dl_status dl_set_fixed_atoms(dl_engine* e, int32_t B, int32_t N, const int8_t* fixed, int32_t T, const float* scalars,
                              void* stream);
+/*
+ * Linker types for DL_SAMPLER_LINKER (no reference API): the engine's next dl_sample_chain* call -- and the recovery rounds
+ * of a dl_sample_chain_retry(_sets) call, each row with its molecule's mask -- gives every linker atom of molecule b a type
+ * that bit c of the HOST mask masks[b] allows (type channel c, c < F). On every free linker row (linker_mask non-zero, not
+ * kept by dl_set_fixed_atoms) each step constrains the data prediction of the excluded channels to the one-hot's
+ * normalised off value, off = (0 - norm[2]) / norm[1]:
+ *   ancestral update        eps_c = (z_t,c - alpha_t off) / sigma_t, which gives xhat_c = (z_t,c - sigma_t eps_c) / alpha_t
+ *                           = off; (alpha_t, sigma_t) is row t - 1 of the (T + 1, 2) HOST fp32 `scalars` at a step from
+ *                           t >= 1 (dl_step_coef's row order, so row r holds step s = T-1-r), and row T at the step from T
+ *   dl_set_solver           xhat_c = off, which also enters the DPM-Solver++(2M) history
+ *   final step              the one-hot of chain[0] takes the argmax over the allowed channels only
+ * so every linker atom of chain[0] has an allowed type by construction. Kept rows and fragment and pocket rows are not
+ * changed. No draw is added or moved, so seeds, offsets and noise tensors mean what they mean without this call.
+ * Intermediate frames (keep_frames > 1) hold continuous states, which carry no such guarantee. EDM.fixed_atom_scalars builds
+ * `scalars`. Per-call input like dl_set_anchors: masks and scalars are copied into host memory here and uploaded on the loop
+ * stream by the call; every dl_sample_chain* call reads and clears the setting, whether or not it uses it. masks = NULL
+ * switches it off (the other arguments are ignored): the calls then launch exactly what they launch without it.
+ * DL_ERR_INVALID: here, B < 1, F other than dl_config.in_node_nf, a mask of 0 or with bits at or above F, T outside
+ * [1, 2^24], NULL scalars or a non-finite one; at the sampling call, a B or T other than the ones set, DL_SAMPLER_INPAINT,
+ * and, with dl_set_fixed_atoms, a kept row whose one-hot type its molecule's mask excludes (vetted in the blocking check
+ * of dl_set_fixed_atoms).
+ */
+dl_status dl_set_linker_types(dl_engine* e, int32_t B, int32_t F, const uint32_t* masks, int32_t T, const float* scalars);
 /* The (n_draws,B,N,3+F) tensor the device-side stream of dl_sample_chain_rng stands for (tests, debugging). DEVICE out. */
 dl_status dl_noise_fill(dl_engine* e, int32_t n_draws, int32_t B, int32_t N, uint64_t seed, uint64_t offset, float* out,
                         uint64_t* offset_consumed, void* stream);
